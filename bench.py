@@ -1,6 +1,6 @@
-"""bench.py - LLaMA-7B gptq.int4 batch-1 decode throughput on B200 (BASELINE.json configs[1]).
+"""bench.py - LLaMA-7B gptq.int4 batch-1 decode throughput on H100 (BASELINE.json configs[1]).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 A step = one decoded token (one pass of generate()'s loop body, generate.py:63-89: model forward + top-k / softmax /
 multinomial sampling) on random-init 7B gptq.int4 weights, KV cache S = 2048.  The K timed steps are spread EVENLY over
@@ -22,6 +22,10 @@ N > 1: `value` = independent replicas, one process per GPU (the reference has no
 2.1; 7B fits one GPU): weak scaling, no data-path collective.  The same run then measures the TENSOR-PARALLEL path on
 the same ranks and reports it under "tp": LLaMA-7B split N ways, and LLaMA-65B gptq.int4 TP = 8 (BASELINE.json
 configs[4]) when N = 8 -- fused per-rank step, two one-shot all-reduces per Block over peer memory (tools/tp_bench.py).
+
+--dump-outputs DIR (rank 0): after the timed loop, what its LAST step returned to the caller -- DIR/logits.npy (float32,
+the vocab row the step's forward produced) and DIR/token.npy (float64, the token sampled from it).  Weights, prompt and
+the sampling noise are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -96,7 +100,7 @@ def synth_state(name, seed=1234, dev=None):
 
 
 def build_synthetic_model(name, dev, seed=1234, state=None):
-    """The B200 model of the named size holding synth_state(name, seed) (same tensors as the CPU reference arm)."""
+    """The model of the named size holding synth_state(name, seed) (same tensors as the CPU reference arm)."""
     import torch
 
     import lit_llama_b200 as P
@@ -334,14 +338,9 @@ def build_line(args, world, K, warm, t_dev, t_e2e, Ke, timed_pos, points, clk, t
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except OSError:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    which = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+    peak = float(peaks.get("hbm_gbs", 3350.0))
+    which = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 3350 GB/s (H100 SXM data sheet)"
     ach = W / t_q4 / 1e9
-    traffic = None
-    try:  # dram bytes of the kernel's launches of one token, from the committed ncu capture
-        traffic = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))["bytes_per_token"]
-    except (OSError, KeyError, ValueError):
-        pass
     return {
         "metric": "LLaMA-7B gptq.int4 decode tokens/sec", "value": aggregate_throughput(world, K, t_dev), "unit": "tokens/s", "n_gpus": world,
         "steps": K, "warmup": warm, "ms_per_step": t_dev / K * 1e3, "higher_is_better": True, "scaling": "weak",
@@ -350,16 +349,25 @@ def build_line(args, world, K, warm, t_dev, t_e2e, Ke, timed_pos, points, clk, t
                    "positions": f"{K} positions spread evenly over {lo}..{S_CTX - 1} (mean {mean_p:.0f})",
                    "points": {**points, "unit": "tokens/s at fixed position"}, "sampling": f"top_k={TOP_K} temperature={TEMPERATURE}",
                    "parallelism": f"replicas x{world}" if world > 1 else "single GPU",
-                   "l2": "weights 3.31 GB per token >> 126 MB L2 (inputs larger than L2)"},
+                   "l2": "weights 3.31 GB per token >> 50 MB L2 (inputs larger than L2)"},
         "clocks": clk,
         "e2e": {"value": aggregate_throughput(world, Ke, t_e2e), "unit": "tokens/s", "h2d_bytes_per_step": 12, "d2h_bytes_per_step": 8, "steps": Ke},
         "gpu_launches": (launches + 1) * K,  # b2l_decode_step's kernels + the fused sampling kernel, per token
-        "roofline": {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": traffic,
+        "roofline": {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
                      "kernel": q4_name, "launches_per_token": n_q4, "bytes_per_token_launches": W,
                      "peak_source": which,
                      "whole_token_bytes": bytes_per_token, "whole_token_achieved": bytes_per_token * K / t_dev / 1e9,
                      "whole_token_frac": bytes_per_token * K / t_dev / 1e9 / peak},
     }
+
+
+def dump_outputs(out_dir, logits, tok):
+    """The last timed step's results as a caller receives them: logits (float32) and the sampled token (float64)."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "logits.npy"), logits.reshape(-1).float().cpu().numpy())
+    np.save(os.path.join(out_dir, "token.npy"), tok.reshape(-1).double().cpu().numpy())
 
 
 def reduce_max(times, device):
@@ -387,6 +395,7 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-tp", action="store_true", help="N > 1: skip the tensor-parallel block")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's logits and token as .npy files into DIR")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -400,6 +409,7 @@ def main():
 
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
+    torch.manual_seed(1234 + rank)   # the sampling noise: the same arguments decode the same tokens
     if world > 1:
         dist.init_process_group("nccl", device_id=dev)
     warm = max(3, args.warmup)
@@ -439,12 +449,15 @@ def main():
         tw0 = time.time()
         e0.record()
         for i in range(warm, warm + K):
-            tok = sample_next(model(tok.view(1, 1), S_CTX, pos_all[i])).to(torch.int32)
+            logits = model(tok.view(1, 1), S_CTX, pos_all[i])
+            tok = sample_next(logits).to(torch.int32)
         e1.record()
         barrier()
         tw1 = time.time()
         t_dev = e0.elapsed_time(e1) * 1e-3
         clk = clocks.stop(tw0, tw1)
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, logits, tok)
 
         # ---- e2e: host buffers; per step H2D (token, position) from pinned memory, D2H sampled token
         h_tok = torch.empty(1, dtype=torch.int32).pin_memory()

@@ -1,5 +1,5 @@
 /*
- * b2l.h - C ABI of libb200llama.so: the B200 (sm_100a) quantized-decode path for
+ * b2l.h - C ABI of libb200llama.so: the H100 (sm_90a) quantized-decode path for
  * Lightning-AI/lit-llama.
  *
  * The reference has no native boundary of its own: its "operator API" for this path
@@ -67,7 +67,7 @@ int b2l_q_linear(const void* x, int ldx, const void* qw, const void* scales, con
                  int tile_cols, b2l_stream_t stream);
 
 /* One-time (load-time) re-tiling of a 4-bit, one-group-per-row weight for the
- * tcgen05 kernel: [N/128 tiles][K/32 slabs][128 rows][16 B].  N is padded up to a
+ * wgmma kernels: [N/128 tiles][K/32 slabs][128 rows][16 B].  N is padded up to a
  * multiple of 128 with zero levels.  Pure permutation of nibbles (bit-exact,
  * invertible: b2l_q4_untile).  Precedent for load-time transforms in the
  * reference: Linear8bitLt._load_from_state_dict, quantization.py:52-67. */
@@ -75,7 +75,7 @@ size_t b2l_q4_tiled_bytes(int N, int K);
 int b2l_q4_tile(const void* qw, void* qw_tiled, int N, int K, b2l_stream_t stream);
 int b2l_q4_untile(const void* qw_tiled, void* qw, int N, int K, b2l_stream_t stream);
 
-/* Prologue / epilogue selectors of the fused tcgen05 linear. */
+/* Prologue / epilogue selectors of the fused linears. */
 enum { B2L_PRO_NONE = 0, B2L_PRO_RMSNORM = 1 };
 enum {
   B2L_EPI_STORE = 0,    /* y = bf16(acc)                                              */
@@ -127,23 +127,23 @@ typedef struct b2l_q4_linear_args {
 
 enum {
   B2L_F_PDL = 1,        /* launch with programmatic dependent launch                   */
-  B2L_F_NO_ALIAS_N = 2, /* debug: do not alias B operand rows 8..15 onto rows 0..7     */
+  B2L_F_NO_ALIAS_N = 2, /* debug: b2l_q4_linear_tc uses 16-column MMAs even for M <= 8  */
   B2L_F_ROPE_ROWS = 4,  /* b2l_attention: `rope` holds the T rows already selected by
                            input_pos (the reference's call convention, model.py:93)    */
   B2L_F_ATTN_UNFUSED = 8, /* debug: force the three-kernel attention path for T == 1   */
   B2L_F_DEBUG_NOCOMPUTE = 16 /* debug: b2l_q4_gemv streams the weights but skips the math */
 };
 
-/* Fused [RMSNorm ->] int4 linear [-> residual | SwiGLU] on tcgen05.  Replaces
+/* Fused [RMSNorm ->] int4 linear [-> residual | SwiGLU] on wgmma (M <= 16).  Replaces
  * RMSNorm.forward (model.py:270-277) + ColBlockQuantizedLinear.forward
  * (quantization.py:413-423) + the residual add / silu*mul of Block/MLP.forward
  * (model.py:166-167, 252). */
 int b2l_q4_linear_tc(const b2l_q4_linear_args* args, b2l_stream_t stream);
 
-/* Prefill-shaped linear (any M; meant for M > 16): y[M, N] = x[M, K] . dequant(W)^T on tcgen05 (csrc/q4_gemm.cu):
- * 256 x 256 output tile per CTA, both operands from shared memory (producer warps dequantise the packed levels with
+/* Prefill-shaped linear (any M; meant for M > 16): y[M, N] = x[M, K] . dequant(W)^T on wgmma (csrc/q4_gemm.cu):
+ * 128 x 128 output tile per CTA, both operands from shared memory (producer warps dequantise the packed levels with
  * the reference's own bf16 roundings, so the tensor core multiplies exactly get_weight()'s matrix), fp32 accumulators
- * in tensor memory.  Same argument block as b2l_q4_linear_tc; qw_tiled from b2l_q4_tile; prologue / epilogue must be
+ * in registers.  Same argument block as b2l_q4_linear_tc; qw_tiled from b2l_q4_tile; prologue / epilogue must be
  * NONE / STORE; K % 64 == 0; ldx % 8 == 0.  Replaces quantization.py:187-333 (Triton tile kernel) / :413-423. */
 int b2l_q4_gemm(const b2l_q4_linear_args* args, b2l_stream_t stream);
 
@@ -289,7 +289,7 @@ int b2l_kv_unroll(const void* cache, const int32_t* ring_start, void* out, int B
  * every kernel of the step enqueued by one call.
  * ---------------------------------------------------------------------------- */
 typedef struct b2l_q4_weight {
-  const void* qw_tiled;   /* b2l_q4_tile layout (tcgen05 kernel), used when B > 1; may be NULL if B == 1 */
+  const void* qw_tiled;   /* b2l_q4_tile layout (wgmma kernel), used when B > 1; may be NULL if B == 1 */
   const void* qw_mma;     /* mma.sync kernels: b2l_q4_tile_i8 layout when B == 1 (b2l_q4_gemv), b2l_q4_tile_mma
                              layout when B in 2..8 (b2l_q4_gemv_batch); may be NULL if B > 8 */
   const void* scales;
@@ -337,7 +337,7 @@ typedef struct b2l_decode_args {
                                 [(5*n_layer+1)*16] per-op stamps of the persistent kernel   */
   void* batch_work;          /* B in 2..8: scratch of b2l_q4_gemv_batch_workspace_bytes(max K) bytes; the
                                 linears then run on the mma.sync batch kernel (weights need qw_mma).
-                                NULL: tcgen05 kernel (weights need qw_tiled)              */
+                                NULL: wgmma kernel (weights need qw_tiled)                */
   void* plan;                /* B == 1, head_size 128: device buffer of b2l_decode_plan_bytes() bytes prepared by
                                 b2l_decode_plan_build -> the whole step runs as ONE persistent kernel
                                 (csrc/decode_mega.cu; weights need the b2l_q4_tile_i8 layout in qw_mma).

@@ -9,17 +9,6 @@ extern "C" {
 
 const char* b2l_diag_last_error(void);
 
-/* Debug only (tools/diag.py): tcgen05.mma issue / completion cycle counts of one CTA.
- * out: device uint64[rounds*3] = {cycles to issue n_mma MMAs, cycles to issue the commit,
- * cycles until the commit's mbarrier arrives}. */
-int b2l_debug_mma_rate(void* out, int n_mma, int n_acc, int a_from_smem, int rounds,
-                       b2l_stream_t stream);
-
-/* Debug only (tools/diag.py mma_issuers): 1..4 warps of one CTA each issue 16 tcgen05.mma (own accumulator) and a
- * commit.  out: device uint64[rounds][8] = {cycles until warp w's commit arrived (w = 0..3), cycles warp w spent
- * issuing (w = 0..3)}: does MMA issue scale with the number of issuing threads? */
-int b2l_debug_mma_issuers(void* out, int n_issuers, int rounds, b2l_stream_t stream);
-
 /* Debug only (tools/diag.py grid_flag): latency of a grid-wide arrive-and-wait on a global counter (red.release +
  * ld.acquire polling) with ctas_per_sm * SMs co-resident CTAs.  counter: zeroed device uint32; out: device
  * uint64[2 * rounds], first half zeroed (max ns per round), second half set to ~0 (min ns per round). */

@@ -1,4 +1,4 @@
-"""lit-llama_b200: B200 (sm_100a) quantized-decode path for Lightning-AI/lit-llama.
+"""lit-llama_b200: H100 (sm_90a) quantized-decode path for Lightning-AI/lit-llama.
 
 Mirrors the reference's public surface for this path (lit_llama/__init__.py):
 `LLaMA, LLaMAConfig, RMSNorm, build_rope_cache, apply_rope`, the quantized linears of

@@ -30,10 +30,10 @@ int cuda_fail(cudaError_t e, const char* what) {
 int sm_count() {
   static int n[B2L_MAX_DEVICES] = {};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= B2L_MAX_DEVICES) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= B2L_MAX_DEVICES) return 132;
   if (n[dev] == 0) {
     int v = 0;
-    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
     n[dev] = v;
   }
   return n[dev];

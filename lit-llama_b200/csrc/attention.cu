@@ -212,13 +212,12 @@ __global__ void kv_unroll_kernel(const __nv_bfloat16* __restrict__ cache, const 
 // dims (32 B) per lane, a score needs 3 shuffles.  The new token's key / value never touch the tile: they are
 // rotated, appended to the cache and scored from registers.
 // Round 1 used one 128-key tile per CTA (64 KB, 3 CTAs per SM): at position 2047 its 512 CTAs needed a second
-// wave and 16 partials per head had to be merged (profiles/r01_ncu_attn_decode_fused_kernel.txt: 0.19 of HBM
-// peak); 256 keys per CTA keep every position a single wave (<= 8 x n_head CTAs) with half the partials.
+// wave and 16 partials per head had to be merged; 256 keys per CTA keep every position a single wave (<= 8 x n_head CTAs) with half the partials.
 // ----------------------------------------------------------------------------------
 constexpr int FD_CHUNK = 256;   // most keys per CTA
 constexpr int FD_SUB = 64;      // keys per sub-tile = smallest number of keys per CTA
 constexpr int FD_WARPS = 8;
-constexpr int FD_TARGET_CTAS = 400;  // working CTAs aimed at (148 SMs x 3 resident CTAs = 444 slots: one wave)
+constexpr int FD_CTAS_PER_SM = 3;   // resident CTAs per SM (shared memory): the working CTAs aimed at are one wave of them
 constexpr int WS_CHUNK = FD_SUB;     // workspace sizing granularity (finest split of any kernel that uses it)
 
 __device__ __forceinline__ void bf16x8_to_f32(const uint4& u, float* f) {
@@ -245,7 +244,7 @@ __global__ void __launch_bounds__(FD_WARPS * 32)
                              const int64_t* __restrict__ input_pos, const int32_t* __restrict__ ring_start,
                              __nv_bfloat16* __restrict__ y, float* __restrict__ work, int* __restrict__ tickets,
                              int n_head, int S, int block_size, int n_split, unsigned long long* tl, int pre_tiles,
-                             int smem_merge) {
+                             int smem_merge, int target_ctas) {
   constexpr int HS = 128;
   extern __shared__ __align__(128) uint8_t fsm[];
   float* sm_acc = reinterpret_cast<float*>(fsm + 4 * FD_SUB_BYTES);                // [FD_WARPS][HS]
@@ -270,11 +269,11 @@ __global__ void __launch_bounds__(FD_WARPS * 32)
   const long long p = input_pos[0];
   const int w_slot = (int)(p < S ? p : (long long)S - 1);  // logical slot of the new token
   const int L = w_slot + 1;                                 // valid logical slots 0..L-1
-  // keys per CTA: a multiple of 64 in [64, 256], chosen (identically by every CTA) so that about FD_TARGET_CTAS CTAs
+  // keys per CTA: a multiple of 64 in [64, 256], chosen (identically by every CTA) so that at most target_ctas CTAs
   // have work: few long chunks would serialise sub-tiles inside a CTA, many short ones would need a second wave
-  // (measured, tools/diag.py bench_ctx: a sub-tile costs a CTA ~0.7 us, the cross-CTA merge ~3 us -- up to 256
-  // keys stay in ONE CTA per head, with no merge at all)
-  const int want_splits = max(1, FD_TARGET_CTAS / (int)gridDim.x);
+  // (a sub-tile costs a CTA much less than the cross-CTA merge, tools/diag.py bench_ctx -- up to 256 keys stay in ONE
+  // CTA per head, with no merge at all)
+  const int want_splits = max(1, target_ctas / (int)gridDim.x);
   const int chunk = L <= FD_CHUNK ? FD_CHUNK
                                   : min(FD_CHUNK, max(FD_SUB, FD_SUB * ((L + FD_SUB * want_splits - 1) / (FD_SUB * want_splits))));
   const int n_active = (L + chunk - 1) / chunk;
@@ -828,13 +827,14 @@ extern "C" int b2l_attention(void* qkv, void* k_cache, void* v_cache, const void
     // B2L_ATTN_PRE (read once): sub-tiles requested before griddepcontrol.wait, 1 (default) or 2
     static const int env_pre = [] { const char* e = getenv("B2L_ATTN_PRE"); return e ? atoi(e) : 1; }();
     // B2L_ATTN_SMEM_MERGE (read once): 1 = all 32 key groups merge through shared memory, 0 = shuffles inside a warp first
-    // (default 0: same-box A/B at position 1030, 1125.7 vs 1138.8 us per 7B token -- the extra block barrier costs more than the shuffles)
+    // (default 0: the extra block barrier of 1 is not free)
     static const int env_smem_merge = [] { const char* e = getenv("B2L_ATTN_SMEM_MERGE"); return e ? atoi(e) : 0; }();
     if (int rc = ensure_dyn_smem(attn_decode_fused_kernel, FD_SMEM_BYTES, smem_cache)) return rc;
     LaunchCfg lc(dim3(B * n_head, n_split), dim3(FD_WARPS * 32), FD_SMEM_BYTES, st, (flags & B2L_F_PDL) != 0);
     B2L_CUDA(cudaLaunchKernelEx(&lc.cfg, attn_decode_fused_kernel, (const __nv_bfloat16*)qkv, (__nv_bfloat16*)k_cache,
                                 (__nv_bfloat16*)v_cache, (const float*)rope, input_pos, ring_start, (__nv_bfloat16*)y,
-                                (float*)work, tickets, n_head, S, block_size, n_split, (unsigned long long*)g_attn_timeline, env_pre, env_smem_merge));
+                                (float*)work, tickets, n_head, S, block_size, n_split, (unsigned long long*)g_attn_timeline, env_pre, env_smem_merge,
+                                FD_CTAS_PER_SM * sm_count()));
     return 0;
   }
   int rt = head_size / 2 < 32 ? 32 : head_size / 2;

@@ -1,4 +1,4 @@
-// Shared device/host helpers for libb200llama (sm_100a only).
+// Shared device/host helpers for libb200llama (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -9,8 +9,8 @@
 
 #include "../../include/b2l.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libb200llama is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "libb200llama is written for sm_90a (H100) only"
 #endif
 
 namespace b2l {

@@ -60,7 +60,7 @@ struct Params {
 
 // One CTA per SM: 16 consumer warps + producer warp + epilogue warp.  (Two 10-warp CTAs per SM, the per-op kernels'
 // shape, were measured first: both CTAs of an SM ran the same activation prologue -- ~150 instructions per 8
-// elements, 1.6 us for K = 11008 -- and kept two copies of the digit planes; profiles/r02_mega_timeline_v1.txt.)
+// elements, 1.6 us for K = 11008 -- and kept two copies of the digit planes: tools/diag.py mega_timeline.)
 constexpr int MW = 16;                     // consumer warps
 constexpr int MT = MW * 32;                // consumer threads
 constexpr int M_PRODUCER = MW;             // warp 16
@@ -406,7 +406,7 @@ __global__ void __launch_bounds__(M_THREADS, 1) decode_mega_kernel(const Params 
           const int posB = halves == 2 ? warp : warp + MW;   // k-block position (inside a stage) of this warp's second tile
           // Two stages per round: both full-barrier waits, then 8 shared-memory loads, then 8 IMMAs, then both releases.
           // (One stage per round left each warp 4 IMMAs behind a ~250-cycle wait/load/arrive chain: measured 590
-          // cycles per 16 KB stage per SM, barely above the HBM rate; profiles/r02_mega_timeline_v2.txt.)
+          // cycles per 16 KB stage per SM, barely above the HBM rate: tools/diag.py mega_timeline.)
           // A warp's tiles sit at the same addresses for one- and two-half units: tile w and tile 16 + w of the stage.
           for (int s0 = 0; s0 < n_st; s0 += 2) {
             const bool two = s0 + 1 < n_st;

@@ -1,5 +1,5 @@
 // model.py element-wise pieces as stand-alone kernels (module-level drop-ins, prefill).
-// In the decode step these are fused into the tcgen05 linear's prologue/epilogue.
+// In the decode step these are fused into the tensor-core linears' prologue/epilogue.
 #include "b2l_common.cuh"
 
 namespace b2l {

@@ -1,4 +1,4 @@
-// Debug-only microbenchmarks (tools/diag.py): tcgen05 issue/completion costs, legacy tensor-pipe issue rates,
+// Debug-only microbenchmarks (tools/diag.py): mma.sync tensor-pipe issue rates, the decode consumer loop,
 // grid-wide flag latency.  Built into libb200diag.so (include/b2l_diag.h), NOT into the product library.
 #include "b2l_common.cuh"
 #include "../../include/b2l_diag.h"
@@ -19,169 +19,13 @@ int cuda_fail(cudaError_t e, const char* what) {
 }
 int sm_count() {
   int dev = 0, v = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
   return v;
 }
 }  // namespace b2l
 
 extern "C" const char* b2l_diag_last_error(void) { return b2l::g_diag_err; }
 
-namespace b2l {
-namespace q4tc {
-// PTX wrappers shared with q4_tc.cu (kept in sync by inclusion order: this file re-declares the few it needs)
-__device__ __forceinline__ uint32_t mb_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-}  // namespace q4tc
-
-__global__ void __launch_bounds__(128) mma_rate_kernel(unsigned long long* out, int n_mma, int n_acc, int a_from_smem, int rounds) {
-  __shared__ __align__(128) uint8_t bsm[16 * 1024];
-  __shared__ __align__(8) unsigned long long bar;
-  __shared__ uint32_t tmem_slot;
-  const int tid = threadIdx.x, warp = tid >> 5;
-  const uint32_t bar_a = q4tc::mb_smem_u32(&bar);
-  for (int i = tid; i < 16 * 1024 / 4; i += 128) reinterpret_cast<uint32_t*>(bsm)[i] = 0x3f803f80u;  // bf16 1.0
-  if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar_a) : "memory");
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 256;" ::"r"(q4tc::mb_smem_u32(&tmem_slot)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = tmem_slot;
-  // A operand in TMEM: 128 lanes x 8 columns of bf16 pairs (1.0, 1.0)
-  {
-    uint32_t taddr = tmem + ((uint32_t)(warp * 32) << 16);
-    uint32_t v = 0x3f803f80u;
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %1, %1, %1, %1, %1, %1, %1};" ::"r"(taddr), "r"(v) : "memory");
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  if (tid == 0) {
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((16u >> 3) << 17) | ((128u >> 4) << 24);
-    const uint32_t sb = q4tc::mb_smem_u32(bsm);
-    // B: K-major no-swizzle, LBO = 256 (next 8-k column), SBO = 128 (next 8 rows of N)
-    uint64_t bdesc = (uint64_t)((sb & 0x3FFFFu) >> 4) | ((uint64_t)(256 >> 4) << 16) | ((uint64_t)(128 >> 4) << 32) | ((uint64_t)1 << 46);
-    // A from smem (SS): 128 rows K-major: LBO = 2048 (next 8-k column), SBO = 128 (next 8 rows)
-    uint64_t adesc = (uint64_t)((sb & 0x3FFFFu) >> 4) | ((uint64_t)(2048 >> 4) << 16) | ((uint64_t)(128 >> 4) << 32) | ((uint64_t)1 << 46);
-    uint32_t parity = 0;
-    for (int r = 0; r < rounds; ++r) {
-      long long t0 = clock64();
-      // fully unrolled, compile-time addresses: n_mma in {1,4,16}, n_acc in {1,4}
-#define B2L_MMA(I, NACC)                                                                                                     \
-  do {                                                                                                                       \
-    const uint32_t d_ = tmem + 64 + (uint32_t)(((I) % (NACC)) * 16);                                                          \
-    if (a_from_smem)                                                                                                         \
-      asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_), \
-                   "l"(adesc), "l"(bdesc), "r"(idesc), "r"((I) >= (NACC) ? 1u : 0u) : "memory");                               \
-    else                                                                                                                     \
-      asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_), \
-                   "r"(tmem), "l"(bdesc), "r"(idesc), "r"((I) >= (NACC) ? 1u : 0u) : "memory");                                \
-  } while (0)
-#define B2L_MMA4(I, NACC) B2L_MMA(I, NACC); B2L_MMA(I + 1, NACC); B2L_MMA(I + 2, NACC); B2L_MMA(I + 3, NACC)
-      if (n_acc == 1) {
-        if (n_mma >= 1) B2L_MMA(0, 1);
-        if (n_mma >= 4) { B2L_MMA(1, 1); B2L_MMA(2, 1); B2L_MMA(3, 1); }
-        if (n_mma >= 16) { B2L_MMA4(4, 1); B2L_MMA4(8, 1); B2L_MMA4(12, 1); }
-      } else {
-        if (n_mma >= 1) B2L_MMA(0, 4);
-        if (n_mma >= 4) { B2L_MMA(1, 4); B2L_MMA(2, 4); B2L_MMA(3, 4); }
-        if (n_mma >= 16) { B2L_MMA4(4, 4); B2L_MMA4(8, 4); B2L_MMA4(12, 4); }
-      }
-      long long t1 = clock64();
-      asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar_a) : "memory");
-      long long t2 = clock64();
-      uint32_t ok;
-      do {
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                     : "=r"(ok) : "r"(bar_a), "r"(parity) : "memory");
-      } while (!ok);
-      long long t3 = clock64();
-      parity ^= 1;
-      out[r * 3 + 0] = (unsigned long long)(t1 - t0);
-      out[r * 3 + 1] = (unsigned long long)(t2 - t1);
-      out[r * 3 + 2] = (unsigned long long)(t3 - t0);
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 256;" ::"r"(tmem) : "memory");
-}
-
-
-// ---- can several threads of one CTA keep the tensor pipe fed better than one?  `n_issuers` warps (1..4) each
-// elect lane 0 to issue 16 back-to-back 128x16x16 tcgen05.mma (A in TMEM, shared; own 16-column accumulator) and
-// one commit on their own mbarrier.  out[r * 8 + w] = cycles from the common start until warp w's commit arrived,
-// out[r * 8 + 4 + w] = cycles warp w spent issuing.  If the per-warp time does not grow with n_issuers, MMA issue
-// is a per-thread limit and a multi-issuer kernel scales; if it grows linearly it is a per-SM limit.
-__global__ void __launch_bounds__(128) mma_multi_issuer_kernel(unsigned long long* out, int n_issuers, int rounds) {
-  __shared__ __align__(128) uint8_t bsm[16 * 1024];
-  __shared__ __align__(8) unsigned long long bars[4];
-  __shared__ uint32_t tmem_slot;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  for (int i = tid; i < 16 * 1024 / 4; i += 128) reinterpret_cast<uint32_t*>(bsm)[i] = 0x3f803f80u;  // bf16 1.0
-  if (tid == 0) {
-    for (int i = 0; i < 4; ++i)
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(q4tc::mb_smem_u32(&bars[i])) : "memory");
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 256;" ::"r"(q4tc::mb_smem_u32(&tmem_slot)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = tmem_slot;
-  {
-    uint32_t taddr = tmem + ((uint32_t)(warp * 32) << 16);
-    uint32_t v = 0x3f803f80u;
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %1, %1, %1, %1, %1, %1, %1};" ::"r"(taddr), "r"(v) : "memory");
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-  }
-  const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((16u >> 3) << 17) | ((128u >> 4) << 24);
-  const uint32_t sb = q4tc::mb_smem_u32(bsm);
-  const uint64_t bdesc = (uint64_t)((sb & 0x3FFFFu) >> 4) | ((uint64_t)(256 >> 4) << 16) | ((uint64_t)(128 >> 4) << 32) | ((uint64_t)1 << 46);
-  const uint32_t bar_a = q4tc::mb_smem_u32(&bars[warp]);
-  const uint32_t d = tmem + 64 + (uint32_t)(warp * 16);
-  uint32_t parity = 0;
-  for (int r = 0; r < rounds; ++r) {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    if (warp < n_issuers && lane == 0) {
-      const long long t0 = clock64();
-#pragma unroll
-      for (int i = 0; i < 16; ++i)
-        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d),
-                     "r"(tmem), "l"(bdesc), "r"(idesc), "r"(i > 0 ? 1u : 0u) : "memory");
-      const long long t1 = clock64();
-      asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar_a) : "memory");
-      uint32_t ok;
-      do {
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                     : "=r"(ok) : "r"(bar_a), "r"(parity) : "memory");
-      } while (!ok);
-      const long long t2 = clock64();
-      out[r * 8 + warp] = (unsigned long long)(t2 - t0);
-      out[r * 8 + 4 + warp] = (unsigned long long)(t1 - t0);
-    }
-    parity ^= 1;
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 256;" ::"r"(tmem) : "memory");
-}
-
-}  // namespace b2l
-
-// out: uint64[rounds * 3] = {issue cycles of n_mma MMAs, commit issue cycles, total cycles until the commit arrives}
 // ---- legacy tensor pipe: how often can one SM sub-partition issue mma.sync.m16n8k16 (HMMA.16816.F32)?
 // One CTA, `warps` warps, each with CH independent accumulator chains; optionally the 5 ALU ops per MMA
 // of the int4 unpack (1 shift + 4 LOP3 per word) in front of every MMA.
@@ -384,19 +228,5 @@ extern "C" int b2l_debug_grid_flag(void* out, void* counter, int ctas_per_sm, in
   // the caller zero-fills `counter` (uint32) and out[0 .. rounds) and fills out[rounds .. 2 rounds) with ~0
   grid_flag_kernel<<<ctas_per_sm * b2l::sm_count(), 128, 0, (cudaStream_t)stream>>>((unsigned long long*)out, (unsigned int*)counter, rounds);
   B2L_LAUNCH_CHECK("grid_flag_kernel");
-  return 0;
-}
-
-extern "C" int b2l_debug_mma_issuers(void* out, int n_issuers, int rounds, b2l_stream_t stream) {
-  B2L_CHECK_ARG(out && n_issuers >= 1 && n_issuers <= 4 && rounds > 0, "b2l_debug_mma_issuers: bad argument");
-  b2l::mma_multi_issuer_kernel<<<1, 128, 0, (cudaStream_t)stream>>>((unsigned long long*)out, n_issuers, rounds);
-  B2L_LAUNCH_CHECK("mma_multi_issuer_kernel");
-  return 0;
-}
-
-extern "C" int b2l_debug_mma_rate(void* out, int n_mma, int n_acc, int a_from_smem, int rounds, b2l_stream_t stream) {
-  B2L_CHECK_ARG(out && n_mma > 0 && n_acc > 0 && n_acc <= 8 && rounds > 0, "b2l_debug_mma_rate: bad argument");
-  b2l::mma_rate_kernel<<<1, 128, 0, (cudaStream_t)stream>>>((unsigned long long*)out, n_mma, n_acc, a_from_smem, rounds);
-  B2L_LAUNCH_CHECK("mma_rate_kernel");
   return 0;
 }

@@ -1,55 +1,46 @@
-// Prefill-shaped int4 weight-only GEMM on the 5th-generation tensor cores: y[M, N] = x[M, K] . dequant(W)[N, K]^T
+// Prefill-shaped int4 weight-only GEMM on the Hopper tensor cores (wgmma): y[M, N] = x[M, K] . dequant(W)[N, K]^T
 // for M > 16 (prompt processing, no-cache forward, evaluation; BASELINE.json configs[3] prefill 8 x 512).
 //
 // Replaces ColBlockQuantizedLinear.forward (lit_llama/quantization.py:413-423) and the Triton kernel
 // linear_kernel_4bit_weight (quantization.py:187-333: tiles up to 256 x 256, dequantise inside the tile loop) for
-// 4-bit weights with one (scale, zero) per output row.  Round 1 sent this shape to a dequantise + library GEMM.
+// 4-bit weights with one (scale, zero) per output row.
 //
-// One CTA computes a 256 (tokens) x 256 (output features) tile of y over the full K:
-//   warp 0, one elected lane: tcgen05.mma.cta_group::1.kind::f16 (bf16 x bf16 -> fp32), M = 128, N = 256, K = 16,
-//       both operands from shared memory (K-major canonical core-matrix layout, no swizzle), two accumulators
-//       (token rows 0..127 and 128..255) of 256 columns each = all 512 columns of tensor memory;
-//       tcgen05.commit releases a stage to the producers and finally hands the accumulators to the epilogue;
-//   warps 1..8 (256 threads = the 256 weight rows of the tile), per 64-wide k stage:
-//       * the activation tile [256 tokens][64 k]: ONE tensor-map TMA copy (cp.async.bulk.tensor.3d) per stage.  x is
+// One CTA computes a 128 (tokens) x 128 (output features) tile of y over the full K:
+//   warpgroups 0 and 1 (warps 0..7): wgmma.mma_async.m64n128k16 (bf16 x bf16 -> fp32), both operands from shared
+//       memory (K-major canonical core-matrix layout, no swizzle); warpgroup h owns token rows 64 h .. 64 h + 63 and
+//       keeps its 64 x 128 fp32 accumulator in registers; a stage is released to the producers once the wgmma group
+//       that read it has completed (wgmma.wait_group 1 keeps one group in flight);
+//   warpgroup 2 (warps 8..11, 128 threads = the 128 weight rows of the tile), per 64-wide k stage:
+//       * the activation tile [128 tokens][64 k]: ONE tensor-map TMA copy (cp.async.bulk.tensor.3d) per stage.  x is
 //         described to the TMA unit as a 3-D tensor (8 elements = 16 B | M rows, stride ldx | K/8 chunks, stride 16 B),
-//         so a box of 8 x 256 x 8 lands in shared memory as [k chunk][row][16 B] -- exactly the no-swizzle
-//         K-major core-matrix order tcgen05 reads; rows beyond M are zero-filled by the TMA unit;
+//         so a box of 8 x 128 x 8 lands in shared memory as [k chunk][row][16 B] -- exactly the no-swizzle
+//         K-major core-matrix order wgmma reads; rows beyond M are zero-filled by the TMA unit;
 //       * two LDG.128 of packed levels per thread (load-time tiling b2l_q4_tile: a row's 32 levels of a k slab in
 //         16 bytes, nibble order chosen so that (w >> 4s) & 0x000f000f | 0x43004300 IS the bf16 pair
 //         (128 + level[k], 128 + level[k+1])), dequantised with the reference's own rounding:
 //         level = v - 128 (exact), level - zero (bf16), * scale (bf16) -- bit-identical to get_weight
 //         (quantization.py:392-411), so the GEMM sees exactly the matrix the reference's dense branch multiplies;
 //       * 16-byte st.shared of 8 consecutive k of a row = one row of a core matrix; fence.proxy.async; mbarrier arrive;
-//   afterwards the same 8 warps are the epilogue: tcgen05.ld 32x32b (a warp reaches the TMEM lanes of its
-//   warp_id % 4 quarter), fp32 -> bf16, 32-byte stores.
-// The dequantisation costs the 8 producer warps ~400 issue cycles per stage against 1024 tensor-pipe cycles
-// (8 MMAs of 128 x 256 x 16), so the tensor pipe is the bound; a 4-deep ring (64 KB per stage) hides the loads.
+//   epilogue: each MMA thread converts its accumulator fragment to bf16 and stores pairs of output features.
 #include <cuda.h>   // CUtensorMap and its enums only: the encoder is fetched with cudaGetDriverEntryPoint (no libcuda link)
-
-#include <cstdlib>
 
 #include "b2l_common.cuh"
 
 namespace b2l {
 namespace q4gm {
 
-// NACC = accumulators = 128-token row groups per CTA: 2 (256 x 256 tile) for large problems; 1 (128 x 256) when the
-// 256-row tiling would leave the last wave of CTAs mostly empty (e.g. N = 5120, M = 4096: 320 tiles on 148 SMs)
-constexpr int BN = 256, BK = 64;
-constexpr int B_BYTES = BN * BK * 2;           // 32 KB: [8 k-columns][256 rows][16 B]
-constexpr int NPROD = 256;                     // producer threads = weight rows of the tile
-constexpr int NTHREADS = 32 + NPROD;
+constexpr int BM = 128, BN = 128, BK = 64;
+constexpr int A_BYTES = BM * BK * 2;           // 16 KB: [8 k-columns][128 token rows][16 B]
+constexpr int B_BYTES = BN * BK * 2;           // 16 KB: [8 k-columns][128 weight rows][16 B]
+constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+constexpr int NSTAGE = 4;
+constexpr int SMEM_BYTES = NSTAGE * STAGE_BYTES + 256;
+constexpr int NMMA = 256;                      // two MMA warpgroups
+constexpr int NPROD = 128;                     // producer threads = weight rows of the tile
+constexpr int NTHREADS = NMMA + NPROD;
+constexpr int LBO_A = BM * 16;                 // bytes between adjacent 8-k columns of the activation operand
 constexpr int LBO_B = BN * 16;                 // bytes between adjacent 8-k columns of the weight operand
 constexpr int SBO = 128;                       // bytes between adjacent 8-row groups
-template <int NACC> struct Cfg {
-  static constexpr int BM = 128 * NACC;
-  static constexpr int A_BYTES = BM * BK * 2;  // [8 k-columns][BM rows][16 B]
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int NSTAGE = NACC == 2 ? 3 : 4;
-  static constexpr int SMEM_BYTES = NSTAGE * STAGE_BYTES + 256;
-  static constexpr int LBO_A = BM * 16;
-};
 
 struct Params {
   CUtensorMap xmap;        // 3-D view of x (see above); must stay the first member (64-byte alignment)
@@ -79,40 +70,39 @@ __device__ __forceinline__ void mbar_wait(uint32_t a, uint32_t parity) {
         : "memory");
   } while (!ok);
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t mbar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(mbar) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]
-__device__ __forceinline__ void tc_mma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// K-major, no-swizzle shared-memory matrix descriptor (sm_100): core matrix = 8 rows x 16 B, contiguous
+// K-major, no-swizzle shared-memory matrix descriptor (sm_90 wgmma): core matrix = 8 rows x 16 B, contiguous
 __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;
   return d;
 }
-// kind::f16: D = f32, A = B = bf16 (K-major), M = 128, N = 256
-constexpr uint32_t IDESC = (1u << 4) | (1u << 7) | (1u << 10) | ((256u >> 3) << 17) | ((128u >> 4) << 24);
+// D[64 x 128] (fp32, registers) += A[64 x 16] (smem) * B[16 x 128] (smem), both K-major bf16
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+      "}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(1)
+      : "memory");
+}
+__device__ __forceinline__ void reg_fence(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
 
 __device__ __forceinline__ void mbar_expect_tx(uint32_t a, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(a), "r"(bytes) : "memory");
@@ -123,15 +113,11 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
                : "memory");
 }
 
-template <int NACC>
 __global__ void __launch_bounds__(NTHREADS, 1) q4_gemm_kernel(const __grid_constant__ Params p) {
-  constexpr int BM = Cfg<NACC>::BM, A_BYTES = Cfg<NACC>::A_BYTES, STAGE_BYTES = Cfg<NACC>::STAGE_BYTES, NSTAGE = Cfg<NACC>::NSTAGE;
-  constexpr int LBO_A = Cfg<NACC>::LBO_A;
   extern __shared__ __align__(1024) uint8_t smem[];
   const uint32_t sbase = smem_u32(smem);
-  const uint32_t bars = sbase + NSTAGE * STAGE_BYTES;      // full[NSTAGE], empty[NSTAGE], accum
-  const uint32_t bar_full = bars, bar_empty = bars + NSTAGE * 8, bar_acc = bars + 2 * NSTAGE * 8;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + NSTAGE * STAGE_BYTES + (2 * NSTAGE + 1) * 8);
+  const uint32_t bars = sbase + NSTAGE * STAGE_BYTES;      // full[NSTAGE], empty[NSTAGE]
+  const uint32_t bar_full = bars, bar_empty = bars + NSTAGE * 8;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int n0 = blockIdx.x * BN, m0 = blockIdx.y * BM;
   const int n_kt = p.K / BK;
@@ -139,43 +125,58 @@ __global__ void __launch_bounds__(NTHREADS, 1) q4_gemm_kernel(const __grid_const
   if (tid == 0) {
     for (int i = 0; i < NSTAGE; ++i) {
       mbar_init(bar_full + i * 8, NPROD / 32 + 1);   // one elected arrival per producer warp + the TMA issuer's expect_tx
-      mbar_init(bar_empty + i * 8, 1);           // tcgen05.commit
+      mbar_init(bar_empty + i * 8, NMMA / 32);       // one arrival per MMA warp once its wgmma group has completed
     }
-    mbar_init(bar_acc, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(256 * NACC) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
-  if (warp == 0) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      for (int kt = 0; kt < n_kt; ++kt) {
-        const int st = kt % NSTAGE;
-        mbar_wait(bar_full + st * 8, (uint32_t)(kt / NSTAGE) & 1u);
-        tc_fence_after();
-        const uint32_t a_base = sbase + st * STAGE_BYTES, b_base = a_base + A_BYTES;
+  if (warp < NMMA / 32) {
+    // ===================== MMA warpgroups =====================
+    const int h = warp >> 2;                       // token rows 64 h .. 64 h + 63 of the tile
+    float acc[64];
 #pragma unroll
-        for (int j = 0; j < BK / 16; ++j) {
-          const uint64_t bd = make_desc(b_base + j * 2 * LBO_B, LBO_B, SBO);
-          // token rows 0..127 -> accumulator columns 0..255, rows 128..255 -> columns 256..511
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    for (int kt = 0; kt < n_kt; ++kt) {
+      const int st = kt % NSTAGE;
+      mbar_wait(bar_full + st * 8, (uint32_t)(kt / NSTAGE) & 1u);
+      const uint32_t a_base = sbase + st * STAGE_BYTES, b_base = a_base + A_BYTES;
+      asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+      reg_fence(acc);
 #pragma unroll
-          for (int h = 0; h < NACC; ++h)
-            tc_mma_ss(tmem + 256 * h, make_desc(a_base + h * 128 * 16 + j * 2 * LBO_A, LBO_A, SBO), bd, IDESC, (kt > 0 || j > 0) ? 1u : 0u);
+      for (int j = 0; j < BK / 16; ++j)
+        wgmma_m64n128k16(acc, make_desc(a_base + h * 64 * 16 + j * 2 * LBO_A, LBO_A, SBO), make_desc(b_base + j * 2 * LBO_B, LBO_B, SBO));
+      asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+      asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");   // the group of stage kt - 1 has completed
+      reg_fence(acc);
+      if (kt > 0 && lane == 0) mbar_arrive(bar_empty + ((kt - 1) % NSTAGE) * 8);
+    }
+    asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+    reg_fence(acc);
+    // ===================== epilogue: registers -> bf16 -> y.  acc[4 c + e]: token row 16 (warp % 4) + lane / 4
+    // (+ 8 for e >= 2), output feature 8 c + 2 (lane % 4) + (e & 1)
+    const int mr = m0 + h * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int nc = n0 + 2 * (lane & 3);
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int m = mr + 8 * hh;
+      if (m >= p.M) continue;
+      __nv_bfloat16* dst = p.y + (size_t)m * p.ldy;
+#pragma unroll
+      for (int c = 0; c < BN / 8; ++c) {
+        const int n = nc + 8 * c;
+        const float v0 = acc[4 * c + 2 * hh], v1 = acc[4 * c + 2 * hh + 1];
+        if (n + 1 < p.N && ((reinterpret_cast<uintptr_t>(dst + n) & 3) == 0)) {
+          *reinterpret_cast<__nv_bfloat162*>(dst + n) = __floats2bfloat162_rn(v0, v1);
+        } else {
+          if (n < p.N) dst[n] = f2bf(v0);
+          if (n + 1 < p.N) dst[n + 1] = f2bf(v1);
         }
-        tc_commit(bar_empty + st * 8);   // the stage may be refilled once these MMAs have read it
       }
-      tc_commit(bar_acc);                // accumulators complete
     }
   } else {
-    // ===================== producers: activations (cp.async) + dequantised weights =====================
-    const int pt = tid - 32;                       // 0..255 = weight row of the tile
+    // ===================== producers: activations (TMA) + dequantised weights =====================
+    const int pt = tid - NMMA;                     // 0..127 = weight row of the tile
     const int row_n = n0 + pt;
     const int n_slab = p.K / 32;
     const bool row_ok = row_n < ((p.N + 127) / 128) * 128;     // rows inside the (128-padded) tiling
@@ -197,7 +198,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) q4_gemm_kernel(const __grid_const
       const int st = kt % NSTAGE;
       if (kt >= NSTAGE) mbar_wait(bar_empty + st * 8, (uint32_t)(kt / NSTAGE - 1) & 1u);
       const uint32_t a_base = sbase + st * STAGE_BYTES, b_base = a_base + A_BYTES;
-      // ---- activations: one tensor-map TMA copy of the whole [8 k chunks][256 rows][16 B] tile
+      // ---- activations: one tensor-map TMA copy of the whole [8 k chunks][128 rows][16 B] tile
       if (pt == 0) {
         mbar_expect_tx(bar_full + st * 8, A_BYTES);
         tma_load_3d(a_base, &p.xmap, 0, m0, kt * (BK / 8), bar_full + st * 8);
@@ -222,43 +223,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) q4_gemm_kernel(const __grid_const
       __syncwarp();
       if (lane == 0) mbar_arrive(bar_full + st * 8);
     }
-    // ===================== epilogue: TMEM -> bf16 -> y =====================
-    mbar_wait(bar_acc, 0);
-    tc_fence_after();
-    const int quarter = warp & 3;                 // TMEM lanes 32 * quarter .. + 31 are reachable from this warp
-    // two accumulators: warps 1..4 drain accumulator 0 (tokens 0..127), warps 5..8 accumulator 1, all 256 columns each;
-    // one accumulator: warps 1..4 drain columns 0..127, warps 5..8 columns 128..255
-    const int grp = (warp - 1) >> 2;
-    const int chalf = NACC == 2 ? grp : 0;
-    const int cb_lo = NACC == 2 ? 0 : grp * (BN / 32), cb_hi = NACC == 2 ? BN / 16 : cb_lo + BN / 32;
-    const int m = m0 + chalf * 128 + quarter * 32 + lane;
-#pragma unroll 1
-    for (int cb = cb_lo; cb < cb_hi; ++cb) {
-      uint32_t r[16];
-      tmem_ld16(tmem + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(chalf * 256 + cb * 16), r);
-      if (m < p.M) {
-        const int n = n0 + cb * 16;
-        __nv_bfloat16* dst = p.y + (size_t)m * p.ldy + n;
-        if (n + 16 <= p.N && ((reinterpret_cast<uintptr_t>(dst) & 15) == 0)) {
-          uint32_t o[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const __nv_bfloat162 t = __floats2bfloat162_rn(__uint_as_float(r[2 * i]), __uint_as_float(r[2 * i + 1]));
-            o[i] = *reinterpret_cast<const uint32_t*>(&t);
-          }
-          reinterpret_cast<uint4*>(dst)[0] = make_uint4(o[0], o[1], o[2], o[3]);
-          reinterpret_cast<uint4*>(dst)[1] = make_uint4(o[4], o[5], o[6], o[7]);
-        } else {
-#pragma unroll
-          for (int i = 0; i < 16; ++i)
-            if (n + i < p.N) dst[i] = f2bf(__uint_as_float(r[i]));
-        }
-      }
-    }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(256 * NACC) : "memory");
 }
 
 }  // namespace q4gm
@@ -289,18 +254,12 @@ extern "C" int b2l_q4_gemm(const b2l_q4_linear_args* a, b2l_stream_t stream) {
     set_error("b2l_q4_gemm: cuTensorMapEncodeTiled is not available from this driver");
     return B2L_E_STATE;
   }
-  // tile height: 256 token rows unless that tiling would fill the last wave of CTAs less than half (then 128)
-  const long tiles256 = (long)((a->N + BN - 1) / BN) * ((a->M + 255) / 256);
-  const int sms = sm_count();
-  static const int env_nacc = [] { const char* e = getenv("B2L_GEMM_NACC"); return e ? atoi(e) : 0; }();
-  int nacc = (a->M <= 128 || (tiles256 % sms != 0 && tiles256 % sms < sms / 2 && tiles256 < 4 * sms)) ? 1 : 2;
-  if (env_nacc == 1 || env_nacc == 2) nacc = env_nacc;
   Params p;
   {
-    // x[M, K] (leading dimension ldx) as (8 elements | M rows | K/8 chunks): a box of 8 x 256 x 8 is one stage's tile
+    // x[M, K] (leading dimension ldx) as (8 elements | M rows | K/8 chunks): a box of 8 x 128 x 8 is one stage's tile
     const cuuint64_t dims[3] = {8, (cuuint64_t)a->M, (cuuint64_t)(a->K / 8)};
     const cuuint64_t strides[2] = {(cuuint64_t)a->ldx * 2, 16};
-    const cuuint32_t box[3] = {8, (cuuint32_t)(128 * nacc), (cuuint32_t)(BK / 8)};
+    const cuuint32_t box[3] = {8, (cuuint32_t)BM, (cuuint32_t)(BK / 8)};
     const cuuint32_t estr[3] = {1, 1, 1};
     const CUresult cr = encode(&p.xmap, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(a->x), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                                CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -314,16 +273,10 @@ extern "C" int b2l_q4_gemm(const b2l_q4_linear_args* a, b2l_stream_t stream) {
   p.scales = a->scales; p.zeros = a->zeros; p.szdt = a->sz_dtype;
   p.y = (__nv_bfloat16*)a->y; p.ldy = a->ldy;
   p.M = a->M; p.N = a->N; p.K = a->K;
-  static DynSmemCache smem_cache[2];
-  if (nacc == 2) {
-    if (int rc = ensure_dyn_smem(q4_gemm_kernel<2>, Cfg<2>::SMEM_BYTES, smem_cache[1])) return rc;
-    dim3 grid((a->N + BN - 1) / BN, (a->M + 255) / 256);
-    q4_gemm_kernel<2><<<grid, NTHREADS, Cfg<2>::SMEM_BYTES, (cudaStream_t)stream>>>(p);
-  } else {
-    if (int rc = ensure_dyn_smem(q4_gemm_kernel<1>, Cfg<1>::SMEM_BYTES, smem_cache[0])) return rc;
-    dim3 grid((a->N + BN - 1) / BN, (a->M + 127) / 128);
-    q4_gemm_kernel<1><<<grid, NTHREADS, Cfg<1>::SMEM_BYTES, (cudaStream_t)stream>>>(p);
-  }
+  static DynSmemCache smem_cache;
+  if (int rc = ensure_dyn_smem(q4_gemm_kernel, SMEM_BYTES, smem_cache)) return rc;
+  dim3 grid((a->N + BN - 1) / BN, (a->M + BM - 1) / BM);
+  q4_gemm_kernel<<<grid, NTHREADS, SMEM_BYTES, (cudaStream_t)stream>>>(p);
   B2L_LAUNCH_CHECK("q4_gemm_kernel");
   return 0;
 }

@@ -18,15 +18,13 @@
 //     one LOP3 per word, and the epilogue recovers row g = D[g] - D[g+8], row g + 8 = D[g+8] / 16;
 //   * int32 accumulators cannot overflow for K <= 65536 (255 * 127 * K < 2^31); digits are recombined in int64 and
 //     the zero point is removed with the exact sum of X: y = scale * 2^-sh * (sum level X - zero * sum X).
-// Measured on B200 (tools/diag.py imma_rate / hmma_rate, profiles/r02_micro_imma_rate.txt): IMMA.16832 issues every
-// 8.1 cycles per SM sub-partition like HMMA.16816, but consumes 512 levels behind 2 LOP3 where the f16 form consumed
-// 256 behind 5 ALU ops: 10-12 issue cycles per 512 levels instead of 30.  Results no longer depend on the order of
-// the K split, carry no 1024-bias cancellation, and have no fp16 range limit on the activations.
+// An IMMA.16832 consumes 512 levels behind 2 LOP3 where the f16 form (HMMA.16816) consumes 256 behind 5 ALU ops
+// (issue rates: tools/diag.py imma_rate / hmma_rate).  Results do not depend on the order of the K split, carry no
+// 1024-bias cancellation, and have no fp16 range limit on the activations.
 //
-// Why not tcgen05 here: one thread issues a 128x16x16 tcgen05.mma every ~55 cycles (4 issuing warps: 15 cycles,
-// profiles/r02_micro_issuers_gridflag.txt), but its A operand must first be expanded to 16-bit lanes by the same
-// ALUs (>= 4 LOP3 per packed word) and handed over through tensor memory (300-500 cycles per hand-off, DESIGN.md
-// section 3); the IMMA form needs 1 LOP3 per packed word and no hand-off.  tcgen05 carries the M > 8 shapes.
+// Why not wgmma here: its A operand would first have to be expanded to 16-bit lanes by the same ALUs (>= 4 LOP3 per
+// packed word), and a 64-row wgmma tile wastes 63 of 64 rows on a single activation row; the IMMA form needs 1 LOP3
+// per packed word.  wgmma carries the M > 8 shapes.
 //
 // Data movement is unchanged from round 1: a persistent CTA owns 16-row blocks over the FULL K, a producer warp
 // streams 16 KB stages with TMA bulk copies into an mbarrier ring (issued before griddepcontrol.wait, so the

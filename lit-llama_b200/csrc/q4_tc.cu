@@ -1,5 +1,5 @@
 // Fused [RMSNorm ->] int4 weight-only linear [-> residual | SwiGLU] for M <= 16 rows
-// (decode and short prefill) on the Blackwell tensor cores.
+// (decode and short prefill) on the Hopper tensor cores (wgmma).
 //
 // Replaces, for gptq.int4 with one (scale, zero) per output row:
 //   ColBlockQuantizedLinear.forward      lit_llama/quantization.py:413-423
@@ -11,11 +11,11 @@
 // form a thread-block cluster and are reduced through distributed shared memory):
 //
 //   HBM --TMA bulk copy--> smem ring of packed slabs [128 rows][16 B = 32 nibbles]
-//       --LDS.128, LOP3--> registers: bf16 pairs (128 + level), exact
-//       --tcgen05.st-----> TMEM A operand (lane = output row, column = k pair)
+//       --LDS.128, LOP3--> registers: bf16 pairs (128 + level), exact, in the wgmma A-fragment order
 //   x (bf16, RMSNorm'd on the fly) --> smem B operand (K-major core matrices)
-//   tcgen05.mma.kind::f16  D[128 x 16] (TMEM, fp32) += A(TMEM) * B(smem)
-//   tcgen05.ld --> y[o] = scale[o] * (acc - (128 + zero[o]) * sum_k x[k])
+//   wgmma.m64nNk16 (N = 8 or 16 token columns), one warpgroup per 64 output rows:
+//       D (registers, fp32) += A (registers) * B (smem descriptor)
+//   y[o] = scale[o] * (acc - (128 + zero[o]) * sum_k x[k])
 //
 // The scale/zero are hoisted out of the K loop (exact algebra, fp32): the tensor core
 // only ever sees the integers 128..143 and the bf16 activations.
@@ -30,17 +30,11 @@ namespace q4tc {
 constexpr int TILE_N = 128;
 constexpr int SLAB_K = 32;
 constexpr int SLAB_BYTES = TILE_N * 16;  // 2048
-constexpr int G = 2;                     // slabs per stage / per A buffer
+constexpr int G = 2;                     // slabs per stage
 constexpr int STAGE_BYTES = G * SLAB_BYTES;
-constexpr int NAB = 3;                   // A buffers in TMEM
-constexpr int A_COLS = G * 16;           // 32-bit columns per A buffer (K = 64 bf16)
-constexpr int D_COL = NAB * A_COLS;      // accumulator columns start (96)
-constexpr int TMEM_COLS = 128;
-constexpr int NGROUPS = 2;               // convert warp groups, alternating stages
-constexpr int NCONV = 128 * NGROUPS;     // convert threads (warps 0..7)
-constexpr int PRODUCER_WARP = NCONV / 32;      // warp 8: TMA producer, TMEM alloc/dealloc
-constexpr int MMA_WARP = PRODUCER_WARP + 1;    // warp 9: MMA issuer
-constexpr int NTHREADS = NCONV + 64;
+constexpr int NCONV = 256;               // two MMA warpgroups (warps 0..7), 64 output rows each
+constexpr int PRODUCER_WARP = NCONV / 32;      // warp 8: TMA producer
+constexpr int NTHREADS = NCONV + 32;
 constexpr int MAX_M = 16;
 constexpr int MAX_STAGES = 16;
 constexpr int SMEM_BUDGET = 74 * 1024;   // three CTAs per SM
@@ -55,7 +49,7 @@ struct Params {
   int epilogue; const __nv_bfloat16* res; int ldres;
   int S;          // cluster size (split-K)
   int nst_ring;   // ring stages
-  int kcb;        // bytes per 8-k core-matrix column of the B operand (256, or 128 when rows 8..15 alias)
+  int kcb;        // bytes per 8-k core-matrix column of the B operand (256 for 16 token rows, 128 for 8)
   int kseg_max;   // max K elements of one rank
   unsigned long long* trace;  // debug: clock64 stamps of CTA 0 (nullptr = off)
 };
@@ -91,45 +85,6 @@ __device__ __forceinline__ void tma_bulk_g2s(uint32_t dst, const void* src, uint
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_commit(uint32_t mbar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(mbar) : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]
-__device__ __forceinline__ void tc_mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -149,7 +104,7 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-// K-major, no-swizzle shared-memory matrix descriptor (sm_100 format):
+// K-major, no-swizzle shared-memory matrix descriptor (sm_90 wgmma format):
 //   core matrix = 8 rows x 16 bytes, contiguous (128 B)
 //   LBO = byte distance between the two K halves of one K=16 MMA (next 8-k column)
 //   SBO = byte distance between 8-row groups along N
@@ -158,20 +113,43 @@ __device__ __forceinline__ uint64_t make_b_desc(uint32_t smem_addr, uint32_t lbo
   d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;  // descriptor version for sm_100
   return d;                // layout_type = 0 (no swizzle), base_offset = 0
 }
-// kind::f16, A = B = bf16 (K-major), D = f32, M = 128, N = 16
-constexpr uint32_t IDESC = (1u << 4) | (1u << 7) | (1u << 10) | ((16u >> 3) << 17) | ((128u >> 4) << 24);
 
-// 8 nibbles of one word -> 4 registers of bf16 pairs (128 + level):
-// 0x4300 is bf16 128.0 whose ulp is 1, so OR-ing a 4-bit level into the mantissa is exact.
-__device__ __forceinline__ void unpack_word(uint32_t w, uint32_t* out) {
-  out[0] = (w & 0x000f000fu) | 0x43004300u;
-  out[1] = ((w >> 4) & 0x000f000fu) | 0x43004300u;
-  out[2] = ((w >> 8) & 0x000f000fu) | 0x43004300u;
-  out[3] = ((w >> 12) & 0x000f000fu) | 0x43004300u;
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+template <int NR> __device__ __forceinline__ void reg_fence(float (&d)[NR]) {
+#pragma unroll
+  for (int i = 0; i < NR; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+
+// D[64 x NN] (fp32, registers) += A[64 x 16] (bf16, registers) * B[16 x NN] (bf16, smem, K-major)
+template <int NN> struct Wgmma;
+template <> struct Wgmma<16> {
+  static __device__ __forceinline__ void mma(float (&d)[8], const uint32_t (&a)[4], uint64_t bdesc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(1)
+        : "memory");
+  }
+};
+template <> struct Wgmma<8> {
+  static __device__ __forceinline__ void mma(float (&d)[4], const uint32_t (&a)[4], uint64_t bdesc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %9, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n8k16.f32.bf16.bf16 {%0, %1, %2, %3}, {%4, %5, %6, %7}, %8, p, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(1)
+        : "memory");
+  }
+};
+
+// Nibble pair s of one word -> the bf16 pair (128 + level[k], 128 + level[k+1]), k = 8 * word + 2 * s:
+// 0x4300 is bf16 128.0 whose ulp is 1, so OR-ing a 4-bit level into the mantissa is exact.
+__device__ __forceinline__ uint32_t unpack_pair(uint32_t w, int s) { return ((w >> (4 * s)) & 0x000f000fu) | 0x43004300u; }
 
 #define B2L_TRACE(slot)                                                      \
   do {                                                                       \
@@ -180,7 +158,7 @@ __device__ __forceinline__ void unpack_word(uint32_t w, uint32_t* out) {
 
 // ---------------------------------------------------------------- shared memory map
 struct SmemLayout {
-  uint32_t ring, xb, part, xsum, red, bars, tmem_slot, total;
+  uint32_t ring, xb, part, xsum, red, bars, total;
 };
 __host__ __device__ inline SmemLayout smem_layout(int nst_ring, int kseg_max, int kcb, int M) {
   SmemLayout L;
@@ -191,22 +169,12 @@ __host__ __device__ inline SmemLayout smem_layout(int nst_ring, int kseg_max, in
   L.xsum = o; o += MAX_M * 4;
   L.red = o;  o += (NCONV / 32) * MAX_M * 4;  // per-warp partials
   o = (o + 7u) & ~7u;
-  L.bars = o; o += (2 * MAX_STAGES + 2 * NAB + 2) * 8;
-  L.tmem_slot = o; o += 8;
+  L.bars = o; o += 2 * MAX_STAGES * 8;
   L.total = (o + 127u) & ~127u;
   return L;
 }
 
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
-}
-
+template <int NN>
 __global__ void __launch_bounds__(NTHREADS, 3) q4_linear_tc_kernel(const Params p) {
   extern __shared__ __align__(128) uint8_t smem[];
   const SmemLayout L = smem_layout(p.nst_ring, p.kseg_max, p.kcb, p.M);
@@ -226,36 +194,24 @@ __global__ void __launch_bounds__(NTHREADS, 3) q4_linear_tc_kernel(const Params 
 
   const uint32_t bar_w_full = sbase + L.bars;
   const uint32_t bar_w_empty = bar_w_full + MAX_STAGES * 8;
-  const uint32_t bar_a_full = bar_w_empty + MAX_STAGES * 8;
-  const uint32_t bar_a_empty = bar_a_full + NAB * 8;
-  const uint32_t bar_d_full = bar_a_empty + NAB * 8;
-  const uint32_t bar_x_ready = bar_d_full + 8;
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem + L.tmem_slot);
 
   if (tid == 0) B2L_TRACE(0);
   if (tid == 0) {
     for (int i = 0; i < p.nst_ring; ++i) {
       mbar_init(bar_w_full + i * 8, 1);
-      mbar_init(bar_w_empty + i * 8, 4);
+      mbar_init(bar_w_empty + i * 8, NCONV / 32);   // every MMA warp reads every slab
     }
-    for (int i = 0; i < NAB; ++i) {
-      mbar_init(bar_a_full + i * 8, 4);
-      mbar_init(bar_a_empty + i * 8, 1);
-    }
-    mbar_init(bar_d_full, 1);
-    mbar_init(bar_x_ready, 1);
     fence_barrier_init();
   }
   __syncthreads();
 
-  // ===================== TMA producer (warp 8, lane 0): stream the packed slabs of this rank ==========
-  // The first ring-full of stages is requested before anything else (TMEM allocation included):
-  // the weights do not depend on the previous kernel, and under PDL this CTA may have to wait
-  // for TMEM while the previous kernel still holds it.
-  const uint8_t* w_src = p.qwt + ((size_t)nt * slabs_total + slab0) * SLAB_BYTES;
-  const int n_first = min(nstages, p.nst_ring);
   if (warp == PRODUCER_WARP) {
+    // ===================== TMA producer (warp 8, lane 0): stream the packed slabs of this rank ==========
+    // The first ring-full of stages is requested before the dependent-launch trigger: the weights do not
+    // depend on the previous kernel.
     if (lane == 0) {
+      const uint8_t* w_src = p.qwt + ((size_t)nt * slabs_total + slab0) * SLAB_BYTES;
+      const int n_first = min(nstages, p.nst_ring);
       for (int st = 0; st < n_first; ++st) {
         const int ns = min(G, nslab - st * G);
         const uint32_t bytes = (uint32_t)ns * SLAB_BYTES;
@@ -264,18 +220,6 @@ __global__ void __launch_bounds__(NTHREADS, 3) q4_linear_tc_kernel(const Params 
         if (st < 20) B2L_TRACE(108 + st);
       }
       pdl_launch_dependents();  // the next kernel's CTAs may start prefetching their weights
-    }
-    __syncwarp();
-  }
-  if (warp == PRODUCER_WARP) tmem_alloc(sbase + L.tmem_slot, TMEM_COLS);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  if (tid == 0) B2L_TRACE(1);
-
-  if (warp == PRODUCER_WARP) {
-    if (lane == 0) {
       int slot = 0;
       uint32_t phase = 0;  // second use of slot 0 waits for its first release
       for (int st = n_first; st < nstages; ++st) {
@@ -289,45 +233,8 @@ __global__ void __launch_bounds__(NTHREADS, 3) q4_linear_tc_kernel(const Params 
       }
     }
     __syncwarp();
-  } else if (warp == MMA_WARP) {
-    // ===================== MMA issuer (whole warp converged, one elected lane issues) =====================
-    mbar_wait(bar_x_ready, 0);
-    tc_fence_after();
-    const uint32_t d_tmem = tmem_base + D_COL;
-    const uint32_t kcb16 = (uint32_t)p.kcb >> 4;
-    // descriptor of the first 8-k column; one K=16 MMA advances it by two columns
-    uint64_t bdesc = make_b_desc(sbase + L.xb, p.kcb, p.kcb == 256 ? 128 : 0);
-    uint32_t accumulate = 0;
-    int ab = 0;
-    uint32_t aphase = 0;
-    for (int st = 0; st < nstages; ++st) {
-      mbar_wait(bar_a_full + ab * 8, aphase);
-      tc_fence_after();
-      if (st < 20 && lane == 0) B2L_TRACE(64 + st);
-      const int ns = min(G, nslab - st * G);
-      if (elect_one()) {
-        const uint32_t a_tmem = tmem_base + ab * A_COLS;
-#pragma unroll
-        for (int j = 0; j < 2 * G; ++j) {
-          if (j < 2 * ns) {
-            tc_mma_ts(d_tmem, a_tmem + j * 8, bdesc + (uint64_t)(2 * j * kcb16), IDESC, accumulate);
-            accumulate = 1;
-          }
-        }
-        tc_commit(bar_a_empty + ab * 8);  // arrives when the MMAs above have read A
-      }
-      __syncwarp();
-      accumulate = 1;
-      bdesc += (uint64_t)(4 * G * kcb16);
-      if (st < 20 && lane == 0) B2L_TRACE(84 + st);
-      if (++ab == NAB) { ab = 0; aphase ^= 1; }
-    }
-    if (elect_one()) tc_commit(bar_d_full);
-    __syncwarp();
-  } else if (warp < PRODUCER_WARP) {
-    // ===================== convert warps (thread = output row of the tile; two groups alternate stages) =====
-    const int group = warp >> 2;       // 0 or 1
-    const int row = tid & (TILE_N - 1);
+  } else {
+    // ===================== MMA warpgroups (warpgroup wg = output rows 64 wg .. 64 wg + 63 of the tile) =====
     // -- activations: wait for the producing kernel, normalise, lay out as the B operand
     pdl_wait();
     if (tid == 0) B2L_TRACE(2);
@@ -436,71 +343,80 @@ __global__ void __launch_bounds__(NTHREADS, 3) q4_linear_tc_kernel(const Params 
       }
       fence_proxy_async_smem();  // B operand written with generic stores, read by the tensor core
       named_bar_sync(1, NCONV);
-      if (tid == 0) mbar_arrive(bar_x_ready);
       if (tid == 0) B2L_TRACE(3);
     }
 
-    // -- weights: smem slab -> registers -> TMEM A operand.  Group g takes stages g, g+2, ...
-    const uint32_t lane_base = (uint32_t)((warp & 3) * 32) << 16;
-    int slot = group % p.nst_ring;
-    uint32_t rphase = (group >= p.nst_ring) ? 1u : 0u;
-    int ab = group;                   // NAB == 3: (st % 3) advances by 2 each step
-    uint32_t aphase = 1;              // parity to wait on for "A buffer free"; flips when ab wraps
-    for (int st = group; st < nstages; st += NGROUPS) {
+    // -- weights: smem slab -> registers (A fragments) -> wgmma.  Thread (g = lane / 4, t = lane % 4) of warp wq of
+    // warpgroup wg holds rows r0 = 64 wg + 16 wq + g and r0 + 8; within a slab, k16 step j reads words 2j (k 0..7)
+    // and 2j + 1 (k 8..15) of those rows, nibble pair t = k 2t, 2t + 1 of each.
+    const int r0 = (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2), tq = lane & 3;
+    float acc[NN / 2];
+#pragma unroll
+    for (int i = 0; i < NN / 2; ++i) acc[i] = 0.f;
+    const uint64_t bdesc0 = make_b_desc(sbase + L.xb, p.kcb, 128);
+    const uint32_t kcb16 = (uint32_t)p.kcb >> 4;   // descriptor address units per 8-k column
+    int slot = 0;
+    uint32_t rphase = 0;
+    for (int st = 0; st < nstages; ++st) {
       const int ns = min(G, nslab - st * G);
       mbar_wait(bar_w_full + slot * 8, rphase);
       if (tid == 0 && st < 20) B2L_TRACE(4 + st);
-      uint4 wv[G];
-#pragma unroll
-      for (int s = 0; s < G; ++s)
-        if (s < ns) wv[s] = *reinterpret_cast<const uint4*>(smem + L.ring + slot * STAGE_BYTES + s * SLAB_BYTES + row * 16);
-      mbar_wait(bar_a_empty + ab * 8, aphase);
-      tc_fence_after();
-      if (tid == 0 && st < 20) B2L_TRACE(24 + st);
+      uint32_t a[G][2][4];
 #pragma unroll
       for (int s = 0; s < G; ++s) {
         if (s < ns) {
-          uint32_t r[16];
-          unpack_word(wv[s].x, r + 0);
-          unpack_word(wv[s].y, r + 4);
-          unpack_word(wv[s].z, r + 8);
-          unpack_word(wv[s].w, r + 12);
-          tmem_st16(tmem_base + lane_base + ab * A_COLS + s * 16, r);
+          const uint8_t* sl = smem + L.ring + slot * STAGE_BYTES + s * SLAB_BYTES;
+          const uint4 lo = *reinterpret_cast<const uint4*>(sl + r0 * 16);
+          const uint4 hi = *reinterpret_cast<const uint4*>(sl + (r0 + 8) * 16);
+          a[s][0][0] = unpack_pair(lo.x, tq); a[s][0][1] = unpack_pair(hi.x, tq);
+          a[s][0][2] = unpack_pair(lo.y, tq); a[s][0][3] = unpack_pair(hi.y, tq);
+          a[s][1][0] = unpack_pair(lo.z, tq); a[s][1][1] = unpack_pair(hi.z, tq);
+          a[s][1][2] = unpack_pair(lo.w, tq); a[s][1][3] = unpack_pair(hi.w, tq);
         }
       }
-      tmem_wait_st();
-      tc_fence_before();
       __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(bar_w_empty + slot * 8);  // slab bytes are in registers/TMEM: slot may be refilled
-        mbar_arrive(bar_a_full + ab * 8);
+      if (lane == 0) mbar_arrive(bar_w_empty + slot * 8);  // slab bytes are in registers: slot may be refilled
+      wgmma_fence();
+      reg_fence(acc);
+#pragma unroll
+      for (int s = 0; s < G; ++s) {
+        if (s < ns) {
+#pragma unroll
+          for (int j = 0; j < 2; ++j) {
+            const uint32_t kstep = (uint32_t)((st * G + s) * 2 + j);   // k16 step within this rank's segment
+            Wgmma<NN>::mma(acc, a[s][j], bdesc0 + (uint64_t)(2 * kstep * kcb16));
+          }
+        }
       }
+      wgmma_commit();
+      wgmma_wait_all();   // the A registers are rewritten next stage
+      reg_fence(acc);
       if (tid == 0 && st < 20) B2L_TRACE(44 + st);
-      slot += NGROUPS;
-      while (slot >= p.nst_ring) { slot -= p.nst_ring; rphase ^= 1; }
-      ab += NGROUPS;
-      if (ab >= NAB) { ab -= NAB; aphase ^= 1; }
+      if (++slot == p.nst_ring) { slot = 0; rphase ^= 1; }
     }
 
-    // -- epilogue part 1 (group 0): accumulator -> scaled partial of this rank
-    if (group == 0) {
-      mbar_wait(bar_d_full, 0);
-      tc_fence_after();
-      if (tid == 0) B2L_TRACE(104);
-      uint32_t acc[16];
-      tmem_ld16(tmem_base + lane_base + D_COL, acc);
+    // -- epilogue part 1: accumulator -> scaled partial of this rank.  acc[4 c + e] = row r0 (+ 8 for e >= 2),
+    // token column 8 c + 2 tq + (e & 1)
+    float* part = reinterpret_cast<float*>(smem + L.part);
+    if (tid == 0) B2L_TRACE(104);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = r0 + 8 * h;
       const int o = min(nt * TILE_N + row, p.N - 1);  // padded rows of the last tile are never stored
       const float sc = load_sz(p.scales, p.szdt, o);
       const float zz = 128.0f + load_sz(p.zeros, p.szdt, o);
-      float* part = reinterpret_cast<float*>(smem + L.part);
 #pragma unroll
-      for (int m = 0; m < MAX_M; ++m)
-        if (m < p.M) part[m * TILE_N + row] = sc * (__uint_as_float(acc[m]) - zz * xsum[m]);
+      for (int c = 0; c < NN / 8; ++c) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int m = 8 * c + 2 * tq + e;
+          if (m < p.M) part[m * TILE_N + row] = sc * (acc[4 * c + 2 * h + e] - zz * xsum[m]);
+        }
+      }
     }
   }
 
-  // ===================== cross-rank reduction + epilogue (rank 0, group 0) =====================
-  tc_fence_before();
+  // ===================== cross-rank reduction + epilogue (rank 0, warps 0..3: thread = output row) ==========
   if (S > 1) cluster_sync_all(); else __syncthreads();
   if (tid == 0) B2L_TRACE(105);
   if (rank == 0 && warp < 4) {
@@ -546,8 +462,7 @@ __global__ void __launch_bounds__(NTHREADS, 3) q4_linear_tc_kernel(const Params 
     }
   }
   if (tid == 0) B2L_TRACE(106);
-  if (S > 1) cluster_sync_all(); else __syncthreads();
-  if (warp == PRODUCER_WARP) tmem_dealloc(tmem_base, TMEM_COLS);
+  if (S > 1) cluster_sync_all();   // peers keep their partials alive until rank 0 has read them
   if (tid == 0) B2L_TRACE(107);
 }
 
@@ -677,7 +592,7 @@ extern "C" int b2l_q4_linear_tc(const b2l_q4_linear_args* a, b2l_stream_t stream
   p.trace = (unsigned long long*)a->trace;
   const int max_slabs = (slabs_total + S - 1) / S;
   p.kseg_max = max_slabs * SLAB_K;
-  p.kcb = (!(a->flags & B2L_F_NO_ALIAS_N) && a->M <= 8) ? 128 : 256;  // rows 8..15 of B alias rows 0..7
+  p.kcb = (!(a->flags & B2L_F_NO_ALIAS_N) && a->M <= 8) ? 128 : 256;  // 8 or 16 token rows in the B operand
   B2L_CHECK_SUPPORTED(p.kseg_max <= 2 * NCONV * 8, "b2l_q4_linear_tc: K/split_k = %d > %d: raise split_k (K=%d, split_k=%d)",
                       p.kseg_max, 2 * NCONV * 8, a->K, S);
   const int stages_needed = (max_slabs + G - 1) / G;
@@ -691,9 +606,14 @@ extern "C" int b2l_q4_linear_tc(const b2l_q4_linear_args* a, b2l_stream_t stream
   const SmemLayout L = smem_layout(p.nst_ring, p.kseg_max, p.kcb, p.M);
   B2L_CHECK_SUPPORTED(L.total <= 200 * 1024, "b2l_q4_linear_tc: shared memory %u B too large (K=%d, split_k=%d)", L.total, a->K, S);
 
-  static DynSmemCache smem_cache;
-  if (int rc = ensure_dyn_smem(q4_linear_tc_kernel, L.total, smem_cache)) return rc;
+  static DynSmemCache smem_cache[2];
   LaunchCfg lc(dim3(n_tiles * S), dim3(NTHREADS), L.total, (cudaStream_t)stream, (a->flags & B2L_F_PDL) != 0, S);
-  B2L_CUDA(cudaLaunchKernelEx(&lc.cfg, q4_linear_tc_kernel, p));
+  if (p.kcb == 256) {   // 16 token columns per MMA
+    if (int rc = ensure_dyn_smem(q4_linear_tc_kernel<16>, L.total, smem_cache[1])) return rc;
+    B2L_CUDA(cudaLaunchKernelEx(&lc.cfg, q4_linear_tc_kernel<16>, p));
+  } else {              // at most 8 token rows: n8 MMAs on an 8-row B operand
+    if (int rc = ensure_dyn_smem(q4_linear_tc_kernel<8>, L.total, smem_cache[0])) return rc;
+    B2L_CUDA(cudaLaunchKernelEx(&lc.cfg, q4_linear_tc_kernel<8>, p));
+  }
   return 0;
 }

@@ -1,7 +1,7 @@
 // Generic ColBlockQuantizedLinear kernels: read the reference storage directly
 // (quantization.py:350-369): uint8 [in/epb][out] row-major, scales/zeros [out][n_groups].
 // Any bits in {4,8}, any tile_cols, any M.  This is the always-correct path; the
-// tcgen05 kernel in q4_tc.cu is the fast path for bits=4 / one group per row.
+// wgmma kernel in q4_tc.cu is the fast path for bits=4 / one group per row.
 #include "b2l_common.cuh"
 
 namespace b2l {

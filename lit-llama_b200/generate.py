@@ -1,4 +1,4 @@
-"""generate.py of the reference (generate.py:20-91, 94-155) over the B200 modules.
+"""generate.py of the reference (generate.py:20-91, 94-155) over the H100 modules.
 
 `generate()` keeps the reference's Python token loop and torch sampling ops (so the
 RNG stream of `torch.multinomial` is the reference's); the model call inside it is one

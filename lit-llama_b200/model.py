@@ -3,14 +3,14 @@
 Same classes, constructor signatures, parameter/buffer names and forward signatures as
 the reference, so `with quantization(mode): model = LLaMA.from_name(name)` followed by
 `model.load_state_dict(checkpoint)` and the reference's `generate()` work unchanged.
-Every forward runs hand-written sm_100a kernels (include/b2l.h); tensors must be CUDA
+Every forward runs hand-written sm_90a kernels (include/b2l.h); tensors must be CUDA
 bf16 - there is no CPU fallback.
 
 Two execution paths behind `LLaMA.forward`:
   * decode (T == 1 with a KV cache, every Linear a gptq.int4 layer with one (scale, zero) per row):
     one C call enqueues the whole token (`b2l_decode_step`: int8-MMA GEMV kernels for batch 1, f16-MMA for 2..8 rows,
-    tcgen05 for 9..16), replayed as a CUDA graph.
-  * everything else (prefill on the tcgen05 GEMM, no-cache forward, other Linear kinds): module by module.
+    wgmma for 9..16), replayed as a CUDA graph.
+  * everything else (prefill on the wgmma GEMM, no-cache forward, other Linear kinds): module by module.
 """
 import ctypes as C
 import math
@@ -252,7 +252,7 @@ class _DecodeState:
 
         from .quantization import BATCH_GEMV, batch_workspace
 
-        # batch 1..8: mma.sync kernels (q4_gemv / q4_gemv_batch) and their tiling; 9..16: tcgen05 kernel and its tiling
+        # batch 1..8: mma.sync kernels (q4_gemv / q4_gemv_batch) and their tiling; 9..16: wgmma kernel and its tiling
         gemv = (B == 1) or (B <= 8 and BATCH_GEMV)
         self.batch_ws = None
         if gemv and B > 1:
@@ -322,8 +322,7 @@ class LLaMA(nn.Module):
     #: return a fresh logits tensor per call like the reference (False: a view of the static buffer)
     copy_logits: bool = True
     #: batch-1 decode (head_size 128) as ONE persistent kernel per token (csrc/decode_mega.cu) instead of one kernel
-    #: per op.  Opt-in (B2L_PERSISTENT=1): measured on B200 it is correct but slower than the per-op path under
-    #: programmatic dependent launch (DESIGN.md section 4: 1330 vs 964 us per 7B token).
+    #: per op.  Opt-in (B2L_PERSISTENT=1): the default is the per-op path under programmatic dependent launch.
     persistent: bool = os.environ.get("B2L_PERSISTENT", "0") == "1"
 
     def __init__(self, config: LLaMAConfig) -> None:
@@ -383,7 +382,7 @@ class LLaMA(nn.Module):
     # ------------------------------------------------------------------ helpers
     def _fc12(self, i: int, kind: str):
         """c_fc1 and c_fc2 of layer i interleaved (8 rows / 8 rows per 16-row block for the
-        batch-1 kernel, 64 / 64 per 128-row tile for the tcgen05 kernel) and re-tiled, so one
+        batch-1 kernel, 64 / 64 per 128-row tile for the wgmma kernel) and re-tiled, so one
         tile holds silu's argument and its multiplier and SwiGLU runs in the epilogue."""
         mlp = self.transformer.h[i].mlp
         gemv = kind != "tc"

@@ -1,4 +1,4 @@
-"""Plug the B200 modules into an UNMODIFIED reference checkout.
+"""Plug the H100 modules into an UNMODIFIED reference checkout.
 
 The reference resolves its classes through module globals at construction time
 (lit_llama/model.py:61,152,154 and the torch.nn.Linear swap of utils.py:156-162 - the
@@ -7,7 +7,7 @@ same trick its own lora() context uses, lit_llama/lora.py:472-476).  After
     import lit_llama, lit_llama_b200
     lit_llama_b200.patch_reference(lit_llama)
 
-the reference's own `generate.py` (`main()`, `--quantize gptq.int4`) builds B200
+the reference's own `generate.py` (`main()`, `--quantize gptq.int4`) builds H100
 modules: `lit_llama.LLaMA`, `lit_llama.model.{LLaMA,Block,CausalSelfAttention,MLP,
 RMSNorm,apply_rope,build_rope_cache}`, `lit_llama.quantization.{ColBlockQuantizedLinear,
 Linear8bitLt}` and `lit_llama.utils.{quantization,EmptyInitOnDevice,lazy_load}`
@@ -45,7 +45,7 @@ def patch_reference(lit_llama_module=None):
     ref_quant.qlinear_4bit_weight = q.qlinear_4bit_weight
     # The offline converter stays the reference's own (quantize/gptq.py + quantization.GPTQQuantizer, host-side torch,
     # out of the decode path): it builds `ColBlockQuantizedLinear` through the name patched above and calls
-    # pack_weight(), so it converts straight into B200 modules.
+    # pack_weight(), so it converts straight into H100 modules.
     for name in ("EmptyInitOnDevice", "lazy_load"):
         saved[("utils", name)] = getattr(ref_utils, name, None)
         setattr(ref_utils, name, getattr(u, name))

@@ -3,8 +3,8 @@
 `ColBlockQuantizedLinear` keeps the reference's constructor, attributes, buffers
 (names, shapes, dtypes, strides) and `state_dict` keys (quantization.py:340-374), so a
 `llama-gptq.4bit.pth` produced by the reference's quantize/gptq.py loads unchanged.
-`forward` runs hand-written sm_100a kernels through the C ABI of include/b2l.h (M = 1: exact int8-digit MMA GEMV;
-2..8: f16 MMA batch kernel; 9..16: tcgen05 from tensor memory; > 16: tcgen05 256 x 256 tile GEMM); there is no
+`forward` runs hand-written sm_90a kernels through the C ABI of include/b2l.h (M = 1: exact int8-digit MMA GEMV;
+2..8: f16 MMA batch kernel; 9..16: wgmma with weights from registers; > 16: wgmma 128 x 128 tile GEMM); there is no
 Triton, no library GEMM, no dense fallback and no CPU path.
 """
 import ctypes as C
@@ -16,7 +16,7 @@ import torch
 from . import _lib as L
 
 
-# 2..8 activation rows go through the mma.sync batch kernel (B2L_BATCH_GEMV=0: tcgen05 kernel instead)
+# 2..8 activation rows go through the mma.sync batch kernel (B2L_BATCH_GEMV=0: wgmma kernel instead)
 BATCH_GEMV = os.environ.get("B2L_BATCH_GEMV", "1") != "0"
 _BATCH_WS = {}
 _BATCH_WS_OLD = []
@@ -181,7 +181,7 @@ class ColBlockQuantizedLinear(torch.nn.Module):
 
     @property
     def tc_capable(self) -> bool:
-        """Eligible for the tcgen05 kernel: 4 bits, one (scale, zero) per row, K % 32 == 0, no bias."""
+        """Eligible for the wgmma kernels: 4 bits, one (scale, zero) per row, K % 32 == 0, no bias."""
         return (self.bits == 4 and self.scales.shape[1] == 1 and self.in_features % 32 == 0 and self.bias is None
                 and self.zeros.dtype == self.scales.dtype)
 
@@ -280,7 +280,7 @@ class ColBlockQuantizedLinear(torch.nn.Module):
                 ldres=0, split_k=0, flags=0)
             L.check(L.lib().b2l_q4_linear_tc(C.byref(a), L.stream_ptr()), "b2l_q4_linear_tc")
         elif self.tc_capable and aligned and K % 64 == 0:
-            # prefill-shaped: 256 x 256 tcgen05 tiles, weights dequantised on the fly with get_weight's roundings
+            # prefill-shaped: 128 x 128 wgmma tiles, weights dequantised on the fly with get_weight's roundings
             wt = self.tiled()
             a = L.Q4LinearArgs(
                 x=x.data_ptr(), ldx=x.stride(0), qw_tiled=wt.data_ptr(), scales=self.scales.data_ptr(),

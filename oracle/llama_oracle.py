@@ -13,9 +13,9 @@ build container by `oracle/make_golden.py`, whose outputs are committed under
 `tests/test_oracle_golden.py`.  The gptq.int4/int8 + model.py + generate.py part
 is pinned that way.  The llm.int8 part restates the published bitsandbytes
 LLM.int8() algorithm (bitsandbytes is unpinned in pyproject.toml:19, absent from
-/root/reference and not installed) and is therefore **parity unpinned**.
+the reference checkout and not installed) and is therefore **parity unpinned**.
 
-Every function cites the reference lines (relative to /root/reference) it follows.
+Every function cites the reference lines (relative to the reference checkout) it follows.
 """
 from __future__ import annotations
 

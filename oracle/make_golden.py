@@ -1,10 +1,10 @@
 """Generates tests/golden/*.pt by running the UNMODIFIED reference on the CPU.
 
-Run in the build container only (needs /root/reference):
+Needs the lit-llama checkout (default /root/reference; LIT_LLAMA_DIR overrides it):
 
     python oracle/make_golden.py
 
-The reference is imported from /root/reference with oracle/_shim on sys.path (a
+The reference is imported from that checkout with oracle/_shim on sys.path (a
 stand-in for the absent `lightning` package, which the decode path never calls).
 The fixtures pin oracle/llama_oracle.py (tests/test_oracle_golden.py) and are the
 vectors the GPU parity tests compare the CUDA path against.  TEST INFRASTRUCTURE.
@@ -16,7 +16,7 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-REF = os.environ.get("B2L_REFERENCE", "/root/reference")
+REF = os.environ.get("LIT_LLAMA_DIR", "/root/reference")
 sys.path.insert(0, os.path.join(HERE, "_shim"))
 sys.path.insert(0, REF)
 sys.path.insert(0, ROOT)
@@ -164,8 +164,37 @@ def golden_dense_model():
     torch.save(dict(cfg=cfg, seed=3, prompt=prompt, gen=y), os.path.join(OUT, "tiny_dense_f32.pt"))
 
 
+def golden_surface():
+    """The reference's import surface that patch_reference() rewires: for the package, its model / quantization /
+    utils modules and generate.py, every class or function they bind, as `name -> "defining_module.qualname"`
+    (names bound to the same object share the origin).  tests/test_modules_cpu.py rebuilds these namespaces from it."""
+    import json
+
+    import lit_llama
+    import lit_llama.model
+    import lit_llama.quantization
+    import lit_llama.utils
+
+    mods = {"pkg": lit_llama, "model": lit_llama.model, "quant": lit_llama.quantization, "utils": lit_llama.utils,
+            "generate": ref_generate}
+    out = {}
+    for key, mod in mods.items():
+        names = {}
+        for name, obj in sorted(vars(mod).items()):
+            origin = getattr(obj, "__module__", None)
+            if name.startswith("__") or not callable(obj) or not isinstance(origin, str):
+                continue
+            if origin.startswith("lit_llama") or origin == mod.__name__:
+                names[name] = f"{origin}.{getattr(obj, '__qualname__', name)}"
+        out[key] = names
+    with open(os.path.join(OUT, "reference_surface.json"), "w") as f:
+        json.dump({"modules": out}, f, indent=1, sort_keys=True)
+        f.write("\n")
+
+
 def main():
     os.makedirs(OUT, exist_ok=True)
+    golden_surface()
     torch.manual_seed(0)
     torch.save(golden_quant(), os.path.join(OUT, "quant_cases.pt"))
     torch.save(golden_ops(), os.path.join(OUT, "ops.pt"))

@@ -225,7 +225,7 @@ def test_gemv_13b_65b_shapes(dev, name, N, K):
 @pytest.mark.parametrize("M,N,K", [(17, 256, 64), (100, 384, 128), (300, 130, 256), (256, 512, 512), (257, 768, 256), (1000, 4096, 4096),
                                    (64, 32000, 4096), (4096, 15360, 5120), (4096, 5120, 13824)])
 def test_q4_gemm_prefill_shapes(dev, M, N, K):
-    """The tcgen05 prefill GEMM (M > 16) against the reference's dense branch evaluated by torch in fp32 on the SAME
+    """The wgmma prefill GEMM (M > 16) against the reference's dense branch evaluated by torch in fp32 on the SAME
     bf16-rounded dequantised matrix (quantization.py:392-423: get_weight rounds (level - zero) * scale to bf16, F.linear
     accumulates): ragged M / N tiles, one k stage, the 13B widths of BASELINE configs[3] at M = 8 x 512."""
     import ctypes as C
@@ -279,7 +279,7 @@ def test_tc_linear_7b_shapes(dev, name, N, K):
     y1, err = gemv_call(L, x[0:1], tile_i8(L, qw, N, K), sc, z, N, K)
     assert err is None, err
     assert relerr(y1, want[0:1]) < 1e-3 + 2.0 ** -9
-    # two independent kernels: same bf16 results up to 1-ulp flips (the tcgen05 kernel accumulates (128 + level) * x
+    # two independent kernels: same bf16 results up to 1-ulp flips (the wgmma kernel accumulates (128 + level) * x
     # in fp32, the batch-1 kernel is exact: a percent or two of outputs sit on the other side of a rounding boundary)
     assert float((y1 == want[0:1].float().bfloat16()).float().mean()) > 0.995
     assert float((y1 == y[0:1]).float().mean()) > 0.9

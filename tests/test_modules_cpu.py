@@ -13,9 +13,6 @@ import lit_llama_b200 as P
 from lit_llama_b200.utils import quantization
 from oracle import llama_oracle as O
 
-REF = "/root/reference"
-
-
 def test_find_multiple_and_lookup():
     for n, k, want in load_golden("ops.pt")["find_multiple"]:
         assert P.find_multiple(n, k) == want
@@ -104,34 +101,51 @@ def test_product_does_not_import_the_oracle():
                 assert "oracle" not in src, f"{f} references oracle/"
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference checkout not present")
 def test_patch_reference_plugs_into_unmodified_reference():
-    here = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    sys.path.insert(0, os.path.join(here, "oracle", "_shim"))
-    sys.path.insert(0, REF)
-    import lit_llama
-    import lit_llama.quantization  # noqa: F401
-    import generate as ref_generate
+    """patch_reference() against the import surface of the unmodified reference (tests/golden/reference_surface.json,
+    recorded from lit-llama by oracle/make_golden.py): the package, its model / quantization / utils modules and
+    generate.py are rebuilt with one stand-in object per reference class or function (names bound to the same object
+    share it), so every name the patch rewires must exist there, and every alias generate.py holds must follow."""
+    import json
+    import types
 
-    saved = P.patch_reference(lit_llama)
+    surface = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_surface.json")))["modules"]
+    objs = {}
+
+    def stand_in(origin):
+        return objs.setdefault(origin, type(origin.rsplit(".", 1)[-1], (), {"origin": origin}))
+
+    pkg = "lit_llama_surface"
+    mods = {"pkg": pkg, "model": pkg + ".model", "quant": pkg + ".quantization", "utils": pkg + ".utils", "generate": pkg + "_generate"}
+    mods = {key: types.ModuleType(name) for key, name in mods.items()}
+    for key, names in surface.items():
+        for name, origin in names.items():
+            setattr(mods[key], name, stand_in(origin))
+    ref = {key: dict(vars(mod)) for key, mod in mods.items()}
+    sys.modules.update({mod.__name__: mod for mod in mods.values()})
     try:
-        from lit_llama.utils import quantization as ref_q
-        from lit_llama.model import LLaMA as RefLLaMA, LLaMAConfig as RefCfg
+        saved = P.patch_reference(mods["pkg"])
+        from lit_llama_b200 import int8, quantization as q, utils as u
 
-        assert RefLLaMA is P.LLaMA and ref_generate.LLaMA is P.LLaMA
-        with ref_q("gptq.int4"):
-            m = RefLLaMA(RefCfg(block_size=16, vocab_size=64, n_layer=1, n_head=2, n_embd=64))
+        for name in ("LLaMA", "LLaMAConfig", "Block", "CausalSelfAttention", "MLP", "RMSNorm", "apply_rope", "build_rope_cache"):
+            assert getattr(mods["model"], name) is getattr(P, name) and saved[("model", name)] is ref["model"][name]
+            if name in ref["pkg"]:
+                assert getattr(mods["pkg"], name) is getattr(P, name)
+        assert mods["quant"].ColBlockQuantizedLinear is P.ColBlockQuantizedLinear
+        assert mods["quant"].qlinear_4bit_weight is q.qlinear_4bit_weight and mods["quant"].Linear8bitLt is int8.Linear8bitLt
+        assert mods["quant"].GPTQQuantizer is ref["quant"]["GPTQQuantizer"]   # the offline converter stays the reference's
+        for name in ("quantization", "EmptyInitOnDevice", "lazy_load"):
+            assert getattr(mods["utils"], name) is getattr(u, name) and saved[("utils", name)] is ref["utils"][name]
+        # generate.py imported LLaMA and quantization by name: the patch follows those aliases
+        assert mods["generate"].LLaMA is P.LLaMA and mods["generate"].quantization is u.quantization
+        assert mods["generate"].generate is ref["generate"]["generate"]
+        with mods["utils"].quantization("gptq.int4"):
+            m = mods["model"].LLaMA(mods["model"].LLaMAConfig(block_size=16, vocab_size=64, n_layer=1, n_head=2, n_embd=64))
         assert isinstance(m, P.LLaMA) and isinstance(m.lm_head, P.ColBlockQuantizedLinear)
         assert isinstance(m.transformer.h[0], P.Block)
     finally:
-        import lit_llama.model as rm, lit_llama.utils as ru, lit_llama.quantization as rq
-
-        for (where, name), val in saved.items():
-            tgt = {"model": rm, "pkg": lit_llama, "quant": rq, "utils": ru}[where]
-            if val is not None:
-                setattr(tgt, name, val)
-        ref_generate.LLaMA = saved[("model", "LLaMA")]
-        ref_generate.quantization = saved[("utils", "quantization")]
+        for mod in mods.values():
+            sys.modules.pop(mod.__name__, None)
 
 
 def test_linear8bitlt_contract_on_cpu():

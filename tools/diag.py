@@ -14,7 +14,7 @@ import time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-SECTIONS = ["generic", "tile", "tc_small", "tc_shapes", "tc_modes", "gemv", "mma_rate", "mma_issuers", "grid_flag", "hmma_rate", "imma_rate", "consumer_rate", "bench_gemm", "trace", "bench_layers", "bench_gemv", "bench_step", "bench_ctx", "bench_13b_b8", "bench_sizes", "batch_debug", "bench_step_int8", "timeline", "mega_timeline"]
+SECTIONS = ["generic", "tile", "tc_small", "tc_shapes", "tc_modes", "gemv", "grid_flag", "hmma_rate", "imma_rate", "consumer_rate", "bench_gemm", "bench_tc", "trace", "bench_layers", "bench_gemv", "bench_step", "bench_ctx", "bench_13b_b8", "bench_sizes", "batch_debug", "bench_step_int8", "timeline", "mega_timeline"]
 
 
 _DLIB = None
@@ -26,8 +26,7 @@ def dlib():
     if _DLIB is None:
         h = C.CDLL(os.path.join(ROOT, "tools", "libb200diag.so"))
         vp, ci = C.c_void_p, C.c_int
-        for name, args in {"b2l_debug_mma_rate": [vp, ci, ci, ci, ci, vp], "b2l_debug_mma_issuers": [vp, ci, ci, vp],
-                           "b2l_debug_grid_flag": [vp, vp, ci, ci, vp], "b2l_debug_hmma_rate": [vp, ci, ci, ci, ci, vp],
+        for name, args in {"b2l_debug_grid_flag": [vp, vp, ci, ci, vp], "b2l_debug_hmma_rate": [vp, ci, ci, ci, ci, vp],
                            "b2l_debug_imma_rate": [vp, ci, ci, ci, ci, vp],
                            "b2l_debug_consumer_rate": [vp, ci, ci, ci, ci, vp]}.items():
             getattr(h, name).restype = ci
@@ -310,7 +309,7 @@ def sec_tc_small():
     print(f"  N=128 K=64 M=1 S=1 relerr={relerr(y, want):.3e}")
     print("  got ", [round(float(v), 4) for v in y[0, :6]])
     print("  want", [round(float(v), 4) for v in want[0, :6]])
-    # hypotheses if wrong: pair order swapped inside a TMEM column / B rows
+    # hypotheses if wrong: pair order swapped inside an A fragment / B rows
     xs = x.clone().reshape(M, K // 2, 2).flip(-1).reshape(M, K)
     print(f"  hypothesis pair-swapped relerr={relerr(y, ref_linear(xs, lv, sc, z)):.3e}")
     xh = x.clone().reshape(M, K // 16, 2, 8).flip(2).reshape(M, K)
@@ -423,41 +422,6 @@ def make_args(L, x, qt, scales, zeros, N, K, y, *, prologue=0, norm_scale=None, 
                           split_k=split_k, flags=flags, trace=None if trace is None else trace.data_ptr())
 
 
-def sec_mma_rate():
-    import torch
-    from lit_llama_b200 import _lib as L
-
-    dev = torch.device("cuda")
-    out = torch.zeros(64 * 3, dtype=torch.int64, device=dev)
-    for a_smem in (0, 1):
-        for n_acc in (1, 4):
-            for n_mma in (1, 4, 16):
-                out.zero_()
-                dcheck(dlib().b2l_debug_mma_rate(out.data_ptr(), n_mma, n_acc, a_smem, 8, L.stream_ptr()), "mma_rate")
-                torch.cuda.synchronize()
-                o = out.cpu().reshape(-1, 3)[:8]
-                r = o[3:].float().mean(0)  # skip cold rounds
-                print(f"A_from_{'smem' if a_smem else 'tmem'} n_acc={n_acc} n_mma={n_mma:3d}: issue={r[0]:.0f} cyc ({r[0] / n_mma:.1f}/mma) "
-                      f"commit_issue={r[1]:.0f} total_until_arrive={r[2]:.0f} ({r[2] / n_mma:.1f}/mma)")
-
-
-def sec_mma_issuers():
-    """tcgen05.mma issue from 1..4 threads of one CTA at once (round-2 question: does a multi-issuer kernel scale?)."""
-    import torch
-    from lit_llama_b200 import _lib as L
-
-    dev = torch.device("cuda")
-    rounds = 6
-    out = torch.zeros(rounds * 8, dtype=torch.int64, device=dev)
-    for n in (1, 2, 3, 4):
-        out.zero_()
-        dcheck(dlib().b2l_debug_mma_issuers(out.data_ptr(), n, rounds, L.stream_ptr()), "mma_issuers")
-        torch.cuda.synchronize()
-        o = out.view(rounds, 8).cpu()
-        print(f"issuers={n}: last round, cycles until commit per warp {o[-1, :n].tolist()}  issue cycles {o[-1, 4:4 + n].tolist()}  "
-              f"-> {float(o[-1, :n].max()) / (16 * n):.1f} cycles per MMA overall", flush=True)
-
-
 def sec_grid_flag():
     """Grid-wide arrive-and-wait through a global counter: the cost of a dependency without a kernel boundary."""
     import torch
@@ -526,19 +490,20 @@ def sec_consumer_rate():
     iters = 200
     names = {1: "weights LDS", 2: "digit LDS", 3: "both LDS", 4: "IMMA only", 5: "weights LDS + IMMA", 7: "all", 15: "all, unused lanes predicated off",
              13: "weights LDS + IMMA + (digits off)"}
+    sms = torch.cuda.get_device_properties(dev).multi_processor_count
     for warps in (16, 8):
-        for ctas in (1, 148):
+        for ctas in (1, sms):
             for mode in (1, 2, 3, 4, 5, 7, 15):
                 for _ in range(2):
                     dcheck(dlib().b2l_debug_consumer_rate(out.data_ptr(), warps, iters, mode, ctas, L.stream_ptr()), "consumer_rate")
                     torch.cuda.synchronize()
                 cyc = int(out[0]) / (iters * 8)
                 print(f"warps={warps:2d} ctas={ctas:3d} mode={mode:2d} ({names.get(mode, '')}): {cyc:.0f} cycles per 16 KB stage  "
-                      f"-> {16384 / cyc:.1f} B/clk/SM = {16384 / cyc * 1.965 * 148 / 1e3:.1f} TB/s-equivalent", flush=True)
+                      f"-> {16384 / cyc:.1f} B/clk/SM = {16384 / cyc * 1.98 * sms / 1e3:.1f} TB/s-equivalent at 1.98 GHz", flush=True)
 
 
 def sec_bench_gemm():
-    """The tcgen05 prefill GEMM at the 13B widths, M = 4096 (BASELINE configs[3] prefill 8 x 512), next to torch.matmul
+    """The wgmma prefill GEMM at the 13B widths, M = 4096 (BASELINE configs[3] prefill 8 x 512), next to torch.matmul
     (library bf16 GEMM on a dense weight of the same shape) as the tensor-pipe yardstick."""
     import torch
     from lit_llama_b200 import _lib as L
@@ -558,6 +523,31 @@ def sec_bench_gemm():
         us_t = _time(lambda: torch.matmul(x, w.t()), iters=10, warm=2)
         fl = 2.0 * M * N * K
         print(f"gemm {name} M={M} N={N} K={K}: {us:.0f} us = {fl / us / 1e6:.0f} TFLOP/s   | torch.matmul bf16: {us_t:.0f} us = {fl / us_t / 1e6:.0f} TFLOP/s", flush=True)
+
+
+def sec_bench_tc():
+    """The 9..16-row wgmma linear on the 7B shapes at M = 16: weight copies rotated past the 50 MB L2, CUDA events;
+    GB/s of packed weights."""
+    import torch
+    from lit_llama_b200 import _lib as L
+
+    dev = torch.device("cuda")
+    M = int(os.environ.get("B2L_TC_M", "16"))
+    for (name, N, K) in [("c_attn", 12288, 4096), ("c_proj", 4096, 4096), ("fc12", 22016, 4096), ("mlp_proj", 4096, 11008), ("lm_head", 32000, 4096)]:
+        lv, qw, sc, z = rand_q4(N, K, dev, seed=3)
+        n_copies = max(2, int(200e6 // (N * K // 2)) + 1)
+        qts = [tile(L, qw, N, K) for _ in range(n_copies)]
+        x = torch.randn(M, K, device=dev).bfloat16()
+        y = torch.zeros(M, N, device=dev, dtype=torch.bfloat16)
+        args = [make_args(L, x, qt, sc, z, N, K, y) for qt in qts]
+
+        def run():
+            for a in args:
+                L.check(L.lib().b2l_q4_linear_tc(C.byref(a), L.stream_ptr()), "tc")
+
+        us = _time(run, iters=10, warm=2) / n_copies
+        print(f"tc {name} M={M} N={N} K={K}: {us:.1f} us = {N * K / 2 / us / 1e3:.0f} GB/s of packed weights", flush=True)
+        del qts
 
 
 def sec_trace():
@@ -583,15 +573,12 @@ def sec_trace():
             t0 = t[0]
             rel = lambda i: (t[i] - t0) if t[i] else None
             nst = (K // 32 // S + 1) // 2
-            print(f"{name} S={S} rep={rep} stages={nst}: init_sync={rel(1)} pdl_wait={rel(2)} x_ready={rel(3)} d_full={rel(104)} "
+            print(f"{name} S={S} rep={rep} stages={nst}: pdl_wait={rel(2)} x_ready={rel(3)} acc_done={rel(104)} "
                   f"csync1={rel(105)} epi={rel(106)} end={rel(107)}")
             k = min(nst, 20)
             print("   tma_issue ", [rel(108 + i) for i in range(k)])
             print("   w_full    ", [rel(4 + i) for i in range(k)])
-            print("   a_empty   ", [rel(24 + i) for i in range(k)])
-            print("   st_done   ", [rel(44 + i) for i in range(k)])
-            print("   a_full@mma", [rel(64 + i) for i in range(k)])
-            print("   commit    ", [rel(84 + i) for i in range(k)])
+            print("   mma_done  ", [rel(44 + i) for i in range(k)])
             del flush
 
 
@@ -725,7 +712,7 @@ def sec_bench_13b_b8():
             e1.record()
             torch.cuda.synchronize()
             ms = e0.elapsed_time(e1)
-        print(f"13B gptq.int4 prefill B={B} T={T}: {ms:.1f} ms  ({B * T / ms * 1e3:.0f} tokens/s; tcgen05 tile GEMM for every linear)")
+        print(f"13B gptq.int4 prefill B={B} T={T}: {ms:.1f} ms  ({B * T / ms * 1e3:.0f} tokens/s; wgmma tile GEMM for every linear)")
         if os.environ.get("B2L_PREFILL_PROFILE"):
             from torch.profiler import ProfilerActivity, profile
             model.reset_cache()
@@ -736,7 +723,7 @@ def sec_bench_13b_b8():
     us = _decode_us(model, B, S, dev, p0=T)
     from lit_llama_b200.quantization import BATCH_GEMV
     print(f"13B gptq.int4 decode B={B} pos~{T}: {us:.0f} us/step  {B * 1e6 / us:.0f} tokens/s  "
-          f"({'mma.sync batch kernel' if BATCH_GEMV else 'tcgen05 kernel'}, M={B})")
+          f"({'mma.sync batch kernel' if BATCH_GEMV else 'wgmma kernel'}, M={B})")
 
 
 def sec_bench_sizes():
@@ -950,7 +937,7 @@ def sec_precision():
             if qt is not None:
                 y2, err = tc_call(L, torch.cat([x, x]), qt, sc, z, N, K)
                 assert err is None, err
-                line += f" | tcgen05: differ {float((y2[0:1] != wb).float().mean()):.4f}  max {float(((y2[0:1].double() - want).abs() / ulp).max()):.3f} ulp"
+                line += f" | wgmma: differ {float((y2[0:1] != wb).float().mean()):.4f}  max {float(((y2[0:1].double() - want).abs() / ulp).max()):.3f} ulp"
             print(line, flush=True)
 
 

@@ -60,31 +60,6 @@ def full(tag, rep, name, title):
     open(os.path.join(P, f"{tag}_ncu_{name}.txt"), "w").write("\n".join(lines) + "\n")
 
 
-UNIT = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-
-
-def traffic(tag, rep="prof_gemv.ncu-rep"):
-    """profiles/traffic.json: measured DRAM bytes of the four per-layer batch-1 launches (x n_layer) plus lm_head
-    scaled by the same measured/algorithmic ratio -> bytes per token that bench.py reports as roofline.traffic."""
-    import json
-
-    raw = subprocess.run(["ncu", "-i", os.path.join(G, rep), "--page", "raw", "--csv"], capture_output=True, text=True).stdout
-    rows = list(csv.reader(raw.splitlines()))
-    h, units = rows[0], rows[1]
-    ir, iw = h.index("dram__bytes_read.sum"), h.index("dram__bytes_write.sum")
-    meas = [float(r[ir].replace(",", "")) * UNIT[units[ir]] + float(r[iw].replace(",", "")) * UNIT[units[iw]] for r in rows[2:6]]
-    shapes = [(12288, 4096), (4096, 4096), (22016, 4096), (4096, 11008)]
-    alg = [n * k // 2 for n, k in shapes]
-    W = 3309646848  # DESIGN.md section 3: algorithmic bytes per token of all batch-1 launches (7B)
-    ratio = sum(meas) / sum(alg)
-    out = {"kernel": "q4_gemv_kernel",
-           "source": f"profiles/{tag}_ncu_q4_gemv_kernel.txt (dram__bytes_read.sum + dram__bytes_write.sum of the four per-layer launches, "
-                     "x32, plus lm_head scaled by the same measured/algorithmic ratio); tools/summarize_profiles.py",
-           "per_layer_launch_bytes": meas, "algorithmic_per_layer_launch_bytes": alg,
-           "bytes_per_token": W * ratio, "algorithmic_bytes_per_token": W, "ratio": ratio}
-    json.dump(out, open(os.path.join(P, "traffic.json"), "w"), indent=1)
-
-
 if __name__ == "__main__":
     tag = sys.argv[1] if len(sys.argv) > 1 else "r01"
     os.makedirs(P, exist_ok=True)
@@ -92,10 +67,8 @@ if __name__ == "__main__":
         launch_list(tag, os.path.join(G, "launches_r1.csv"), "one eager decode step of LLaMA-7B gptq.int4 (tools/prof_step.py), every launch")
     for rep, name, title in [("prof_gemv.ncu-rep", "q4_gemv_kernel", "q4_gemv_kernel: c_attn, attn.c_proj, fc1|fc2, mlp.c_proj of layer 0 and c_attn of layer 1 (7B, batch 1)"),
                              ("prof_attn.ncu-rep", "attn_decode_fused_kernel", "attn_decode_fused_kernel (7B, batch 1)"),
-                             ("prof_gemm.ncu-rep", "q4_gemm_kernel", "q4_gemm_kernel: tcgen05 prefill GEMM, 13B c_attn shape (N 15360, K 5120) at M = 4096 (tools/diag.py bench_gemm)"),
-                             ("prof_q4.ncu-rep", "q4_linear_tc_kernel", "q4_linear_tc_kernel (tcgen05 path; first revision, 4 convert warps)")]:
+                             ("prof_gemm.ncu-rep", "q4_gemm_kernel", "q4_gemm_kernel: wgmma prefill GEMM, 13B c_attn shape (N 15360, K 5120) at M = 4096 (tools/diag.py bench_gemm)"),
+                             ("prof_q4.ncu-rep", "q4_linear_tc_kernel", "q4_linear_tc_kernel (wgmma path, M = 9..16)")]:
         if os.path.exists(os.path.join(G, rep)):
             full(tag, rep, name, title)
-    if os.path.exists(os.path.join(G, "prof_gemv.ncu-rep")):
-        traffic(tag)
     print(os.listdir(P))
