@@ -209,6 +209,17 @@ int b2l_q8_gemv(const void* x, const void* w_tiled, const void* cb, const void* 
                 b2l_stream_t stream);
 int b2l_q8_outlier_mask(const void* x, int ldx, int M, int K, float threshold, void* mask,
                         b2l_stream_t stream);
+/* y[M, N] (bf16, leading dimension ldy) for M activation rows x[M, K] (bf16, leading dimension
+ * ldx, a multiple of 8) on the int8 wgmma tensor cores: every row bit-identical to b2l_q8_gemv
+ * on that row with the batch's outlier mask (b2l_q8_outlier_mask over all M rows).  cb is CB
+ * itself (reference layout, int8 (N, K) row-major); no re-tiled copy is read.  K a multiple of
+ * 128 up to 32768; x, cb and workspace 16-byte aligned; flags must be 0.  workspace (at least
+ * b2l_q8_gemm_workspace_bytes(M, K) bytes, device memory) receives the quantised rows CA, SCA
+ * and the outlier mask; the library allocates nothing. */
+size_t b2l_q8_gemm_workspace_bytes(int M, int K);
+int b2l_q8_gemm(const void* x, int ldx, const void* cb, const void* scb, void* workspace,
+                size_t workspace_bytes, void* y, int ldy, int M, int N, int K, float threshold,
+                int flags, b2l_stream_t stream);
 
 /* generate.py:68-75 up to the probabilities: probs = softmax(where(l < kth, -inf, l)) with
  * l = logits / temperature (bf16, rounded like ATen does on the GPU) and kth the top_k-th

@@ -33,7 +33,7 @@ constexpr int STAGE_BYTES = KBP_PER_STAGE * KB_BYTES;  // 16 KB
 constexpr int MAX_STAGES = 6;
 constexpr int PRODUCER_WARP = NCW;
 constexpr int NTHREADS = (NCW + 2) * 32;
-constexpr int MAX_K = 12288;
+constexpr int MAX_K = 32768;            // LLaMA-65B's n_hidden is 22016
 
 struct Params {
   const __nv_bfloat16* x;     // one row, bf16 [K]
@@ -135,42 +135,36 @@ __global__ void __launch_bounds__(NTHREADS, 2) q8_gemv_kernel(const Params p) {
     __half* ah = reinterpret_cast<__half*>(smem + L.ah);
     uint32_t* mask = reinterpret_cast<uint32_t*>(smem + L.mask);
     constexpr int NT = NCW * 32;
-    constexpr int MAXC = MAX_K / (NT * 8);  // 6
-    // ---- activations: fp16 copy, outlier mask, row-wise absmax over inliers, int8 B fragments
+    // ---- activations: fp16 copy, outlier mask, row-wise absmax over inliers, int8 B fragments.  The row lives in
+    // shared memory only (ah, which the epilogue needs anyway): each thread re-reads the 8-element chunks it wrote,
+    // so no K-sized register array limits K.
     for (int i = tid; i < (p.K + 31) / 32; i += NT) mask[i] = p.mask_in ? p.mask_in[i] : 0u;
     bar_sync_c<1>(NT);
-    float av[MAXC][8];
-    float amax = 0.f;
+    for (int k = tid * 8; k < p.K; k += NT * 8) {
+      const uint4 u = *reinterpret_cast<const uint4*>(p.x + k);
+      const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+      __half hv[8];
+      uint32_t outl = 0;
 #pragma unroll
-    for (int c = 0; c < MAXC; ++c) {
-      const int k = (c * NT + tid) * 8;
-      if (k < p.K) {
-        const uint4 u = *reinterpret_cast<const uint4*>(p.x + k);
-        const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-        uint32_t outl = 0;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          av[c][2 * q] = __half2float(__float2half_rn(__uint_as_float(w[q] << 16)));
-          av[c][2 * q + 1] = __half2float(__float2half_rn(__uint_as_float(w[q] & 0xffff0000u)));
-        }
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          ah[k + e] = __float2half_rn(av[c][e]);
-          if (!p.mask_in && fabsf(av[c][e]) >= p.threshold) outl |= 1u << e;
-        }
-        if (outl) atomicOr(&mask[k >> 5], outl << (k & 31));
+      for (int q = 0; q < 4; ++q) {
+        hv[2 * q] = __float2half_rn(__uint_as_float(w[q] << 16));
+        hv[2 * q + 1] = __float2half_rn(__uint_as_float(w[q] & 0xffff0000u));
       }
+#pragma unroll
+      for (int e = 0; e < 8; ++e)
+        if (!p.mask_in && fabsf(__half2float(hv[e])) >= p.threshold) outl |= 1u << e;
+      *reinterpret_cast<uint4*>(ah + k) = *reinterpret_cast<const uint4*>(hv);
+      if (outl) atomicOr(&mask[k >> 5], outl << (k & 31));
     }
     bar_sync_c<1>(NT);
+    float amax = 0.f;
+    for (int k = tid * 8; k < p.K; k += NT * 8) {
+      const uint4 u = *reinterpret_cast<const uint4*>(ah + k);
+      const __half* hv = reinterpret_cast<const __half*>(&u);
+      const uint32_t mb = (mask[k >> 5] >> (k & 31)) & 0xFFu;
 #pragma unroll
-    for (int c = 0; c < MAXC; ++c) {
-      const int k = (c * NT + tid) * 8;
-      if (k < p.K) {
-        const uint32_t mb = (mask[k >> 5] >> (k & 31)) & 0xFFu;
-#pragma unroll
-        for (int e = 0; e < 8; ++e)
-          if (!((mb >> e) & 1u)) amax = fmaxf(amax, fabsf(av[c][e]));
-      }
+      for (int e = 0; e < 8; ++e)
+        if (!((mb >> e) & 1u)) amax = fmaxf(amax, fabsf(__half2float(hv[e])));
     }
     amax = warp_max(amax);
     if (lane == 0) red[warp] = amax;
@@ -179,24 +173,22 @@ __global__ void __launch_bounds__(NTHREADS, 2) q8_gemv_kernel(const Params p) {
 #pragma unroll
     for (int w = 0; w < NCW; ++w) sca = fmaxf(sca, red[w]);
     const float qs = sca > 0.f ? 127.0f / sca : 0.f;
+    for (int k = tid * 8; k < p.K; k += NT * 8) {
+      const uint4 u = *reinterpret_cast<const uint4*>(ah + k);
+      const __half* hv = reinterpret_cast<const __half*>(&u);
+      const uint32_t mb = (mask[k >> 5] >> (k & 31)) & 0xFFu;
+      uint32_t pk[2] = {0u, 0u};
 #pragma unroll
-    for (int c = 0; c < MAXC; ++c) {
-      const int k = (c * NT + tid) * 8;
-      if (k < p.K) {
-        const uint32_t mb = (mask[k >> 5] >> (k & 31)) & 0xFFu;
-        uint32_t pk[2] = {0u, 0u};
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          int qv = ((mb >> e) & 1u) ? 0 : __float2int_rn(av[c][e] * qs);
-          qv = max(-127, min(127, qv));
-          pk[e >> 2] |= (uint32_t)(qv & 0xFF) << (8 * (e & 3));
-        }
-        // k..k+3 -> lane t = (k % 16) / 4, half = (k % 32) / 16, chunk c32 = (k % 128) / 32; k+4..k+7 -> t + 1
-        const int kb = k >> 7, c32 = (k >> 5) & 3, half = (k >> 4) & 1, t0 = (k >> 2) & 3;
-        uint32_t* dst = reinterpret_cast<uint32_t*>(smem + L.xf + kb * 128);
-        dst[t0 * 8 + c32 * 2 + half] = pk[0];
-        dst[(t0 + 1) * 8 + c32 * 2 + half] = pk[1];
+      for (int e = 0; e < 8; ++e) {
+        int qv = ((mb >> e) & 1u) ? 0 : __float2int_rn(__half2float(hv[e]) * qs);
+        qv = max(-127, min(127, qv));
+        pk[e >> 2] |= (uint32_t)(qv & 0xFF) << (8 * (e & 3));
       }
+      // k..k+3 -> lane t = (k % 16) / 4, half = (k % 32) / 16, chunk c32 = (k % 128) / 32; k+4..k+7 -> t + 1
+      const int kb = k >> 7, c32 = (k >> 5) & 3, half = (k >> 4) & 1, t0 = (k >> 2) & 3;
+      uint32_t* dst = reinterpret_cast<uint32_t*>(smem + L.xf + kb * 128);
+      dst[t0 * 8 + c32 * 2 + half] = pk[0];
+      dst[(t0 + 1) * 8 + c32 * 2 + half] = pk[1];
     }
     if (tid == 0) red[8] = sca;
     bar_sync_c<3>(NT + 32);  // xf, ah, mask, SCA ready (epilogue warp included)
@@ -339,7 +331,8 @@ extern "C" int b2l_q8_gemv(const void* x, const void* w_tiled, const void* cb, c
   const SmemLayout L = smem_layout(nst, K);
   static DynSmemCache smem_cache;
   if (int rc = ensure_dyn_smem(q8_gemv_kernel, L.total, smem_cache)) return rc;
-  int grid = 2 * sm_count();
+  // two CTAs per SM while both fit in its 228 KB (1 KB of each reserved by the hardware); above K ~ 26000 only one does
+  int grid = (L.total <= 113u * 1024u ? 2 : 1) * sm_count();
   if (grid > p.n_rb) grid = p.n_rb;
   LaunchCfg lc(dim3(grid), dim3(NTHREADS), L.total, (cudaStream_t)stream, (flags & B2L_F_PDL) != 0, 1);
   B2L_CUDA(cudaLaunchKernelEx(&lc.cfg, q8_gemv_kernel, p));

@@ -5,7 +5,8 @@ Same construction-time behaviour: the weight is quantised row-wise to int8 as so
 module exists and again whenever a float `*.weight` arrives through `load_state_dict`
 (quantization.py:52-77); `weight.CB` (int8, (out, in)) and `weight.SCB` (fp32 row absmax)
 are attributes of the parameter like in bitsandbytes.  The forward is the LLM.int8()
-algorithm on the tensor cores (csrc/q8_gemv.cu) - no bitsandbytes, no CPU path.
+algorithm on the tensor cores (csrc/q8_gemv.cu for one row, csrc/q8_gemm.cu for more) - no bitsandbytes,
+no CPU path.
 
 bitsandbytes is not part of the reference tree (unpinned dependency, pyproject.toml:19), so the
 arithmetic follows the published algorithm (parity with the reference is unpinned, see DESIGN.md).
@@ -93,24 +94,28 @@ class Linear8bitLt(torch.nn.Module):
             self._tiled, self._tiled_key = t, key
         return self._tiled
 
+    MAX_IN_FEATURES = 32768  # the kernels' limit (csrc/q8_gemv.cu, csrc/q8_gemm.cu); LLaMA-65B's n_hidden is 22016
+
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         L.require_cuda_bf16(x, "Linear8bitLt.forward")
-        if self.in_features % 128 != 0 or self.in_features > 12288:
-            raise RuntimeError(f"Linear8bitLt: in_features {self.in_features} unsupported (multiple of 128, <= 12288)")
+        if self.in_features % 128 != 0 or self.in_features > self.MAX_IN_FEATURES:
+            raise RuntimeError(f"Linear8bitLt: in_features {self.in_features} unsupported (multiple of 128, <= {self.MAX_IN_FEATURES})")
         shape = x.shape
         x2 = x.reshape(-1, shape[-1]).contiguous()
         M, K, N = x2.shape[0], self.in_features, self.out_features
         y = torch.empty((M, N), device=x.device, dtype=x.dtype)
         lib = L.lib()
-        cb, scb, wt = self.weight.data, self.weight.SCB, self.tiled()
-        mask = None
-        if M > 1:  # outlier columns are a property of the whole batch (any row over the threshold)
-            mask = torch.empty((K + 31) // 32, dtype=torch.int32, device=x.device)
-            L.check(lib.b2l_q8_outlier_mask(x2.data_ptr(), K, M, K, self.threshold, mask.data_ptr(), L.stream_ptr()), "b2l_q8_outlier_mask")
-        for m in range(M):
-            rc = lib.b2l_q8_gemv(x2[m].data_ptr(), wt.data_ptr(), cb.data_ptr(), scb.data_ptr(), None if mask is None else mask.data_ptr(),
-                                 y[m].data_ptr(), N, K, self.threshold, 0, L.stream_ptr())
+        cb, scb = self.weight.data, self.weight.SCB
+        if M == 1:
+            rc = lib.b2l_q8_gemv(x2.data_ptr(), self.tiled().data_ptr(), cb.data_ptr(), scb.data_ptr(), None, y.data_ptr(),
+                                 N, K, self.threshold, 0, L.stream_ptr())
             L.check(rc, "b2l_q8_gemv")
+        else:  # outlier columns are a property of the whole batch (any row over the threshold)
+            nbytes = lib.b2l_q8_gemm_workspace_bytes(M, K)
+            work = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+            rc = lib.b2l_q8_gemm(x2.data_ptr(), K, cb.data_ptr(), scb.data_ptr(), work.data_ptr(), nbytes, y.data_ptr(), N,
+                                 M, N, K, self.threshold, 0, L.stream_ptr())
+            L.check(rc, "b2l_q8_gemm")
         if self.bias is not None:
             y = y + self.bias.to(y.dtype)
         return y.reshape(*shape[:-1], N)

@@ -14,7 +14,7 @@ import time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-SECTIONS = ["generic", "tile", "tc_small", "tc_shapes", "tc_modes", "gemv", "grid_flag", "hmma_rate", "imma_rate", "consumer_rate", "bench_gemm", "bench_tc", "trace", "bench_layers", "bench_gemv", "bench_step", "bench_ctx", "bench_13b_b8", "bench_sizes", "batch_debug", "bench_step_int8", "timeline", "mega_timeline"]
+SECTIONS = ["generic", "tile", "tc_small", "tc_shapes", "tc_modes", "gemv", "grid_flag", "hmma_rate", "imma_rate", "consumer_rate", "bench_gemm", "bench_tc", "trace", "bench_layers", "bench_gemv", "bench_step", "bench_ctx", "bench_13b_b8", "bench_sizes", "batch_debug", "bench_step_int8", "bench_q8_gemm", "timeline", "mega_timeline"]
 
 
 _DLIB = None
@@ -775,41 +775,120 @@ def sec_batch_debug():
                   f"decode row diff {float((both[1:].float() - one.float()).abs().max()):.4g}  (|logits| max {float(one.float().abs().max()):.3g})", flush=True)
 
 
+def _card():
+    """The card and its power limit, printed beside every absolute number."""
+    import torch
+
+    try:
+        pl = subprocess.run(["nvidia-smi", "-i", str(torch.cuda.current_device()), "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
+                            capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.TimeoutExpired):
+        pl = "power limit unknown"
+    return f"{torch.cuda.get_device_name()} ({pl})"
+
+
 def sec_bench_step_int8():
-    """LLaMA-7B --quantize llm.int8 decode (BASELINE config 2): module path replayed as a CUDA graph."""
+    """--quantize llm.int8 (BASELINE config 2) at 7B, 13B and 30B: a 512-token prompt (the M >= 2 GEMM) and batch-1
+    decode at ctx ~2048 (module path replayed as a CUDA graph).  B2L_INT8_SIZES picks the sizes."""
     import torch
     import lit_llama_b200 as P
     from lit_llama_b200.utils import quantization
 
     dev = torch.device("cuda")
-    prev = torch.get_default_dtype()
-    torch.set_default_dtype(torch.bfloat16)
-    try:
-        with torch.device(dev), quantization("llm.int8"):
-            model = P.LLaMA.from_name("7B")
-    finally:
-        torch.set_default_dtype(prev)
-    model.eval()
+    print(_card(), flush=True)
     S = 2048
-    model.copy_logits = False
-    idx = torch.randint(0, 32000, (1, 16), device=dev, dtype=torch.int32)
-    with torch.no_grad():
-        model(idx, S, torch.arange(16, device=dev))
-        tok = torch.randint(0, 32000, (1, 1), device=dev, dtype=torch.int32)
-        pos = [torch.tensor([16 + i], device=dev) for i in range(72)]
-        for i in range(6):
-            model(tok, S, pos[i])
-        torch.cuda.synchronize()
+    for name in os.environ.get("B2L_INT8_SIZES", "7B,13B,30B").split(","):
+        prev = torch.get_default_dtype()
+        torch.set_default_dtype(torch.bfloat16)
+        try:
+            with torch.device(dev), quantization("llm.int8"):
+                model = P.LLaMA.from_name(name)
+        finally:
+            torch.set_default_dtype(prev)
+        model.eval()
+        model.copy_logits = False
+        w8 = sum(m.weight.numel() for m in model.modules() if isinstance(m, P.Linear8bitLt))
+        idx = torch.randint(0, 32000, (1, 512), device=dev, dtype=torch.int32)
+        with torch.no_grad():
+            prompt_us = _time(lambda: model(idx, S, torch.arange(512, device=dev)), iters=5, warm=2)
+            model.reset_cache()
+            us = _decode_us(model, 1, S, dev, p0=2000, n=24)
+        print(f"{name} llm.int8: prompt 512 tokens {prompt_us / 1e3:.2f} ms ({512e6 / prompt_us:.0f} tok/s) | decode B=1 ctx~2000-2030 "
+              f"graph={model._module_graph['graph'] is not None}: {us:.1f} us/token {1e6 / us:.1f} tok/s ({w8 / us / 1e3:.0f} GB/s of int8 weights) | "
+              f"{torch.cuda.max_memory_allocated() / 2**30:.1f} GiB peak", flush=True)
+        del model
+        torch.cuda.empty_cache()
+        torch.cuda.reset_peak_memory_stats()
+
+
+def _time_graph(fn, reps):
+    """GPU time of one fn() in us: `reps` calls captured into a CUDA graph (as the model replays decode), so host launch
+    overhead is not part of the number; the graph is replayed 3 times, the median kept."""
+    import torch
+
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s):
+        fn()
+        fn()
+    torch.cuda.current_stream().wait_stream(s)
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        for _ in range(reps):
+            fn()
+    g.replay()
+    ts = []
+    for _ in range(3):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-        for i in range(6, 70):
-            model(tok, S, pos[i])
+        g.replay()
         e1.record()
         torch.cuda.synchronize()
-    us = e0.elapsed_time(e1) / 64 * 1e3
-    W8 = 6.6132e9
-    print(f"decode step 7B llm.int8 pos~16-90 graph={model._module_graph['graph'] is not None}: {us:.1f} us/token  {1e6 / us:.1f} tok/s  "
-          f"({W8 / us / 1e3:.0f} GB/s of weights = {W8 / us / 1e3 / 6573.2:.3f} of measured HBM peak)")
+        ts.append(e0.elapsed_time(e1) * 1e3 / reps)
+    return sorted(ts)[1]
+
+
+def sec_bench_q8_gemm():
+    """The llm.int8 GEMM (b2l_q8_gemm) against the per-row loop it replaced (b2l_q8_outlier_mask + M x b2l_q8_gemv with
+    the batch mask) and torch.matmul on a dense bf16 weight of the same shape, CUDA events around CUDA-graph replays, same
+    run.  TOP/s counts
+    2 M N K int8 operations per call (the bf16 matmul does the same count in FLOP)."""
+    import torch
+    from lit_llama_b200 import _lib as L
+
+    dev = torch.device("cuda")
+    lib = L.lib()
+    print(_card(), flush=True)
+    for (name, N, K) in [("7B c_attn", 12288, 4096), ("7B mlp.c_proj", 4096, 11008), ("13B c_fc1", 13824, 5120), ("13B mlp.c_proj", 5120, 13824)]:
+        cb = torch.randint(-127, 128, (N, K), device=dev, dtype=torch.int8)
+        scb = torch.rand(N, device=dev) * 0.2 + 0.01
+        wt = torch.empty(lib.b2l_q8_tiled_bytes(N, K), dtype=torch.uint8, device=dev)
+        L.check(lib.b2l_q8_tile(cb.data_ptr(), wt.data_ptr(), N, K, L.stream_ptr()), "tile")
+        wd = torch.randn(N, K, device=dev).bfloat16()
+        for M in (2, 8, 64, 512, 4096):
+            x = torch.randn(M, K, device=dev).bfloat16()
+            y = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
+            nbytes = lib.b2l_q8_gemm_workspace_bytes(M, K)
+            work = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+            mask = torch.empty(K // 32, dtype=torch.int32, device=dev)
+            gemm = lambda: L.check(lib.b2l_q8_gemm(x.data_ptr(), K, cb.data_ptr(), scb.data_ptr(), work.data_ptr(), nbytes, y.data_ptr(), N,
+                                                   M, N, K, 6.0, 0, L.stream_ptr()), "gemm")
+
+            def loop():
+                lib.b2l_q8_outlier_mask(x.data_ptr(), K, M, K, 6.0, mask.data_ptr(), L.stream_ptr())
+                for m in range(M):
+                    lib.b2l_q8_gemv(x[m].data_ptr(), wt.data_ptr(), cb.data_ptr(), scb.data_ptr(), mask.data_ptr(), y[m].data_ptr(),
+                                    N, K, 6.0, 0, L.stream_ptr())
+
+            it = 20 if M <= 64 else 4
+            us_g = _time_graph(gemm, it)
+            us_l = _time_graph(loop, it if M <= 64 else 1)
+            us_t = _time_graph(lambda: torch.matmul(x, wd.t()), it)
+            op = 2.0 * M * N * K
+            print(f"{name} N={N} K={K} M={M}: gemm {us_g:.1f} us = {op / us_g / 1e6:.1f} TOP/s | per-row loop {us_l:.1f} us "
+                  f"({us_l / us_g:.1f}x the gemm) | torch.matmul bf16 {us_t:.1f} us = {op / us_t / 1e6:.1f} TFLOP/s", flush=True)
+        del cb, wt, wd
+        torch.cuda.empty_cache()
 
 
 def sec_timeline():
