@@ -207,6 +207,12 @@ int b2l_q8_tile(const void* cb, void* tiled, int N, int K, b2l_stream_t stream);
 int b2l_q8_gemv(const void* x, const void* w_tiled, const void* cb, const void* scb,
                 const void* outlier_mask, void* y, int N, int K, float threshold, int flags,
                 b2l_stream_t stream);
+/* b2l_q8_gemv reading CB itself (reference layout, int8 (N, K) row-major) with one bulk copy per weight row, so
+ * no re-tiled copy has to exist: every output is bit-identical to b2l_q8_gemv on b2l_q8_tile(cb).
+ * K a multiple of 128 up to 32768, N > 0; x and cb 16-byte aligned; flags 0 or B2L_F_PDL.
+ * Bad arguments are rejected before the device is touched. */
+int b2l_q8_gemv_cb(const void* x, const void* cb, const void* scb, const void* outlier_mask,
+                   void* y, int N, int K, float threshold, int flags, b2l_stream_t stream);
 int b2l_q8_outlier_mask(const void* x, int ldx, int M, int K, float threshold, void* mask,
                         b2l_stream_t stream);
 /* y[M, N] (bf16, leading dimension ldy) for M activation rows x[M, K] (bf16, leading dimension

@@ -92,6 +92,7 @@ _SIGS = {
     "b2l_q8_tiled_bytes": (c_size_t, [c_int, c_int]),
     "b2l_q8_tile": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "b2l_q8_gemv": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_int, c_void_p]),
+    "b2l_q8_gemv_cb": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_int, c_void_p]),
     "b2l_q8_outlier_mask": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
     "b2l_q8_gemm_workspace_bytes": (c_size_t, [c_int, c_int]),
     "b2l_q8_gemm": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_int, c_int, c_int, c_int, c_float,

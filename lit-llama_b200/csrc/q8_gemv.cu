@@ -11,9 +11,19 @@
 // persistent CTAs over 16-row blocks and the full K, TMA bulk copies into an mbarrier ring
 // issued before the PDL dependency, deterministic in-CTA reduction.
 //
-// Weight layout (b2l_q8_tile): [N/16 row blocks][K/128 k blocks][4 k32 chunks][32 lanes][16 B];
-// the 16 bytes of lane (g, t) are registers a0..a3 of m16n8k32: rows g, g+8 x k = 32c + 4t..+3
-// and 32c + 16 + 4t..+3.
+// Two weight sources, one kernel body (template parameter WS); only how a stage (16 rows x 1024 k) reaches shared
+// memory and how a warp fetches its A fragments differ:
+//   WS_CB (b2l_q8_gemv_cb, what Linear8bitLt runs): CB itself, int8 (N, K) row-major.  Lanes 0..15 of the producer
+//     warp each issue one bulk copy of their row's 1024 bytes, into a ring whose rows are ROW_PITCH = 1040 bytes
+//     apart; no tensor map is read.  Each warp builds the m16 x k32 A fragment of chunk c with one ldmatrix.x4: its
+//     four 8 x 8 .b16 matrices (rows 0-7 / 8-15 x k 32c..+15 / 32c+16..+31) are exactly registers a0..a3 of the s8
+//     fragment, and the 16-byte pad puts each matrix's eight rows in distinct banks.  Rows past N are not copied:
+//     their accumulators are never stored.  Measured on an H100, this beat a tensor-map copy of the same stage (with
+//     or without the 128-byte swizzle) on every 7B shape and on whole-token 7B decode (DESIGN.md §3).
+//   WS_TILED (b2l_q8_gemv): the b2l_q8_tile layout [N/16 row blocks][K/128 k blocks][4 k32 chunks][32 lanes][16 B];
+//     the 16 bytes of lane (g, t) are registers a0..a3 of m16n8k32: rows g, g+8 x k = 32c + 4t..+3 and
+//     32c + 16 + 4t..+3.  One 16 KB bulk copy per stage.
+// Both contract the same int8 values in the same order, so their outputs are bit-identical.
 //
 // parity: the arithmetic restates the published LLM.int8() algorithm (bitsandbytes is not in
 // the reference tree and not installed): parity with the reference is unpinned (DESIGN.md).
@@ -24,12 +34,16 @@
 namespace b2l {
 namespace q8mv {
 
+enum WeightSource { WS_TILED, WS_CB };
+
 constexpr int RB = 16;
 constexpr int KB = 128;                 // k per k block (4 IMMAs of k32)
 constexpr int KB_BYTES = 2048;          // one (row block, k block)
 constexpr int NCW = 8;
 constexpr int KBP_PER_STAGE = 8;        // one k block per consumer warp per stage
 constexpr int STAGE_BYTES = KBP_PER_STAGE * KB_BYTES;  // 16 KB
+constexpr int ROW_PITCH = KBP_PER_STAGE * KB + 16;     // WS_CB: one weight row of a stage + 16 B (conflict-free ldmatrix)
+template <WeightSource WS> __host__ __device__ constexpr uint32_t stage_bytes() { return WS == WS_CB ? RB * ROW_PITCH : STAGE_BYTES; }
 constexpr int MAX_STAGES = 6;
 constexpr int PRODUCER_WARP = NCW;
 constexpr int NTHREADS = (NCW + 2) * 32;
@@ -37,8 +51,8 @@ constexpr int MAX_K = 32768;            // LLaMA-65B's n_hidden is 22016
 
 struct Params {
   const __nv_bfloat16* x;     // one row, bf16 [K]
-  const uint8_t* wt;          // tiled CB
-  const int8_t* cb;           // reference layout CB (N, K) row-major, for the outlier columns
+  const uint8_t* wt;          // WS_TILED: tiled CB
+  const int8_t* cb;           // reference layout CB (N, K) row-major: WS_CB's weights, and the outlier columns
   const float* scb;           // [N]
   const uint32_t* mask_in;    // optional precomputed outlier mask (K bits), shared by a batch; nullptr = derive from x
   __nv_bfloat16* y;           // [N]
@@ -68,14 +82,19 @@ __device__ __forceinline__ void imma_16832(int (&d)[4], const uint4& a, uint32_t
       : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3])
       : "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w), "r"(b0), "r"(b1));
 }
+__device__ __forceinline__ uint4 ldmatrix_x4(uint32_t addr) {
+  uint4 r;
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "r"(addr) : "memory");
+  return r;
+}
 
 struct SmemLayout {
   uint32_t ring, xf, ah, mask, scratch, red, bars, total;
 };
-__host__ __device__ inline SmemLayout smem_layout(int nst, int K) {
+__host__ __device__ inline SmemLayout smem_layout(int nst, int K, uint32_t stage) {
   SmemLayout L;
   uint32_t o = 0;
-  L.ring = o;    o += (uint32_t)nst * STAGE_BYTES;
+  L.ring = o;    o += (uint32_t)nst * stage;
   L.xf = o;      o += (uint32_t)(K / KB) * 128;   // int8 B fragments: [k block][t (4)][32 B]
   L.ah = o;      o += (uint32_t)K * 2;            // fp16 activations (outlier term)
   L.mask = o;    o += (uint32_t)((K + 31) / 32) * 4;
@@ -88,9 +107,11 @@ __host__ __device__ inline SmemLayout smem_layout(int nst, int K) {
   return L;
 }
 
+template <WeightSource WS>
 __global__ void __launch_bounds__(NTHREADS, 2) q8_gemv_kernel(const Params p) {
   extern __shared__ __align__(128) uint8_t smem[];
-  const SmemLayout L = smem_layout(p.nst, p.K);
+  constexpr uint32_t SB = stage_bytes<WS>();
+  const SmemLayout L = smem_layout(p.nst, p.K, SB);
   const uint32_t sbase = smem_u32(smem);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int n_kb = p.K / KB;
@@ -111,17 +132,31 @@ __global__ void __launch_bounds__(NTHREADS, 2) q8_gemv_kernel(const Params p) {
   __syncthreads();
 
   if (warp == PRODUCER_WARP) {
-    if (lane == 0) {
+    if (lane == 0 || WS == WS_CB) {
       int slot = 0, it = 0;
       uint32_t phase = 1;
       for (int u = 0; u < n_units; ++u) {
-        const uint8_t* src = p.wt + (size_t)(rb_lo + u) * n_kb * KB_BYTES;
         for (int s = 0; s < stages_per_rb; ++s, ++it) {
-          const int nkb = min(KBP_PER_STAGE, n_kb - s * KBP_PER_STAGE);
-          const uint32_t bytes = (uint32_t)nkb * KB_BYTES;
-          mbar_wait(bar_empty + slot * 8, phase);
-          mbar_expect_tx(bar_full + slot * 8, bytes);
-          tma_bulk_g2s(sbase + L.ring + slot * STAGE_BYTES, src + (size_t)s * STAGE_BYTES, bytes, bar_full + slot * 8);
+          if constexpr (WS == WS_CB) {
+            // one bulk copy per weight row (lanes 0..15); rows past N are not copied (their accumulators are never
+            // stored), so the transaction count is what is actually copied
+            const int row0 = (rb_lo + u) * RB, nrows = min(RB, p.N - row0);
+            const uint32_t row_bytes = (uint32_t)min(KBP_PER_STAGE, n_kb - s * KBP_PER_STAGE) * KB;
+            if (lane == 0) {
+              mbar_wait(bar_empty + slot * 8, phase);
+              mbar_expect_tx(bar_full + slot * 8, (uint32_t)nrows * row_bytes);
+            }
+            __syncwarp();
+            if (lane < nrows)
+              tma_bulk_g2s(sbase + L.ring + slot * SB + lane * ROW_PITCH, p.cb + (size_t)(row0 + lane) * p.K + (size_t)s * KBP_PER_STAGE * KB,
+                           row_bytes, bar_full + slot * 8);
+          } else {
+            mbar_wait(bar_empty + slot * 8, phase);
+            const uint32_t bytes = (uint32_t)min(KBP_PER_STAGE, n_kb - s * KBP_PER_STAGE) * KB_BYTES;
+            mbar_expect_tx(bar_full + slot * 8, bytes);
+            const uint8_t* src = p.wt + (size_t)(rb_lo + u) * n_kb * KB_BYTES + (size_t)s * STAGE_BYTES;
+            tma_bulk_g2s(sbase + L.ring + slot * STAGE_BYTES, src, bytes, bar_full + slot * 8);
+          }
           if (++slot == p.nst) { slot = 0; phase ^= 1; }
           if (it + 1 == min(total_stages, p.nst)) pdl_launch_dependents();
         }
@@ -199,19 +234,26 @@ __global__ void __launch_bounds__(NTHREADS, 2) q8_gemv_kernel(const Params p) {
     uint32_t phase = 0;
     int* scratch = reinterpret_cast<int*>(smem + L.scratch);
     const uint8_t* xf_lane = smem + L.xf + t4 * 32;
+    // WS_CB: lane i addresses row i % 8 of ldmatrix matrix j = i / 8, i.e. weight row i % 8 + 8 (j % 2) and 16-byte unit
+    // 2c + j / 2 of the warp's k block
+    const uint32_t lm_row = (uint32_t)((lane & 7) + 8 * ((lane >> 3) & 1)) * ROW_PITCH;
+    const uint32_t lm_unit = (uint32_t)(lane >> 4);
     for (int u = 0; u < n_units; ++u) {
       int acc[2][4] = {{0, 0, 0, 0}, {0, 0, 0, 0}};
       for (int s = 0; s < stages_per_rb; ++s) {
         const int nkb = min(KBP_PER_STAGE, n_kb - s * KBP_PER_STAGE);
         mbar_wait(bar_full + slot * 8, phase);
         if (warp < nkb) {
-          const uint8_t* wb = smem + L.ring + slot * STAGE_BYTES + warp * KB_BYTES + lane * 16;
           const uint4* xp = reinterpret_cast<const uint4*>(xf_lane + (s * KBP_PER_STAGE + warp) * 128);
           const uint4 xa = xp[0], xb = xp[1];
           const uint32_t bb[8] = {xa.x, xa.y, xa.z, xa.w, xb.x, xb.y, xb.z, xb.w};
 #pragma unroll
           for (int c = 0; c < 4; ++c) {
-            const uint4 a = *reinterpret_cast<const uint4*>(wb + c * 512);
+            uint4 a;
+            if constexpr (WS == WS_CB)
+              a = ldmatrix_x4(sbase + L.ring + slot * SB + lm_row + warp * KB + (2 * c + lm_unit) * 16);
+            else
+              a = *reinterpret_cast<const uint4*>(smem + L.ring + slot * STAGE_BYTES + warp * KB_BYTES + lane * 16 + c * 512);
             imma_16832(acc[c & 1], a, bb[2 * c], bb[2 * c + 1]);
           }
         }
@@ -314,29 +356,55 @@ extern "C" int b2l_q8_tile(const void* cb, void* tiled, int N, int K, b2l_stream
   return 0;
 }
 
+// stage count, grid and launch, shared by both weight sources; p holds everything but nst
+template <WeightSource WS>
+static int launch_gemv(Params& p, int flags, b2l_stream_t stream) {
+  constexpr uint32_t SB = stage_bytes<WS>();
+  const uint32_t fixed = smem_layout(0, p.K, SB).total;
+  int nst = (int)((110u * 1024u - fixed) / SB);
+  if (nst > MAX_STAGES) nst = MAX_STAGES;
+  if (nst < 2) nst = 2;
+  p.nst = nst;
+  const SmemLayout L = smem_layout(nst, p.K, SB);
+  static DynSmemCache smem_cache;
+  if (int rc = ensure_dyn_smem(q8_gemv_kernel<WS>, L.total, smem_cache)) return rc;
+  // two CTAs per SM while both fit in its 228 KB (1 KB of each reserved by the hardware); above K ~ 26000 only one does
+  int grid = (L.total <= 113u * 1024u ? 2 : 1) * sm_count();
+  if (grid > p.n_rb) grid = p.n_rb;
+  LaunchCfg lc(dim3(grid), dim3(NTHREADS), L.total, (cudaStream_t)stream, (flags & B2L_F_PDL) != 0, 1);
+  B2L_CUDA(cudaLaunchKernelEx(&lc.cfg, q8_gemv_kernel<WS>, p));
+  return 0;
+}
+
+static void fill_params(Params& p, const void* x, const void* cb, const void* scb, const void* outlier_mask, void* y, int N, int K,
+                        float threshold) {
+  p = Params{};   // every kernel parameter defined, wt included where it is unused
+  p.x = (const __nv_bfloat16*)x; p.cb = (const int8_t*)cb; p.scb = (const float*)scb;
+  p.mask_in = (const uint32_t*)outlier_mask; p.y = (__nv_bfloat16*)y;
+  p.N = N; p.K = K; p.n_rb = (N + RB - 1) / RB; p.threshold = threshold;
+}
+
 extern "C" int b2l_q8_gemv(const void* x, const void* w_tiled, const void* cb, const void* scb, const void* outlier_mask, void* y,
                            int N, int K, float threshold, int flags, b2l_stream_t stream) {
   B2L_CHECK_ARG(x && w_tiled && cb && scb && y && N > 0, "b2l_q8_gemv: bad argument");
   B2L_CHECK_SUPPORTED(K > 0 && K % KB == 0 && K <= MAX_K, "b2l_q8_gemv: K=%d must be a multiple of %d and <= %d", K, KB, MAX_K);
   B2L_CHECK_ARG(((uintptr_t)x % 16 == 0) && ((uintptr_t)w_tiled % 16 == 0), "b2l_q8_gemv: x / w_tiled must be 16-byte aligned");
   Params p;
-  p.x = (const __nv_bfloat16*)x; p.wt = (const uint8_t*)w_tiled; p.cb = (const int8_t*)cb; p.scb = (const float*)scb;
-  p.mask_in = (const uint32_t*)outlier_mask; p.y = (__nv_bfloat16*)y;
-  p.N = N; p.K = K; p.n_rb = (N + RB - 1) / RB; p.threshold = threshold;
-  const uint32_t fixed = smem_layout(0, K).total;
-  int nst = (int)((110u * 1024u - fixed) / STAGE_BYTES);
-  if (nst > MAX_STAGES) nst = MAX_STAGES;
-  if (nst < 2) nst = 2;
-  p.nst = nst;
-  const SmemLayout L = smem_layout(nst, K);
-  static DynSmemCache smem_cache;
-  if (int rc = ensure_dyn_smem(q8_gemv_kernel, L.total, smem_cache)) return rc;
-  // two CTAs per SM while both fit in its 228 KB (1 KB of each reserved by the hardware); above K ~ 26000 only one does
-  int grid = (L.total <= 113u * 1024u ? 2 : 1) * sm_count();
-  if (grid > p.n_rb) grid = p.n_rb;
-  LaunchCfg lc(dim3(grid), dim3(NTHREADS), L.total, (cudaStream_t)stream, (flags & B2L_F_PDL) != 0, 1);
-  B2L_CUDA(cudaLaunchKernelEx(&lc.cfg, q8_gemv_kernel, p));
-  return 0;
+  fill_params(p, x, cb, scb, outlier_mask, y, N, K, threshold);
+  p.wt = (const uint8_t*)w_tiled;
+  return launch_gemv<WS_TILED>(p, flags, stream);
+}
+
+extern "C" int b2l_q8_gemv_cb(const void* x, const void* cb, const void* scb, const void* outlier_mask, void* y, int N, int K,
+                              float threshold, int flags, b2l_stream_t stream) {
+  B2L_CHECK_ARG(x && cb && scb && y, "b2l_q8_gemv_cb: null pointer");
+  B2L_CHECK_SUPPORTED(K > 0 && K % KB == 0 && K <= MAX_K, "b2l_q8_gemv_cb: K=%d must be a multiple of %d and <= %d", K, KB, MAX_K);
+  B2L_CHECK_ARG(N > 0, "b2l_q8_gemv_cb: bad shape N=%d", N);
+  B2L_CHECK_ARG(((uintptr_t)x % 16 == 0) && ((uintptr_t)cb % 16 == 0), "b2l_q8_gemv_cb: x / cb must be 16-byte aligned");
+  B2L_CHECK_SUPPORTED((flags & ~B2L_F_PDL) == 0, "b2l_q8_gemv_cb: unknown flags 0x%x (only B2L_F_PDL)", (unsigned)flags);
+  Params p;
+  fill_params(p, x, cb, scb, outlier_mask, y, N, K, threshold);
+  return launch_gemv<WS_CB>(p, flags, stream);
 }
 
 // outlier columns of a batch: bit k set iff any row has |fp16(x[m][k])| >= threshold

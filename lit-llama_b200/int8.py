@@ -85,6 +85,8 @@ class Linear8bitLt(torch.nn.Module):
             super()._load_from_state_dict(local_state_dict, prefix, *args, **kwargs)
 
     def tiled(self) -> torch.Tensor:
+        """CB re-tiled for `b2l_q8_gemv` (b2l_q8_tile), built on demand and cached.  forward does not use it: both of
+        its kernels read CB directly, so a model that only runs forward holds one copy of its int8 weights."""
         cb = self.weight.data
         key = (cb.data_ptr(), cb._version)
         if self._tiled is None or self._tiled_key != key:
@@ -107,9 +109,9 @@ class Linear8bitLt(torch.nn.Module):
         lib = L.lib()
         cb, scb = self.weight.data, self.weight.SCB
         if M == 1:
-            rc = lib.b2l_q8_gemv(x2.data_ptr(), self.tiled().data_ptr(), cb.data_ptr(), scb.data_ptr(), None, y.data_ptr(),
-                                 N, K, self.threshold, 0, L.stream_ptr())
-            L.check(rc, "b2l_q8_gemv")
+            rc = lib.b2l_q8_gemv_cb(x2.data_ptr(), cb.data_ptr(), scb.data_ptr(), None, y.data_ptr(), N, K, self.threshold, 0,
+                                    L.stream_ptr())
+            L.check(rc, "b2l_q8_gemv_cb")
         else:  # outlier columns are a property of the whole batch (any row over the threshold)
             nbytes = lib.b2l_q8_gemm_workspace_bytes(M, K)
             work = torch.empty(nbytes, dtype=torch.uint8, device=x.device)

@@ -14,7 +14,7 @@ import time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-SECTIONS = ["generic", "tile", "tc_small", "tc_shapes", "tc_modes", "gemv", "grid_flag", "hmma_rate", "imma_rate", "consumer_rate", "bench_gemm", "bench_tc", "trace", "bench_layers", "bench_gemv", "bench_step", "bench_ctx", "bench_13b_b8", "bench_sizes", "batch_debug", "bench_step_int8", "bench_q8_gemm", "timeline", "mega_timeline"]
+SECTIONS = ["generic", "tile", "tc_small", "tc_shapes", "tc_modes", "gemv", "grid_flag", "hmma_rate", "imma_rate", "consumer_rate", "bench_gemm", "bench_tc", "trace", "bench_layers", "bench_gemv", "bench_step", "bench_ctx", "bench_13b_b8", "bench_sizes", "batch_debug", "bench_step_int8", "bench_q8_gemm", "bench_q8_gemv", "timeline", "mega_timeline"]
 
 
 _DLIB = None
@@ -787,9 +787,59 @@ def _card():
     return f"{torch.cuda.get_device_name()} ({pl})"
 
 
+def _q8_tiled_forward(cb_forward):
+    """Linear8bitLt.forward before b2l_q8_gemv_cb: at M = 1, b2l_q8_gemv on the cached re-tiled copy (Linear8bitLt.tiled)."""
+    import torch
+    from lit_llama_b200 import _lib as L
+
+    def forward(self, x):
+        shape = x.shape
+        x2 = x.reshape(-1, shape[-1]).contiguous()
+        if x2.shape[0] != 1:
+            return cb_forward(self, x)
+        y = torch.empty(self.out_features, dtype=x.dtype, device=x.device)
+        L.check(L.lib().b2l_q8_gemv(x2.data_ptr(), self.tiled().data_ptr(), self.weight.data.data_ptr(), self.weight.SCB.data_ptr(), None,
+                                    y.data_ptr(), self.out_features, self.in_features, self.threshold, 0, L.stream_ptr()), "b2l_q8_gemv")
+        return y.reshape(*shape[:-1], self.out_features)
+
+    return forward
+
+
+def _int8_old_vs_new(model, S, dev, rounds=3):
+    """7B batch-1 decode with Linear8bitLt.forward (CB read directly) and the parent's forward (re-tiled copy), alternated
+    in one process.  Each run writes the same tokens at the same positions, then decodes one fixed token whose logits
+    must be bit-identical between the two."""
+    import torch
+    import lit_llama_b200 as P
+
+    new_forward = P.Linear8bitLt.forward
+    old_forward = _q8_tiled_forward(new_forward)
+    us = {"new": [], "old": []}
+    logits = {}
+    try:
+        for _ in range(rounds):
+            for kind, fwd in (("new", new_forward), ("old", old_forward)):
+                P.Linear8bitLt.forward = fwd
+                model._module_graph = None   # the graph bakes the launches: capture it again with this forward
+                torch.manual_seed(0)
+                us[kind].append(_decode_us(model, 1, S, dev, p0=2000, n=24))
+                with torch.no_grad():
+                    out = model(torch.tensor([[1234]], device=dev, dtype=torch.int32), S, torch.tensor([2040], device=dev)).clone()
+                if kind in logits:
+                    assert torch.equal(out, logits[kind]), f"{kind} forward is not deterministic"
+                logits[kind] = out
+    finally:
+        P.Linear8bitLt.forward = new_forward
+    assert torch.equal(logits["new"], logits["old"]), "CB-direct and tiled batch-1 decode give different logits"
+    fmt = lambda v: " ".join(f"{x:.1f}" for x in v)
+    print(f"  7B decode B=1, alternated: new forward (CB read directly) {fmt(us['new'])} us/token | parent forward (re-tiled copy) "
+          f"{fmt(us['old'])} us/token | logits bit-identical", flush=True)
+
+
 def sec_bench_step_int8():
-    """--quantize llm.int8 (BASELINE config 2) at 7B, 13B and 30B: a 512-token prompt (the M >= 2 GEMM) and batch-1
-    decode at ctx ~2048 (module path replayed as a CUDA graph).  B2L_INT8_SIZES picks the sizes."""
+    """--quantize llm.int8 (BASELINE config 2) at 7B, 13B, 30B and 65B: a 512-token prompt (the M >= 2 GEMM) and batch-1
+    decode at ctx ~2048 (module path replayed as a CUDA graph).  B2L_INT8_SIZES picks the sizes.  The peak memory is
+    taken before 7B's old-against-new decode comparison, which builds the parent's re-tiled copy."""
     import torch
     import lit_llama_b200 as P
     from lit_llama_b200.utils import quantization
@@ -797,7 +847,7 @@ def sec_bench_step_int8():
     dev = torch.device("cuda")
     print(_card(), flush=True)
     S = 2048
-    for name in os.environ.get("B2L_INT8_SIZES", "7B,13B,30B").split(","):
+    for name in os.environ.get("B2L_INT8_SIZES", "7B,13B,30B,65B").split(","):
         prev = torch.get_default_dtype()
         torch.set_default_dtype(torch.bfloat16)
         try:
@@ -816,6 +866,8 @@ def sec_bench_step_int8():
         print(f"{name} llm.int8: prompt 512 tokens {prompt_us / 1e3:.2f} ms ({512e6 / prompt_us:.0f} tok/s) | decode B=1 ctx~2000-2030 "
               f"graph={model._module_graph['graph'] is not None}: {us:.1f} us/token {1e6 / us:.1f} tok/s ({w8 / us / 1e3:.0f} GB/s of int8 weights) | "
               f"{torch.cuda.max_memory_allocated() / 2**30:.1f} GiB peak", flush=True)
+        if name == "7B":
+            _int8_old_vs_new(model, S, dev)
         del model
         torch.cuda.empty_cache()
         torch.cuda.reset_peak_memory_stats()
@@ -888,6 +940,62 @@ def sec_bench_q8_gemm():
             print(f"{name} N={N} K={K} M={M}: gemm {us_g:.1f} us = {op / us_g / 1e6:.1f} TOP/s | per-row loop {us_l:.1f} us "
                   f"({us_l / us_g:.1f}x the gemm) | torch.matmul bf16 {us_t:.1f} us = {op / us_t / 1e6:.1f} TFLOP/s", flush=True)
         del cb, wt, wd
+        torch.cuda.empty_cache()
+
+
+def sec_bench_q8_gemv():
+    """The batch-1 llm.int8 kernel from its two weight sources: b2l_q8_gemv on the re-tiled copy against b2l_q8_gemv_cb on
+    CB itself, CUDA events around CUDA-graph replays, alternated in one process (5 rounds, each number is the median of 3
+    replays).  Each shape cycles through enough weight copies (>= 200 MB) that no call finds its weights in the 50 MB L2,
+    as in a decode step.  GB/s counts the int8 weight bytes N K per call.  The input row has three outlier columns."""
+    import torch
+    from lit_llama_b200 import _lib as L
+
+    dev = torch.device("cuda")
+    lib = L.lib()
+    print(_card(), flush=True)
+    shapes = [("7B c_attn", 12288, 4096), ("7B attn.c_proj", 4096, 4096), ("7B c_fc1", 11008, 4096), ("7B mlp.c_proj", 4096, 11008),
+              ("7B lm_head", 32000, 4096), ("13B c_fc1", 13824, 5120), ("13B mlp.c_proj", 5120, 13824), ("30B c_fc1", 17920, 6656),
+              ("30B mlp.c_proj", 6656, 17920), ("65B c_fc1", 22016, 8192), ("65B mlp.c_proj", 8192, 22016)]
+    for (name, N, K) in shapes:
+        ncopy = max(2, -(-200_000_000 // (N * K)))
+        cbs = [torch.randint(-127, 128, (N, K), device=dev, dtype=torch.int8) for _ in range(ncopy)]
+        scbs = [torch.rand(N, device=dev) * 0.2 + 0.01 for _ in range(ncopy)]
+        wts = []
+        for cb in cbs:
+            wts.append(torch.empty(lib.b2l_q8_tiled_bytes(N, K), dtype=torch.uint8, device=dev))
+            L.check(lib.b2l_q8_tile(cb.data_ptr(), wts[-1].data_ptr(), N, K, L.stream_ptr()), "tile")
+        x = torch.randn(K, device=dev)
+        x[[7, K // 3, K - 5]] = torch.tensor([9.0, -7.5, 6.5], device=dev)
+        x = x.bfloat16()
+        ys = [torch.empty(N, device=dev, dtype=torch.bfloat16) for _ in range(ncopy)]
+        y2 = [torch.empty(N, device=dev, dtype=torch.bfloat16) for _ in range(ncopy)]
+        reps = ncopy * max(1, -(-8_000_000_000 // (ncopy * N * K)))   # >= 8 GB of weights per replay
+
+        def tiled():
+            for i in range(reps):
+                c = i % ncopy
+                lib.b2l_q8_gemv(x.data_ptr(), wts[c].data_ptr(), cbs[c].data_ptr(), scbs[c].data_ptr(), None, ys[c].data_ptr(), N, K, 6.0, 0,
+                                L.stream_ptr())
+
+        def direct():
+            for i in range(reps):
+                c = i % ncopy
+                lib.b2l_q8_gemv_cb(x.data_ptr(), cbs[c].data_ptr(), scbs[c].data_ptr(), None, y2[c].data_ptr(), N, K, 6.0, 0, L.stream_ptr())
+
+        tiled()
+        direct()
+        torch.cuda.synchronize()
+        assert all(torch.equal(a, b) for a, b in zip(ys, y2)), name
+        t_t, t_c = [], []
+        for _ in range(5):
+            t_t.append(_time_graph(tiled, 1) / reps)
+            t_c.append(_time_graph(direct, 1) / reps)
+        med = lambda v: sorted(v)[len(v) // 2]
+        fmt = lambda v: " ".join(f"{u:.2f}" for u in v)
+        print(f"{name} N={N} K={K} ({ncopy} copies): tiled {med(t_t):.2f} us = {N * K / med(t_t) / 1e3:.0f} GB/s [{fmt(t_t)}] | "
+              f"CB direct {med(t_c):.2f} us = {N * K / med(t_c) / 1e3:.0f} GB/s [{fmt(t_c)}] | CB/tiled {med(t_c) / med(t_t):.3f}", flush=True)
+        del cbs, scbs, wts, ys, y2
         torch.cuda.empty_cache()
 
 
