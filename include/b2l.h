@@ -131,7 +131,9 @@ enum {
   B2L_F_ROPE_ROWS = 4,  /* b2l_attention: `rope` holds the T rows already selected by
                            input_pos (the reference's call convention, model.py:93)    */
   B2L_F_ATTN_UNFUSED = 8, /* debug: force the three-kernel attention path for T == 1   */
-  B2L_F_DEBUG_NOCOMPUTE = 16 /* debug: b2l_q4_gemv streams the weights but skips the math */
+  B2L_F_DEBUG_NOCOMPUTE = 16, /* debug: b2l_q4_gemv streams the weights but skips the math */
+  B2L_F_W8 = 32         /* b2l_decode_step: every linear is gptq.int8, qw_mma from b2l_w8_tile_i8
+                           (b2l_w8_gemv); B == 1 and no plan only                     */
 };
 
 /* Fused [RMSNorm ->] int4 linear [-> residual | SwiGLU] on wgmma (M <= 16).  Replaces
@@ -159,6 +161,25 @@ size_t b2l_q4_tiled_i8_bytes(int N, int K);
 int b2l_q4_tile_i8(const void* qw, void* qw_tiled, int N, int K, b2l_stream_t stream);
 int b2l_q4_untile_i8(const void* qw_tiled, void* qw, int N, int K, b2l_stream_t stream);
 int b2l_q4_gemv(const b2l_q4_linear_args* args, b2l_stream_t stream);
+
+/* gptq.int8 (8-bit levels, one (scale, zero) per row, no bias): the batch-1 kernel above with 8-bit weights.  Same
+ * argument block, prologues, epilogues, B2L_F_PDL and split_k grid override as b2l_q4_gemv; flags other than
+ * B2L_F_PDL / B2L_F_DEBUG_NOCOMPUTE are rejected.  qw_tiled from b2l_w8_tile_i8: [N/16 row blocks][K/64 k blocks]
+ * [2 chunks][32 lanes][16 B]; in chunk c lane (g, t) holds rows g, g + 8, g, g + 8 at k = k0 .. k0+3, k0 .. k0+3,
+ * k0+4 .. k0+7, k0+4 .. k0+7 (k0 = 64 kb + 32 c + 8 t), rows beyond N zero.  For B2L_EPI_SWIGLU the rows of a 16-row
+ * block are [8 of c_fc1 | 8 of c_fc2].  K % 64 == 0, K <= 24576.  qw for (un)tiling: quant_weight in the reference
+ * layout, uint8 [K][N]. */
+size_t b2l_w8_tiled_i8_bytes(int N, int K);
+int b2l_w8_tile_i8(const void* qw, void* qw_tiled, int N, int K, b2l_stream_t stream);
+int b2l_w8_untile_i8(const void* qw_tiled, void* qw, int N, int K, b2l_stream_t stream);
+int b2l_w8_gemv(const b2l_q4_linear_args* args, b2l_stream_t stream);
+
+/* gptq.int8 for M >= 1 rows (meant for M >= 2: prompts, batched decode) on the wgmma GEMM of b2l_q4_gemm: the
+ * producers dequantise the 8-bit levels with get_weight's roundings, so the tensor core multiplies exactly
+ * get_weight()'s bf16 matrix.  qw_tiled is quant_weight itself in the reference layout (uint8 [K][N], no
+ * re-tiled copy); other requirements as b2l_q4_gemm (K % 64 == 0, ldx % 8 == 0, 16-byte aligned x and weights,
+ * NONE / STORE), flags must be 0. */
+int b2l_w8_gemm(const b2l_q4_linear_args* args, b2l_stream_t stream);
 
 /* The same fused linear for 1..8 activation rows (batched decode) on mma.sync.m16n8k16 (f16), weight tiling
  * b2l_q4_tile_mma ([N/16 row blocks][K/64 k blocks][32 lanes][16 B] in m16n8k16 A-fragment order), argument block of

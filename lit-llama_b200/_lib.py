@@ -13,6 +13,7 @@ B2L_BF16, B2L_F32 = 0, 1
 PRO_NONE, PRO_RMSNORM = 0, 1
 EPI_STORE, EPI_RESIDUAL, EPI_SWIGLU = 0, 1, 2
 F_PDL, F_NO_ALIAS_N, F_ROPE_ROWS = 1, 2, 4
+F_W8 = 32   # b2l_decode_step: every linear is gptq.int8 (b2l_w8_gemv)
 
 c_void_p, c_int, c_float, c_size_t = C.c_void_p, C.c_int, C.c_float, C.c_size_t
 
@@ -81,6 +82,11 @@ _SIGS = {
     "b2l_q4_tile_i8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "b2l_q4_untile_i8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "b2l_q4_gemv": (c_int, [C.POINTER(Q4LinearArgs), c_void_p]),
+    "b2l_w8_tiled_i8_bytes": (c_size_t, [c_int, c_int]),
+    "b2l_w8_tile_i8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p]),
+    "b2l_w8_untile_i8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p]),
+    "b2l_w8_gemv": (c_int, [C.POINTER(Q4LinearArgs), c_void_p]),
+    "b2l_w8_gemm": (c_int, [C.POINTER(Q4LinearArgs), c_void_p]),
     "b2l_q4_gemv_batch": (c_int, [C.POINTER(Q4LinearArgs), c_void_p]),
     "b2l_q4_gemv_batch_workspace_bytes": (c_size_t, [c_int]),
     "b2l_rmsnorm": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),

@@ -81,7 +81,10 @@ static size_t prefetch_distance() {
 
 static std::vector<PfWindow> prefetch_windows(const b2l_decode_args* d) {
   std::vector<std::pair<const uint8_t*, size_t>> ops;
-  auto add = [&](const b2l_q4_weight& w) { ops.push_back({(const uint8_t*)w.qw_mma, b2l_q4_tiled_i8_bytes(w.N, w.K)}); };
+  const bool w8 = (d->flags & B2L_F_W8) != 0;
+  auto add = [&](const b2l_q4_weight& w) {
+    ops.push_back({(const uint8_t*)w.qw_mma, w8 ? b2l_w8_tiled_i8_bytes(w.N, w.K) : b2l_q4_tiled_i8_bytes(w.N, w.K)});
+  };
   for (int l = 0; l < d->n_layer; ++l) {
     add(d->layers[l].c_attn); add(d->layers[l].c_proj); add(d->layers[l].c_fc12); add(d->layers[l].mlp_proj);
   }
@@ -140,6 +143,10 @@ static int q4_call(const b2l_q4_weight& w, const void* x, int ldx, void* y, int 
   a.split_k = 0;
   a.flags = flags;
   a.trace = gemv ? trace : nullptr;
+  if (flags & B2L_F_W8) {   // gptq.int8: batch 1 only (checked by b2l_decode_step); only the kernel's own flags pass
+    a.flags = flags & (B2L_F_PDL | B2L_F_DEBUG_NOCOMPUTE);
+    return b2l_w8_gemv(&a, stream);
+  }
   if (gemv) return b2l_q4_gemv(&a, stream);
   if (batch) {
     a.workspace = batch_work;
@@ -168,9 +175,14 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
   B2L_CHECK_ARG(d->wte && d->ln_f && d->rope && d->idx && d->input_pos && d->ring_start && d->x && d->qkv && d->att &&
                     d->hid && d->attn_work && d->logits,
                 "b2l_decode_step: null pointer");
+  if (d->flags & B2L_F_W8) {
+    B2L_CHECK_SUPPORTED(d->B == 1, "b2l_decode_step: B2L_F_W8 (gptq.int8) runs batch 1 only, got B=%d", d->B);
+    B2L_CHECK_SUPPORTED(d->plan == nullptr, "b2l_decode_step: B2L_F_W8 (gptq.int8) does not run in the persistent kernel (plan must be NULL)");
+  }
   if (d->plan != nullptr) return decode_step_persistent(d, stream);   // one persistent kernel per token (decode_mega.cu)
   const int C = d->n_embd, hs = C / d->n_head, B = d->B;
-  const int fl = d->flags;
+  const int fl = d->flags;               // the linears' flags (q4_call routes B2L_F_W8 to b2l_w8_gemv)
+  const int afl = fl & ~B2L_F_W8;        // everything else
   int rc;
   // debug timeline: launch i of the step writes uint64[64] at timeline + 512*i (order: per Block c_attn,
   // attention, c_proj, fc12, mlp_proj; then lm_head)
@@ -194,7 +206,7 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
       return rc;
     g_attn_timeline = tl();
     if ((rc = b2l_attention(d->qkv, L.k_cache, L.v_cache, d->rope, d->input_pos, d->ring_start, d->att, d->attn_work, B,
-                            1, d->n_head, hs, d->S, d->block_size, fl, stream))) {
+                            1, d->n_head, hs, d->S, d->block_size, afl, stream))) {
       g_attn_timeline = nullptr;
       return rc;
     }

@@ -807,6 +807,7 @@ inline int plan_n_ops(const b2l_decode_args* d) { return 5 * d->n_layer + 1; }
 
 bool mega_shape_ok(const b2l_decode_args* d) {
   if (d->B != 1 || d->n_embd % d->n_head != 0 || d->n_embd / d->n_head != mega::HS) return false;
+  if (d->flags & B2L_F_W8) return false;   // the persistent kernel's GEMV reads int4 tilings only
   auto ok = [](const b2l_q4_weight& w) { return w.qw_mma != nullptr && w.K % KB == 0 && w.K <= 12288 && w.N > 0; };
   if (!ok(d->lm_head)) return false;
   for (int l = 0; l < d->n_layer; ++l) {

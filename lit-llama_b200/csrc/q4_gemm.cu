@@ -22,6 +22,7 @@
 //         (quantization.py:392-411), so the GEMM sees exactly the matrix the reference's dense branch multiplies;
 //       * 16-byte st.shared of 8 consecutive k of a row = one row of a core matrix; fence.proxy.async; mbarrier arrive;
 //   epilogue: each MMA thread converts its accumulator fragment to bf16 and stores pairs of output features.
+// gptq.int8 (b2l_w8_gemm) is the same kernel with W8 = true: only the producers differ (w8_load below).
 #include <cuda.h>   // CUtensorMap and its enums only: the encoder is fetched with cudaGetDriverEntryPoint (no libcuda link)
 
 #include "b2l_common.cuh"
@@ -45,7 +46,7 @@ constexpr int SBO = 128;                       // bytes between adjacent 8-row g
 struct Params {
   CUtensorMap xmap;        // 3-D view of x (see above); must stay the first member (64-byte alignment)
   const __nv_bfloat16* x; int ldx;
-  const uint8_t* qwt;      // b2l_q4_tile layout: [N/128 tiles][K/32 slabs][128 rows][16 B]
+  const uint8_t* qwt;      // b2l_q4_tile layout: [N/128 tiles][K/32 slabs][128 rows][16 B]; 8 bits: quant_weight [K][N]
   const void* scales; const void* zeros; int szdt;
   __nv_bfloat16* y; int ldy;
   int M, N, K;
@@ -113,6 +114,27 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
                : "memory");
 }
 
+// 8-bit levels (gptq.int8): producer thread pt owns weight rows n0 + 4 (pt % 32) .. + 3 and k 16 (pt / 32) .. + 15 of
+// a stage.  Sixteen 4-byte loads from quant_weight in the reference layout (uint8 [K][N], N-contiguous: a warp reads
+// 128 consecutive bytes per k) give 4 rows x 16 k; each level becomes bf16 exactly through the fp32 mantissa
+// (2^23 + lv - 2^23: every level 0..255 is a bf16 value, which the int4 trick 0x4300 | lv is not beyond 127).
+__device__ __forceinline__ void w8_load(uint32_t (&wq)[16], const uint8_t* qw, int N, int row0, int k0, bool vec) {
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const uint8_t* src = qw + (size_t)(k0 + j) * N + row0;
+    if (vec) {
+      wq[j] = __ldg(reinterpret_cast<const uint32_t*>(src));
+    } else {   // ragged N (not a multiple of 4) or the last rows: byte loads, zero beyond N
+      uint32_t w = 0;
+#pragma unroll
+      for (int r = 0; r < 4; ++r)
+        if (row0 + r < N) w |= (uint32_t)__ldg(src + r) << (8 * r);
+      wq[j] = w;
+    }
+  }
+}
+
+template <bool W8>
 __global__ void __launch_bounds__(NTHREADS, 1) q4_gemm_kernel(const __grid_constant__ Params p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   const uint32_t sbase = smem_u32(smem);
@@ -174,6 +196,55 @@ __global__ void __launch_bounds__(NTHREADS, 1) q4_gemm_kernel(const __grid_const
         }
       }
     }
+  } else if constexpr (W8) {
+    // ===================== producers, 8-bit levels: activations (TMA) + dequantised weights =====================
+    const int pt = tid - NMMA;
+    const int row0 = n0 + 4 * lane, kq = 16 * (pt >> 5);    // 4 rows x 16 k of every stage
+    const bool vec = (p.N % 4 == 0) && row0 + 4 <= p.N;
+    __nv_bfloat162 sc2[4], z2[4];
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      float sc_f = 0.f, z_f = 0.f;
+      if (row0 + r < p.N) { sc_f = load_sz(p.scales, p.szdt, row0 + r); z_f = load_sz(p.zeros, p.szdt, row0 + r); }
+      sc2[r] = __float2bfloat162_rn(sc_f); z2[r] = __float2bfloat162_rn(z_f);
+    }
+    const float two23 = 8388608.f;
+    uint32_t wq[16];
+    if (row0 < p.N) w8_load(wq, p.qwt, p.N, row0, kq, vec);
+    for (int kt = 0; kt < n_kt; ++kt) {
+      const int st = kt % NSTAGE;
+      if (kt >= NSTAGE) mbar_wait(bar_empty + st * 8, (uint32_t)(kt / NSTAGE - 1) & 1u);
+      const uint32_t a_base = sbase + st * STAGE_BYTES, b_base = a_base + A_BYTES;
+      if (pt == 0) {
+        mbar_expect_tx(bar_full + st * 8, A_BYTES);
+        tma_load_3d(a_base, &p.xmap, 0, m0, kt * (BK / 8), bar_full + st * 8);
+      }
+      uint32_t w[16];
+#pragma unroll
+      for (int j = 0; j < 16; ++j) w[j] = row0 < p.N ? wq[j] : 0u;
+      if (kt + 1 < n_kt && row0 < p.N) w8_load(wq, p.qwt, p.N, row0, (kt + 1) * BK + kq, vec);
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {       // k-column 2 (pt / 32) + c: 8 consecutive k of row row0 + r
+          uint32_t o[4];
+#pragma unroll
+          for (int s = 0; s < 4; ++s) {
+            const uint32_t sel = 0x7540u | (uint32_t)r;   // level byte r under the exponent byte of 2^23
+            const float f0 = __uint_as_float(__byte_perm(w[8 * c + 2 * s], 0x4B000000u, sel)) - two23;
+            const float f1 = __uint_as_float(__byte_perm(w[8 * c + 2 * s + 1], 0x4B000000u, sel)) - two23;
+            __nv_bfloat162 t = __floats2bfloat162_rn(f0, f1);   // level pair, exact
+            t = __hmul2(__hsub2(t, z2[r]), sc2[r]);            // (level - zero) * scale with the reference's bf16 roundings
+            o[s] = *reinterpret_cast<const uint32_t*>(&t);
+          }
+          asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(b_base + (2 * (pt >> 5) + c) * LBO_B + (4 * lane + r) * 16),
+                       "r"(o[0]), "r"(o[1]), "r"(o[2]), "r"(o[3]) : "memory");
+        }
+      }
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_full + st * 8);
+    }
   } else {
     // ===================== producers: activations (TMA) + dequantised weights =====================
     const int pt = tid - NMMA;                     // 0..127 = weight row of the tile
@@ -232,15 +303,20 @@ __global__ void __launch_bounds__(NTHREADS, 1) q4_gemm_kernel(const __grid_const
 using namespace b2l;
 using namespace b2l::q4gm;
 
-extern "C" int b2l_q4_gemm(const b2l_q4_linear_args* a, b2l_stream_t stream) {
-  B2L_CHECK_ARG(a != nullptr, "b2l_q4_gemm: null args");
-  B2L_CHECK_ARG(a->x && a->qw_tiled && a->scales && a->zeros && a->y, "b2l_q4_gemm: null pointer");
-  B2L_CHECK_ARG(a->M > 0 && a->N > 0 && a->K > 0, "b2l_q4_gemm: bad shape");
-  B2L_CHECK_SUPPORTED(a->K % BK == 0, "b2l_q4_gemm: K=%d must be a multiple of %d", a->K, BK);
-  B2L_CHECK_ARG(a->ldx >= a->K && a->ldx % 8 == 0 && a->ldy >= a->N, "b2l_q4_gemm: bad leading dimension (ldx %% 8 == 0)");
-  B2L_CHECK_ARG(((uintptr_t)a->x % 16 == 0) && ((uintptr_t)a->qw_tiled % 16 == 0), "b2l_q4_gemm: x / qw_tiled must be 16-byte aligned");
-  B2L_CHECK_ARG(a->sz_dtype == B2L_BF16 || a->sz_dtype == B2L_F32, "b2l_q4_gemm: bad sz_dtype");
-  B2L_CHECK_SUPPORTED(a->prologue == B2L_PRO_NONE && a->epilogue == B2L_EPI_STORE, "b2l_q4_gemm: plain linear only (no fused prologue / epilogue)");
+namespace {
+// b2l_q4_gemm (W8 = false: qw_tiled from b2l_q4_tile) and b2l_w8_gemm (W8 = true: quant_weight, uint8 [K][N])
+template <bool W8>
+int gemm_entry(const b2l_q4_linear_args* a, b2l_stream_t stream) {
+  const char* fn = W8 ? "b2l_w8_gemm" : "b2l_q4_gemm";
+  B2L_CHECK_ARG(a != nullptr, "%s: null args", fn);
+  B2L_CHECK_ARG(a->x && a->qw_tiled && a->scales && a->zeros && a->y, "%s: null pointer", fn);
+  B2L_CHECK_ARG(a->M > 0 && a->N > 0 && a->K > 0, "%s: bad shape", fn);
+  B2L_CHECK_SUPPORTED(a->K % BK == 0, "%s: K=%d must be a multiple of %d", fn, a->K, BK);
+  B2L_CHECK_ARG(a->ldx >= a->K && a->ldx % 8 == 0 && a->ldy >= a->N, "%s: bad leading dimension (ldx %% 8 == 0)", fn);
+  B2L_CHECK_ARG(((uintptr_t)a->x % 16 == 0) && ((uintptr_t)a->qw_tiled % 16 == 0), "%s: x / qw_tiled must be 16-byte aligned", fn);
+  B2L_CHECK_ARG(a->sz_dtype == B2L_BF16 || a->sz_dtype == B2L_F32, "%s: bad sz_dtype", fn);
+  if (W8) B2L_CHECK_SUPPORTED(a->flags == 0, "%s: unknown flags 0x%x", fn, a->flags);
+  B2L_CHECK_SUPPORTED(a->prologue == B2L_PRO_NONE && a->epilogue == B2L_EPI_STORE, "%s: plain linear only (no fused prologue / epilogue)", fn);
   // cuTensorMapEncodeTiled through the runtime (resolved once)
   typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                                const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -251,7 +327,7 @@ extern "C" int b2l_q4_gemm(const b2l_q4_linear_args* a, b2l_stream_t stream) {
     return (EncodeFn)fn;
   }();
   if (encode == nullptr) {
-    set_error("b2l_q4_gemm: cuTensorMapEncodeTiled is not available from this driver");
+    set_error("%s: cuTensorMapEncodeTiled is not available from this driver", fn);
     return B2L_E_STATE;
   }
   Params p;
@@ -264,7 +340,7 @@ extern "C" int b2l_q4_gemm(const b2l_q4_linear_args* a, b2l_stream_t stream) {
     const CUresult cr = encode(&p.xmap, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(a->x), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                                CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (cr != CUDA_SUCCESS) {
-      set_error("b2l_q4_gemm: cuTensorMapEncodeTiled failed (%d) for M=%d K=%d ldx=%d", (int)cr, a->M, a->K, a->ldx);
+      set_error("%s: cuTensorMapEncodeTiled failed (%d) for M=%d K=%d ldx=%d", fn, (int)cr, a->M, a->K, a->ldx);
       return B2L_E_ARG;
     }
   }
@@ -274,9 +350,14 @@ extern "C" int b2l_q4_gemm(const b2l_q4_linear_args* a, b2l_stream_t stream) {
   p.y = (__nv_bfloat16*)a->y; p.ldy = a->ldy;
   p.M = a->M; p.N = a->N; p.K = a->K;
   static DynSmemCache smem_cache;
-  if (int rc = ensure_dyn_smem(q4_gemm_kernel, SMEM_BYTES, smem_cache)) return rc;
+  if (int rc = ensure_dyn_smem(q4_gemm_kernel<W8>, SMEM_BYTES, smem_cache)) return rc;
   dim3 grid((a->N + BN - 1) / BN, (a->M + BM - 1) / BM);
-  q4_gemm_kernel<<<grid, NTHREADS, SMEM_BYTES, (cudaStream_t)stream>>>(p);
+  q4_gemm_kernel<W8><<<grid, NTHREADS, SMEM_BYTES, (cudaStream_t)stream>>>(p);
   B2L_LAUNCH_CHECK("q4_gemm_kernel");
   return 0;
 }
+}  // namespace
+
+extern "C" int b2l_q4_gemm(const b2l_q4_linear_args* a, b2l_stream_t stream) { return gemm_entry<false>(a, stream); }
+
+extern "C" int b2l_w8_gemm(const b2l_q4_linear_args* a, b2l_stream_t stream) { return gemm_entry<true>(a, stream); }

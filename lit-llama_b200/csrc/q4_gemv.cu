@@ -35,6 +35,10 @@
 // level[16 rb + g + 8][k], k = 64 kb + 32 c + 8 t + 4 j + i.  (The k order inside a chunk is a free choice as long as
 // the activation digits use the same one; this one gives every prologue thread, which owns 8 consecutive k, both
 // B registers of one lane.)
+//
+// gptq.int8 (8-bit levels, b2l_w8_gemv) runs the same kernel with W8 = true: weight layout b2l_w8_tile_i8,
+// [N/16 row blocks][K/64 k blocks][2 chunks][32 lanes][16 B], whose four words per lane are the u8 A fragment itself
+// (no LOP3, no row-pair recovery in the epilogue).  The int32 accumulators hold 255 * 128 * K < 2^31 for K <= 24576.
 #include <cstdlib>
 
 #include "q4_mma_common.cuh"
@@ -109,36 +113,50 @@ __device__ __forceinline__ void tma_bulk_g2s_hint(uint32_t dst, const void* src,
 // X (|X| < 2^30) -> word whose bytes are its balanced base-256 digits (byte 3 = signed top digit)
 __device__ __forceinline__ uint32_t balanced_digits(int X) { return ((uint32_t)X + 0x00808080u) ^ 0x00808080u; }
 
-// One k-block position (64 k = two k32 chunks) of NH 16-row halves: LDS.128 per half, 1 LOP3 + 1 IMMA per packed word pair.
-template <int NH>
-__device__ __forceinline__ void kblock_imma(int (&acc)[MAX_HALVES][2][4], const uint8_t* wbase, const uint4& xb) {
-#pragma unroll
-  for (int h = 0; h < NH; ++h) {
-    const uint4 wv = *reinterpret_cast<const uint4*>(wbase + h * HALF_STAGE_BYTES);
-    mma_u8s8_16832(acc[h][0], wv.x, wv.x & 0xf0f0f0f0u, wv.y, wv.y & 0xf0f0f0f0u, xb.x, xb.y);
-    mma_u8s8_16832(acc[h][1], wv.z, wv.z & 0xf0f0f0f0u, wv.w, wv.w & 0xf0f0f0f0u, xb.z, xb.w);
+// Weight width W8 (false: 4-bit levels, b2l_q4_tile_i8; true: 8-bit levels, b2l_w8_tile_i8).  A (16-row block, k block)
+// tile is 512 B of packed nibbles or 1024 B of bytes; a half stage is 8 KB either way, so the ring, the stage count
+// and the producer are shared and a stage carries half as many k-block positions at 8 bits.
+template <bool W8> struct WTile {
+  static constexpr int KB_BYTES = W8 ? 1024 : 512;
+  static constexpr int KBP = HALF_STAGE_BYTES / KB_BYTES;   // k-block positions per half stage: 16 / 8
+};
+
+// One tile (16 rows x 64 k) into one accumulator set.  4 bits: one LDS.128, 1 LOP3 + 1 IMMA per packed word pair
+// (a byte feeds rows g and g + 8); 8 bits: chunk c is its own LDS.128 whose four words ARE the A fragment.
+template <bool W8>
+__device__ __forceinline__ void single_imma(int (&a)[2][4], const uint8_t* tile, const uint4& xb) {
+  if constexpr (W8) {
+    const uint4 w0 = *reinterpret_cast<const uint4*>(tile), w1 = *reinterpret_cast<const uint4*>(tile + 512);
+    mma_u8s8_16832(a[0], w0.x, w0.y, w0.z, w0.w, xb.x, xb.y);
+    mma_u8s8_16832(a[1], w1.x, w1.y, w1.z, w1.w, xb.z, xb.w);
+  } else {
+    const uint4 wv = *reinterpret_cast<const uint4*>(tile);
+    mma_u8s8_16832(a[0], wv.x, wv.x & 0xf0f0f0f0u, wv.y, wv.y & 0xf0f0f0f0u, xb.x, xb.y);
+    mma_u8s8_16832(a[1], wv.z, wv.z & 0xf0f0f0f0u, wv.w, wv.w & 0xf0f0f0f0u, xb.z, xb.w);
   }
 }
 
-// One tile (16 rows x 64 k) into one accumulator set.
-__device__ __forceinline__ void single_imma(int (&a)[2][4], const uint8_t* tile, const uint4& xb) {
-  const uint4 wv = *reinterpret_cast<const uint4*>(tile);
-  mma_u8s8_16832(a[0], wv.x, wv.x & 0xf0f0f0f0u, wv.y, wv.y & 0xf0f0f0f0u, xb.x, xb.y);
-  mma_u8s8_16832(a[1], wv.z, wv.z & 0xf0f0f0f0u, wv.w, wv.w & 0xf0f0f0f0u, xb.z, xb.w);
+// One k-block position of NH 16-row halves (the activation fragments are loaded once for all of them).
+template <int NH, bool W8>
+__device__ __forceinline__ void kblock_imma(int (&acc)[MAX_HALVES][2][4], const uint8_t* wbase, const uint4& xb) {
+#pragma unroll
+  for (int h = 0; h < NH; ++h) single_imma<W8>(acc[h], wbase + h * HALF_STAGE_BYTES, xb);
 }
 
 // MAXC = activation chunks (2048 elements each) a thread block caches in registers during the prologue:
 // 6 covers K <= 12288 (every 7B/13B/30B layer), 12 covers K <= 24576 (65B mlp.c_proj, K = 22016).
-// NDIG = base-256 digits of the scaled activations: 3 (|X| < 2^22).
-template <int MAXC, int NDIG>
+// NDIG = base-256 digits of the scaled activations: 3 (|X| < 2^22).  W8: 8-bit weight levels (see WTile).
+template <int MAXC, int NDIG, bool W8>
 __global__ void __launch_bounds__(NTHREADS, 2) q4_gemv_kernel(const Params p) {
+  constexpr int KB_BYTES = WTile<W8>::KB_BYTES, KBP_PER_STAGE = WTile<W8>::KBP;
   extern __shared__ __align__(128) uint8_t smem[];
   const SmemLayout L = smem_layout(p.nst, p.K, NDIG);
   const uint32_t sbase = smem_u32(smem);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int n_kb = p.K / KB;                                              // k blocks per 16-row block
-  // A 16 KB stage holds 32 tiles of 512 B: 16 k-block positions of BOTH 16-row blocks of a pair, or 32 positions
-  // of a single block (the ring slot is always used in full).  The last stage of a unit may be short.
+  // A 16 KB stage holds 32 tiles of 512 B (16 of 1024 B at 8 bits): KBP_PER_STAGE k-block positions of BOTH 16-row
+  // blocks of a pair, or twice as many of a single block (the ring slot is always used in full).  The last stage of
+  // a unit may be short.
   const int spu2 = (n_kb + KBP_PER_STAGE - 1) / KBP_PER_STAGE, spu1 = (n_kb + 2 * KBP_PER_STAGE - 1) / (2 * KBP_PER_STAGE);
   // this CTA's contiguous range of 16-row blocks, processed as pairs and at most one single
   const int rb_lo = (int)(((long long)blockIdx.x * p.n_rb) / gridDim.x);
@@ -386,32 +404,33 @@ __global__ void __launch_bounds__(NTHREADS, 2) q4_gemv_kernel(const Params p) {
         const uint8_t* st_base = smem + L.ring + slot * STAGE_BYTES + lane * 16;
         const uint8_t* xq = xf_lane + kb0 * xf_step;
         if (!p.nocompute) {
+          constexpr int NPAIR = KBP_PER_STAGE / NCW, NSINGLE = 2 * KBP_PER_STAGE / NCW;   // positions per warp
           if (halves == MAX_HALVES) {
             if (nkb == KBP_PER_STAGE) {
 #pragma unroll
-              for (int i = 0; i < 2; ++i) {
+              for (int i = 0; i < NPAIR; ++i) {
                 const int kbl = i * NCW + warp;
-                kblock_imma<MAX_HALVES>(acc, st_base + kbl * KB_BYTES, *reinterpret_cast<const uint4*>(xq + kbl * xf_step));
+                kblock_imma<MAX_HALVES, W8>(acc, st_base + kbl * KB_BYTES, *reinterpret_cast<const uint4*>(xq + kbl * xf_step));
               }
             } else {
 #pragma unroll
-              for (int i = 0; i < 2; ++i) {
+              for (int i = 0; i < NPAIR; ++i) {
                 const int kbl = i * NCW + warp;
-                if (kbl < nkb) kblock_imma<MAX_HALVES>(acc, st_base + kbl * KB_BYTES, *reinterpret_cast<const uint4*>(xq + kbl * xf_step));
+                if (kbl < nkb) kblock_imma<MAX_HALVES, W8>(acc, st_base + kbl * KB_BYTES, *reinterpret_cast<const uint4*>(xq + kbl * xf_step));
               }
             }
           } else {
             if (nkb == 2 * KBP_PER_STAGE) {
 #pragma unroll
-              for (int i = 0; i < 4; ++i) {
+              for (int i = 0; i < NSINGLE; ++i) {
                 const int kbl = i * NCW + warp;
-                single_imma(acc[i & 1], st_base + kbl * KB_BYTES, *reinterpret_cast<const uint4*>(xq + kbl * xf_step));
+                single_imma<W8>(acc[i & 1], st_base + kbl * KB_BYTES, *reinterpret_cast<const uint4*>(xq + kbl * xf_step));
               }
             } else {
 #pragma unroll
-              for (int i = 0; i < 4; ++i) {
+              for (int i = 0; i < NSINGLE; ++i) {
                 const int kbl = i * NCW + warp;
-                if (kbl < nkb) single_imma(acc[i & 1], st_base + kbl * KB_BYTES, *reinterpret_cast<const uint4*>(xq + kbl * xf_step));
+                if (kbl < nkb) single_imma<W8>(acc[i & 1], st_base + kbl * KB_BYTES, *reinterpret_cast<const uint4*>(xq + kbl * xf_step));
               }
             }
           }
@@ -421,7 +440,8 @@ __global__ void __launch_bounds__(NTHREADS, 2) q4_gemv_kernel(const Params p) {
         if (++slot == p.nst) { slot = 0; phase ^= 1; }
       }
       // 16 x 8 result: lane (g, t) holds rows g (c0, c1) and g + 8 (c2, c3) of columns 2t, 2t + 1 = digits 2t, 2t + 1.
-      // row g = D[g] - D[g+8] (the unmasked byte carried 16 * level[g+8] as well), row g + 8 = D[g+8] / 16 (exact)
+      // 4 bits: row g = D[g] - D[g+8] (the unmasked byte carried 16 * level[g+8] as well), row g + 8 = D[g+8] / 16
+      // (exact); 8 bits: the rows are D[g] and D[g+8] themselves
       const int buf = u & 1;
       named_bar_sync(4 + buf, NCW * 32 + 32);  // the epilogue warp has drained this scratch buffer (two units ago)
       if (t4 < 2) {
@@ -436,8 +456,13 @@ __global__ void __launch_bounds__(NTHREADS, 2) q4_gemv_kernel(const Params p) {
           const int c0 = acc[h][0][0] + acc[h][1][0], c1 = acc[h][0][1] + acc[h][1][1];
           const int c2 = acc[h][0][2] + acc[h][1][2], c3 = acc[h][0][3] + acc[h][1][3];
           int* dst = scratch + (((buf * NCW + warp) * MAX_HALVES + h) * RB + (lane >> 2)) * 4 + 2 * t4;
-          *reinterpret_cast<int2*>(dst) = make_int2(c0 - c2, c1 - c3);
-          *reinterpret_cast<int2*>(dst + 8 * 4) = make_int2(c2 >> 4, c3 >> 4);
+          if constexpr (W8) {
+            *reinterpret_cast<int2*>(dst) = make_int2(c0, c1);
+            *reinterpret_cast<int2*>(dst + 8 * 4) = make_int2(c2, c3);
+          } else {
+            *reinterpret_cast<int2*>(dst) = make_int2(c0 - c2, c1 - c3);
+            *reinterpret_cast<int2*>(dst + 8 * 4) = make_int2(c2 >> 4, c3 >> 4);
+          }
         }
       }
       __syncwarp();
@@ -560,6 +585,40 @@ __global__ void q4_untile_i8_kernel(const uint32_t* __restrict__ tiled, uint8_t*
   qw[idx] = b;
 }
 
+// 8-bit levels (reference layout: byte [k][o], quantization.py:386-390 with one entry per byte) ->
+// [N/16 row blocks][K/64 k blocks][2 chunks][32 lanes][4 words]: word w of lane (g, t) in chunk c holds row
+// g + 8 (w & 1), k = 64 kb + 32 c + 8 t + 4 (w >> 1) + (0..3) -- the A fragment of mma.m16n8k32 against the
+// activation words the prologue builds (k = 64 kb + 32 c + 8 t + 4 j + i).  Rows beyond N are zero.
+__global__ void w8_tile_i8_kernel(const uint8_t* __restrict__ qw, uint32_t* __restrict__ out, int N, int K) {
+  const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;  // one output word
+  const int n_kb = K / KB;
+  const int n_rb = (N + RB - 1) / RB;
+  const size_t total = (size_t)n_rb * n_kb * 2 * 32 * 4;
+  if (idx >= total) return;
+  const int wd = idx & 3, lane = (idx >> 2) & 31, c = (idx >> 7) & 1;
+  const size_t rest = idx >> 8;
+  const int kb = (int)(rest % n_kb), rb = (int)(rest / n_kb);
+  const int row = rb * RB + (lane >> 2) + 8 * (wd & 1);
+  const int k0 = kb * KB + 32 * c + 8 * (lane & 3) + 4 * (wd >> 1);
+  uint32_t w = 0;
+  if (row < N) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) w |= (uint32_t)qw[(size_t)(k0 + i) * N + row] << (8 * i);
+  }
+  out[idx] = w;
+}
+
+__global__ void w8_untile_i8_kernel(const uint8_t* __restrict__ tiled, uint8_t* __restrict__ qw, int N, int K) {
+  const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;  // one byte [k][o]
+  const size_t total = (size_t)K * N;
+  if (idx >= total) return;
+  const int o = (int)(idx % N), k = (int)(idx / N);
+  const int kb = k / KB, kl = k % KB, c = kl >> 5, t = (kl >> 3) & 3, j = (kl >> 2) & 1, i = kl & 3;
+  const int rb = o / RB, rl = o % RB;
+  const size_t word = ((((size_t)rb * (K / KB) + kb) * 2 + c) * 32 + (rl & 7) * 4 + t) * 4 + 2 * j + (rl >> 3);
+  qw[idx] = tiled[word * 4 + i];
+}
+
 }  // namespace q4mv
 }  // namespace b2l
 
@@ -589,10 +648,33 @@ extern "C" int b2l_q4_untile_i8(const void* qw_tiled, void* qw, int N, int K, b2
   return 0;
 }
 
+extern "C" size_t b2l_w8_tiled_i8_bytes(int N, int K) {
+  if (N <= 0 || K <= 0 || K % KB != 0) return 0;
+  return (size_t)((N + RB - 1) / RB) * (K / KB) * WTile<true>::KB_BYTES;
+}
+
+extern "C" int b2l_w8_tile_i8(const void* qw, void* qw_tiled, int N, int K, b2l_stream_t stream) {
+  B2L_CHECK_ARG(qw && qw_tiled && N > 0 && K > 0, "b2l_w8_tile_i8: bad argument");
+  B2L_CHECK_SUPPORTED(K % KB == 0, "b2l_w8_tile_i8: in_features %d must be a multiple of %d", K, KB);
+  const size_t total = b2l_w8_tiled_i8_bytes(N, K) / 4;
+  w8_tile_i8_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>((const uint8_t*)qw, (uint32_t*)qw_tiled, N, K);
+  B2L_LAUNCH_CHECK("w8_tile_i8_kernel");
+  return 0;
+}
+
+extern "C" int b2l_w8_untile_i8(const void* qw_tiled, void* qw, int N, int K, b2l_stream_t stream) {
+  B2L_CHECK_ARG(qw && qw_tiled && N > 0 && K > 0, "b2l_w8_untile_i8: bad argument");
+  B2L_CHECK_SUPPORTED(K % KB == 0, "b2l_w8_untile_i8: in_features %d must be a multiple of %d", K, KB);
+  const size_t total = (size_t)K * N;
+  w8_untile_i8_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>((const uint8_t*)qw_tiled, (uint8_t*)qw, N, K);
+  B2L_LAUNCH_CHECK("w8_untile_i8_kernel");
+  return 0;
+}
+
 namespace {
 constexpr int MAX_K = 12 * NCW * 32 * 8;   // 24576
 
-template <int MAXC, int NDIG>
+template <int MAXC, int NDIG, bool W8>
 int launch_gemv(const Params& p0, int ctas_per_sm, int grid_override, bool pdl, cudaStream_t stream) {
   Params p = p0;
   // ring: as deep as fits `ctas_per_sm` CTAs per SM
@@ -611,30 +693,34 @@ int launch_gemv(const Params& p0, int ctas_per_sm, int grid_override, bool pdl, 
   p.nst = nst;
   const SmemLayout L = smem_layout(nst, p.K, NDIG);
   static DynSmemCache smem_cache;
-  if (int rc = ensure_dyn_smem(q4_gemv_kernel<MAXC, NDIG>, L.total, smem_cache)) return rc;
+  if (int rc = ensure_dyn_smem(q4_gemv_kernel<MAXC, NDIG, W8>, L.total, smem_cache)) return rc;
   int grid = grid_override > 0 ? grid_override : ctas_per_sm * sm_count();
   if (grid > p.n_rb) grid = p.n_rb;
   LaunchCfg lc(dim3(grid), dim3(NTHREADS), L.total, stream, pdl, 1);
-  B2L_CUDA(cudaLaunchKernelEx(&lc.cfg, q4_gemv_kernel<MAXC, NDIG>, p));
+  B2L_CUDA(cudaLaunchKernelEx(&lc.cfg, q4_gemv_kernel<MAXC, NDIG, W8>, p));
   return 0;
 }
-}  // namespace
 
-extern "C" int b2l_q4_gemv(const b2l_q4_linear_args* a, b2l_stream_t stream) {
-  B2L_CHECK_ARG(a != nullptr, "b2l_q4_gemv: null args");
-  B2L_CHECK_ARG(a->x && a->qw_tiled && a->scales && a->zeros && a->y, "b2l_q4_gemv: null pointer");
-  B2L_CHECK_SUPPORTED(a->M == 1, "b2l_q4_gemv: M=%d (this kernel is the batch-1 path; use b2l_q4_gemv_batch / b2l_q4_linear_tc)", a->M);
-  B2L_CHECK_SUPPORTED(a->K > 0 && a->K % KB == 0 && a->K <= MAX_K, "b2l_q4_gemv: K=%d must be a multiple of %d and <= %d", a->K, KB, MAX_K);
-  B2L_CHECK_ARG(a->N > 0, "b2l_q4_gemv: bad N");
-  B2L_CHECK_ARG(((uintptr_t)a->x % 16 == 0) && ((uintptr_t)a->qw_tiled % 16 == 0), "b2l_q4_gemv: x / qw_tiled must be 16-byte aligned");
-  B2L_CHECK_ARG(a->sz_dtype == B2L_BF16 || a->sz_dtype == B2L_F32, "b2l_q4_gemv: bad sz_dtype");
+// b2l_q4_gemv (W8 = false) and b2l_w8_gemv (W8 = true): the same checks, argument block and launch policy
+template <bool W8>
+int gemv_entry(const b2l_q4_linear_args* a, b2l_stream_t stream) {
+  const char* fn = W8 ? "b2l_w8_gemv" : "b2l_q4_gemv";
+  B2L_CHECK_ARG(a != nullptr, "%s: null args", fn);
+  B2L_CHECK_ARG(a->x && a->qw_tiled && a->scales && a->zeros && a->y, "%s: null pointer", fn);
+  B2L_CHECK_SUPPORTED(a->M == 1, "%s: M=%d (this kernel is the batch-1 path; use %s)", fn, a->M,
+                      W8 ? "b2l_w8_gemm" : "b2l_q4_gemv_batch / b2l_q4_linear_tc");
+  B2L_CHECK_SUPPORTED(a->K > 0 && a->K % KB == 0 && a->K <= MAX_K, "%s: K=%d must be a multiple of %d and <= %d", fn, a->K, KB, MAX_K);
+  B2L_CHECK_ARG(a->N > 0, "%s: bad N", fn);
+  B2L_CHECK_ARG(((uintptr_t)a->x % 16 == 0) && ((uintptr_t)a->qw_tiled % 16 == 0), "%s: x / qw_tiled must be 16-byte aligned", fn);
+  B2L_CHECK_ARG(a->sz_dtype == B2L_BF16 || a->sz_dtype == B2L_F32, "%s: bad sz_dtype", fn);
+  if (W8) B2L_CHECK_SUPPORTED((a->flags & ~(B2L_F_PDL | B2L_F_DEBUG_NOCOMPUTE)) == 0, "%s: unknown flags 0x%x", fn, a->flags);
   if (a->prologue == B2L_PRO_RMSNORM)
-    B2L_CHECK_ARG(a->norm_scale && ((uintptr_t)a->norm_scale % 16 == 0), "b2l_q4_gemv: RMSNorm prologue needs a 16-byte aligned scale");
+    B2L_CHECK_ARG(a->norm_scale && ((uintptr_t)a->norm_scale % 16 == 0), "%s: RMSNorm prologue needs a 16-byte aligned scale", fn);
   else
-    B2L_CHECK_ARG(a->prologue == B2L_PRO_NONE, "b2l_q4_gemv: bad prologue %d", a->prologue);
-  if (a->epilogue == B2L_EPI_RESIDUAL) B2L_CHECK_ARG(a->res != nullptr, "b2l_q4_gemv: RESIDUAL epilogue needs res");
-  else if (a->epilogue == B2L_EPI_SWIGLU) B2L_CHECK_SUPPORTED(a->N % RB == 0, "b2l_q4_gemv: SWIGLU needs N %% 16 == 0");
-  else B2L_CHECK_ARG(a->epilogue == B2L_EPI_STORE, "b2l_q4_gemv: bad epilogue %d", a->epilogue);
+    B2L_CHECK_ARG(a->prologue == B2L_PRO_NONE, "%s: bad prologue %d", fn, a->prologue);
+  if (a->epilogue == B2L_EPI_RESIDUAL) B2L_CHECK_ARG(a->res != nullptr, "%s: RESIDUAL epilogue needs res", fn);
+  else if (a->epilogue == B2L_EPI_SWIGLU) B2L_CHECK_SUPPORTED(a->N % RB == 0, "%s: SWIGLU needs N %% 16 == 0", fn);
+  else B2L_CHECK_ARG(a->epilogue == B2L_EPI_STORE, "%s: bad epilogue %d", fn, a->epilogue);
 
   Params p;
   p.x = (const __nv_bfloat16*)a->x;
@@ -659,7 +745,7 @@ extern "C" int b2l_q4_gemv(const b2l_q4_linear_args* a, b2l_stream_t stream) {
     B2L_CHECK_ARG(a->pf_kv[1] != nullptr && a->pf_rows != nullptr && a->pf_rows_max > 0 && a->pf_nseg > 0 && a->pf_row_bytes > 0 &&
                       a->pf_row_bytes % 16 == 0 && a->pf_seg_stride % 16 == 0 && ((uintptr_t)a->pf_kv[0] % 16 == 0) &&
                       ((uintptr_t)a->pf_kv[1] % 16 == 0) && (unsigned long long)a->pf_rows_max * a->pf_row_bytes < (1ull << 31),
-                  "b2l_q4_gemv: bad strided prefetch hint");
+                  "%s: bad strided prefetch hint", fn);
     p.pf_kv[0] = (const uint8_t*)a->pf_kv[0]; p.pf_kv[1] = (const uint8_t*)a->pf_kv[1];
     p.pf_rows = a->pf_rows; p.pf_rows_max = a->pf_rows_max; p.pf_nseg = a->pf_nseg; p.pf_row_bytes = a->pf_row_bytes;
     p.pf_seg_stride = a->pf_seg_stride;
@@ -669,7 +755,7 @@ extern "C" int b2l_q4_gemv(const b2l_q4_linear_args* a, b2l_stream_t stream) {
     p.pf_bytes[i] = 0;
     if (a->pf_ptr[i] != nullptr && a->pf_bytes[i] != 0) {
       B2L_CHECK_ARG(((uintptr_t)a->pf_ptr[i] % 16 == 0) && (a->pf_bytes[i] % 16 == 0) && a->pf_bytes[i] < (1ull << 31),
-                    "b2l_q4_gemv: prefetch segment %d must be 16-byte aligned, a multiple of 16 and < 2 GiB", i);
+                    "%s: prefetch segment %d must be 16-byte aligned, a multiple of 16 and < 2 GiB", fn, i);
       p.pf_bytes[i] = (uint32_t)a->pf_bytes[i];
       p.pf_mode = env_pf_mode;
     }
@@ -680,7 +766,12 @@ extern "C" int b2l_q4_gemv(const b2l_q4_linear_args* a, b2l_stream_t stream) {
   cudaStream_t st = (cudaStream_t)stream;
   const int grid = a->split_k;  // split_k doubles as a grid override
   // three digits (|X| < 2^22) everywhere: the prologue's fma conversion needs the integer inside a float mantissa
-  if (a->K <= 12288) return launch_gemv<6, 3>(p, env_cps > 0 ? env_cps : 2, grid, pdl, st);
-  if (a->K <= 16384) return launch_gemv<12, 3>(p, env_cps > 0 ? env_cps : 2, grid, pdl, st);
-  return launch_gemv<12, 3>(p, 1, grid, pdl, st);
+  if (a->K <= 12288) return launch_gemv<6, 3, W8>(p, env_cps > 0 ? env_cps : 2, grid, pdl, st);
+  if (a->K <= 16384) return launch_gemv<12, 3, W8>(p, env_cps > 0 ? env_cps : 2, grid, pdl, st);
+  return launch_gemv<12, 3, W8>(p, 1, grid, pdl, st);
 }
+}  // namespace
+
+extern "C" int b2l_q4_gemv(const b2l_q4_linear_args* a, b2l_stream_t stream) { return gemv_entry<false>(a, stream); }
+
+extern "C" int b2l_w8_gemv(const b2l_q4_linear_args* a, b2l_stream_t stream) { return gemv_entry<true>(a, stream); }

@@ -125,7 +125,7 @@ def main(
     model.load_state_dict(checkpoint)
     print(f"Time to load model: {time.time() - t0:.02f} seconds.", file=sys.stderr)
     model.eval()
-    if quantize == "gptq.int4" and os.environ.get("B2L_COMPACT", "1") != "0":
+    if quantize in ("gptq.int4", "gptq.int8") and os.environ.get("B2L_COMPACT", "1") != "0":
         try:
             model.compact()   # one resident copy of the weights (the reference-layout buffers come back on state_dict())
         except RuntimeError:  # a layer the fused decode step cannot run (grouped scales, odd widths): keep everything

@@ -9,7 +9,8 @@ bf16 - there is no CPU fallback.
 Two execution paths behind `LLaMA.forward`:
   * decode (T == 1 with a KV cache, every Linear a gptq.int4 layer with one (scale, zero) per row):
     one C call enqueues the whole token (`b2l_decode_step`: int8-MMA GEMV kernels for batch 1, f16-MMA for 2..8 rows,
-    wgmma for 9..16), replayed as a CUDA graph.
+    wgmma for 9..16), replayed as a CUDA graph.  Every Linear a per-row gptq.int8 layer: the same step at batch 1
+    (B2L_F_W8: the GEMV kernel with 8-bit weights); batches of 2 or more go module by module (on the wgmma GEMM).
   * everything else (prefill on the wgmma GEMM, no-cache forward, other Linear kinds): module by module.
 """
 import ctypes as C
@@ -252,7 +253,10 @@ class _DecodeState:
 
         from .quantization import BATCH_GEMV, batch_workspace
 
-        # batch 1..8: mma.sync kernels (q4_gemv / q4_gemv_batch) and their tiling; 9..16: wgmma kernel and its tiling
+        # batch 1..8: mma.sync kernels (q4_gemv / q4_gemv_batch) and their tiling; 9..16: wgmma kernel and its tiling.
+        # gptq.int8 (batch 1 only): the batch-1 kernel with 8-bit weights (b2l_w8_tile_i8 tilings)
+        w8 = model._fast_ok == "w8"
+        assert B == 1 or not w8
         gemv = (B == 1) or (B <= 8 and BATCH_GEMV)
         self.batch_ws = None
         if gemv and B > 1:
@@ -291,12 +295,13 @@ class _DecodeState:
             idx_is_i64=1 if idx_dtype == torch.int64 else 0, input_pos=self.pos.data_ptr(),
             ring_start=model._ring.data_ptr(), block_size=cfg.block_size, x=self.x.data_ptr(), qkv=self.qkv.data_ptr(),
             att=self.att.data_ptr(), hid=self.hid.data_ptr(), attn_work=self.work.data_ptr(),
-            logits=self.logits.data_ptr(), flags=model.decode_flags,
+            logits=self.logits.data_ptr(), flags=model.decode_flags | (L.F_W8 if w8 else 0),
             batch_work=None if self.batch_ws is None else self.batch_ws.data_ptr())
-        # batch 1, head_size 128: the whole step as ONE persistent kernel (csrc/decode_mega.cu)
+        # batch 1, head_size 128: the whole step as ONE persistent kernel (csrc/decode_mega.cu; int4 weights only, so
+        # gptq.int8 keeps one kernel per op under B2L_PERSISTENT=1 too)
         self.plan = None
         kmax = max(C_, n_hidden)
-        if model.persistent and B == 1 and hs == 128 and kmax <= 12288:
+        if model.persistent and not w8 and B == 1 and hs == 128 and kmax <= 12288:
             self.plan = torch.zeros(lib.b2l_decode_plan_bytes(C.byref(self.args)), dtype=torch.uint8, device=device)
             self.args.plan = self.plan.data_ptr()
             L.check(lib.b2l_decode_plan_build(C.byref(self.args), L.stream_ptr()), "b2l_decode_plan_build")
@@ -346,7 +351,9 @@ class LLaMA(nn.Module):
         self._kv_store: Optional[torch.Tensor] = None
         self._decode: Optional[_DecodeState] = None
         self._module_graph = None  # CUDA graph of the module-by-module decode step (non-fused Linear kinds)
-        self._fast_ok: Optional[bool] = None  # every Linear is a per-row gptq.int4 layer the fused step can run (checked once)
+        # the fused step can run every Linear (checked once): "q4" (per-row gptq.int4, any B <= 16), "w8" (per-row
+        # gptq.int8, B == 1), False (module path)
+        self._fast_ok: Union[None, bool, str] = None
         self._fc12_cache = {}
 
     def _init_weights(self, module: nn.Module) -> None:
@@ -383,7 +390,8 @@ class LLaMA(nn.Module):
     def _fc12(self, i: int, kind: str):
         """c_fc1 and c_fc2 of layer i interleaved (8 rows / 8 rows per 16-row block for the
         batch-1 kernel, 64 / 64 per 128-row tile for the wgmma kernel) and re-tiled, so one
-        tile holds silu's argument and its multiplier and SwiGLU runs in the epilogue."""
+        tile holds silu's argument and its multiplier and SwiGLU runs in the epilogue.
+        "i8" tiles 4-bit layers with b2l_q4_tile_i8 and 8-bit ones with b2l_w8_tile_i8."""
         mlp = self.transformer.h[i].mlp
         gemv = kind != "tc"
         hit = self._fc12_cache.get((i, kind))
@@ -405,8 +413,9 @@ class LLaMA(nn.Module):
         zeros = inter(mlp.c_fc1.zeros, mlp.c_fc2.zeros).contiguous()
         lib = L.lib()
         if kind == "i8":
-            tiled = torch.empty(lib.b2l_q4_tiled_i8_bytes(2 * nh, K), dtype=torch.uint8, device=qw.device)
-            L.check(lib.b2l_q4_tile_i8(qw.data_ptr(), tiled.data_ptr(), 2 * nh, K, L.stream_ptr()), "b2l_q4_tile_i8")
+            from .quantization import tile_i8
+
+            tiled = tile_i8(qw, 2 * nh, K, mlp.c_fc1.bits)
         elif kind == "mma":
             tiled = torch.empty(lib.b2l_q4_tiled_mma_bytes(2 * nh, K), dtype=torch.uint8, device=qw.device)
             L.check(lib.b2l_q4_tile_mma(qw.data_ptr(), tiled.data_ptr(), 2 * nh, K, L.stream_ptr()), "b2l_q4_tile_mma")
@@ -426,17 +435,19 @@ class LLaMA(nn.Module):
 
     def _fc_from_fc12(self, i: int, which: int) -> torch.Tensor:
         """c_fc1 (which = 0) or c_fc2 (1) of layer i in the reference layout, rebuilt from the interleaved batch-1
-        tiling (compacted models keep only that copy): untile (a nibble permutation) and take every other 8 rows."""
+        tiling (compacted models keep only that copy): untile (a permutation, by bit width) and take every other 8
+        rows."""
         tiled, _, _ = self._fc12_cache[(i, "i8")][1]
         mlp = self.transformer.h[i].mlp
-        nh, K = mlp.c_fc1.out_features, mlp.c_fc1.in_features
-        both = torch.empty((K // 2, 2 * nh), dtype=torch.uint8, device=tiled.device).t()
-        L.check(L.lib().b2l_q4_untile_i8(tiled.data_ptr(), both.data_ptr(), 2 * nh, K, L.stream_ptr()), "b2l_q4_untile_i8")
-        return both.contiguous().reshape(nh // 8, 2, 8, K // 2)[:, which].reshape(nh, K // 2).t().contiguous().t()
+        nh, K, epb = mlp.c_fc1.out_features, mlp.c_fc1.in_features, mlp.c_fc1.entries_per_byte
+        name = "b2l_w8_untile_i8" if mlp.c_fc1.bits == 8 else "b2l_q4_untile_i8"
+        both = torch.empty((K // epb, 2 * nh), dtype=torch.uint8, device=tiled.device).t()
+        L.check(getattr(L.lib(), name)(tiled.data_ptr(), both.data_ptr(), 2 * nh, K, L.stream_ptr()), name)
+        return both.contiguous().reshape(nh // 8, 2, 8, K // epb)[:, which].reshape(nh, K // epb).t().contiguous().t()
 
     def compact(self) -> "LLaMA":
-        """Keep ONE resident copy of every gptq.int4 weight: the batch-1 decode tiling (c_fc1 / c_fc2: the interleaved
-        fc1|fc2 tiling).  The reference-layout buffers and the per-kernel duplicates are freed; `state_dict()`, prefill
+        """Keep ONE resident copy of every gptq.int4 (or, uniformly, gptq.int8) weight: the batch-1 decode tiling
+        (c_fc1 / c_fc2: the interleaved fc1|fc2 tiling).  The reference-layout buffers and the per-kernel duplicates are freed; `state_dict()`, prefill
         and batched decode rebuild what they need transiently from that copy (bit-exact permutations).  7B: 3.3 GB of
         weights + 0.26 GB embedding + KV cache instead of 2-3 copies (the reference's gptq.int4 figure is "~5 GB",
         howto/inference.md:37).  Returns self."""
@@ -445,7 +456,8 @@ class LLaMA(nn.Module):
         if self._fast_ok is None:
             self._fast_ok = self._fast_decode_ok()
         if not self._fast_ok:
-            raise RuntimeError("compact() needs a gptq.int4 model the fused batch-1 decode step can run")
+            raise RuntimeError("compact() needs a gptq.int4 or gptq.int8 model the fused batch-1 decode step can run "
+                               "(one bit width for every linear)")
         for i, blk in enumerate(self.transformer.h):
             self._fc12(i, "i8")
             for kind in ("mma", "tc"):
@@ -459,11 +471,18 @@ class LLaMA(nn.Module):
         torch.cuda.empty_cache()
         return self
 
-    def _fast_decode_ok(self) -> bool:
+    def _fast_decode_ok(self) -> Union[bool, str]:
+        """"q4" / "w8" when every Linear is a per-row gptq.int4 / gptq.int8 layer the fused step can run, else False."""
         from .quantization import ColBlockQuantizedLinear
 
+        if not isinstance(self.lm_head, ColBlockQuantizedLinear):
+            return False
+        kind = "w8" if self.lm_head.bits == 8 else "q4"
+
         def ok(m):
-            return isinstance(m, ColBlockQuantizedLinear) and m.tc_capable and m.gemv_capable
+            if not isinstance(m, ColBlockQuantizedLinear):
+                return False
+            return m.w8_gemv_capable if kind == "w8" else (m.tc_capable and m.gemv_capable)
 
         if not ok(self.lm_head) or self.config.n_embd % 8 != 0:
             return False
@@ -474,7 +493,7 @@ class LLaMA(nn.Module):
                 return False
             if blk.mlp.c_fc1.out_features % 64 != 0:
                 return False
-        return True
+        return kind
 
     def logical_kv_caches(self) -> List[KVCache]:
         """kv_caches in the reference's slot order.  Identical to `kv_caches` until the
@@ -533,7 +552,8 @@ class LLaMA(nn.Module):
             if st is None or st.B != B or st.S != max_seq_length or st.idx.dtype != idx.dtype or st.idx.device != idx.device:
                 if self._fast_ok is None:
                     self._fast_ok = self._fast_decode_ok()
-                st = self._decode = _DecodeState(self, B, max_seq_length, idx.device, idx.dtype) if self._fast_ok else None
+                fast = bool(self._fast_ok) and (self._fast_ok != "w8" or B == 1)   # gptq.int8: batch 1 only
+                st = self._decode = _DecodeState(self, B, max_seq_length, idx.device, idx.dtype) if fast else None
         if st is not None:
             st.idx.copy_(idx.reshape(-1))
             st.pos.copy_(input_pos.reshape(-1)[-1:])
@@ -550,8 +570,8 @@ class LLaMA(nn.Module):
             st.calls += 1
             return st.logits.clone() if self.copy_logits else st.logits
 
-        # ---- single-token decode with any other Linear kind (llm.int8, gptq.int8, grouped scales, dense):
-        #      the module-by-module launch sequence, replayed as a CUDA graph once warm
+        # ---- single-token decode the fused step does not run (llm.int8, grouped or biased gptq, dense, gptq.int8 at
+        #      B >= 2): the module-by-module launch sequence, replayed as a CUDA graph once warm
         if input_pos is not None and T == 1 and self.graph_after and idx.dtype in (torch.int32, torch.int64):
             key = (B, max_seq_length, idx.dtype, idx.device, WEIGHTS_GENERATION[0])   # the graph bakes weight pointers too
             mg = self._module_graph

@@ -4,8 +4,9 @@
 (names, shapes, dtypes, strides) and `state_dict` keys (quantization.py:340-374), so a
 `llama-gptq.4bit.pth` produced by the reference's quantize/gptq.py loads unchanged.
 `forward` runs hand-written sm_90a kernels through the C ABI of include/b2l.h (M = 1: exact int8-digit MMA GEMV;
-2..8: f16 MMA batch kernel; 9..16: wgmma with weights from registers; > 16: wgmma 128 x 128 tile GEMM); there is no
-Triton, no library GEMM, no dense fallback and no CPU path.
+2..8: f16 MMA batch kernel; 9..16: wgmma with weights from registers; > 16: wgmma 128 x 128 tile GEMM; gptq.int8:
+the same GEMV at M = 1 and the same GEMM for M >= 2); there is no Triton, no library GEMM, no dense fallback and no
+CPU path.
 """
 import ctypes as C
 import os
@@ -113,16 +114,19 @@ class ColBlockQuantizedLinear(torch.nn.Module):
 
     # ------------------------------------------------------------------ one resident copy of the weights
     def reference_quant_weight(self) -> torch.Tensor:
-        """`quant_weight` in the reference layout (uint8 (out, in/2), strides (1, out), quantization.py:350-359).  The
+        """`quant_weight` in the reference layout (uint8 (out, in/epb), strides (1, out), quantization.py:350-359).  The
         registered buffer itself unless release_reference_layout() freed it: then a TRANSIENT tensor rebuilt from the
-        batch-1 kernel's tiling (b2l_q4_untile_i8: a pure nibble permutation, tested bit-exact) or by `_source`."""
+        batch-1 kernel's tiling (b2l_q4_untile_i8 / b2l_w8_untile_i8: pure permutations, tested bit-exact) or by
+        `_source`."""
         if not self._released:
             return self.quant_weight
         if self._source is not None:
             return self._source()
-        out = torch.empty((self.in_features // 2, self.out_features), dtype=torch.uint8, device=self._tiled_i8.device).t()
-        L.check(L.lib().b2l_q4_untile_i8(self._tiled_i8.data_ptr(), out.data_ptr(), self.out_features, self.in_features, L.stream_ptr()),
-                "b2l_q4_untile_i8")
+        out = torch.empty((self.in_features // self.entries_per_byte, self.out_features), dtype=torch.uint8,
+                          device=self._tiled_i8.device).t()
+        name = "b2l_w8_untile_i8" if self.bits == 8 else "b2l_q4_untile_i8"
+        L.check(getattr(L.lib(), name)(self._tiled_i8.data_ptr(), out.data_ptr(), self.out_features, self.in_features, L.stream_ptr()),
+                name)
         return out
 
     def release_reference_layout(self, source=None) -> None:
@@ -133,8 +137,11 @@ class ColBlockQuantizedLinear(torch.nn.Module):
         case this module keeps no tiling of its own.  Loading a state dict brings the buffer back."""
         if self._released:
             return
-        if not self.gemv_capable:
-            raise RuntimeError("release_reference_layout needs a gptq.int4 layer the batch-1 kernel can run (4 bits, per-row scales, in % 64 == 0)")
+        if not self.scales.is_cuda:
+            raise RuntimeError(f"release_reference_layout: the layer is on {self.scales.device}; its tiling is built on CUDA only")
+        if not (self.gemv_capable or self.w8_gemv_capable):
+            raise RuntimeError("release_reference_layout needs a gptq.int4 / gptq.int8 layer the batch-1 kernel can run "
+                               "(per-row scales, no bias, in % 64 == 0)")
         if source is None:
             self.tiled_i8()
         self._released, self._source = True, source
@@ -201,22 +208,17 @@ class ColBlockQuantizedLinear(torch.nn.Module):
         return self._tiled
 
     def tiled_i8(self) -> torch.Tensor:
-        """The [N/16][K/64][32 lanes][16 B] re-tiling of the batch-1 kernel (b2l_q4_tile_i8: int8-MMA fragments)."""
+        """The re-tiling of the batch-1 kernel (int8-MMA fragments): [N/16][K/64][32 lanes][16 B] of packed nibbles
+        (b2l_q4_tile_i8) at 4 bits, [N/16][K/64][2][32 lanes][16 B] of levels (b2l_w8_tile_i8) at 8 bits."""
         if self._released and self._source is None:
             return self._tiled_i8     # the resident copy
         qw = self.reference_quant_weight()
         key = (qw.data_ptr(), qw._version)
-        if self._released:            # c_fc1 / c_fc2 after compaction: transient, from the interleaved copy
-            t = torch.empty(L.lib().b2l_q4_tiled_i8_bytes(self.out_features, self.in_features), dtype=torch.uint8, device=qw.device)
-            L.check(L.lib().b2l_q4_tile_i8(qw.data_ptr(), t.data_ptr(), self.out_features, self.in_features, L.stream_ptr()),
-                    "b2l_q4_tile_i8")
-            return t
-        if self._tiled_i8 is None or self._tiled_i8_key != key:
+        if self._released or self._tiled_i8 is None or self._tiled_i8_key != key:
             self._check_layout()
-            nbytes = L.lib().b2l_q4_tiled_i8_bytes(self.out_features, self.in_features)
-            t = torch.empty(nbytes, dtype=torch.uint8, device=qw.device)
-            L.check(L.lib().b2l_q4_tile_i8(qw.data_ptr(), t.data_ptr(), self.out_features, self.in_features, L.stream_ptr()),
-                    "b2l_q4_tile_i8")
+            t = tile_i8(qw, self.out_features, self.in_features, self.bits)
+            if self._released:        # c_fc1 / c_fc2 after compaction: transient, from the interleaved copy
+                return t
             self._tiled_i8, self._tiled_i8_key = t, key
         return self._tiled_i8
 
@@ -239,6 +241,17 @@ class ColBlockQuantizedLinear(torch.nn.Module):
     def gemv_capable(self) -> bool:
         return self.tc_capable and self.in_features % 64 == 0 and self.in_features <= 24576
 
+    @property
+    def w8_capable(self) -> bool:
+        """gptq.int8 on the wgmma GEMM (M >= 2): 8 bits, one (scale, zero) per row, K % 64 == 0, no bias."""
+        return (self.bits == 8 and self.scales.shape[1] == 1 and self.in_features % 64 == 0 and self.bias is None
+                and self.zeros.dtype == self.scales.dtype)
+
+    @property
+    def w8_gemv_capable(self) -> bool:
+        """gptq.int8 on the batch-1 kernel (M == 1): w8_capable and K <= 24576."""
+        return self.w8_capable and self.in_features <= 24576
+
     def forward(self, inp):
         L.require_cuda_bf16(inp, "ColBlockQuantizedLinear.forward")
         if self.scales.device != inp.device:
@@ -255,7 +268,24 @@ class ColBlockQuantizedLinear(torch.nn.Module):
         aligned = x.data_ptr() % 16 == 0 and x.stride(0) % 8 == 0
         # `wt` keeps a transient tiling (released layers) alive until its launch is enqueued; the caching allocator
         # hands freed blocks out in stream order, so the kernel has finished before anybody else writes there
-        if self.gemv_capable and aligned and M == 1:
+        if self.w8_gemv_capable and aligned and M == 1:
+            wt = self.tiled_i8()
+            a = L.Q4LinearArgs(
+                x=x.data_ptr(), ldx=x.stride(0), qw_tiled=wt.data_ptr(), scales=self.scales.data_ptr(),
+                zeros=self.zeros.data_ptr(), sz_dtype=L.sz_dtype_of(self.scales), y=y.data_ptr(), ldy=N, M=1, N=N, K=K,
+                prologue=L.PRO_NONE, norm_scale=None, eps=0.0, epilogue=L.EPI_STORE, res=None, ldres=0, split_k=0, flags=0)
+            L.check(L.lib().b2l_w8_gemv(C.byref(a), L.stream_ptr()), "b2l_w8_gemv")
+        elif self.w8_capable and aligned:
+            # the wgmma GEMM reads quant_weight in the reference layout (a compacted layer rebuilds it transiently)
+            self._check_layout()
+            wt = self.reference_quant_weight()
+            a = L.Q4LinearArgs(
+                x=x.data_ptr(), ldx=x.stride(0), qw_tiled=wt.data_ptr(), scales=self.scales.data_ptr(),
+                zeros=self.zeros.data_ptr(), sz_dtype=L.sz_dtype_of(self.scales), y=y.data_ptr(), ldy=N,
+                M=M, N=N, K=K, prologue=L.PRO_NONE, norm_scale=None, eps=0.0, epilogue=L.EPI_STORE, res=None,
+                ldres=0, split_k=0, flags=0)
+            L.check(L.lib().b2l_w8_gemm(C.byref(a), L.stream_ptr()), "b2l_w8_gemm")
+        elif self.gemv_capable and aligned and M == 1:
             wt = self.tiled_i8()
             a = L.Q4LinearArgs(
                 x=x.data_ptr(), ldx=x.stride(0), qw_tiled=wt.data_ptr(), scales=self.scales.data_ptr(),
@@ -297,6 +327,16 @@ class ColBlockQuantizedLinear(torch.nn.Module):
                                       M, N, K, self.bits, self.tile_cols, L.stream_ptr())
             L.check(rc, "b2l_q_linear")
         return y.reshape(*shape[:-1], N)
+
+
+def tile_i8(qw: torch.Tensor, N: int, K: int, bits: int) -> torch.Tensor:
+    """The batch-1 kernel's tiling of quant_weight `qw` (reference layout) for `bits` 4 or 8: a new tensor."""
+    if not qw.is_cuda:
+        raise RuntimeError(f"tile_i8: quant_weight is on {qw.device}; the tiling kernels run on CUDA only")
+    kind = "w8" if bits == 8 else "q4"
+    t = torch.empty(getattr(L.lib(), f"b2l_{kind}_tiled_i8_bytes")(N, K), dtype=torch.uint8, device=qw.device)
+    L.check(getattr(L.lib(), f"b2l_{kind}_tile_i8")(qw.data_ptr(), t.data_ptr(), N, K, L.stream_ptr()), f"b2l_{kind}_tile_i8")
+    return t
 
 
 def qlinear_4bit_weight(inp, weight, scales, zeros):

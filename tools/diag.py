@@ -6,6 +6,7 @@ kernel only loses its section).  Usage on the GPU box:
     python tools/diag.py tc_small   # one section
 """
 import ctypes as C
+import gc
 import os
 import subprocess
 import sys
@@ -14,7 +15,7 @@ import time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-SECTIONS = ["generic", "tile", "tc_small", "tc_shapes", "tc_modes", "gemv", "grid_flag", "hmma_rate", "imma_rate", "consumer_rate", "bench_gemm", "bench_tc", "trace", "bench_layers", "bench_gemv", "bench_step", "bench_ctx", "bench_13b_b8", "bench_sizes", "batch_debug", "bench_step_int8", "bench_q8_gemm", "bench_q8_gemv", "timeline", "mega_timeline"]
+SECTIONS = ["generic", "tile", "tc_small", "tc_shapes", "tc_modes", "gemv", "grid_flag", "hmma_rate", "imma_rate", "consumer_rate", "bench_gemm", "bench_tc", "trace", "bench_layers", "bench_gemv", "bench_step", "bench_ctx", "bench_13b_b8", "bench_sizes", "batch_debug", "bench_step_int8", "bench_q8_gemm", "bench_q8_gemv", "bench_w8_gemv", "bench_w8_gemm", "bench_step_w8", "timeline", "mega_timeline"]
 
 
 _DLIB = None
@@ -898,6 +899,249 @@ def _time_graph(fn, reps):
         torch.cuda.synchronize()
         ts.append(e0.elapsed_time(e1) * 1e3 / reps)
     return sorted(ts)[1]
+
+
+
+def _w8_args(L, x, qt, sc, z, N, K, y, M=1, flags=0):
+    return L.Q4LinearArgs(x=x.data_ptr(), ldx=K, qw_tiled=qt.data_ptr(), scales=sc.data_ptr(), zeros=z.data_ptr(), sz_dtype=L.B2L_BF16,
+                          y=y.data_ptr(), ldy=N, M=M, N=N, K=K, prologue=0, norm_scale=None, eps=1e-5, epilogue=0, res=None, ldres=0,
+                          split_k=0, flags=flags)
+
+
+def sec_bench_w8_gemv():
+    """gptq.int8 batch-1 kernel (b2l_w8_gemv) next to the int4 one (b2l_q4_gemv) and the generic kernel (b2l_q_linear at
+    bits 8) on the same shapes, CUDA events around CUDA-graph replays in one process.  Each shape cycles through enough
+    weight copies (>= 200 MB of 8-bit levels) that no call finds its weights in the 50 MB L2.  GB/s counts the weight
+    bytes each kernel reads per call: N K at 8 bits, N K / 2 at 4 bits."""
+    import torch
+    from lit_llama_b200 import _lib as L
+
+    dev = torch.device("cuda")
+    lib = L.lib()
+    print(_card(), flush=True)
+    shapes = [("7B c_attn", 12288, 4096), ("7B attn.c_proj", 4096, 4096), ("7B fc1|fc2", 22016, 4096), ("7B mlp.c_proj", 4096, 11008),
+              ("7B lm_head", 32000, 4096), ("13B c_fc1", 13824, 5120), ("13B mlp.c_proj", 5120, 13824), ("65B c_fc1", 22016, 8192),
+              ("65B mlp.c_proj", 8192, 22016)]
+    for (name, N, K) in shapes:
+        ncopy = max(2, -(-200_000_000 // (N * K)))
+        x = torch.randn(1, K, device=dev).bfloat16()
+        sc = (torch.rand(N, 1, device=dev) * 0.01 + 0.002).bfloat16()
+        z = torch.randint(0, 256, (N, 1), device=dev).bfloat16()
+        y = torch.empty(1, N, device=dev, dtype=torch.bfloat16)
+        w8, q4, ref = [], [], []
+        for i in range(ncopy):
+            qw = torch.randint(0, 256, (K, N), device=dev, dtype=torch.uint8).t()     # reference layout: [K][N]
+            t = torch.empty(lib.b2l_w8_tiled_i8_bytes(N, K), dtype=torch.uint8, device=dev)
+            L.check(lib.b2l_w8_tile_i8(qw.data_ptr(), t.data_ptr(), N, K, L.stream_ptr()), "w8 tile")
+            w8.append(t)
+            t4 = torch.empty(lib.b2l_q4_tiled_i8_bytes(N, K), dtype=torch.uint8, device=dev)
+            L.check(lib.b2l_q4_tile_i8(qw.data_ptr(), t4.data_ptr(), N, K, L.stream_ptr()), "q4 tile")   # any bytes: timing only
+            q4.append(t4)
+            if i < 2:
+                ref.append(qw)
+        a8 = [_w8_args(L, x, t, sc, z, N, K, y) for t in w8]
+        a4 = [_w8_args(L, x, t, sc, z, N, K, y) for t in q4]
+        reps = ncopy * max(1, -(-8_000_000_000 // (ncopy * N * K)))
+        f8 = lambda: [lib.b2l_w8_gemv(C.byref(a8[i % ncopy]), L.stream_ptr()) for i in range(reps)]
+        f4 = lambda: [lib.b2l_q4_gemv(C.byref(a4[i % ncopy]), L.stream_ptr()) for i in range(reps)]
+        fg = lambda: [lib.b2l_q_linear(x.data_ptr(), K, ref[i % 2].data_ptr(), sc.data_ptr(), z.data_ptr(), L.B2L_BF16, None, y.data_ptr(),
+                                       N, 1, N, K, 8, K, L.stream_ptr()) for i in range(8)]
+        r8, r4 = [], []
+        for _ in range(3):
+            r8.append(_time_graph(f8, 1) / reps)
+            r4.append(_time_graph(f4, 1) / reps)
+        rg = _time_graph(fg, 1) / 8
+        u8, u4 = sorted(r8)[1], sorted(r4)[1]
+        print(f"{name} N={N} K={K}: w8_gemv {u8:.1f} us = {N * K / u8 / 1e3:.0f} GB/s | q4_gemv {u4:.1f} us = {N * K / 2 / u4 / 1e3:.0f} GB/s "
+              f"| generic bits=8 {rg:.1f} us = {N * K / rg / 1e3:.0f} GB/s (L2-warm: 2 copies)", flush=True)
+        del w8, q4, ref
+        torch.cuda.empty_cache()
+
+
+def sec_bench_w8_gemm():
+    """gptq.int8 GEMM (b2l_w8_gemm, reference-layout levels) next to the int4 GEMM (b2l_q4_gemm), the generic kernel at
+    bits 8 (small M only) and torch.matmul on a dense bf16 weight, CUDA events around CUDA-graph replays, same run.
+    TFLOP/s counts 2 M N K."""
+    import torch
+    from lit_llama_b200 import _lib as L
+
+    dev = torch.device("cuda")
+    lib = L.lib()
+    print(_card(), flush=True)
+    for (name, N, K) in [("7B c_attn", 12288, 4096), ("7B mlp.c_proj", 4096, 11008), ("13B c_attn", 15360, 5120), ("13B mlp.c_proj", 5120, 13824)]:
+        qw = torch.randint(0, 256, (K, N), device=dev, dtype=torch.uint8).t()
+        sc = (torch.rand(N, 1, device=dev) * 0.01 + 0.002).bfloat16()
+        z = torch.randint(0, 256, (N, 1), device=dev).bfloat16()
+        q4 = torch.empty(lib.b2l_q4_tiled_bytes(N, K), dtype=torch.uint8, device=dev)
+        L.check(lib.b2l_q4_tile(qw.data_ptr(), q4.data_ptr(), N, K, L.stream_ptr()), "q4 tile")   # any bytes: timing only
+        wd = torch.randn(N, K, device=dev).bfloat16()
+        for M in (2, 8, 64, 512, 4096):
+            x = torch.randn(M, K, device=dev).bfloat16()
+            y = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
+            a8, a4 = _w8_args(L, x, qw, sc, z, N, K, y, M=M), _w8_args(L, x, q4, sc, z, N, K, y, M=M)
+            it = 20 if M <= 64 else 4
+            u8 = _time_graph(lambda: L.check(lib.b2l_w8_gemm(C.byref(a8), L.stream_ptr()), "w8 gemm"), it)
+            u4 = _time_graph(lambda: L.check(lib.b2l_q4_gemm(C.byref(a4), L.stream_ptr()), "q4 gemm"), it)
+            ut = _time_graph(lambda: torch.matmul(x, wd.t()), it)
+            gen = ""
+            if M <= 8:
+                ug = _time_graph(lambda: lib.b2l_q_linear(x.data_ptr(), K, qw.data_ptr(), sc.data_ptr(), z.data_ptr(), L.B2L_BF16, None,
+                                                          y.data_ptr(), N, M, N, K, 8, K, L.stream_ptr()), it)
+                gen = f" | generic bits=8 {ug:.1f} us"
+            op = 2.0 * M * N * K
+            print(f"{name} N={N} K={K} M={M}: w8_gemm {u8:.1f} us = {op / u8 / 1e6:.1f} TFLOP/s | q4_gemm {u4:.1f} us = {op / u4 / 1e6:.1f} "
+                  f"TFLOP/s | torch.matmul bf16 {ut:.1f} us = {op / ut / 1e6:.1f} TFLOP/s{gen}", flush=True)
+        del qw, q4, wd
+        torch.cuda.empty_cache()
+
+
+def _random_w8_model(name, dev, seed=0, n_layer=None):
+    """A gptq.int8 LLaMA at `name`'s widths (`n_layer` blocks if given) with random per-row levels, zeros and scales.
+    The scales give every linear a gain of about one (rms (level - zero) is about 76), as in a trained model: with
+    larger gains the attention scores saturate and the softmax turns rounding differences into different outputs."""
+    import torch
+    import lit_llama_b200 as P
+    from lit_llama_b200.quantization import ColBlockQuantizedLinear, weights_changed
+    from lit_llama_b200.utils import quantization
+
+    prev = torch.get_default_dtype()
+    torch.set_default_dtype(torch.bfloat16)
+    try:
+        with torch.device(dev), quantization("gptq.int8"):
+            cfg = P.LLaMAConfig.from_name(name)
+            if n_layer is not None:
+                cfg.n_layer = n_layer
+            model = P.LLaMA(cfg)
+    finally:
+        torch.set_default_dtype(prev)
+    g = torch.Generator(device=dev).manual_seed(seed)
+    with torch.no_grad():
+        for m in model.modules():
+            if isinstance(m, ColBlockQuantizedLinear):
+                m.quant_weight.copy_(torch.randint(0, 256, m.quant_weight.shape, generator=g, device=dev, dtype=torch.uint8))
+                m.scales.copy_((torch.rand(m.scales.shape, generator=g, device=dev) + 0.5) / (76 * m.in_features ** 0.5))
+                m.zeros.copy_(torch.randint(96, 160, m.zeros.shape, generator=g, device=dev))
+            elif isinstance(m, P.RMSNorm):
+                m.scale.fill_(1)
+        model.transformer.wte.weight.normal_(0, 1, generator=g)
+    weights_changed()
+    return model.eval()
+
+
+def _generic_forward(self, inp):
+    """ColBlockQuantizedLinear.forward of the parent commit for gptq.int8: every call on the generic kernel."""
+    import torch
+    from lit_llama_b200 import _lib as L
+
+    x = inp.reshape(-1, inp.shape[-1]).contiguous()
+    y = torch.empty((x.shape[0], self.out_features), device=inp.device, dtype=inp.dtype)
+    qw = self.reference_quant_weight()
+    L.check(L.lib().b2l_q_linear(x.data_ptr(), x.stride(0), qw.data_ptr(), self.scales.data_ptr(), self.zeros.data_ptr(),
+                                 L.sz_dtype_of(self.scales), None, y.data_ptr(), self.out_features, x.shape[0], self.out_features,
+                                 self.in_features, self.bits, self.tile_cols, L.stream_ptr()), "b2l_q_linear")
+    return y.reshape(*inp.shape[:-1], self.out_features)
+
+
+def _w8_exact_anchor(dev, n_layer=4, T=16, steps=4, S=64):
+    """Which path is nearer the exact result: the first `n_layer` blocks of a random 7B gptq.int8 model, a T-token
+    prompt and `steps` decode steps, on the fused step and on the parent's path (generic kernel), both against the
+    oracle with exact linears (fp64 dequantisation and accumulation, one rounding to bf16; every other op with the
+    reference's bf16 rounding points).  Prints the largest normwise logit distance over the steps."""
+    import torch
+    from lit_llama_b200.quantization import ColBlockQuantizedLinear
+    from oracle import llama_oracle as O
+
+    model = _random_w8_model("7B", dev, seed=9, n_layer=n_layer)
+    cfg = model.config
+    sd = {k: v.detach().cpu() for k, v in model.state_dict().items()}
+    oracle = O.OracleLLaMA.from_state_dict(sd, n_layer, cfg.n_head, cfg.block_size, "gptq.int8", exact_linears=True)
+    g = torch.Generator().manual_seed(3)
+    prompt = torch.randint(0, 32000, (1, T), generator=g)
+    toks = torch.randint(0, 32000, (steps,), generator=g).tolist()
+
+    def run(fwd):
+        fwd.reset_cache()
+        dv = "cpu" if fwd is oracle else dev
+        out = [fwd.forward(prompt.to(dv), S, torch.arange(T, device=dv))[:, -1]]
+        for i, t in enumerate(toks):
+            out.append(fwd.forward(torch.tensor([[t]], device=dv), S, torch.tensor([T + i], device=dv)).reshape(1, -1))
+        return [o.float().cpu() for o in out]
+
+    new_forward = ColBlockQuantizedLinear.forward
+    with torch.no_grad():
+        want = run(oracle)
+        fused = run(model)
+        assert model._decode is not None
+        try:
+            ColBlockQuantizedLinear.forward = _generic_forward
+            model._fast_ok = False
+            generic = run(model)
+        finally:
+            ColBlockQuantizedLinear.forward = new_forward
+            model._fast_ok = None
+    d = lambda a, b: max(float((x - y).norm() / y.norm()) for x, y in zip(a, b))
+    print(f"  7B widths, {n_layer} blocks, {T}-token prompt + {steps} decode steps, logits against the oracle with exact linears: "
+          f"fused step {d(fused, want):.2e} | parent path (generic kernel) {d(generic, want):.2e} | between the two "
+          f"{d(fused, generic):.2e}", flush=True)
+    del model
+    gc.collect()
+    torch.cuda.empty_cache()
+
+
+def sec_bench_step_w8():
+    """--quantize gptq.int8 at 7B, 13B, 30B and 65B (random levels, compacted: one resident copy): a 512-token prompt (the
+    wgmma GEMM) and batch-1 decode at ctx ~2000 (the fused step, CUDA graph).  B2L_W8_SIZES picks the sizes.  For 7B
+    the fused step is alternated with the parent's path (module by module on the generic kernel) before compaction, and
+    both are compared with an exact evaluation of the first blocks (_w8_exact_anchor)."""
+    import torch
+    import lit_llama_b200 as P
+    from lit_llama_b200.quantization import ColBlockQuantizedLinear
+
+    dev = torch.device("cuda")
+    print(_card(), flush=True)
+    S = 2048
+    for name in os.environ.get("B2L_W8_SIZES", "7B,13B,30B,65B").split(","):
+        model = _random_w8_model(name, dev, seed=8)
+        model.copy_logits = False
+        if name == "7B":
+            new_forward = ColBlockQuantizedLinear.forward
+            us = {"fused": [], "generic": []}
+            logits = {}
+            try:
+                for _ in range(2):
+                    for kind in ("fused", "generic"):
+                        ColBlockQuantizedLinear.forward = new_forward if kind == "fused" else _generic_forward
+                        model.reset_cache()
+                        model._fast_ok = None if kind == "fused" else False
+                        model._module_graph = None
+                        torch.manual_seed(0)   # the same tokens at the same positions: the KV caches agree
+                        us[kind].append(_decode_us(model, 1, S, dev, p0=2000, n=24))
+                        with torch.no_grad():
+                            logits[kind] = model(torch.tensor([[1234]], device=dev, dtype=torch.int32), S,
+                                                 torch.tensor([2040], device=dev)).float().clone()
+            finally:
+                ColBlockQuantizedLinear.forward = new_forward
+                model._fast_ok = None
+            a, b = logits["fused"], logits["generic"]
+            print(f"  7B decode B=1, alternated: fused step {' '.join(f'{v:.1f}' for v in us['fused'])} us/token | parent path (generic "
+                  f"kernel) {' '.join(f'{v:.1f}' for v in us['generic'])} us/token | logits rel. diff {float((a - b).norm() / b.norm()):.2e}",
+                  flush=True)
+            model.reset_cache()
+            _w8_exact_anchor(dev)
+        model.compact()
+        torch.cuda.reset_peak_memory_stats()
+        levels = sum(m.out_features * m.in_features for m in model.modules() if isinstance(m, ColBlockQuantizedLinear))
+        idx = torch.randint(0, 32000, (1, 512), device=dev, dtype=torch.int32)
+        with torch.no_grad():
+            prompt_us = _time(lambda: model(idx, S, torch.arange(512, device=dev)), iters=3, warm=1)
+            model.reset_cache()
+            us = _decode_us(model, 1, S, dev, p0=2000, n=24)
+        print(f"{name} gptq.int8: prompt 512 tokens {prompt_us / 1e3:.2f} ms | decode B=1 ctx~2000-2030 fused="
+              f"{model._decode is not None and model._decode.graph is not None}: {us:.1f} us/token {1e6 / us:.1f} tok/s "
+              f"({levels / us / 1e3:.0f} GB/s of levels) | {torch.cuda.max_memory_allocated() / 2**30:.1f} GiB peak", flush=True)
+        del model
+        gc.collect()   # a compacted model's c_fc1 / c_fc2 refer back to it (their layout source): a cycle
+        torch.cuda.empty_cache()
 
 
 def sec_bench_q8_gemm():
