@@ -317,6 +317,35 @@ int b2l_ring_advance(const int64_t* input_pos, int T, int32_t* ring_start, int S
 int b2l_attention_nocache(void* qkv, const void* rope, void* y, void* work, int B, int T,
                           int n_head, int head_size, int block_size, b2l_stream_t stream);
 
+/* ------------------------------------------------------------------------------
+ * LLaMA-Adapter (lit_llama/adapter.py:88-174): the attention above plus the gated
+ * attention over a learned prefix, adapter.py:151-167:
+ *   y = bf16(bf16(y) + bf16(gate[h] * bf16(softmax(q ak^T / sqrt(hs)) av)))
+ * with q the rotated query, no mask and no RoPE on the prefix, and a softmax of its
+ * own (not joint with the cache keys).  The prefix keys / values are the k and v
+ * thirds of c_attn(adapter_wte.weight), computed once by the caller.
+ *   k, v  bf16 [n_head][len][head_size], 16-byte aligned (shared by every sequence of the batch)
+ *   gate  bf16 [n_head] (gating_factor)
+ *   len   1..64 (adapter_prompt_length)
+ * Bad arguments are rejected before any launch.  T == 1 at head_size 128 runs the
+ * fused decode kernel's adapter variant (the same single launch); every other shape
+ * adds one small kernel behind the attention.
+ * ---------------------------------------------------------------------------- */
+typedef struct b2l_adapter_prefix {
+  const void* k;
+  const void* v;
+  const void* gate;
+  int len;
+} b2l_adapter_prefix;
+#define B2L_ADAPTER_MAX_LEN 64
+int b2l_attention_adapter(void* qkv, void* k_cache, void* v_cache, const void* rope,
+                          const int64_t* input_pos, const int32_t* ring_start, void* y, void* work,
+                          int B, int T, int n_head, int head_size, int S, int block_size, int flags,
+                          const b2l_adapter_prefix* prefix, b2l_stream_t stream);
+int b2l_attention_nocache_adapter(void* qkv, const void* rope, void* y, void* work, int B, int T,
+                                  int n_head, int head_size, int block_size,
+                                  const b2l_adapter_prefix* prefix, b2l_stream_t stream);
+
 /* kv_caches as the reference would hold them (logical order): un-rotates the ring
  * into `out` [B, nh, S, hs]. */
 int b2l_kv_unroll(const void* cache, const int32_t* ring_start, void* out, int B, int n_head,
@@ -380,6 +409,9 @@ typedef struct b2l_decode_args {
                                 b2l_decode_plan_build -> the whole step runs as ONE persistent kernel
                                 (csrc/decode_mega.cu; weights need the b2l_q4_tile_i8 layout in qw_mma).
                                 NULL: one kernel per op                                   */
+  const b2l_adapter_prefix* adapters; /* HOST array [n_layer] of LLaMA-Adapter prefixes (b2l_attention_adapter);
+                                NULL = no adapter anywhere, an entry with len == 0 = none in that layer.
+                                Not with `plan`.                                          */
 } b2l_decode_args;
 
 int b2l_decode_step(const b2l_decode_args* args, b2l_stream_t stream);

@@ -45,6 +45,14 @@ class Layer(C.Structure):
     ]
 
 
+class AdapterPrefix(C.Structure):
+    """b2l_adapter_prefix: one layer's LLaMA-Adapter prefix keys / values ([n_head][len][hs] bf16) and gate ([n_head])."""
+    _fields_ = [("k", c_void_p), ("v", c_void_p), ("gate", c_void_p), ("len", c_int)]
+
+
+ADAPTER_MAX_LEN = 64   # B2L_ADAPTER_MAX_LEN
+
+
 class DecodeArgs(C.Structure):
     _fields_ = [
         ("n_layer", c_int), ("n_head", c_int), ("n_embd", c_int), ("n_hidden", c_int), ("vocab", c_int),
@@ -55,7 +63,7 @@ class DecodeArgs(C.Structure):
         ("input_pos", c_void_p), ("ring_start", c_void_p), ("block_size", c_int),
         ("x", c_void_p), ("qkv", c_void_p), ("att", c_void_p), ("hid", c_void_p), ("attn_work", c_void_p),
         ("logits", c_void_p), ("flags", c_int), ("timeline", c_void_p), ("batch_work", c_void_p),
-        ("plan", c_void_p),
+        ("plan", c_void_p), ("adapters", C.POINTER(AdapterPrefix)),
     ]
 
 
@@ -106,6 +114,10 @@ _SIGS = {
     "b2l_attn_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
     "b2l_attention": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
                               c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "b2l_attention_adapter": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
+                                      c_int, c_int, c_int, c_int, c_int, c_int, C.POINTER(AdapterPrefix), c_void_p]),
+    "b2l_attention_nocache_adapter": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                              C.POINTER(AdapterPrefix), c_void_p]),
     "b2l_tp_buffer_bytes": (c_size_t, [c_int, c_int]),
     "b2l_tp_allreduce": (c_int, [C.POINTER(TPComm), c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "b2l_ring_advance": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p]),

@@ -11,6 +11,7 @@ namespace b2l {
 
 extern void* g_attn_timeline;
 int decode_step_persistent(const b2l_decode_args* d, b2l_stream_t stream);   // decode_mega.cu
+int check_adapter_prefix(const b2l_adapter_prefix* pre, const char* who);     // attention.cu
 
 static thread_local char g_err[512] = "";
 
@@ -162,9 +163,15 @@ static int q4_call(const b2l_q4_weight& w, const void* x, int ldx, void* y, int 
 extern "C" int b2l_decode_step_launches(const b2l_decode_args* d) {
   if (!d) return 0;
   if (d->plan != nullptr) return 1;   // the persistent kernel
-  const int attn = (d->n_embd / d->n_head == 128) ? 1 : 3;  // fused single-token attention for head_size 128
+  // fused single-token attention for head_size 128 (B2L_F_ATTN_UNFUSED: the three-kernel path)
+  const bool fused = d->n_embd / d->n_head == 128 && !(d->flags & B2L_F_ATTN_UNFUSED);
+  const int attn = fused ? 1 : 3;
   const int lin = (d->B > 1 && d->B <= 8 && d->batch_work) ? 2 : 1;  // the batch kernel is two launches per linear
-  return 2 + d->n_layer * (4 * lin + attn) + lin;  // ring advance + embedding, per Block 4 linears + attention, ln_f+lm_head
+  int n = 2 + d->n_layer * (4 * lin + attn) + lin;  // ring advance + embedding, per Block 4 linears + attention, ln_f+lm_head
+  // an adapter layer adds the prefix kernel behind the three-kernel attention (the fused kernel does it in-launch)
+  if (!fused && d->adapters != nullptr)
+    for (int l = 0; l < d->n_layer; ++l) n += d->adapters[l].len != 0;
+  return n;
 }
 
 extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
@@ -178,6 +185,13 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
   if (d->flags & B2L_F_W8) {
     B2L_CHECK_SUPPORTED(d->B == 1, "b2l_decode_step: B2L_F_W8 (gptq.int8) runs batch 1 only, got B=%d", d->B);
     B2L_CHECK_SUPPORTED(d->plan == nullptr, "b2l_decode_step: B2L_F_W8 (gptq.int8) does not run in the persistent kernel (plan must be NULL)");
+  }
+  if (d->adapters != nullptr) {
+    for (int l = 0; l < d->n_layer; ++l) {
+      if (d->adapters[l].len == 0) continue;   // no adapter in this layer
+      B2L_CHECK_SUPPORTED(d->plan == nullptr, "b2l_decode_step: adapters do not run in the persistent kernel (plan must be NULL)");
+      if (int rc = check_adapter_prefix(&d->adapters[l], "b2l_decode_step")) return rc;
+    }
   }
   if (d->plan != nullptr) return decode_step_persistent(d, stream);   // one persistent kernel per token (decode_mega.cu)
   const int C = d->n_embd, hs = C / d->n_head, B = d->B;
@@ -205,8 +219,12 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
                       nullptr, 0, fl, stream, tl(), d->batch_work, pf(), (kv_ok && kv_prefetch == 2) ? d : nullptr, l)))
       return rc;
     g_attn_timeline = tl();
-    if ((rc = b2l_attention(d->qkv, L.k_cache, L.v_cache, d->rope, d->input_pos, d->ring_start, d->att, d->attn_work, B,
-                            1, d->n_head, hs, d->S, d->block_size, afl, stream))) {
+    const b2l_adapter_prefix* pre = (d->adapters != nullptr && d->adapters[l].len != 0) ? &d->adapters[l] : nullptr;
+    if ((rc = pre != nullptr
+                  ? b2l_attention_adapter(d->qkv, L.k_cache, L.v_cache, d->rope, d->input_pos, d->ring_start, d->att,
+                                          d->attn_work, B, 1, d->n_head, hs, d->S, d->block_size, afl, pre, stream)
+                  : b2l_attention(d->qkv, L.k_cache, L.v_cache, d->rope, d->input_pos, d->ring_start, d->att,
+                                  d->attn_work, B, 1, d->n_head, hs, d->S, d->block_size, afl, stream))) {
       g_attn_timeline = nullptr;
       return rc;
     }

@@ -238,13 +238,64 @@ __device__ __forceinline__ void fd_bulk(uint32_t dst, const void* src, uint32_t 
 constexpr int FD_SUB_BYTES = FD_SUB * 128 * 2;
 constexpr int FD_SMEM_BYTES = 4 * FD_SUB_BYTES + FD_WARPS * 128 * 4 + 2 * FD_WARPS * 4 + 16;
 
-__global__ void __launch_bounds__(FD_WARPS * 32)
+// LLaMA-Adapter prefix term for one head of one query (adapter.py:164-167), called by every thread of a working CTA
+// of the fused decode kernel.  sq: the rotated, 1/sqrt(hs)-scaled query [HS] (fp32, shared memory); ssc: score scratch
+// [B2L_ADAPTER_MAX_LEN].  Warp w scores prefix keys w, w + 8, ... (4 dims per lane); thread d < HS then returns
+// softmax(scores) . av[:, d] in fp32.
+__device__ __forceinline__ float fd_adapter_prefix(const float* sq, float* ssc, const __nv_bfloat16* __restrict__ ak,
+                                                   const __nv_bfloat16* __restrict__ av, int alen, int warp, int lane,
+                                                   int d, bool writer) {
+  constexpr int HS = 128;
+  const float4 qv = reinterpret_cast<const float4*>(sq)[lane];
+#pragma unroll 2
+  for (int j = warp; j < alen; j += FD_WARPS) {
+    const uint2 ku = __ldg(reinterpret_cast<const uint2*>(ak + (size_t)j * HS) + lane);
+    float s = qv.x * __uint_as_float(ku.x << 16);
+    s = fmaf(qv.y, __uint_as_float(ku.x & 0xffff0000u), s);
+    s = fmaf(qv.z, __uint_as_float(ku.y << 16), s);
+    s = fmaf(qv.w, __uint_as_float(ku.y & 0xffff0000u), s);
+    s = warp_sum(s);
+    if (lane == 0) ssc[j] = s;
+  }
+  __syncthreads();
+  float ay = 0.f;
+  if (writer) {
+    float mx = -INFINITY;
+    for (int j = 0; j < alen; ++j) mx = fmaxf(mx, ssc[j]);
+    float l = 0.f;
+    // 8 value loads in flight per round: this runs in the tail of the launch, where every L2 round trip is exposed
+#pragma unroll 8
+    for (int j = 0; j < alen; ++j) {
+      const float p = __expf(ssc[j] - mx);
+      l += p;
+      ay = fmaf(p, bf2f(av[(size_t)j * HS + d]), ay);
+    }
+    ay /= l;
+  }
+  return ay;
+}
+
+// adapter.py:167 under bf16: y, the prefix attention and the gated term are each rounded, then their sum
+__device__ __forceinline__ __nv_bfloat16 adapter_combine(float y, float ay, float gate) {
+  return f2bf(rbf(y) + rbf(gate * rbf(ay)));
+}
+
+// ADAPTER: the LLaMA-Adapter variant.  Every working CTA asks the L2 for its head's prefix rows before
+// griddepcontrol.wait (they do not depend on the current token) and computes the prefix attention as soon as its q
+// is ready, while its first KV sub-tiles are still landing (q waits in the otherwise unused merge scratch).  The CTA
+// that writes the head's output (the only one, or the last to arrive) adds the gated term before its store; the
+// others drop it, so the term's two dependent L2 round trips overlap the KV stream instead of sitting in the tail of
+// the writing CTA (DESIGN.md, LLaMA-Adapter, has the measurements of both placements).
+template <bool ADAPTER>
+__global__ void __launch_bounds__(FD_WARPS * 32, ADAPTER ? FD_CTAS_PER_SM : 0)
     attn_decode_fused_kernel(const __nv_bfloat16* qkv, __nv_bfloat16* __restrict__ k_cache,
                              __nv_bfloat16* __restrict__ v_cache, const float* __restrict__ rope,
                              const int64_t* __restrict__ input_pos, const int32_t* __restrict__ ring_start,
                              __nv_bfloat16* __restrict__ y, float* __restrict__ work, int* __restrict__ tickets,
                              int n_head, int S, int block_size, int n_split, unsigned long long* tl, int pre_tiles,
-                             int smem_merge, int target_ctas) {
+                             int smem_merge, int target_ctas, const __nv_bfloat16* __restrict__ pre_k,
+                             const __nv_bfloat16* __restrict__ pre_v, const __nv_bfloat16* __restrict__ pre_gate,
+                             int pre_len) {
   constexpr int HS = 128;
   extern __shared__ __align__(128) uint8_t fsm[];
   float* sm_acc = reinterpret_cast<float*>(fsm + 4 * FD_SUB_BYTES);                // [FD_WARPS][HS]
@@ -310,6 +361,14 @@ __global__ void __launch_bounds__(FD_WARPS * 32)
     if (n_sub > 0) request(0);
     if (pre > 1 && n_sub > 1) request(1);
   }
+  if constexpr (ADAPTER) {
+    if (threadIdx.x == 0) {   // the head's prefix rows
+      const size_t off = (size_t)h * pre_len * HS;
+      const uint32_t bytes = (uint32_t)pre_len * HS * 2;
+      asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(pre_k + off), "r"(bytes) : "memory");
+      asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(pre_v + off), "r"(bytes) : "memory");
+    }
+  }
   // the RoPE row of this position is a constant table entry: fetch it before the dependency too
   const long long prow = p < block_size ? p : (long long)block_size - 1;
   const int grp = lane >> 3, sub = lane & 7, d0 = sub * 16;
@@ -349,6 +408,17 @@ __global__ void __launch_bounds__(FD_WARPS * 32)
       q[2 * i] = e * scale;
       q[2 * i + 1] = o * scale;
     }
+  }
+  float ay = 0.f;   // ADAPTER: the prefix attention of dim threadIdx.x (threads < HS), fp32
+  if constexpr (ADAPTER) {
+    if (warp == 0 && grp == 0) {   // lanes 0..7 hold the whole head
+      float4* dq = reinterpret_cast<float4*>(sm_acc + d0);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) dq[i] = make_float4(q[4 * i], q[4 * i + 1], q[4 * i + 2], q[4 * i + 3]);
+    }
+    __syncthreads();
+    ay = fd_adapter_prefix(sm_acc, sm_acc + HS, pre_k + (size_t)h * pre_len * HS, pre_v + (size_t)h * pre_len * HS,
+                           pre_len, warp, lane, threadIdx.x & (HS - 1), threadIdx.x < HS);
   }
 
   float m = -INFINITY, l = 0.f, acc[16];
@@ -506,7 +576,11 @@ __global__ void __launch_bounds__(FD_WARPS * 32)
   }
   stamp();
   if (n_active == 1) {  // nothing to merge
-    if (writer) y[(size_t)b * C + h * HS + d] = f2bf(a / Ls);
+    if constexpr (ADAPTER) {
+      if (writer) y[(size_t)b * C + h * HS + d] = adapter_combine(a / Ls, ay, bf2f(pre_gate[h]));
+    } else {
+      if (writer) y[(size_t)b * C + h * HS + d] = f2bf(a / Ls);
+    }
     if (threadIdx.x == 0) tl_max(tl, 4);
     stamp();
     return;
@@ -551,8 +625,53 @@ __global__ void __launch_bounds__(FD_WARPS * 32)
     }
     MM = bm;
   }
-  if (writer) y[(size_t)b * C + h * HS + d] = f2bf(aa / LL);
+  if constexpr (ADAPTER) {
+    if (writer) y[(size_t)b * C + h * HS + d] = adapter_combine(aa / LL, ay, bf2f(pre_gate[h]));
+  } else {
+    if (writer) y[(size_t)b * C + h * HS + d] = f2bf(aa / LL);
+  }
   if (threadIdx.x == 0) tl_max(tl, 4);
+}
+
+// ----------------------------------------------------------------------------------
+// LLaMA-Adapter prefix term for every attention shape the fused kernel above does not cover (T > 1, no cache, other
+// head sizes, B2L_F_ATTN_UNFUSED): grid (B*T, n_head), 4 warps.  Reads the rotated q that rope_append_kernel left in
+// qkv and adds the gated prefix attention into y in place (adapter.py:164-167, same rounding chain as the fused kernel).
+// ----------------------------------------------------------------------------------
+__global__ void __launch_bounds__(ATT_WARPS * 32)
+    attn_adapter_prefix_kernel(const __nv_bfloat16* __restrict__ qkv, const __nv_bfloat16* __restrict__ pk,
+                               const __nv_bfloat16* __restrict__ pv, const __nv_bfloat16* __restrict__ gate,
+                               __nv_bfloat16* __restrict__ y, int n_head, int hs, int alen) {
+  pdl_launch_dependents();
+  __shared__ float sq[32 * ATT_MAX_EPL];
+  __shared__ float ssc[B2L_ADAPTER_MAX_LEN];
+  const int bt = blockIdx.x, h = blockIdx.y;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int C = n_head * hs;
+  const float scale = rsqrtf((float)hs);
+  const __nv_bfloat16* q = qkv + (size_t)bt * 3 * C + h * hs;
+  for (int d = threadIdx.x; d < hs; d += blockDim.x) sq[d] = bf2f(q[d]) * scale;
+  __syncthreads();
+  const __nv_bfloat16* kb = pk + (size_t)h * alen * hs;
+  const __nv_bfloat16* vb = pv + (size_t)h * alen * hs;
+  for (int j = warp; j < alen; j += ATT_WARPS) {
+    float s = 0.f;
+    for (int d = lane; d < hs; d += 32) s = fmaf(sq[d], bf2f(kb[(size_t)j * hs + d]), s);
+    s = warp_sum(s);
+    if (lane == 0) ssc[j] = s;
+  }
+  __syncthreads();
+  float mx = -INFINITY;
+  for (int j = 0; j < alen; ++j) mx = fmaxf(mx, ssc[j]);
+  float l = 0.f;
+  for (int j = 0; j < alen; ++j) l += __expf(ssc[j] - mx);
+  const float g = bf2f(gate[h]);
+  __nv_bfloat16* yr = y + (size_t)bt * C + h * hs;
+  for (int d = threadIdx.x; d < hs; d += blockDim.x) {
+    float a = 0.f;
+    for (int j = 0; j < alen; ++j) a = fmaf(__expf(ssc[j] - mx), bf2f(vb[(size_t)j * hs + d]), a);
+    yr[d] = adapter_combine(bf2f(yr[d]), a / l, g);
+  }
 }
 
 // ----------------------------------------------------------------------------------
@@ -786,6 +905,17 @@ static int launch_attn(const __nv_bfloat16* qkv, KvView kv, const int64_t* input
   return 0;
 }
 
+// a LLaMA-Adapter prefix (b2l_adapter_prefix) before any launch: 0, or B2L_E_* with the message naming `who`
+int check_adapter_prefix(const b2l_adapter_prefix* pre, const char* who) {
+  B2L_CHECK_ARG(pre != nullptr && pre->k != nullptr && pre->v != nullptr && pre->gate != nullptr,
+                "%s: null adapter prefix pointer", who);
+  B2L_CHECK_SUPPORTED(pre->len > 0 && pre->len <= B2L_ADAPTER_MAX_LEN, "%s: adapter prefix length %d unsupported (1..%d)",
+                      who, pre->len, B2L_ADAPTER_MAX_LEN);
+  B2L_CHECK_ARG(((uintptr_t)pre->k & 15) == 0 && ((uintptr_t)pre->v & 15) == 0 && ((uintptr_t)pre->gate & 1) == 0,
+                "%s: adapter prefix k / v must be 16-byte aligned, gate 2-byte aligned", who);
+  return 0;
+}
+
 }  // namespace b2l
 
 using namespace b2l;
@@ -811,30 +941,45 @@ extern "C" int b2l_ring_advance(const int64_t* input_pos, int T, int32_t* ring_s
   return 0;
 }
 
-extern "C" int b2l_attention(void* qkv, void* k_cache, void* v_cache, const void* rope, const int64_t* input_pos,
-                             const int32_t* ring_start, void* y, void* work, int B, int T, int n_head,
-                             int head_size, int S, int block_size, int flags, b2l_stream_t stream) {
-  B2L_CHECK_ARG(qkv && k_cache && v_cache && rope && input_pos && ring_start && y && work,
-                "b2l_attention: null pointer");
-  B2L_CHECK_ARG(B > 0 && T > 0 && n_head > 0 && S > 0 && T <= S && block_size > 0, "b2l_attention: bad shape");
-  B2L_CHECK_SUPPORTED(head_size % 2 == 0 && head_size >= 2 && head_size <= 32 * ATT_MAX_EPL,
-                      "b2l_attention: head_size %d unsupported (even, <= %d)", head_size, 32 * ATT_MAX_EPL);
-  cudaStream_t st = (cudaStream_t)stream;
+static int launch_adapter_prefix(const void* qkv, const b2l_adapter_prefix* pre, void* y, int B, int T, int n_head,
+                                 int head_size, cudaStream_t st) {
+  attn_adapter_prefix_kernel<<<dim3(B * T, n_head), ATT_WARPS * 32, 0, st>>>(
+      (const __nv_bfloat16*)qkv, (const __nv_bfloat16*)pre->k, (const __nv_bfloat16*)pre->v,
+      (const __nv_bfloat16*)pre->gate, (__nv_bfloat16*)y, n_head, head_size, pre->len);
+  B2L_LAUNCH_CHECK("attn_adapter_prefix_kernel");
+  return 0;
+}
+
+// b2l_attention and b2l_attention_adapter (pre != nullptr: already checked)
+static int attention_impl(void* qkv, void* k_cache, void* v_cache, const void* rope, const int64_t* input_pos,
+                          const int32_t* ring_start, void* y, void* work, int B, int T, int n_head, int head_size,
+                          int S, int block_size, int flags, const b2l_adapter_prefix* pre, cudaStream_t st) {
   if (T == 1 && head_size == 128 && !(flags & B2L_F_ROPE_ROWS) && !(flags & B2L_F_ATTN_UNFUSED)) {
     const int n_split = (S + FD_SUB - 1) / FD_SUB;
     int* tickets = reinterpret_cast<int*>(reinterpret_cast<char*>(work) + ws_partials_bytes(B, n_head, head_size, T, S));
-    static DynSmemCache smem_cache;
     // B2L_ATTN_PRE (read once): sub-tiles requested before griddepcontrol.wait, 1 (default) or 2
     static const int env_pre = [] { const char* e = getenv("B2L_ATTN_PRE"); return e ? atoi(e) : 1; }();
     // B2L_ATTN_SMEM_MERGE (read once): 1 = all 32 key groups merge through shared memory, 0 = shuffles inside a warp first
     // (default 0: the extra block barrier of 1 is not free)
     static const int env_smem_merge = [] { const char* e = getenv("B2L_ATTN_SMEM_MERGE"); return e ? atoi(e) : 0; }();
-    if (int rc = ensure_dyn_smem(attn_decode_fused_kernel, FD_SMEM_BYTES, smem_cache)) return rc;
     LaunchCfg lc(dim3(B * n_head, n_split), dim3(FD_WARPS * 32), FD_SMEM_BYTES, st, (flags & B2L_F_PDL) != 0);
-    B2L_CUDA(cudaLaunchKernelEx(&lc.cfg, attn_decode_fused_kernel, (const __nv_bfloat16*)qkv, (__nv_bfloat16*)k_cache,
-                                (__nv_bfloat16*)v_cache, (const float*)rope, input_pos, ring_start, (__nv_bfloat16*)y,
-                                (float*)work, tickets, n_head, S, block_size, n_split, (unsigned long long*)g_attn_timeline, env_pre, env_smem_merge,
-                                FD_CTAS_PER_SM * sm_count()));
+    if (pre == nullptr) {
+      static DynSmemCache smem_cache;
+      if (int rc = ensure_dyn_smem(attn_decode_fused_kernel<false>, FD_SMEM_BYTES, smem_cache)) return rc;
+      B2L_CUDA(cudaLaunchKernelEx(&lc.cfg, attn_decode_fused_kernel<false>, (const __nv_bfloat16*)qkv, (__nv_bfloat16*)k_cache,
+                                  (__nv_bfloat16*)v_cache, (const float*)rope, input_pos, ring_start, (__nv_bfloat16*)y,
+                                  (float*)work, tickets, n_head, S, block_size, n_split, (unsigned long long*)g_attn_timeline, env_pre, env_smem_merge,
+                                  FD_CTAS_PER_SM * sm_count(), (const __nv_bfloat16*)nullptr, (const __nv_bfloat16*)nullptr,
+                                  (const __nv_bfloat16*)nullptr, 0));
+    } else {
+      static DynSmemCache smem_cache;
+      if (int rc = ensure_dyn_smem(attn_decode_fused_kernel<true>, FD_SMEM_BYTES, smem_cache)) return rc;
+      B2L_CUDA(cudaLaunchKernelEx(&lc.cfg, attn_decode_fused_kernel<true>, (const __nv_bfloat16*)qkv, (__nv_bfloat16*)k_cache,
+                                  (__nv_bfloat16*)v_cache, (const float*)rope, input_pos, ring_start, (__nv_bfloat16*)y,
+                                  (float*)work, tickets, n_head, S, block_size, n_split, (unsigned long long*)g_attn_timeline, env_pre, env_smem_merge,
+                                  FD_CTAS_PER_SM * sm_count(), (const __nv_bfloat16*)pre->k, (const __nv_bfloat16*)pre->v,
+                                  (const __nv_bfloat16*)pre->gate, pre->len));
+    }
     return 0;
   }
   int rt = head_size / 2 < 32 ? 32 : head_size / 2;
@@ -844,17 +989,40 @@ extern "C" int b2l_attention(void* qkv, void* k_cache, void* v_cache, const void
   B2L_LAUNCH_CHECK("rope_append_kernel");
   KvView kv{(const __nv_bfloat16*)k_cache, (const __nv_bfloat16*)v_cache, (size_t)n_head * S * head_size,
             (size_t)S * head_size, (size_t)head_size, S};
-  return launch_attn((const __nv_bfloat16*)qkv, kv, input_pos, ring_start, (float*)work, (__nv_bfloat16*)y, B, T,
-                     n_head, head_size, S, st);
+  if (int rc = launch_attn((const __nv_bfloat16*)qkv, kv, input_pos, ring_start, (float*)work, (__nv_bfloat16*)y, B, T,
+                           n_head, head_size, S, st))
+    return rc;
+  return pre == nullptr ? 0 : launch_adapter_prefix(qkv, pre, y, B, T, n_head, head_size, st);
 }
 
-extern "C" int b2l_attention_nocache(void* qkv, const void* rope, void* y, void* work, int B, int T, int n_head,
-                                     int head_size, int block_size, b2l_stream_t stream) {
-  B2L_CHECK_ARG(qkv && rope && y && work && B > 0 && T > 0 && n_head > 0 && T <= block_size,
-                "b2l_attention_nocache: bad argument");
+extern "C" int b2l_attention(void* qkv, void* k_cache, void* v_cache, const void* rope, const int64_t* input_pos,
+                             const int32_t* ring_start, void* y, void* work, int B, int T, int n_head,
+                             int head_size, int S, int block_size, int flags, b2l_stream_t stream) {
+  B2L_CHECK_ARG(qkv && k_cache && v_cache && rope && input_pos && ring_start && y && work,
+                "b2l_attention: null pointer");
+  B2L_CHECK_ARG(B > 0 && T > 0 && n_head > 0 && S > 0 && T <= S && block_size > 0, "b2l_attention: bad shape");
   B2L_CHECK_SUPPORTED(head_size % 2 == 0 && head_size >= 2 && head_size <= 32 * ATT_MAX_EPL,
-                      "b2l_attention_nocache: head_size %d unsupported", head_size);
-  cudaStream_t st = (cudaStream_t)stream;
+                      "b2l_attention: head_size %d unsupported (even, <= %d)", head_size, 32 * ATT_MAX_EPL);
+  return attention_impl(qkv, k_cache, v_cache, rope, input_pos, ring_start, y, work, B, T, n_head, head_size, S,
+                        block_size, flags, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int b2l_attention_adapter(void* qkv, void* k_cache, void* v_cache, const void* rope,
+                                     const int64_t* input_pos, const int32_t* ring_start, void* y, void* work, int B,
+                                     int T, int n_head, int head_size, int S, int block_size, int flags,
+                                     const b2l_adapter_prefix* prefix, b2l_stream_t stream) {
+  B2L_CHECK_ARG(qkv && k_cache && v_cache && rope && input_pos && ring_start && y && work,
+                "b2l_attention_adapter: null pointer");
+  B2L_CHECK_ARG(B > 0 && T > 0 && n_head > 0 && S > 0 && T <= S && block_size > 0, "b2l_attention_adapter: bad shape");
+  B2L_CHECK_SUPPORTED(head_size % 2 == 0 && head_size >= 2 && head_size <= 32 * ATT_MAX_EPL,
+                      "b2l_attention_adapter: head_size %d unsupported (even, <= %d)", head_size, 32 * ATT_MAX_EPL);
+  if (int rc = check_adapter_prefix(prefix, "b2l_attention_adapter")) return rc;
+  return attention_impl(qkv, k_cache, v_cache, rope, input_pos, ring_start, y, work, B, T, n_head, head_size, S,
+                        block_size, flags, prefix, (cudaStream_t)stream);
+}
+
+static int attention_nocache_impl(void* qkv, const void* rope, void* y, void* work, int B, int T, int n_head,
+                                  int head_size, int block_size, cudaStream_t st) {
   int rt = head_size / 2 < 32 ? 32 : head_size / 2;
   rope_append_kernel<<<dim3(B * T, n_head), rt, 0, st>>>((__nv_bfloat16*)qkv, nullptr, nullptr, (const float*)rope,
                                                         nullptr, nullptr, T, n_head, head_size, 0, block_size, 0);
@@ -863,6 +1031,28 @@ extern "C" int b2l_attention_nocache(void* qkv, const void* rope, void* y, void*
   const __nv_bfloat16* base = (const __nv_bfloat16*)qkv;
   KvView kv{base + C, base + 2 * C, (size_t)T * 3 * C, (size_t)head_size, (size_t)3 * C, 0};
   return launch_attn(base, kv, nullptr, nullptr, (float*)work, (__nv_bfloat16*)y, B, T, n_head, head_size, T, st);
+}
+
+extern "C" int b2l_attention_nocache(void* qkv, const void* rope, void* y, void* work, int B, int T, int n_head,
+                                     int head_size, int block_size, b2l_stream_t stream) {
+  B2L_CHECK_ARG(qkv && rope && y && work && B > 0 && T > 0 && n_head > 0 && T <= block_size,
+                "b2l_attention_nocache: bad argument");
+  B2L_CHECK_SUPPORTED(head_size % 2 == 0 && head_size >= 2 && head_size <= 32 * ATT_MAX_EPL,
+                      "b2l_attention_nocache: head_size %d unsupported", head_size);
+  return attention_nocache_impl(qkv, rope, y, work, B, T, n_head, head_size, block_size, (cudaStream_t)stream);
+}
+
+extern "C" int b2l_attention_nocache_adapter(void* qkv, const void* rope, void* y, void* work, int B, int T,
+                                             int n_head, int head_size, int block_size,
+                                             const b2l_adapter_prefix* prefix, b2l_stream_t stream) {
+  B2L_CHECK_ARG(qkv && rope && y && work && B > 0 && T > 0 && n_head > 0 && T <= block_size,
+                "b2l_attention_nocache_adapter: bad argument");
+  B2L_CHECK_SUPPORTED(head_size % 2 == 0 && head_size >= 2 && head_size <= 32 * ATT_MAX_EPL,
+                      "b2l_attention_nocache_adapter: head_size %d unsupported", head_size);
+  if (int rc = check_adapter_prefix(prefix, "b2l_attention_nocache_adapter")) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (int rc = attention_nocache_impl(qkv, rope, y, work, B, T, n_head, head_size, block_size, st)) return rc;
+  return launch_adapter_prefix(qkv, prefix, y, B, T, n_head, head_size, st);
 }
 
 extern "C" int b2l_kv_unroll(const void* cache, const int32_t* ring_start, void* out, int B, int n_head, int S,

@@ -148,12 +148,18 @@ class CausalSelfAttention(nn.Module):
         lib = L.lib()
         rope32 = rope if rope.dtype == torch.float32 else rope.float()
         rope32 = rope32.contiguous()
+        prefix = self._adapter_prefix(kv_cache is not None)   # LLaMA-Adapter layers only (adapter.py)
         if kv_cache is None:
             work = torch.empty(lib.b2l_attn_workspace_bytes(B, self.n_head, hs, T, T) // 4 + 1, device=x.device, dtype=torch.float32)
             rows = rope32 if not _rope_is_table else rope32[:T]
-            rc = lib.b2l_attention_nocache(qkv.data_ptr(), rows.data_ptr(), y.data_ptr(), work.data_ptr(), B, T,
-                                           self.n_head, hs, rows.shape[0], L.stream_ptr())
-            L.check(rc, "b2l_attention_nocache")
+            if prefix is None:
+                rc = lib.b2l_attention_nocache(qkv.data_ptr(), rows.data_ptr(), y.data_ptr(), work.data_ptr(), B, T,
+                                               self.n_head, hs, rows.shape[0], L.stream_ptr())
+                L.check(rc, "b2l_attention_nocache")
+            else:
+                rc = lib.b2l_attention_nocache_adapter(qkv.data_ptr(), rows.data_ptr(), y.data_ptr(), work.data_ptr(), B, T,
+                                                       self.n_head, hs, rows.shape[0], C.byref(prefix), L.stream_ptr())
+                L.check(rc, "b2l_attention_nocache_adapter")
         else:
             cache_k, cache_v = kv_cache
             S = cache_k.shape[2]
@@ -165,12 +171,18 @@ class CausalSelfAttention(nn.Module):
                 L.check(lib.b2l_ring_advance(pos.data_ptr(), T, self._ring.data_ptr(), S, L.stream_ptr()), "b2l_ring_advance")
             work = torch.zeros(lib.b2l_attn_workspace_bytes(B, self.n_head, hs, T, S) // 4 + 1, device=x.device, dtype=torch.float32)
             flags = 0 if _rope_is_table else 4  # B2L_F_ROPE_ROWS
-            rc = lib.b2l_attention(qkv.data_ptr(), cache_k.data_ptr(), cache_v.data_ptr(), rope32.data_ptr(), pos.data_ptr(),
-                                   self._ring.data_ptr(), y.data_ptr(), work.data_ptr(), B, T, self.n_head, hs, S,
-                                   rope32.shape[0], flags, L.stream_ptr())
-            L.check(rc, "b2l_attention")
+            args = (qkv.data_ptr(), cache_k.data_ptr(), cache_v.data_ptr(), rope32.data_ptr(), pos.data_ptr(),
+                    self._ring.data_ptr(), y.data_ptr(), work.data_ptr(), B, T, self.n_head, hs, S, rope32.shape[0], flags)
+            if prefix is None:
+                L.check(lib.b2l_attention(*args, L.stream_ptr()), "b2l_attention")
+            else:
+                L.check(lib.b2l_attention_adapter(*args, C.byref(prefix), L.stream_ptr()), "b2l_attention_adapter")
         y = self.c_proj(y)
         return y, kv_cache
+
+    def _adapter_prefix(self, cached: bool) -> Optional[L.AdapterPrefix]:
+        """The LLaMA-Adapter prefix this layer attends to besides the cache (lit_llama_b200.adapter); None here."""
+        return None
 
 
 class MLP(nn.Module):
@@ -207,9 +219,13 @@ class Block(nn.Module):
     def __init__(self, config: LLaMAConfig) -> None:
         super().__init__()
         self.rms_1 = RMSNorm(config.n_embd)
-        self.attn = CausalSelfAttention(config)
+        self.attn = self._attention(config)
         self.rms_2 = RMSNorm(config.n_embd)
         self.mlp = MLP(config)
+
+    def _attention(self, config: LLaMAConfig) -> nn.Module:
+        """The Block's attention (lit_llama_b200.adapter passes the block index down, adapter.py:200)."""
+        return CausalSelfAttention(config)
 
     def forward(
         self,
@@ -297,11 +313,15 @@ class _DecodeState:
             att=self.att.data_ptr(), hid=self.hid.data_ptr(), attn_work=self.work.data_ptr(),
             logits=self.logits.data_ptr(), flags=model.decode_flags | (L.F_W8 if w8 else 0),
             batch_work=None if self.batch_ws is None else self.batch_ws.data_ptr())
+        adapters = model._adapter_prefixes()
+        if adapters is not None:   # LLaMA-Adapter: the step's attention adds each layer's gated prefix term
+            self.keep.append(adapters)
+            self.args.adapters = C.cast(adapters, C.POINTER(L.AdapterPrefix))
         # batch 1, head_size 128: the whole step as ONE persistent kernel (csrc/decode_mega.cu; int4 weights only, so
-        # gptq.int8 keeps one kernel per op under B2L_PERSISTENT=1 too)
+        # gptq.int8 keeps one kernel per op under B2L_PERSISTENT=1 too, and so do adapter models)
         self.plan = None
         kmax = max(C_, n_hidden)
-        if model.persistent and not w8 and B == 1 and hs == 128 and kmax <= 12288:
+        if model.persistent and not w8 and adapters is None and B == 1 and hs == 128 and kmax <= 12288:
             self.plan = torch.zeros(lib.b2l_decode_plan_bytes(C.byref(self.args)), dtype=torch.uint8, device=device)
             self.args.plan = self.plan.data_ptr()
             L.check(lib.b2l_decode_plan_build(C.byref(self.args), L.stream_ptr()), "b2l_decode_plan_build")
@@ -339,7 +359,7 @@ class LLaMA(nn.Module):
         self.transformer = nn.ModuleDict(
             dict(
                 wte=nn.Embedding(config.padded_vocab_size, config.n_embd),
-                h=nn.ModuleList(Block(config) for _ in range(config.n_layer)),
+                h=nn.ModuleList(self._block(config, i) for i in range(config.n_layer)),
                 ln_f=RMSNorm(config.n_embd),
             )
         )
@@ -355,6 +375,14 @@ class LLaMA(nn.Module):
         # gptq.int8, B == 1), False (module path)
         self._fast_ok: Union[None, bool, str] = None
         self._fc12_cache = {}
+
+    def _block(self, config: LLaMAConfig, block_idx: int) -> nn.Module:
+        """Block `block_idx` of the stack (lit_llama_b200.adapter passes the index down, adapter.py:236)."""
+        return Block(config)
+
+    def _adapter_prefixes(self):
+        """HOST array [n_layer] of b2l_adapter_prefix for b2l_decode_args::adapters, or None (no adapter)."""
+        return None
 
     def _init_weights(self, module: nn.Module) -> None:
         """model.py:70-74."""
@@ -432,6 +460,10 @@ class LLaMA(nn.Module):
         self._fc12_cache = {k: (key, tuple(fn(t) for t in val)) for k, (key, val) in self._fc12_cache.items()}
         self._decode, self._module_graph, self._fast_ok = None, None, None
         return out
+
+    def _fc12_is_only_copy(self, i: int) -> bool:
+        mlp = self.transformer.h[i].mlp
+        return getattr(mlp.c_fc1, "_released", False) and getattr(mlp.c_fc2, "_released", False)
 
     def _fc_from_fc12(self, i: int, which: int) -> torch.Tensor:
         """c_fc1 (which = 0) or c_fc2 (1) of layer i in the reference layout, rebuilt from the interleaved batch-1
@@ -548,7 +580,10 @@ class LLaMA(nn.Module):
                 # bakes weight pointers is stale (fc1|fc2 interleave, eligibility, module graph included)
                 st = self._decode = None
                 self._module_graph, self._fast_ok = None, None
-                self._fc12_cache.clear()
+                # the interleaved fc1|fc2 copies are rebuilt from the reference buffers, except where compact() made
+                # one the ONLY copy of both layers (still released: nothing was loaded into them)
+                self._fc12_cache = {k: v for k, v in self._fc12_cache.items()
+                                    if k[1] == "i8" and self._fc12_is_only_copy(k[0])}
             if st is None or st.B != B or st.S != max_seq_length or st.idx.dtype != idx.dtype or st.idx.device != idx.device:
                 if self._fast_ok is None:
                     self._fast_ok = self._fast_decode_ok()

@@ -10,8 +10,9 @@ same trick its own lora() context uses, lit_llama/lora.py:472-476).  After
 the reference's own `generate.py` (`main()`, `--quantize gptq.int4`) builds H100
 modules: `lit_llama.LLaMA`, `lit_llama.model.{LLaMA,Block,CausalSelfAttention,MLP,
 RMSNorm,apply_rope,build_rope_cache}`, `lit_llama.quantization.{ColBlockQuantizedLinear,
-Linear8bitLt}` and `lit_llama.utils.{quantization,EmptyInitOnDevice,lazy_load}`
-all point at this package.
+Linear8bitLt}`, `lit_llama.utils.{quantization,EmptyInitOnDevice,lazy_load}` and, when the
+package has it, `lit_llama.adapter.{LLaMA,LLaMAConfig,Block,CausalSelfAttention}` (LLaMA-Adapter,
+`generate/adapter.py`) all point at this package.
 """
 import sys
 
@@ -51,9 +52,28 @@ def patch_reference(lit_llama_module=None):
         setattr(ref_utils, name, getattr(u, name))
     saved[("utils", "quantization")] = ref_utils.quantization
     ref_utils.quantization = u.quantization
+    # LLaMA-Adapter (lit_llama/adapter.py), when the package has it
+    ref_adapter = sys.modules.get(lit_llama_module.__name__ + ".adapter")
+    if ref_adapter is None:
+        import importlib
+
+        try:
+            ref_adapter = importlib.import_module(lit_llama_module.__name__ + ".adapter")
+        except ImportError:
+            ref_adapter = None
+    if ref_adapter is not None:
+        from . import adapter as a
+
+        for name in ("LLaMA", "LLaMAConfig", "Block", "CausalSelfAttention"):
+            saved[("adapter", name)] = getattr(ref_adapter, name, None)
+            setattr(ref_adapter, name, getattr(a, name))
     for mod in list(sys.modules.values()):  # scripts that did `from lit_llama.utils import quantization`
         if mod is not None and getattr(mod, "quantization", None) is saved[("utils", "quantization")]:
             setattr(mod, "quantization", u.quantization)
         if mod is not None and getattr(mod, "LLaMA", None) is saved[("model", "LLaMA")]:
             setattr(mod, "LLaMA", m.LLaMA)
+        # generate/adapter.py did `from lit_llama.adapter import LLaMA`
+        if ref_adapter is not None and mod is not None and saved[("adapter", "LLaMA")] is not None \
+                and getattr(mod, "LLaMA", None) is saved[("adapter", "LLaMA")]:
+            setattr(mod, "LLaMA", a.LLaMA)
     return saved

@@ -98,13 +98,15 @@ class ColBlockQuantizedLinear(torch.nn.Module):
         self._tiled = self._tiled_mma = self._tiled_i8 = None
         weights_changed()
 
-    def _load_from_state_dict(self, *args, **kwargs):
-        if self._released:   # a new checkpoint is coming: the buffer it is copied into has to exist again
+    def _load_from_state_dict(self, state_dict, prefix, *args, **kwargs):
+        # a checkpoint with this layer's levels is coming: the buffer it is copied into has to exist again.  A dict
+        # without them (e.g. adapter weights loaded with strict=False) leaves a compacted layer's only copy alone.
+        if self._released and prefix + "quant_weight" in state_dict:
             self.quant_weight = torch.empty((self.in_features // self.entries_per_byte, self.out_features), dtype=torch.uint8,
                                             device=self.scales.device).t()
             self._released, self._source = False, None
             self._tiled = self._tiled_mma = self._tiled_i8 = None
-        super()._load_from_state_dict(*args, **kwargs)   # copies in place: pointers stay, contents (and _version) change
+        super()._load_from_state_dict(state_dict, prefix, *args, **kwargs)   # copies in place: pointers stay, contents (and _version) change
         weights_changed()
 
     def _save_to_state_dict(self, destination, prefix, keep_vars):

@@ -15,7 +15,7 @@ import time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-SECTIONS = ["generic", "tile", "tc_small", "tc_shapes", "tc_modes", "gemv", "grid_flag", "hmma_rate", "imma_rate", "consumer_rate", "bench_gemm", "bench_tc", "trace", "bench_layers", "bench_gemv", "bench_step", "bench_ctx", "bench_13b_b8", "bench_sizes", "batch_debug", "bench_step_int8", "bench_q8_gemm", "bench_q8_gemv", "bench_w8_gemv", "bench_w8_gemm", "bench_step_w8", "timeline", "mega_timeline"]
+SECTIONS = ["generic", "tile", "tc_small", "tc_shapes", "tc_modes", "gemv", "grid_flag", "hmma_rate", "imma_rate", "consumer_rate", "bench_gemm", "bench_tc", "trace", "bench_layers", "bench_gemv", "bench_step", "bench_ctx", "bench_13b_b8", "bench_sizes", "batch_debug", "bench_step_int8", "bench_q8_gemm", "bench_q8_gemv", "bench_w8_gemv", "bench_w8_gemm", "bench_step_w8", "bench_step_adapter", "timeline", "mega_timeline"]
 
 
 _DLIB = None
@@ -1241,6 +1241,58 @@ def sec_bench_q8_gemv():
               f"CB direct {med(t_c):.2f} us = {N * K / med(t_c) / 1e3:.0f} GB/s [{fmt(t_c)}] | CB/tiled {med(t_c) / med(t_t):.3f}", flush=True)
         del cbs, scbs, wts, ys, y2
         torch.cuda.empty_cache()
+
+
+def sec_bench_step_adapter():
+    """LLaMA-Adapter on the fused step: 7B gptq.int4 synthetic weights compacted, batch-1 decode at ctx ~2000 under the
+    graph, with a random adapter (aT = 10, start layer 2, non-zero gates) against the same weights without it,
+    alternated in one process.  The prefix term runs inside the fused attention launch (5 n_layer + 3 launches)."""
+    import ctypes
+
+    import torch
+    import lit_llama_b200 as P
+    from lit_llama_b200 import adapter as PA
+    from lit_llama_b200.utils import quantization
+    from bench import build_synthetic_model, synth_state
+
+    dev = torch.device("cuda")
+    sd = synth_state("7B", 1234, dev)
+    plain = build_synthetic_model("7B", dev, state=sd).compact()
+    prev = torch.get_default_dtype()
+    torch.set_default_dtype(torch.bfloat16)
+    try:
+        with torch.device(dev), quantization("gptq.int4"):
+            ada = PA.LLaMA.from_name("7B")
+    finally:
+        torch.set_default_dtype(prev)
+    g = torch.Generator(device=dev).manual_seed(7)
+    with torch.no_grad():
+        own = ada.state_dict()
+        for k, v in sd.items():
+            own[k].copy_(v)
+        for blk in ada.transformer.h[ada.config.adapter_start_layer:]:
+            blk.attn.adapter_wte.weight.copy_(torch.randn(blk.attn.adapter_wte.weight.shape, generator=g, device=dev))
+            blk.attn.gating_factor.copy_((torch.rand(blk.attn.gating_factor.shape, generator=g, device=dev) + 0.5))
+    del sd, own
+    ada = ada.eval().compact()
+    torch.cuda.empty_cache()
+    S = 2048
+    for m in (plain, ada):
+        m.copy_logits = False
+        with torch.no_grad():
+            m(torch.randint(0, 32000, (1, 16), device=dev, dtype=torch.int32), S, torch.arange(16, device=dev))
+    lib = P._lib.lib()
+    res = {"plain": [], "adapter": []}
+    for r in range(4):
+        for name, m in (("plain", plain), ("adapter", ada)):
+            res[name].append(_decode_us(m, 1, S, dev, p0=1960, n=24))
+            if r == 0:
+                n = lib.b2l_decode_step_launches(ctypes.byref(m._decode.args))
+                print(f"{name}: fused step {m._decode is not None}, graph {m._decode.graph is not None}, {n} launches", flush=True)
+    a, b = min(res["plain"]), min(res["adapter"])
+    print(f"7B gptq.int4 compacted, batch 1, ctx ~1966-1990, graph + PDL on {_card()}")
+    print(f"  plain   : {' '.join(f'{x:.1f}' for x in res['plain'])} us/token (best {a:.1f})")
+    print(f"  adapter : {' '.join(f'{x:.1f}' for x in res['adapter'])} us/token (best {b:.1f})  -> {100 * (b - a) / a:+.2f} %")
 
 
 def sec_timeline():
