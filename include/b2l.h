@@ -346,6 +346,37 @@ int b2l_attention_nocache_adapter(void* qkv, const void* rope, void* y, void* wo
                                   int n_head, int head_size, int block_size,
                                   const b2l_adapter_prefix* prefix, b2l_stream_t stream);
 
+/* ------------------------------------------------------------------------------
+ * LoRA (lit_llama/lora.py:92-326): the low-rank term of an UNMERGED MergedLinear,
+ * added in place to the output y of its base linear (lora.py:308-326):
+ *   u_m = bf16(A_g . xh_m)   d = bf16(B_g . u_m)   y = bf16(y + bf16(d * scaling))
+ * for every enabled group g (zero_pad, lora.py:205-241), fp32 accumulation.  A quantized
+ * base (gptq.int4 / gptq.int8 / llm.int8) cannot absorb the merge of lora.py:243-280,
+ * so this term runs per token.
+ *   A        bf16 lora_A [r * n_on][K], 16-byte aligned (n_on = enabled groups)
+ *   B        bf16 lora_B [N / n_groups * n_on][r]
+ *   scaling  lora_alpha / r (lora.py:171)
+ *   r        1..64
+ *   n_groups len(enable_lora), 1..32, divides N;  enabled: bit g = enable_lora[g]
+ * ---------------------------------------------------------------------------- */
+typedef struct b2l_lora {
+  const void* A;
+  const void* B;
+  float scaling;
+  int r;
+  int n_groups;
+  unsigned enabled;
+} b2l_lora;
+#define B2L_LORA_MAX_R 64
+/* y[M, N] (leading dim ldy) += the term for M rows of x[M, K] (leading dim ldx, a multiple
+ * of 8, 16-byte aligned; K a multiple of 8).  norm_scale != NULL: xh = RMSNorm(x) with
+ * norm_scale / eps and b2l_rmsnorm's rounding points (x is then the residual stream, as in
+ * the whole-token step); NULL: xh = x.  flags 0 or B2L_F_PDL (lora_A / lora_B are requested
+ * from L2 before griddepcontrol.wait; x and y are read only after it).  Any M.  Bad
+ * arguments are rejected before any launch. */
+int b2l_lora_apply(const b2l_lora* lora, const void* x, int ldx, const void* norm_scale, float eps,
+                   void* y, int ldy, int M, int N, int K, int flags, b2l_stream_t stream);
+
 /* kv_caches as the reference would hold them (logical order): un-rotates the ring
  * into `out` [B, nh, S, hs]. */
 int b2l_kv_unroll(const void* cache, const int32_t* ring_start, void* out, int B, int n_head,
@@ -411,6 +442,10 @@ typedef struct b2l_decode_args {
                                 NULL: one kernel per op                                   */
   const b2l_adapter_prefix* adapters; /* HOST array [n_layer] of LLaMA-Adapter prefixes (b2l_attention_adapter);
                                 NULL = no adapter anywhere, an entry with len == 0 = none in that layer.
+                                Not with `plan`.                                          */
+  const b2l_lora* loras;     /* HOST array [n_layer] of c_attn LoRA terms (lora.py:405-446; b2l_lora_apply with
+                                rms_1 as the norm, enqueued between c_attn and the attention, without timeline
+                                stamps).  NULL = no LoRA anywhere, an entry with r == 0 = none in that layer.
                                 Not with `plan`.                                          */
 } b2l_decode_args;
 

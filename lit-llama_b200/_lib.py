@@ -53,6 +53,16 @@ class AdapterPrefix(C.Structure):
 ADAPTER_MAX_LEN = 64   # B2L_ADAPTER_MAX_LEN
 
 
+class LoRA(C.Structure):
+    """b2l_lora: one linear's LoRA weights (lora_A [r n_on][K], lora_B [N/n_groups n_on][r], bf16), scaling = alpha / r,
+    len(enable_lora) groups and the mask of the enabled ones."""
+    _fields_ = [("A", c_void_p), ("B", c_void_p), ("scaling", c_float), ("r", c_int), ("n_groups", c_int),
+                ("enabled", C.c_uint)]
+
+
+LORA_MAX_R = 64   # B2L_LORA_MAX_R
+
+
 class DecodeArgs(C.Structure):
     _fields_ = [
         ("n_layer", c_int), ("n_head", c_int), ("n_embd", c_int), ("n_hidden", c_int), ("vocab", c_int),
@@ -63,7 +73,7 @@ class DecodeArgs(C.Structure):
         ("input_pos", c_void_p), ("ring_start", c_void_p), ("block_size", c_int),
         ("x", c_void_p), ("qkv", c_void_p), ("att", c_void_p), ("hid", c_void_p), ("attn_work", c_void_p),
         ("logits", c_void_p), ("flags", c_int), ("timeline", c_void_p), ("batch_work", c_void_p),
-        ("plan", c_void_p), ("adapters", C.POINTER(AdapterPrefix)),
+        ("plan", c_void_p), ("adapters", C.POINTER(AdapterPrefix)), ("loras", C.POINTER(LoRA)),
     ]
 
 
@@ -118,6 +128,8 @@ _SIGS = {
                                       c_int, c_int, c_int, c_int, c_int, c_int, C.POINTER(AdapterPrefix), c_void_p]),
     "b2l_attention_nocache_adapter": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                               C.POINTER(AdapterPrefix), c_void_p]),
+    "b2l_lora_apply": (c_int, [C.POINTER(LoRA), c_void_p, c_int, c_void_p, c_float, c_void_p, c_int, c_int, c_int, c_int,
+                               c_int, c_void_p]),
     "b2l_tp_buffer_bytes": (c_size_t, [c_int, c_int]),
     "b2l_tp_allreduce": (c_int, [C.POINTER(TPComm), c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "b2l_ring_advance": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p]),

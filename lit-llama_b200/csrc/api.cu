@@ -12,6 +12,7 @@ namespace b2l {
 extern void* g_attn_timeline;
 int decode_step_persistent(const b2l_decode_args* d, b2l_stream_t stream);   // decode_mega.cu
 int check_adapter_prefix(const b2l_adapter_prefix* pre, const char* who);     // attention.cu
+int check_lora(const b2l_lora* lo, int N, int K, const char* who);            // lora.cu
 
 static thread_local char g_err[512] = "";
 
@@ -171,6 +172,9 @@ extern "C" int b2l_decode_step_launches(const b2l_decode_args* d) {
   // an adapter layer adds the prefix kernel behind the three-kernel attention (the fused kernel does it in-launch)
   if (!fused && d->adapters != nullptr)
     for (int l = 0; l < d->n_layer; ++l) n += d->adapters[l].len != 0;
+  // a LoRA layer adds its low-rank term's launch behind c_attn
+  if (d->loras != nullptr)
+    for (int l = 0; l < d->n_layer; ++l) n += d->loras[l].r != 0;
   return n;
 }
 
@@ -191,6 +195,13 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
       if (d->adapters[l].len == 0) continue;   // no adapter in this layer
       B2L_CHECK_SUPPORTED(d->plan == nullptr, "b2l_decode_step: adapters do not run in the persistent kernel (plan must be NULL)");
       if (int rc = check_adapter_prefix(&d->adapters[l], "b2l_decode_step")) return rc;
+    }
+  }
+  if (d->loras != nullptr) {
+    for (int l = 0; l < d->n_layer; ++l) {
+      if (d->loras[l].r == 0) continue;   // no LoRA in this layer
+      B2L_CHECK_SUPPORTED(d->plan == nullptr, "b2l_decode_step: LoRA layers do not run in the persistent kernel (plan must be NULL)");
+      if (int rc = check_lora(&d->loras[l], 3 * d->n_embd, d->n_embd, "b2l_decode_step")) return rc;
     }
   }
   if (d->plan != nullptr) return decode_step_persistent(d, stream);   // one persistent kernel per token (decode_mega.cu)
@@ -217,6 +228,10 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
     const b2l_layer& L = d->layers[l];
     if ((rc = q4_call(L.c_attn, d->x, C, d->qkv, 3 * C, B, d->sz_dtype, B2L_PRO_RMSNORM, L.rms_1, d->eps, B2L_EPI_STORE,
                       nullptr, 0, fl, stream, tl(), d->batch_work, pf(), (kv_ok && kv_prefetch == 2) ? d : nullptr, l)))
+      return rc;
+    // LoRA on c_attn (lora.py:308-326): the low-rank term from rms_1(x), added into qkv in place
+    if (d->loras != nullptr && d->loras[l].r != 0 &&
+        (rc = b2l_lora_apply(&d->loras[l], d->x, C, L.rms_1, d->eps, d->qkv, 3 * C, B, 3 * C, C, fl & B2L_F_PDL, stream)))
       return rc;
     g_attn_timeline = tl();
     const b2l_adapter_prefix* pre = (d->adapters != nullptr && d->adapters[l].len != 0) ? &d->adapters[l] : nullptr;

@@ -184,6 +184,10 @@ class CausalSelfAttention(nn.Module):
         """The LLaMA-Adapter prefix this layer attends to besides the cache (lit_llama_b200.adapter); None here."""
         return None
 
+    def _lora(self):
+        """(b2l_lora, tensors it points at) of a quantized LoRA c_attn (lit_llama_b200.lora); None here."""
+        return None
+
 
 class MLP(nn.Module):
     """model.py:240-254."""
@@ -317,11 +321,14 @@ class _DecodeState:
         if adapters is not None:   # LLaMA-Adapter: the step's attention adds each layer's gated prefix term
             self.keep.append(adapters)
             self.args.adapters = C.cast(adapters, C.POINTER(L.AdapterPrefix))
+        loras = model._loras(self.keep)
+        if loras is not None:      # LoRA: the step adds each layer's low-rank term behind c_attn
+            self.args.loras = C.cast(loras, C.POINTER(L.LoRA))
         # batch 1, head_size 128: the whole step as ONE persistent kernel (csrc/decode_mega.cu; int4 weights only, so
-        # gptq.int8 keeps one kernel per op under B2L_PERSISTENT=1 too, and so do adapter models)
+        # gptq.int8 keeps one kernel per op under B2L_PERSISTENT=1 too, and so do adapter and LoRA models)
         self.plan = None
         kmax = max(C_, n_hidden)
-        if model.persistent and not w8 and adapters is None and B == 1 and hs == 128 and kmax <= 12288:
+        if model.persistent and not w8 and adapters is None and loras is None and B == 1 and hs == 128 and kmax <= 12288:
             self.plan = torch.zeros(lib.b2l_decode_plan_bytes(C.byref(self.args)), dtype=torch.uint8, device=device)
             self.args.plan = self.plan.data_ptr()
             L.check(lib.b2l_decode_plan_build(C.byref(self.args), L.stream_ptr()), "b2l_decode_plan_build")
@@ -383,6 +390,20 @@ class LLaMA(nn.Module):
     def _adapter_prefixes(self):
         """HOST array [n_layer] of b2l_adapter_prefix for b2l_decode_args::adapters, or None (no adapter)."""
         return None
+
+    def _loras(self, keep: list):
+        """HOST array [n_layer] of b2l_lora for b2l_decode_args::loras, or None (no LoRA layer); what it points at is
+        appended to `keep`."""
+        terms = [blk.attn._lora() for blk in self.transformer.h]
+        if all(t is None for t in terms):
+            return None
+        arr = (L.LoRA * len(terms))()
+        for i, t in enumerate(terms):
+            if t is not None:
+                arr[i] = t[0]
+                keep.append(t[1])
+        keep.append(arr)
+        return arr
 
     def _init_weights(self, module: nn.Module) -> None:
         """model.py:70-74."""

@@ -12,7 +12,8 @@ modules: `lit_llama.LLaMA`, `lit_llama.model.{LLaMA,Block,CausalSelfAttention,ML
 RMSNorm,apply_rope,build_rope_cache}`, `lit_llama.quantization.{ColBlockQuantizedLinear,
 Linear8bitLt}`, `lit_llama.utils.{quantization,EmptyInitOnDevice,lazy_load}` and, when the
 package has it, `lit_llama.adapter.{LLaMA,LLaMAConfig,Block,CausalSelfAttention}` (LLaMA-Adapter,
-`generate/adapter.py`) all point at this package.
+`generate/adapter.py`) and `lit_llama.lora.{lora,MergedLinear,LoRALayer,LoRAConfig,CausalSelfAttention,
+mark_only_lora_as_trainable,lora_state_dict}` (LoRA, `generate/lora.py`) all point at this package.
 """
 import sys
 
@@ -67,6 +68,22 @@ def patch_reference(lit_llama_module=None):
         for name in ("LLaMA", "LLaMAConfig", "Block", "CausalSelfAttention"):
             saved[("adapter", name)] = getattr(ref_adapter, name, None)
             setattr(ref_adapter, name, getattr(a, name))
+    # LoRA (lit_llama/lora.py), when the package has it
+    ref_lora = sys.modules.get(lit_llama_module.__name__ + ".lora")
+    if ref_lora is None:
+        import importlib
+
+        try:
+            ref_lora = importlib.import_module(lit_llama_module.__name__ + ".lora")
+        except ImportError:
+            ref_lora = None
+    if ref_lora is not None:
+        from . import lora as lo
+
+        for name in ("LoRALayer", "MergedLinear", "LoRAConfig", "CausalSelfAttention", "lora", "mark_only_lora_as_trainable",
+                     "lora_state_dict"):
+            saved[("lora", name)] = getattr(ref_lora, name, None)
+            setattr(ref_lora, name, getattr(lo, name))
     for mod in list(sys.modules.values()):  # scripts that did `from lit_llama.utils import quantization`
         if mod is not None and getattr(mod, "quantization", None) is saved[("utils", "quantization")]:
             setattr(mod, "quantization", u.quantization)
@@ -76,4 +93,8 @@ def patch_reference(lit_llama_module=None):
         if ref_adapter is not None and mod is not None and saved[("adapter", "LLaMA")] is not None \
                 and getattr(mod, "LLaMA", None) is saved[("adapter", "LLaMA")]:
             setattr(mod, "LLaMA", a.LLaMA)
+        # generate/lora.py did `from lit_llama.lora import lora`
+        if ref_lora is not None and mod is not None and saved[("lora", "lora")] is not None \
+                and getattr(mod, "lora", None) is saved[("lora", "lora")]:
+            setattr(mod, "lora", lo.lora)
     return saved

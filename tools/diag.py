@@ -15,7 +15,7 @@ import time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-SECTIONS = ["generic", "tile", "tc_small", "tc_shapes", "tc_modes", "gemv", "grid_flag", "hmma_rate", "imma_rate", "consumer_rate", "bench_gemm", "bench_tc", "trace", "bench_layers", "bench_gemv", "bench_step", "bench_ctx", "bench_13b_b8", "bench_sizes", "batch_debug", "bench_step_int8", "bench_q8_gemm", "bench_q8_gemv", "bench_w8_gemv", "bench_w8_gemm", "bench_step_w8", "bench_step_adapter", "timeline", "mega_timeline"]
+SECTIONS = ["generic", "tile", "tc_small", "tc_shapes", "tc_modes", "gemv", "grid_flag", "hmma_rate", "imma_rate", "consumer_rate", "bench_gemm", "bench_tc", "trace", "bench_layers", "bench_gemv", "bench_step", "bench_ctx", "bench_13b_b8", "bench_sizes", "batch_debug", "bench_step_int8", "bench_q8_gemm", "bench_q8_gemv", "bench_w8_gemv", "bench_w8_gemm", "bench_step_w8", "bench_step_adapter", "bench_step_lora", "bench_lora_kernel", "lora_timeline", "timeline", "mega_timeline"]
 
 
 _DLIB = None
@@ -1293,6 +1293,159 @@ def sec_bench_step_adapter():
     print(f"7B gptq.int4 compacted, batch 1, ctx ~1966-1990, graph + PDL on {_card()}")
     print(f"  plain   : {' '.join(f'{x:.1f}' for x in res['plain'])} us/token (best {a:.1f})")
     print(f"  adapter : {' '.join(f'{x:.1f}' for x in res['adapter'])} us/token (best {b:.1f})  -> {100 * (b - a) / a:+.2f} %")
+
+
+def _lora_7b(dev):
+    """7B gptq.int4 synthetic weights, compacted, without and with a random r = 8 LoRA on q and v in all 32 layers
+    (alpha 16, non-zero lora_B): (plain, lora) on the same base weights."""
+    import torch
+    import lit_llama_b200 as P
+    from lit_llama_b200 import lora as PL
+    from lit_llama_b200.utils import quantization
+    from bench import build_synthetic_model, synth_state
+
+    sd = synth_state("7B", 1234, dev)
+    plain = build_synthetic_model("7B", dev, state=sd).compact()
+    prev = torch.get_default_dtype()
+    torch.set_default_dtype(torch.bfloat16)
+    try:
+        with torch.device(dev), quantization("gptq.int4"), PL.lora(r=8, alpha=16, dropout=0.05):
+            lm = P.LLaMA.from_name("7B")
+    finally:
+        torch.set_default_dtype(prev)
+    g = torch.Generator(device=dev).manual_seed(7)
+    with torch.no_grad():
+        own = lm.state_dict()
+        for k, v in sd.items():
+            own[k].copy_(v)
+        for blk in lm.transformer.h:
+            c = blk.attn.c_attn
+            c.lora_A.copy_((torch.rand(c.lora_A.shape, generator=g, device=dev) * 2 - 1) / 64)
+            c.lora_B.copy_(torch.randn(c.lora_B.shape, generator=g, device=dev) * 0.05)
+    del sd, own
+    lm = lm.eval().compact()
+    torch.cuda.empty_cache()
+    return plain, lm
+
+
+def sec_bench_step_lora():
+    """LoRA on the fused step: 7B gptq.int4 synthetic weights compacted, batch-1 decode at ctx ~2000 under the graph,
+    with a random r = 8 LoRA on q and v in all 32 layers (alpha 16, non-zero lora_B) against the same weights without
+    it, alternated in one process; then a 512-token prompt with and without it.  The LoRA model's step is one launch
+    per layer longer (5 n_layer + 3 + n_layer)."""
+    import ctypes
+    import time
+
+    import torch
+    import lit_llama_b200 as P
+
+    dev = torch.device("cuda")
+    plain, lm = _lora_7b(dev)
+    S = 2048
+    for m in (plain, lm):
+        m.copy_logits = False
+        with torch.no_grad():
+            m(torch.randint(0, 32000, (1, 16), device=dev, dtype=torch.int32), S, torch.arange(16, device=dev))
+    lib = P._lib.lib()
+    res = {"plain": [], "lora": []}
+    for r in range(4):
+        for name, m in (("plain", plain), ("lora", lm)):
+            res[name].append(_decode_us(m, 1, S, dev, p0=1960, n=24))
+            if r == 0:
+                n = lib.b2l_decode_step_launches(ctypes.byref(m._decode.args))
+                print(f"{name}: fused step {m._decode is not None}, graph {m._decode.graph is not None}, {n} launches", flush=True)
+    a, b = min(res["plain"]), min(res["lora"])
+    card = _card()
+    print(f"7B gptq.int4 compacted, batch 1, ctx ~1966-1990, graph + PDL on {card}")
+    print(f"  plain : {' '.join(f'{x:.1f}' for x in res['plain'])} us/token (best {a:.1f})")
+    print(f"  lora  : {' '.join(f'{x:.1f}' for x in res['lora'])} us/token (best {b:.1f})  -> {100 * (b - a) / a:+.2f} %, "
+          f"{(b - a) / 32:.2f} us per layer")
+    prompt = torch.randint(0, 32000, (1, 512), device=dev, dtype=torch.int32)
+    pres = {"plain": [], "lora": []}
+    for r in range(4):
+        for name, m in (("plain", plain), ("lora", lm)):
+            m.reset_cache()
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            with torch.no_grad():
+                m(prompt, S, torch.arange(512, device=dev))
+            torch.cuda.synchronize()
+            pres[name].append((time.perf_counter() - t0) * 1e3)
+    pa, pb = min(pres["plain"][1:]), min(pres["lora"][1:])
+    print(f"512-token prompt on {card}: plain {' '.join(f'{x:.2f}' for x in pres['plain'])} ms (best {pa:.2f}), "
+          f"lora {' '.join(f'{x:.2f}' for x in pres['lora'])} ms (best {pb:.2f}) -> {100 * (pb - pa) / pa:+.2f} %")
+
+
+def sec_bench_lora_kernel():
+    """b2l_lora_apply alone on the 7B c_attn shape (r = 8, q and v): GPU time per launch in a graph of back-to-back
+    launches, with and without the RMSNorm prologue, over M.  Back to back, each launch waits for the previous one
+    (no PDL), so this is the kernel's own latency, not the dependency link inside the step."""
+    import ctypes
+
+    import torch
+    from lit_llama_b200 import _lib as L
+
+    dev = torch.device("cuda")
+    C_, r = 4096, 8
+    A = ((torch.rand(2 * r, C_, device=dev) * 2 - 1) / 64).to(torch.bfloat16)
+    B = (torch.randn(2 * C_, r, device=dev) * 0.05).to(torch.bfloat16)
+    sc = torch.ones(C_, device=dev, dtype=torch.bfloat16)
+    spec = L.LoRA(A.data_ptr(), B.data_ptr(), 2.0, r, 3, 0b101)
+    lib = L.lib()
+    for M in (1, 4, 16, 512):
+        x = torch.randn(M, C_, device=dev).to(torch.bfloat16)
+        y = torch.zeros(M, 3 * C_, device=dev, dtype=torch.bfloat16)
+        row = []
+        for norm in (None, sc):
+            def fn():
+                lib.b2l_lora_apply(ctypes.byref(spec), x.data_ptr(), C_, None if norm is None else norm.data_ptr(), 1e-5,
+                                   y.data_ptr(), 3 * C_, M, 3 * C_, C_, 0, L.stream_ptr())
+            row.append(_time_graph(fn, 200))
+        print(f"M={M}: {row[0]:.2f} us plain input, {row[1]:.2f} us with the RMSNorm prologue", flush=True)
+    print(f"on {_card()}")
+
+
+def sec_lora_timeline():
+    """Where a LoRA layer's time goes in the fused step (7B gptq.int4, compacted, r = 8 on q and v, one eager step at
+    ctx ~1970, PDL on): %globaltimer stamps of c_attn, the attention and c_proj of layers 4..5, the plain model and the
+    LoRA model on the same weights.  The LoRA launch itself has no stamps: it sits between c_attn's end and the
+    attention's wait_done."""
+    import torch
+
+    dev = torch.device("cuda")
+    plain, lm = _lora_7b(dev)
+    S, pos0 = 2048, 1960
+    tok = torch.randint(0, 32000, (1, 1), device=dev, dtype=torch.int32)
+    for name, model in (("plain", plain), ("lora", lm)):
+        model.graph_after = 0
+        model.copy_logits = False
+        with torch.no_grad():
+            model(torch.randint(0, 32000, (1, 16), device=dev, dtype=torch.int32), S, torch.arange(16, device=dev))
+            for rep in range(3):
+                for i in range(3):
+                    model(tok, S, torch.tensor([pos0 + i], device=dev))
+                st = model._decode
+                n = 5 * model.config.n_layer + 1
+                tl = torch.zeros((n, 64), dtype=torch.int64, device=dev)
+                tl[:, 0] = 2**62
+                tl[:, 60] = 2**62
+                tl[:, 61] = 2**62
+                st.args.timeline = tl.data_ptr()
+                model(tok, S, torch.tensor([pos0 + 3], device=dev))
+                torch.cuda.synchronize()
+                st.args.timeline = None
+                t = tl.cpu()
+                l4, l5 = 5 * 4, 5 * 5
+
+                def us(a, b):
+                    return (int(a) - int(b)) / 1e3
+
+                print(f"{name} rep {rep}: layer 4 -> 5 start {us(t[l5, 0], t[l4, 0]):.2f} us | c_attn start->end "
+                      f"{us(t[l4, 4], t[l4, 0]):.2f} | c_attn end -> attn start {us(t[l4 + 1, 0], t[l4, 4]):.2f} | "
+                      f"c_attn end -> attn wait_done {us(t[l4 + 1, 1], t[l4, 4]):.2f} | attn wait_done -> end "
+                      f"{us(t[l4 + 1, 4], t[l4 + 1, 1]):.2f} | attn end -> c_proj end {us(t[l4 + 2, 4], t[l4 + 1, 4]):.2f} | "
+                      f"whole step {us(t[n - 1, 4], t[0, 0]):.1f} us", flush=True)
+    print(f"on {_card()}")
 
 
 def sec_timeline():
