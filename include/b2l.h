@@ -84,6 +84,15 @@ enum {
                            y = bf16(bf16(silu(bf16(a))) * bf16(b))   model.py:252     */
 };
 
+/* LLaMA-Adapter v2's per-output-feature affine of a linear (lit_llama/adapter_v2.py:30-47):
+ *   y = bf16(scale * bf16(linear(x) + bias))
+ * scale, bias bf16 [N] in the row order of the weight layout in use (for B2L_EPI_SWIGLU: interleaved like the
+ * weight rows).  Both NULL = off; exactly one NULL is B2L_E_ARG. */
+typedef struct b2l_out_affine {
+  const void* scale;
+  const void* bias;
+} b2l_out_affine;
+
 #define B2L_PF_SEGMENTS 4
 typedef struct b2l_q4_linear_args {
   const void* x;        /* bf16 [M, K], leading dim ldx                               */
@@ -123,6 +132,10 @@ typedef struct b2l_q4_linear_args {
   const long long* pf_rows;
   int pf_rows_max, pf_nseg, pf_row_bytes;
   unsigned long long pf_seg_stride;
+  b2l_out_affine out_affine; /* b2l_q4_gemv / b2l_w8_gemv only: the affine above, applied to the linear's bf16
+                           output before the STORE / RESIDUAL / SWIGLU epilogue.  b2l_q4_linear_tc, b2l_q4_gemm,
+                           b2l_w8_gemm and b2l_q4_gemv_batch return B2L_E_UNSUPPORTED when it is set (their
+                           callers apply b2l_linear_affine to the output instead)                        */
 } b2l_q4_linear_args;
 
 enum {
@@ -212,6 +225,12 @@ int b2l_silu_mul(const void* a, const void* b, void* y, size_t n, b2l_stream_t s
 
 /* x + h, model.py:166-167. */
 int b2l_add(const void* a, const void* b, void* y, size_t n, b2l_stream_t stream);
+
+/* LLaMA-Adapter v2's linear affine (adapter_v2.py:30-33) in place on a linear's output:
+ * y[m, n] = bf16(scale[n] * bf16(y[m, n] + bias[n])) for M rows of N columns, leading dimension ldy >= N.
+ * y, scale, bias bf16.  Bad arguments are rejected before any launch. */
+int b2l_linear_affine(void* y, int ldy, int M, int N, const void* scale, const void* bias,
+                      b2l_stream_t stream);
 
 /* ------------------------------------------------------------------------------
  * Linear8bitLt  (lit_llama/quantization.py:38-77; forward inherited from bitsandbytes:
@@ -408,6 +427,12 @@ typedef struct b2l_layer {
   void* v_cache;
 } b2l_layer;
 
+/* LLaMA-Adapter v2: the affine of each of a Block's linears (adapter_v2.py:30-47); c_fc12's vectors are
+ * [2*n_hidden] in the row order of c_fc12.qw_mma (8 of c_fc1 | 8 of c_fc2 per 16 rows). */
+typedef struct b2l_layer_affine {
+  b2l_out_affine c_attn, c_proj, c_fc12, mlp_proj;
+} b2l_layer_affine;
+
 typedef struct b2l_decode_args {
   int n_layer, n_head, n_embd, n_hidden, vocab; /* vocab = padded_vocab_size          */
   int B, S;                                     /* batch, max_seq_length              */
@@ -447,6 +472,11 @@ typedef struct b2l_decode_args {
                                 rms_1 as the norm, enqueued between c_attn and the attention, without timeline
                                 stamps).  NULL = no LoRA anywhere, an entry with r == 0 = none in that layer.
                                 Not with `plan`.                                          */
+  const b2l_layer_affine* affines; /* HOST array [n_layer] of LLaMA-Adapter v2 affines, applied inside each linear's
+                                launch (b2l_q4_linear_args::out_affine), so the launch count does not change.
+                                NULL = none.  Only at B == 1 on the batch-1 kernels (every weight needs qw_mma);
+                                not with `plan` or `loras`.                               */
+  b2l_out_affine lm_head_affine; /* the same for lm_head (both NULL = none)                 */
 } b2l_decode_args;
 
 int b2l_decode_step(const b2l_decode_args* args, b2l_stream_t stream);

@@ -18,6 +18,11 @@ F_W8 = 32   # b2l_decode_step: every linear is gptq.int8 (b2l_w8_gemv)
 c_void_p, c_int, c_float, c_size_t = C.c_void_p, C.c_int, C.c_float, C.c_size_t
 
 
+class OutAffine(C.Structure):
+    """b2l_out_affine: LLaMA-Adapter v2's per-output-feature scale and bias (bf16 [N]) of one linear; NULL / NULL = off."""
+    _fields_ = [("scale", c_void_p), ("bias", c_void_p)]
+
+
 class Q4LinearArgs(C.Structure):
     _fields_ = [
         ("x", c_void_p), ("ldx", c_int),
@@ -29,7 +34,7 @@ class Q4LinearArgs(C.Structure):
         ("split_k", c_int), ("flags", c_int), ("trace", c_void_p), ("workspace", c_void_p),
         ("pf_ptr", c_void_p * 4), ("pf_bytes", C.c_ulonglong * 4),
         ("pf_kv", c_void_p * 2), ("pf_rows", c_void_p), ("pf_rows_max", c_int), ("pf_nseg", c_int), ("pf_row_bytes", c_int),
-        ("pf_seg_stride", C.c_ulonglong),
+        ("pf_seg_stride", C.c_ulonglong), ("out_affine", OutAffine),
     ]
 
 
@@ -63,6 +68,11 @@ class LoRA(C.Structure):
 LORA_MAX_R = 64   # B2L_LORA_MAX_R
 
 
+class LayerAffine(C.Structure):
+    """b2l_layer_affine: the LLaMA-Adapter v2 affines of a Block's linears (c_fc12 interleaved like its weight rows)."""
+    _fields_ = [("c_attn", OutAffine), ("c_proj", OutAffine), ("c_fc12", OutAffine), ("mlp_proj", OutAffine)]
+
+
 class DecodeArgs(C.Structure):
     _fields_ = [
         ("n_layer", c_int), ("n_head", c_int), ("n_embd", c_int), ("n_hidden", c_int), ("vocab", c_int),
@@ -74,6 +84,7 @@ class DecodeArgs(C.Structure):
         ("x", c_void_p), ("qkv", c_void_p), ("att", c_void_p), ("hid", c_void_p), ("attn_work", c_void_p),
         ("logits", c_void_p), ("flags", c_int), ("timeline", c_void_p), ("batch_work", c_void_p),
         ("plan", c_void_p), ("adapters", C.POINTER(AdapterPrefix)), ("loras", C.POINTER(LoRA)),
+        ("affines", C.POINTER(LayerAffine)), ("lm_head_affine", OutAffine),
     ]
 
 
@@ -111,6 +122,7 @@ _SIGS = {
     "b2l_embedding": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "b2l_silu_mul": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "b2l_add": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "b2l_linear_affine": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "b2l_topk_softmax": (c_int, [c_void_p, c_float, c_int, c_void_p, c_int, c_void_p]),
     "b2l_topk_softmax_sample": (c_int, [c_void_p, c_float, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "b2l_q8_tiled_bytes": (c_size_t, [c_int, c_int]),

@@ -123,8 +123,9 @@ static std::vector<PfWindow> prefetch_windows(const b2l_decode_args* d) {
 static int q4_call(const b2l_q4_weight& w, const void* x, int ldx, void* y, int ldy, int M, int sz_dtype, int prologue,
                    const void* norm_scale, float eps, int epilogue, const void* res, int ldres, int flags,
                    b2l_stream_t stream, void* trace = nullptr, void* batch_work = nullptr, const PfWindow* pf = nullptr,
-                   const b2l_decode_args* kv_of = nullptr, int kv_layer = 0) {
+                   const b2l_decode_args* kv_of = nullptr, int kv_layer = 0, const b2l_out_affine* aff = nullptr) {
   b2l_q4_linear_args a{};
+  if (aff != nullptr) a.out_affine = *aff;   // batch-1 kernels only (b2l_decode_step checks B == 1 and qw_mma)
   if (kv_of != nullptr) {   // this linear also asks the L2 for the KV-cache rows of layer `kv_layer`'s attention
     const int hs = kv_of->n_embd / kv_of->n_head;
     a.pf_kv[0] = kv_of->layers[kv_layer].k_cache; a.pf_kv[1] = kv_of->layers[kv_layer].v_cache;
@@ -204,6 +205,24 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
       if (int rc = check_lora(&d->loras[l], 3 * d->n_embd, d->n_embd, "b2l_decode_step")) return rc;
     }
   }
+  // LLaMA-Adapter v2: every linear's affine runs in its own batch-1 launch (b2l_q4_linear_args::out_affine)
+  const bool any_affine = d->affines != nullptr || d->lm_head_affine.scale != nullptr || d->lm_head_affine.bias != nullptr;
+  if (any_affine) {
+    B2L_CHECK_SUPPORTED(d->B == 1, "b2l_decode_step: LLaMA-Adapter v2 affines run at batch 1 only, got B=%d", d->B);
+    B2L_CHECK_SUPPORTED(d->plan == nullptr, "b2l_decode_step: LLaMA-Adapter v2 affines do not run in the persistent kernel (plan must be NULL)");
+    B2L_CHECK_SUPPORTED(d->loras == nullptr, "b2l_decode_step: LLaMA-Adapter v2 affines and LoRA do not combine");
+    auto ok = [](const b2l_out_affine& f) { return (f.scale == nullptr) == (f.bias == nullptr); };
+    B2L_CHECK_ARG(ok(d->lm_head_affine), "b2l_decode_step: lm_head_affine needs both scale and bias (or neither)");
+    B2L_CHECK_SUPPORTED(d->lm_head.qw_mma != nullptr, "b2l_decode_step: affines need the batch-1 tiling (qw_mma) of every weight");
+    for (int l = 0; d->affines != nullptr && l < d->n_layer; ++l) {
+      const b2l_layer_affine& f = d->affines[l];
+      B2L_CHECK_ARG(ok(f.c_attn) && ok(f.c_proj) && ok(f.c_fc12) && ok(f.mlp_proj),
+                    "b2l_decode_step: affines[%d] needs both scale and bias (or neither) per linear", l);
+      const b2l_layer& L = d->layers[l];
+      B2L_CHECK_SUPPORTED(L.c_attn.qw_mma && L.c_proj.qw_mma && L.c_fc12.qw_mma && L.mlp_proj.qw_mma,
+                          "b2l_decode_step: affines need the batch-1 tiling (qw_mma) of every weight");
+    }
+  }
   if (d->plan != nullptr) return decode_step_persistent(d, stream);   // one persistent kernel per token (decode_mega.cu)
   const int C = d->n_embd, hs = C / d->n_head, B = d->B;
   const int fl = d->flags;               // the linears' flags (q4_call routes B2L_F_W8 to b2l_w8_gemv)
@@ -226,8 +245,10 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
   if ((rc = b2l_embedding(d->idx, d->idx_is_i64, d->wte, d->x, B, C, d->vocab, stream))) return rc;
   for (int l = 0; l < d->n_layer; ++l) {
     const b2l_layer& L = d->layers[l];
+    const b2l_layer_affine* af = d->affines != nullptr ? &d->affines[l] : nullptr;
     if ((rc = q4_call(L.c_attn, d->x, C, d->qkv, 3 * C, B, d->sz_dtype, B2L_PRO_RMSNORM, L.rms_1, d->eps, B2L_EPI_STORE,
-                      nullptr, 0, fl, stream, tl(), d->batch_work, pf(), (kv_ok && kv_prefetch == 2) ? d : nullptr, l)))
+                      nullptr, 0, fl, stream, tl(), d->batch_work, pf(), (kv_ok && kv_prefetch == 2) ? d : nullptr, l,
+                      af ? &af->c_attn : nullptr)))
       return rc;
     // LoRA on c_attn (lora.py:308-326): the low-rank term from rms_1(x), added into qkv in place
     if (d->loras != nullptr && d->loras[l].r != 0 &&
@@ -245,18 +266,19 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
     }
     g_attn_timeline = nullptr;
     if ((rc = q4_call(L.c_proj, d->att, C, d->x, C, B, d->sz_dtype, B2L_PRO_NONE, nullptr, 0.f, B2L_EPI_RESIDUAL, d->x, C,
-                      fl, stream, tl(), d->batch_work, pf())))
+                      fl, stream, tl(), d->batch_work, pf(), nullptr, 0, af ? &af->c_proj : nullptr)))
       return rc;
     if ((rc = q4_call(L.c_fc12, d->x, C, d->hid, d->n_hidden, B, d->sz_dtype, B2L_PRO_RMSNORM, L.rms_2, d->eps,
-                      B2L_EPI_SWIGLU, nullptr, 0, fl, stream, tl(), d->batch_work, pf())))
+                      B2L_EPI_SWIGLU, nullptr, 0, fl, stream, tl(), d->batch_work, pf(), nullptr, 0, af ? &af->c_fc12 : nullptr)))
       return rc;
     // mlp.c_proj fits the weight ring entirely, so HBM idles while it converts its activations: it asks the L2 for
     // the NEXT Block's KV-cache rows (B2L_KV_PREFETCH=0 switches that off)
     const bool kvpf = kv_prefetch == 1 && kv_ok && l + 1 < d->n_layer;
     if ((rc = q4_call(L.mlp_proj, d->hid, d->n_hidden, d->x, C, B, d->sz_dtype, B2L_PRO_NONE, nullptr, 0.f,
-                      B2L_EPI_RESIDUAL, d->x, C, fl, stream, tl(), d->batch_work, pf(), kvpf ? d : nullptr, l + 1)))
+                      B2L_EPI_RESIDUAL, d->x, C, fl, stream, tl(), d->batch_work, pf(), kvpf ? d : nullptr, l + 1,
+                      af ? &af->mlp_proj : nullptr)))
       return rc;
   }
   return q4_call(d->lm_head, d->x, C, d->logits, d->vocab, B, d->sz_dtype, B2L_PRO_RMSNORM, d->ln_f, d->eps,
-                 B2L_EPI_STORE, nullptr, 0, fl, stream, tl(), d->batch_work, pf());
+                 B2L_EPI_STORE, nullptr, 0, fl, stream, tl(), d->batch_work, pf(), nullptr, 0, &d->lm_head_affine);
 }

@@ -843,6 +843,8 @@ extern "C" int b2l_decode_plan_build(const b2l_decode_args* d, b2l_stream_t stre
   if (d->loras != nullptr)
     for (int l = 0; l < d->n_layer; ++l)
       B2L_CHECK_SUPPORTED(d->loras[l].r == 0, "b2l_decode_plan_build: LoRA layers (loras[%d].r = %d) do not run in the persistent kernel", l, d->loras[l].r);
+  B2L_CHECK_SUPPORTED(d->affines == nullptr && d->lm_head_affine.scale == nullptr && d->lm_head_affine.bias == nullptr,
+                      "b2l_decode_plan_build: LLaMA-Adapter v2 affines do not run in the persistent kernel");
   B2L_CHECK_SUPPORTED(mega_shape_ok(d), "b2l_decode_plan_build: the persistent kernel needs batch 1, head_size 128, int8-tiled per-row int4 weights, K %% 64 == 0, K <= 12288");
   const int n_ops = plan_n_ops(d);
   std::vector<mega::Op> ops((size_t)n_ops);

@@ -1,5 +1,7 @@
 // model.py element-wise pieces as stand-alone kernels (module-level drop-ins, prefill).
 // In the decode step these are fused into the tensor-core linears' prologue/epilogue.
+#include <algorithm>
+
 #include "b2l_common.cuh"
 
 namespace b2l {
@@ -100,9 +102,57 @@ static int launch_binary(const void* a, const void* b, void* y, size_t n, cudaSt
   return 0;
 }
 
+// LLaMA-Adapter v2's affine of a linear's output, adapter_v2.py:30-33: y = bf16(s * bf16(y + b)) per column, in
+// place.  VEC: 8 columns (16 bytes) per thread, N, ldy multiples of 8 and 16-byte aligned pointers.
+__device__ __forceinline__ float affine1(float y, float s, float b) { return s * rbf(y + b); }
+template <bool VEC>
+__global__ void __launch_bounds__(256) linear_affine_kernel(__nv_bfloat16* y, int ldy, int M, int N,
+                                                            const __nv_bfloat16* __restrict__ scale,
+                                                            const __nv_bfloat16* __restrict__ bias) {
+  const int per = VEC ? 8 : 1;
+  const int cols = N / per;
+  const size_t total = (size_t)M * cols;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int m = (int)(i / cols), c = (int)(i - (size_t)m * cols) * per;
+    __nv_bfloat16* row = y + (size_t)m * ldy + c;
+    if (VEC) {
+      const uint4 yv = *reinterpret_cast<const uint4*>(row);
+      const uint4 sv = *reinterpret_cast<const uint4*>(scale + c), bv = *reinterpret_cast<const uint4*>(bias + c);
+      const uint32_t yw[4] = {yv.x, yv.y, yv.z, yv.w}, sw[4] = {sv.x, sv.y, sv.z, sv.w}, bw[4] = {bv.x, bv.y, bv.z, bv.w};
+      uint32_t o[4];
+#pragma unroll
+      for (int q = 0; q < 4; ++q)
+        o[q] = pack_bf16x2(affine1(__uint_as_float(yw[q] << 16), __uint_as_float(sw[q] << 16), __uint_as_float(bw[q] << 16)),
+                           affine1(__uint_as_float(yw[q] & 0xffff0000u), __uint_as_float(sw[q] & 0xffff0000u),
+                                   __uint_as_float(bw[q] & 0xffff0000u)));
+      *reinterpret_cast<uint4*>(row) = make_uint4(o[0], o[1], o[2], o[3]);
+    } else {
+      *row = f2bf(affine1(bf2f(*row), bf2f(scale[c]), bf2f(bias[c])));
+    }
+  }
+}
+
 }  // namespace b2l
 
 using namespace b2l;
+
+extern "C" int b2l_linear_affine(void* y, int ldy, int M, int N, const void* scale, const void* bias,
+                                 b2l_stream_t stream) {
+  B2L_CHECK_ARG(y && scale && bias, "b2l_linear_affine: null pointer");
+  B2L_CHECK_ARG(M >= 0 && N > 0 && ldy >= N, "b2l_linear_affine: bad shape (M=%d, N=%d, ldy=%d)", M, N, ldy);
+  B2L_CHECK_ARG((uintptr_t)y % 2 == 0 && (uintptr_t)scale % 2 == 0 && (uintptr_t)bias % 2 == 0,
+                "b2l_linear_affine: y / scale / bias must be 2-byte aligned bf16");
+  if (M == 0) return 0;
+  const bool vec = N % 8 == 0 && ldy % 8 == 0 && (((uintptr_t)y | (uintptr_t)scale | (uintptr_t)bias) & 15) == 0;
+  const size_t work = (size_t)M * (vec ? N / 8 : N);
+  const unsigned grid = (unsigned)std::min<size_t>((work + 255) / 256, (size_t)sm_count() * 16);
+  cudaStream_t st = (cudaStream_t)stream;
+  const __nv_bfloat16 *s = (const __nv_bfloat16*)scale, *b = (const __nv_bfloat16*)bias;
+  if (vec) linear_affine_kernel<true><<<grid, 256, 0, st>>>((__nv_bfloat16*)y, ldy, M, N, s, b);
+  else linear_affine_kernel<false><<<grid, 256, 0, st>>>((__nv_bfloat16*)y, ldy, M, N, s, b);
+  B2L_LAUNCH_CHECK("linear_affine_kernel");
+  return 0;
+}
 
 extern "C" int b2l_rmsnorm(const void* x, const void* scale, void* y, int rows, int C, float eps,
                            b2l_stream_t stream) {

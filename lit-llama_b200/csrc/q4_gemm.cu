@@ -310,6 +310,8 @@ int gemm_entry(const b2l_q4_linear_args* a, b2l_stream_t stream) {
   const char* fn = W8 ? "b2l_w8_gemm" : "b2l_q4_gemm";
   B2L_CHECK_ARG(a != nullptr, "%s: null args", fn);
   B2L_CHECK_ARG(a->x && a->qw_tiled && a->scales && a->zeros && a->y, "%s: null pointer", fn);
+  B2L_CHECK_SUPPORTED(a->out_affine.scale == nullptr && a->out_affine.bias == nullptr,
+                      "%s: out_affine is not supported (apply b2l_linear_affine to y)", fn);
   B2L_CHECK_ARG(a->M > 0 && a->N > 0 && a->K > 0, "%s: bad shape", fn);
   B2L_CHECK_SUPPORTED(a->K % BK == 0, "%s: K=%d must be a multiple of %d", fn, a->K, BK);
   B2L_CHECK_ARG(a->ldx >= a->K && a->ldx % 8 == 0 && a->ldy >= a->N, "%s: bad leading dimension (ldx %% 8 == 0)", fn);

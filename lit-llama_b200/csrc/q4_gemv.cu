@@ -65,6 +65,8 @@ struct Params {
   // strided form (KV-cache rows of a following attention launch; b2l_q4_linear_args::pf_kv)
   const uint8_t* pf_kv[2]; const long long* pf_rows; int pf_rows_max, pf_nseg, pf_row_bytes; unsigned long long pf_seg_stride;
   int evict_first;         // demand loads carry an L2 evict_first policy (a weight byte is read once per token)
+  // LLaMA-Adapter v2 affine (AFFINE instantiations only): bf16 [N] in weight row order
+  const __nv_bfloat16* aff_scale; const __nv_bfloat16* aff_bias;
 };
 
 constexpr uint32_t PF_CHUNK = 16384;   // bytes per bulk L2 prefetch instruction
@@ -146,7 +148,8 @@ __device__ __forceinline__ void kblock_imma(int (&acc)[MAX_HALVES][2][4], const 
 // MAXC = activation chunks (2048 elements each) a thread block caches in registers during the prologue:
 // 6 covers K <= 12288 (every 7B/13B/30B layer), 12 covers K <= 24576 (65B mlp.c_proj, K = 22016).
 // NDIG = base-256 digits of the scaled activations: 3 (|X| < 2^22).  W8: 8-bit weight levels (see WTile).
-template <int MAXC, int NDIG, bool W8>
+// AFFINE: LLaMA-Adapter v2's v = bf16(s * bf16(v + b)) per row before the epilogue (adapter_v2.py:30-33).
+template <int MAXC, int NDIG, bool W8, bool AFFINE>
 __global__ void __launch_bounds__(NTHREADS, 2) q4_gemv_kernel(const Params p) {
   constexpr int KB_BYTES = WTile<W8>::KB_BYTES, KBP_PER_STAGE = WTile<W8>::KBP;
   extern __shared__ __align__(128) uint8_t smem[];
@@ -482,6 +485,17 @@ __global__ void __launch_bounds__(NTHREADS, 2) q4_gemv_kernel(const Params p) {
         for (uint32_t o = lo + lane * step; o < hi; o += 32 * step) l2_prefetch_line(p.pf_ptr[sgi] + o);
       }
     }
+    // the affine vectors are weights: the first unit's are loaded before the wait, later units' ahead of their reduction
+    float aff_s = 1.f, aff_b = 0.f;
+    auto load_affine = [&](int u) {
+      const int orow = (rb_lo + 2 * u + (lane >> 4)) * RB + (lane & 15);
+      const int o = min(orow, p.N - 1);
+      aff_s = bf2f(p.aff_scale[o]);
+      aff_b = bf2f(p.aff_bias[o]);
+    };
+    if constexpr (AFFINE) {
+      if (n_units > 0) load_affine(0);
+    }
     pdl_wait();
     const int* red_sh = reinterpret_cast<const int*>(smem + L.red + 128);
     const int* scratch = reinterpret_cast<const int*>(smem + L.scratch);
@@ -510,6 +524,9 @@ __global__ void __launch_bounds__(NTHREADS, 2) q4_gemv_kernel(const Params p) {
       const int o = min(orow, p.N - 1);
       const float sc = load_sz(p.scales, p.szdt, o);
       const float zero = load_sz(p.zeros, p.szdt, o);
+      if constexpr (AFFINE) {
+        if (u > 0) load_affine(u);
+      }
       float resv = 0.f;
       if (p.epilogue == B2L_EPI_RESIDUAL && active && orow < p.N) resv = bf2f(p.res[orow]);
       named_bar_sync(6 + buf, NCW * 32 + 32);
@@ -523,7 +540,8 @@ __global__ void __launch_bounds__(NTHREADS, 2) q4_gemv_kernel(const Params p) {
       // sum_k level X = d0 + 256 d1 + 65536 d2 + 2^24 d3 (exact in int64, < 2^53)
       const long long tq = (long long)d0 + ((long long)d1 << 8) + ((long long)d2 << 16) + ((long long)d3 << 24);
       const float tf = (float)(((double)tq - (double)zero * dsum_x) * inv_scale);   // sum (level - zero) x, one rounding
-      const float v = rbf(sc * tf);
+      float v = rbf(sc * tf);
+      if constexpr (AFFINE) v = rbf(aff_s * rbf(v + aff_b));
       if (p.epilogue == B2L_EPI_SWIGLU) {
         // rows 0..7 of a 16-row block are c_fc1[o..o+7], rows 8..15 are c_fc2[o..o+7]
         const float b = __shfl_down_sync(0xffffffffu, v, 8);
@@ -674,8 +692,8 @@ extern "C" int b2l_w8_untile_i8(const void* qw_tiled, void* qw, int N, int K, b2
 namespace {
 constexpr int MAX_K = 12 * NCW * 32 * 8;   // 24576
 
-template <int MAXC, int NDIG, bool W8>
-int launch_gemv(const Params& p0, int ctas_per_sm, int grid_override, bool pdl, cudaStream_t stream) {
+template <int MAXC, int NDIG, bool W8, bool AFFINE>
+int launch_gemv_variant(const Params& p0, int ctas_per_sm, int grid_override, bool pdl, cudaStream_t stream) {
   Params p = p0;
   // ring: as deep as fits `ctas_per_sm` CTAs per SM
   // B2L_GEMV_SMEM_KB: shared-memory budget of a CTA (default: 110 KB for two CTAs per SM, 224 KB for one)
@@ -693,12 +711,18 @@ int launch_gemv(const Params& p0, int ctas_per_sm, int grid_override, bool pdl, 
   p.nst = nst;
   const SmemLayout L = smem_layout(nst, p.K, NDIG);
   static DynSmemCache smem_cache;
-  if (int rc = ensure_dyn_smem(q4_gemv_kernel<MAXC, NDIG, W8>, L.total, smem_cache)) return rc;
+  if (int rc = ensure_dyn_smem(q4_gemv_kernel<MAXC, NDIG, W8, AFFINE>, L.total, smem_cache)) return rc;
   int grid = grid_override > 0 ? grid_override : ctas_per_sm * sm_count();
   if (grid > p.n_rb) grid = p.n_rb;
   LaunchCfg lc(dim3(grid), dim3(NTHREADS), L.total, stream, pdl, 1);
-  B2L_CUDA(cudaLaunchKernelEx(&lc.cfg, q4_gemv_kernel<MAXC, NDIG, W8>, p));
+  B2L_CUDA(cudaLaunchKernelEx(&lc.cfg, q4_gemv_kernel<MAXC, NDIG, W8, AFFINE>, p));
   return 0;
+}
+
+template <int MAXC, int NDIG, bool W8>
+int launch_gemv(const Params& p, int ctas_per_sm, int grid_override, bool pdl, cudaStream_t stream) {
+  if (p.aff_scale != nullptr) return launch_gemv_variant<MAXC, NDIG, W8, true>(p, ctas_per_sm, grid_override, pdl, stream);
+  return launch_gemv_variant<MAXC, NDIG, W8, false>(p, ctas_per_sm, grid_override, pdl, stream);
 }
 
 // b2l_q4_gemv (W8 = false) and b2l_w8_gemv (W8 = true): the same checks, argument block and launch policy
@@ -721,8 +745,12 @@ int gemv_entry(const b2l_q4_linear_args* a, b2l_stream_t stream) {
   if (a->epilogue == B2L_EPI_RESIDUAL) B2L_CHECK_ARG(a->res != nullptr, "%s: RESIDUAL epilogue needs res", fn);
   else if (a->epilogue == B2L_EPI_SWIGLU) B2L_CHECK_SUPPORTED(a->N % RB == 0, "%s: SWIGLU needs N %% 16 == 0", fn);
   else B2L_CHECK_ARG(a->epilogue == B2L_EPI_STORE, "%s: bad epilogue %d", fn, a->epilogue);
+  B2L_CHECK_ARG((a->out_affine.scale == nullptr) == (a->out_affine.bias == nullptr),
+                "%s: out_affine needs both scale and bias (or neither)", fn);
 
   Params p;
+  p.aff_scale = (const __nv_bfloat16*)a->out_affine.scale;
+  p.aff_bias = (const __nv_bfloat16*)a->out_affine.bias;
   p.x = (const __nv_bfloat16*)a->x;
   p.qwt = (const uint8_t*)a->qw_tiled;
   p.scales = a->scales; p.zeros = a->zeros; p.szdt = a->sz_dtype;

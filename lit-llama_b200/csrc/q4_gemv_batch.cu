@@ -400,6 +400,8 @@ extern "C" size_t b2l_q4_gemv_batch_workspace_bytes(int K) {
 extern "C" int b2l_q4_gemv_batch(const b2l_q4_linear_args* a, b2l_stream_t stream) {
   B2L_CHECK_ARG(a != nullptr, "b2l_q4_gemv_batch: null args");
   B2L_CHECK_ARG(a->x && a->qw_tiled && a->scales && a->zeros && a->y && a->workspace, "b2l_q4_gemv_batch: null pointer");
+  B2L_CHECK_SUPPORTED(a->out_affine.scale == nullptr && a->out_affine.bias == nullptr,
+                      "b2l_q4_gemv_batch: out_affine is not supported (apply b2l_linear_affine to y)");
   B2L_CHECK_SUPPORTED(a->M >= 1 && a->M <= MAXB, "b2l_q4_gemv_batch: M=%d (1..%d activation rows)", a->M, MAXB);
   B2L_CHECK_SUPPORTED(a->K > 0 && a->K % KB == 0 && a->K <= 12 * 256 * 8, "b2l_q4_gemv_batch: K=%d must be a multiple of %d and <= %d", a->K, KB,
                       12 * 256 * 8);

@@ -560,6 +560,8 @@ int q4_pick_split(int n_tiles, int slabs_total) {
 extern "C" int b2l_q4_linear_tc(const b2l_q4_linear_args* a, b2l_stream_t stream) {
   B2L_CHECK_ARG(a != nullptr, "b2l_q4_linear_tc: null args");
   B2L_CHECK_ARG(a->x && a->qw_tiled && a->scales && a->zeros && a->y, "b2l_q4_linear_tc: null pointer");
+  B2L_CHECK_SUPPORTED(a->out_affine.scale == nullptr && a->out_affine.bias == nullptr,
+                      "b2l_q4_linear_tc: out_affine is not supported (apply b2l_linear_affine to y)");
   B2L_CHECK_SUPPORTED(a->M >= 1 && a->M <= MAX_M, "b2l_q4_linear_tc: M=%d outside 1..%d", a->M, MAX_M);
   B2L_CHECK_SUPPORTED(a->K > 0 && a->K % SLAB_K == 0, "b2l_q4_linear_tc: K=%d must be a multiple of %d", a->K, SLAB_K);
   B2L_CHECK_ARG(a->N > 0 && a->ldx >= a->K, "b2l_q4_linear_tc: bad N/ldx");

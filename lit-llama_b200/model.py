@@ -63,6 +63,19 @@ def _linear(module: nn.Module, x: torch.Tensor) -> torch.Tensor:
     return module(x)
 
 
+def affine_of(lin: nn.Module) -> Optional[Tuple[torch.Tensor, torch.Tensor]]:
+    """(adapter_scale, adapter_bias) of a LLaMA-Adapter v2 linear (lit_llama_b200.adapter_v2) as contiguous bf16
+    tensors (the parameters themselves when they already are), or None for a plain linear."""
+    if not hasattr(lin, "adapter_scale"):
+        return None
+
+    def bf16(p: torch.Tensor) -> torch.Tensor:
+        t = p.detach()
+        return (t if t.dtype == torch.bfloat16 else t.to(torch.bfloat16)).contiguous()
+
+    return bf16(lin.adapter_scale), bf16(lin.adapter_bias)
+
+
 class RMSNorm(nn.Module):
     """model.py:257-277; the kernel keeps the reference's bf16 rounding points."""
 
@@ -324,11 +337,16 @@ class _DecodeState:
         loras = model._loras(self.keep)
         if loras is not None:      # LoRA: the step adds each layer's low-rank term behind c_attn
             self.args.loras = C.cast(loras, C.POINTER(L.LoRA))
+        affines = model._affines(self.keep)
+        if affines is not None:    # LLaMA-Adapter v2 (B == 1): every linear's launch applies its scale and bias
+            self.args.affines = C.cast(affines[0], C.POINTER(L.LayerAffine))
+            self.args.lm_head_affine = affines[1]
         # batch 1, head_size 128: the whole step as ONE persistent kernel (csrc/decode_mega.cu; int4 weights only, so
-        # gptq.int8 keeps one kernel per op under B2L_PERSISTENT=1 too, and so do adapter and LoRA models)
+        # gptq.int8 keeps one kernel per op under B2L_PERSISTENT=1 too, and so do adapter, LoRA and adapter-v2 models)
         self.plan = None
         kmax = max(C_, n_hidden)
-        if model.persistent and not w8 and adapters is None and loras is None and B == 1 and hs == 128 and kmax <= 12288:
+        if (model.persistent and not w8 and adapters is None and loras is None and affines is None and B == 1 and hs == 128
+                and kmax <= 12288):
             self.plan = torch.zeros(lib.b2l_decode_plan_bytes(C.byref(self.args)), dtype=torch.uint8, device=device)
             self.args.plan = self.plan.data_ptr()
             L.check(lib.b2l_decode_plan_build(C.byref(self.args), L.stream_ptr()), "b2l_decode_plan_build")
@@ -404,6 +422,39 @@ class LLaMA(nn.Module):
                 keep.append(t[1])
         keep.append(arr)
         return arr
+
+    def _has_affines(self) -> bool:
+        return any(hasattr(m, "adapter_scale") for m in self.modules())
+
+    def _affines(self, keep: list):
+        """(HOST array [n_layer] of b2l_layer_affine, lm_head's b2l_out_affine) for b2l_decode_args::affines /
+        lm_head_affine, or None (no LLaMA-Adapter v2 linear); what they point at is appended to `keep`.  c_fc1 and
+        c_fc2's vectors are interleaved 8 / 8 like the batch-1 fc1|fc2 tiling (_fc12 "i8")."""
+        if not self._has_affines():
+            return None
+
+        def spec(t) -> L.OutAffine:
+            if t is None:
+                return L.OutAffine()
+            keep.extend(t)
+            return L.OutAffine(t[0].data_ptr(), t[1].data_ptr())
+
+        arr = (L.LayerAffine * len(self.transformer.h))()
+        for i, blk in enumerate(self.transformer.h):
+            mlp = blk.mlp
+            f1, f2 = affine_of(mlp.c_fc1), affine_of(mlp.c_fc2)
+            fc12 = None
+            if f1 is not None or f2 is not None:
+                nh = mlp.c_fc1.out_features
+                like = (f1 or f2)[0]
+                one, zero = torch.ones(nh, dtype=like.dtype, device=like.device), torch.zeros(nh, dtype=like.dtype, device=like.device)
+                f1, f2 = f1 or (one, zero), f2 or (one, zero)
+                fc12 = tuple(torch.stack((a.view(nh // 8, 8), b.view(nh // 8, 8)), dim=1).reshape(2 * nh)
+                             for a, b in zip(f1, f2))
+            arr[i] = L.LayerAffine(spec(affine_of(blk.attn.c_attn)), spec(affine_of(blk.attn.c_proj)), spec(fc12),
+                                   spec(affine_of(mlp.c_proj)))
+        keep.append(arr)
+        return arr, spec(affine_of(self.lm_head))
 
     def _init_weights(self, module: nn.Module) -> None:
         """model.py:70-74."""
@@ -608,7 +659,8 @@ class LLaMA(nn.Module):
             if st is None or st.B != B or st.S != max_seq_length or st.idx.dtype != idx.dtype or st.idx.device != idx.device:
                 if self._fast_ok is None:
                     self._fast_ok = self._fast_decode_ok()
-                fast = bool(self._fast_ok) and (self._fast_ok != "w8" or B == 1)   # gptq.int8: batch 1 only
+                # gptq.int8 and LLaMA-Adapter v2: batch 1 only
+                fast = bool(self._fast_ok) and (B == 1 or (self._fast_ok != "w8" and not self._has_affines()))
                 st = self._decode = _DecodeState(self, B, max_seq_length, idx.device, idx.dtype) if fast else None
         if st is not None:
             st.idx.copy_(idx.reshape(-1))

@@ -13,7 +13,10 @@ RMSNorm,apply_rope,build_rope_cache}`, `lit_llama.quantization.{ColBlockQuantize
 Linear8bitLt}`, `lit_llama.utils.{quantization,EmptyInitOnDevice,lazy_load}` and, when the
 package has it, `lit_llama.adapter.{LLaMA,LLaMAConfig,Block,CausalSelfAttention}` (LLaMA-Adapter,
 `generate/adapter.py`) and `lit_llama.lora.{lora,MergedLinear,LoRALayer,LoRAConfig,CausalSelfAttention,
-mark_only_lora_as_trainable,lora_state_dict}` (LoRA, `generate/lora.py`) all point at this package.
+mark_only_lora_as_trainable,lora_state_dict}` (LoRA, `generate/lora.py`) and `lit_llama.adapter_v2.{get_adapter_substrings,
+mark_only_adapter_v2_as_trainable,adapter_v2_state_from_state_dict,adapter_v2_new_forward,
+adapter_v2_linear_with_bias_and_scale,add_adapter_v2_parameters_to_linear_layers}` (LLaMA-Adapter v2,
+`generate/adapter_v2.py`) all point at this package.
 """
 import sys
 
@@ -84,6 +87,23 @@ def patch_reference(lit_llama_module=None):
                      "lora_state_dict"):
             saved[("lora", name)] = getattr(ref_lora, name, None)
             setattr(ref_lora, name, getattr(lo, name))
+    # LLaMA-Adapter v2 (lit_llama/adapter_v2.py), when the package has it
+    ref_v2 = sys.modules.get(lit_llama_module.__name__ + ".adapter_v2")
+    if ref_v2 is None:
+        import importlib
+
+        try:
+            ref_v2 = importlib.import_module(lit_llama_module.__name__ + ".adapter_v2")
+        except ImportError:
+            ref_v2 = None
+    if ref_v2 is not None:
+        from . import adapter_v2 as a2
+
+        for name in ("get_adapter_substrings", "mark_only_adapter_v2_as_trainable", "adapter_v2_state_from_state_dict",
+                     "adapter_v2_new_forward", "adapter_v2_linear_with_bias_and_scale",
+                     "add_adapter_v2_parameters_to_linear_layers"):
+            saved[("adapter_v2", name)] = getattr(ref_v2, name, None)
+            setattr(ref_v2, name, getattr(a2, name))
     for mod in list(sys.modules.values()):  # scripts that did `from lit_llama.utils import quantization`
         if mod is not None and getattr(mod, "quantization", None) is saved[("utils", "quantization")]:
             setattr(mod, "quantization", u.quantization)
@@ -97,4 +117,9 @@ def patch_reference(lit_llama_module=None):
         if ref_lora is not None and mod is not None and saved[("lora", "lora")] is not None \
                 and getattr(mod, "lora", None) is saved[("lora", "lora")]:
             setattr(mod, "lora", lo.lora)
+        # generate/adapter_v2.py did `from lit_llama.adapter_v2 import add_adapter_v2_parameters_to_linear_layers`
+        name = "add_adapter_v2_parameters_to_linear_layers"
+        if ref_v2 is not None and mod is not None and saved[("adapter_v2", name)] is not None \
+                and getattr(mod, name, None) is saved[("adapter_v2", name)]:
+            setattr(mod, name, getattr(a2, name))
     return saved

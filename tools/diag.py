@@ -15,7 +15,7 @@ import time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-SECTIONS = ["generic", "tile", "tc_small", "tc_shapes", "tc_modes", "gemv", "grid_flag", "hmma_rate", "imma_rate", "consumer_rate", "bench_gemm", "bench_tc", "trace", "bench_layers", "bench_gemv", "bench_step", "bench_ctx", "bench_13b_b8", "bench_sizes", "batch_debug", "bench_step_int8", "bench_q8_gemm", "bench_q8_gemv", "bench_w8_gemv", "bench_w8_gemm", "bench_step_w8", "bench_step_adapter", "bench_step_lora", "bench_lora_kernel", "lora_timeline", "timeline", "mega_timeline"]
+SECTIONS = ["generic", "tile", "tc_small", "tc_shapes", "tc_modes", "gemv", "grid_flag", "hmma_rate", "imma_rate", "consumer_rate", "bench_gemm", "bench_tc", "trace", "bench_layers", "bench_gemv", "bench_step", "bench_ctx", "bench_13b_b8", "bench_sizes", "batch_debug", "bench_step_int8", "bench_q8_gemm", "bench_q8_gemv", "bench_w8_gemv", "bench_w8_gemm", "bench_step_w8", "bench_step_adapter", "bench_step_adapter_v2", "bench_step_lora", "bench_lora_kernel", "lora_timeline", "timeline", "mega_timeline"]
 
 
 _DLIB = None
@@ -1293,6 +1293,84 @@ def sec_bench_step_adapter():
     print(f"7B gptq.int4 compacted, batch 1, ctx ~1966-1990, graph + PDL on {_card()}")
     print(f"  plain   : {' '.join(f'{x:.1f}' for x in res['plain'])} us/token (best {a:.1f})")
     print(f"  adapter : {' '.join(f'{x:.1f}' for x in res['adapter'])} us/token (best {b:.1f})  -> {100 * (b - a) / a:+.2f} %")
+
+
+def sec_bench_step_adapter_v2():
+    """LLaMA-Adapter v2 on the fused step: 7B gptq.int4 (synth_state) and 7B gptq.int8 (_random_w8_model) weights,
+    compacted, batch-1 decode at ctx ~2000 under the graph.  On the same base weights: the plain model, the v1-adapter
+    model (aT = 10, start layer 2, non-zero gates) and the v2 model (the same prefix plus a non-trivial scale and bias
+    on every linear), alternated in one process over 4 rounds.  The affine runs inside each linear's launch."""
+    import ctypes
+
+    import torch
+    import lit_llama_b200 as P
+    from lit_llama_b200 import adapter as PA
+    from lit_llama_b200 import adapter_v2 as PV
+    from lit_llama_b200.quantization import weights_changed
+    from lit_llama_b200.utils import quantization
+    from bench import build_synthetic_model, synth_state
+
+    dev = torch.device("cuda")
+    print(_card(), flush=True)
+    S = 2048
+    for mode in ("gptq.int4", "gptq.int8"):
+        if mode == "gptq.int4":
+            sd = synth_state("7B", 1234, dev)
+            plain = build_synthetic_model("7B", dev, state=sd)
+        else:
+            plain = _random_w8_model("7B", dev, seed=8)
+            sd = {k: v.clone() for k, v in plain.state_dict().items()}
+
+        def adapter_model(v2):
+            prev = torch.get_default_dtype()
+            torch.set_default_dtype(torch.bfloat16)
+            try:
+                with torch.device(dev), quantization(mode):
+                    m = PA.LLaMA.from_name("7B")
+                    if v2:
+                        PV.add_adapter_v2_parameters_to_linear_layers(m)
+            finally:
+                torch.set_default_dtype(prev)
+            g = torch.Generator(device=dev).manual_seed(7)
+            with torch.no_grad():
+                own = m.state_dict()
+                for k, v in sd.items():
+                    own[k].copy_(v)
+                for blk in m.transformer.h[m.config.adapter_start_layer:]:
+                    blk.attn.adapter_wte.weight.copy_(torch.randn(blk.attn.adapter_wte.weight.shape, generator=g, device=dev))
+                    blk.attn.gating_factor.copy_(torch.rand(blk.attn.gating_factor.shape, generator=g, device=dev) + 0.5)
+                for lin in m.modules():
+                    if hasattr(lin, "adapter_scale"):
+                        lin.adapter_scale.copy_(torch.rand(lin.adapter_scale.shape, generator=g, device=dev) * 0.2 + 0.9)
+                        lin.adapter_bias.copy_(torch.randn(lin.adapter_bias.shape, generator=g, device=dev) * 0.01)
+            weights_changed()
+            return m.eval().compact()
+
+        models = {"plain": plain.compact(), "v1": adapter_model(False), "v2": adapter_model(True)}
+        del sd
+        torch.cuda.empty_cache()
+        for m in models.values():
+            m.copy_logits = False
+            with torch.no_grad():
+                m(torch.randint(0, 32000, (1, 16), device=dev, dtype=torch.int32), S, torch.arange(16, device=dev))
+        lib = P._lib.lib()
+        res = {k: [] for k in models}
+        for r in range(4):
+            for name, m in models.items():
+                res[name].append(_decode_us(m, 1, S, dev, p0=1960, n=24))
+                if r == 0:
+                    n = lib.b2l_decode_step_launches(ctypes.byref(m._decode.args))
+                    print(f"{mode} {name}: fused step {m._decode is not None}, graph {m._decode.graph is not None}, {n} launches",
+                          flush=True)
+        best = {k: min(v) for k, v in res.items()}
+        print(f"7B {mode} compacted, batch 1, ctx ~1966-1990, graph + PDL on {_card()}")
+        for name in models:
+            print(f"  {name:5s}: {' '.join(f'{x:.1f}' for x in res[name])} us/token (best {best[name]:.1f}, "
+                  f"{100 * (best[name] - best['plain']) / best['plain']:+.2f} % vs plain, "
+                  f"{100 * (best[name] - best['v1']) / best['v1']:+.2f} % vs v1)", flush=True)
+        del models, plain
+        gc.collect()
+        torch.cuda.empty_cache()
 
 
 def _lora_7b(dev):
