@@ -194,6 +194,36 @@ int b2l_w8_gemv(const b2l_q4_linear_args* args, b2l_stream_t stream);
  * NONE / STORE), flags must be 0. */
 int b2l_w8_gemm(const b2l_q4_linear_args* args, b2l_stream_t stream);
 
+/* ------------------------------------------------------------------------------
+ * Perplexity (evaluate/full.py:120-129 and its lora / adapter / adapter_v2 twins): the next-token NLL of one
+ * window, cross_entropy(logits[:-1], inp[1:]), from the bf16 logits L of M = T - 1 rows and N columns:
+ *   nll[m] = logsumexp_n(float(L[m, n])) - float(L[m, targets[m]])      (fp32, maximum-subtracted expf)
+ *   *nll_sum = sum_m nll[m]                                             (fp64, fixed order)
+ * Rows are reduced per 128-column tile to (max, sum of exp) in a fixed order and the tiles merged in ascending
+ * order (csrc/nll.cu).  A target < 0 or >= N gives NaN for that row (and the sum).
+ *   targets    int32 (targets_i64 == 0) or int64 [M], device
+ *   nll        fp32 [M], device; nll_sum: one fp64, device (written, not accumulated)
+ *   workspace  b2l_nll_workspace_bytes(M, N) bytes of device scratch, 16-byte aligned
+ * Every call only enqueues work.
+ * ---------------------------------------------------------------------------- */
+typedef struct b2l_nll_args {
+  const void* targets;
+  int targets_i64;
+  float* nll;
+  double* nll_sum;
+  void* workspace;
+} b2l_nll_args;
+size_t b2l_nll_workspace_bytes(int M, int N);
+/* b2l_q4_gemm / b2l_w8_gemm with the loss in the epilogue: the fp32 accumulators are rounded to bf16 exactly as the
+ * STORE epilogue would write them and reduced per tile; nothing is stored to y (y / ldy are ignored).  Same
+ * requirements as b2l_q4_gemm / b2l_w8_gemm.  The result is bit-identical to b2l_logits_nll on the logits the plain
+ * GEMM writes. */
+int b2l_q4_gemm_nll(const b2l_q4_linear_args* args, const b2l_nll_args* nll, b2l_stream_t stream);
+int b2l_w8_gemm_nll(const b2l_q4_linear_args* args, const b2l_nll_args* nll, b2l_stream_t stream);
+/* The same from a bf16 logits matrix [M, N] with leading dimension ldl >= N (any N, M >= 0): for lm_heads the
+ * fused form does not cover (dense, llm.int8, gptq.int4 at M <= 16, LLaMA-Adapter v2's affine). */
+int b2l_logits_nll(const void* logits, int ldl, int M, int N, const b2l_nll_args* nll, b2l_stream_t stream);
+
 /* The same fused linear for 1..8 activation rows (batched decode) on mma.sync.m16n8k16 (f16), weight tiling
  * b2l_q4_tile_mma ([N/16 row blocks][K/64 k blocks][32 lanes][16 B] in m16n8k16 A-fragment order), argument block of
  * b2l_q4_gemv plus `workspace`; x [M, K] with leading dimension ldx (ldx % 8 == 0), y / res

@@ -13,8 +13,10 @@ from .utils import find_multiple, llama_model_lookup
 from .generate import generate, sample_probs, sample_token
 from .patch import patch_reference
 from .tp import TPLLaMA, shard_state_dict
+from . import evaluate
 
 __all__ = [
     "LLaMA", "LLaMAConfig", "Block", "CausalSelfAttention", "MLP", "RMSNorm", "build_rope_cache", "apply_rope",
     "ColBlockQuantizedLinear", "Linear8bitLt", "find_multiple", "llama_model_lookup", "generate", "sample_probs", "sample_token", "patch_reference", "TPLLaMA", "shard_state_dict",
+    "evaluate",
 ]

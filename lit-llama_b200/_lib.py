@@ -88,6 +88,13 @@ class DecodeArgs(C.Structure):
     ]
 
 
+class NLLArgs(C.Structure):
+    """b2l_nll_args: a window's next-token targets (int32 / int64 [M]), the per-token NLL (fp32 [M]), the window sum
+    (one fp64) and b2l_nll_workspace_bytes(M, N) bytes of scratch, all on the device."""
+    _fields_ = [("targets", c_void_p), ("targets_i64", c_int), ("nll", c_void_p), ("nll_sum", c_void_p),
+                ("workspace", c_void_p)]
+
+
 class TPComm(C.Structure):
     _fields_ = [("peer_buf", c_void_p * 8), ("rank", c_int), ("world", c_int), ("max_elems", c_int), ("epoch", c_void_p), ("status", c_void_p)]
 
@@ -116,6 +123,10 @@ _SIGS = {
     "b2l_w8_untile_i8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "b2l_w8_gemv": (c_int, [C.POINTER(Q4LinearArgs), c_void_p]),
     "b2l_w8_gemm": (c_int, [C.POINTER(Q4LinearArgs), c_void_p]),
+    "b2l_nll_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "b2l_q4_gemm_nll": (c_int, [C.POINTER(Q4LinearArgs), C.POINTER(NLLArgs), c_void_p]),
+    "b2l_w8_gemm_nll": (c_int, [C.POINTER(Q4LinearArgs), C.POINTER(NLLArgs), c_void_p]),
+    "b2l_logits_nll": (c_int, [c_void_p, c_int, c_int, c_int, C.POINTER(NLLArgs), c_void_p]),
     "b2l_q4_gemv_batch": (c_int, [C.POINTER(Q4LinearArgs), c_void_p]),
     "b2l_q4_gemv_batch_workspace_bytes": (c_size_t, [c_int]),
     "b2l_rmsnorm": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),

@@ -23,9 +23,13 @@
 //       * 16-byte st.shared of 8 consecutive k of a row = one row of a core matrix; fence.proxy.async; mbarrier arrive;
 //   epilogue: each MMA thread converts its accumulator fragment to bf16 and stores pairs of output features.
 // gptq.int8 (b2l_w8_gemm) is the same kernel with W8 = true: only the producers differ (w8_load below).
+// NLL = true (b2l_q4_gemm_nll / b2l_w8_gemm_nll) replaces the epilogue's store: the quad of lanes holding a token row
+// reduces the bf16-rounded accumulators of the tile's 128 columns to (max, sum of exp) into a workspace, and the lane
+// holding the row's target column records its logit (nll_common.cuh; csrc/nll.cu merges the tiles).
 #include <cuda.h>   // CUtensorMap and its enums only: the encoder is fetched with cudaGetDriverEntryPoint (no libcuda link)
 
 #include "b2l_common.cuh"
+#include "nll_common.cuh"
 
 namespace b2l {
 namespace q4gm {
@@ -50,6 +54,8 @@ struct Params {
   const void* scales; const void* zeros; int szdt;
   __nv_bfloat16* y; int ldy;
   int M, N, K;
+  const void* targets; int tgt_i64;   // NLL only: targets [M], partials [N/128][M], target logits [M]
+  float2* part; float* tl;
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -134,7 +140,7 @@ __device__ __forceinline__ void w8_load(uint32_t (&wq)[16], const uint8_t* qw, i
   }
 }
 
-template <bool W8>
+template <bool W8, bool NLL>
 __global__ void __launch_bounds__(NTHREADS, 1) q4_gemm_kernel(const __grid_constant__ Params p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   const uint32_t sbase = smem_u32(smem);
@@ -179,20 +185,34 @@ __global__ void __launch_bounds__(NTHREADS, 1) q4_gemm_kernel(const __grid_const
     // (+ 8 for e >= 2), output feature 8 c + 2 (lane % 4) + (e & 1)
     const int mr = m0 + h * 64 + (warp & 3) * 16 + (lane >> 2);
     const int nc = n0 + 2 * (lane & 3);
+    if constexpr (NLL) {
 #pragma unroll
-    for (int hh = 0; hh < 2; ++hh) {
-      const int m = mr + 8 * hh;
-      if (m >= p.M) continue;
-      __nv_bfloat16* dst = p.y + (size_t)m * p.ldy;
+      for (int hh = 0; hh < 2; ++hh) {
+        float v[32];
 #pragma unroll
-      for (int c = 0; c < BN / 8; ++c) {
-        const int n = nc + 8 * c;
-        const float v0 = acc[4 * c + 2 * hh], v1 = acc[4 * c + 2 * hh + 1];
-        if (n + 1 < p.N && ((reinterpret_cast<uintptr_t>(dst + n) & 3) == 0)) {
-          *reinterpret_cast<__nv_bfloat162*>(dst + n) = __floats2bfloat162_rn(v0, v1);
-        } else {
-          if (n < p.N) dst[n] = f2bf(v0);
-          if (n + 1 < p.N) dst[n + 1] = f2bf(v1);
+        for (int c = 0; c < BN / 8; ++c) {   // bf16(acc) as the store below would write it; -inf past N
+          const int n = nc + 8 * c;
+          v[2 * c] = n < p.N ? rbf(acc[4 * c + 2 * hh]) : -INFINITY;
+          v[2 * c + 1] = n + 1 < p.N ? rbf(acc[4 * c + 2 * hh + 1]) : -INFINITY;
+        }
+        nll::tile_row(v, mr + 8 * hh, p.M, blockIdx.x, nc, p.N, p.targets, p.tgt_i64, p.part, p.tl);
+      }
+    } else {
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int m = mr + 8 * hh;
+        if (m >= p.M) continue;
+        __nv_bfloat16* dst = p.y + (size_t)m * p.ldy;
+#pragma unroll
+        for (int c = 0; c < BN / 8; ++c) {
+          const int n = nc + 8 * c;
+          const float v0 = acc[4 * c + 2 * hh], v1 = acc[4 * c + 2 * hh + 1];
+          if (n + 1 < p.N && ((reinterpret_cast<uintptr_t>(dst + n) & 3) == 0)) {
+            *reinterpret_cast<__nv_bfloat162*>(dst + n) = __floats2bfloat162_rn(v0, v1);
+          } else {
+            if (n < p.N) dst[n] = f2bf(v0);
+            if (n + 1 < p.N) dst[n + 1] = f2bf(v1);
+          }
         }
       }
     }
@@ -304,21 +324,26 @@ using namespace b2l;
 using namespace b2l::q4gm;
 
 namespace {
-// b2l_q4_gemm (W8 = false: qw_tiled from b2l_q4_tile) and b2l_w8_gemm (W8 = true: quant_weight, uint8 [K][N])
+// b2l_q4_gemm (W8 = false: qw_tiled from b2l_q4_tile) and b2l_w8_gemm (W8 = true: quant_weight, uint8 [K][N]);
+// with `nl` (b2l_*_gemm_nll) the NLL epilogue instead of the store, then the combine kernel
 template <bool W8>
-int gemm_entry(const b2l_q4_linear_args* a, b2l_stream_t stream) {
-  const char* fn = W8 ? "b2l_w8_gemm" : "b2l_q4_gemm";
+int gemm_entry(const b2l_q4_linear_args* a, const b2l_nll_args* nl, b2l_stream_t stream) {
+  const bool with_nll = nl != nullptr;
+  const char* fn = with_nll ? (W8 ? "b2l_w8_gemm_nll" : "b2l_q4_gemm_nll") : (W8 ? "b2l_w8_gemm" : "b2l_q4_gemm");
   B2L_CHECK_ARG(a != nullptr, "%s: null args", fn);
-  B2L_CHECK_ARG(a->x && a->qw_tiled && a->scales && a->zeros && a->y, "%s: null pointer", fn);
+  B2L_CHECK_ARG(a->x && a->qw_tiled && a->scales && a->zeros && (a->y || with_nll), "%s: null pointer", fn);
   B2L_CHECK_SUPPORTED(a->out_affine.scale == nullptr && a->out_affine.bias == nullptr,
                       "%s: out_affine is not supported (apply b2l_linear_affine to y)", fn);
   B2L_CHECK_ARG(a->M > 0 && a->N > 0 && a->K > 0, "%s: bad shape", fn);
   B2L_CHECK_SUPPORTED(a->K % BK == 0, "%s: K=%d must be a multiple of %d", fn, a->K, BK);
-  B2L_CHECK_ARG(a->ldx >= a->K && a->ldx % 8 == 0 && a->ldy >= a->N, "%s: bad leading dimension (ldx %% 8 == 0)", fn);
+  B2L_CHECK_ARG(a->ldx >= a->K && a->ldx % 8 == 0 && (a->ldy >= a->N || with_nll), "%s: bad leading dimension (ldx %% 8 == 0)", fn);
   B2L_CHECK_ARG(((uintptr_t)a->x % 16 == 0) && ((uintptr_t)a->qw_tiled % 16 == 0), "%s: x / qw_tiled must be 16-byte aligned", fn);
   B2L_CHECK_ARG(a->sz_dtype == B2L_BF16 || a->sz_dtype == B2L_F32, "%s: bad sz_dtype", fn);
   if (W8) B2L_CHECK_SUPPORTED(a->flags == 0, "%s: unknown flags 0x%x", fn, a->flags);
   B2L_CHECK_SUPPORTED(a->prologue == B2L_PRO_NONE && a->epilogue == B2L_EPI_STORE, "%s: plain linear only (no fused prologue / epilogue)", fn);
+  if (with_nll) {
+    if (int rc = nll::check_args(nl, a->M, fn)) return rc;
+  }
   // cuTensorMapEncodeTiled through the runtime (resolved once)
   typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                                const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -351,15 +376,36 @@ int gemm_entry(const b2l_q4_linear_args* a, b2l_stream_t stream) {
   p.scales = a->scales; p.zeros = a->zeros; p.szdt = a->sz_dtype;
   p.y = (__nv_bfloat16*)a->y; p.ldy = a->ldy;
   p.M = a->M; p.N = a->N; p.K = a->K;
-  static DynSmemCache smem_cache;
-  if (int rc = ensure_dyn_smem(q4_gemm_kernel<W8>, SMEM_BYTES, smem_cache)) return rc;
+  p.targets = nullptr; p.tgt_i64 = 0; p.part = nullptr; p.tl = nullptr;
   dim3 grid((a->N + BN - 1) / BN, (a->M + BM - 1) / BM);
-  q4_gemm_kernel<W8><<<grid, NTHREADS, SMEM_BYTES, (cudaStream_t)stream>>>(p);
-  B2L_LAUNCH_CHECK("q4_gemm_kernel");
-  return 0;
+  if (!with_nll) {
+    static DynSmemCache smem_cache;
+    if (int rc = ensure_dyn_smem(q4_gemm_kernel<W8, false>, SMEM_BYTES, smem_cache)) return rc;
+    q4_gemm_kernel<W8, false><<<grid, NTHREADS, SMEM_BYTES, (cudaStream_t)stream>>>(p);
+    B2L_LAUNCH_CHECK("q4_gemm_kernel");
+    return 0;
+  }
+  uint8_t* ws = (uint8_t*)nl->workspace;
+  p.targets = nl->targets; p.tgt_i64 = nl->targets_i64;
+  p.part = (float2*)ws; p.tl = (float*)(ws + nll::part_bytes(a->M, a->N));
+  static DynSmemCache smem_cache_nll;
+  if (int rc = ensure_dyn_smem(q4_gemm_kernel<W8, true>, SMEM_BYTES, smem_cache_nll)) return rc;
+  q4_gemm_kernel<W8, true><<<grid, NTHREADS, SMEM_BYTES, (cudaStream_t)stream>>>(p);
+  B2L_LAUNCH_CHECK("q4_gemm_kernel (nll)");
+  return nll::launch_combine(nl->targets, nl->targets_i64, a->M, a->N, nl->workspace, nl->nll, nl->nll_sum, (cudaStream_t)stream);
 }
 }  // namespace
 
-extern "C" int b2l_q4_gemm(const b2l_q4_linear_args* a, b2l_stream_t stream) { return gemm_entry<false>(a, stream); }
+extern "C" int b2l_q4_gemm(const b2l_q4_linear_args* a, b2l_stream_t stream) { return gemm_entry<false>(a, nullptr, stream); }
 
-extern "C" int b2l_w8_gemm(const b2l_q4_linear_args* a, b2l_stream_t stream) { return gemm_entry<true>(a, stream); }
+extern "C" int b2l_w8_gemm(const b2l_q4_linear_args* a, b2l_stream_t stream) { return gemm_entry<true>(a, nullptr, stream); }
+
+extern "C" int b2l_q4_gemm_nll(const b2l_q4_linear_args* a, const b2l_nll_args* nl, b2l_stream_t stream) {
+  B2L_CHECK_ARG(nl != nullptr, "b2l_q4_gemm_nll: null nll args");
+  return gemm_entry<false>(a, nl, stream);
+}
+
+extern "C" int b2l_w8_gemm_nll(const b2l_q4_linear_args* a, const b2l_nll_args* nl, b2l_stream_t stream) {
+  B2L_CHECK_ARG(nl != nullptr, "b2l_w8_gemm_nll: null nll args");
+  return gemm_entry<true>(a, nl, stream);
+}

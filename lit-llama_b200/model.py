@@ -618,22 +618,7 @@ class LLaMA(nn.Module):
         self, idx: torch.Tensor, max_seq_length: Optional[int] = None, input_pos: Optional[torch.Tensor] = None
     ) -> Union[torch.Tensor, Tuple[torch.Tensor, List[KVCache]]]:
         B, T = idx.size()
-        if not idx.is_cuda:
-            raise RuntimeError(f"LLaMA.forward: idx is on {idx.device}; lit_llama_b200 runs on CUDA only (no CPU fallback)")
-
-        block_size = self.config.block_size
-        if max_seq_length is None:
-            max_seq_length = block_size
-        assert T <= max_seq_length, f"Cannot forward sequence of length {T}, max seq length is only {max_seq_length}"
-        assert max_seq_length <= block_size, f"Cannot attend to {max_seq_length}, block size is only {block_size}"
-        assert T <= block_size, f"Cannot forward sequence of length {T}, block size is only {block_size}"
-
-        if self.rope_cache is None or self.rope_cache.device != idx.device:
-            self.rope_cache = self.build_rope_cache(idx).float().contiguous()
-        if self._ring is None or self._ring.device != idx.device:
-            self._ring = torch.zeros(1, dtype=torch.int32, device=idx.device)
-            for blk in self.transformer.h:
-                blk.attn._ring, blk.attn._ring_shared = self._ring, True
+        max_seq_length = self._prepare(idx, max_seq_length)
 
         if input_pos is not None and not self.kv_caches:
             cfg = self.config
@@ -701,8 +686,34 @@ class LLaMA(nn.Module):
                 return mg["out"].clone() if self.copy_logits else mg["out"]
         return self._forward_modules(idx, max_seq_length, input_pos)
 
+    def _prepare(self, idx: torch.Tensor, max_seq_length: Optional[int]) -> int:
+        """model.py:79-91: the shape checks, and the RoPE table and KV ring on idx's device.  Returns max_seq_length."""
+        B, T = idx.size()
+        if not idx.is_cuda:
+            raise RuntimeError(f"LLaMA.forward: idx is on {idx.device}; lit_llama_b200 runs on CUDA only (no CPU fallback)")
+
+        block_size = self.config.block_size
+        if max_seq_length is None:
+            max_seq_length = block_size
+        assert T <= max_seq_length, f"Cannot forward sequence of length {T}, max seq length is only {max_seq_length}"
+        assert max_seq_length <= block_size, f"Cannot attend to {max_seq_length}, block size is only {block_size}"
+        assert T <= block_size, f"Cannot forward sequence of length {T}, block size is only {block_size}"
+
+        if self.rope_cache is None or self.rope_cache.device != idx.device:
+            self.rope_cache = self.build_rope_cache(idx).float().contiguous()
+        if self._ring is None or self._ring.device != idx.device:
+            self._ring = torch.zeros(1, dtype=torch.int32, device=idx.device)
+            for blk in self.transformer.h:
+                blk.attn._ring, blk.attn._ring_shared = self._ring, True
+        return max_seq_length
+
     def _forward_modules(self, idx: torch.Tensor, max_seq_length: int, input_pos: Optional[torch.Tensor]) -> torch.Tensor:
         """Prefill, no-cache forward and non-fused decode: one kernel (or two) per reference module."""
+        return self.lm_head(self._forward_hidden(idx, max_seq_length, input_pos))  # (b, t, vocab_size)
+
+    def _forward_hidden(self, idx: torch.Tensor, max_seq_length: int, input_pos: Optional[torch.Tensor]) -> torch.Tensor:
+        """_forward_modules up to lm_head's input: the embedding, the Blocks and ln_f (lit_llama_b200.evaluate runs
+        lm_head with the loss in its epilogue instead)."""
         B, T = idx.size()
         x = torch.empty((B, T, self.config.n_embd), device=idx.device, dtype=torch.bfloat16)
         wte = self.transformer.wte.weight
@@ -724,6 +735,4 @@ class LLaMA(nn.Module):
             for i, block in enumerate(self.transformer.h):
                 x, self.kv_caches[i] = block(x, self.rope_cache, None, max_seq_length, pos, self.kv_caches[i], _rope_is_table=True)
 
-        x = self.transformer.ln_f(x)
-        logits = self.lm_head(x)  # (b, t, vocab_size)
-        return logits
+        return self.transformer.ln_f(x)
