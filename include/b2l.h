@@ -145,8 +145,10 @@ enum {
                            input_pos (the reference's call convention, model.py:93)    */
   B2L_F_ATTN_UNFUSED = 8, /* debug: force the three-kernel attention path for T == 1   */
   B2L_F_DEBUG_NOCOMPUTE = 16, /* debug: b2l_q4_gemv streams the weights but skips the math */
-  B2L_F_W8 = 32         /* b2l_decode_step: every linear is gptq.int8, qw_mma from b2l_w8_tile_i8
+  B2L_F_W8 = 32,        /* b2l_decode_step: every linear is gptq.int8, qw_mma from b2l_w8_tile_i8
                            (b2l_w8_gemv); B == 1 and no plan only                     */
+  B2L_F_Q8 = 64         /* b2l_decode_step: every linear is llm.int8 (b2l_decode_args::q8_layers / q8_lm_head,
+                           b2l_q8_linear); B == 1, no plan, not with B2L_F_W8          */
 };
 
 /* Fused [RMSNorm ->] int4 linear [-> residual | SwiGLU] on wgmma (M <= 16).  Replaces
@@ -285,6 +287,38 @@ int b2l_q8_gemv_cb(const void* x, const void* cb, const void* scb, const void* o
                    void* y, int N, int K, float threshold, int flags, b2l_stream_t stream);
 int b2l_q8_outlier_mask(const void* x, int ldx, int M, int K, float threshold, void* mask,
                         b2l_stream_t stream);
+/* The batch-1 linear above fused with its neighbours of Block.forward, for the whole-token step (B2L_F_Q8):
+ *   x^ = RMSNorm(x) (prologue RMSNORM, b2l_rmsnorm's rounding points and order; NONE: x^ = x)
+ *   y  = Linear8bitLt.forward(x^) exactly as b2l_q8_gemv_cb computes it (outliers, SCA and CA from x^)
+ *   then out_affine (LLaMA-Adapter v2, as b2l_linear_affine), then the epilogue:
+ *     STORE     out = y                     (bf16 [N])
+ *     RESIDUAL  out = bf16(y + res)         (as b2l_add; res may alias out)
+ *     SWIGLU    out = silu(y1) * y2         (as b2l_silu_mul on the bf16 outputs y1 of cb / scb and y2 of cb2 /
+ *               scb2, both [N, K]: each 16-row block streams 8 rows of each, so no interleaved copy exists)
+ * Every output is bit-identical to the module sequence b2l_rmsnorm -> b2l_q8_gemv_cb [-> b2l_linear_affine]
+ * [-> b2l_add | second b2l_q8_gemv_cb + b2l_silu_mul].  For SWIGLU, out_affine's vectors hold 16 entries per 8
+ * outputs: 8 of c_fc1 | 8 of c_fc2 (the layout of b2l_layer_affine::c_fc12).  K a multiple of 128 up to 32768, any
+ * N > 0; x, cb, cb2 and norm_scale 16-byte aligned; out must not overlap x.  flags 0 or B2L_F_PDL: the weight ring
+ * fills and norm_scale, SCB and the affine are read before griddepcontrol.wait, x and res after it.  Bad arguments
+ * are rejected before the device is touched. */
+typedef struct b2l_q8_linear_args {
+  const void* x;            /* bf16 [K]                                                   */
+  const void* cb;           /* int8 [N, K] row-major (weight.CB)                          */
+  const void* scb;          /* fp32 [N]   (weight.SCB)                                    */
+  const void* cb2;          /* SWIGLU only: the second linear's CB / SCB                  */
+  const void* scb2;
+  void* y;                  /* bf16 [N]                                                   */
+  int N, K;
+  float threshold;          /* outlier threshold (Linear8bitLt.threshold)                 */
+  int prologue;             /* B2L_PRO_NONE / B2L_PRO_RMSNORM                             */
+  const void* norm_scale;   /* bf16 [K] when prologue == RMSNORM                          */
+  float eps;
+  int epilogue;             /* B2L_EPI_STORE / RESIDUAL / SWIGLU                          */
+  const void* res;          /* bf16 [N] for RESIDUAL                                      */
+  b2l_out_affine out_affine;
+  int flags;                /* 0 or B2L_F_PDL                                             */
+} b2l_q8_linear_args;
+int b2l_q8_linear(const b2l_q8_linear_args* args, b2l_stream_t stream);
 /* y[M, N] (bf16, leading dimension ldy) for M activation rows x[M, K] (bf16, leading dimension
  * ldx, a multiple of 8) on the int8 wgmma tensor cores: every row bit-identical to b2l_q8_gemv
  * on that row with the batch's outlier mask (b2l_q8_outlier_mask over all M rows).  cb is CB
@@ -463,6 +497,17 @@ typedef struct b2l_layer_affine {
   b2l_out_affine c_attn, c_proj, c_fc12, mlp_proj;
 } b2l_layer_affine;
 
+/* llm.int8 weights of the step (B2L_F_Q8): Linear8bitLt's weight.CB (int8 [N, K] row-major) and weight.SCB (fp32 [N])
+ * themselves, read in place. */
+typedef struct b2l_q8_weight {
+  const void* cb;
+  const void* scb;
+  int N, K;
+} b2l_q8_weight;
+typedef struct b2l_q8_layer {
+  b2l_q8_weight c_attn, c_proj, c_fc1, c_fc2, mlp_proj;
+} b2l_q8_layer;
+
 typedef struct b2l_decode_args {
   int n_layer, n_head, n_embd, n_hidden, vocab; /* vocab = padded_vocab_size          */
   int B, S;                                     /* batch, max_seq_length              */
@@ -507,6 +552,13 @@ typedef struct b2l_decode_args {
                                 NULL = none.  Only at B == 1 on the batch-1 kernels (every weight needs qw_mma);
                                 not with `plan` or `loras`.                               */
   b2l_out_affine lm_head_affine; /* the same for lm_head (both NULL = none)                 */
+  const b2l_q8_layer* q8_layers; /* B2L_F_Q8: HOST array [n_layer] of llm.int8 weights; the b2l_q4_weight members of
+                                layers[] and lm_head are then unused (layers[] still supplies the norms and the
+                                KV cache).  Every linear runs b2l_q8_linear, the same 5*n_layer + 3 launches
+                                (+1 per LoRA layer); affines are applied inside them (c_fc12's interleaved
+                                8 / 8 as documented above).                               */
+  b2l_q8_weight q8_lm_head;
+  float q8_threshold;        /* B2L_F_Q8: Linear8bitLt.threshold of every linear          */
 } b2l_decode_args;
 
 int b2l_decode_step(const b2l_decode_args* args, b2l_stream_t stream);

@@ -14,6 +14,7 @@ PRO_NONE, PRO_RMSNORM = 0, 1
 EPI_STORE, EPI_RESIDUAL, EPI_SWIGLU = 0, 1, 2
 F_PDL, F_NO_ALIAS_N, F_ROPE_ROWS = 1, 2, 4
 F_W8 = 32   # b2l_decode_step: every linear is gptq.int8 (b2l_w8_gemv)
+F_Q8 = 64   # b2l_decode_step: every linear is llm.int8 (b2l_q8_linear)
 
 c_void_p, c_int, c_float, c_size_t = C.c_void_p, C.c_int, C.c_float, C.c_size_t
 
@@ -73,6 +74,25 @@ class LayerAffine(C.Structure):
     _fields_ = [("c_attn", OutAffine), ("c_proj", OutAffine), ("c_fc12", OutAffine), ("mlp_proj", OutAffine)]
 
 
+class Q8LinearArgs(C.Structure):
+    """b2l_q8_linear_args: the batch-1 llm.int8 linear with RMSNorm prologue and affine / residual / SwiGLU epilogue."""
+    _fields_ = [
+        ("x", c_void_p), ("cb", c_void_p), ("scb", c_void_p), ("cb2", c_void_p), ("scb2", c_void_p), ("y", c_void_p),
+        ("N", c_int), ("K", c_int), ("threshold", c_float),
+        ("prologue", c_int), ("norm_scale", c_void_p), ("eps", c_float),
+        ("epilogue", c_int), ("res", c_void_p), ("out_affine", OutAffine), ("flags", c_int),
+    ]
+
+
+class Q8Weight(C.Structure):
+    """b2l_q8_weight: a Linear8bitLt's weight.CB (int8 [N, K]) and weight.SCB (fp32 [N])."""
+    _fields_ = [("cb", c_void_p), ("scb", c_void_p), ("N", c_int), ("K", c_int)]
+
+
+class Q8Layer(C.Structure):
+    _fields_ = [("c_attn", Q8Weight), ("c_proj", Q8Weight), ("c_fc1", Q8Weight), ("c_fc2", Q8Weight), ("mlp_proj", Q8Weight)]
+
+
 class DecodeArgs(C.Structure):
     _fields_ = [
         ("n_layer", c_int), ("n_head", c_int), ("n_embd", c_int), ("n_hidden", c_int), ("vocab", c_int),
@@ -85,6 +105,7 @@ class DecodeArgs(C.Structure):
         ("logits", c_void_p), ("flags", c_int), ("timeline", c_void_p), ("batch_work", c_void_p),
         ("plan", c_void_p), ("adapters", C.POINTER(AdapterPrefix)), ("loras", C.POINTER(LoRA)),
         ("affines", C.POINTER(LayerAffine)), ("lm_head_affine", OutAffine),
+        ("q8_layers", C.POINTER(Q8Layer)), ("q8_lm_head", Q8Weight), ("q8_threshold", c_float),
     ]
 
 
@@ -141,6 +162,7 @@ _SIGS = {
     "b2l_q8_gemv": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_int, c_void_p]),
     "b2l_q8_gemv_cb": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_int, c_void_p]),
     "b2l_q8_outlier_mask": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
+    "b2l_q8_linear": (c_int, [C.POINTER(Q8LinearArgs), c_void_p]),
     "b2l_q8_gemm_workspace_bytes": (c_size_t, [c_int, c_int]),
     "b2l_q8_gemm": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_int, c_int, c_int, c_int, c_float,
                             c_int, c_void_p]),

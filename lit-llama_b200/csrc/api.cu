@@ -162,6 +162,48 @@ static int q4_call(const b2l_q4_weight& w, const void* x, int ldx, void* y, int 
   return b2l_q4_linear_tc(&a, stream);
 }
 
+// llm.int8 (B2L_F_Q8): one b2l_q8_linear launch per linear; w2 = c_fc2 for the SwiGLU pair
+static int q8_call(const b2l_decode_args* d, const b2l_q8_weight& w, const b2l_q8_weight* w2, const void* x, void* y,
+                   const void* norm_scale, int epilogue, const void* res, const b2l_out_affine* aff, b2l_stream_t stream) {
+  b2l_q8_linear_args a{};
+  a.x = x; a.cb = w.cb; a.scb = w.scb;
+  if (w2 != nullptr) { a.cb2 = w2->cb; a.scb2 = w2->scb; }
+  a.y = y; a.N = w.N; a.K = w.K; a.threshold = d->q8_threshold;
+  a.prologue = norm_scale != nullptr ? B2L_PRO_RMSNORM : B2L_PRO_NONE; a.norm_scale = norm_scale; a.eps = d->eps;
+  a.epilogue = epilogue; a.res = res;
+  if (aff != nullptr) a.out_affine = *aff;
+  a.flags = d->flags & B2L_F_PDL;
+  return b2l_q8_linear(&a, stream);
+}
+
+// every llm.int8 weight of the step has the shape its place in the Block implies and one the kernel runs
+static int check_q8_weight(const b2l_q8_weight& w, int N, int K, const char* what, int l) {
+  B2L_CHECK_ARG(w.cb != nullptr && w.scb != nullptr, "b2l_decode_step: B2L_F_Q8 %s of layer %d has no CB / SCB", what, l);
+  B2L_CHECK_ARG(w.N == N && w.K == K, "b2l_decode_step: B2L_F_Q8 %s of layer %d is [%d, %d], expected [%d, %d]", what, l,
+                w.N, w.K, N, K);
+  B2L_CHECK_SUPPORTED(K % 128 == 0 && K <= 32768, "b2l_decode_step: B2L_F_Q8 %s: in_features %d must be a multiple of 128 and <= 32768",
+                      what, K);
+  B2L_CHECK_ARG((uintptr_t)w.cb % 16 == 0, "b2l_decode_step: B2L_F_Q8 %s of layer %d: CB must be 16-byte aligned", what, l);
+  return 0;
+}
+
+static int check_q8(const b2l_decode_args* d) {
+  B2L_CHECK_SUPPORTED(!(d->flags & B2L_F_W8), "b2l_decode_step: B2L_F_Q8 (llm.int8) and B2L_F_W8 (gptq.int8) exclude each other");
+  B2L_CHECK_SUPPORTED(d->B == 1, "b2l_decode_step: B2L_F_Q8 (llm.int8) runs batch 1 only, got B=%d", d->B);
+  B2L_CHECK_SUPPORTED(d->plan == nullptr, "b2l_decode_step: B2L_F_Q8 (llm.int8) does not run in the persistent kernel (plan must be NULL)");
+  B2L_CHECK_ARG(d->q8_layers != nullptr, "b2l_decode_step: B2L_F_Q8 needs q8_layers");
+  const int C = d->n_embd, H = d->n_hidden;
+  for (int l = 0; l < d->n_layer; ++l) {
+    const b2l_q8_layer& q = d->q8_layers[l];
+    int rc;
+    if ((rc = check_q8_weight(q.c_attn, 3 * C, C, "c_attn", l)) || (rc = check_q8_weight(q.c_proj, C, C, "c_proj", l)) ||
+        (rc = check_q8_weight(q.c_fc1, H, C, "c_fc1", l)) || (rc = check_q8_weight(q.c_fc2, H, C, "c_fc2", l)) ||
+        (rc = check_q8_weight(q.mlp_proj, C, H, "mlp.c_proj", l)))
+      return rc;
+  }
+  return check_q8_weight(d->q8_lm_head, d->vocab, C, "lm_head", -1);
+}
+
 extern "C" int b2l_decode_step_launches(const b2l_decode_args* d) {
   if (!d) return 0;
   if (d->plan != nullptr) return 1;   // the persistent kernel
@@ -187,6 +229,9 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
   B2L_CHECK_ARG(d->wte && d->ln_f && d->rope && d->idx && d->input_pos && d->ring_start && d->x && d->qkv && d->att &&
                     d->hid && d->attn_work && d->logits,
                 "b2l_decode_step: null pointer");
+  const bool q8 = (d->flags & B2L_F_Q8) != 0;
+  if (q8)
+    if (int rc = check_q8(d)) return rc;
   if (d->flags & B2L_F_W8) {
     B2L_CHECK_SUPPORTED(d->B == 1, "b2l_decode_step: B2L_F_W8 (gptq.int8) runs batch 1 only, got B=%d", d->B);
     B2L_CHECK_SUPPORTED(d->plan == nullptr, "b2l_decode_step: B2L_F_W8 (gptq.int8) does not run in the persistent kernel (plan must be NULL)");
@@ -213,20 +258,20 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
     B2L_CHECK_SUPPORTED(d->loras == nullptr, "b2l_decode_step: LLaMA-Adapter v2 affines and LoRA do not combine");
     auto ok = [](const b2l_out_affine& f) { return (f.scale == nullptr) == (f.bias == nullptr); };
     B2L_CHECK_ARG(ok(d->lm_head_affine), "b2l_decode_step: lm_head_affine needs both scale and bias (or neither)");
-    B2L_CHECK_SUPPORTED(d->lm_head.qw_mma != nullptr, "b2l_decode_step: affines need the batch-1 tiling (qw_mma) of every weight");
+    B2L_CHECK_SUPPORTED(q8 || d->lm_head.qw_mma != nullptr, "b2l_decode_step: affines need the batch-1 tiling (qw_mma) of every weight");
     for (int l = 0; d->affines != nullptr && l < d->n_layer; ++l) {
       const b2l_layer_affine& f = d->affines[l];
       B2L_CHECK_ARG(ok(f.c_attn) && ok(f.c_proj) && ok(f.c_fc12) && ok(f.mlp_proj),
                     "b2l_decode_step: affines[%d] needs both scale and bias (or neither) per linear", l);
       const b2l_layer& L = d->layers[l];
-      B2L_CHECK_SUPPORTED(L.c_attn.qw_mma && L.c_proj.qw_mma && L.c_fc12.qw_mma && L.mlp_proj.qw_mma,
+      B2L_CHECK_SUPPORTED(q8 || (L.c_attn.qw_mma && L.c_proj.qw_mma && L.c_fc12.qw_mma && L.mlp_proj.qw_mma),
                           "b2l_decode_step: affines need the batch-1 tiling (qw_mma) of every weight");
     }
   }
   if (d->plan != nullptr) return decode_step_persistent(d, stream);   // one persistent kernel per token (decode_mega.cu)
   const int C = d->n_embd, hs = C / d->n_head, B = d->B;
   const int fl = d->flags;               // the linears' flags (q4_call routes B2L_F_W8 to b2l_w8_gemv)
-  const int afl = fl & ~B2L_F_W8;        // everything else
+  const int afl = fl & ~(B2L_F_W8 | B2L_F_Q8);   // everything else
   int rc;
   // debug timeline: launch i of the step writes uint64[64] at timeline + 512*i (order: per Block c_attn,
   // attention, c_proj, fc12, mlp_proj; then lm_head)
@@ -246,9 +291,12 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
   for (int l = 0; l < d->n_layer; ++l) {
     const b2l_layer& L = d->layers[l];
     const b2l_layer_affine* af = d->affines != nullptr ? &d->affines[l] : nullptr;
-    if ((rc = q4_call(L.c_attn, d->x, C, d->qkv, 3 * C, B, d->sz_dtype, B2L_PRO_RMSNORM, L.rms_1, d->eps, B2L_EPI_STORE,
-                      nullptr, 0, fl, stream, tl(), d->batch_work, pf(), (kv_ok && kv_prefetch == 2) ? d : nullptr, l,
-                      af ? &af->c_attn : nullptr)))
+    const b2l_q8_layer* Q = q8 ? &d->q8_layers[l] : nullptr;   // llm.int8: b2l_q8_linear (no timeline stamps)
+    void* t = tl();
+    if ((rc = Q ? q8_call(d, Q->c_attn, nullptr, d->x, d->qkv, L.rms_1, B2L_EPI_STORE, nullptr, af ? &af->c_attn : nullptr, stream)
+                : q4_call(L.c_attn, d->x, C, d->qkv, 3 * C, B, d->sz_dtype, B2L_PRO_RMSNORM, L.rms_1, d->eps, B2L_EPI_STORE,
+                          nullptr, 0, fl, stream, t, d->batch_work, pf(), (kv_ok && kv_prefetch == 2) ? d : nullptr, l,
+                          af ? &af->c_attn : nullptr)))
       return rc;
     // LoRA on c_attn (lora.py:308-326): the low-rank term from rms_1(x), added into qkv in place
     if (d->loras != nullptr && d->loras[l].r != 0 &&
@@ -265,20 +313,27 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
       return rc;
     }
     g_attn_timeline = nullptr;
-    if ((rc = q4_call(L.c_proj, d->att, C, d->x, C, B, d->sz_dtype, B2L_PRO_NONE, nullptr, 0.f, B2L_EPI_RESIDUAL, d->x, C,
-                      fl, stream, tl(), d->batch_work, pf(), nullptr, 0, af ? &af->c_proj : nullptr)))
+    t = tl();
+    if ((rc = Q ? q8_call(d, Q->c_proj, nullptr, d->att, d->x, nullptr, B2L_EPI_RESIDUAL, d->x, af ? &af->c_proj : nullptr, stream)
+                : q4_call(L.c_proj, d->att, C, d->x, C, B, d->sz_dtype, B2L_PRO_NONE, nullptr, 0.f, B2L_EPI_RESIDUAL, d->x, C,
+                          fl, stream, t, d->batch_work, pf(), nullptr, 0, af ? &af->c_proj : nullptr)))
       return rc;
-    if ((rc = q4_call(L.c_fc12, d->x, C, d->hid, d->n_hidden, B, d->sz_dtype, B2L_PRO_RMSNORM, L.rms_2, d->eps,
-                      B2L_EPI_SWIGLU, nullptr, 0, fl, stream, tl(), d->batch_work, pf(), nullptr, 0, af ? &af->c_fc12 : nullptr)))
+    t = tl();
+    if ((rc = Q ? q8_call(d, Q->c_fc1, &Q->c_fc2, d->x, d->hid, L.rms_2, B2L_EPI_SWIGLU, nullptr, af ? &af->c_fc12 : nullptr, stream)
+                : q4_call(L.c_fc12, d->x, C, d->hid, d->n_hidden, B, d->sz_dtype, B2L_PRO_RMSNORM, L.rms_2, d->eps,
+                          B2L_EPI_SWIGLU, nullptr, 0, fl, stream, t, d->batch_work, pf(), nullptr, 0, af ? &af->c_fc12 : nullptr)))
       return rc;
     // mlp.c_proj fits the weight ring entirely, so HBM idles while it converts its activations: it asks the L2 for
     // the NEXT Block's KV-cache rows (B2L_KV_PREFETCH=0 switches that off)
     const bool kvpf = kv_prefetch == 1 && kv_ok && l + 1 < d->n_layer;
-    if ((rc = q4_call(L.mlp_proj, d->hid, d->n_hidden, d->x, C, B, d->sz_dtype, B2L_PRO_NONE, nullptr, 0.f,
-                      B2L_EPI_RESIDUAL, d->x, C, fl, stream, tl(), d->batch_work, pf(), kvpf ? d : nullptr, l + 1,
-                      af ? &af->mlp_proj : nullptr)))
+    t = tl();
+    if ((rc = Q ? q8_call(d, Q->mlp_proj, nullptr, d->hid, d->x, nullptr, B2L_EPI_RESIDUAL, d->x, af ? &af->mlp_proj : nullptr, stream)
+                : q4_call(L.mlp_proj, d->hid, d->n_hidden, d->x, C, B, d->sz_dtype, B2L_PRO_NONE, nullptr, 0.f,
+                          B2L_EPI_RESIDUAL, d->x, C, fl, stream, t, d->batch_work, pf(), kvpf ? d : nullptr, l + 1,
+                          af ? &af->mlp_proj : nullptr)))
       return rc;
   }
+  if (q8) return q8_call(d, d->q8_lm_head, nullptr, d->x, d->logits, d->ln_f, B2L_EPI_STORE, nullptr, &d->lm_head_affine, stream);
   return q4_call(d->lm_head, d->x, C, d->logits, d->vocab, B, d->sz_dtype, B2L_PRO_RMSNORM, d->ln_f, d->eps,
                  B2L_EPI_STORE, nullptr, 0, fl, stream, tl(), d->batch_work, pf(), nullptr, 0, &d->lm_head_affine);
 }

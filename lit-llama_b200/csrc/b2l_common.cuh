@@ -127,6 +127,11 @@ __device__ __forceinline__ uint4 ld_coherent_u4(const void* p) {
   asm volatile("ld.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p) : "memory");
   return v;
 }
+__device__ __forceinline__ float ld_coherent_bf16(const __nv_bfloat16* p) {
+  unsigned short v;
+  asm volatile("ld.global.u16 %0, [%1];" : "=h"(v) : "l"(p) : "memory");
+  return __uint_as_float((uint32_t)v << 16);
+}
 
 // RMSNorm with the reference's bf16 rounding points (model.py:270-277, no upcast):
 //   ms = bf16(mean(bf16(x*x)));  r = bf16(rsqrt(bf16(ms + eps)));  y = bf16(scale * bf16(x * r))
@@ -138,6 +143,15 @@ __device__ __forceinline__ float rms_rinv(float sumsq, int C, float eps) {
 }
 __device__ __forceinline__ float rms_apply(float x, float rinv, float scale) {
   return rbf(scale * rbf(x * rinv));
+}
+
+// silu(a) * b, model.py:252: silu rounds to bf16, then the product rounds to bf16 (at the caller's store).
+__device__ __forceinline__ float silu_mul1(float av, float bv) { return rbf(av / (1.0f + expf(-av))) * bv; }
+// LLaMA-Adapter v2's affine of one output feature, adapter_v2.py:30-33: bf16(s * bf16(y + b)) (rounded at the store).
+__device__ __forceinline__ float affine1(float y, float s, float b) { return s * rbf(y + b); }
+__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
+  const __nv_bfloat162 t = __floats2bfloat162_rn(lo, hi);
+  return *reinterpret_cast<const uint32_t*>(&t);
 }
 
 // Launch helper: optional PDL attribute and cluster dimension.

@@ -62,12 +62,7 @@ __global__ void embedding_kernel(const IdxT* __restrict__ idx, const __nv_bfloat
   for (int i = threadIdx.x; i < C; i += blockDim.x) dst[i] = src[i];
 }
 
-// silu(a) * b, model.py:252: silu rounds to bf16, then the product rounds to bf16.
-__device__ __forceinline__ float silu_mul1(float av, float bv) { return rbf(av / (1.0f + expf(-av))) * bv; }
-__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
-  const __nv_bfloat162 t = __floats2bfloat162_rn(lo, hi);
-  return *reinterpret_cast<const uint32_t*>(&t);
-}
+// silu_mul1 / pack_bf16x2 / affine1: b2l_common.cuh (the batch-1 llm.int8 linear fuses the same arithmetic).
 // 8 elements (16 bytes) per thread when the pointers allow it (VEC), else one
 template <bool VEC, bool SILU>
 __global__ void __launch_bounds__(256) binary_kernel(const __nv_bfloat16* __restrict__ a, const __nv_bfloat16* __restrict__ b,
@@ -104,7 +99,6 @@ static int launch_binary(const void* a, const void* b, void* y, size_t n, cudaSt
 
 // LLaMA-Adapter v2's affine of a linear's output, adapter_v2.py:30-33: y = bf16(s * bf16(y + b)) per column, in
 // place.  VEC: 8 columns (16 bytes) per thread, N, ldy multiples of 8 and 16-byte aligned pointers.
-__device__ __forceinline__ float affine1(float y, float s, float b) { return s * rbf(y + b); }
 template <bool VEC>
 __global__ void __launch_bounds__(256) linear_affine_kernel(__nv_bfloat16* y, int ldy, int M, int N,
                                                             const __nv_bfloat16* __restrict__ scale,

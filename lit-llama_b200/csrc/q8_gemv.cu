@@ -25,6 +25,13 @@
 //     32c + 16 + 4t..+3.  One 16 KB bulk copy per stage.
 // Both contract the same int8 values in the same order, so their outputs are bit-identical.
 //
+// FUSED (b2l_q8_linear, WS_CB only): the whole-token step's llm.int8 linear.  The consumers first apply RMSNorm exactly
+// as b2l_rmsnorm does (same 256-thread chunking and reduction order, the scale staged in `ah` before the dependency),
+// so the outlier mask and SCA are those of the module path.  For SWIGLU a 16-row block holds 8 rows of cb and the
+// same 8 rows of cb2; the epilogue warp rounds each row to bf16 as the module's store would, applies the v2 affine,
+// then adds the residual or combines lane r with lane r + 8 through silu_mul1.  The non-FUSED instantiations compile
+// to the same SASS as before the FUSED code existed.
+//
 // parity: the arithmetic restates the published LLM.int8() algorithm (bitsandbytes is not in
 // the reference tree and not installed): parity with the reference is unpinned (DESIGN.md).
 #include <cuda_fp16.h>
@@ -58,6 +65,15 @@ struct Params {
   __nv_bfloat16* y;           // [N]
   int N, K, n_rb, nst;
   float threshold;
+  // FUSED (b2l_q8_linear) only
+  const int8_t* cb2;          // SWIGLU: the second CB / SCB (rows 8..15 of every block; rows 0..7 come from cb)
+  const float* scb2;
+  const __nv_bfloat16* norm_scale;   // RMSNorm prologue; nullptr = none
+  float eps;
+  int epilogue;               // B2L_EPI_*
+  const __nv_bfloat16* res;   // RESIDUAL
+  const __nv_bfloat16* aff_s; // LLaMA-Adapter v2 affine; nullptr = none
+  const __nv_bfloat16* aff_b;
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -107,7 +123,36 @@ __host__ __device__ inline SmemLayout smem_layout(int nst, int K, uint32_t stage
   return L;
 }
 
-template <WeightSource WS>
+// One output row of a 16-row block as the FUSED epilogue needs it.  SWIGLU: rows 0..7 are outputs rb*8 .. rb*8+7 of
+// cb, rows 8..15 the same outputs of cb2; the affine vectors are interleaved the same way (16 entries per block).
+struct FusedRow {
+  const int8_t* w;   // the weight row (outlier term)
+  float scb, s, b;   // SCB and the affine's scale / bias (1, 0 without one)
+  int col;           // output index
+  bool valid;
+};
+__device__ __forceinline__ FusedRow fused_row(const Params& p, int rb, int row) {
+  const bool glu = p.epilogue == B2L_EPI_SWIGLU;
+  FusedRow r;
+  r.col = glu ? rb * 8 + (row & 7) : rb * RB + row;
+  r.valid = r.col < p.N;
+  const int o = min(r.col, p.N - 1);
+  const bool second = glu && row >= 8;
+  r.w = (second ? p.cb2 : p.cb) + (size_t)o * p.K;
+  r.scb = (second ? p.scb2 : p.scb)[o];
+  r.s = 1.f;
+  r.b = 0.f;
+  if (p.aff_s != nullptr) {
+    const int ai = glu ? (r.valid ? rb * 16 + row : 0) : o;
+    r.s = bf2f(p.aff_s[ai]);
+    r.b = bf2f(p.aff_b[ai]);
+  }
+  return r;
+}
+
+// FUSED = false: b2l_q8_gemv / b2l_q8_gemv_cb.  FUSED = true (WS_CB only): b2l_q8_linear, the same body plus the
+// RMSNorm prologue, two weight sources for SWIGLU and the affine / residual / SwiGLU epilogue.
+template <WeightSource WS, bool FUSED>
 __global__ void __launch_bounds__(NTHREADS, 2) q8_gemv_kernel(const Params p) {
   extern __shared__ __align__(128) uint8_t smem[];
   constexpr uint32_t SB = stage_bytes<WS>();
@@ -137,7 +182,22 @@ __global__ void __launch_bounds__(NTHREADS, 2) q8_gemv_kernel(const Params p) {
       uint32_t phase = 1;
       for (int u = 0; u < n_units; ++u) {
         for (int s = 0; s < stages_per_rb; ++s, ++it) {
-          if constexpr (WS == WS_CB) {
+          if constexpr (FUSED) {
+            // as WS_CB below; SWIGLU: lanes 0..7 copy rows of cb, lanes 8..15 the same rows of cb2
+            const bool glu = p.epilogue == B2L_EPI_SWIGLU;
+            const int per = glu ? 8 : RB, i = glu ? (lane & 7) : lane;
+            const int row0 = (rb_lo + u) * per, nrows = min(per, p.N - row0);
+            const uint32_t row_bytes = (uint32_t)min(KBP_PER_STAGE, n_kb - s * KBP_PER_STAGE) * KB;
+            if (lane == 0) {
+              mbar_wait(bar_empty + slot * 8, phase);
+              mbar_expect_tx(bar_full + slot * 8, (uint32_t)(glu ? 2 : 1) * nrows * row_bytes);
+            }
+            __syncwarp();
+            if (lane < RB && i < nrows)
+              tma_bulk_g2s(sbase + L.ring + slot * SB + lane * ROW_PITCH,
+                           ((glu && lane >= 8) ? p.cb2 : p.cb) + (size_t)(row0 + i) * p.K + (size_t)s * KBP_PER_STAGE * KB,
+                           row_bytes, bar_full + slot * 8);
+          } else if constexpr (WS == WS_CB) {
             // one bulk copy per weight row (lanes 0..15); rows past N are not copied (their accumulators are never
             // stored), so the transaction count is what is actually copied
             const int row0 = (rb_lo + u) * RB, nrows = min(RB, p.N - row0);
@@ -165,18 +225,60 @@ __global__ void __launch_bounds__(NTHREADS, 2) q8_gemv_kernel(const Params p) {
     }
   } else if (warp < NCW) {
     // ===================== consumer warps =====================
-    pdl_wait();
+    if constexpr (!FUSED) pdl_wait();
     float* red = reinterpret_cast<float*>(smem + L.red);
     __half* ah = reinterpret_cast<__half*>(smem + L.ah);
     uint32_t* mask = reinterpret_cast<uint32_t*>(smem + L.mask);
     constexpr int NT = NCW * 32;
+    float rinv = 0.f;
+    if constexpr (FUSED) {
+      // RMSNorm: the scale (a weight) is staged in `ah` before the dependency; each thread later overwrites exactly the
+      // chunks it staged.  Sum of squares in rmsnorm_kernel's order: these 256 threads take its 256 threads' 8-element
+      // chunks, then its block_sum (warp_sum, partials of 8 warps, warp_sum).
+      if (p.norm_scale != nullptr)
+        for (int k = tid * 8; k < p.K; k += NT * 8)
+          *reinterpret_cast<uint4*>(ah + k) = *reinterpret_cast<const uint4*>(p.norm_scale + k);
+      pdl_wait();
+      if (p.norm_scale != nullptr) {
+        float ss = 0.f;
+        for (int k = tid * 8; k < p.K; k += NT * 8) {
+          const uint4 v = ld_coherent_u4(p.x + k);
+          const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            const float lo = __uint_as_float(w[q] << 16), hi = __uint_as_float(w[q] & 0xffff0000u);
+            ss += rbf(lo * lo) + rbf(hi * hi);
+          }
+        }
+        ss = warp_sum(ss);
+        if (lane == 0) red[warp] = ss;
+        bar_sync_c<1>(NT);
+        ss = warp_sum(lane < NCW ? red[lane] : 0.f);
+        rinv = rms_rinv(ss, p.K, p.eps);   // red is next written after two more bar_sync_c<1>
+      }
+    }
     // ---- activations: fp16 copy, outlier mask, row-wise absmax over inliers, int8 B fragments.  The row lives in
     // shared memory only (ah, which the epilogue needs anyway): each thread re-reads the 8-element chunks it wrote,
     // so no K-sized register array limits K.
     for (int i = tid; i < (p.K + 31) / 32; i += NT) mask[i] = p.mask_in ? p.mask_in[i] : 0u;
     bar_sync_c<1>(NT);
     for (int k = tid * 8; k < p.K; k += NT * 8) {
-      const uint4 u = *reinterpret_cast<const uint4*>(p.x + k);
+      uint4 u;
+      if constexpr (FUSED) {
+        u = ld_coherent_u4(p.x + k);
+        if (p.norm_scale != nullptr) {   // x^ = rms_apply (b2l_rmsnorm's bf16 values), scale from `ah`
+          const uint4 g = *reinterpret_cast<const uint4*>(ah + k);
+          const uint32_t xw[4] = {u.x, u.y, u.z, u.w}, gw[4] = {g.x, g.y, g.z, g.w};
+          uint32_t o[4];
+#pragma unroll
+          for (int q = 0; q < 4; ++q)
+            o[q] = pack_bf16x2(rms_apply(__uint_as_float(xw[q] << 16), rinv, __uint_as_float(gw[q] << 16)),
+                               rms_apply(__uint_as_float(xw[q] & 0xffff0000u), rinv, __uint_as_float(gw[q] & 0xffff0000u)));
+          u = make_uint4(o[0], o[1], o[2], o[3]);
+        }
+      } else {
+        u = *reinterpret_cast<const uint4*>(p.x + k);
+      }
       const uint32_t w[4] = {u.x, u.y, u.z, u.w};
       __half hv[8];
       uint32_t outl = 0;
@@ -273,6 +375,9 @@ __global__ void __launch_bounds__(NTHREADS, 2) q8_gemv_kernel(const Params p) {
     }
   } else {
     // ===================== epilogue warp: lanes 0..15 = rows of the block =====================
+    FusedRow fr{};
+    if constexpr (FUSED)   // the first block's SCB and affine are weights: read before the dependency
+      if (n_units > 0) fr = fused_row(p, rb_lo, lane & 15);
     pdl_wait();
     const float* red = reinterpret_cast<const float*>(smem + L.red);
     const int* scratch = reinterpret_cast<const int*>(smem + L.scratch);
@@ -288,7 +393,9 @@ __global__ void __launch_bounds__(NTHREADS, 2) q8_gemv_kernel(const Params p) {
       const int row = lane & 15;
       const int orow = (rb_lo + u) * RB + row;
       const int o = min(orow, p.N - 1);
-      const float scb = p.scb[o];
+      if constexpr (FUSED)
+        if (u > 0) fr = fused_row(p, rb_lo + u, row);
+      const float scb = FUSED ? fr.scb : p.scb[o];
       // outlier term first (global loads overlap the consumers' work): fp16 weights, fp32 accumulate, k ascending
       float term = 0.f;
       bool any = false;
@@ -299,7 +406,7 @@ __global__ void __launch_bounds__(NTHREADS, 2) q8_gemv_kernel(const Params p) {
           const int e = __ffs(mb) - 1;
           mb &= mb - 1;
           const int k = wi * 32 + e;
-          const float wv = __half2float(__float2half_rn((float)p.cb[(size_t)o * p.K + k] * wsc));
+          const float wv = __half2float(__float2half_rn((float)(FUSED ? fr.w[k] : p.cb[(size_t)o * p.K + k]) * wsc));
           term = fmaf(__half2float(ah[k]), wv, term);
           any = true;
         }
@@ -311,7 +418,19 @@ __global__ void __launch_bounds__(NTHREADS, 2) q8_gemv_kernel(const Params p) {
       if (u + 2 < n_units) { if (buf) bar_arrive_c<5>(NCW * 32 + 32); else bar_arrive_c<4>(NCW * 32 + 32); }
       float v = __half2float(__float2half_rn((float)t * (sca * scb * (1.0f / (127.0f * 127.0f)))));
       if (any) v = __half2float(__float2half_rn(v + __half2float(__float2half_rn(term))));
-      if (lane < 16 && orow < p.N) p.y[orow] = f2bf(v);
+      if constexpr (FUSED) {
+        // the module path's bf16 output, then b2l_linear_affine, then b2l_add / b2l_silu_mul
+        float yv = rbf(v);
+        if (p.aff_s != nullptr) yv = rbf(affine1(yv, fr.s, fr.b));
+        if (p.epilogue == B2L_EPI_SWIGLU) {
+          const float up = __shfl_down_sync(0xffffffffu, yv, 8);   // row r + 8: c_fc2's output of the same column
+          if (lane < 8 && fr.valid) p.y[fr.col] = f2bf(silu_mul1(yv, up));
+        } else if (lane < 16 && fr.valid) {
+          p.y[fr.col] = f2bf(p.epilogue == B2L_EPI_RESIDUAL ? yv + ld_coherent_bf16(p.res + fr.col) : yv);
+        }
+      } else {
+        if (lane < 16 && orow < p.N) p.y[orow] = f2bf(v);
+      }
     }
   }
 }
@@ -357,7 +476,7 @@ extern "C" int b2l_q8_tile(const void* cb, void* tiled, int N, int K, b2l_stream
 }
 
 // stage count, grid and launch, shared by both weight sources; p holds everything but nst
-template <WeightSource WS>
+template <WeightSource WS, bool FUSED = false>
 static int launch_gemv(Params& p, int flags, b2l_stream_t stream) {
   constexpr uint32_t SB = stage_bytes<WS>();
   const uint32_t fixed = smem_layout(0, p.K, SB).total;
@@ -367,12 +486,12 @@ static int launch_gemv(Params& p, int flags, b2l_stream_t stream) {
   p.nst = nst;
   const SmemLayout L = smem_layout(nst, p.K, SB);
   static DynSmemCache smem_cache;
-  if (int rc = ensure_dyn_smem(q8_gemv_kernel<WS>, L.total, smem_cache)) return rc;
+  if (int rc = ensure_dyn_smem(q8_gemv_kernel<WS, FUSED>, L.total, smem_cache)) return rc;
   // two CTAs per SM while both fit in its 228 KB (1 KB of each reserved by the hardware); above K ~ 26000 only one does
   int grid = (L.total <= 113u * 1024u ? 2 : 1) * sm_count();
   if (grid > p.n_rb) grid = p.n_rb;
   LaunchCfg lc(dim3(grid), dim3(NTHREADS), L.total, (cudaStream_t)stream, (flags & B2L_F_PDL) != 0, 1);
-  B2L_CUDA(cudaLaunchKernelEx(&lc.cfg, q8_gemv_kernel<WS>, p));
+  B2L_CUDA(cudaLaunchKernelEx(&lc.cfg, q8_gemv_kernel<WS, FUSED>, p));
   return 0;
 }
 
@@ -405,6 +524,36 @@ extern "C" int b2l_q8_gemv_cb(const void* x, const void* cb, const void* scb, co
   Params p;
   fill_params(p, x, cb, scb, outlier_mask, y, N, K, threshold);
   return launch_gemv<WS_CB>(p, flags, stream);
+}
+
+extern "C" int b2l_q8_linear(const b2l_q8_linear_args* a, b2l_stream_t stream) {
+  B2L_CHECK_ARG(a != nullptr && a->x && a->cb && a->scb && a->y, "b2l_q8_linear: null pointer");
+  const int N = a->N, K = a->K;
+  B2L_CHECK_SUPPORTED(K > 0 && K % KB == 0 && K <= MAX_K, "b2l_q8_linear: K=%d must be a multiple of %d and <= %d", K, KB, MAX_K);
+  B2L_CHECK_ARG(N > 0, "b2l_q8_linear: bad shape N=%d", N);
+  B2L_CHECK_ARG(a->prologue == B2L_PRO_NONE || a->prologue == B2L_PRO_RMSNORM, "b2l_q8_linear: bad prologue %d", a->prologue);
+  B2L_CHECK_ARG(a->epilogue == B2L_EPI_STORE || a->epilogue == B2L_EPI_RESIDUAL || a->epilogue == B2L_EPI_SWIGLU,
+                "b2l_q8_linear: bad epilogue %d", a->epilogue);
+  const bool norm = a->prologue == B2L_PRO_RMSNORM, glu = a->epilogue == B2L_EPI_SWIGLU;
+  B2L_CHECK_ARG(!norm || a->norm_scale, "b2l_q8_linear: RMSNORM needs norm_scale");
+  B2L_CHECK_ARG(a->epilogue != B2L_EPI_RESIDUAL || a->res, "b2l_q8_linear: RESIDUAL needs res");
+  B2L_CHECK_ARG(!glu || (a->cb2 && a->scb2), "b2l_q8_linear: SWIGLU needs cb2 and scb2");
+  B2L_CHECK_ARG((a->out_affine.scale == nullptr) == (a->out_affine.bias == nullptr),
+                "b2l_q8_linear: out_affine needs both scale and bias (or neither)");
+  B2L_CHECK_ARG(((uintptr_t)a->x | (uintptr_t)a->cb | (uintptr_t)(glu ? a->cb2 : nullptr) |
+                 (uintptr_t)(norm ? a->norm_scale : nullptr)) % 16 == 0,
+                "b2l_q8_linear: x / cb / cb2 / norm_scale must be 16-byte aligned");
+  const uintptr_t x0 = (uintptr_t)a->x, y0 = (uintptr_t)a->y;
+  B2L_CHECK_ARG(y0 + 2 * (size_t)N <= x0 || x0 + 2 * (size_t)K <= y0, "b2l_q8_linear: y overlaps x");
+  B2L_CHECK_SUPPORTED((a->flags & ~B2L_F_PDL) == 0, "b2l_q8_linear: unknown flags 0x%x (only B2L_F_PDL)", (unsigned)a->flags);
+  Params p;
+  fill_params(p, a->x, a->cb, a->scb, nullptr, a->y, N, K, a->threshold);
+  p.n_rb = glu ? (N + 7) / 8 : (N + RB - 1) / RB;
+  p.cb2 = (const int8_t*)a->cb2; p.scb2 = (const float*)a->scb2;
+  p.norm_scale = norm ? (const __nv_bfloat16*)a->norm_scale : nullptr; p.eps = a->eps;
+  p.epilogue = a->epilogue; p.res = (const __nv_bfloat16*)a->res;
+  p.aff_s = (const __nv_bfloat16*)a->out_affine.scale; p.aff_b = (const __nv_bfloat16*)a->out_affine.bias;
+  return launch_gemv<WS_CB, true>(p, a->flags, stream);
 }
 
 // outlier columns of a batch: bit k set iff any row has |fp16(x[m][k])| >= threshold

@@ -11,6 +11,8 @@ Two execution paths behind `LLaMA.forward`:
     one C call enqueues the whole token (`b2l_decode_step`: int8-MMA GEMV kernels for batch 1, f16-MMA for 2..8 rows,
     wgmma for 9..16), replayed as a CUDA graph.  Every Linear a per-row gptq.int8 layer: the same step at batch 1
     (B2L_F_W8: the GEMV kernel with 8-bit weights); batches of 2 or more go module by module (on the wgmma GEMM).
+    Every Linear an llm.int8 layer, with `LLaMA.int8_step` (B2L_INT8_STEP=1): the same step at batch 1 (B2L_F_Q8:
+    b2l_q8_linear reading CB / SCB in place), bit-identical to the module path.
   * everything else (prefill on the wgmma GEMM, no-cache forward, other Linear kinds): module by module.
 """
 import ctypes as C
@@ -289,7 +291,9 @@ class _DecodeState:
         # batch 1..8: mma.sync kernels (q4_gemv / q4_gemv_batch) and their tiling; 9..16: wgmma kernel and its tiling.
         # gptq.int8 (batch 1 only): the batch-1 kernel with 8-bit weights (b2l_w8_tile_i8 tilings)
         w8 = model._fast_ok == "w8"
-        assert B == 1 or not w8
+        # llm.int8 (batch 1 only): b2l_q8_linear on every weight's CB / SCB in place (no copy, no tiling)
+        q8 = model._fast_ok == "q8"
+        assert B == 1 or not (w8 or q8)
         gemv = (B == 1) or (B <= 8 and BATCH_GEMV)
         self.batch_ws = None
         if gemv and B > 1:
@@ -308,13 +312,23 @@ class _DecodeState:
                 self.keep.append(t)
             return t
 
+        def q8w(lin) -> L.Q8Weight:
+            return L.Q8Weight(lin.weight.data.data_ptr(), lin.weight.SCB.data_ptr(), lin.out_features, lin.in_features)
+
         layers = (L.Layer * cfg.n_layer)()
+        q8_layers = (L.Q8Layer * cfg.n_layer)() if q8 else None
         for i, blk in enumerate(model.transformer.h):
-            fc12 = model._fc12(i, "i8" if B == 1 else ("mma" if gemv else "tc"))
             k, v = model.kv_caches[i]
+            rms = dict(rms_1=bf16(blk.rms_1.scale).data_ptr(), rms_2=bf16(blk.rms_2.scale).data_ptr())
+            if q8:   # layers[i] supplies the norms and the KV cache only
+                mlp = blk.mlp
+                q8_layers[i] = L.Q8Layer(q8w(blk.attn.c_attn), q8w(blk.attn.c_proj), q8w(mlp.c_fc1), q8w(mlp.c_fc2),
+                                         q8w(mlp.c_proj))
+                layers[i] = L.Layer(**rms, k_cache=k.data_ptr(), v_cache=v.data_ptr())
+                continue
+            fc12 = model._fc12(i, "i8" if B == 1 else ("mma" if gemv else "tc"))
             layers[i] = L.Layer(
-                rms_1=bf16(blk.rms_1.scale).data_ptr(), rms_2=bf16(blk.rms_2.scale).data_ptr(),
-                c_attn=q4(blk.attn.c_attn), c_proj=q4(blk.attn.c_proj),
+                **rms, c_attn=q4(blk.attn.c_attn), c_proj=q4(blk.attn.c_proj),
                 c_fc12=L.Q4Weight(None if gemv else fc12[0].data_ptr(), fc12[0].data_ptr() if gemv else None,
                                   fc12[1].data_ptr(), fc12[2].data_ptr(), 2 * n_hidden, C_),
                 mlp_proj=q4(blk.mlp.c_proj), k_cache=k.data_ptr(), v_cache=v.data_ptr())
@@ -322,14 +336,19 @@ class _DecodeState:
         lin0 = model.lm_head
         self.args = L.DecodeArgs(
             n_layer=cfg.n_layer, n_head=nh, n_embd=C_, n_hidden=n_hidden, vocab=cfg.padded_vocab_size, B=B, S=S,
-            sz_dtype=L.sz_dtype_of(lin0.scales), eps=float(model.transformer.ln_f.eps), layers=layers,
+            sz_dtype=0 if q8 else L.sz_dtype_of(lin0.scales), eps=float(model.transformer.ln_f.eps), layers=layers,
             wte=bf16(model.transformer.wte.weight).data_ptr(), ln_f=bf16(model.transformer.ln_f.scale).data_ptr(),
-            lm_head=q4(lin0), rope=model.rope_cache.data_ptr(), idx=self.idx.data_ptr(),
+            lm_head=L.Q4Weight() if q8 else q4(lin0), rope=model.rope_cache.data_ptr(), idx=self.idx.data_ptr(),
             idx_is_i64=1 if idx_dtype == torch.int64 else 0, input_pos=self.pos.data_ptr(),
             ring_start=model._ring.data_ptr(), block_size=cfg.block_size, x=self.x.data_ptr(), qkv=self.qkv.data_ptr(),
             att=self.att.data_ptr(), hid=self.hid.data_ptr(), attn_work=self.work.data_ptr(),
-            logits=self.logits.data_ptr(), flags=model.decode_flags | (L.F_W8 if w8 else 0),
+            logits=self.logits.data_ptr(), flags=model.decode_flags | (L.F_W8 if w8 else 0) | (L.F_Q8 if q8 else 0),
             batch_work=None if self.batch_ws is None else self.batch_ws.data_ptr())
+        if q8:
+            self.q8_layers = q8_layers
+            self.args.q8_layers = C.cast(q8_layers, C.POINTER(L.Q8Layer))
+            self.args.q8_lm_head = q8w(lin0)
+            self.args.q8_threshold = float(lin0.threshold)
         adapters = model._adapter_prefixes()
         if adapters is not None:   # LLaMA-Adapter: the step's attention adds each layer's gated prefix term
             self.keep.append(adapters)
@@ -345,7 +364,7 @@ class _DecodeState:
         # gptq.int8 keeps one kernel per op under B2L_PERSISTENT=1 too, and so do adapter, LoRA and adapter-v2 models)
         self.plan = None
         kmax = max(C_, n_hidden)
-        if (model.persistent and not w8 and adapters is None and loras is None and affines is None and B == 1 and hs == 128
+        if (model.persistent and not w8 and not q8 and adapters is None and loras is None and affines is None and B == 1 and hs == 128
                 and kmax <= 12288):
             self.plan = torch.zeros(lib.b2l_decode_plan_bytes(C.byref(self.args)), dtype=torch.uint8, device=device)
             self.args.plan = self.plan.data_ptr()
@@ -374,6 +393,10 @@ class LLaMA(nn.Module):
     #: batch-1 decode (head_size 128) as ONE persistent kernel per token (csrc/decode_mega.cu) instead of one kernel
     #: per op.  Opt-in (B2L_PERSISTENT=1): the default is the per-op path under programmatic dependent launch.
     persistent: bool = os.environ.get("B2L_PERSISTENT", "0") == "1"
+    #: batch-1 decode of an llm.int8 model (plain, LLaMA-Adapter v1 / v2 or LoRA) on the whole-token step
+    #: (b2l_decode_step under B2L_F_Q8: b2l_q8_linear with RMSNorm / residual / SwiGLU / affine fused), bit-identical
+    #: to the module path.  Opt-in (B2L_INT8_STEP=1): by default llm.int8 decodes module by module.
+    int8_step: bool = os.environ.get("B2L_INT8_STEP", "0") == "1"
 
     def __init__(self, config: LLaMAConfig) -> None:
         super().__init__()
@@ -559,7 +582,7 @@ class LLaMA(nn.Module):
 
         if self._fast_ok is None:
             self._fast_ok = self._fast_decode_ok()
-        if not self._fast_ok:
+        if self._fast_ok not in ("q4", "w8"):   # llm.int8 ("q8") already holds one copy: CB, read in place
             raise RuntimeError("compact() needs a gptq.int4 or gptq.int8 model the fused batch-1 decode step can run "
                                "(one bit width for every linear)")
         for i, blk in enumerate(self.transformer.h):
@@ -576,9 +599,13 @@ class LLaMA(nn.Module):
         return self
 
     def _fast_decode_ok(self) -> Union[bool, str]:
-        """"q4" / "w8" when every Linear is a per-row gptq.int4 / gptq.int8 layer the fused step can run, else False."""
+        """"q4" / "w8" when every Linear is a per-row gptq.int4 / gptq.int8 layer the fused step can run, "q8" when every
+        Linear is a bias-free llm.int8 layer b2l_q8_linear can run (one threshold throughout), else False."""
+        from .int8 import Linear8bitLt
         from .quantization import ColBlockQuantizedLinear
 
+        if isinstance(self.lm_head, Linear8bitLt):
+            return "q8" if self._int8_decode_ok() else False
         if not isinstance(self.lm_head, ColBlockQuantizedLinear):
             return False
         kind = "w8" if self.lm_head.bits == 8 else "q4"
@@ -598,6 +625,24 @@ class LLaMA(nn.Module):
             if blk.mlp.c_fc1.out_features % 64 != 0:
                 return False
         return kind
+
+    def _int8_decode_ok(self) -> bool:
+        from .int8 import Linear8bitLt
+
+        thr = self.lm_head.threshold
+
+        def ok(m) -> bool:
+            if not isinstance(m, Linear8bitLt) or m.bias is not None or m.threshold != thr:
+                return False
+            cb, scb = m.weight.data, getattr(m.weight, "SCB", None)
+            return (m.in_features % 128 == 0 and m.in_features <= Linear8bitLt.MAX_IN_FEATURES and cb.is_cuda
+                    and cb.dtype == torch.int8 and cb.is_contiguous() and cb.data_ptr() % 16 == 0 and scb is not None
+                    and scb.dtype == torch.float32 and scb.is_contiguous() and scb.device == cb.device)
+
+        lins = [self.lm_head]
+        for blk in self.transformer.h:
+            lins += [blk.attn.c_attn, blk.attn.c_proj, blk.mlp.c_fc1, blk.mlp.c_fc2, blk.mlp.c_proj]
+        return all(ok(m) for m in lins)
 
     def logical_kv_caches(self) -> List[KVCache]:
         """kv_caches in the reference's slot order.  Identical to `kv_caches` until the
@@ -644,8 +689,9 @@ class LLaMA(nn.Module):
             if st is None or st.B != B or st.S != max_seq_length or st.idx.dtype != idx.dtype or st.idx.device != idx.device:
                 if self._fast_ok is None:
                     self._fast_ok = self._fast_decode_ok()
-                # gptq.int8 and LLaMA-Adapter v2: batch 1 only
-                fast = bool(self._fast_ok) and (B == 1 or (self._fast_ok != "w8" and not self._has_affines()))
+                # gptq.int8, llm.int8 and LLaMA-Adapter v2: batch 1 only; llm.int8 on request (int8_step)
+                fast = (bool(self._fast_ok) and (self._fast_ok != "q8" or self.int8_step)
+                        and (B == 1 or (self._fast_ok not in ("w8", "q8") and not self._has_affines())))
                 st = self._decode = _DecodeState(self, B, max_seq_length, idx.device, idx.dtype) if fast else None
         if st is not None:
             st.idx.copy_(idx.reshape(-1))

@@ -1655,6 +1655,107 @@ def sec_precision():
             print(line, flush=True)
 
 
+def sec_bench_q8_linear():
+    """b2l_q8_linear (the llm.int8 linear of the B2L_F_Q8 step) per 7B / 13B / 65B shape, next to b2l_q8_gemv_cb (the
+    module path's linear) and b2l_w8_gemv (gptq.int8, the same bytes of int8 weights): us per launch (200 launches in
+    a graph, PDL on for the fused kernels) and GB/s of weights streamed."""
+    import ctypes
+
+    import torch
+    from lit_llama_b200 import _lib as L
+    from lit_llama_b200.int8 import quantize_rows_int8
+    from lit_llama_b200.quantization import tile_i8
+
+    dev = torch.device("cuda")
+    print(_card(), flush=True)
+    shapes = [("7B c_attn", 12288, 4096, 0), ("7B c_proj", 4096, 4096, 0), ("7B fc1|fc2", 11008, 4096, 1),
+              ("7B mlp.c_proj", 4096, 11008, 0), ("13B c_attn", 15360, 5120, 0), ("13B fc1|fc2", 13824, 5120, 1),
+              ("13B mlp.c_proj", 5120, 13824, 0), ("65B c_attn", 24576, 8192, 0), ("65B fc1|fc2", 22016, 8192, 1),
+              ("65B mlp.c_proj", 8192, 22016, 0), ("lm_head", 32000, 4096, 0)]
+    lib = L.lib()
+    for name, N, K, glu in shapes:
+        cb, scb = quantize_rows_int8(torch.randn(N, K, device=dev) * 0.05)
+        cb2, scb2 = quantize_rows_int8(torch.randn(N, K, device=dev) * 0.05) if glu else (cb, scb)
+        x = torch.randn(K, device=dev).bfloat16()
+        g = (torch.rand(K, device=dev) + 0.5).bfloat16()
+        y = torch.empty(N, device=dev, dtype=torch.bfloat16)
+        a = L.Q8LinearArgs(x=x.data_ptr(), cb=cb.data_ptr(), scb=scb.data_ptr(), cb2=cb2.data_ptr(), scb2=scb2.data_ptr(),
+                           y=y.data_ptr(), N=N, K=K, threshold=6.0, prologue=L.PRO_NONE if K > 8192 else L.PRO_RMSNORM,
+                           norm_scale=g.data_ptr(), eps=1e-5, epilogue=L.EPI_SWIGLU if glu else L.EPI_STORE, flags=L.F_PDL)
+        fused = _time_graph(lambda: lib.b2l_q8_linear(ctypes.byref(a), L.stream_ptr()), 200)
+        cbs = [(cb, scb)] + ([(cb2, scb2)] if glu else [])
+        module = _time_graph(lambda: [lib.b2l_q8_gemv_cb(x.data_ptr(), c.data_ptr(), s.data_ptr(), None, y.data_ptr(), N, K, 6.0, 0,
+                                                         L.stream_ptr()) for c, s in cbs], 200)
+        nw = N * (2 if glu else 1)
+        qw = torch.randint(0, 256, (K, nw), dtype=torch.uint8, device=dev)
+        qt = tile_i8(qw, nw, K, 8)
+        sc, z = torch.rand(nw, device=dev).bfloat16(), torch.full((nw,), 128.0, device=dev).bfloat16()
+        y2 = torch.empty(nw, device=dev, dtype=torch.bfloat16)
+        w8 = None
+        if K <= 24576:
+            wa = L.Q4LinearArgs(x=x.data_ptr(), ldx=K, qw_tiled=qt.data_ptr(), scales=sc.data_ptr(), zeros=z.data_ptr(), sz_dtype=0,
+                                y=y2.data_ptr(), ldy=nw, M=1, N=nw, K=K, flags=L.F_PDL)
+            w8 = _time_graph(lambda: lib.b2l_w8_gemv(ctypes.byref(wa), L.stream_ptr()), 200)
+        gb = nw * K / 1e3
+        print(f"{name:15s} N={nw:6d} K={K:6d}: q8_linear {fused:7.1f} us {gb / fused:6.0f} GB/s | q8_gemv_cb x{len(cbs)} {module:7.1f} us "
+              f"{gb / module:6.0f} GB/s" + (f" | w8_gemv {w8:7.1f} us {gb / w8:6.0f} GB/s" if w8 else ""), flush=True)
+        del cb, cb2, qw, qt
+        torch.cuda.empty_cache()
+
+
+def sec_bench_step_q8():
+    """llm.int8 batch-1 decode at ctx ~2000: the B2L_F_Q8 step (LLaMA.int8_step) against the module path (both replayed
+    as CUDA graphs), alternated over 3 rounds in one process, for the sizes in B2L_INT8_SIZES (default 7B,65B) and for
+    7B with a LLaMA-Adapter v1 prefix (aT = 10, start layer 2).  The last token's logits must be bit-identical."""
+    import torch
+    import lit_llama_b200 as P
+    from lit_llama_b200 import adapter as PA
+    from lit_llama_b200.utils import quantization
+
+    dev = torch.device("cuda")
+    print(_card(), flush=True)
+    S = 2048
+    runs = [(n, False) for n in os.environ.get("B2L_INT8_SIZES", "7B,65B").split(",")] + [("7B", True)]
+    for name, adapter in runs:
+        prev = torch.get_default_dtype()
+        torch.set_default_dtype(torch.bfloat16)
+        try:
+            with torch.device(dev), quantization("llm.int8"):
+                if adapter:
+                    model = PA.LLaMA(PA.LLaMAConfig(**dict(P.LLaMAConfig.from_name(name).__dict__, adapter_prompt_length=10,
+                                                            adapter_start_layer=2)))
+                    for blk in model.transformer.h:
+                        if hasattr(blk.attn, "gating_factor"):
+                            blk.attn.gating_factor.data.fill_(0.5)
+                else:
+                    model = P.LLaMA.from_name(name)
+        finally:
+            torch.set_default_dtype(prev)
+        model.eval()
+        model.copy_logits = False
+        torch.cuda.reset_peak_memory_stats()
+        us = {True: [], False: []}
+        logits = {}
+        for _ in range(3):
+            for fused in (True, False):
+                model.int8_step = fused
+                model.reset_cache()
+                with torch.no_grad():
+                    model(torch.randint(0, 32000, (1, 16), device=dev, dtype=torch.int32), S, torch.arange(16, device=dev))
+                torch.manual_seed(0)
+                us[fused].append(_decode_us(model, 1, S, dev, p0=2000, n=24))
+                assert (model._decode is not None) == fused
+                with torch.no_grad():
+                    logits[fused] = model(torch.tensor([[1234]], device=dev, dtype=torch.int32), S,
+                                          torch.tensor([2040], device=dev)).clone()
+        fmt = lambda v: " ".join(f"{u:.1f}" for u in v)
+        print(f"{name}{' adapter' if adapter else ''} llm.int8 decode B=1 ctx~2000: fused step {fmt(us[True])} us/token | module path "
+              f"{fmt(us[False])} us/token | logits bit-identical: {torch.equal(logits[True], logits[False])} | "
+              f"peak {torch.cuda.max_memory_allocated() / 2**30:.2f} GiB", flush=True)
+        del model
+        torch.cuda.empty_cache()
+
+
 def main():
     which = sys.argv[1:] or SECTIONS
     if len(which) == 1 and os.environ.get("B2L_DIAG_CHILD") == "1":
