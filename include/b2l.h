@@ -146,9 +146,12 @@ enum {
   B2L_F_ATTN_UNFUSED = 8, /* debug: force the three-kernel attention path for T == 1   */
   B2L_F_DEBUG_NOCOMPUTE = 16, /* debug: b2l_q4_gemv streams the weights but skips the math */
   B2L_F_W8 = 32,        /* b2l_decode_step: every linear is gptq.int8, qw_mma from b2l_w8_tile_i8
-                           (b2l_w8_gemv); B == 1 and no plan only                     */
-  B2L_F_Q8 = 64         /* b2l_decode_step: every linear is llm.int8 (b2l_decode_args::q8_layers / q8_lm_head,
+                           (b2l_w8_gemv); B == 1 (2..16 with B2L_F_W8_BATCH), no plan */
+  B2L_F_Q8 = 64,        /* b2l_decode_step: every linear is llm.int8 (b2l_decode_args::q8_layers / q8_lm_head,
                            b2l_q8_linear); B == 1, no plan, not with B2L_F_W8          */
+  B2L_F_W8_BATCH = 128  /* b2l_decode_step with B2L_F_W8 at B in 2..16: every linear runs b2l_w8_gemv_batch on
+                           the b2l_w8_tile_i8 tilings in qw_mma; batch_work must hold
+                           b2l_w8_gemv_batch_workspace_bytes(max K, B) bytes; no plan, no affines */
 };
 
 /* Fused [RMSNorm ->] int4 linear [-> residual | SwiGLU] on wgmma (M <= 16).  Replaces
@@ -188,6 +191,18 @@ size_t b2l_w8_tiled_i8_bytes(int N, int K);
 int b2l_w8_tile_i8(const void* qw, void* qw_tiled, int N, int K, b2l_stream_t stream);
 int b2l_w8_untile_i8(const void* qw_tiled, void* qw, int N, int K, b2l_stream_t stream);
 int b2l_w8_gemv(const b2l_q4_linear_args* args, b2l_stream_t stream);
+
+/* gptq.int8 for 2..16 activation rows (batched decode) on the same resident tiling (qw_tiled from b2l_w8_tile_i8)
+ * and in the same exact integer form as b2l_w8_gemv: every row is scaled, rounded and split into three base-256
+ * digit planes as b2l_w8_gemv does it, and the 3 M planes are the columns of mma.m16n8k32.  Row n of y is
+ * bit-identical to b2l_w8_gemv on row n alone (csrc/w8_gemv_batch.cu).  Same argument block, prologues, epilogues
+ * and split_k grid override as b2l_w8_gemv, plus: x [M, K] with leading dimension ldx (ldx >= K, ldx % 8 == 0), y
+ * and res with ldy / ldres, and `workspace`, b2l_w8_gemv_batch_workspace_bytes(K, M) bytes of 16-byte aligned device
+ * scratch (may be shared by all launches of one stream).  M in 2..16, K % 64 == 0, K <= 24576, flags 0 or B2L_F_PDL,
+ * out_affine must be unset.  Two launches: the rows' digit planes are built once (w8_batch_prep_kernel), then
+ * streamed stage by stage next to the weights (w8_gemv_batch_kernel). */
+size_t b2l_w8_gemv_batch_workspace_bytes(int K, int M);
+int b2l_w8_gemv_batch(const b2l_q4_linear_args* args, b2l_stream_t stream);
 
 /* gptq.int8 for M >= 1 rows (meant for M >= 2: prompts, batched decode) on the wgmma GEMM of b2l_q4_gemm: the
  * producers dequantise the 8-bit levels with get_weight's roundings, so the tensor core multiplies exactly
@@ -472,7 +487,8 @@ int b2l_kv_unroll(const void* cache, const int32_t* ring_start, void* out, int B
 typedef struct b2l_q4_weight {
   const void* qw_tiled;   /* b2l_q4_tile layout (wgmma kernel), used when B > 1; may be NULL if B == 1 */
   const void* qw_mma;     /* mma.sync kernels: b2l_q4_tile_i8 layout when B == 1 (b2l_q4_gemv), b2l_q4_tile_mma
-                             layout when B in 2..8 (b2l_q4_gemv_batch); may be NULL if B > 8 */
+                             layout when B in 2..8 (b2l_q4_gemv_batch); may be NULL if B > 8.  B2L_F_W8:
+                             b2l_w8_tile_i8 layout at B == 1 and, with B2L_F_W8_BATCH, at B = 2..16 */
   const void* scales;
   const void* zeros;
   int N, K;
@@ -535,7 +551,9 @@ typedef struct b2l_decode_args {
                                 [(5*n_layer+1)*16] per-op stamps of the persistent kernel   */
   void* batch_work;          /* B in 2..8: scratch of b2l_q4_gemv_batch_workspace_bytes(max K) bytes; the
                                 linears then run on the mma.sync batch kernel (weights need qw_mma).
-                                NULL: wgmma kernel (weights need qw_tiled)                */
+                                NULL: wgmma kernel (weights need qw_tiled).
+                                B2L_F_W8 | B2L_F_W8_BATCH: b2l_w8_gemv_batch_workspace_bytes(max K, B) bytes
+                                (required)                                                */
   void* plan;                /* B == 1, head_size 128: device buffer of b2l_decode_plan_bytes() bytes prepared by
                                 b2l_decode_plan_build -> the whole step runs as ONE persistent kernel
                                 (csrc/decode_mega.cu; weights need the b2l_q4_tile_i8 layout in qw_mma).

@@ -10,7 +10,9 @@ Two execution paths behind `LLaMA.forward`:
   * decode (T == 1 with a KV cache, every Linear a gptq.int4 layer with one (scale, zero) per row):
     one C call enqueues the whole token (`b2l_decode_step`: int8-MMA GEMV kernels for batch 1, f16-MMA for 2..8 rows,
     wgmma for 9..16), replayed as a CUDA graph.  Every Linear a per-row gptq.int8 layer: the same step at batch 1
-    (B2L_F_W8: the GEMV kernel with 8-bit weights); batches of 2 or more go module by module (on the wgmma GEMM).
+    (B2L_F_W8: the GEMV kernel with 8-bit weights); batches of 2 or more go module by module (on the wgmma GEMM),
+    or, with `LLaMA.w8_batch_step` (B2L_W8_BATCH_STEP=1), batches of 2..16 run the same step (B2L_F_W8_BATCH:
+    b2l_w8_gemv_batch on the resident batch-1 tilings, each row bit-identical to the batch-1 kernel on that row).
     Every Linear an llm.int8 layer, with `LLaMA.int8_step` (B2L_INT8_STEP=1): the same step at batch 1 (B2L_F_Q8:
     b2l_q8_linear reading CB / SCB in place), bit-identical to the module path.
   * everything else (prefill on the wgmma GEMM, no-cache forward, other Linear kinds): module by module.
@@ -289,18 +291,25 @@ class _DecodeState:
         from .quantization import BATCH_GEMV, batch_workspace
 
         # batch 1..8: mma.sync kernels (q4_gemv / q4_gemv_batch) and their tiling; 9..16: wgmma kernel and its tiling.
-        # gptq.int8 (batch 1 only): the batch-1 kernel with 8-bit weights (b2l_w8_tile_i8 tilings)
+        # gptq.int8: the batch-1 kernel with 8-bit weights (b2l_w8_tile_i8 tilings); with `w8_batch_step`, batches of
+        # 2..16 run b2l_w8_gemv_batch on the same resident tilings (B2L_F_W8_BATCH)
         w8 = model._fast_ok == "w8"
+        w8b = w8 and B > 1
         # llm.int8 (batch 1 only): b2l_q8_linear on every weight's CB / SCB in place (no copy, no tiling)
         q8 = model._fast_ok == "q8"
-        assert B == 1 or not (w8 or q8)
-        gemv = (B == 1) or (B <= 8 and BATCH_GEMV)
+        assert B == 1 or not q8
+        assert not w8b or (model.w8_batch_step and B <= 16)
+        gemv = (B == 1) or w8b or (B <= 8 and BATCH_GEMV)
+        i8 = B == 1 or w8b    # the b2l_q4_tile_i8 / b2l_w8_tile_i8 tilings (the resident copy of a compacted model)
         self.batch_ws = None
-        if gemv and B > 1:
+        if w8b:
+            nb = lib.b2l_w8_gemv_batch_workspace_bytes(max(C_, n_hidden), B)
+            self.batch_ws = torch.empty(nb, dtype=torch.uint8, device=device)
+        elif gemv and B > 1:
             self.batch_ws = batch_workspace(device, max(C_, n_hidden))
 
         def q4(lin: ColBlockQuantizedLinear) -> L.Q4Weight:
-            t = (lin.tiled_i8() if B == 1 else lin.tiled_mma()) if gemv else lin.tiled()
+            t = (lin.tiled_i8() if i8 else lin.tiled_mma()) if gemv else lin.tiled()
             self.keep.append(t)   # a compacted layer hands out transient tilings: this state owns the ones it points at
             return L.Q4Weight(None if gemv else t.data_ptr(), t.data_ptr() if gemv else None, lin.scales.data_ptr(),
                               lin.zeros.data_ptr(), lin.out_features, lin.in_features)
@@ -326,7 +335,7 @@ class _DecodeState:
                                          q8w(mlp.c_proj))
                 layers[i] = L.Layer(**rms, k_cache=k.data_ptr(), v_cache=v.data_ptr())
                 continue
-            fc12 = model._fc12(i, "i8" if B == 1 else ("mma" if gemv else "tc"))
+            fc12 = model._fc12(i, "i8" if i8 else ("mma" if gemv else "tc"))
             layers[i] = L.Layer(
                 **rms, c_attn=q4(blk.attn.c_attn), c_proj=q4(blk.attn.c_proj),
                 c_fc12=L.Q4Weight(None if gemv else fc12[0].data_ptr(), fc12[0].data_ptr() if gemv else None,
@@ -342,7 +351,8 @@ class _DecodeState:
             idx_is_i64=1 if idx_dtype == torch.int64 else 0, input_pos=self.pos.data_ptr(),
             ring_start=model._ring.data_ptr(), block_size=cfg.block_size, x=self.x.data_ptr(), qkv=self.qkv.data_ptr(),
             att=self.att.data_ptr(), hid=self.hid.data_ptr(), attn_work=self.work.data_ptr(),
-            logits=self.logits.data_ptr(), flags=model.decode_flags | (L.F_W8 if w8 else 0) | (L.F_Q8 if q8 else 0),
+            logits=self.logits.data_ptr(),
+            flags=model.decode_flags | (L.F_W8 if w8 else 0) | (L.F_W8_BATCH if w8b else 0) | (L.F_Q8 if q8 else 0),
             batch_work=None if self.batch_ws is None else self.batch_ws.data_ptr())
         if q8:
             self.q8_layers = q8_layers
@@ -397,6 +407,11 @@ class LLaMA(nn.Module):
     #: (b2l_decode_step under B2L_F_Q8: b2l_q8_linear with RMSNorm / residual / SwiGLU / affine fused), bit-identical
     #: to the module path.  Opt-in (B2L_INT8_STEP=1): by default llm.int8 decodes module by module.
     int8_step: bool = os.environ.get("B2L_INT8_STEP", "0") == "1"
+    #: batched (B = 2..16) decode of a gptq.int8 model (plain, LLaMA-Adapter v1 or LoRA) on the whole-token step
+    #: (b2l_decode_step under B2L_F_W8 | B2L_F_W8_BATCH: b2l_w8_gemv_batch on the resident batch-1 tilings, each row
+    #: bit-identical to b2l_w8_gemv on that row).  Opt-in (B2L_W8_BATCH_STEP=1): by default batched gptq.int8 decodes
+    #: module by module, on the wgmma GEMM.
+    w8_batch_step: bool = os.environ.get("B2L_W8_BATCH_STEP", "0") == "1"
 
     def __init__(self, config: LLaMAConfig) -> None:
         super().__init__()
@@ -689,9 +704,11 @@ class LLaMA(nn.Module):
             if st is None or st.B != B or st.S != max_seq_length or st.idx.dtype != idx.dtype or st.idx.device != idx.device:
                 if self._fast_ok is None:
                     self._fast_ok = self._fast_decode_ok()
-                # gptq.int8, llm.int8 and LLaMA-Adapter v2: batch 1 only; llm.int8 on request (int8_step)
+                # gptq.int8, llm.int8 and LLaMA-Adapter v2: batch 1 only; llm.int8 on request (int8_step); gptq.int8
+                # without v2 affines at batch 2..16 on request (w8_batch_step)
                 fast = (bool(self._fast_ok) and (self._fast_ok != "q8" or self.int8_step)
-                        and (B == 1 or (self._fast_ok not in ("w8", "q8") and not self._has_affines())))
+                        and (B == 1 or (self._fast_ok not in ("w8", "q8") and not self._has_affines())
+                             or (self._fast_ok == "w8" and self.w8_batch_step and not self._has_affines())))
                 st = self._decode = _DecodeState(self, B, max_seq_length, idx.device, idx.dtype) if fast else None
         if st is not None:
             st.idx.copy_(idx.reshape(-1))

@@ -1756,6 +1756,114 @@ def sec_bench_step_q8():
         torch.cuda.empty_cache()
 
 
+def sec_bench_w8_batch():
+    """gptq.int8 at 2..16 rows: b2l_w8_gemv_batch (resident b2l_w8_tile_i8 tiling, fused prologue / epilogue as in the
+    step) at M = 2, 4, 8, 16 next to b2l_w8_gemv at M = 1 and b2l_w8_gemm (the module path's GEMM, reference-layout
+    levels) at the same M, for the 7B / 13B / 65B linears.  us per launch: 200 launches in a CUDA graph, PDL on for the
+    fused kernels, the weights rotated over enough copies (>= 200 MB) that no launch finds them in the 50 MB L2.  GB/s
+    counts N K bytes of levels per launch (the batch kernel also reads 3 M K bytes of digits, from L2)."""
+    import ctypes
+
+    import torch
+    from lit_llama_b200 import _lib as L
+    from lit_llama_b200.quantization import tile_i8
+
+    dev = torch.device("cuda")
+    lib = L.lib()
+    print(_card(), flush=True)
+    # (name, N, K, prologue, epilogue): fused as b2l_decode_step fuses them
+    R, NO, ST, RE, SW = L.PRO_RMSNORM, L.PRO_NONE, L.EPI_STORE, L.EPI_RESIDUAL, L.EPI_SWIGLU
+    shapes = [("7B c_attn", 12288, 4096, R, ST), ("7B attn.c_proj", 4096, 4096, NO, RE), ("7B fc1|fc2", 22016, 4096, R, SW),
+              ("7B mlp.c_proj", 4096, 11008, NO, RE), ("7B lm_head", 32000, 4096, R, ST),
+              ("13B c_attn", 15360, 5120, R, ST), ("13B attn.c_proj", 5120, 5120, NO, RE), ("13B fc1|fc2", 27648, 5120, R, SW),
+              ("13B mlp.c_proj", 5120, 13824, NO, RE), ("13B lm_head", 32000, 5120, R, ST),
+              ("65B c_attn", 24576, 8192, R, ST), ("65B attn.c_proj", 8192, 8192, NO, RE), ("65B fc1|fc2", 44032, 8192, R, SW),
+              ("65B mlp.c_proj", 8192, 22016, NO, RE), ("65B lm_head", 32000, 8192, R, ST)]
+    for name, N, K, pro, epi in shapes:
+        ncopy = max(2, -(-200_000_000 // (N * K)))
+        sc = (torch.rand(N, device=dev) * 0.01 + 0.002).bfloat16()
+        z = torch.randint(96, 160, (N,), device=dev).bfloat16()
+        g = (torch.rand(K, device=dev) + 0.5).bfloat16()
+        ref = [torch.randint(0, 256, (K, N), device=dev, dtype=torch.uint8).t() for _ in range(ncopy)]
+        til = [tile_i8(q, N, K, 8) for q in ref]
+        n_out = N // 2 if epi == SW else N
+        line = f"{name:16s} N={N:6d} K={K:6d}:"
+        for M in (1, 2, 4, 8, 16):
+            x = torch.randn(M, K, device=dev).bfloat16()
+            y = torch.empty(M, n_out, device=dev, dtype=torch.bfloat16)
+            res = torch.randn(M, N, device=dev).bfloat16()
+            ws = torch.empty(max(16, lib.b2l_w8_gemv_batch_workspace_bytes(K, M)), dtype=torch.uint8, device=dev)
+            fused = [L.Q4LinearArgs(x=x.data_ptr(), ldx=K, qw_tiled=t.data_ptr(), scales=sc.data_ptr(), zeros=z.data_ptr(),
+                                    sz_dtype=L.B2L_BF16, y=y.data_ptr(), ldy=n_out, M=M, N=N, K=K, prologue=pro,
+                                    norm_scale=g.data_ptr(), eps=1e-5, epilogue=epi, res=res.data_ptr(), ldres=N, flags=L.F_PDL,
+                                    workspace=ws.data_ptr()) for t in til]
+            fn = lib.b2l_w8_gemv if M == 1 else lib.b2l_w8_gemv_batch
+            uf = _time_graph(lambda: [L.check(fn(ctypes.byref(fused[i % ncopy]), L.stream_ptr()), "w8 fused") for i in range(200)], 1) / 200
+            line += f" | M={M} {'w8_gemv' if M == 1 else 'batch'} {uf:7.1f} us {N * K / uf / 1e3:5.0f} GB/s"
+            if M > 1:
+                yg = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
+                gemm = [_w8_args(L, x, q, sc, z, N, K, yg, M=M) for q in ref]
+                ug = _time_graph(lambda: [L.check(lib.b2l_w8_gemm(ctypes.byref(gemm[i % ncopy]), L.stream_ptr()), "w8 gemm")
+                                          for i in range(40)], 1) / 40
+                line += f" gemm {ug:7.1f} us"
+        print(line, flush=True)
+        del ref, til
+        torch.cuda.empty_cache()
+
+
+def sec_bench_step_w8_batch():
+    """Batched gptq.int8 decode: the B2L_F_W8_BATCH step (LLaMA.w8_batch_step) against the module path (b2l_w8_gemm per
+    linear), both replayed as CUDA graphs, at B = 1, 2, 4, 8, 16 on random-level compacted models (B2L_W8_BATCH_SIZES,
+    default 7B,65B), after a 512-token prompt, alternated over 3 rounds in one process.  B = 1 runs the batch-1 step
+    in both arms.  65B keeps max_seq_length at 576 so that the KV cache of 8 sequences fits beside its 62 GiB of
+    weights; 16 sequences do not fit and are skipped, and 8 timed tokens per round (24 at 7B) keep the module path's
+    rounds short.  Prints us per token, GB/s of levels per token, the largest
+    per-row relative logits difference between the two paths and the peak memory."""
+    import torch
+    from lit_llama_b200.quantization import ColBlockQuantizedLinear
+
+    dev = torch.device("cuda")
+    print(_card(), flush=True)
+    S = 576
+    for name in os.environ.get("B2L_W8_BATCH_SIZES", "7B,65B").split(","):
+        model = _random_w8_model(name, dev, seed=8)
+        model.copy_logits = False
+        model.compact()
+        gc.collect()
+        torch.cuda.empty_cache()
+        levels = sum(m.out_features * m.in_features for m in model.modules() if isinstance(m, ColBlockQuantizedLinear))
+        for B in (1, 2, 4, 8, 16):
+            if name == "65B" and B > 8:
+                print(f"{name} B={B}: skipped (the KV cache does not fit beside the weights)", flush=True)
+                continue
+            torch.cuda.reset_peak_memory_stats()
+            us = {True: [], False: []}
+            logits = {}
+            g = torch.Generator(device=dev).manual_seed(B)
+            prompt = torch.randint(0, 32000, (B, 512), device=dev, dtype=torch.int32, generator=g)
+            for _ in range(3):
+                for step in (True, False):
+                    model.w8_batch_step = step
+                    model.reset_cache()
+                    with torch.no_grad():
+                        model(prompt, S, torch.arange(512, device=dev))
+                    torch.manual_seed(0)
+                    us[step].append(_decode_us(model, B, S, dev, p0=512, n=8 if name == "65B" else 24))
+                    assert (model._decode is not None) == (step or B == 1), (name, B, step)
+                    with torch.no_grad():
+                        logits[step] = model(torch.arange(B, device=dev, dtype=torch.int32).view(B, 1) + 7, S,
+                                             torch.tensor([542], device=dev)).float().clone()
+            a, b = logits[True].reshape(B, -1), logits[False].reshape(B, -1)
+            diff = max(float((a[n] - b[n]).norm() / b[n].norm()) for n in range(B))
+            fmt = lambda v: " ".join(f"{u:.0f}" for u in v)   # noqa: E731
+            print(f"{name} gptq.int8 decode B={B:2d} ctx~512-542: step {fmt(us[True])} us/token "
+                  f"({levels / min(us[True]) / 1e3:.0f} GB/s) | module path {fmt(us[False])} us/token | "
+                  f"max row rel. diff {diff:.2e} | peak {torch.cuda.max_memory_allocated() / 2**30:.2f} GiB", flush=True)
+        del model
+        gc.collect()
+        torch.cuda.empty_cache()
+
+
 def main():
     which = sys.argv[1:] or SECTIONS
     if len(which) == 1 and os.environ.get("B2L_DIAG_CHILD") == "1":
