@@ -149,9 +149,13 @@ enum {
                            (b2l_w8_gemv); B == 1 (2..16 with B2L_F_W8_BATCH), no plan */
   B2L_F_Q8 = 64,        /* b2l_decode_step: every linear is llm.int8 (b2l_decode_args::q8_layers / q8_lm_head,
                            b2l_q8_linear); B == 1, no plan, not with B2L_F_W8          */
-  B2L_F_W8_BATCH = 128  /* b2l_decode_step with B2L_F_W8 at B in 2..16: every linear runs b2l_w8_gemv_batch on
+  B2L_F_W8_BATCH = 128, /* b2l_decode_step with B2L_F_W8 at B in 2..16: every linear runs b2l_w8_gemv_batch on
                            the b2l_w8_tile_i8 tilings in qw_mma; batch_work must hold
                            b2l_w8_gemv_batch_workspace_bytes(max K, B) bytes; no plan, no affines */
+  B2L_F_Q4_BATCH_I8 = 256 /* b2l_decode_step (gptq.int4) at B in 2..16: every linear runs b2l_q4_gemv_batch_i8 on
+                           the b2l_q4_tile_i8 tilings in qw_mma; batch_work must hold
+                           b2l_w8_gemv_batch_workspace_bytes(max K, B) bytes; not with B2L_F_W8, B2L_F_Q8 or
+                           B2L_F_W8_BATCH; no plan, no affines */
 };
 
 /* Fused [RMSNorm ->] int4 linear [-> residual | SwiGLU] on wgmma (M <= 16).  Replaces
@@ -203,6 +207,15 @@ int b2l_w8_gemv(const b2l_q4_linear_args* args, b2l_stream_t stream);
  * streamed stage by stage next to the weights (w8_gemv_batch_kernel). */
 size_t b2l_w8_gemv_batch_workspace_bytes(int K, int M);
 int b2l_w8_gemv_batch(const b2l_q4_linear_args* args, b2l_stream_t stream);
+
+/* gptq.int4 for 2..16 activation rows (batched decode) on the resident batch-1 tiling (qw_tiled from b2l_q4_tile_i8)
+ * and in b2l_q4_gemv's exact integer form: the kernel above with 4-bit levels, each packed byte fed to the MMA as
+ * b2l_q4_gemv does (unmasked for row g, high nibble for row g + 8) and the row pair recovered from the two results.
+ * Row n of y is bit-identical to b2l_q4_gemv on row n alone.  Same argument block, checks, prologues, epilogues and
+ * split_k grid override as b2l_w8_gemv_batch; the digit planes are the same, so `workspace` is
+ * b2l_w8_gemv_batch_workspace_bytes(K, M) bytes.  M in 2..16, K % 64 == 0, K <= 24576, flags 0 or B2L_F_PDL,
+ * out_affine must be unset.  Two launches (w8_batch_prep_kernel, then w8_gemv_batch_kernel<.., false>). */
+int b2l_q4_gemv_batch_i8(const b2l_q4_linear_args* args, b2l_stream_t stream);
 
 /* gptq.int8 for M >= 1 rows (meant for M >= 2: prompts, batched decode) on the wgmma GEMM of b2l_q4_gemm: the
  * producers dequantise the 8-bit levels with get_weight's roundings, so the tensor core multiplies exactly
@@ -488,7 +501,8 @@ typedef struct b2l_q4_weight {
   const void* qw_tiled;   /* b2l_q4_tile layout (wgmma kernel), used when B > 1; may be NULL if B == 1 */
   const void* qw_mma;     /* mma.sync kernels: b2l_q4_tile_i8 layout when B == 1 (b2l_q4_gemv), b2l_q4_tile_mma
                              layout when B in 2..8 (b2l_q4_gemv_batch); may be NULL if B > 8.  B2L_F_W8:
-                             b2l_w8_tile_i8 layout at B == 1 and, with B2L_F_W8_BATCH, at B = 2..16 */
+                             b2l_w8_tile_i8 layout at B == 1 and, with B2L_F_W8_BATCH, at B = 2..16.
+                             B2L_F_Q4_BATCH_I8: b2l_q4_tile_i8 layout at B = 2..16 too */
   const void* scales;
   const void* zeros;
   int N, K;
@@ -552,8 +566,8 @@ typedef struct b2l_decode_args {
   void* batch_work;          /* B in 2..8: scratch of b2l_q4_gemv_batch_workspace_bytes(max K) bytes; the
                                 linears then run on the mma.sync batch kernel (weights need qw_mma).
                                 NULL: wgmma kernel (weights need qw_tiled).
-                                B2L_F_W8 | B2L_F_W8_BATCH: b2l_w8_gemv_batch_workspace_bytes(max K, B) bytes
-                                (required)                                                */
+                                B2L_F_W8 | B2L_F_W8_BATCH and B2L_F_Q4_BATCH_I8:
+                                b2l_w8_gemv_batch_workspace_bytes(max K, B) bytes (required) */
   void* plan;                /* B == 1, head_size 128: device buffer of b2l_decode_plan_bytes() bytes prepared by
                                 b2l_decode_plan_build -> the whole step runs as ONE persistent kernel
                                 (csrc/decode_mega.cu; weights need the b2l_q4_tile_i8 layout in qw_mma).

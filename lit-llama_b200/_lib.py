@@ -16,6 +16,7 @@ F_PDL, F_NO_ALIAS_N, F_ROPE_ROWS = 1, 2, 4
 F_W8 = 32   # b2l_decode_step: every linear is gptq.int8 (b2l_w8_gemv)
 F_Q8 = 64   # b2l_decode_step: every linear is llm.int8 (b2l_q8_linear)
 F_W8_BATCH = 128   # b2l_decode_step with F_W8 at B in 2..16: every linear runs b2l_w8_gemv_batch
+F_Q4_BATCH_I8 = 256   # b2l_decode_step (gptq.int4) at B in 2..16: every linear runs b2l_q4_gemv_batch_i8
 
 c_void_p, c_int, c_float, c_size_t = C.c_void_p, C.c_int, C.c_float, C.c_size_t
 
@@ -147,6 +148,7 @@ _SIGS = {
     "b2l_w8_gemm": (c_int, [C.POINTER(Q4LinearArgs), c_void_p]),
     "b2l_w8_gemv_batch": (c_int, [C.POINTER(Q4LinearArgs), c_void_p]),
     "b2l_w8_gemv_batch_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "b2l_q4_gemv_batch_i8": (c_int, [C.POINTER(Q4LinearArgs), c_void_p]),
     "b2l_nll_workspace_bytes": (c_size_t, [c_int, c_int]),
     "b2l_q4_gemm_nll": (c_int, [C.POINTER(Q4LinearArgs), C.POINTER(NLLArgs), c_void_p]),
     "b2l_w8_gemm_nll": (c_int, [C.POINTER(Q4LinearArgs), C.POINTER(NLLArgs), c_void_p]),

@@ -146,6 +146,11 @@ static int q4_call(const b2l_q4_weight& w, const void* x, int ldx, void* y, int 
   a.split_k = 0;
   a.flags = flags;
   a.trace = gemv ? trace : nullptr;
+  if ((flags & B2L_F_Q4_BATCH_I8) && M > 1) {   // gptq.int4 at 2..16 rows on the batch-1 b2l_q4_tile_i8 tiling
+    a.qw_tiled = w.qw_mma; a.trace = nullptr; a.workspace = batch_work;
+    a.flags = flags & B2L_F_PDL;
+    return b2l_q4_gemv_batch_i8(&a, stream);
+  }
   if (flags & B2L_F_W8) {   // gptq.int8: batch 1, or 2..16 under B2L_F_W8_BATCH (checked by b2l_decode_step)
     if (M > 1) {            // the batch kernel on the same b2l_w8_tile_i8 tiling
       a.qw_tiled = w.qw_mma; a.trace = nullptr; a.workspace = batch_work;
@@ -215,9 +220,10 @@ extern "C" int b2l_decode_step_launches(const b2l_decode_args* d) {
   // fused single-token attention for head_size 128 (B2L_F_ATTN_UNFUSED: the three-kernel path)
   const bool fused = d->n_embd / d->n_head == 128 && !(d->flags & B2L_F_ATTN_UNFUSED);
   const int attn = fused ? 1 : 3;
-  // the batch kernels (int4 at 2..8 rows, gptq.int8 at 2..16) are two launches per linear
-  const bool w8b = (d->flags & B2L_F_W8_BATCH) && d->B > 1 && d->B <= 16 && d->batch_work;
-  const int lin = (w8b || (d->B > 1 && d->B <= 8 && d->batch_work)) ? 2 : 1;
+  // the batch kernels (int4 at 2..8 rows, gptq.int8 and, under B2L_F_Q4_BATCH_I8, int4 at 2..16) are two launches
+  // per linear
+  const bool b16 = (d->flags & (B2L_F_W8_BATCH | B2L_F_Q4_BATCH_I8)) && d->B > 1 && d->B <= 16 && d->batch_work;
+  const int lin = (b16 || (d->B > 1 && d->B <= 8 && d->batch_work)) ? 2 : 1;
   int n = 2 + d->n_layer * (4 * lin + attn) + lin;  // ring advance + embedding, per Block 4 linears + attention, ln_f+lm_head
   // an adapter layer adds the prefix kernel behind the three-kernel attention (the fused kernel does it in-launch)
   if (!fused && d->adapters != nullptr)
@@ -236,6 +242,15 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
   B2L_CHECK_ARG(d->wte && d->ln_f && d->rope && d->idx && d->input_pos && d->ring_start && d->x && d->qkv && d->att &&
                     d->hid && d->attn_work && d->logits,
                 "b2l_decode_step: null pointer");
+  if (d->flags & B2L_F_Q4_BATCH_I8) {
+    B2L_CHECK_SUPPORTED(!(d->flags & (B2L_F_W8 | B2L_F_Q8 | B2L_F_W8_BATCH)),
+                        "b2l_decode_step: B2L_F_Q4_BATCH_I8 (gptq.int4) does not combine with B2L_F_W8, B2L_F_Q8 or B2L_F_W8_BATCH");
+    B2L_CHECK_SUPPORTED(d->B >= 2 && d->B <= 16, "b2l_decode_step: B2L_F_Q4_BATCH_I8 runs batches of 2..16, got B=%d", d->B);
+    B2L_CHECK_SUPPORTED(d->plan == nullptr, "b2l_decode_step: B2L_F_Q4_BATCH_I8 does not run in the persistent kernel (plan must be NULL)");
+    B2L_CHECK_SUPPORTED(d->affines == nullptr && d->lm_head_affine.scale == nullptr && d->lm_head_affine.bias == nullptr,
+                        "b2l_decode_step: B2L_F_Q4_BATCH_I8 does not apply LLaMA-Adapter v2 affines (batch 1 only)");
+    B2L_CHECK_ARG(d->batch_work != nullptr, "b2l_decode_step: B2L_F_Q4_BATCH_I8 needs batch_work (b2l_w8_gemv_batch_workspace_bytes(max K, B) bytes)");
+  }
   const bool q8 = (d->flags & B2L_F_Q8) != 0;
   if (q8)
     if (int rc = check_q8(d)) return rc;
@@ -285,7 +300,7 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
   if (d->plan != nullptr) return decode_step_persistent(d, stream);   // one persistent kernel per token (decode_mega.cu)
   const int C = d->n_embd, hs = C / d->n_head, B = d->B;
   const int fl = d->flags;               // the linears' flags (q4_call routes B2L_F_W8 to b2l_w8_gemv)
-  const int afl = fl & ~(B2L_F_W8 | B2L_F_Q8 | B2L_F_W8_BATCH);   // everything else
+  const int afl = fl & ~(B2L_F_W8 | B2L_F_Q8 | B2L_F_W8_BATCH | B2L_F_Q4_BATCH_I8);   // everything else
   int rc;
   // debug timeline: launch i of the step writes uint64[64] at timeline + 512*i (order: per Block c_attn,
   // attention, c_proj, fc12, mlp_proj; then lm_head)

@@ -26,6 +26,17 @@
 //
 // Workspace (b2l_w8_gemv_batch_workspace_bytes): [K/64 k blocks][3M planes (row n digit d = plane 3n + d)][4 t][16 B]
 // in the batch-1 plane order, then int64 sum X [16] and int sh [16].
+//
+// gptq.int4 (b2l_q4_gemv_batch_i8) runs the same prep kernel, workspace, ring, reduction and epilogue with W8 = false,
+// on the resident batch-1 int4 tiling (b2l_q4_tile_i8, q4_gemv.cu): a (16-row block, k block) tile is 512 B of packed
+// nibbles, fed to the MMA as in single_imma<false> -- the unmasked word as the operand of row g, the word & 0xf0f0f0f0
+// as that of row g + 8, one LOP3 per word shared by every column group -- and each partial is turned back into the
+// row pair (row g = D[g] - D[g+8], row g + 8 = D[g+8] >> 4, exact and linear) before it is added into the unit's
+// buffer.  Stage geometry: still 8 k blocks per stage, one per consumer warp, so the 4-bit half stages are 4 KB.
+// Sixteen k blocks per stage (two per warp) would keep 8 KB half stages but halve the number of stages the same
+// shared memory holds; at 8 KB of weights per stage a 110 KB CTA still keeps >= 72 KB of weights in flight.  The
+// digits of a stage are the same 3 M x 512 B at either width, so per byte of weights streamed from HBM the kernel
+// reads 3 M / 16 bytes of digits from L2 at 4 bits (3 at M = 16) against 3 M / 32 at 8 bits.
 #include <cstdlib>
 
 #include "q4_mma_common.cuh"
@@ -36,15 +47,18 @@ using namespace q4mv;
 
 constexpr int MAXB = 16;                     // activation rows
 constexpr int NDIG = 3;                      // base-256 digits per row (|X| < 2^22)
-constexpr int W8_KB_BYTES = 1024;            // one (16-row block, k block) tile of 8-bit levels
-constexpr int KBP = HALF_STAGE_BYTES / W8_KB_BYTES;   // 8 k blocks per stage, one per consumer warp
+// one (16-row block, k block) tile: 1024 B of 8-bit levels (b2l_w8_tile_i8) or 512 B of packed nibbles (b2l_q4_tile_i8)
+__host__ __device__ constexpr int tile_bytes(bool w8) { return w8 ? 1024 : 512; }
+constexpr int KBP = HALF_STAGE_BYTES / tile_bytes(true);   // 8 k blocks per stage, one per consumer warp
 static_assert(KBP == NCW, "one k block per consumer warp and stage");
 constexpr int PLANE_KB_BYTES = 64;           // one digit plane of one k block: [4 t][16 B]
 constexpr int BMAX_STAGES = 12;
 constexpr int MAX_K = 12 * 256 * 8;          // 24576, as b2l_w8_gemv
 
 __host__ __device__ inline uint32_t xkb_bytes(int M) { return (uint32_t)(NDIG * M * PLANE_KB_BYTES); }   // digits of one k block
-__host__ __device__ inline uint32_t bstage_bytes(int M) { return STAGE_BYTES + KBP * xkb_bytes(M); }      // [weights][digits]
+// weights of a stage: KBP k blocks of both 16-row blocks of a unit (16 KB at 8 bits, 8 KB at 4 bits)
+__host__ __device__ constexpr uint32_t wstage_bytes(bool w8) { return (uint32_t)(2 * KBP * tile_bytes(w8)); }
+__host__ __device__ inline uint32_t bstage_bytes(int M, bool w8) { return wstage_bytes(w8) + KBP * xkb_bytes(M); }   // [weights][digits]
 __host__ __device__ inline int scratch_stride(int M) { return (NDIG * M) | 1; }   // ints per result row (odd: no bank conflicts)
 __host__ __device__ inline size_t frag_bytes(int K, int M) { return (size_t)NDIG * M * K; }
 
@@ -63,10 +77,10 @@ struct BParams {
 struct BSmem {
   uint32_t ring, scratch, rowc, bars, total;
 };
-__host__ __device__ inline BSmem bsmem_layout(int nst, int M) {
+__host__ __device__ inline BSmem bsmem_layout(int nst, int M, bool w8) {
   BSmem L;
   uint32_t o = 0;
-  L.ring = o;    o += (uint32_t)nst * bstage_bytes(M);
+  L.ring = o;    o += (uint32_t)nst * bstage_bytes(M, w8);
   L.scratch = o; o += (2u * 2 * RB * scratch_stride(M) * 4 + 15u) & ~15u;   // [buf][32 result rows][stride] int32
   L.rowc = o;    o += 2 * MAXB * 8;                                        // double[16] sum X, double[16] 2^-sh
   L.bars = o;    o += 2 * BMAX_STAGES * 8;
@@ -211,10 +225,12 @@ __global__ void __launch_bounds__(256) w8_batch_prep_kernel(const __nv_bfloat16*
 
 // ---------------------------------------------------------------- step 2: the streaming contraction
 // NG = ceil(3M / 8) column groups of the MMA.  Lane (g, t) of group G feeds column g = plane 8G + g (zero past 3M).
-template <int NG>
+// W8: 8-bit levels (b2l_w8_tile_i8); false: 4-bit levels (b2l_q4_tile_i8).
+template <int NG, bool W8>
 __global__ void __launch_bounds__(NTHREADS, NG <= 2 ? 2 : 1) w8_gemv_batch_kernel(const BParams p) {
+  constexpr uint32_t TILE = tile_bytes(W8), WHALF = KBP * TILE, WSTAGE = 2 * WHALF;
   extern __shared__ __align__(128) uint8_t smem[];
-  const BSmem L = bsmem_layout(p.nst, p.M);
+  const BSmem L = bsmem_layout(p.nst, p.M, W8);
   const uint32_t sbase = smem_u32(smem);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int n_kb = p.K / KB;
@@ -224,7 +240,7 @@ __global__ void __launch_bounds__(NTHREADS, NG <= 2 ? 2 : 1) w8_gemv_batch_kerne
   const int n_units = (rb_hi - rb_lo + 1) / 2;
   const int total_stages = n_units * spu;
   const uint32_t bar_full = sbase + L.bars, bar_empty = bar_full + BMAX_STAGES * 8;
-  const uint32_t SB = bstage_bytes(p.M), XKB = xkb_bytes(p.M);
+  const uint32_t SB = bstage_bytes(p.M, W8), XKB = xkb_bytes(p.M);
   const int NP = NDIG * p.M, RS = scratch_stride(p.M);
 
   if (tid == 0) {
@@ -246,16 +262,16 @@ __global__ void __launch_bounds__(NTHREADS, NG <= 2 ? 2 : 1) w8_gemv_batch_kerne
         const int rb = rb_lo + 2 * u;
         const int halves = min(2, rb_hi - rb);
         const int nkb = min(KBP, n_kb - s * KBP);
-        const uint32_t wbytes = (uint32_t)nkb * W8_KB_BYTES, xbytes = (uint32_t)nkb * XKB;
+        const uint32_t wbytes = (uint32_t)nkb * TILE, xbytes = (uint32_t)nkb * XKB;
         const uint32_t stage = sbase + L.ring + slot * SB;
         mbar_wait(bar_empty + slot * 8, phase);
         mbar_expect_tx(bar_full + slot * 8, wbytes * halves + xbytes);
-        const uint8_t* wsrc = p.qwt + (size_t)rb * n_kb * W8_KB_BYTES;
+        const uint8_t* wsrc = p.qwt + (size_t)rb * n_kb * TILE;
         for (int h = 0; h < halves; ++h)
-          tma_bulk_g2s(stage + h * HALF_STAGE_BYTES, wsrc + ((size_t)h * n_kb + (size_t)s * KBP) * W8_KB_BYTES, wbytes,
+          tma_bulk_g2s(stage + h * WHALF, wsrc + ((size_t)h * n_kb + (size_t)s * KBP) * TILE, wbytes,
                        bar_full + slot * 8);
         if (it >= pre) {
-          tma_bulk_g2s(stage + STAGE_BYTES, p.xfrag + (size_t)s * KBP * XKB, xbytes, bar_full + slot * 8);
+          tma_bulk_g2s(stage + WSTAGE, p.xfrag + (size_t)s * KBP * XKB, xbytes, bar_full + slot * 8);
         } else if (it + 1 == pre) {
           // ring full of weights: let the next kernel in, wait for the digits' producer, then request the digits of
           // every stage issued so far
@@ -266,7 +282,7 @@ __global__ void __launch_bounds__(NTHREADS, NG <= 2 ? 2 : 1) w8_gemv_batch_kerne
           for (int j = 0; j < pre; ++j) {
             const int uj = j / spu, sj = j - uj * spu;
             const int nkbj = min(KBP, n_kb - sj * KBP);
-            tma_bulk_g2s(sbase + L.ring + (j % p.nst) * SB + STAGE_BYTES, p.xfrag + (size_t)sj * KBP * XKB,
+            tma_bulk_g2s(sbase + L.ring + (j % p.nst) * SB + WSTAGE, p.xfrag + (size_t)sj * KBP * XKB,
                          (uint32_t)nkbj * XKB, bar_full + (j % p.nst) * 8);
           }
         }
@@ -296,23 +312,44 @@ __global__ void __launch_bounds__(NTHREADS, NG <= 2 ? 2 : 1) w8_gemv_batch_kerne
         mbar_wait(bar_full + slot * 8, phase);
         if (warp < nkb) {
           const uint8_t* st = smem + L.ring + slot * SB;
-          const uint8_t* wt = st + warp * W8_KB_BYTES + lane * 16;
-          const uint8_t* xs = st + STAGE_BYTES + warp * XKB;
-          const uint4 a0 = *reinterpret_cast<const uint4*>(wt), a1 = *reinterpret_cast<const uint4*>(wt + 512);
-          uint4 b0 = make_uint4(0, 0, 0, 0), b1 = b0;
-          if (halves == MAX_HALVES) {
-            b0 = *reinterpret_cast<const uint4*>(wt + HALF_STAGE_BYTES);
-            b1 = *reinterpret_cast<const uint4*>(wt + HALF_STAGE_BYTES + 512);
-          }
-#pragma unroll
-          for (int G = 0; G < NG; ++G) {
-            uint4 xb = make_uint4(0, 0, 0, 0);
-            if (xoff[G] >= 0) xb = *reinterpret_cast<const uint4*>(xs + xoff[G]);
-            mma_u8s8_16832(acc[G][0], a0.x, a0.y, a0.z, a0.w, xb.x, xb.y);
-            mma_u8s8_16832(acc[G][0], a1.x, a1.y, a1.z, a1.w, xb.z, xb.w);
+          const uint8_t* wt = st + warp * TILE + lane * 16;
+          const uint8_t* xs = st + WSTAGE + warp * XKB;
+          if constexpr (W8) {
+            const uint4 a0 = *reinterpret_cast<const uint4*>(wt), a1 = *reinterpret_cast<const uint4*>(wt + 512);
+            uint4 b0 = make_uint4(0, 0, 0, 0), b1 = b0;
             if (halves == MAX_HALVES) {
-              mma_u8s8_16832(acc[G][1], b0.x, b0.y, b0.z, b0.w, xb.x, xb.y);
-              mma_u8s8_16832(acc[G][1], b1.x, b1.y, b1.z, b1.w, xb.z, xb.w);
+              b0 = *reinterpret_cast<const uint4*>(wt + WHALF);
+              b1 = *reinterpret_cast<const uint4*>(wt + WHALF + 512);
+            }
+#pragma unroll
+            for (int G = 0; G < NG; ++G) {
+              uint4 xb = make_uint4(0, 0, 0, 0);
+              if (xoff[G] >= 0) xb = *reinterpret_cast<const uint4*>(xs + xoff[G]);
+              mma_u8s8_16832(acc[G][0], a0.x, a0.y, a0.z, a0.w, xb.x, xb.y);
+              mma_u8s8_16832(acc[G][0], a1.x, a1.y, a1.z, a1.w, xb.z, xb.w);
+              if (halves == MAX_HALVES) {
+                mma_u8s8_16832(acc[G][1], b0.x, b0.y, b0.z, b0.w, xb.x, xb.y);
+                mma_u8s8_16832(acc[G][1], b1.x, b1.y, b1.z, b1.w, xb.z, xb.w);
+              }
+            }
+          } else {
+            // a packed byte is level[g] + 16 level[g + 8]: unmasked for row g, high nibble only for row g + 8
+            constexpr uint32_t HI = 0xf0f0f0f0u;
+            const uint4 a = *reinterpret_cast<const uint4*>(wt);
+            uint4 b = make_uint4(0, 0, 0, 0);
+            if (halves == MAX_HALVES) b = *reinterpret_cast<const uint4*>(wt + WHALF);
+            const uint4 ah = make_uint4(a.x & HI, a.y & HI, a.z & HI, a.w & HI);
+            const uint4 bh = make_uint4(b.x & HI, b.y & HI, b.z & HI, b.w & HI);
+#pragma unroll
+            for (int G = 0; G < NG; ++G) {
+              uint4 xb = make_uint4(0, 0, 0, 0);
+              if (xoff[G] >= 0) xb = *reinterpret_cast<const uint4*>(xs + xoff[G]);
+              mma_u8s8_16832(acc[G][0], a.x, ah.x, a.y, ah.y, xb.x, xb.y);
+              mma_u8s8_16832(acc[G][0], a.z, ah.z, a.w, ah.w, xb.z, xb.w);
+              if (halves == MAX_HALVES) {
+                mma_u8s8_16832(acc[G][1], b.x, bh.x, b.y, bh.y, xb.x, xb.y);
+                mma_u8s8_16832(acc[G][1], b.z, bh.z, b.w, bh.w, xb.z, xb.w);
+              }
             }
           }
         }
@@ -320,7 +357,8 @@ __global__ void __launch_bounds__(NTHREADS, NG <= 2 ? 2 : 1) w8_gemv_batch_kerne
         if (lane == 0) mbar_arrive(bar_empty + slot * 8);
         if (++slot == p.nst) { slot = 0; phase ^= 1; }
       }
-      // 16 x 8 tile of group G: lane (g, t) holds rows g (c0, c1) and g + 8 (c2, c3) of columns 8G + 2t, 8G + 2t + 1
+      // 16 x 8 tile of group G: lane (g, t) holds rows g (c0, c1) and g + 8 (c2, c3) of columns 8G + 2t, 8G + 2t + 1.
+      // 4 bits: row g = D[g] - D[g+8], row g + 8 = D[g+8] >> 4 (every term of D[g+8] is a multiple of 16: exact)
       const int buf = u & 1;
       named_bar_sync(4 + buf, NCW * 32 + 32);   // the epilogue warp has read and cleared this buffer (two units ago)
       int* sb = scratch + buf * 2 * RB * RS;
@@ -332,8 +370,13 @@ __global__ void __launch_bounds__(NTHREADS, NG <= 2 ? 2 : 1) w8_gemv_batch_kerne
           if (h < halves) {
             int* r0 = sb + (h * RB + g) * RS + col;
             int* r8 = r0 + 8 * RS;
-            if (col < NP) { atomicAdd(r0, acc[G][h][0]); atomicAdd(r8, acc[G][h][2]); }
-            if (col + 1 < NP) { atomicAdd(r0 + 1, acc[G][h][1]); atomicAdd(r8 + 1, acc[G][h][3]); }
+            int c0 = acc[G][h][0], c1 = acc[G][h][1], c2 = acc[G][h][2], c3 = acc[G][h][3];
+            if constexpr (!W8) {
+              c0 -= c2; c1 -= c3;
+              c2 >>= 4; c3 >>= 4;
+            }
+            if (col < NP) { atomicAdd(r0, c0); atomicAdd(r8, c2); }
+            if (col + 1 < NP) { atomicAdd(r0 + 1, c1); atomicAdd(r8 + 1, c3); }
           }
         }
       }
@@ -404,39 +447,41 @@ extern "C" size_t b2l_w8_gemv_batch_workspace_bytes(int K, int M) {
 }
 
 namespace {
-template <int NG>
-int launch_batch(const BParams& p0, int grid_override, bool pdl, cudaStream_t stream) {
+template <int NG, bool W8>
+int launch_batch(const BParams& p0, int grid_override, bool pdl, cudaStream_t stream, const char* fn) {
   BParams p = p0;
   // 1..2 column groups (M <= 5): two CTAs per SM; more: one CTA per SM with a deeper ring
   const int ctas_per_sm = NG <= 2 ? 2 : 1;
   const uint32_t budget = (ctas_per_sm >= 2 ? 110u : 224u) * 1024u;
-  const uint32_t fixed = bsmem_layout(0, p.M).total, sb = bstage_bytes(p.M);
+  const uint32_t fixed = bsmem_layout(0, p.M, W8).total, sb = bstage_bytes(p.M, W8);
   int nst = fixed + 2 * sb <= budget ? (int)((budget - fixed) / sb) : 0;
   if (nst > BMAX_STAGES) nst = BMAX_STAGES;
   if (nst < 2) {
-    set_error("b2l_w8_gemv_batch: M=%d does not leave room for the weight ring", p.M);
+    set_error("%s: M=%d does not leave room for the weight ring", fn, p.M);
     return B2L_E_UNSUPPORTED;
   }
   p.nst = nst;
-  const BSmem L = bsmem_layout(nst, p.M);
+  const BSmem L = bsmem_layout(nst, p.M, W8);
   static DynSmemCache smem_cache;
-  if (int rc = ensure_dyn_smem(w8_gemv_batch_kernel<NG>, L.total, smem_cache)) return rc;
+  if (int rc = ensure_dyn_smem(w8_gemv_batch_kernel<NG, W8>, L.total, smem_cache)) return rc;
   int grid = grid_override > 0 ? grid_override : ctas_per_sm * sm_count();
   if (grid > p.n_rb) grid = p.n_rb;
   LaunchCfg lc(dim3(grid), dim3(NTHREADS), L.total, stream, pdl, 1);
-  B2L_CUDA(cudaLaunchKernelEx(&lc.cfg, w8_gemv_batch_kernel<NG>, p));
+  B2L_CUDA(cudaLaunchKernelEx(&lc.cfg, w8_gemv_batch_kernel<NG, W8>, p));
   return 0;
 }
-}  // namespace
 
-extern "C" int b2l_w8_gemv_batch(const b2l_q4_linear_args* a, b2l_stream_t stream) {
-  const char* fn = "b2l_w8_gemv_batch";
+// b2l_w8_gemv_batch (W8 = true) and b2l_q4_gemv_batch_i8 (W8 = false): the same checks, workspace and launches
+template <bool W8>
+int batch_entry(const b2l_q4_linear_args* a, b2l_stream_t stream) {
+  const char* fn = W8 ? "b2l_w8_gemv_batch" : "b2l_q4_gemv_batch_i8";
   B2L_CHECK_ARG(a != nullptr, "%s: null args", fn);
   B2L_CHECK_ARG(a->x && a->qw_tiled && a->scales && a->zeros && a->y, "%s: null pointer", fn);
   B2L_CHECK_ARG(a->workspace != nullptr, "%s: null workspace (b2l_w8_gemv_batch_workspace_bytes(K, M) bytes)", fn);
   B2L_CHECK_SUPPORTED(a->out_affine.scale == nullptr && a->out_affine.bias == nullptr,
                       "%s: out_affine is not supported (apply b2l_linear_affine to y)", fn);
-  B2L_CHECK_SUPPORTED(a->M >= 2 && a->M <= MAXB, "%s: M=%d (2..%d activation rows; use b2l_w8_gemv for 1)", fn, a->M, MAXB);
+  B2L_CHECK_SUPPORTED(a->M >= 2 && a->M <= MAXB, "%s: M=%d (2..%d activation rows; use %s for 1)", fn, a->M, MAXB,
+                      W8 ? "b2l_w8_gemv" : "b2l_q4_gemv");
   B2L_CHECK_SUPPORTED(a->K > 0 && a->K % KB == 0 && a->K <= MAX_K, "%s: K=%d must be a multiple of %d and <= %d", fn, a->K, KB, MAX_K);
   B2L_CHECK_ARG(a->N > 0, "%s: bad N", fn);
   B2L_CHECK_ARG(a->ldx >= a->K && a->ldx % 8 == 0, "%s: ldx=%d must be >= K and a multiple of 8", fn, a->ldx);
@@ -483,11 +528,16 @@ extern "C" int b2l_w8_gemv_batch(const b2l_q4_linear_args* a, b2l_stream_t strea
   p.nst = 0;
   const int grid = a->split_k;   // split_k doubles as a grid override
   switch ((NDIG * a->M + 7) / 8) {
-    case 1: return launch_batch<1>(p, grid, pdl, st);
-    case 2: return launch_batch<2>(p, grid, pdl, st);
-    case 3: return launch_batch<3>(p, grid, pdl, st);
-    case 4: return launch_batch<4>(p, grid, pdl, st);
-    case 5: return launch_batch<5>(p, grid, pdl, st);
-    default: return launch_batch<6>(p, grid, pdl, st);
+    case 1: return launch_batch<1, W8>(p, grid, pdl, st, fn);
+    case 2: return launch_batch<2, W8>(p, grid, pdl, st, fn);
+    case 3: return launch_batch<3, W8>(p, grid, pdl, st, fn);
+    case 4: return launch_batch<4, W8>(p, grid, pdl, st, fn);
+    case 5: return launch_batch<5, W8>(p, grid, pdl, st, fn);
+    default: return launch_batch<6, W8>(p, grid, pdl, st, fn);
   }
 }
+}  // namespace
+
+extern "C" int b2l_w8_gemv_batch(const b2l_q4_linear_args* a, b2l_stream_t stream) { return batch_entry<true>(a, stream); }
+
+extern "C" int b2l_q4_gemv_batch_i8(const b2l_q4_linear_args* a, b2l_stream_t stream) { return batch_entry<false>(a, stream); }

@@ -9,7 +9,9 @@ bf16 - there is no CPU fallback.
 Two execution paths behind `LLaMA.forward`:
   * decode (T == 1 with a KV cache, every Linear a gptq.int4 layer with one (scale, zero) per row):
     one C call enqueues the whole token (`b2l_decode_step`: int8-MMA GEMV kernels for batch 1, f16-MMA for 2..8 rows,
-    wgmma for 9..16), replayed as a CUDA graph.  Every Linear a per-row gptq.int8 layer: the same step at batch 1
+    wgmma for 9..16), replayed as a CUDA graph; with `LLaMA.q4_batch_step` (B2L_Q4_BATCH_STEP=1) batches of 2..16 run
+    b2l_q4_gemv_batch_i8 on the resident batch-1 tilings instead (B2L_F_Q4_BATCH_I8: each row bit-identical to the
+    batch-1 kernel on that row).  Every Linear a per-row gptq.int8 layer: the same step at batch 1
     (B2L_F_W8: the GEMV kernel with 8-bit weights); batches of 2 or more go module by module (on the wgmma GEMM),
     or, with `LLaMA.w8_batch_step` (B2L_W8_BATCH_STEP=1), batches of 2..16 run the same step (B2L_F_W8_BATCH:
     b2l_w8_gemv_batch on the resident batch-1 tilings, each row bit-identical to the batch-1 kernel on that row).
@@ -292,17 +294,19 @@ class _DecodeState:
 
         # batch 1..8: mma.sync kernels (q4_gemv / q4_gemv_batch) and their tiling; 9..16: wgmma kernel and its tiling.
         # gptq.int8: the batch-1 kernel with 8-bit weights (b2l_w8_tile_i8 tilings); with `w8_batch_step`, batches of
-        # 2..16 run b2l_w8_gemv_batch on the same resident tilings (B2L_F_W8_BATCH)
+        # 2..16 run b2l_w8_gemv_batch on the same resident tilings (B2L_F_W8_BATCH).  gptq.int4 with `q4_batch_step`:
+        # batches of 2..16 run b2l_q4_gemv_batch_i8 on the batch-1 tilings (B2L_F_Q4_BATCH_I8)
         w8 = model._fast_ok == "w8"
         w8b = w8 and B > 1
+        q4b = model._fast_ok == "q4" and B > 1 and model.q4_batch_step
         # llm.int8 (batch 1 only): b2l_q8_linear on every weight's CB / SCB in place (no copy, no tiling)
         q8 = model._fast_ok == "q8"
         assert B == 1 or not q8
         assert not w8b or (model.w8_batch_step and B <= 16)
-        gemv = (B == 1) or w8b or (B <= 8 and BATCH_GEMV)
-        i8 = B == 1 or w8b    # the b2l_q4_tile_i8 / b2l_w8_tile_i8 tilings (the resident copy of a compacted model)
+        gemv = (B == 1) or w8b or q4b or (B <= 8 and BATCH_GEMV)
+        i8 = B == 1 or w8b or q4b   # the b2l_q4_tile_i8 / b2l_w8_tile_i8 tilings (the resident copy of a compacted model)
         self.batch_ws = None
-        if w8b:
+        if w8b or q4b:   # the two batch kernels share their digit-plane workspace
             nb = lib.b2l_w8_gemv_batch_workspace_bytes(max(C_, n_hidden), B)
             self.batch_ws = torch.empty(nb, dtype=torch.uint8, device=device)
         elif gemv and B > 1:
@@ -352,7 +356,8 @@ class _DecodeState:
             ring_start=model._ring.data_ptr(), block_size=cfg.block_size, x=self.x.data_ptr(), qkv=self.qkv.data_ptr(),
             att=self.att.data_ptr(), hid=self.hid.data_ptr(), attn_work=self.work.data_ptr(),
             logits=self.logits.data_ptr(),
-            flags=model.decode_flags | (L.F_W8 if w8 else 0) | (L.F_W8_BATCH if w8b else 0) | (L.F_Q8 if q8 else 0),
+            flags=(model.decode_flags | (L.F_W8 if w8 else 0) | (L.F_W8_BATCH if w8b else 0) | (L.F_Q8 if q8 else 0)
+                   | (L.F_Q4_BATCH_I8 if q4b else 0)),
             batch_work=None if self.batch_ws is None else self.batch_ws.data_ptr())
         if q8:
             self.q8_layers = q8_layers
@@ -412,6 +417,11 @@ class LLaMA(nn.Module):
     #: bit-identical to b2l_w8_gemv on that row).  Opt-in (B2L_W8_BATCH_STEP=1): by default batched gptq.int8 decodes
     #: module by module, on the wgmma GEMM.
     w8_batch_step: bool = os.environ.get("B2L_W8_BATCH_STEP", "0") == "1"
+    #: batched (B = 2..16) decode of a gptq.int4 model (plain, LLaMA-Adapter v1 or LoRA) on the resident batch-1
+    #: tilings (b2l_decode_step under B2L_F_Q4_BATCH_I8: b2l_q4_gemv_batch_i8, each row bit-identical to b2l_q4_gemv on
+    #: that row), so a compacted model holds no second weight copy while it decodes a batch.  Opt-in
+    #: (B2L_Q4_BATCH_STEP=1): by default batches of 2..8 run b2l_q4_gemv_batch and 9..16 b2l_q4_linear_tc.
+    q4_batch_step: bool = os.environ.get("B2L_Q4_BATCH_STEP", "0") == "1"
 
     def __init__(self, config: LLaMAConfig) -> None:
         super().__init__()

@@ -15,7 +15,7 @@ import time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-SECTIONS = ["generic", "tile", "tc_small", "tc_shapes", "tc_modes", "gemv", "grid_flag", "hmma_rate", "imma_rate", "consumer_rate", "bench_gemm", "bench_tc", "trace", "bench_layers", "bench_gemv", "bench_step", "bench_ctx", "bench_13b_b8", "bench_sizes", "batch_debug", "bench_step_int8", "bench_q8_gemm", "bench_q8_gemv", "bench_w8_gemv", "bench_w8_gemm", "bench_step_w8", "bench_step_adapter", "bench_step_adapter_v2", "bench_step_lora", "bench_lora_kernel", "lora_timeline", "timeline", "mega_timeline"]
+SECTIONS = ["generic", "tile", "tc_small", "tc_shapes", "tc_modes", "gemv", "grid_flag", "hmma_rate", "imma_rate", "consumer_rate", "bench_gemm", "bench_tc", "trace", "bench_layers", "bench_gemv", "bench_step", "bench_ctx", "bench_13b_b8", "bench_sizes", "batch_debug", "bench_step_int8", "bench_q8_gemm", "bench_q8_gemv", "bench_w8_gemv", "bench_w8_gemm", "bench_step_w8", "bench_q4_batch", "bench_step_q4_batch", "bench_step_adapter", "bench_step_adapter_v2", "bench_step_lora", "bench_lora_kernel", "lora_timeline", "timeline", "mega_timeline"]
 
 
 _DLIB = None
@@ -995,10 +995,11 @@ def sec_bench_w8_gemm():
         torch.cuda.empty_cache()
 
 
-def _random_w8_model(name, dev, seed=0, n_layer=None):
-    """A gptq.int8 LLaMA at `name`'s widths (`n_layer` blocks if given) with random per-row levels, zeros and scales.
-    The scales give every linear a gain of about one (rms (level - zero) is about 76), as in a trained model: with
-    larger gains the attention scores saturate and the softmax turns rounding differences into different outputs."""
+def _random_w8_model(name, dev, seed=0, n_layer=None, bits=8):
+    """A gptq.int8 (bits = 4: gptq.int4) LLaMA at `name`'s widths (`n_layer` blocks if given) with random per-row
+    levels, zeros and scales.  The scales give every linear a gain of about one (rms (level - zero) is about 76 at 8
+    bits, 4.6 at 4), as in a trained model: with larger gains the attention scores saturate and the softmax turns
+    rounding differences into different outputs."""
     import torch
     import lit_llama_b200 as P
     from lit_llama_b200.quantization import ColBlockQuantizedLinear, weights_changed
@@ -1007,7 +1008,7 @@ def _random_w8_model(name, dev, seed=0, n_layer=None):
     prev = torch.get_default_dtype()
     torch.set_default_dtype(torch.bfloat16)
     try:
-        with torch.device(dev), quantization("gptq.int8"):
+        with torch.device(dev), quantization("gptq.int8" if bits == 8 else "gptq.int4"):
             cfg = P.LLaMAConfig.from_name(name)
             if n_layer is not None:
                 cfg.n_layer = n_layer
@@ -1019,8 +1020,9 @@ def _random_w8_model(name, dev, seed=0, n_layer=None):
         for m in model.modules():
             if isinstance(m, ColBlockQuantizedLinear):
                 m.quant_weight.copy_(torch.randint(0, 256, m.quant_weight.shape, generator=g, device=dev, dtype=torch.uint8))
-                m.scales.copy_((torch.rand(m.scales.shape, generator=g, device=dev) + 0.5) / (76 * m.in_features ** 0.5))
-                m.zeros.copy_(torch.randint(96, 160, m.zeros.shape, generator=g, device=dev))
+                rms, zlo, zhi = (76, 96, 160) if bits == 8 else (4.6, 6, 10)
+                m.scales.copy_((torch.rand(m.scales.shape, generator=g, device=dev) + 0.5) / (rms * m.in_features ** 0.5))
+                m.zeros.copy_(torch.randint(zlo, zhi, m.zeros.shape, generator=g, device=dev))
             elif isinstance(m, P.RMSNorm):
                 m.scale.fill_(1)
         model.transformer.wte.weight.normal_(0, 1, generator=g)
@@ -1859,6 +1861,176 @@ def sec_bench_step_w8_batch():
             print(f"{name} gptq.int8 decode B={B:2d} ctx~512-542: step {fmt(us[True])} us/token "
                   f"({levels / min(us[True]) / 1e3:.0f} GB/s) | module path {fmt(us[False])} us/token | "
                   f"max row rel. diff {diff:.2e} | peak {torch.cuda.max_memory_allocated() / 2**30:.2f} GiB", flush=True)
+        del model
+        gc.collect()
+        torch.cuda.empty_cache()
+
+
+def sec_bench_q4_batch():
+    """gptq.int4 at 2..16 rows: b2l_q4_gemv_batch_i8 (the resident b2l_q4_tile_i8 tiling) at M = 2, 4, 8, 16 next to
+    b2l_q4_gemv at M = 1 and today's batched kernels at the same M -- b2l_q4_gemv_batch (b2l_q4_tile_mma) at 2..8 and
+    b2l_q4_linear_tc (b2l_q4_tile) at 9..16 -- for the 7B / 13B / 65B linears, fused as b2l_decode_step fuses them.  us
+    per launch: 200 launches in a CUDA graph, PDL on, the weights rotated over enough copies (>= 200 MB of packed
+    levels) that no launch finds them in the 50 MB L2.  GB/s counts N K / 2 bytes of levels per launch (the i8 batch
+    kernel also reads 3 M K bytes of digits per 32-row unit from L2: 3 M / 16 bytes per byte of levels)."""
+    import ctypes
+
+    import torch
+    from lit_llama_b200 import _lib as L
+    from lit_llama_b200.quantization import tile_i8
+
+    dev = torch.device("cuda")
+    lib = L.lib()
+    print(_card(), flush=True)
+    R, NO, ST, RE, SW = L.PRO_RMSNORM, L.PRO_NONE, L.EPI_STORE, L.EPI_RESIDUAL, L.EPI_SWIGLU
+    shapes = [("7B c_attn", 12288, 4096, R, ST), ("7B attn.c_proj", 4096, 4096, NO, RE), ("7B fc1|fc2", 22016, 4096, R, SW),
+              ("7B mlp.c_proj", 4096, 11008, NO, RE), ("7B lm_head", 32000, 4096, R, ST),
+              ("13B c_attn", 15360, 5120, R, ST), ("13B attn.c_proj", 5120, 5120, NO, RE), ("13B fc1|fc2", 27648, 5120, R, SW),
+              ("13B mlp.c_proj", 5120, 13824, NO, RE), ("13B lm_head", 32000, 5120, R, ST),
+              ("65B c_attn", 24576, 8192, R, ST), ("65B attn.c_proj", 8192, 8192, NO, RE), ("65B fc1|fc2", 44032, 8192, R, SW),
+              ("65B mlp.c_proj", 8192, 22016, NO, RE), ("65B lm_head", 32000, 8192, R, ST)]
+    for name, N, K, pro, epi in shapes:
+        nbytes = N * K // 2
+        ncopy = max(2, -(-200_000_000 // nbytes))
+        sc = (torch.rand(N, device=dev) * 0.01 + 0.002).bfloat16()
+        z = torch.randint(6, 10, (N,), device=dev).bfloat16()
+        g = (torch.rand(K, device=dev) + 0.5).bfloat16()
+        ref = [torch.randint(0, 256, (K // 2, N), device=dev, dtype=torch.uint8).t() for _ in range(ncopy)]
+        til = {"i8": [tile_i8(q, N, K, 4) for q in ref], "mma": [tile_mma(L, q, N, K) for q in ref],
+               "tc": [tile(L, q, N, K) for q in ref]}
+        n_out = N // 2 if epi == SW else N
+        line = f"{name:16s} N={N:6d} K={K:6d}:"
+        for M in (1, 2, 4, 8, 16):
+            x = torch.randn(M, K, device=dev).bfloat16()
+            y = torch.empty(M, n_out, device=dev, dtype=torch.bfloat16)
+            res = torch.randn(M, N, device=dev).bfloat16()
+            ws = torch.empty(max(16, lib.b2l_w8_gemv_batch_workspace_bytes(K, M), lib.b2l_q4_gemv_batch_workspace_bytes(K)),
+                             dtype=torch.uint8, device=dev)
+
+            def args(kind):
+                return [L.Q4LinearArgs(x=x.data_ptr(), ldx=K, qw_tiled=t.data_ptr(), scales=sc.data_ptr(), zeros=z.data_ptr(),
+                                       sz_dtype=L.B2L_BF16, y=y.data_ptr(), ldy=n_out, M=M, N=N, K=K, prologue=pro,
+                                       norm_scale=g.data_ptr(), eps=1e-5, epilogue=epi, res=res.data_ptr(), ldres=N,
+                                       flags=L.F_PDL, workspace=ws.data_ptr()) for t in til[kind]]
+
+            def time_of(fn, a):
+                return _time_graph(lambda: [L.check(fn(ctypes.byref(a[i % ncopy]), L.stream_ptr()), "q4 linear")
+                                            for i in range(200)], 1) / 200
+
+            if M == 1:
+                u = time_of(lib.b2l_q4_gemv, args("i8"))
+                line += f" | M=1 q4_gemv {u:6.1f} us {nbytes / u / 1e3:5.0f} GB/s"
+                continue
+            u = time_of(lib.b2l_q4_gemv_batch_i8, args("i8"))
+            old, kind = (lib.b2l_q4_gemv_batch, "mma") if M <= 8 else (lib.b2l_q4_linear_tc, "tc")
+            uo = time_of(old, args(kind))
+            line += (f" | M={M} i8 {u:6.1f} us {nbytes / u / 1e3:5.0f} GB/s, "
+                     f"{'gemv_batch' if M <= 8 else 'linear_tc'} {uo:6.1f} us")
+        print(line, flush=True)
+        del ref, til
+        torch.cuda.empty_cache()
+
+
+def sec_bench_step_q4_batch():
+    """Batched gptq.int4 decode on compacted random-level models (B2L_Q4_BATCH_SIZES, default 7B,13B,65B): the
+    B2L_F_Q4_BATCH_I8 step (LLaMA.q4_batch_step, the resident tilings only) against today's batched step
+    (b2l_q4_gemv_batch at 2..8, b2l_q4_linear_tc at 9..16, on transient second tilings), both replayed as CUDA graphs,
+    at B = 1, 2, 4, 8, 16 after a 512-token prompt, alternated over 3 rounds in one process (B = 1 runs the batch-1 step
+    in both arms).  max_seq_length 576.  Prints us per token, GB/s of levels per token, the largest per-row relative
+    logits difference between the two paths and each arm's peak memory.  An arm runs only where the arithmetic (weights
+    + KV cache [+ today's second copy]) leaves 2 GiB of the card free; otherwise that arithmetic is printed.  65B then
+    runs the new step alone at B = 8, max_seq_length 2048, and prints its peak memory and the arithmetic for today's."""
+    import torch
+    from lit_llama_b200 import _lib as L
+    from lit_llama_b200.quantization import ColBlockQuantizedLinear
+
+    dev = torch.device("cuda")
+    lib = L.lib()
+    print(_card(), flush=True)
+    total = torch.cuda.mem_get_info()[1]
+    GiB = 2**30
+
+    def second_copy(model, B):
+        """Bytes of the tilings today's batched step builds beside the resident copy (b2l_q4_tile_mma at B <= 8,
+        b2l_q4_tile above)."""
+        size = lib.b2l_q4_tiled_mma_bytes if B <= 8 else lib.b2l_q4_tiled_bytes
+        n = 0
+        for blk in model.transformer.h:
+            for lin in (blk.attn.c_attn, blk.attn.c_proj, blk.mlp.c_proj):
+                n += size(lin.out_features, lin.in_features)
+            n += size(2 * blk.mlp.c_fc1.out_features, blk.mlp.c_fc1.in_features)
+        return n + size(model.lm_head.out_features, model.lm_head.in_features)
+
+    def kv_bytes(cfg, B, S):
+        return cfg.n_layer * 2 * B * cfg.n_embd * S * 2
+
+    def run_arm(model, step, B, S, n, prompt):
+        model.q4_batch_step = step
+        model.reset_cache()
+        # today's fc1|fc2 copies outlive its state: drop them so that each arm's peak is its own
+        model._fc12_cache = {k: v for k, v in model._fc12_cache.items() if k[1] == "i8"}
+        gc.collect()
+        torch.cuda.empty_cache()
+        torch.cuda.reset_peak_memory_stats()
+        with torch.no_grad():
+            model(prompt, S, torch.arange(prompt.shape[1], device=dev))
+        torch.manual_seed(0)
+        us = _decode_us(model, B, S, dev, p0=prompt.shape[1], n=n)
+        assert model._decode is not None and bool(model._decode.args.flags & L.F_Q4_BATCH_I8) == (step and B > 1)
+        with torch.no_grad():
+            lg = model(torch.arange(B, device=dev, dtype=torch.int32).view(B, 1) + 7, S,
+                       torch.tensor([prompt.shape[1] + n + 6], device=dev)).float().clone()
+        return us, lg, torch.cuda.max_memory_allocated()
+
+    for name in os.environ.get("B2L_Q4_BATCH_SIZES", "7B,13B,65B").split(","):
+        model = _random_w8_model(name, dev, seed=4, bits=4)
+        model.copy_logits = False
+        model.compact()
+        gc.collect()
+        torch.cuda.empty_cache()
+        cfg = model.config
+        resident = torch.cuda.memory_allocated()
+        extra = second_copy(model, 8)
+        levels = sum(m.out_features * m.in_features // 2 for m in model.modules() if isinstance(m, ColBlockQuantizedLinear))
+        print(f"{name}: resident model {resident / GiB:.2f} GiB, today's second copy {extra / GiB:.2f} GiB, "
+              f"card {total / GiB:.2f} GiB", flush=True)
+        S, n = 576, 8 if name == "65B" else 24
+        for B in (1, 2, 4, 8, 16):
+            need_new = resident + kv_bytes(cfg, B, S)
+            need_old = need_new + (second_copy(model, B) if B > 1 else 0)
+            arms = [a for a, need in ((True, need_new), (False, need_old)) if need + 2 * GiB <= total]
+            if False not in arms:
+                print(f"{name} B={B:2d}: today's step not run: {resident / GiB:.2f} GiB model + "
+                      f"{kv_bytes(cfg, B, S) / GiB:.2f} GiB KV cache + {(need_old - need_new) / GiB:.2f} GiB second copy = "
+                      f"{need_old / GiB:.2f} GiB > {total / GiB:.2f} GiB card - 2 GiB", flush=True)
+            if not arms:
+                continue
+            g = torch.Generator(device=dev).manual_seed(B)
+            prompt = torch.randint(0, 32000, (B, 512), device=dev, dtype=torch.int32, generator=g)
+            us, logits, peak = {a: [] for a in arms}, {}, {}
+            for _ in range(3):
+                for a in arms:
+                    u, logits[a], peak[a] = run_arm(model, a, B, S, n, prompt)
+                    us[a].append(u)
+            fmt = lambda v: " ".join(f"{u:.0f}" for u in v)   # noqa: E731
+            line = (f"{name} gptq.int4 decode B={B:2d} ctx~512-{512 + n + 6}: i8 step {fmt(us[True])} us/token "
+                    f"({levels / min(us[True]) / 1e3:.0f} GB/s), peak {peak[True] / GiB:.2f} GiB")
+            if False in arms:
+                a, b = logits[True].reshape(B, -1), logits[False].reshape(B, -1)
+                diff = max(float((a[r] - b[r]).norm() / b[r].norm()) for r in range(B))
+                line += (f" | today's step {fmt(us[False])} us/token, peak {peak[False] / GiB:.2f} GiB"
+                         f" | max row rel. diff {diff:.2e}")
+            print(line, flush=True)
+        if name == "65B":
+            B, S = 8, 2048
+            need_old = resident + kv_bytes(cfg, B, S) + extra
+            print(f"65B B=8 max_seq_length 2048: today's step not run: {resident / GiB:.2f} GiB model + "
+                  f"{kv_bytes(cfg, B, S) / GiB:.2f} GiB KV cache + {extra / GiB:.2f} GiB second copy = "
+                  f"{need_old / GiB:.2f} GiB against a {total / GiB:.2f} GiB card", flush=True)
+            prompt = torch.randint(0, 32000, (B, 512), device=dev, dtype=torch.int32)
+            u, _, peak = run_arm(model, True, B, S, n, prompt)
+            print(f"65B gptq.int4 decode B=8 max_seq_length 2048, ctx~512-{512 + n + 6}: i8 step {u:.0f} us/token, "
+                  f"peak {peak / GiB:.2f} GiB (KV cache {kv_bytes(cfg, B, S) / GiB:.2f} GiB)", flush=True)
         del model
         gc.collect()
         torch.cuda.empty_cache()
