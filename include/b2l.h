@@ -152,10 +152,13 @@ enum {
   B2L_F_W8_BATCH = 128, /* b2l_decode_step with B2L_F_W8 at B in 2..16: every linear runs b2l_w8_gemv_batch on
                            the b2l_w8_tile_i8 tilings in qw_mma; batch_work must hold
                            b2l_w8_gemv_batch_workspace_bytes(max K, B) bytes; no plan, no affines */
-  B2L_F_Q4_BATCH_I8 = 256 /* b2l_decode_step (gptq.int4) at B in 2..16: every linear runs b2l_q4_gemv_batch_i8 on
+  B2L_F_Q4_BATCH_I8 = 256, /* b2l_decode_step (gptq.int4) at B in 2..16: every linear runs b2l_q4_gemv_batch_i8 on
                            the b2l_q4_tile_i8 tilings in qw_mma; batch_work must hold
                            b2l_w8_gemv_batch_workspace_bytes(max K, B) bytes; not with B2L_F_W8, B2L_F_Q8 or
                            B2L_F_W8_BATCH; no plan, no affines */
+  B2L_F_Q8_BATCH = 512  /* b2l_decode_step with B2L_F_Q8 at B in 2..16: every linear runs b2l_q8_linear_batch on
+                           CB / SCB in place; batch_work must hold b2l_q8_linear_batch_workspace_bytes(max K, B)
+                           bytes; v2 affines allowed; not with B2L_F_W8, B2L_F_W8_BATCH or B2L_F_Q4_BATCH_I8; no plan */
 };
 
 /* Fused [RMSNorm ->] int4 linear [-> residual | SwiGLU] on wgmma (M <= 16).  Replaces
@@ -347,6 +350,20 @@ typedef struct b2l_q8_linear_args {
   int flags;                /* 0 or B2L_F_PDL                                             */
 } b2l_q8_linear_args;
 int b2l_q8_linear(const b2l_q8_linear_args* args, b2l_stream_t stream);
+/* b2l_q8_linear for M = 2..16 activation rows (batched decode on the whole-token step, B2L_F_Q8_BATCH): the same
+ * argument block, prologues, epilogues and affine, with x [M, K] and y / res [M, N], all contiguous.  Every output is
+ * bit-identical to the module sequence at M rows: b2l_rmsnorm -> b2l_q8_gemm (one outlier mask for the whole batch:
+ * bit k set iff any row has |fp16(x^[m][k])| >= threshold) [-> b2l_linear_affine] [-> b2l_add | second b2l_q8_gemm +
+ * b2l_silu_mul].  A row's outputs therefore depend on its batch-mates through that mask.  workspace: at least
+ * b2l_q8_linear_batch_workspace_bytes(K, M) bytes of 16-byte aligned device memory (may be shared by all launches of
+ * one stream).  Two launches: q8_batch_prep_kernel (one cluster of M CTAs: RMSNorm, the batch mask, SCA, CA and the
+ * outlier data, into the workspace), then q8_gemv_batch_kernel, which streams CB as b2l_q8_linear does and contracts
+ * all M rows per weight tile (csrc/q8_gemv_batch.cu).  K a multiple of 128 up to 32768, N > 0; x, cb, cb2,
+ * norm_scale and workspace 16-byte aligned; y must not overlap x; flags 0 or B2L_F_PDL.  Bad arguments are rejected
+ * before the device is touched. */
+size_t b2l_q8_linear_batch_workspace_bytes(int K, int M);
+int b2l_q8_linear_batch(const b2l_q8_linear_args* args, int M, void* workspace, size_t workspace_bytes,
+                        b2l_stream_t stream);
 /* y[M, N] (bf16, leading dimension ldy) for M activation rows x[M, K] (bf16, leading dimension
  * ldx, a multiple of 8) on the int8 wgmma tensor cores: every row bit-identical to b2l_q8_gemv
  * on that row with the batch's outlier mask (b2l_q8_outlier_mask over all M rows).  cb is CB
@@ -567,7 +584,9 @@ typedef struct b2l_decode_args {
                                 linears then run on the mma.sync batch kernel (weights need qw_mma).
                                 NULL: wgmma kernel (weights need qw_tiled).
                                 B2L_F_W8 | B2L_F_W8_BATCH and B2L_F_Q4_BATCH_I8:
-                                b2l_w8_gemv_batch_workspace_bytes(max K, B) bytes (required) */
+                                b2l_w8_gemv_batch_workspace_bytes(max K, B) bytes (required).
+                                B2L_F_Q8 | B2L_F_Q8_BATCH: b2l_q8_linear_batch_workspace_bytes(max K, B) bytes
+                                (required) */
   void* plan;                /* B == 1, head_size 128: device buffer of b2l_decode_plan_bytes() bytes prepared by
                                 b2l_decode_plan_build -> the whole step runs as ONE persistent kernel
                                 (csrc/decode_mega.cu; weights need the b2l_q4_tile_i8 layout in qw_mma).
@@ -588,7 +607,8 @@ typedef struct b2l_decode_args {
                                 layers[] and lm_head are then unused (layers[] still supplies the norms and the
                                 KV cache).  Every linear runs b2l_q8_linear, the same 5*n_layer + 3 launches
                                 (+1 per LoRA layer); affines are applied inside them (c_fc12's interleaved
-                                8 / 8 as documented above).                               */
+                                8 / 8 as documented above).  With B2L_F_Q8_BATCH at B = 2..16 every linear
+                                runs b2l_q8_linear_batch instead: two launches per linear. */
   b2l_q8_weight q8_lm_head;
   float q8_threshold;        /* B2L_F_Q8: Linear8bitLt.threshold of every linear          */
 } b2l_decode_args;

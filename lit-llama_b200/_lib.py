@@ -17,6 +17,7 @@ F_W8 = 32   # b2l_decode_step: every linear is gptq.int8 (b2l_w8_gemv)
 F_Q8 = 64   # b2l_decode_step: every linear is llm.int8 (b2l_q8_linear)
 F_W8_BATCH = 128   # b2l_decode_step with F_W8 at B in 2..16: every linear runs b2l_w8_gemv_batch
 F_Q4_BATCH_I8 = 256   # b2l_decode_step (gptq.int4) at B in 2..16: every linear runs b2l_q4_gemv_batch_i8
+F_Q8_BATCH = 512   # b2l_decode_step with F_Q8 at B in 2..16: every linear runs b2l_q8_linear_batch
 
 c_void_p, c_int, c_float, c_size_t = C.c_void_p, C.c_int, C.c_float, C.c_size_t
 
@@ -168,6 +169,8 @@ _SIGS = {
     "b2l_q8_gemv_cb": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_int, c_void_p]),
     "b2l_q8_outlier_mask": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
     "b2l_q8_linear": (c_int, [C.POINTER(Q8LinearArgs), c_void_p]),
+    "b2l_q8_linear_batch_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "b2l_q8_linear_batch": (c_int, [C.POINTER(Q8LinearArgs), c_int, c_void_p, c_size_t, c_void_p]),
     "b2l_q8_gemm_workspace_bytes": (c_size_t, [c_int, c_int]),
     "b2l_q8_gemm": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_int, c_int, c_int, c_int, c_float,
                             c_int, c_void_p]),

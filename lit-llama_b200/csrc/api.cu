@@ -172,7 +172,8 @@ static int q4_call(const b2l_q4_weight& w, const void* x, int ldx, void* y, int 
   return b2l_q4_linear_tc(&a, stream);
 }
 
-// llm.int8 (B2L_F_Q8): one b2l_q8_linear launch per linear; w2 = c_fc2 for the SwiGLU pair
+// llm.int8 (B2L_F_Q8): one b2l_q8_linear launch per linear, or at B = 2..16 under B2L_F_Q8_BATCH b2l_q8_linear_batch
+// (checked by b2l_decode_step); w2 = c_fc2 for the SwiGLU pair
 static int q8_call(const b2l_decode_args* d, const b2l_q8_weight& w, const b2l_q8_weight* w2, const void* x, void* y,
                    const void* norm_scale, int epilogue, const void* res, const b2l_out_affine* aff, b2l_stream_t stream) {
   b2l_q8_linear_args a{};
@@ -183,6 +184,8 @@ static int q8_call(const b2l_decode_args* d, const b2l_q8_weight& w, const b2l_q
   a.epilogue = epilogue; a.res = res;
   if (aff != nullptr) a.out_affine = *aff;
   a.flags = d->flags & B2L_F_PDL;
+  if (d->flags & B2L_F_Q8_BATCH)
+    return b2l_q8_linear_batch(&a, d->B, d->batch_work, b2l_q8_linear_batch_workspace_bytes(w.K, d->B), stream);
   return b2l_q8_linear(&a, stream);
 }
 
@@ -199,7 +202,16 @@ static int check_q8_weight(const b2l_q8_weight& w, int N, int K, const char* wha
 
 static int check_q8(const b2l_decode_args* d) {
   B2L_CHECK_SUPPORTED(!(d->flags & B2L_F_W8), "b2l_decode_step: B2L_F_Q8 (llm.int8) and B2L_F_W8 (gptq.int8) exclude each other");
-  B2L_CHECK_SUPPORTED(d->B == 1, "b2l_decode_step: B2L_F_Q8 (llm.int8) runs batch 1 only, got B=%d", d->B);
+  if (d->flags & B2L_F_Q8_BATCH) {
+    B2L_CHECK_SUPPORTED(!(d->flags & (B2L_F_W8_BATCH | B2L_F_Q4_BATCH_I8)),
+                        "b2l_decode_step: B2L_F_Q8_BATCH (llm.int8) does not combine with B2L_F_W8_BATCH or B2L_F_Q4_BATCH_I8");
+    B2L_CHECK_SUPPORTED(d->B >= 2 && d->B <= 16, "b2l_decode_step: B2L_F_Q8_BATCH runs batches of 2..16, got B=%d", d->B);
+    B2L_CHECK_SUPPORTED(d->plan == nullptr, "b2l_decode_step: B2L_F_Q8_BATCH does not run in the persistent kernel (plan must be NULL)");
+    B2L_CHECK_ARG(d->batch_work != nullptr,
+                  "b2l_decode_step: B2L_F_Q8_BATCH needs batch_work (b2l_q8_linear_batch_workspace_bytes(max K, B) bytes)");
+  } else {
+    B2L_CHECK_SUPPORTED(d->B == 1, "b2l_decode_step: B2L_F_Q8 (llm.int8) runs batch 1 only, got B=%d", d->B);
+  }
   B2L_CHECK_SUPPORTED(d->plan == nullptr, "b2l_decode_step: B2L_F_Q8 (llm.int8) does not run in the persistent kernel (plan must be NULL)");
   B2L_CHECK_ARG(d->q8_layers != nullptr, "b2l_decode_step: B2L_F_Q8 needs q8_layers");
   const int C = d->n_embd, H = d->n_hidden;
@@ -220,9 +232,9 @@ extern "C" int b2l_decode_step_launches(const b2l_decode_args* d) {
   // fused single-token attention for head_size 128 (B2L_F_ATTN_UNFUSED: the three-kernel path)
   const bool fused = d->n_embd / d->n_head == 128 && !(d->flags & B2L_F_ATTN_UNFUSED);
   const int attn = fused ? 1 : 3;
-  // the batch kernels (int4 at 2..8 rows, gptq.int8 and, under B2L_F_Q4_BATCH_I8, int4 at 2..16) are two launches
-  // per linear
-  const bool b16 = (d->flags & (B2L_F_W8_BATCH | B2L_F_Q4_BATCH_I8)) && d->B > 1 && d->B <= 16 && d->batch_work;
+  // the batch kernels (int4 at 2..8 rows, gptq.int8, llm.int8 under B2L_F_Q8_BATCH and, under B2L_F_Q4_BATCH_I8,
+  // int4 at 2..16) are two launches per linear
+  const bool b16 = (d->flags & (B2L_F_W8_BATCH | B2L_F_Q4_BATCH_I8 | B2L_F_Q8_BATCH)) && d->B > 1 && d->B <= 16 && d->batch_work;
   const int lin = (b16 || (d->B > 1 && d->B <= 8 && d->batch_work)) ? 2 : 1;
   int n = 2 + d->n_layer * (4 * lin + attn) + lin;  // ring advance + embedding, per Block 4 linears + attention, ln_f+lm_head
   // an adapter layer adds the prefix kernel behind the three-kernel attention (the fused kernel does it in-launch)
@@ -252,6 +264,7 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
     B2L_CHECK_ARG(d->batch_work != nullptr, "b2l_decode_step: B2L_F_Q4_BATCH_I8 needs batch_work (b2l_w8_gemv_batch_workspace_bytes(max K, B) bytes)");
   }
   const bool q8 = (d->flags & B2L_F_Q8) != 0;
+  B2L_CHECK_SUPPORTED(q8 || !(d->flags & B2L_F_Q8_BATCH), "b2l_decode_step: B2L_F_Q8_BATCH needs B2L_F_Q8 (llm.int8)");
   if (q8)
     if (int rc = check_q8(d)) return rc;
   if (d->flags & B2L_F_W8_BATCH) {
@@ -282,7 +295,9 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
   // LLaMA-Adapter v2: every linear's affine runs in its own batch-1 launch (b2l_q4_linear_args::out_affine)
   const bool any_affine = d->affines != nullptr || d->lm_head_affine.scale != nullptr || d->lm_head_affine.bias != nullptr;
   if (any_affine) {
-    B2L_CHECK_SUPPORTED(d->B == 1, "b2l_decode_step: LLaMA-Adapter v2 affines run at batch 1 only, got B=%d", d->B);
+    // llm.int8's batch kernel applies them in its epilogue too
+    B2L_CHECK_SUPPORTED(d->B == 1 || (d->flags & B2L_F_Q8_BATCH),
+                        "b2l_decode_step: LLaMA-Adapter v2 affines run at batch 1 only, got B=%d", d->B);
     B2L_CHECK_SUPPORTED(d->plan == nullptr, "b2l_decode_step: LLaMA-Adapter v2 affines do not run in the persistent kernel (plan must be NULL)");
     B2L_CHECK_SUPPORTED(d->loras == nullptr, "b2l_decode_step: LLaMA-Adapter v2 affines and LoRA do not combine");
     auto ok = [](const b2l_out_affine& f) { return (f.scale == nullptr) == (f.bias == nullptr); };
@@ -300,7 +315,7 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
   if (d->plan != nullptr) return decode_step_persistent(d, stream);   // one persistent kernel per token (decode_mega.cu)
   const int C = d->n_embd, hs = C / d->n_head, B = d->B;
   const int fl = d->flags;               // the linears' flags (q4_call routes B2L_F_W8 to b2l_w8_gemv)
-  const int afl = fl & ~(B2L_F_W8 | B2L_F_Q8 | B2L_F_W8_BATCH | B2L_F_Q4_BATCH_I8);   // everything else
+  const int afl = fl & ~(B2L_F_W8 | B2L_F_Q8 | B2L_F_W8_BATCH | B2L_F_Q4_BATCH_I8 | B2L_F_Q8_BATCH);   // everything else
   int rc;
   // debug timeline: launch i of the step writes uint64[64] at timeline + 512*i (order: per Block c_attn,
   // attention, c_proj, fc12, mlp_proj; then lm_head)

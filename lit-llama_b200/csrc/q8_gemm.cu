@@ -24,6 +24,7 @@
 #include <cuda_fp16.h>
 
 #include "b2l_common.cuh"
+#include "q8_common.cuh"
 
 namespace b2l {
 namespace q8gm {
@@ -240,8 +241,8 @@ __global__ void __launch_bounds__(Cfg<BT, NWG>::NTHREADS, 1) q8_gemm_kernel(cons
             const int k = wi * 32 + __ffs(mb) - 1;
             mb &= mb - 1;
             const float a0 = fp16_of_bf16(x0[k]), a1 = fp16_of_bf16(x1[k]);
-            const float wv0 = __half2float(__float2half_rn((float)w0[k] * wsc[0]));
-            const float wv1 = __half2float(__float2half_rn((float)w1[k] * wsc[1]));
+            const float wv0 = q8_outlier_weight(w0[k], wsc[0]);
+            const float wv1 = q8_outlier_weight(w1[k], wsc[1]);
             term[0] = fmaf(a0, wv0, term[0]);
             term[1] = fmaf(a1, wv0, term[1]);
             term[2] = fmaf(a0, wv1, term[2]);
@@ -254,8 +255,8 @@ __global__ void __launch_bounds__(Cfg<BT, NWG>::NTHREADS, 1) q8_gemm_kernel(cons
         const int r = e >> 1, t = e & 1;
         const int n = nr + 8 * r, m = mt + t;
         if (n >= p.N || m >= p.M) continue;
-        float v = __half2float(__float2half_rn((float)acc[4 * c + e] * (sca[t] * scb[r] * (1.0f / (127.0f * 127.0f)))));
-        if (any) v = __half2float(__float2half_rn(v + __half2float(__float2half_rn(term[2 * r + t]))));
+        float v = q8_dequant(acc[4 * c + e], sca[t], scb[r]);
+        if (any) v = q8_add_outliers(v, term[2 * r + t]);
         p.y[(size_t)m * p.ldy + n] = f2bf(v);
       }
     }

@@ -37,6 +37,7 @@
 #include <cuda_fp16.h>
 
 #include "b2l_common.cuh"
+#include "q8_common.cuh"
 
 namespace b2l {
 namespace q8mv {
@@ -406,7 +407,7 @@ __global__ void __launch_bounds__(NTHREADS, 2) q8_gemv_kernel(const Params p) {
           const int e = __ffs(mb) - 1;
           mb &= mb - 1;
           const int k = wi * 32 + e;
-          const float wv = __half2float(__float2half_rn((float)(FUSED ? fr.w[k] : p.cb[(size_t)o * p.K + k]) * wsc));
+          const float wv = q8_outlier_weight(FUSED ? fr.w[k] : p.cb[(size_t)o * p.K + k], wsc);
           term = fmaf(__half2float(ah[k]), wv, term);
           any = true;
         }
@@ -416,8 +417,8 @@ __global__ void __launch_bounds__(NTHREADS, 2) q8_gemv_kernel(const Params p) {
 #pragma unroll
       for (int w = 0; w < NCW; ++w) t += scratch[(buf * NCW + w) * RB + row];
       if (u + 2 < n_units) { if (buf) bar_arrive_c<5>(NCW * 32 + 32); else bar_arrive_c<4>(NCW * 32 + 32); }
-      float v = __half2float(__float2half_rn((float)t * (sca * scb * (1.0f / (127.0f * 127.0f)))));
-      if (any) v = __half2float(__float2half_rn(v + __half2float(__float2half_rn(term))));
+      float v = q8_dequant(t, sca, scb);
+      if (any) v = q8_add_outliers(v, term);
       if constexpr (FUSED) {
         // the module path's bf16 output, then b2l_linear_affine, then b2l_add / b2l_silu_mul
         float yv = rbf(v);

@@ -16,7 +16,8 @@ Two execution paths behind `LLaMA.forward`:
     or, with `LLaMA.w8_batch_step` (B2L_W8_BATCH_STEP=1), batches of 2..16 run the same step (B2L_F_W8_BATCH:
     b2l_w8_gemv_batch on the resident batch-1 tilings, each row bit-identical to the batch-1 kernel on that row).
     Every Linear an llm.int8 layer, with `LLaMA.int8_step` (B2L_INT8_STEP=1): the same step at batch 1 (B2L_F_Q8:
-    b2l_q8_linear reading CB / SCB in place), bit-identical to the module path.
+    b2l_q8_linear reading CB / SCB in place) and at batches of 2..16 (B2L_F_Q8 | B2L_F_Q8_BATCH: b2l_q8_linear_batch,
+    also in place), bit-identical to the module path.
   * everything else (prefill on the wgmma GEMM, no-cache forward, other Linear kinds): module by module.
 """
 import ctypes as C
@@ -299,9 +300,10 @@ class _DecodeState:
         w8 = model._fast_ok == "w8"
         w8b = w8 and B > 1
         q4b = model._fast_ok == "q4" and B > 1 and model.q4_batch_step
-        # llm.int8 (batch 1 only): b2l_q8_linear on every weight's CB / SCB in place (no copy, no tiling)
+        # llm.int8: b2l_q8_linear (batch 1) or b2l_q8_linear_batch (2..16, B2L_F_Q8_BATCH) on every weight's CB / SCB in
+        # place (no copy, no tiling)
         q8 = model._fast_ok == "q8"
-        assert B == 1 or not q8
+        q8b = q8 and B > 1
         assert not w8b or (model.w8_batch_step and B <= 16)
         gemv = (B == 1) or w8b or q4b or (B <= 8 and BATCH_GEMV)
         i8 = B == 1 or w8b or q4b   # the b2l_q4_tile_i8 / b2l_w8_tile_i8 tilings (the resident copy of a compacted model)
@@ -309,7 +311,10 @@ class _DecodeState:
         if w8b or q4b:   # the two batch kernels share their digit-plane workspace
             nb = lib.b2l_w8_gemv_batch_workspace_bytes(max(C_, n_hidden), B)
             self.batch_ws = torch.empty(nb, dtype=torch.uint8, device=device)
-        elif gemv and B > 1:
+        elif q8b:
+            self.batch_ws = torch.empty(lib.b2l_q8_linear_batch_workspace_bytes(max(C_, n_hidden), B), dtype=torch.uint8,
+                                        device=device)
+        elif gemv and B > 1 and not q8:
             self.batch_ws = batch_workspace(device, max(C_, n_hidden))
 
         def q4(lin: ColBlockQuantizedLinear) -> L.Q4Weight:
@@ -357,7 +362,7 @@ class _DecodeState:
             att=self.att.data_ptr(), hid=self.hid.data_ptr(), attn_work=self.work.data_ptr(),
             logits=self.logits.data_ptr(),
             flags=(model.decode_flags | (L.F_W8 if w8 else 0) | (L.F_W8_BATCH if w8b else 0) | (L.F_Q8 if q8 else 0)
-                   | (L.F_Q4_BATCH_I8 if q4b else 0)),
+                   | (L.F_Q4_BATCH_I8 if q4b else 0) | (L.F_Q8_BATCH if q8b else 0)),
             batch_work=None if self.batch_ws is None else self.batch_ws.data_ptr())
         if q8:
             self.q8_layers = q8_layers
@@ -372,7 +377,7 @@ class _DecodeState:
         if loras is not None:      # LoRA: the step adds each layer's low-rank term behind c_attn
             self.args.loras = C.cast(loras, C.POINTER(L.LoRA))
         affines = model._affines(self.keep)
-        if affines is not None:    # LLaMA-Adapter v2 (B == 1): every linear's launch applies its scale and bias
+        if affines is not None:    # LLaMA-Adapter v2 (B == 1, llm.int8 at any B): every linear's launch applies them
             self.args.affines = C.cast(affines[0], C.POINTER(L.LayerAffine))
             self.args.lm_head_affine = affines[1]
         # batch 1, head_size 128: the whole step as ONE persistent kernel (csrc/decode_mega.cu; int4 weights only, so
@@ -408,9 +413,10 @@ class LLaMA(nn.Module):
     #: batch-1 decode (head_size 128) as ONE persistent kernel per token (csrc/decode_mega.cu) instead of one kernel
     #: per op.  Opt-in (B2L_PERSISTENT=1): the default is the per-op path under programmatic dependent launch.
     persistent: bool = os.environ.get("B2L_PERSISTENT", "0") == "1"
-    #: batch-1 decode of an llm.int8 model (plain, LLaMA-Adapter v1 / v2 or LoRA) on the whole-token step
-    #: (b2l_decode_step under B2L_F_Q8: b2l_q8_linear with RMSNorm / residual / SwiGLU / affine fused), bit-identical
-    #: to the module path.  Opt-in (B2L_INT8_STEP=1): by default llm.int8 decodes module by module.
+    #: decode of an llm.int8 model (plain, LLaMA-Adapter v1 / v2 or LoRA) at batch 1..16 on the whole-token step
+    #: (b2l_decode_step under B2L_F_Q8: b2l_q8_linear with RMSNorm / residual / SwiGLU / affine fused at batch 1, and
+    #: with B2L_F_Q8_BATCH b2l_q8_linear_batch at 2..16), bit-identical to the module path.  Opt-in (B2L_INT8_STEP=1):
+    #: by default llm.int8 decodes module by module, and so do batches over 16.
     int8_step: bool = os.environ.get("B2L_INT8_STEP", "0") == "1"
     #: batched (B = 2..16) decode of a gptq.int8 model (plain, LLaMA-Adapter v1 or LoRA) on the whole-token step
     #: (b2l_decode_step under B2L_F_W8 | B2L_F_W8_BATCH: b2l_w8_gemv_batch on the resident batch-1 tilings, each row
@@ -714,10 +720,11 @@ class LLaMA(nn.Module):
             if st is None or st.B != B or st.S != max_seq_length or st.idx.dtype != idx.dtype or st.idx.device != idx.device:
                 if self._fast_ok is None:
                     self._fast_ok = self._fast_decode_ok()
-                # gptq.int8, llm.int8 and LLaMA-Adapter v2: batch 1 only; llm.int8 on request (int8_step); gptq.int8
-                # without v2 affines at batch 2..16 on request (w8_batch_step)
+                # gptq.int8 and LLaMA-Adapter v2: batch 1 only; gptq.int8 without v2 affines at batch 2..16 on request
+                # (w8_batch_step); llm.int8 at batch 1..16 (v2 affines included) on request (int8_step)
                 fast = (bool(self._fast_ok) and (self._fast_ok != "q8" or self.int8_step)
-                        and (B == 1 or (self._fast_ok not in ("w8", "q8") and not self._has_affines())
+                        and (B == 1 or self._fast_ok == "q8"
+                             or (self._fast_ok != "w8" and not self._has_affines())
                              or (self._fast_ok == "w8" and self.w8_batch_step and not self._has_affines())))
                 st = self._decode = _DecodeState(self, B, max_seq_length, idx.device, idx.dtype) if fast else None
         if st is not None:

@@ -2036,6 +2036,117 @@ def sec_bench_step_q4_batch():
         torch.cuda.empty_cache()
 
 
+def sec_bench_q8_batch():
+    """llm.int8 at 2..16 rows: b2l_q8_linear_batch (prep launch included) against the module ops it replaces
+    (b2l_rmsnorm + b2l_q8_gemm [+ b2l_add | second GEMM + b2l_silu_mul]) at M = 2, 4, 8, 16, and b2l_q8_linear at M = 1,
+    for the 7B / 13B / 65B linears.  us per linear: 200 launches in a CUDA graph, PDL on for the fused kernels.  The
+    weights are not rotated, so a layer under 50 MB (7B c_proj) is partly served from L2.  GB/s counts the CB bytes."""
+    import ctypes
+
+    import torch
+    from lit_llama_b200 import _lib as L
+    from lit_llama_b200.int8 import quantize_rows_int8
+
+    dev = torch.device("cuda")
+    print(_card(), flush=True)
+    shapes = [("7B c_attn", 12288, 4096, 1), ("7B c_proj", 4096, 4096, 2), ("7B fc1|fc2", 11008, 4096, 3),
+              ("7B mlp.c_proj", 4096, 11008, 2), ("13B c_attn", 15360, 5120, 1), ("13B mlp.c_proj", 5120, 13824, 2),
+              ("65B fc1|fc2", 22016, 8192, 3), ("65B mlp.c_proj", 8192, 22016, 2), ("lm_head", 32000, 4096, 1)]
+    lib = L.lib()
+    for name, N, K, kind in shapes:   # kind 1: RMSNorm + store, 2: residual, 3: RMSNorm + SwiGLU
+        glu = kind == 3
+        cb, scb = quantize_rows_int8(torch.randn(N, K, device=dev) * 0.05)
+        cb2, scb2 = quantize_rows_int8(torch.randn(N, K, device=dev) * 0.05) if glu else (cb, scb)
+        g = (torch.rand(K, device=dev) + 0.5).bfloat16()
+        line = []
+        for M in (1, 2, 4, 8, 16):
+            x = torch.randn(M, K, device=dev).bfloat16()
+            xh = torch.empty_like(x)
+            y = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
+            y2, h = torch.empty_like(y), torch.empty_like(y)
+            res = torch.randn(M, N, device=dev).bfloat16()
+            a = L.Q8LinearArgs(x=x.data_ptr(), cb=cb.data_ptr(), scb=scb.data_ptr(), cb2=cb2.data_ptr(), scb2=scb2.data_ptr(),
+                               y=y.data_ptr(), N=N, K=K, threshold=6.0, prologue=L.PRO_NONE if kind == 2 else L.PRO_RMSNORM,
+                               norm_scale=g.data_ptr(), eps=1e-5, res=res.data_ptr(), flags=L.F_PDL,
+                               epilogue={1: L.EPI_STORE, 2: L.EPI_RESIDUAL, 3: L.EPI_SWIGLU}[kind])
+            if M == 1:
+                t = _time_graph(lambda: lib.b2l_q8_linear(ctypes.byref(a), L.stream_ptr()), 200)
+                line.append(f"M=1 q8_linear {t:6.1f} us {N * K * (2 if glu else 1) / 1e3 / t:5.0f} GB/s")
+                continue
+            nb = lib.b2l_q8_linear_batch_workspace_bytes(K, M)
+            ws = torch.empty(nb, dtype=torch.uint8, device=dev)
+            new = _time_graph(lambda: lib.b2l_q8_linear_batch(ctypes.byref(a), M, ws.data_ptr(), nb, L.stream_ptr()), 200)
+            gnb = lib.b2l_q8_gemm_workspace_bytes(M, K)
+            gws = torch.empty(gnb, dtype=torch.uint8, device=dev)
+
+            def module():
+                src = x
+                if kind != 2:
+                    lib.b2l_rmsnorm(x.data_ptr(), g.data_ptr(), xh.data_ptr(), M, K, 1e-5, L.stream_ptr())
+                    src = xh
+                lib.b2l_q8_gemm(src.data_ptr(), K, cb.data_ptr(), scb.data_ptr(), gws.data_ptr(), gnb, y.data_ptr(), N, M, N, K, 6.0, 0,
+                                L.stream_ptr())
+                if glu:
+                    lib.b2l_q8_gemm(src.data_ptr(), K, cb2.data_ptr(), scb2.data_ptr(), gws.data_ptr(), gnb, y2.data_ptr(), N, M, N, K,
+                                    6.0, 0, L.stream_ptr())
+                    lib.b2l_silu_mul(y.data_ptr(), y2.data_ptr(), h.data_ptr(), M * N, L.stream_ptr())
+                elif kind == 2:
+                    lib.b2l_add(res.data_ptr(), y.data_ptr(), h.data_ptr(), M * N, L.stream_ptr())
+            old = _time_graph(module, 200)
+            gb = N * K * (2 if glu else 1) / 1e3
+            line.append(f"M={M} batch {new:6.1f} us {gb / new:5.0f} GB/s / module {old:6.1f} us")
+        print(f"{name:15s} N={N:6d} K={K:6d}: " + " | ".join(line), flush=True)
+        del cb, cb2
+        torch.cuda.empty_cache()
+
+
+def sec_bench_step_q8_batch():
+    """llm.int8 batched decode at ctx ~512: the B2L_F_Q8 | B2L_F_Q8_BATCH step (LLaMA.int8_step) against the module
+    path (both replayed as CUDA graphs), alternated over 2 rounds in one process, at B = 2, 4, 8, 16 for the sizes in
+    B2L_INT8_SIZES (default 7B,13B).  The logits must be bit-identical."""
+    import torch
+    import lit_llama_b200 as P
+    from lit_llama_b200.utils import quantization
+
+    dev = torch.device("cuda")
+    print(_card(), flush=True)
+    for name in os.environ.get("B2L_INT8_SIZES", "7B,13B").split(","):
+        S = 1024
+        prev = torch.get_default_dtype()
+        torch.set_default_dtype(torch.bfloat16)
+        try:
+            with torch.device(dev), quantization("llm.int8"):
+                model = P.LLaMA.from_name(name)
+        finally:
+            torch.set_default_dtype(prev)
+        model.eval()
+        model.copy_logits = False
+        for B in ((2, 4, 8) if name == "65B" else (2, 4, 8, 16)):
+            torch.cuda.reset_peak_memory_stats()
+            us = {True: [], False: []}
+            logits = {}
+            for _ in range(2):
+                for fused in (True, False):
+                    model.int8_step = fused
+                    model.reset_cache()
+                    with torch.no_grad():
+                        torch.manual_seed(B)
+                        model(torch.randint(0, 32000, (B, 16), device=dev, dtype=torch.int32), S, torch.arange(16, device=dev))
+                    torch.manual_seed(0)
+                    us[fused].append(_decode_us(model, B, S, dev, p0=512, n=16))
+                    assert (model._decode is not None) == fused
+                    with torch.no_grad():
+                        logits[fused] = model(torch.randint(0, 32000, (B, 1), device=dev, dtype=torch.int32,
+                                                            generator=torch.Generator(dev).manual_seed(1)), S,
+                                              torch.tensor([600], device=dev)).clone()
+            assert torch.equal(logits[True], logits[False])
+            fmt = lambda v: " ".join(f"{u / 1e3:.2f}" for u in v)
+            print(f"{name} llm.int8 decode B={B} max_seq_length {S}: step {fmt(us[True])} ms/token | module path {fmt(us[False])} "
+                  f"ms/token | logits bit-identical | peak {torch.cuda.max_memory_allocated() / 2**30:.2f} GiB", flush=True)
+        del model
+        torch.cuda.empty_cache()
+
+
 def main():
     which = sys.argv[1:] or SECTIONS
     if len(which) == 1 and os.environ.get("B2L_DIAG_CHILD") == "1":
