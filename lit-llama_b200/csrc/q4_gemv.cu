@@ -85,7 +85,7 @@ __host__ __device__ inline SmemLayout smem_layout(int nst, int K, int ndig) {
   L.xf = o;      o += (uint32_t)ndig * plane_stride(K);   // digit planes: [digit][k block][t (4)][16 B]
   L.zero = o;    o += 16;                                 // the B operand of the unused MMA columns
   L.scratch = o; o += 2 * NCW * MAX_HALVES * RB * 16;     // [buf][warp][half][row][digit (4)] int32 partials
-  L.red = o;     o += 192;                                // reductions: float[8] sumsq, float[8] max, int64[8] sum X, int sh, float[8] max|g|
+  L.red = o;     o += 144;                                // reductions: float[8] sumsq, float[8] max, int64[8] sum X, int sh
   L.sxp = o;     o += NCW * 32 * 4;                       // per-thread partial sums of X
   L.bars = o;    o += 2 * MAX_STAGES * 8;
   L.total = (o + 127u) & ~127u;
@@ -257,23 +257,12 @@ __global__ void __launch_bounds__(NTHREADS, 2) q4_gemv_kernel(const Params p) {
       constexpr int NT = NCW * 32;   // 256 threads, 8 elements each per pass
       constexpr uint32_t MAGIC_BITS = 0x4B400000u;   // 1.5 * 2^23
       uint4 xv[MAXC], gv[MAXC];
-      // the RMSNorm scale is a weight: fetch it (and reduce its max) BEFORE waiting for the producing kernel
-      __nv_bfloat162 gmax2 = __float2bfloat162_rn(0.f);
+      // the RMSNorm scale is a weight: fetch it BEFORE waiting for the producing kernel
 #pragma unroll
       for (int c = 0; c < MAXC; ++c) {
         const int k = (c * NT + tid) * 8;
         gv[c] = make_uint4(0, 0, 0, 0);
         if (norm && k < p.K) gv[c] = *reinterpret_cast<const uint4*>(p.norm_scale + k);
-      }
-      if (norm) {
-#pragma unroll
-        for (int c = 0; c < MAXC; ++c) {
-          const uint32_t g[4] = {gv[c].x, gv[c].y, gv[c].z, gv[c].w};
-#pragma unroll
-          for (int q = 0; q < 4; ++q) gmax2 = __hmax2(gmax2, __habs2(*reinterpret_cast<const __nv_bfloat162*>(&g[q])));
-        }
-        const float gw = warp_max(fmaxf(__low2float(gmax2), __high2float(gmax2)));
-        if (lane == 0) red[36 + warp] = gw;      // read after the pass-1 barrier below
       }
       pdl_wait();
       if (tid == 0) tl_max(p.tl, 1);
@@ -286,21 +275,24 @@ __global__ void __launch_bounds__(NTHREADS, 2) q4_gemv_kernel(const Params p) {
       }
       const int nchunk = (p.K + NT * 8 - 1) / (NT * 8);  // warp-uniform: chunks that hold data
       // pass 1: sum of bf16-rounded squares (RMSNorm, model.py:274: one HMUL2 is the exactly-rounded bf16 product the
-      // reference computes) and max |x| (with max |scale| it bounds the normalised values)
+      // reference computes) and max |x|, or with RMSNorm max_k |bf16(g_k x_k)|, which bounds the normalised values
       float ss = 0.f;
       __nv_bfloat162 amax2 = __float2bfloat162_rn(0.f);
 #pragma unroll
       for (int c = 0; c < MAXC; ++c) {
         if (c < nchunk) {
           const uint32_t w[4] = {xv[c].x, xv[c].y, xv[c].z, xv[c].w};
+          const uint32_t g[4] = {gv[c].x, gv[c].y, gv[c].z, gv[c].w};
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
             const __nv_bfloat162 v = *reinterpret_cast<const __nv_bfloat162*>(&w[q]);
-            amax2 = __hmax2(amax2, __habs2(v));
             if (norm) {
+              amax2 = __hmax2(amax2, __habs2(__hmul2(v, *reinterpret_cast<const __nv_bfloat162*>(&g[q]))));
               const __nv_bfloat162 sq = __hmul2(v, v);
               const uint32_t su = *reinterpret_cast<const uint32_t*>(&sq);
               ss += __uint_as_float(su << 16) + __uint_as_float(su & 0xffff0000u);
+            } else {
+              amax2 = __hmax2(amax2, __habs2(v));
             }
           }
         }
@@ -310,14 +302,22 @@ __global__ void __launch_bounds__(NTHREADS, 2) q4_gemv_kernel(const Params p) {
       mx = warp_max(mx);
       if (lane == 0) { red[warp] = ss; red[8 + warp] = mx; }
       named_bar_sync(1, NT);
-      float gm = 0.f;
       ss = 0.f; mx = 0.f;
 #pragma unroll
-      for (int w = 0; w < NCW; ++w) { ss += red[w]; mx = fmaxf(mx, red[8 + w]); if (norm) gm = fmaxf(gm, red[36 + w]); }
+      for (int w = 0; w < NCW; ++w) { ss += red[w]; mx = fmaxf(mx, red[8 + w]); }
       float rinv = 1.f;
       if (norm) {
+        // The normalised value is v_k = bf16(g_k bf16(x_k rinv)) (rinv is a bf16 value), and pass 1 took
+        // p_k = bf16(g_k x_k).  With u = 2^-8, the unit roundoff of bf16:
+        //   |v_k| <= |g_k x_k| rinv (1 + u)^2 <= |p_k| rinv (1 + u)^2 / (1 - u) < 1.012 |p_k| rinv,
+        // and the two fp32 roundings below lose less than 2^-23, so mx > max_k |v_k|: |X| < 2^22 follows from the
+        // choice of sh.  (A product below bf16's normal range 2^-126 may round further; such elements have
+        // |v_k| < 2^-125 rinv, and sh <= 126 keeps them below 2^22 for any rinv < 2^21, i.e. eps > 2^-42.)
+        // A bound on max|x| max|g|
+        // instead overshoots by up to max|g| / g_k when the largest activation carries a small scale (LLaMA's
+        // massive channels do), and the digit grid below coarsens by the same factor.
         rinv = rms_rinv(ss, p.K, p.eps);
-        mx = mx * gm * rinv * 1.01f;     // |bf16(g * bf16(x * rinv))| <= max|g| max|x| rinv (1 + 2^-8)^2
+        mx = mx * rinv * 1.02f;
       }
       // 2^sh: the largest power of two with max|v| * 2^sh < 2^(8 NDIG - 2)
       const int e = (int)((__float_as_uint(mx) >> 23) & 0xffu) - 127;   // mx < 2^(e + 1)

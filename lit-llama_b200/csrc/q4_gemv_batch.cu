@@ -9,9 +9,11 @@
 // What changes is the activation side.  8 rows of K fp16 fragments (up to 8 * 24576 * 2 B) do not fit in
 // shared memory next to the weight ring, so
 //   1. q4_batch_prep_kernel (one CTA per activation row) applies RMSNorm with the reference's bf16 rounding
-//      points, converts to fp16 in MMA B-fragment order (upper k half of every k16 chunk pre-divided by 16,
-//      see q4_gemv.cu) and writes them, plus the two per-row sums the zero-point correction needs, to a
-//      workspace that stays in L2;
+//      points, scales row n by a power of two 2^sh_n that puts its largest magnitude in [2^14, 2^15), converts
+//      to fp16 in MMA B-fragment order (upper k half of every k16 chunk pre-divided by 16, see q4_gemv.cu) and
+//      writes them, plus the two per-row sums the zero-point correction needs and 2^-sh_n, to a workspace that
+//      stays in L2.  The epilogue multiplies by 2^-sh_n before its bf16 rounding, so a row's result does not
+//      depend on its magnitude: y(2^e x) = 2^e y(x) bit for bit, whatever the other rows hold;
 //   2. q4_gemv_batch_kernel streams, per 16 KB weight stage, the matching 16 KB of activation fragments
 //      through the same mbarrier ring (one more TMA bulk copy per stage).  The weight copies of the first
 //      ring-full are issued before griddepcontrol.wait; the fragment copies, which depend on step 1, after.
@@ -19,7 +21,8 @@
 // bit-deterministic.
 //
 // Workspace (b2l_q4_gemv_batch_workspace_bytes): [K/64 k blocks][2 planes][32 lanes][16 B] fragments, lane
-// 4n + t holding row n; then float[8][2] = {sum over the lower k halves, sum over the upper k halves}.
+// 4n + t holding row n; then float[8][2] = {sum over the lower k halves, sum over the upper k halves} of the scaled
+// values, then float[8] = 2^-sh_n.
 #include <cstdlib>
 
 #include "q4_mma_common.cuh"
@@ -64,7 +67,7 @@ template <int MAXC>
 __global__ void __launch_bounds__(256) q4_batch_prep_kernel(const __nv_bfloat16* x, int ldx, int M, int K,
                                                             const __nv_bfloat16* __restrict__ norm_scale, float eps,
                                                             uint32_t* __restrict__ xfrag, float* __restrict__ sums) {
-  __shared__ float red[24];
+  __shared__ float red[32];   // [0..7] sum of squares, [8..23] the two half sums, [24..31] max |v|
   const int n = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   constexpr int NT = 256;
   pdl_launch_dependents();  // the linear may start streaming its weights
@@ -109,30 +112,49 @@ __global__ void __launch_bounds__(256) q4_batch_prep_kernel(const __nv_bfloat16*
     for (int w = 0; w < 8; ++w) ss += red[w];
     rinv = rms_rinv(ss, K, eps);
   }
+  // the values the reference feeds its linear (RMSNorm applied in place), and their largest magnitude
   const __nv_bfloat162 rinv2 = __float2bfloat162_rn(rinv);
+  __nv_bfloat162 amax2 = __float2bfloat162_rn(0.f);
+#pragma unroll
+  for (int c = 0; c < MAXC; ++c) {
+    if (c < nchunk) {
+      uint32_t w[4] = {xv[c].x, xv[c].y, xv[c].z, xv[c].w};
+      const uint32_t g[4] = {gv[c].x, gv[c].y, gv[c].z, gv[c].w};
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        __nv_bfloat162 v = *reinterpret_cast<const __nv_bfloat162*>(&w[q]);
+        if (norm) v = __hmul2(*reinterpret_cast<const __nv_bfloat162*>(&g[q]), __hmul2(v, rinv2));
+        amax2 = __hmax2(amax2, __habs2(v));
+        w[q] = *reinterpret_cast<const uint32_t*>(&v);
+      }
+      xv[c] = make_uint4(w[0], w[1], w[2], w[3]);
+    }
+  }
+  const float mx = warp_max(fmaxf(__low2float(amax2), __high2float(amax2)));
+  if (lane == 0) red[24 + warp] = mx;
+  __syncthreads();
+  float rmax = 0.f;
+#pragma unroll
+  for (int w = 0; w < 8; ++w) rmax = fmaxf(rmax, red[24 + w]);
+  // Row scale 2^sh: the largest magnitude lands in [2^14, 2^15).  The fp16 operands and the fp32 sums are then the
+  // same numbers for x and 2^e x (power-of-two scaling is exact), nothing saturates (|lower half| < 2^15, upper half
+  // < 2^11), and a bf16 element converts to fp16 exactly unless it lies more than 2^27 below the row's largest.
+  const int e = (int)((__float_as_uint(rmax) >> 23) & 0xffu) - 127;   // rmax in [2^e, 2^(e + 1)); a zero row: e = -127
+  const int sh = max(-126, min(126, 14 - e));
+  const float scale = __uint_as_float((uint32_t)(sh + 127) << 23);
   float sx = 0.f;
 #pragma unroll
   for (int c = 0; c < MAXC; ++c) {
     const int k = (c * NT + tid) * 8;
     if (c < nchunk && k < K) {
-      uint32_t w[4] = {xv[c].x, xv[c].y, xv[c].z, xv[c].w};
-      if (norm) {
-        const uint32_t g[4] = {gv[c].x, gv[c].y, gv[c].z, gv[c].w};
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const __nv_bfloat162 v = *reinterpret_cast<const __nv_bfloat162*>(&w[q]);
-          const __nv_bfloat162 gg = *reinterpret_cast<const __nv_bfloat162*>(&g[q]);
-          const __nv_bfloat162 y2 = __hmul2(gg, __hmul2(v, rinv2));
-          w[q] = *reinterpret_cast<const uint32_t*>(&y2);
-        }
-      }
+      const uint32_t w[4] = {xv[c].x, xv[c].y, xv[c].z, xv[c].w};
       // 8 consecutive k = one half of a k16 chunk; pair q belongs to lane 4n + q, register (c16, half)
       const int kb = k >> 6, c16 = (k >> 4) & 3, half = (k >> 3) & 1;
       const float pre = half ? 0.0625f : 1.0f;
       uint32_t* dst = xfrag + ((size_t)(kb * 2 + (c16 >> 1)) * 32 + n * 4) * 4 + (c16 & 1) * 2 + half;
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
-        const float lo = __uint_as_float(w[q] << 16), hi = __uint_as_float(w[q] & 0xffff0000u);
+        const float lo = __uint_as_float(w[q] << 16) * scale, hi = __uint_as_float(w[q] & 0xffff0000u) * scale;
         sx += lo + hi;
         dst[q * 4] = pack_f16x2(lo * pre, hi * pre);
       }
@@ -148,6 +170,7 @@ __global__ void __launch_bounds__(256) q4_batch_prep_kernel(const __nv_bfloat16*
 #pragma unroll
     for (int w = 0; w < 8; ++w) t += red[8 + 8 * tid + w];   // fixed order
     sums[n * 2 + tid] = t;
+    if (tid == 0) sums[2 * MAXB + n] = __uint_as_float((uint32_t)(127 - sh) << 23);   // 2^-sh
   }
 }
 
@@ -266,9 +289,9 @@ __global__ void __launch_bounds__(NTHREADS, 2) q4_gemv_batch_kernel(const BParam
     // ===================== epilogue warp: lane = row of the 32-row unit, all 8 columns =====================
     pdl_wait();
     const float* scratch = reinterpret_cast<const float*>(smem + L.scratch);
-    float sum_lo[MAXB], sum_hi[MAXB];
+    float sum_lo[MAXB], sum_hi[MAXB], rscale[MAXB];
 #pragma unroll
-    for (int n = 0; n < MAXB; ++n) { sum_lo[n] = p.sums[2 * n]; sum_hi[n] = p.sums[2 * n + 1]; }
+    for (int n = 0; n < MAXB; ++n) { sum_lo[n] = p.sums[2 * n]; sum_hi[n] = p.sums[2 * n + 1]; rscale[n] = p.sums[2 * MAXB + n]; }
     if (n_units > 0) named_bar_arrive(4, NCW * 32 + 32);
     if (n_units > 1) named_bar_arrive(5, NCW * 32 + 32);
     for (int u = 0; u < n_units; ++u) {
@@ -301,8 +324,8 @@ __global__ void __launch_bounds__(NTHREADS, 2) q4_gemv_batch_kernel(const BParam
       if (u + 2 < n_units) named_bar_arrive(4 + buf, NCW * 32 + 32);
 #pragma unroll
       for (int n = 0; n < MAXB; ++n) {
-        // t = sum q x + 1024 sum_lo + 64 sum_hi  (see q4_gemv.cu)
-        const float v = rbf(sc * ((t[n] - (1024.0f + zero) * sum_lo[n]) - (64.0f + zero) * sum_hi[n]));
+        // t = sum q x + 64 sum_hi (see kblock_mma), in units of 2^-sh_n: exact
+        const float v = rbf(sc * ((t[n] - zero * sum_lo[n]) - (64.0f + zero) * sum_hi[n]) * rscale[n]);
         if (p.epilogue == B2L_EPI_SWIGLU) {
           const float b = __shfl_down_sync(0xffffffffu, v, 8);
           if (active && row < 8 && n < p.M) {
@@ -394,7 +417,7 @@ extern "C" int b2l_q4_untile_mma(const void* qw_tiled, void* qw, int N, int K, b
 
 extern "C" size_t b2l_q4_gemv_batch_workspace_bytes(int K) {
   if (K <= 0 || K % KB) return 0;
-  return (size_t)(K / KB) * XKB_BYTES + MAXB * 2 * sizeof(float);
+  return (size_t)(K / KB) * XKB_BYTES + MAXB * 3 * sizeof(float);
 }
 
 extern "C" int b2l_q4_gemv_batch(const b2l_q4_linear_args* a, b2l_stream_t stream) {

@@ -90,14 +90,25 @@ __device__ __forceinline__ uint32_t lop_and_or(uint32_t a, uint32_t mask, uint32
   asm("lop3.b32 %0, %1, %2, %3, 0xEA;" : "=r"(d) : "r"(a), "r"(mask), "r"(magic));
   return d;
 }
-// two fp32 -> packed fp16 (lo in bits 0..15), saturating: an activation beyond +-65504 clamps instead of becoming inf
+// two fp32 -> packed fp16 (lo in bits 0..15), saturating (q4_batch_prep_kernel scales every row below 2^15 first)
 __device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi) {
   uint32_t d;
   asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi), "f"(lo));
   return d;
 }
 
-// One k-block position (64 k) of NH 16-row halves: LDS.128 per half, 1 shift + 4 LOP3 per word, 4 MMAs per half.
+// packed fp16 a - b
+__device__ __forceinline__ uint32_t hsub2_u32(uint32_t a, uint32_t b) {
+  uint32_t d;
+  asm("sub.rn.f16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
+  return d;
+}
+
+// One k-block position (64 k) of NH 16-row halves: LDS.128 per half, 1 shift + 4 LOP3 + 2 HADD2 per word, 4 MMAs per
+// half.  The lower k half gets q itself (1024 + q - 1024, exact): with the 1024 left in, the fp32 accumulator would
+// carry 1024 x for every activation x and round at that magnitude, so an output whose level sits at its zero point on
+// a massive channel (|x| ~ 1e4) would be off by many ulps.  The upper half keeps 1024 + 16 q against x / 16, i.e.
+// q x + 64 x: a bias 16 times smaller, removed with the exact row sums in the epilogue.
 template <int NH>
 __device__ __forceinline__ void kblock_mma(float (&acc)[MAX_HALVES][2][4], const uint8_t* wbase, const uint4& xa, const uint4& xb,
                                            uint32_t kmask, uint32_t kmask4, uint32_t kmagic) {
@@ -110,8 +121,8 @@ __device__ __forceinline__ void kblock_mma(float (&acc)[MAX_HALVES][2][4], const
     for (int c = 0; c < 4; ++c) {
       uint32_t a[4];
       const uint32_t w8 = ww[c] >> 8;
-      a[0] = lop_and_or(ww[c], kmask, kmagic);   // row g,     k 2t..2t+1     : 1024 + q
-      a[1] = lop_and_or(w8, kmask, kmagic);      // row g + 8, k 2t..2t+1     : 1024 + q
+      a[0] = hsub2_u32(lop_and_or(ww[c], kmask, kmagic), kmagic);   // row g,     k 2t..2t+1 : q
+      a[1] = hsub2_u32(lop_and_or(w8, kmask, kmagic), kmagic);      // row g + 8, k 2t..2t+1 : q
       a[2] = lop_and_or(ww[c], kmask4, kmagic);  // row g,     k 2t+8..2t+9   : 1024 + 16 q  (x / 16 in B)
       a[3] = lop_and_or(w8, kmask4, kmagic);     // row g + 8, k 2t+8..2t+9   : 1024 + 16 q
       mma_f16_16816(acc[h][c & 1], a, bb[2 * c], bb[2 * c + 1]);

@@ -11,14 +11,14 @@
 // form a thread-block cluster and are reduced through distributed shared memory):
 //
 //   HBM --TMA bulk copy--> smem ring of packed slabs [128 rows][16 B = 32 nibbles]
-//       --LDS.128, LOP3--> registers: bf16 pairs (128 + level), exact, in the wgmma A-fragment order
+//       --LDS.128, LOP3, HSUB2--> registers: bf16 pairs (level), exact, in the wgmma A-fragment order
 //   x (bf16, RMSNorm'd on the fly) --> smem B operand (K-major core matrices)
 //   wgmma.m64nNk16 (N = 8 or 16 token columns), one warpgroup per 64 output rows:
 //       D (registers, fp32) += A (registers) * B (smem descriptor)
-//   y[o] = scale[o] * (acc - (128 + zero[o]) * sum_k x[k])
+//   y[o] = scale[o] * (acc - zero[o] * sum_k x[k])
 //
 // The scale/zero are hoisted out of the K loop (exact algebra, fp32): the tensor core
-// only ever sees the integers 128..143 and the bf16 activations.
+// only ever sees the integers 0..15 and the bf16 activations.
 //
 // Weights do not depend on the previous kernel, so with programmatic dependent launch
 // the TMA producer starts streaming before `griddepcontrol.wait`; only the x load waits.
@@ -147,9 +147,15 @@ template <> struct Wgmma<8> {
   }
 };
 
-// Nibble pair s of one word -> the bf16 pair (128 + level[k], 128 + level[k+1]), k = 8 * word + 2 * s:
-// 0x4300 is bf16 128.0 whose ulp is 1, so OR-ing a 4-bit level into the mantissa is exact.
-__device__ __forceinline__ uint32_t unpack_pair(uint32_t w, int s) { return ((w >> (4 * s)) & 0x000f000fu) | 0x43004300u; }
+// Nibble pair s of one word -> the bf16 pair (level[k], level[k+1]), k = 8 * word + 2 * s: 0x4300 is bf16 128.0
+// whose ulp is 1, so OR-ing a 4-bit level into the mantissa gives 128 + level exactly, and subtracting 128 is exact.
+// Feeding 128 + level would make the fp32 accumulator carry 128 x for every activation and round at that magnitude:
+// an output whose level sits at its zero point on a massive channel (|x| ~ 1e4) would be off by several ulps.
+__device__ __forceinline__ uint32_t unpack_pair(uint32_t w, int s) {
+  uint32_t d;
+  asm("sub.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(((w >> (4 * s)) & 0x000f000fu) | 0x43004300u), "r"(0x43004300u));
+  return d;
+}
 
 #define B2L_TRACE(slot)                                                      \
   do {                                                                       \
@@ -404,7 +410,7 @@ __global__ void __launch_bounds__(NTHREADS, 3) q4_linear_tc_kernel(const Params 
       const int row = r0 + 8 * h;
       const int o = min(nt * TILE_N + row, p.N - 1);  // padded rows of the last tile are never stored
       const float sc = load_sz(p.scales, p.szdt, o);
-      const float zz = 128.0f + load_sz(p.zeros, p.szdt, o);
+      const float zz = load_sz(p.zeros, p.szdt, o);
 #pragma unroll
       for (int c = 0; c < NN / 8; ++c) {
 #pragma unroll

@@ -94,7 +94,7 @@ template <int MAXC>
 __global__ void __launch_bounds__(256) w8_batch_prep_kernel(const __nv_bfloat16* x, int ldx, int M, int K,
                                                             const __nv_bfloat16* __restrict__ norm_scale, float eps,
                                                             uint8_t* __restrict__ ws) {
-  __shared__ float red[24];          // [0..7] sum of squares, [8..15] max |x|, [16..23] max |g|
+  __shared__ float red[16];          // [0..7] sum of squares, [8..15] max |x| (max |bf16(g x)| with RMSNorm)
   __shared__ long long sred[8];
   const int n = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   constexpr int NT = 256;
@@ -102,22 +102,11 @@ __global__ void __launch_bounds__(256) w8_batch_prep_kernel(const __nv_bfloat16*
   pdl_launch_dependents();  // the linear may start streaming its weights
   const bool norm = norm_scale != nullptr;
   uint4 xv[MAXC], gv[MAXC];
-  __nv_bfloat162 gmax2 = __float2bfloat162_rn(0.f);
 #pragma unroll
   for (int c = 0; c < MAXC; ++c) {
     const int k = (c * NT + tid) * 8;
     gv[c] = make_uint4(0, 0, 0, 0);
     if (norm && k < K) gv[c] = *reinterpret_cast<const uint4*>(norm_scale + k);
-  }
-  if (norm) {
-#pragma unroll
-    for (int c = 0; c < MAXC; ++c) {
-      const uint32_t g[4] = {gv[c].x, gv[c].y, gv[c].z, gv[c].w};
-#pragma unroll
-      for (int q = 0; q < 4; ++q) gmax2 = __hmax2(gmax2, __habs2(*reinterpret_cast<const __nv_bfloat162*>(&g[q])));
-    }
-    const float gw = warp_max(fmaxf(__low2float(gmax2), __high2float(gmax2)));
-    if (lane == 0) red[16 + warp] = gw;
   }
   pdl_wait();
 #pragma unroll
@@ -133,14 +122,17 @@ __global__ void __launch_bounds__(256) w8_batch_prep_kernel(const __nv_bfloat16*
   for (int c = 0; c < MAXC; ++c) {
     if (c < nchunk) {
       const uint32_t w[4] = {xv[c].x, xv[c].y, xv[c].z, xv[c].w};
+      const uint32_t g[4] = {gv[c].x, gv[c].y, gv[c].z, gv[c].w};
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
         const __nv_bfloat162 v = *reinterpret_cast<const __nv_bfloat162*>(&w[q]);
-        amax2 = __hmax2(amax2, __habs2(v));
         if (norm) {
+          amax2 = __hmax2(amax2, __habs2(__hmul2(v, *reinterpret_cast<const __nv_bfloat162*>(&g[q]))));
           const __nv_bfloat162 sq = __hmul2(v, v);
           const uint32_t su = *reinterpret_cast<const uint32_t*>(&sq);
           ss += __uint_as_float(su << 16) + __uint_as_float(su & 0xffff0000u);
+        } else {
+          amax2 = __hmax2(amax2, __habs2(v));
         }
       }
     }
@@ -150,14 +142,13 @@ __global__ void __launch_bounds__(256) w8_batch_prep_kernel(const __nv_bfloat16*
   mx = warp_max(mx);
   if (lane == 0) { red[warp] = ss; red[8 + warp] = mx; }
   __syncthreads();
-  float gm = 0.f;
   ss = 0.f; mx = 0.f;
 #pragma unroll
-  for (int w = 0; w < 8; ++w) { ss += red[w]; mx = fmaxf(mx, red[8 + w]); if (norm) gm = fmaxf(gm, red[16 + w]); }
+  for (int w = 0; w < 8; ++w) { ss += red[w]; mx = fmaxf(mx, red[8 + w]); }
   float rinv = 1.f;
   if (norm) {
     rinv = rms_rinv(ss, K, eps);
-    mx = mx * gm * rinv * 1.01f;
+    mx = mx * rinv * 1.02f;   // > max |bf16(g bf16(x rinv))|: the bound and its proof are q4_gemv.cu's
   }
   const int e = (int)((__float_as_uint(mx) >> 23) & 0xffu) - 127;
   int sh = (8 * NDIG - 3) - e;

@@ -32,7 +32,7 @@ def build_tiny(dev, cfg, mode="gptq.int4", seed=1234, tile_cols=-1, exact_linear
 def assert_q4_linear_close(y, x, lv, sc, z, min_equal=0.8):
     """An int4 linear output against exact arithmetic: every element within the final bf16 rounding (2^-8
     relative) plus 2^-12 of the row's magnitude sum_k |(lv - z) s x| (the 2..8-row kernel accumulates
-    (1024 + lv) x in fp32, DESIGN.md Numerics: measured ~2^-15 of that magnitude), and at least `min_equal` of the
+    lv x + 64 x over half of k in fp32, DESIGN.md Numerics), and at least `min_equal` of the
     elements bit-equal to the correctly rounded result (the batch-1 kernel is exact integer arithmetic up to one
     fp32 and one bf16 rounding: callers pass min_equal=0.995 for it)."""
     want = ref_linear(x, lv, sc, z)
