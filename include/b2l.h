@@ -391,6 +391,22 @@ int b2l_topk_softmax(const void* logits, float temperature, int top_k, void* pro
 int b2l_topk_softmax_sample(const void* logits, float temperature, int top_k, const void* noise, void* probs,
                             int64_t* token, int V, b2l_stream_t stream);
 
+/* The two entry points above over B rows in one launch (one CTA per row): parallel samples of one prompt,
+ * generate.py:68-76 for every row of a batched decode step (lit_llama_b200.generate_batch).  Row b reads
+ * logits + b * ld (bf16; ld == 0: every row reads the same V logits, e.g. the prefill's last position when all
+ * samples share a prompt) and noise + b * V (bf16 [B, V], q ~ Exp(1) drawn by the caller as
+ * `torch.empty_like(probs).exponential_(1)` on probs [B, V]), and writes probs + b * V (bf16 [B, V], may be NULL
+ * for the _sample_ form) and tokens[b] (device int64 [B]).  Row b equals the B = 1 call on that row: probs bit for
+ * bit, and tokens[b] == torch.multinomial(probs, 1)[b] for the same generator state (argmax(probs / q) per row, ties
+ * to the lower index).  logits and noise 16-byte aligned; rows that do not start on 16 bytes (V or ld not a multiple
+ * of 8) are read element-wise.  Null pointers, B < 1, 0 < ld < V (or ld < 0) and misaligned logits / noise are
+ * B2L_E_ARG, with a message naming the argument, before the device is touched.  b2l_topk_softmax and
+ * b2l_topk_softmax_sample are the B = 1, ld = V case. */
+int b2l_topk_softmax_rows(const void* logits, int64_t ld, float temperature, int top_k, void* probs, int B, int V,
+                          b2l_stream_t stream);
+int b2l_topk_softmax_sample_rows(const void* logits, int64_t ld, float temperature, int top_k, const void* noise,
+                                 void* probs, int64_t* tokens, int B, int V, b2l_stream_t stream);
+
 /* ------------------------------------------------------------------------------
  * CausalSelfAttention.forward without the two linears, model.py:197-232:
  * split qkv, apply_rope(q), apply_rope(k) (model.py:306-323), append k,v to the

@@ -163,6 +163,9 @@ _SIGS = {
     "b2l_linear_affine": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "b2l_topk_softmax": (c_int, [c_void_p, c_float, c_int, c_void_p, c_int, c_void_p]),
     "b2l_topk_softmax_sample": (c_int, [c_void_p, c_float, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
+    "b2l_topk_softmax_rows": (c_int, [c_void_p, C.c_int64, c_float, c_int, c_void_p, c_int, c_int, c_void_p]),
+    "b2l_topk_softmax_sample_rows": (c_int, [c_void_p, C.c_int64, c_float, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                                             c_void_p]),
     "b2l_q8_tiled_bytes": (c_size_t, [c_int, c_int]),
     "b2l_q8_tile": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "b2l_q8_gemv": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_int, c_void_p]),

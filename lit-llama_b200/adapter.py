@@ -139,6 +139,12 @@ class LLaMA(llama.LLaMA):
         self.adapter_kv_caches.clear()
         self._adapter_gen = None
 
+    def expand_cache(self, B: int) -> None:
+        """model.LLaMA.expand_cache; the prefix store does not depend on B, so only its (B, nh, aT, hs) views follow."""
+        super().expand_cache(B)
+        self.adapter_kv_caches = [None if c is None else (c[0][:1].expand(B, -1, -1, -1), c[1][:1].expand(B, -1, -1, -1))
+                                  for c in self.adapter_kv_caches]
+
     def _apply(self, fn, recurse=True):
         out = super()._apply(fn, recurse)
         self._adapter_store = self._adapter_gates = self._adapter_arr = None

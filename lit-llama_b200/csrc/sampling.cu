@@ -1,10 +1,13 @@
 // The sampling tail of generate() (generate.py:68-75) up to the probabilities:
 //   logits / temperature -> top-k threshold -> where(logits < thr, -inf, logits) -> softmax
-// as ONE single-CTA kernel (the reference spends ~10 launches, including a radix sort for
-// topk), optionally followed in the same kernel by the draw itself: torch.multinomial(probs, 1) is
-// argmax(probs / q) with q ~ Exp(1) (ATen/native/Distributions.cpp); the caller draws q with torch
-// (`empty_like(probs).exponential_(1)`, the same RNG consumption as multinomial) so the sampled
-// token equals the reference's for the same generator state, without multinomial's ~12 launches.
+// as ONE kernel with one CTA per logits row (the reference spends ~10 launches per row, including a
+// radix sort for topk), optionally followed in the same kernel by the draw itself:
+// torch.multinomial(probs, 1) is argmax(probs / q) per row with q ~ Exp(1)
+// (ATen/native/Distributions.cpp); the caller draws q [B, V] with torch (`empty_like(probs).exponential_(1)`,
+// the same RNG consumption as multinomial) so each row's token equals the reference's for the same
+// generator state, without multinomial's ~12 launches.  B rows (generate_batch's parallel samples) run
+// as B CTAs of the same launch; row b reads logits + b * ld (ld == 0: every row draws from the same
+// logits, the prefill's last position), noise + b * V, and writes probs + b * V and token[b].
 //
 // Rounding points follow the reference as it runs on the GPU in bf16:
 //   * logits / temperature is a bf16 tensor: ATen multiplies by the fp32 reciprocal of the
@@ -56,11 +59,28 @@ __device__ __forceinline__ void find_bin(const int* hist, int want, int* sel_bin
 
 __device__ __forceinline__ float bits_f(uint32_t bits16) { return __uint_as_float(bits16 << 16); }
 
+// elements 8i..8i+7 of a bf16 row: one 16-byte load, or eight 2-byte loads for a row that does not start on 16 bytes
+// (V or ld not a multiple of 8)
+__device__ __forceinline__ uint4 load8(const __nv_bfloat16* p, int i, bool vec) {
+  if (vec) return reinterpret_cast<const uint4*>(p)[i];
+  const uint16_t* s = reinterpret_cast<const uint16_t*>(p) + 8 * i;
+  return make_uint4(s[0] | ((uint32_t)s[1] << 16), s[2] | ((uint32_t)s[3] << 16), s[4] | ((uint32_t)s[5] << 16),
+                    s[6] | ((uint32_t)s[7] << 16));
+}
+
 __global__ void __launch_bounds__(SAMP_THREADS)
-    topk_softmax_kernel(const __nv_bfloat16* __restrict__ logits, float inv_temperature, int top_k,
+    topk_softmax_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, float inv_temperature, int top_k,
                         __nv_bfloat16* __restrict__ probs, const __nv_bfloat16* __restrict__ noise,
                         long long* __restrict__ token, int V) {
   extern __shared__ __align__(16) uint8_t ssm[];
+  {  // this CTA's row
+    const size_t row = blockIdx.x;
+    logits += row * (size_t)ld;
+    if (noise != nullptr) noise += row * (size_t)V;
+    if (probs != nullptr) probs += row * (size_t)V;
+    if (token != nullptr) token += row;
+  }
+  const bool vec = ((reinterpret_cast<uintptr_t>(logits) | reinterpret_cast<uintptr_t>(noise)) & 15) == 0;
   const int Vp = (V + 7) & ~7;
   uint16_t* sv = reinterpret_cast<uint16_t*>(ssm);  // scaled logits as bf16 bits [Vp]
   uint16_t* sq = sv + Vp;                            // Exp(1) noise as bf16 bits [Vp] (only with `noise`)
@@ -81,8 +101,8 @@ __global__ void __launch_bounds__(SAMP_THREADS)
     lpre[r] = make_uint4(0, 0, 0, 0);
     npre[r] = make_uint4(0, 0, 0, 0);
     if (i < nvec) {
-      lpre[r] = reinterpret_cast<const uint4*>(logits)[i];
-      if (noise != nullptr) npre[r] = reinterpret_cast<const uint4*>(noise)[i];
+      lpre[r] = load8(logits, i, vec);
+      if (noise != nullptr) npre[r] = load8(noise, i, vec);
     }
   }
 
@@ -100,7 +120,7 @@ __global__ void __launch_bounds__(SAMP_THREADS)
       const int i = r * SAMP_THREADS + tid;
       const bool valid = i < nvec;
       uint4 v = lpre[rr];
-      if (r0 > 0) { v = make_uint4(0, 0, 0, 0); if (valid) v = reinterpret_cast<const uint4*>(logits)[i]; }
+      if (r0 > 0) { v = make_uint4(0, 0, 0, 0); if (valid) v = load8(logits, i, vec); }
       const uint32_t w[4] = {v.x, v.y, v.z, v.w};
       uint32_t o[4];
 #pragma unroll
@@ -119,7 +139,7 @@ __global__ void __launch_bounds__(SAMP_THREADS)
         reinterpret_cast<uint4*>(sv)[i] = make_uint4(o[0], o[1], o[2], o[3]);
         if (noise != nullptr) {
           uint4 n = npre[rr];
-          if (r0 > 0) n = reinterpret_cast<const uint4*>(noise)[i];
+          if (r0 > 0) n = load8(noise, i, vec);
           reinterpret_cast<uint4*>(sq)[i] = n;
         }
       }
@@ -279,9 +299,10 @@ __global__ void __launch_bounds__(SAMP_THREADS)
 
 using namespace b2l;
 
-static int launch_topk(const void* logits, float temperature, int top_k, void* probs, const void* noise, void* token, int V,
-                       b2l_stream_t stream, const char* who) {
+static int launch_topk(const void* logits, long long ld, float temperature, int top_k, void* probs, const void* noise, void* token,
+                       int B, int V, b2l_stream_t stream, const char* who) {
   B2L_CHECK_ARG(logits && V > 0 && temperature > 0.f && top_k >= 0, "%s: bad argument", who);
+  B2L_CHECK_ARG(ld == 0 || ld >= V, "%s: ld = %lld: 0 (every row reads the same logits) or at least V = %d", who, ld, V);
   B2L_CHECK_ARG(((uintptr_t)logits % 16) == 0, "%s: logits must be 16-byte aligned", who);
   B2L_CHECK_ARG(noise == nullptr || ((uintptr_t)noise % 16) == 0, "%s: noise must be 16-byte aligned", who);
   const size_t Vp = ((size_t)V + 7) & ~(size_t)7;
@@ -290,7 +311,7 @@ static int launch_topk(const void* logits, float temperature, int top_k, void* p
   static DynSmemCache smem_cache;
   if (smem > 48 * 1024)
     if (int rc = ensure_dyn_smem(topk_softmax_kernel, smem, smem_cache)) return rc;
-  topk_softmax_kernel<<<1, SAMP_THREADS, smem, (cudaStream_t)stream>>>((const __nv_bfloat16*)logits, 1.0f / temperature, top_k,
+  topk_softmax_kernel<<<B, SAMP_THREADS, smem, (cudaStream_t)stream>>>((const __nv_bfloat16*)logits, ld, 1.0f / temperature, top_k,
                                                                       (__nv_bfloat16*)probs, (const __nv_bfloat16*)noise,
                                                                       (long long*)token, V);
   B2L_LAUNCH_CHECK("topk_softmax_kernel");
@@ -299,11 +320,38 @@ static int launch_topk(const void* logits, float temperature, int top_k, void* p
 
 extern "C" int b2l_topk_softmax(const void* logits, float temperature, int top_k, void* probs, int V, b2l_stream_t stream) {
   B2L_CHECK_ARG(probs != nullptr, "b2l_topk_softmax: null probs");
-  return launch_topk(logits, temperature, top_k, probs, nullptr, nullptr, V, stream, "b2l_topk_softmax");
+  return launch_topk(logits, V, temperature, top_k, probs, nullptr, nullptr, 1, V, stream, "b2l_topk_softmax");
 }
 
 extern "C" int b2l_topk_softmax_sample(const void* logits, float temperature, int top_k, const void* noise, void* probs,
                                        int64_t* token, int V, b2l_stream_t stream) {
   B2L_CHECK_ARG(noise != nullptr && token != nullptr, "b2l_topk_softmax_sample: null noise / token");
-  return launch_topk(logits, temperature, top_k, probs, noise, token, V, stream, "b2l_topk_softmax_sample");
+  return launch_topk(logits, V, temperature, top_k, probs, noise, token, 1, V, stream, "b2l_topk_softmax_sample");
+}
+
+// the checks every row entry point makes before launch_topk's, each naming its argument
+static int check_rows(const void* logits, int B, int V, float temperature, int top_k, const char* who) {
+  B2L_CHECK_ARG(logits != nullptr, "%s: null logits", who);
+  B2L_CHECK_ARG(B >= 1, "%s: B = %d rows, at least 1", who, B);
+  B2L_CHECK_ARG(V > 0, "%s: V = %d, at least 1", who, V);
+  B2L_CHECK_ARG(temperature > 0.f, "%s: temperature %g, must be positive", who, (double)temperature);
+  B2L_CHECK_ARG(top_k >= 0, "%s: top_k = %d, 0 (no filter) or positive", who, top_k);
+  return 0;
+}
+
+extern "C" int b2l_topk_softmax_rows(const void* logits, int64_t ld, float temperature, int top_k, void* probs, int B, int V,
+                                     b2l_stream_t stream) {
+  const char* who = "b2l_topk_softmax_rows";
+  if (int rc = check_rows(logits, B, V, temperature, top_k, who)) return rc;
+  B2L_CHECK_ARG(probs != nullptr, "%s: null probs", who);
+  return launch_topk(logits, ld, temperature, top_k, probs, nullptr, nullptr, B, V, stream, who);
+}
+
+extern "C" int b2l_topk_softmax_sample_rows(const void* logits, int64_t ld, float temperature, int top_k, const void* noise,
+                                            void* probs, int64_t* tokens, int B, int V, b2l_stream_t stream) {
+  const char* who = "b2l_topk_softmax_sample_rows";
+  if (int rc = check_rows(logits, B, V, temperature, top_k, who)) return rc;
+  B2L_CHECK_ARG(noise != nullptr, "%s: null noise", who);
+  B2L_CHECK_ARG(tokens != nullptr, "%s: null tokens", who);
+  return launch_topk(logits, ld, temperature, top_k, probs, noise, tokens, B, V, stream, who);
 }

@@ -2,13 +2,15 @@
 
 `generate()` keeps the reference's Python token loop and torch sampling ops (so the
 RNG stream of `torch.multinomial` is the reference's); the model call inside it is one
-CUDA-graph replay per token.  `main()` mirrors the reference CLI with argparse
+CUDA-graph replay per token.  `generate_batch()` draws up to 16 samples of one prompt
+at once: one batch-1 prefill, then one batched decode step and one sampling launch per
+token for all samples.  `main()` mirrors the reference CLI with argparse
 (jsonargparse and lightning are not dependencies of this path)."""
 import os
 import sys
 import time
 from pathlib import Path
-from typing import Optional
+from typing import List, Optional
 
 import torch
 
@@ -20,10 +22,42 @@ from .utils import llama_model_lookup, quantization
 _TORCH_MULTINOMIAL = torch.multinomial
 
 
+#: most samples generate_batch() draws at once: the range of the batched decode step (B = 2..16)
+MAX_SAMPLES = 16
+
+
+def _rows(logits: torch.Tensor):
+    """(x, ld) for the row entry points: (B, V) logits with unit stride along V and 16-byte aligned, rows ld >= V
+    elements apart, or ld = 0 for one row expanded to B rows (`row.expand(B, -1)`); read in place when they already
+    are, else copied."""
+    B, V = logits.shape
+    if B > 1 and logits.stride(0) == 0:   # one row for every sample
+        row = logits[0].contiguous()
+        if row.data_ptr() % 16:
+            row = row.clone()
+        return row, 0
+    x = logits
+    if (V > 1 and x.stride(1) != 1) or (B > 1 and x.stride(0) < V):
+        x = x.contiguous()
+    if x.data_ptr() % 16:
+        x = x.clone(memory_format=torch.contiguous_format)   # the kernel reads 16-byte vectors
+    return x, (x.stride(0) if B > 1 else V)
+
+
 def sample_probs(logits_row: torch.Tensor, temperature: float = 1.0, top_k: Optional[int] = None) -> torch.Tensor:
     """generate.py:68-75: probabilities of the next token from the last position's logits
-    (V,) bf16: temperature, top-k filter and softmax fused in one kernel (b2l_topk_softmax)."""
+    (V,) bf16: temperature, top-k filter and softmax fused in one kernel (b2l_topk_softmax).
+    (B, V) logits give (B, V) probabilities, every row in the same launch (b2l_topk_softmax_rows), each row bit-equal
+    to the (V,) call on it."""
     L.require_cuda_bf16(logits_row, "sample_probs")
+    if logits_row.dim() == 2:
+        x, ld = _rows(logits_row)
+        B, V = logits_row.shape
+        probs = torch.empty((B, V), dtype=x.dtype, device=x.device)
+        k = 0 if top_k is None else min(int(top_k), V)
+        L.check(L.lib().b2l_topk_softmax_rows(x.data_ptr(), ld, float(temperature), k, probs.data_ptr(), B, V, L.stream_ptr()),
+                "b2l_topk_softmax_rows")
+        return probs
     x = logits_row.contiguous()
     if x.data_ptr() % 16:
         x = x.clone()  # the kernel reads 16-byte vectors
@@ -39,8 +73,20 @@ def sample_token(logits_row: torch.Tensor, temperature: float = 1.0, top_k: Opti
     `torch.multinomial(probs, num_samples=1)` is `argmax(probs / q)` with `q = empty_like(probs).exponential_(1)`
     (ATen/native/Distributions.cpp); q is drawn here with torch -- the RNG consumption of multinomial, so for the same
     generator state the token equals `torch.multinomial(sample_probs(...), 1)` -- and everything else is one
-    launch (b2l_topk_softmax_sample) instead of multinomial's dozen."""
+    launch (b2l_topk_softmax_sample) instead of multinomial's dozen.
+    (B, V) logits give (B,) tokens: q is one [B, V] draw, as multinomial makes on [B, V] probabilities, so token b
+    equals `torch.multinomial(sample_probs(logits), 1)[b]`, and all rows are drawn in one launch
+    (b2l_topk_softmax_sample_rows)."""
     L.require_cuda_bf16(logits_row, "sample_token")
+    if logits_row.dim() == 2:
+        x, ld = _rows(logits_row)
+        B, V = logits_row.shape
+        q = torch.empty((B, V), dtype=x.dtype, device=x.device).exponential_(1)
+        tokens = torch.empty(B, dtype=torch.int64, device=x.device)
+        k = 0 if top_k is None else min(int(top_k), V)
+        L.check(L.lib().b2l_topk_softmax_sample_rows(x.data_ptr(), ld, float(temperature), k, q.data_ptr(), None, tokens.data_ptr(),
+                                                     B, V, L.stream_ptr()), "b2l_topk_softmax_sample_rows")
+        return tokens
     x = logits_row.contiguous()
     if x.data_ptr() % 16:
         x = x.clone()  # the kernel reads 16-byte vectors
@@ -92,6 +138,77 @@ def generate(
     return idx
 
 
+@torch.no_grad()
+def generate_batch(
+    model: LLaMA,
+    idx: torch.Tensor,
+    num_samples: int,
+    max_new_tokens: int,
+    *,
+    max_seq_length: Optional[int] = None,
+    temperature: float = 1.0,
+    top_k: Optional[int] = None,
+    eos_id: Optional[int] = None,
+) -> List[torch.Tensor]:
+    """`num_samples` (1..16) continuations of one prompt `idx` (T,), drawn together: a list of `num_samples` 1-D
+    tensors, each the prompt plus that sample's new tokens (generate.py:20-91 per row).
+
+    The prompt is prefilled once, at batch 1, and `LLaMA.expand_cache` copies its KV cache to every row; the first
+    tokens are all drawn from the prefill's last position.  Each later token is one batched model call (whatever path
+    the model runs at B = num_samples) and one sampling launch for all rows; positions are shared, so the roll branch
+    (model.py:214-218) applies when T + max_new_tokens > max_seq_length.  Row b's token is
+    `torch.multinomial(probs, 1)[b]` of the step's [B, V] probabilities, with multinomial's RNG consumption, so
+    `num_samples=1` gives `generate()`'s tokens for the same seed.
+
+    With `eos_id`, a row that draws it ends there, the eos token included; finished rows keep riding along (their
+    later tokens are dropped) and the loop stops once every row has finished, reading one flag per step.  The cache
+    is left at B = num_samples: call `model.reset_cache()` before the next prompt, as after `generate()`."""
+    if not 1 <= int(num_samples) <= MAX_SAMPLES:
+        raise ValueError(f"generate_batch: num_samples = {num_samples}; 1..{MAX_SAMPLES} (the batched decode step's range)")
+    if idx.dim() != 1:
+        raise ValueError(f"generate_batch: idx must be one prompt of shape (T,), got {tuple(idx.shape)}")
+    if not idx.is_cuda:
+        raise RuntimeError(f"generate_batch: idx is on {idx.device}; lit_llama_b200 runs on CUDA only (no CPU fallback)")
+    B = int(num_samples)
+    T = idx.size(0)
+    T_new = T + max_new_tokens
+    if max_seq_length is None:
+        max_seq_length = min(T_new, model.config.block_size)
+
+    device, dtype = idx.device, idx.dtype
+    out = torch.empty((B, T_new), dtype=dtype, device=device)
+    out[:, :T] = idx
+    input_pos = torch.arange(0, T, device=device)
+    x = idx.view(1, -1)
+    end = torch.full((B,), T_new, dtype=torch.int64, device=device) if eos_id is not None else None
+    done = torch.zeros(B, dtype=torch.bool, device=device) if eos_id is not None else None
+
+    for i in range(max_new_tokens):
+        logits = model(x, max_seq_length, input_pos)
+        if i == 0:
+            model.expand_cache(B)
+            rows = logits[0, -1].expand(B, -1)   # every sample's first token comes from the prompt's last position
+        else:
+            rows = logits[:, -1]
+        if torch.multinomial is _TORCH_MULTINOMIAL:
+            idx_next = sample_token(rows, temperature, top_k).to(dtype=dtype)   # one RNG draw + one launch for all rows
+        else:
+            # torch.multinomial has been replaced (as in generate()): keep calling it, on the fused [B, V] probabilities
+            idx_next = torch.multinomial(sample_probs(rows, temperature, top_k), num_samples=1).view(B).to(dtype=dtype)
+        input_pos = input_pos[-1:] + 1
+        out[:, T + i] = idx_next
+        x = idx_next.view(B, 1)
+        if eos_id is not None:
+            hit = (idx_next == eos_id) & ~done
+            end = torch.where(hit, T + i + 1, end)   # include the eos token
+            done |= hit
+            if bool(done.all()):
+                break
+    if end is None:
+        return list(out.unbind(0))
+    return [out[b, :n] for b, n in enumerate(end.tolist())]
+
+
 def main(
     prompt: str = "Hello, my name is",
     *,
@@ -102,8 +219,12 @@ def main(
     checkpoint_path: Path = Path("checkpoints/lit-llama/7B/lit-llama.pth"),
     tokenizer_path: Path = Path("checkpoints/lit-llama/tokenizer.model"),
     quantize: Optional[str] = None,
+    batch_size: int = 1,
 ) -> None:
-    """generate.py:94-155 without Fabric: bf16 on cuda:0, same prints on stderr."""
+    """generate.py:94-155 without Fabric: bf16 on cuda:0, same prints on stderr.  `batch_size` > 1 draws the samples
+    in groups of up to `batch_size` (at most 16) through `generate_batch`, on the model's exact batched decode step."""
+    if not 1 <= batch_size <= MAX_SAMPLES:
+        raise ValueError(f"batch_size = {batch_size}; 1..{MAX_SAMPLES}")
     from sentencepiece import SentencePieceProcessor
 
     checkpoint_path, tokenizer_path = Path(checkpoint_path), Path(tokenizer_path)
@@ -136,16 +257,38 @@ def main(
     prompt_length = encoded.size(0)
 
     torch.manual_seed(1234)
-    for i in range(num_samples):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        y = generate(model, encoded, max_new_tokens, temperature=temperature, top_k=top_k)
-        torch.cuda.synchronize()
-        t = time.perf_counter() - t0
-        model.reset_cache()
-        print(sp.decode(y.tolist()))
-        tokens_generated = y.size(0) - prompt_length
-        print(f"Time for inference {i + 1}: {t:.02f} sec total, {tokens_generated / t:.02f} tokens/sec", file=sys.stderr)
+    if batch_size == 1:
+        for i in range(num_samples):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            y = generate(model, encoded, max_new_tokens, temperature=temperature, top_k=top_k)
+            torch.cuda.synchronize()
+            t = time.perf_counter() - t0
+            model.reset_cache()
+            print(sp.decode(y.tolist()))
+            tokens_generated = y.size(0) - prompt_length
+            print(f"Time for inference {i + 1}: {t:.02f} sec total, {tokens_generated / t:.02f} tokens/sec", file=sys.stderr)
+    else:
+        # the exact 2..16-row decode step of each quantized base (each row bit-identical to the batch-1 step on it);
+        # without it a compacted gptq.int4 model re-tiles every linear at B >= 2 and gptq.int8 runs module by module
+        if quantize == "gptq.int4":
+            model.q4_batch_step = True
+        elif quantize == "gptq.int8":
+            model.w8_batch_step = True
+        elif quantize == "llm.int8":
+            model.int8_step = True
+        for i, first in enumerate(range(0, num_samples, batch_size)):
+            n = min(batch_size, num_samples - first)
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            ys = generate_batch(model, encoded, n, max_new_tokens, temperature=temperature, top_k=top_k)
+            torch.cuda.synchronize()
+            t = time.perf_counter() - t0
+            model.reset_cache()
+            for y in ys:
+                print(sp.decode(y.tolist()))
+            tokens_generated = sum(y.size(0) - prompt_length for y in ys)
+            print(f"Time for inference {i + 1}: {t:.02f} sec total, {tokens_generated / t:.02f} tokens/sec", file=sys.stderr)
     print(f"Memory used: {torch.cuda.max_memory_reserved() / 1e9:.02f} GB", file=sys.stderr)
 
 
@@ -161,6 +304,8 @@ def cli() -> None:
     ap.add_argument("--checkpoint_path", type=Path, default=Path("checkpoints/lit-llama/7B/lit-llama.pth"))
     ap.add_argument("--tokenizer_path", type=Path, default=Path("checkpoints/lit-llama/tokenizer.model"))
     ap.add_argument("--quantize", default=None, choices=[None, "llm.int8", "gptq.int4", "gptq.int8"])
+    ap.add_argument("--batch_size", type=int, default=1,
+                    help=f"samples drawn together per generate_batch call (1..{MAX_SAMPLES}; 1: one generate() per sample)")
     a = ap.parse_args()
     main(**vars(a))
 

@@ -540,6 +540,24 @@ class LLaMA(nn.Module):
         if self._ring is not None:
             self._ring.zero_()
 
+    def expand_cache(self, B: int) -> None:
+        """Broadcast a batch-1 KV cache to B rows: every row then holds the prompt's keys and values, so B samples of one
+        prompt decode from one batch-1 prefill (generate_batch) instead of a (B, T) prefill at B times the GEMM work.
+        One device copy of the KV store; `kv_caches` become views of the new store, the ring offset (shared by all rows)
+        is kept, and the decode state and module graph, which point at the old store, are rebuilt on the next step.
+        `reset_cache()` returns the model to batch 1."""
+        if self._kv_store is None:
+            raise RuntimeError("expand_cache: no KV cache yet (run the prompt through forward with input_pos first)")
+        n_layer, two, B0, nh, S, hs = self._kv_store.shape
+        if B == B0:
+            return
+        if B0 != 1 or B < 1:
+            raise ValueError(f"expand_cache: the cache holds {B0} rows; only a batch-1 cache expands (to {B} rows)")
+        self._kv_store = self._kv_store.expand(n_layer, two, B, nh, S, hs).contiguous()
+        self.kv_caches = [(self._kv_store[i, 0], self._kv_store[i, 1]) for i in range(n_layer)]
+        self._decode = None
+        self._module_graph = None
+
     # ------------------------------------------------------------------ helpers
     def _fc12(self, i: int, kind: str):
         """c_fc1 and c_fc2 of layer i interleaved (8 rows / 8 rows per 16-row block for the
