@@ -205,8 +205,8 @@ __global__ void kv_unroll_kernel(const __nv_bfloat16* __restrict__ cache, const 
 // slots, and the cross-split merge (last CTA of a head, atomic ticket).
 //
 // grid (B*n_head, ceil(S / 64)), 8 warps; CTAs beyond the position-dependent split count exit at once.  A CTA owns
-// 64..256 keys of one head (chosen from the position so that ~400 CTAs work) and streams them as 64-key
-// sub-tiles (K 16 KB + V 16 KB) through a two-deep shared-memory ring with TMA bulk copies: the first two
+// 64..256 keys of one head (chosen from the position and n_head so that ~400 CTAs work per batch row) and streams
+// them as 64-key sub-tiles (K 16 KB + V 16 KB) through a two-deep shared-memory ring with TMA bulk copies: the first two
 // sub-tiles are requested BEFORE griddepcontrol.wait (old cache rows do not depend on the current token), the
 // next one as soon as a buffer has been consumed.  A warp handles 4 keys per round: 8 lanes per key, 16 head
 // dims (32 B) per lane, a score needs 3 shuffles.  The new token's key / value never touch the tile: they are
@@ -321,10 +321,12 @@ __global__ void __launch_bounds__(FD_WARPS * 32, ADAPTER ? FD_CTAS_PER_SM : 0)
   const int w_slot = (int)(p < S ? p : (long long)S - 1);  // logical slot of the new token
   const int L = w_slot + 1;                                 // valid logical slots 0..L-1
   // keys per CTA: a multiple of 64 in [64, 256], chosen (identically by every CTA) so that at most target_ctas CTAs
-  // have work: few long chunks would serialise sub-tiles inside a CTA, many short ones would need a second wave
-  // (a sub-tile costs a CTA much less than the cross-CTA merge, tools/diag.py bench_ctx -- up to 256 keys stay in ONE
-  // CTA per head, with no merge at all)
-  const int want_splits = max(1, target_ctas / (int)gridDim.x);
+  // per batch row have work: few long chunks would serialise sub-tiles inside a CTA, many short ones would need a
+  // second wave (a sub-tile costs a CTA much less than the cross-CTA merge, tools/diag.py bench_ctx -- up to 256 keys
+  // stay in ONE CTA per head, with no merge at all).  The plan is a function of (L, n_head, SM count) only, never of
+  // B: it fixes the fp32 order of the online softmax and of the merge, so every row of a B-row launch equals the
+  // B = 1 launch on that row's cache bit for bit (at B >= 2 and long context that is more than one wave of CTAs).
+  const int want_splits = max(1, target_ctas / n_head);
   const int chunk = L <= FD_CHUNK ? FD_CHUNK
                                   : min(FD_CHUNK, max(FD_SUB, FD_SUB * ((L + FD_SUB * want_splits - 1) / (FD_SUB * want_splits))));
   const int n_active = (L + chunk - 1) / chunk;
