@@ -156,9 +156,13 @@ enum {
                            the b2l_q4_tile_i8 tilings in qw_mma; batch_work must hold
                            b2l_w8_gemv_batch_workspace_bytes(max K, B) bytes; not with B2L_F_W8, B2L_F_Q8 or
                            B2L_F_W8_BATCH; no plan, no affines */
-  B2L_F_Q8_BATCH = 512  /* b2l_decode_step with B2L_F_Q8 at B in 2..16: every linear runs b2l_q8_linear_batch on
+  B2L_F_Q8_BATCH = 512, /* b2l_decode_step with B2L_F_Q8 at B in 2..16: every linear runs b2l_q8_linear_batch on
                            CB / SCB in place; batch_work must hold b2l_q8_linear_batch_workspace_bytes(max K, B)
                            bytes; v2 affines allowed; not with B2L_F_W8, B2L_F_W8_BATCH or B2L_F_Q4_BATCH_I8; no plan */
+  B2L_F_ROW_POS = 1024  /* b2l_attention(_adapter) at T == 1 and b2l_decode_step: one position per row.
+                           input_pos is int64[B] (row b's token is at input_pos[b]) and ring_start int32[B] (row b's
+                           own ring offset); not with B2L_F_ROPE_ROWS or a persistent plan.  The step advances each
+                           row's ring on its own (b2l_ring_advance_rows) */
 };
 
 /* Fused [RMSNorm ->] int4 linear [-> residual | SwiGLU] on wgmma (M <= 16).  Replaces
@@ -419,6 +423,9 @@ int b2l_topk_softmax_sample_rows(const void* logits, int64_t ld, float temperatu
  * input_pos int64 [T] on the device (never read by the host).  Query t writes its
  *            k,v at logical slot min(input_pos[t], S-1) and attends slots <= that.
  * ring_start int32 [1] on the device, read-only here; b2l_ring_advance moves it
+ * With B2L_F_ROW_POS (T == 1): input_pos int64 [B] and ring_start int32 [B], row b at
+ *            its own position and ring offset (b2l_ring_advance_rows moves them).  Each
+ *            row's y and cache rows equal a B = 1 launch on that row bit for bit.
  * y     bf16 [B, T, C]
  * work  scratch of b2l_attn_workspace_bytes(...) bytes (split-S partials + tickets);
  *       the caller zero-fills it ONCE after allocating it
@@ -455,6 +462,10 @@ int b2l_tp_allreduce(const b2l_tp_comm* comm, const void* partial, void* out, in
  * overwrite of slot S-1 does).  Call once per forward, before the layers. */
 int b2l_ring_advance(const int64_t* input_pos, int T, int32_t* ring_start, int S,
                      b2l_stream_t stream);
+/* The same for B rows at their own positions (B2L_F_ROW_POS): input_pos int64 [B], ring_start
+ * int32 [B]; row b's ring advances when input_pos[b] >= S. */
+int b2l_ring_advance_rows(const int64_t* input_pos, int B, int32_t* ring_start, int S,
+                          b2l_stream_t stream);
 
 /* Same without a cache (input_pos is None, model.py:104-106): positions 0..T-1.
  * qkv is rotated in place; work as for b2l_attention with S = T. */
@@ -525,6 +536,9 @@ int b2l_lora_apply(const b2l_lora* lora, const void* x, int ldx, const void* nor
  * into `out` [B, nh, S, hs]. */
 int b2l_kv_unroll(const void* cache, const int32_t* ring_start, void* out, int B, int n_head,
                   int S, int head_size, b2l_stream_t stream);
+/* The same with one ring offset per row (B2L_F_ROW_POS): ring_start int32 [B]. */
+int b2l_kv_unroll_rows(const void* cache, const int32_t* ring_start, void* out, int B, int n_head,
+                       int S, int head_size, b2l_stream_t stream);
 
 /* ------------------------------------------------------------------------------
  * Whole decode step: LLaMA.forward for T == 1 with a KV cache (model.py:76-122),
@@ -583,8 +597,8 @@ typedef struct b2l_decode_args {
   const void* rope;          /* f32 [block_size, hs/2, 2]                             */
   const void* idx;           /* int32/int64 [B] tokens of this step                   */
   int idx_is_i64;
-  const int64_t* input_pos;  /* int64 [1]                                             */
-  int32_t* ring_start;       /* int32 [1]; advanced by the step when the cache is full */
+  const int64_t* input_pos;  /* int64 [1]; [B] under B2L_F_ROW_POS                    */
+  int32_t* ring_start;       /* int32 [1] ([B] under B2L_F_ROW_POS); advanced by the step when the cache is full */
   int block_size;            /* rows of the rope table                                */
   void* x;                   /* bf16 [B, C]   residual stream scratch                 */
   void* qkv;                 /* bf16 [B, 3C]                                          */

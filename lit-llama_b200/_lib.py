@@ -18,6 +18,7 @@ F_Q8 = 64   # b2l_decode_step: every linear is llm.int8 (b2l_q8_linear)
 F_W8_BATCH = 128   # b2l_decode_step with F_W8 at B in 2..16: every linear runs b2l_w8_gemv_batch
 F_Q4_BATCH_I8 = 256   # b2l_decode_step (gptq.int4) at B in 2..16: every linear runs b2l_q4_gemv_batch_i8
 F_Q8_BATCH = 512   # b2l_decode_step with F_Q8 at B in 2..16: every linear runs b2l_q8_linear_batch
+F_ROW_POS = 1024   # b2l_attention (T == 1) and b2l_decode_step: input_pos int64[B] and ring_start int32[B], one per row
 
 c_void_p, c_int, c_float, c_size_t = C.c_void_p, C.c_int, C.c_float, C.c_size_t
 
@@ -189,8 +190,10 @@ _SIGS = {
     "b2l_tp_buffer_bytes": (c_size_t, [c_int, c_int]),
     "b2l_tp_allreduce": (c_int, [C.POINTER(TPComm), c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "b2l_ring_advance": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p]),
+    "b2l_ring_advance_rows": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p]),
     "b2l_attention_nocache": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "b2l_kv_unroll": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "b2l_kv_unroll_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "b2l_decode_step": (c_int, [C.POINTER(DecodeArgs), c_void_p]),
     "b2l_decode_step_launches": (c_int, [C.POINTER(DecodeArgs)]),
     "b2l_decode_plan_bytes": (c_size_t, [C.POINTER(DecodeArgs)]),

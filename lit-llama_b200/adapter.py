@@ -142,6 +142,15 @@ class LLaMA(llama.LLaMA):
     def expand_cache(self, B: int) -> None:
         """model.LLaMA.expand_cache; the prefix store does not depend on B, so only its (B, nh, aT, hs) views follow."""
         super().expand_cache(B)
+        self._prefix_views(B)
+
+    def prefill_rows(self, prompts, max_seq_length: int) -> torch.Tensor:
+        """model.LLaMA.prefill_rows; the prefix views follow B as in expand_cache."""
+        out = super().prefill_rows(prompts, max_seq_length)
+        self._prefix_views(len(prompts))
+        return out
+
+    def _prefix_views(self, B: int) -> None:
         self.adapter_kv_caches = [None if c is None else (c[0][:1].expand(B, -1, -1, -1), c[1][:1].expand(B, -1, -1, -1))
                                   for c in self.adapter_kv_caches]
 

@@ -254,6 +254,10 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
   B2L_CHECK_ARG(d->wte && d->ln_f && d->rope && d->idx && d->input_pos && d->ring_start && d->x && d->qkv && d->att &&
                     d->hid && d->attn_work && d->logits,
                 "b2l_decode_step: null pointer");
+  const bool row_pos = (d->flags & B2L_F_ROW_POS) != 0;   // input_pos / ring_start hold one entry per row
+  B2L_CHECK_SUPPORTED(!row_pos || d->plan == nullptr,
+                      "b2l_decode_step: B2L_F_ROW_POS does not run in the persistent kernel (plan must be NULL)");
+  B2L_CHECK_SUPPORTED(!row_pos || !(d->flags & B2L_F_ROPE_ROWS), "b2l_decode_step: B2L_F_ROW_POS does not combine with B2L_F_ROPE_ROWS");
   if (d->flags & B2L_F_Q4_BATCH_I8) {
     B2L_CHECK_SUPPORTED(!(d->flags & (B2L_F_W8 | B2L_F_Q8 | B2L_F_W8_BATCH)),
                         "b2l_decode_step: B2L_F_Q4_BATCH_I8 (gptq.int4) does not combine with B2L_F_W8, B2L_F_Q8 or B2L_F_W8_BATCH");
@@ -314,8 +318,8 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
   }
   if (d->plan != nullptr) return decode_step_persistent(d, stream);   // one persistent kernel per token (decode_mega.cu)
   const int C = d->n_embd, hs = C / d->n_head, B = d->B;
-  const int fl = d->flags;               // the linears' flags (q4_call routes B2L_F_W8 to b2l_w8_gemv)
-  const int afl = fl & ~(B2L_F_W8 | B2L_F_Q8 | B2L_F_W8_BATCH | B2L_F_Q4_BATCH_I8 | B2L_F_Q8_BATCH);   // everything else
+  const int fl = d->flags & ~B2L_F_ROW_POS;   // the linears' flags (q4_call routes B2L_F_W8 to b2l_w8_gemv)
+  const int afl = d->flags & ~(B2L_F_W8 | B2L_F_Q8 | B2L_F_W8_BATCH | B2L_F_Q4_BATCH_I8 | B2L_F_Q8_BATCH);   // the attention's
   int rc;
   // debug timeline: launch i of the step writes uint64[64] at timeline + 512*i (order: per Block c_attn,
   // attention, c_proj, fc12, mlp_proj; then lm_head)
@@ -330,7 +334,9 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
   const bool kv_ok = B == 1 && hs == 128 && d->lm_head.qw_mma != nullptr;
   int oi = 0;
   auto pf = [&]() -> const PfWindow* { const PfWindow* r = pfw.empty() ? nullptr : &pfw[oi]; ++oi; return r; };
-  if ((rc = b2l_ring_advance(d->input_pos, 1, d->ring_start, d->S, stream))) return rc;
+  if ((rc = row_pos ? b2l_ring_advance_rows(d->input_pos, B, d->ring_start, d->S, stream)
+                    : b2l_ring_advance(d->input_pos, 1, d->ring_start, d->S, stream)))
+    return rc;
   if ((rc = b2l_embedding(d->idx, d->idx_is_i64, d->wte, d->x, B, C, d->vocab, stream))) return rc;
   for (int l = 0; l < d->n_layer; ++l) {
     const b2l_layer& L = d->layers[l];

@@ -17,16 +17,24 @@ __global__ void ring_advance_kernel(const int64_t* __restrict__ input_pos, int T
   }
 }
 
+// B2L_F_ROW_POS: row b's ring offset ring_start[b] follows its own position input_pos[b]
+__global__ void ring_advance_rows_kernel(const int64_t* __restrict__ input_pos, int B, int32_t* ring_start, int S) {
+  for (int b = threadIdx.x; b < B; b += blockDim.x) {
+    if (input_pos[b] >= (int64_t)S) ring_start[b] = (ring_start[b] + 1) % S;
+  }
+}
+
 // grid (B*T, n_head), block hs/2 threads (one per rotated pair).
 // q is rotated in place inside qkv; k (rotated) and v go to the cache (or, without a
-// cache, k is rotated in place as well).
+// cache, k is rotated in place as well).  pos_stride 1 (B2L_F_ROW_POS, T == 1): row b reads input_pos[b] and
+// ring_start[b]; 0: every row reads the shared entries.
 __global__ void rope_append_kernel(__nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ k_cache,
                                    __nv_bfloat16* __restrict__ v_cache, const float* __restrict__ rope,
                                    const int64_t* __restrict__ input_pos, const int32_t* __restrict__ ring_start,
-                                   int T, int n_head, int hs, int S, int block_size, int rope_rows) {
+                                   int T, int n_head, int hs, int S, int block_size, int rope_rows, int pos_stride) {
   const int bt = blockIdx.x, h = blockIdx.y, b = bt / T, t = bt % T;
   const int C = n_head * hs;
-  long long p = input_pos ? input_pos[t] : (long long)t;
+  long long p = input_pos ? input_pos[b * pos_stride + t] : (long long)t;
   // rope_rows: `rope` already holds the T selected rows (reference call convention, model.py:93)
   const long long prow = rope_rows ? (long long)t : (p < block_size ? p : (long long)block_size - 1);
   __nv_bfloat16* q = qkv + (size_t)bt * 3 * C + h * hs;
@@ -35,7 +43,7 @@ __global__ void rope_append_kernel(__nv_bfloat16* __restrict__ qkv, __nv_bfloat1
   __nv_bfloat16 *kd = k, *vd = nullptr;
   if (k_cache != nullptr) {
     const int w = (int)(p < S ? p : (long long)S - 1);
-    const int phys = (w + *ring_start) % S;
+    const int phys = (w + ring_start[b * pos_stride]) % S;
     const size_t off = (((size_t)b * n_head + h) * S + phys) * hs;
     kd = k_cache + off;
     vd = v_cache + off;
@@ -74,14 +82,14 @@ template <int EPL>  // elements per lane: head_size == 32*EPL when VEC, else gen
 __global__ void __launch_bounds__(ATT_WARPS * 32)
     attn_partial_kernel(const __nv_bfloat16* __restrict__ qkv, KvView kv, const int64_t* __restrict__ input_pos,
                         const int32_t* __restrict__ ring_start, float* __restrict__ work, int T, int n_head,
-                        int hs, int n_split, int chunk) {
+                        int hs, int n_split, int chunk, int pos_stride) {
   const int bh = blockIdx.x, b = bh / n_head, h = bh % n_head, t = blockIdx.y, sp = blockIdx.z;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int C = n_head * hs;
-  long long p = input_pos ? input_pos[t] : (long long)t;
+  long long p = input_pos ? input_pos[b * pos_stride + t] : (long long)t;   // pos_stride as in rope_append_kernel
   const int cap = kv.S > 0 ? kv.S : T;
   const int L = (int)(p < cap ? p : (long long)cap - 1) + 1;  // valid logical slots 0..L-1
-  const int ring = (kv.S > 0 && ring_start) ? *ring_start : 0;
+  const int ring = (kv.S > 0 && ring_start) ? ring_start[b * pos_stride] : 0;
   const int j0 = sp * chunk, j1 = min(L, j0 + chunk);
   float* out = work + (((size_t)bh * T + t) * n_split + sp) * (hs + 2);
   if (j0 >= j1) {  // empty split: neutral partial
@@ -190,9 +198,9 @@ __global__ void attn_combine_kernel(const float* __restrict__ work, __nv_bfloat1
 }
 
 __global__ void kv_unroll_kernel(const __nv_bfloat16* __restrict__ cache, const int32_t* __restrict__ ring_start,
-                                 __nv_bfloat16* __restrict__ out, int S, int hs) {
-  // grid (B*n_head, S): logical slot blockIdx.y <- physical (slot + ring) % S
-  const int ring = *ring_start;
+                                 __nv_bfloat16* __restrict__ out, int S, int hs, int n_head, int ring_stride) {
+  // grid (B*n_head, S): logical slot blockIdx.y <- physical (slot + ring) % S; ring_stride 1: row b's own ring_start[b]
+  const int ring = ring_start[(blockIdx.x / n_head) * ring_stride];
   const int phys = (blockIdx.y + ring) % S;
   const __nv_bfloat16* src = cache + ((size_t)blockIdx.x * S + phys) * hs;
   __nv_bfloat16* dst = out + ((size_t)blockIdx.x * S + blockIdx.y) * hs;
@@ -286,7 +294,9 @@ __device__ __forceinline__ __nv_bfloat16 adapter_combine(float y, float ay, floa
 // that writes the head's output (the only one, or the last to arrive) adds the gated term before its store; the
 // others drop it, so the term's two dependent L2 round trips overlap the KV stream instead of sitting in the tail of
 // the writing CTA (DESIGN.md, LLaMA-Adapter, has the measurements of both placements).
-template <bool ADAPTER>
+// ROWS (B2L_F_ROW_POS): row b reads its own input_pos[b] and ring_start[b]; a template parameter, so the shared-position
+// launch (batch 1 included) runs exactly the instructions it ran before per-row positions existed.
+template <bool ADAPTER, bool ROWS>
 __global__ void __launch_bounds__(FD_WARPS * 32, ADAPTER ? FD_CTAS_PER_SM : 0)
     attn_decode_fused_kernel(const __nv_bfloat16* qkv, __nv_bfloat16* __restrict__ k_cache,
                              __nv_bfloat16* __restrict__ v_cache, const float* __restrict__ rope,
@@ -316,8 +326,10 @@ __global__ void __launch_bounds__(FD_WARPS * 32, ADAPTER ? FD_CTAS_PER_SM : 0)
   const size_t head_base = ((size_t)b * n_head + h) * S * HS;
 
   // input_pos and ring_start are inputs of the step (written by the host side long before), not
-  // products of the previous kernel: they may be read before the dependency is resolved.
-  const long long p = input_pos[0];
+  // products of the previous kernel: they may be read before the dependency is resolved.  ROWS: row b is at its own
+  // position input_pos[b] with its own ring offset ring_start[b], and everything below (write slot, key count, split
+  // plan, ring wrap, merge) follows from that row's L.
+  const long long p = input_pos[ROWS ? b : 0];
   const int w_slot = (int)(p < S ? p : (long long)S - 1);  // logical slot of the new token
   const int L = w_slot + 1;                                 // valid logical slots 0..L-1
   // keys per CTA: a multiple of 64 in [64, 256], chosen (identically by every CTA) so that at most target_ctas CTAs
@@ -331,7 +343,7 @@ __global__ void __launch_bounds__(FD_WARPS * 32, ADAPTER ? FD_CTAS_PER_SM : 0)
                                   : min(FD_CHUNK, max(FD_SUB, FD_SUB * ((L + FD_SUB * want_splits - 1) / (FD_SUB * want_splits))));
   const int n_active = (L + chunk - 1) / chunk;
   if (sp >= n_active) return;
-  const int ring = *ring_start;
+  const int ring = ring_start[ROWS ? b : 0];
   const int j0 = sp * chunk, j1 = min(L, j0 + chunk);
   const int n_old = min(j1, L - 1) - j0;  // rows written by earlier steps (slot L-1 is written by this one)
   const int n_sub = (n_old + FD_SUB - 1) / FD_SUB;
@@ -885,7 +897,8 @@ static inline void split_plan(int T, int S, int* n_split, int* chunk) {
 }
 
 static int launch_attn(const __nv_bfloat16* qkv, KvView kv, const int64_t* input_pos, const int32_t* ring_start,
-                       float* work, __nv_bfloat16* y, int B, int T, int n_head, int hs, int cap, cudaStream_t st) {
+                       float* work, __nv_bfloat16* y, int B, int T, int n_head, int hs, int cap, int pos_stride,
+                       cudaStream_t st) {
   static const int env_pf = [] { const char* e = getenv("B2L_ATTN_PREFILL"); return e ? atoi(e) : 1; }();
   if (hs == 128 && T > 1 && env_pf) {   // tiled tensor-core kernel (B2L_ATTN_PREFILL=0: the per-query path below)
     static DynSmemCache smem_cache;
@@ -898,9 +911,11 @@ static int launch_attn(const __nv_bfloat16* qkv, KvView kv, const int64_t* input
   split_plan(T, cap, &n_split, &chunk);
   dim3 grid(B * n_head, T, n_split), block(ATT_WARPS * 32);
   if (hs == 128)
-    attn_partial_kernel<4><<<grid, block, 0, st>>>(qkv, kv, input_pos, ring_start, work, T, n_head, hs, n_split, chunk);
+    attn_partial_kernel<4><<<grid, block, 0, st>>>(qkv, kv, input_pos, ring_start, work, T, n_head, hs, n_split, chunk,
+                                                   pos_stride);
   else
-    attn_partial_kernel<0><<<grid, block, 0, st>>>(qkv, kv, input_pos, ring_start, work, T, n_head, hs, n_split, chunk);
+    attn_partial_kernel<0><<<grid, block, 0, st>>>(qkv, kv, input_pos, ring_start, work, T, n_head, hs, n_split, chunk,
+                                                   pos_stride);
   B2L_LAUNCH_CHECK("attn_partial_kernel");
   attn_combine_kernel<<<dim3(B * n_head, T), 128, 0, st>>>(work, y, T, n_head, hs, n_split);
   B2L_LAUNCH_CHECK("attn_combine_kernel");
@@ -943,6 +958,14 @@ extern "C" int b2l_ring_advance(const int64_t* input_pos, int T, int32_t* ring_s
   return 0;
 }
 
+extern "C" int b2l_ring_advance_rows(const int64_t* input_pos, int B, int32_t* ring_start, int S, b2l_stream_t stream) {
+  B2L_CHECK_ARG(input_pos && ring_start, "b2l_ring_advance_rows: null pointer");
+  B2L_CHECK_ARG(B > 0 && S > 0, "b2l_ring_advance_rows: bad shape (B=%d, S=%d)", B, S);
+  ring_advance_rows_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(input_pos, B, ring_start, S);
+  B2L_LAUNCH_CHECK("ring_advance_rows_kernel");
+  return 0;
+}
+
 static int launch_adapter_prefix(const void* qkv, const b2l_adapter_prefix* pre, void* y, int B, int T, int n_head,
                                  int head_size, cudaStream_t st) {
   attn_adapter_prefix_kernel<<<dim3(B * T, n_head), ATT_WARPS * 32, 0, st>>>(
@@ -952,10 +975,20 @@ static int launch_adapter_prefix(const void* qkv, const b2l_adapter_prefix* pre,
   return 0;
 }
 
+// B2L_F_ROW_POS (input_pos int64[B], ring_start int32[B]) is one query per row: T == 1, and the RoPE table (not
+// B2L_F_ROPE_ROWS, whose T selected rows cannot serve B positions)
+static int check_row_pos(int flags, int T, const char* who) {
+  if (!(flags & B2L_F_ROW_POS)) return 0;
+  B2L_CHECK_SUPPORTED(T == 1, "%s: B2L_F_ROW_POS runs one token per row (T == 1), got T=%d", who, T);
+  B2L_CHECK_SUPPORTED(!(flags & B2L_F_ROPE_ROWS), "%s: B2L_F_ROW_POS does not combine with B2L_F_ROPE_ROWS", who);
+  return 0;
+}
+
 // b2l_attention and b2l_attention_adapter (pre != nullptr: already checked)
 static int attention_impl(void* qkv, void* k_cache, void* v_cache, const void* rope, const int64_t* input_pos,
                           const int32_t* ring_start, void* y, void* work, int B, int T, int n_head, int head_size,
                           int S, int block_size, int flags, const b2l_adapter_prefix* pre, cudaStream_t st) {
+  const int pos_stride = (flags & B2L_F_ROW_POS) ? 1 : 0;
   if (T == 1 && head_size == 128 && !(flags & B2L_F_ROPE_ROWS) && !(flags & B2L_F_ATTN_UNFUSED)) {
     const int n_split = (S + FD_SUB - 1) / FD_SUB;
     int* tickets = reinterpret_cast<int*>(reinterpret_cast<char*>(work) + ws_partials_bytes(B, n_head, head_size, T, S));
@@ -965,34 +998,31 @@ static int attention_impl(void* qkv, void* k_cache, void* v_cache, const void* r
     // (default 0: the extra block barrier of 1 is not free)
     static const int env_smem_merge = [] { const char* e = getenv("B2L_ATTN_SMEM_MERGE"); return e ? atoi(e) : 0; }();
     LaunchCfg lc(dim3(B * n_head, n_split), dim3(FD_WARPS * 32), FD_SMEM_BYTES, st, (flags & B2L_F_PDL) != 0);
-    if (pre == nullptr) {
-      static DynSmemCache smem_cache;
-      if (int rc = ensure_dyn_smem(attn_decode_fused_kernel<false>, FD_SMEM_BYTES, smem_cache)) return rc;
-      B2L_CUDA(cudaLaunchKernelEx(&lc.cfg, attn_decode_fused_kernel<false>, (const __nv_bfloat16*)qkv, (__nv_bfloat16*)k_cache,
+    static DynSmemCache smem_cache[2][2];   // [ADAPTER][ROWS]: the four instantiations share one function type
+    auto launch = [&](auto kernel, const b2l_adapter_prefix* pf) -> int {
+      if (int rc = ensure_dyn_smem(kernel, FD_SMEM_BYTES, smem_cache[pf != nullptr][pos_stride])) return rc;
+      B2L_CUDA(cudaLaunchKernelEx(&lc.cfg, kernel, (const __nv_bfloat16*)qkv, (__nv_bfloat16*)k_cache,
                                   (__nv_bfloat16*)v_cache, (const float*)rope, input_pos, ring_start, (__nv_bfloat16*)y,
                                   (float*)work, tickets, n_head, S, block_size, n_split, (unsigned long long*)g_attn_timeline, env_pre, env_smem_merge,
-                                  FD_CTAS_PER_SM * sm_count(), (const __nv_bfloat16*)nullptr, (const __nv_bfloat16*)nullptr,
-                                  (const __nv_bfloat16*)nullptr, 0));
-    } else {
-      static DynSmemCache smem_cache;
-      if (int rc = ensure_dyn_smem(attn_decode_fused_kernel<true>, FD_SMEM_BYTES, smem_cache)) return rc;
-      B2L_CUDA(cudaLaunchKernelEx(&lc.cfg, attn_decode_fused_kernel<true>, (const __nv_bfloat16*)qkv, (__nv_bfloat16*)k_cache,
-                                  (__nv_bfloat16*)v_cache, (const float*)rope, input_pos, ring_start, (__nv_bfloat16*)y,
-                                  (float*)work, tickets, n_head, S, block_size, n_split, (unsigned long long*)g_attn_timeline, env_pre, env_smem_merge,
-                                  FD_CTAS_PER_SM * sm_count(), (const __nv_bfloat16*)pre->k, (const __nv_bfloat16*)pre->v,
-                                  (const __nv_bfloat16*)pre->gate, pre->len));
-    }
-    return 0;
+                                  FD_CTAS_PER_SM * sm_count(), (const __nv_bfloat16*)(pf ? pf->k : nullptr),
+                                  (const __nv_bfloat16*)(pf ? pf->v : nullptr), (const __nv_bfloat16*)(pf ? pf->gate : nullptr),
+                                  pf ? pf->len : 0));
+      return 0;
+    };
+    if (pre == nullptr)
+      return pos_stride ? launch(attn_decode_fused_kernel<false, true>, nullptr) : launch(attn_decode_fused_kernel<false, false>, nullptr);
+    return pos_stride ? launch(attn_decode_fused_kernel<true, true>, pre) : launch(attn_decode_fused_kernel<true, false>, pre);
   }
   int rt = head_size / 2 < 32 ? 32 : head_size / 2;
   rope_append_kernel<<<dim3(B * T, n_head), rt, 0, st>>>((__nv_bfloat16*)qkv, (__nv_bfloat16*)k_cache,
                                                         (__nv_bfloat16*)v_cache, (const float*)rope, input_pos,
-                                                        ring_start, T, n_head, head_size, S, block_size, (flags & B2L_F_ROPE_ROWS) ? 1 : 0);
+                                                        ring_start, T, n_head, head_size, S, block_size, (flags & B2L_F_ROPE_ROWS) ? 1 : 0,
+                                                        pos_stride);
   B2L_LAUNCH_CHECK("rope_append_kernel");
   KvView kv{(const __nv_bfloat16*)k_cache, (const __nv_bfloat16*)v_cache, (size_t)n_head * S * head_size,
             (size_t)S * head_size, (size_t)head_size, S};
   if (int rc = launch_attn((const __nv_bfloat16*)qkv, kv, input_pos, ring_start, (float*)work, (__nv_bfloat16*)y, B, T,
-                           n_head, head_size, S, st))
+                           n_head, head_size, S, pos_stride, st))
     return rc;
   return pre == nullptr ? 0 : launch_adapter_prefix(qkv, pre, y, B, T, n_head, head_size, st);
 }
@@ -1005,6 +1035,7 @@ extern "C" int b2l_attention(void* qkv, void* k_cache, void* v_cache, const void
   B2L_CHECK_ARG(B > 0 && T > 0 && n_head > 0 && S > 0 && T <= S && block_size > 0, "b2l_attention: bad shape");
   B2L_CHECK_SUPPORTED(head_size % 2 == 0 && head_size >= 2 && head_size <= 32 * ATT_MAX_EPL,
                       "b2l_attention: head_size %d unsupported (even, <= %d)", head_size, 32 * ATT_MAX_EPL);
+  if (int rc = check_row_pos(flags, T, "b2l_attention")) return rc;
   return attention_impl(qkv, k_cache, v_cache, rope, input_pos, ring_start, y, work, B, T, n_head, head_size, S,
                         block_size, flags, nullptr, (cudaStream_t)stream);
 }
@@ -1018,6 +1049,7 @@ extern "C" int b2l_attention_adapter(void* qkv, void* k_cache, void* v_cache, co
   B2L_CHECK_ARG(B > 0 && T > 0 && n_head > 0 && S > 0 && T <= S && block_size > 0, "b2l_attention_adapter: bad shape");
   B2L_CHECK_SUPPORTED(head_size % 2 == 0 && head_size >= 2 && head_size <= 32 * ATT_MAX_EPL,
                       "b2l_attention_adapter: head_size %d unsupported (even, <= %d)", head_size, 32 * ATT_MAX_EPL);
+  if (int rc = check_row_pos(flags, T, "b2l_attention_adapter")) return rc;
   if (int rc = check_adapter_prefix(prefix, "b2l_attention_adapter")) return rc;
   return attention_impl(qkv, k_cache, v_cache, rope, input_pos, ring_start, y, work, B, T, n_head, head_size, S,
                         block_size, flags, prefix, (cudaStream_t)stream);
@@ -1027,12 +1059,12 @@ static int attention_nocache_impl(void* qkv, const void* rope, void* y, void* wo
                                   int head_size, int block_size, cudaStream_t st) {
   int rt = head_size / 2 < 32 ? 32 : head_size / 2;
   rope_append_kernel<<<dim3(B * T, n_head), rt, 0, st>>>((__nv_bfloat16*)qkv, nullptr, nullptr, (const float*)rope,
-                                                        nullptr, nullptr, T, n_head, head_size, 0, block_size, 0);
+                                                        nullptr, nullptr, T, n_head, head_size, 0, block_size, 0, 0);
   B2L_LAUNCH_CHECK("rope_append_kernel");
   const int C = n_head * head_size;
   const __nv_bfloat16* base = (const __nv_bfloat16*)qkv;
   KvView kv{base + C, base + 2 * C, (size_t)T * 3 * C, (size_t)head_size, (size_t)3 * C, 0};
-  return launch_attn(base, kv, nullptr, nullptr, (float*)work, (__nv_bfloat16*)y, B, T, n_head, head_size, T, st);
+  return launch_attn(base, kv, nullptr, nullptr, (float*)work, (__nv_bfloat16*)y, B, T, n_head, head_size, T, 0, st);
 }
 
 extern "C" int b2l_attention_nocache(void* qkv, const void* rope, void* y, void* work, int B, int T, int n_head,
@@ -1062,7 +1094,17 @@ extern "C" int b2l_kv_unroll(const void* cache, const int32_t* ring_start, void*
   B2L_CHECK_ARG(cache && ring_start && out && B > 0 && n_head > 0 && S > 0 && head_size > 0,
                 "b2l_kv_unroll: bad argument");
   kv_unroll_kernel<<<dim3(B * n_head, S), 64, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)cache, ring_start,
-                                                                         (__nv_bfloat16*)out, S, head_size);
+                                                                         (__nv_bfloat16*)out, S, head_size, n_head, 0);
+  B2L_LAUNCH_CHECK("kv_unroll_kernel");
+  return 0;
+}
+
+extern "C" int b2l_kv_unroll_rows(const void* cache, const int32_t* ring_start, void* out, int B, int n_head, int S,
+                                  int head_size, b2l_stream_t stream) {
+  B2L_CHECK_ARG(cache && ring_start && out, "b2l_kv_unroll_rows: null pointer");
+  B2L_CHECK_ARG(B > 0 && n_head > 0 && S > 0 && head_size > 0, "b2l_kv_unroll_rows: bad shape");
+  kv_unroll_kernel<<<dim3(B * n_head, S), 64, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)cache, ring_start,
+                                                                         (__nv_bfloat16*)out, S, head_size, n_head, 1);
   B2L_LAUNCH_CHECK("kv_unroll_kernel");
   return 0;
 }

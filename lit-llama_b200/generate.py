@@ -4,7 +4,10 @@
 RNG stream of `torch.multinomial` is the reference's); the model call inside it is one
 CUDA-graph replay per token.  `generate_batch()` draws up to 16 samples of one prompt
 at once: one batch-1 prefill, then one batched decode step and one sampling launch per
-token for all samples.  `main()` mirrors the reference CLI with argparse
+token for all samples.  `generate_prompts()` continues up to 16 different prompts at
+once: one batch-1 prefill per prompt into its row of the cache, then one batched decode
+step at per-row positions and one sampling launch per token.  `main()` mirrors the
+reference CLI with argparse
 (jsonargparse and lightning are not dependencies of this path)."""
 import os
 import sys
@@ -209,6 +212,74 @@ def generate_batch(
     return [out[b, :n] for b, n in enumerate(end.tolist())]
 
 
+@torch.no_grad()
+def generate_prompts(
+    model: LLaMA,
+    prompts: List[torch.Tensor],
+    max_new_tokens: int,
+    *,
+    max_seq_length: Optional[int] = None,
+    temperature: float = 1.0,
+    top_k: Optional[int] = None,
+    eos_id: Optional[int] = None,
+) -> List[torch.Tensor]:
+    """Continuations of 1..16 different prompts (1-D tensors of any lengths), decoded together: a list of 1-D tensors,
+    row b the prompt `prompts[b]` plus its new tokens (generate.py:20-91 per row).
+
+    `LLaMA.prefill_rows` runs each prompt through the batch-1 prefill into its own row of one cache; the first tokens
+    are drawn from those last positions.  Each later token is one batched model call with a (B, 1) `input_pos`, row b
+    at position len(prompts[b]) + i with its own KV ring (each row takes the roll branch, model.py:214-218, on its own
+    once it passes max_seq_length), and one sampling launch for all rows.  max_seq_length defaults to
+    min(longest prompt + max_new_tokens, block_size).  Row b's token is `torch.multinomial(probs, 1)[b]` of the step's
+    [B, V] probabilities, so one prompt gives `generate()`'s tokens for the same seed.
+
+    With `eos_id`, a row that draws it ends there, the eos token included; finished rows keep riding along (their later
+    tokens are dropped) and the loop stops once every row has finished, reading one flag per step.  The cache is left
+    at B rows: call `model.reset_cache()` before a batch-1 `generate()`."""
+    B = len(prompts)
+    if not 1 <= B <= MAX_SAMPLES:
+        raise ValueError(f"generate_prompts: {B} prompts; 1..{MAX_SAMPLES} (the batched decode step's range)")
+    for p in prompts:
+        if p.dim() != 1:
+            raise ValueError(f"generate_prompts: every prompt must be one sequence of shape (T,), got {tuple(p.shape)}")
+    for p in prompts:
+        if not p.is_cuda:
+            raise RuntimeError(f"generate_prompts: a prompt is on {p.device}; lit_llama_b200 runs on CUDA only (no CPU fallback)")
+    Ts = [p.size(0) for p in prompts]
+    if max_seq_length is None:
+        max_seq_length = min(max(Ts) + max_new_tokens, model.config.block_size)
+    if max(Ts) > max_seq_length:
+        raise ValueError(f"generate_prompts: a prompt of {max(Ts)} tokens is longer than max_seq_length={max_seq_length}")
+
+    device, dtype = prompts[0].device, prompts[0].dtype
+    new = torch.empty((B, max_new_tokens), dtype=dtype, device=device)
+    input_pos = torch.tensor(Ts, dtype=torch.int64, device=device).view(B, 1)   # row b's first new token
+    end = torch.full((B,), max_new_tokens, dtype=torch.int64, device=device) if eos_id is not None else None
+    done = torch.zeros(B, dtype=torch.bool, device=device) if eos_id is not None else None
+
+    for i in range(max_new_tokens):
+        if i == 0:
+            rows = model.prefill_rows(prompts, max_seq_length)
+        else:
+            rows = model(x, max_seq_length, input_pos)[:, -1]
+            input_pos = input_pos + 1
+        if torch.multinomial is _TORCH_MULTINOMIAL:
+            idx_next = sample_token(rows, temperature, top_k).to(dtype=dtype)   # one RNG draw + one launch for all rows
+        else:
+            # torch.multinomial has been replaced (as in generate()): keep calling it, on the fused [B, V] probabilities
+            idx_next = torch.multinomial(sample_probs(rows, temperature, top_k), num_samples=1).view(B).to(dtype=dtype)
+        new[:, i] = idx_next
+        x = idx_next.view(B, 1)
+        if eos_id is not None:
+            hit = (idx_next == eos_id) & ~done
+            end = torch.where(hit, i + 1, end)   # include the eos token
+            done |= hit
+            if bool(done.all()):
+                break
+    ns = [max_new_tokens] * B if end is None else end.tolist()
+    return [torch.cat((p.to(dtype), new[b, :n])) for b, (p, n) in enumerate(zip(prompts, ns))]
+
+
 def main(
     prompt: str = "Hello, my name is",
     *,
@@ -220,9 +291,12 @@ def main(
     tokenizer_path: Path = Path("checkpoints/lit-llama/tokenizer.model"),
     quantize: Optional[str] = None,
     batch_size: int = 1,
+    prompts_file: Optional[Path] = None,
 ) -> None:
     """generate.py:94-155 without Fabric: bf16 on cuda:0, same prints on stderr.  `batch_size` > 1 draws the samples
-    in groups of up to `batch_size` (at most 16) through `generate_batch`, on the model's exact batched decode step."""
+    in groups of up to `batch_size` (at most 16) through `generate_batch`, on the model's exact batched decode step.
+    `prompts_file` (one prompt per line) replaces `prompt`: the prompts are decoded in groups of `batch_size` through
+    `generate_prompts`, `num_samples` times each."""
     if not 1 <= batch_size <= MAX_SAMPLES:
         raise ValueError(f"batch_size = {batch_size}; 1..{MAX_SAMPLES}")
     from sentencepiece import SentencePieceProcessor
@@ -257,7 +331,34 @@ def main(
     prompt_length = encoded.size(0)
 
     torch.manual_seed(1234)
-    if batch_size == 1:
+    if batch_size > 1 or prompts_file is not None:
+        # the exact 2..16-row decode step of each quantized base (each row bit-identical to the batch-1 step on it);
+        # without it a compacted gptq.int4 model re-tiles every linear at B >= 2 and gptq.int8 runs module by module
+        if quantize == "gptq.int4":
+            model.q4_batch_step = True
+        elif quantize == "gptq.int8":
+            model.w8_batch_step = True
+        elif quantize == "llm.int8":
+            model.int8_step = True
+    if prompts_file is not None:
+        lines = [ln for ln in Path(prompts_file).read_text().splitlines() if ln.strip()]
+        prompts = [torch.tensor([sp.bos_id()] + sp.encode(ln), dtype=torch.int, device=device) for ln in lines]
+        k = 0
+        for _ in range(num_samples):
+            for first in range(0, len(prompts), batch_size):
+                group = prompts[first:first + batch_size]
+                k += 1
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                ys = generate_prompts(model, group, max_new_tokens, temperature=temperature, top_k=top_k)
+                torch.cuda.synchronize()
+                t = time.perf_counter() - t0
+                model.reset_cache()
+                for y in ys:
+                    print(sp.decode(y.tolist()))
+                tokens_generated = sum(y.size(0) - p.size(0) for y, p in zip(ys, group))
+                print(f"Time for inference {k}: {t:.02f} sec total, {tokens_generated / t:.02f} tokens/sec", file=sys.stderr)
+    elif batch_size == 1:
         for i in range(num_samples):
             torch.cuda.synchronize()
             t0 = time.perf_counter()
@@ -269,14 +370,6 @@ def main(
             tokens_generated = y.size(0) - prompt_length
             print(f"Time for inference {i + 1}: {t:.02f} sec total, {tokens_generated / t:.02f} tokens/sec", file=sys.stderr)
     else:
-        # the exact 2..16-row decode step of each quantized base (each row bit-identical to the batch-1 step on it);
-        # without it a compacted gptq.int4 model re-tiles every linear at B >= 2 and gptq.int8 runs module by module
-        if quantize == "gptq.int4":
-            model.q4_batch_step = True
-        elif quantize == "gptq.int8":
-            model.w8_batch_step = True
-        elif quantize == "llm.int8":
-            model.int8_step = True
         for i, first in enumerate(range(0, num_samples, batch_size)):
             n = min(batch_size, num_samples - first)
             torch.cuda.synchronize()
@@ -305,7 +398,10 @@ def cli() -> None:
     ap.add_argument("--tokenizer_path", type=Path, default=Path("checkpoints/lit-llama/tokenizer.model"))
     ap.add_argument("--quantize", default=None, choices=[None, "llm.int8", "gptq.int4", "gptq.int8"])
     ap.add_argument("--batch_size", type=int, default=1,
-                    help=f"samples drawn together per generate_batch call (1..{MAX_SAMPLES}; 1: one generate() per sample)")
+                    help=f"samples drawn together per generate_batch call (1..{MAX_SAMPLES}; 1: one generate() per sample); "
+                         "with --prompts_file, prompts decoded together per generate_prompts call")
+    ap.add_argument("--prompts_file", type=Path, default=None,
+                    help="a text file of prompts, one per line, decoded in groups of --batch_size (replaces --prompt)")
     a = ap.parse_args()
     main(**vars(a))
 

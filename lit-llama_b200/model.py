@@ -157,7 +157,8 @@ class CausalSelfAttention(nn.Module):
         _rope_is_table: bool = False,
     ) -> Tuple[torch.Tensor, Optional[KVCache]]:
         """`mask` is accepted for signature parity and ignored: the kernel derives the
-        causal mask from input_pos exactly as model.py:94-96 builds it from tril."""
+        causal mask from input_pos exactly as model.py:94-96 builds it from tril.  A 2-D input_pos of shape (B, 1)
+        puts each row's one token at its own position, with its own ring offset (B2L_F_ROW_POS)."""
         L.require_cuda_bf16(x, "CausalSelfAttention.forward")
         B, T, C_ = x.size()
         hs = C_ // self.n_head
@@ -185,12 +186,25 @@ class CausalSelfAttention(nn.Module):
             S = cache_k.shape[2]
             assert S == max_seq_length and cache_k.is_contiguous() and cache_v.is_contiguous()
             pos = input_pos.reshape(-1).to(torch.int64)
+            rows = input_pos.dim() == 2   # one position (and ring offset) per row
+            if rows and (T != 1 or pos.numel() != B):
+                raise ValueError(f"CausalSelfAttention: a 2-D input_pos is one position per row, shape ({B}, 1); got "
+                                 f"{tuple(input_pos.shape)} for T={T}")
+            n_ring = B if rows else 1
             if self._ring is None or self._ring.device != x.device:
-                self._ring = torch.zeros(1, dtype=torch.int32, device=x.device)
+                self._ring = torch.zeros(n_ring, dtype=torch.int32, device=x.device)
             if not self._ring_shared:  # stand-alone use: this module owns the roll state (model.py:214-218)
-                L.check(lib.b2l_ring_advance(pos.data_ptr(), T, self._ring.data_ptr(), S, L.stream_ptr()), "b2l_ring_advance")
+                if self._ring.numel() != n_ring:   # every row starts from the shared offset
+                    self._ring = self._ring[:1].expand(n_ring).contiguous()
+                if rows:
+                    L.check(lib.b2l_ring_advance_rows(pos.data_ptr(), B, self._ring.data_ptr(), S, L.stream_ptr()),
+                            "b2l_ring_advance_rows")
+                else:
+                    L.check(lib.b2l_ring_advance(pos.data_ptr(), T, self._ring.data_ptr(), S, L.stream_ptr()), "b2l_ring_advance")
+            if self._ring.numel() != n_ring:
+                raise RuntimeError(f"CausalSelfAttention: the KV ring holds {self._ring.numel()} offsets, this call needs {n_ring}")
             work = torch.zeros(lib.b2l_attn_workspace_bytes(B, self.n_head, hs, T, S) // 4 + 1, device=x.device, dtype=torch.float32)
-            flags = 0 if _rope_is_table else 4  # B2L_F_ROPE_ROWS
+            flags = (0 if _rope_is_table else 4) | (L.F_ROW_POS if rows else 0)  # B2L_F_ROPE_ROWS
             args = (qkv.data_ptr(), cache_k.data_ptr(), cache_v.data_ptr(), rope32.data_ptr(), pos.data_ptr(),
                     self._ring.data_ptr(), y.data_ptr(), work.data_ptr(), B, T, self.n_head, hs, S, rope32.shape[0], flags)
             if prefix is None:
@@ -270,17 +284,19 @@ class Block(nn.Module):
 class _DecodeState:
     """Static buffers + the C argument block of b2l_decode_step for one (B, S)."""
 
-    def __init__(self, model: "LLaMA", B: int, S: int, device: torch.device, idx_dtype: torch.dtype) -> None:
+    def __init__(self, model: "LLaMA", B: int, S: int, device: torch.device, idx_dtype: torch.dtype,
+                 row_pos: bool = False) -> None:
         from .quantization import ColBlockQuantizedLinear
 
         cfg = model.config
         C_, nh = cfg.n_embd, cfg.n_head
         hs = C_ // nh
         bf = dict(device=device, dtype=torch.bfloat16)
-        self.B, self.S = B, S
+        self.B, self.S, self.row_pos = B, S, row_pos
         self.generation = WEIGHTS_GENERATION[0]   # raw weight pointers below are valid for this generation only
         self.idx = torch.zeros(B, dtype=idx_dtype, device=device)
-        self.pos = torch.zeros(1, dtype=torch.int64, device=device)
+        # B2L_F_ROW_POS: one position per row (and model._ring holds one offset per row); else one shared position
+        self.pos = torch.zeros(B if row_pos else 1, dtype=torch.int64, device=device)
         self.x = torch.empty((B, C_), **bf)
         self.qkv = torch.empty((B, 3 * C_), **bf)
         self.att = torch.empty((B, C_), **bf)
@@ -362,7 +378,7 @@ class _DecodeState:
             att=self.att.data_ptr(), hid=self.hid.data_ptr(), attn_work=self.work.data_ptr(),
             logits=self.logits.data_ptr(),
             flags=(model.decode_flags | (L.F_W8 if w8 else 0) | (L.F_W8_BATCH if w8b else 0) | (L.F_Q8 if q8 else 0)
-                   | (L.F_Q4_BATCH_I8 if q4b else 0) | (L.F_Q8_BATCH if q8b else 0)),
+                   | (L.F_Q4_BATCH_I8 if q4b else 0) | (L.F_Q8_BATCH if q8b else 0) | (L.F_ROW_POS if row_pos else 0)),
             batch_work=None if self.batch_ws is None else self.batch_ws.data_ptr())
         if q8:
             self.q8_layers = q8_layers
@@ -538,7 +554,54 @@ class LLaMA(nn.Module):
         self._decode = None
         self._module_graph = None
         if self._ring is not None:
-            self._ring.zero_()
+            if self._ring.numel() != 1:   # back to one shared ring offset
+                self._set_ring(torch.zeros(1, dtype=torch.int32, device=self._ring.device))
+            else:
+                self._ring.zero_()
+
+    def _set_ring(self, ring: torch.Tensor) -> None:
+        """The KV ring offset(s) every layer reads: int32 [1] shared by all rows, or [B] after a per-row step."""
+        self._ring = ring
+        for blk in self.transformer.h:
+            blk.attn._ring, blk.attn._ring_shared = ring, True
+        self._decode, self._module_graph = None, None   # they point at the old ring
+
+    @torch.no_grad()
+    def prefill_rows(self, prompts: List[torch.Tensor], max_seq_length: int) -> torch.Tensor:
+        """Prefill 1..16 different prompts (1-D token tensors of any lengths <= max_seq_length) into one B-row KV cache
+        and return each prompt's last-position logits, (B, vocab).
+
+        Each prompt runs through the batch-1 prefill, writing straight into its row of the B-row store, so row b's
+        cache is bit for bit the one `generate()` builds for that prompt (the work is the sum of the prompt lengths; a
+        padded (B, T_max) prefill would cost more and would round differently).  The ring offsets start per row at
+        zero: the next step passes a (B, 1) `input_pos`, row b's first new token at position len(prompts[b])."""
+        B = len(prompts)
+        if not 1 <= B <= 16:
+            raise ValueError(f"prefill_rows: {B} prompts; 1..16 (the batched decode step's range)")
+        for p in prompts:
+            if p.dim() != 1 or p.numel() == 0:
+                raise ValueError(f"prefill_rows: every prompt must be a non-empty 1-D token tensor, got {tuple(p.shape)}")
+            if not p.is_cuda:
+                raise RuntimeError(f"prefill_rows: prompt is on {p.device}; lit_llama_b200 runs on CUDA only (no CPU fallback)")
+            if p.numel() > max_seq_length:
+                raise ValueError(f"prefill_rows: a prompt of {p.numel()} tokens does not fit max_seq_length={max_seq_length}")
+        cfg = self.config
+        dev = prompts[0].device
+        self.reset_cache()
+        store = torch.zeros((cfg.n_layer, 2, B, cfg.n_head, max_seq_length, cfg.n_embd // cfg.n_head), device=dev,
+                            dtype=torch.bfloat16)
+        last = []
+        for b, p in enumerate(prompts):
+            if self._ring is not None:
+                self._ring.zero_()
+            self._kv_store = store[:, :, b:b + 1]
+            self.kv_caches = [(store[i, 0, b:b + 1], store[i, 1, b:b + 1]) for i in range(cfg.n_layer)]   # contiguous
+            self._decode, self._module_graph = None, None   # a one-token prompt's step state points at the last row
+            last.append(self(p.view(1, -1), max_seq_length, torch.arange(p.numel(), device=dev))[0, -1].clone())
+        self._kv_store = store
+        self.kv_caches = [(store[i, 0], store[i, 1]) for i in range(cfg.n_layer)]
+        self._set_ring(torch.zeros(B, dtype=torch.int32, device=dev))
+        return torch.stack(last)
 
     def expand_cache(self, B: int) -> None:
         """Broadcast a batch-1 KV cache to B rows: every row then holds the prompt's keys and values, so B samples of one
@@ -699,11 +762,13 @@ class LLaMA(nn.Module):
         a ring and this returns the un-rotated copies the reference would hold."""
         out = []
         lib = L.lib()
+        name = "b2l_kv_unroll_rows" if self._ring.numel() > 1 else "b2l_kv_unroll"   # one ring offset per row, or shared
+        unroll = getattr(lib, name)
         for k, v in self.kv_caches:
             B, nh, S, hs = k.shape
             ko, vo = torch.empty_like(k), torch.empty_like(v)
-            L.check(lib.b2l_kv_unroll(k.data_ptr(), self._ring.data_ptr(), ko.data_ptr(), B, nh, S, hs, L.stream_ptr()), "b2l_kv_unroll")
-            L.check(lib.b2l_kv_unroll(v.data_ptr(), self._ring.data_ptr(), vo.data_ptr(), B, nh, S, hs, L.stream_ptr()), "b2l_kv_unroll")
+            L.check(unroll(k.data_ptr(), self._ring.data_ptr(), ko.data_ptr(), B, nh, S, hs, L.stream_ptr()), name)
+            L.check(unroll(v.data_ptr(), self._ring.data_ptr(), vo.data_ptr(), B, nh, S, hs, L.stream_ptr()), name)
             out.append((ko, vo))
         return out
 
@@ -712,7 +777,19 @@ class LLaMA(nn.Module):
         self, idx: torch.Tensor, max_seq_length: Optional[int] = None, input_pos: Optional[torch.Tensor] = None
     ) -> Union[torch.Tensor, Tuple[torch.Tensor, List[KVCache]]]:
         B, T = idx.size()
+        # a (B, 1) input_pos: one token per row, each at its own position with its own ring offset (B2L_F_ROW_POS);
+        # at B == 1 that is the shared form
+        rows = input_pos is not None and input_pos.dim() == 2
+        if rows and (T != 1 or tuple(input_pos.shape) != (B, 1)):
+            raise ValueError(f"LLaMA.forward: a 2-D input_pos is one position per row, shape ({B}, 1) for T == 1; got "
+                             f"{tuple(input_pos.shape)} with T={T}")
         max_seq_length = self._prepare(idx, max_seq_length)
+        if rows:
+            if B == 1:
+                input_pos, rows = input_pos.reshape(1), False
+        elif input_pos is not None and self._ring.numel() > 1:
+            raise RuntimeError("LLaMA.forward: the cache holds one position per row (prefill_rows); pass input_pos of "
+                               "shape (B, 1), or reset_cache() first")
 
         if input_pos is not None and not self.kv_caches:
             cfg = self.config
@@ -721,6 +798,11 @@ class LLaMA(nn.Module):
             self.kv_caches = [(self._kv_store[i, 0], self._kv_store[i, 1]) for i in range(cfg.n_layer)]
             self._decode = None
             self._module_graph = None
+        if rows:
+            if self._kv_store.shape[2] != B:
+                raise ValueError(f"LLaMA.forward: {B} rows against a KV cache of {self._kv_store.shape[2]}")
+            if self._ring.numel() != B:   # after expand_cache: every row starts from the shared ring offset
+                self._set_ring(self._ring.expand(B).contiguous())
 
         # ---- decode: one C call per token, replayed as a CUDA graph
         st = None
@@ -735,7 +817,8 @@ class LLaMA(nn.Module):
                 # one the ONLY copy of both layers (still released: nothing was loaded into them)
                 self._fc12_cache = {k: v for k, v in self._fc12_cache.items()
                                     if k[1] == "i8" and self._fc12_is_only_copy(k[0])}
-            if st is None or st.B != B or st.S != max_seq_length or st.idx.dtype != idx.dtype or st.idx.device != idx.device:
+            if (st is None or st.B != B or st.S != max_seq_length or st.idx.dtype != idx.dtype or st.idx.device != idx.device
+                    or st.row_pos != rows):
                 if self._fast_ok is None:
                     self._fast_ok = self._fast_decode_ok()
                 # gptq.int8 and LLaMA-Adapter v2: batch 1 only; gptq.int8 without v2 affines at batch 2..16 on request
@@ -744,10 +827,10 @@ class LLaMA(nn.Module):
                         and (B == 1 or self._fast_ok == "q8"
                              or (self._fast_ok != "w8" and not self._has_affines())
                              or (self._fast_ok == "w8" and self.w8_batch_step and not self._has_affines())))
-                st = self._decode = _DecodeState(self, B, max_seq_length, idx.device, idx.dtype) if fast else None
+                st = self._decode = _DecodeState(self, B, max_seq_length, idx.device, idx.dtype, rows) if fast else None
         if st is not None:
             st.idx.copy_(idx.reshape(-1))
-            st.pos.copy_(input_pos.reshape(-1)[-1:])
+            st.pos.copy_(input_pos.reshape(-1) if rows else input_pos.reshape(-1)[-1:])
             if st.graph is not None:
                 st.graph.replay()
             elif self.graph_after and st.calls >= self.graph_after:
@@ -764,13 +847,14 @@ class LLaMA(nn.Module):
         # ---- single-token decode the fused step does not run (llm.int8, grouped or biased gptq, dense, gptq.int8 at
         #      B >= 2): the module-by-module launch sequence, replayed as a CUDA graph once warm
         if input_pos is not None and T == 1 and self.graph_after and idx.dtype in (torch.int32, torch.int64):
-            key = (B, max_seq_length, idx.dtype, idx.device, WEIGHTS_GENERATION[0])   # the graph bakes weight pointers too
+            key = (B, max_seq_length, idx.dtype, idx.device, WEIGHTS_GENERATION[0], rows)   # the graph bakes weight pointers too
             mg = self._module_graph
             if mg is None or mg["key"] != key:
                 mg = self._module_graph = dict(key=key, calls=0, graph=None, idx=torch.zeros((B, 1), dtype=idx.dtype, device=idx.device),
-                                               pos=torch.zeros(1, dtype=torch.int64, device=idx.device), out=None)
+                                               pos=torch.zeros((B, 1) if rows else (1,), dtype=torch.int64, device=idx.device),
+                                               out=None)
             mg["idx"].copy_(idx)
-            mg["pos"].copy_(input_pos.reshape(-1)[-1:])
+            mg["pos"].copy_(input_pos if rows else input_pos.reshape(-1)[-1:])
             if mg["graph"] is not None:
                 mg["graph"].replay()
                 return mg["out"].clone() if self.copy_logits else mg["out"]
@@ -800,9 +884,7 @@ class LLaMA(nn.Module):
         if self.rope_cache is None or self.rope_cache.device != idx.device:
             self.rope_cache = self.build_rope_cache(idx).float().contiguous()
         if self._ring is None or self._ring.device != idx.device:
-            self._ring = torch.zeros(1, dtype=torch.int32, device=idx.device)
-            for blk in self.transformer.h:
-                blk.attn._ring, blk.attn._ring_shared = self._ring, True
+            self._set_ring(torch.zeros(1, dtype=torch.int32, device=idx.device))
         return max_seq_length
 
     def _forward_modules(self, idx: torch.Tensor, max_seq_length: int, input_pos: Optional[torch.Tensor]) -> torch.Tensor:
@@ -829,7 +911,12 @@ class LLaMA(nn.Module):
                 x, _ = block(x, self.rope_cache, None, max_seq_length, _rope_is_table=True)
         else:
             pos = input_pos.reshape(-1).to(torch.int64)
-            L.check(L.lib().b2l_ring_advance(pos.data_ptr(), T, self._ring.data_ptr(), max_seq_length, L.stream_ptr()), "b2l_ring_advance")
+            if input_pos.dim() == 2:   # one position per row (T == 1): each row's ring advances on its own
+                L.check(L.lib().b2l_ring_advance_rows(pos.data_ptr(), B, self._ring.data_ptr(), max_seq_length, L.stream_ptr()),
+                        "b2l_ring_advance_rows")
+                pos = pos.view(B, 1)
+            else:
+                L.check(L.lib().b2l_ring_advance(pos.data_ptr(), T, self._ring.data_ptr(), max_seq_length, L.stream_ptr()), "b2l_ring_advance")
             for i, block in enumerate(self.transformer.h):
                 x, self.kv_caches[i] = block(x, self.rope_cache, None, max_seq_length, pos, self.kv_caches[i], _rope_is_table=True)
 
