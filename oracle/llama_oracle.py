@@ -175,6 +175,227 @@ def int8_linear(x: Tensor, cb: Tensor, scb: Tensor, threshold: float = 6.0) -> T
     return y.to(x.dtype).reshape(*shape[:-1], cb.shape[0])
 
 
+# LLM.int8() held exactly.  int8_linear above rounds the dequantised part fp64 -> fp32 -> fp16 (a double rounding);
+# int8_linear_exact is the single-rounding statement of the same algorithm, with threshold θ:
+#   x̂ = fp16(x);  O = {k : some row has |x̂[m,k]| >= θ};  SCA_m = max_{k∉O} |x̂[m,k]|;  qs = fl32(127 / SCA_m) (0 if 0)
+#   CA = clamp(rint_even(fl32(x̂ qs)), ±127), 0 on O;  t = CA · CB[o] (exact);  v = fp16(t SCA_m SCB_o / 127²)
+#   w_k = fp16(CB[o,k] SCB_o / 127);  τ = Σ_{k∈O} x̂_k w_k;  y = fp16(fl32(v + fp16(τ))) if O ≠ ∅ else v;  out = bf16(y)
+# Steps with exact operands (mask, SCA, qs, CA, t, the fp32 add of two fp16 values, every conversion) are reproduced
+# bit for bit.  Where a kernel chooses the evaluation order, the result is an admissible set: the correctly rounded
+# value R(e), plus its neighbours across fp16 / bf16 midpoints that lie within the derived bound b of the exact e.
+# Rounding is monotone, so a value computed within b of e rounds into [R(e - b), R(e + b)]; y, the bf16 store and the
+# epilogue are monotone in each operand, so every set is an interval [lo, hi] of the output format (one value away
+# from midpoints; then it is compared bit for bit), plus NaN where a corner of it is NaN.  Bounds, u = 2^-24 and
+# γ_n = n u / (1 - n u):
+#   v: (float)t, fl32(1/127²), sca·scb, ·(1/127²), t·that: five fp32 roundings, |err| <= γ_5 |v|;
+#   w_k: fl32(SCB / 127), then fl32(CB · that): two roundings, γ_2 |w_k|;
+#   τ: a chain of n = |O| fmaf, |err| <= γ_n Σ|x̂_k w_k|, plus |x̂_k| ulp16(w_k) for each w_k with two candidates;
+#   silu: expf within 2 ulp (no fast math), then 1 + e and the IEEE division: |err| <= (2·2u + 2u + γ_2)|silu| < 7u|silu|.
+# float64 slack (the fp64 products, and a float64 GEMM that may reorder its sum) is added on top of each.
+INT8_U = 2.0 ** -24
+
+
+def _gamma(n):
+    return n * INT8_U / (1.0 - n * INT8_U)
+
+
+def round_to(e: Tensor, dtype) -> Tensor:
+    """float64 -> fp16 / bf16 / fp32 rounded once to nearest even (overflow to inf, subnormals, signed zero).  A plain
+    .to(dtype) may go through fp32 and round twice, so the fp32 step rounds to odd: fp32 carries more than two extra
+    bits over fp16 and bf16, and rounding to odd first makes the second rounding the correctly rounded one."""
+    e = e.double()
+    f = e.float()
+    if dtype == torch.float32:
+        return f
+    inexact = (f.double() != e) & torch.isfinite(e)
+    toward0 = torch.where(f.double().abs() > e.abs(), torch.nextafter(f, torch.zeros_like(f)), f)
+    bits = toward0.view(torch.int32)
+    odd = torch.where(inexact, bits | 1, bits).view(torch.float32)
+    return odd.to(dtype)
+
+
+def ulp16(w: Tensor) -> Tensor:
+    """The spacing of fp16 at |w| (subnormal spacing 2^-24 included)."""
+    a = w.double().abs().clamp_min(2.0 ** -14)
+    return torch.pow(2.0, torch.floor(torch.log2(a)) - 10)
+
+
+def _around(e: Tensor, b: Tensor, dtype):
+    """(R(e), R(e - b), R(e + b)); a non-finite e keeps its own value."""
+    b = torch.where(torch.isfinite(e) & torch.isfinite(b), b, torch.zeros_like(b))
+    return round_to(e, dtype), round_to(e - b, dtype), round_to(e + b, dtype)
+
+
+@dataclass
+class Adm:
+    """An admissible set: the values of [lo, hi] in the output format (lo == hi bitwise: that value alone), and NaN
+    where nan; `id` is the single-rounded value."""
+    id: Tensor
+    lo: Tensor
+    hi: Tensor
+    nan: Tensor
+
+    @staticmethod
+    def of(id: Tensor, corners) -> "Adm":
+        c = torch.stack([x.float() for x in corners])
+        isn = torch.isnan(c)
+        lo = torch.where(isn, float("inf"), c).amin(0)
+        hi = torch.where(isn, float("-inf"), c).amax(0)
+        none = isn.all(0)
+        lo = torch.where(none, float("nan"), lo)
+        hi = torch.where(none, float("nan"), hi)
+        # signed zero: -0 and +0 corners give [-0, +0]; corners of one value keep its bits
+        neg0 = ((c == 0) & (torch.signbit(c))).any(0)
+        pos0 = ((c == 0) & ~torch.signbit(c)).any(0)
+        lo = torch.where((lo == 0) & neg0, -0.0, lo)
+        hi = torch.where((hi == 0) & pos0, 0.0, hi)
+        same = (c.view(torch.int32) == c[0:1].view(torch.int32)).all(0)
+        lo = torch.where(same, c[0], lo)
+        hi = torch.where(same, c[0], hi)
+        return Adm(id=id, lo=lo.to(id.dtype), hi=hi.to(id.dtype), nan=isn.any(0))
+
+    def contains(self, y: Tensor) -> Tensor:
+        yb, lb, hb = (t.view(torch.int16) for t in (y, self.lo, self.hi))
+        single = lb == hb
+        yf, lo, hi = y.float(), self.lo.float(), self.hi.float()
+        return (torch.isnan(y) & self.nan) | (single & (yb == lb)) | (~single & (yf >= lo) & (yf <= hi))
+
+    def single(self) -> Tensor:
+        return self.lo.view(torch.int16) == self.hi.view(torch.int16)
+
+    def width(self) -> Tensor:
+        """Steps of the output format from lo to hi (0: one value)."""
+        return _ordinal(self.hi) - _ordinal(self.lo)
+
+
+def _ordinal(x: Tensor) -> Tensor:
+    """16-bit float bits -> integers in the order of the values (-0 and +0 adjacent)."""
+    b = x.view(torch.int16).int()
+    return torch.where(b < 0, -(b & 0x7FFF) - 1, b)
+
+
+def _from_ordinal(o: Tensor, dtype) -> Tensor:
+    b = torch.where(o < 0, (-(o + 1)) | 0x8000, o)
+    return b.to(torch.int32).to(torch.int16).view(dtype) if dtype != torch.int16 else b
+
+
+def _tau_exact(xo: Tensor, w: Tensor) -> Tensor:
+    """Σ_k xo[m,k] w[o,k] in float64; elementwise when an operand is not finite, so inf·0 and inf - inf give NaN exactly
+    as the kernels' fp32 chain does (a GEMM library may not)."""
+    if bool(torch.isfinite(xo).all()) and bool(torch.isfinite(w).all()):
+        return xo @ w.t()
+    return torch.stack([(xo[m].unsqueeze(0) * w).sum(-1) for m in range(xo.shape[0])])
+
+
+@dataclass
+class Int8Exact:
+    """int8_linear_exact's result.  Exact parts: xh (fp16 x̂), mask, sca, qs, ca, t (float64).  Per output: v (fp16
+    single-rounded dequantised part) and its set [v_lo, v_hi], tau (float64 exact τ) and tau_bound, and `out`, the bf16 output's Adm."""
+    xh: Tensor
+    mask: Tensor
+    sca: Tensor
+    qs: Tensor
+    ca: Tensor
+    t: Tensor
+    v: Tensor
+    v_lo: Tensor
+    v_hi: Tensor
+    tau: Tensor
+    tau_bound: Tensor
+    out: Adm
+
+
+def int8_linear_exact(x: Tensor, cb: Tensor, scb: Tensor, threshold: float = 6.0, mask: Optional[Tensor] = None) -> Int8Exact:
+    """The exact restatement above for x [M, K] (bf16 or fp32 values; after the RMSNorm prologue when there is one)
+    against CB [N, K] int8 and SCB [N] fp32.  mask: a given outlier mask (bool [K]) instead of the derived one.  Runs on
+    x's device: the float64 contractions of integers are exact in any order below 2^53.  qs is the IEEE quotient, as
+    the kernels' 127.0f / SCA (int8_linear's `127.0 / sca` is torch's reciprocal-then-multiply, which can differ by an
+    ulp and move a product onto or off a .5 tie)."""
+    xh = x.float().half()
+    a = xh.float()
+    if mask is None:
+        mask = (a.abs() >= threshold).any(0)
+    mask = mask.to(device=a.device, dtype=torch.bool)
+    a_in = a.masked_fill(mask, 0.0)
+    sca = a_in.abs().amax(1)
+    qs = torch.where(sca > 0, torch.tensor(127.0, dtype=torch.float32, device=a.device) / sca, torch.zeros_like(sca))
+    ca = torch.round(a_in * qs.unsqueeze(1)).clamp_(-127, 127).masked_fill_(mask, 0.0)
+    t = ca.double() @ cb.double().t() + 0.0   # + 0.0: an all-zero sum is +0, as the kernels' int32 t converts
+    scbd = scb.double()
+    ev = t * sca.double().unsqueeze(1) * scbd.unsqueeze(0) / 16129.0
+    v_id, v_lo, v_hi = _around(ev, ev.abs() * (_gamma(5) + 2.0 ** -48), torch.float16)
+    n = int(mask.sum())
+    M, N = t.shape
+    bf = lambda y: y.float().bfloat16()
+    if n == 0:
+        tau = torch.zeros(M, N, dtype=torch.float64, device=a.device)
+        tb = torch.zeros_like(tau)
+        out = Adm.of(bf(v_id), [bf(v_lo), bf(v_hi)])
+    else:
+        ew = cb[:, mask].double() * scbd.unsqueeze(1) / 127.0
+        w = round_to(ew, torch.float16).double()
+        wb = ew.abs() * (_gamma(2) + 2.0 ** -48)
+        amb = (round_to(ew - wb, torch.float16) != round_to(ew + wb, torch.float16)).double() * ulp16(w)
+        xo = a[:, mask].double()
+        tau = _tau_exact(xo, w) + 0.0   # the kernels' chain starts from +0
+        s1 = _tau_exact(xo.abs(), w.abs())
+        s2 = _tau_exact(xo.abs(), amb) if bool(amb.any()) else torch.zeros_like(s1)
+        tb = _gamma(n) * (s1 + s2) + s2 + 2.0 ** -40 * s1
+        t_id, t_lo, t_hi = _around(tau, tb, torch.float16)
+        add = lambda p, q: bf((p.float() + q.float()).half())   # bf16(fp16(fl32(v + fp16(τ))))
+        out = Adm.of(add(v_id, t_id), [add(p, q) for p in (v_lo, v_hi) for q in (t_lo, t_hi)])
+    return Int8Exact(xh=xh, mask=mask, sca=sca, qs=qs, ca=ca, t=t, v=v_id, v_lo=v_lo, v_hi=v_hi, tau=tau, tau_bound=tb, out=out)
+
+
+def int8_affine(y: Tensor, s: Tensor, b: Tensor) -> Tensor:
+    """LLaMA-Adapter v2's affine on a bf16 linear output: bf16(s · bf16(y + b)) (adapter_v2.py:30-33), exact."""
+    return ((y.float() + b.float()).bfloat16().float() * s.float()).bfloat16()
+
+
+def int8_adm_affine(y: Adm, s: Tensor, b: Tensor) -> Adm:
+    f = lambda t: int8_affine(t, s, b)
+    r = Adm.of(f(y.id), [f(y.lo), f(y.hi)])   # monotone either way (the sign of s)
+    r.nan = r.nan | y.nan
+    return r
+
+
+def int8_adm_residual(y: Adm, res: Tensor) -> Adm:
+    f = lambda t: (t.float() + res.float()).bfloat16()
+    r = Adm.of(f(y.id), [f(y.lo), f(y.hi)])
+    r.nan = r.nan | y.nan
+    return r
+
+
+def _silu_bf16(y1: Tensor):
+    """bf16(silu(y1)): (correctly rounded, lowest, highest) over the kernels' fp32 y / (1 + expf(-y)) within 7u and the
+    host's own fp32 evaluation of it (which also carries the non-finite cases and expf's overflow below -88.7)."""
+    a = y1.double()
+    e = a / (1.0 + torch.exp(-a))
+    s_id, s_lo, s_hi = _around(e, e.abs() * (7 * INT8_U + 2.0 ** -48), torch.bfloat16)
+    y1f = y1.float()
+    s_host = (y1f / (1.0 + torch.exp(-y1f))).bfloat16()
+    return s_id, [s_lo, s_hi, s_host]
+
+
+SILU_ARGMIN = -1.2784645   # silu falls below it and rises above it; silu(SILU_ARGMIN) = -0.2784645
+
+
+def int8_adm_silu_mul(y1: Adm, y2: Adm) -> Adm:
+    """SwiGLU's bf16(bf16(silu(y1)) · y2) (model.py:252).  silu is monotone on each side of its minimum, so over y1's
+    interval it ranges between its values at the ends, and down to the minimum where the interval straddles it; the
+    product is monotone in each factor, so its corners bound it."""
+    mul = lambda s, t: (s.float() * t.float()).bfloat16()
+    s_id, _ = _silu_bf16(y1.id)
+    ends = _silu_bf16(y1.lo)[1] + _silu_bf16(y1.hi)[1]
+    straddle = (y1.lo.float() < SILU_ARGMIN) & (y1.hi.float() > SILU_ARGMIN)
+    s_min = _silu_bf16(torch.full_like(y1.lo, SILU_ARGMIN, dtype=torch.float64))[1]
+    ends += [torch.where(straddle, m.float(), ends[0].float()).bfloat16() for m in s_min]
+    s = Adm.of(s_id, ends)
+    r = Adm.of(mul(s_id, y2.id), [mul(p, q) for p in (s.lo, s.hi) for q in (y2.lo, y2.hi)])
+    r.nan = r.nan | s.nan | y2.nan
+    return r
+
+
 # ----------------------------------------------------------------------------
 # lit_llama/model.py
 # ----------------------------------------------------------------------------

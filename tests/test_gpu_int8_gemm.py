@@ -29,7 +29,7 @@ def _activations(M, K, pattern, g):
     elif pattern == "exact6":   # |a| == threshold is an outlier, just below is not
         x[0, 5] = 6.0
         x[M - 1, K - 1] = -6.0
-        x[M // 2, K // 2] = 5.984375   # largest bf16 below 6
+        x[M // 2, K // 2] = 5.96875    # largest bf16 below 6
     return x.bfloat16()
 
 
