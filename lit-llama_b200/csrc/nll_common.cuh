@@ -24,16 +24,19 @@ __device__ __forceinline__ long long load_target(const void* t, int i64, int m) 
   return i64 ? reinterpret_cast<const long long*>(t)[m] : (long long)reinterpret_cast<const int*>(t)[m];
 }
 
-// (max, sum of expf(v - max)) of one row's tile; every lane of the quad returns the same pair.
+// (max, sum of expf(v - max)) of one row's tile; every lane of the quad returns the same pair.  A tile whose columns
+// are all -inf gives (-inf, 0), which adds nothing in the combine (0 * expf(-inf - mx) = 0); expf(-inf - -inf) would
+// make it NaN.
 __device__ __forceinline__ float2 quad_partial(const float (&v)[32]) {
   float mx = v[0];
 #pragma unroll
   for (int i = 1; i < 32; ++i) mx = fmaxf(mx, v[i]);
   mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
   mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+  const float base = mx == -INFINITY ? 0.f : mx;
   float s = 0.f;
 #pragma unroll
-  for (int i = 0; i < 32; ++i) s += expf(v[i] - mx);
+  for (int i = 0; i < 32; ++i) s += expf(v[i] - base);
   s += __shfl_xor_sync(0xffffffffu, s, 1);
   s += __shfl_xor_sync(0xffffffffu, s, 2);
   return make_float2(mx, s);

@@ -13,8 +13,11 @@
 //   * logits / temperature is a bf16 tensor: ATen multiplies by the fp32 reciprocal of the
 //     scalar and rounds to bf16;
 //   * the threshold is the k-th largest of those bf16 values; ties at the threshold are kept
-//     (`logits < thr` is false for them), exactly like torch.where;
-//   * softmax is evaluated in fp32 (exp(x - max) / sum) and rounded to bf16.
+//     (`logits < thr` is false for them), exactly like torch.where.  -0 is stored as +0, so keys, ranks and the
+//     threshold follow IEEE equality (-0 == +0) and a -0 at a +0 threshold is kept; exp(±0 - max) is the same;
+//   * softmax is evaluated in fp32 (exp(x - max) / sum) and rounded to bf16;
+//   * the draw is argmax(bf16(p / q)) with torch.argmax's rule: the lowest index among equal maxima, and NaN (a NaN
+//     logit, or scaled logits that overflow to inf) ranks above every number, so the token is always in 0..V-1.
 #include "b2l_common.cuh"
 
 namespace b2l {
@@ -59,6 +62,15 @@ __device__ __forceinline__ void find_bin(const int* hist, int want, int* sel_bin
 
 __device__ __forceinline__ float bits_f(uint32_t bits16) { return __uint_as_float(bits16 << 16); }
 
+// bf16 bits of a scaled logit as stored in `sv`: -0 becomes +0
+__device__ __forceinline__ uint32_t canon_zero(uint32_t bits16) { return bits16 == 0x8000u ? 0u : bits16; }
+
+// the draw's order, torch.argmax(p / q): a larger r wins, equal r go to the lower index.  r = bf16(p / q) is +0..+inf
+// or the canonical NaN of the bf16 rounding (0x7fff), so its bits order it as a number, with NaN above +inf.
+__device__ __forceinline__ bool draw_beats(uint32_t r, int i, uint32_t best, int best_i) {
+  return r > best || (r == best && i < best_i);
+}
+
 // elements 8i..8i+7 of a bf16 row: one 16-byte load, or eight 2-byte loads for a row that does not start on 16 bytes
 // (V or ld not a multiple of 8)
 __device__ __forceinline__ uint4 load8(const __nv_bfloat16* p, int i, bool vec) {
@@ -87,6 +99,7 @@ __global__ void __launch_bounds__(SAMP_THREADS)
   __shared__ int hist[256];
   __shared__ int sel_hi, sel_rank, sel_lo;
   __shared__ float red[32];
+  __shared__ uint32_t red_b[32];
   __shared__ int red_i[32];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const bool select = top_k > 0 && top_k < V;
@@ -127,7 +140,7 @@ __global__ void __launch_bounds__(SAMP_THREADS)
       for (int q = 0; q < 4; ++q) {
         const float a = rbf(__uint_as_float(w[q] << 16) * inv_temperature);
         const float b = rbf(__uint_as_float(w[q] & 0xffff0000u) * inv_temperature);
-        const uint32_t ab = __float_as_uint(a) >> 16, bb = __float_as_uint(b) >> 16;
+        const uint32_t ab = canon_zero(__float_as_uint(a) >> 16), bb = canon_zero(__float_as_uint(b) >> 16);
         o[q] = ab | (bb << 16);
         if (valid) lmax = fmaxf(lmax, fmaxf(a, b));
         if (select) {
@@ -151,7 +164,7 @@ __global__ void __launch_bounds__(SAMP_THREADS)
     uint16_t bits = 0xff80;         // padding: -inf, below every threshold
     if (valid) {
       const float sc = rbf(bf2f(logits[i]) * inv_temperature);
-      bits = (uint16_t)(__float_as_uint(sc) >> 16);
+      bits = (uint16_t)canon_zero(__float_as_uint(sc) >> 16);
       lmax = fmaxf(lmax, sc);
     }
     if (i < Vp) {
@@ -227,7 +240,7 @@ __global__ void __launch_bounds__(SAMP_THREADS)
 
   // 4. probabilities (bf16) and, with `noise` (q ~ Exp(1) drawn by torch), the sample argmax(p / q) --
   // torch.multinomial's own algorithm for one draw (ATen/native/Distributions.cpp), ties to the lower index
-  float best = -INFINITY;
+  uint32_t best = 0;   // the bits of +0: every entry ties or beats it, at a lower index
   int best_i = 0x7fffffff;
   for (int base = 0; base < nvp; base += SAMP_THREADS) {
     const int i = base + tid;
@@ -255,8 +268,8 @@ __global__ void __launch_bounds__(SAMP_THREADS)
           pb2[hf] = __float_as_uint(pr) >> 16;
           if (noise != nullptr) {
             const int idx = 8 * i + 2 * q + hf;
-            const float r = rbf(pr / bits_f(hf ? (nw[q] >> 16) : (nw[q] & 0xffffu)));
-            if (idx < V && (r > best || (r == best && idx < best_i))) { best = r; best_i = idx; }
+            const uint32_t r = __float_as_uint(rbf(pr / bits_f(hf ? (nw[q] >> 16) : (nw[q] & 0xffffu))));
+            if (idx < V && draw_beats(r, idx, best, best_i)) { best = r; best_i = idx; }
           }
         }
         o[q] = pb2[0] | (pb2[1] << 16);
@@ -275,20 +288,20 @@ __global__ void __launch_bounds__(SAMP_THREADS)
   if (noise != nullptr) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
-      const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+      const uint32_t ob = __shfl_xor_sync(0xffffffffu, best, o);
       const int oi = __shfl_xor_sync(0xffffffffu, best_i, o);
-      if (ob > best || (ob == best && oi < best_i)) { best = ob; best_i = oi; }
+      if (draw_beats(ob, oi, best, best_i)) { best = ob; best_i = oi; }
     }
     __syncthreads();
-    if (lane == 0) { red[warp] = best; red_i[warp] = best_i; }
+    if (lane == 0) { red_b[warp] = best; red_i[warp] = best_i; }
     __syncthreads();
     if (warp == 0) {
-      best = red[lane]; best_i = red_i[lane];
+      best = red_b[lane]; best_i = red_i[lane];
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) {
-        const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+        const uint32_t ob = __shfl_xor_sync(0xffffffffu, best, o);
         const int oi = __shfl_xor_sync(0xffffffffu, best_i, o);
-        if (ob > best || (ob == best && oi < best_i)) { best = ob; best_i = oi; }
+        if (draw_beats(ob, oi, best, best_i)) { best = ob; best_i = oi; }
       }
       if (lane == 0) *token = (long long)best_i;
     }

@@ -397,6 +397,160 @@ def int8_adm_silu_mul(y1: Adm, y2: Adm) -> Adm:
 
 
 # ----------------------------------------------------------------------------
+# The logits tail held exactly: generate.py:68-76 (temperature, top-k, softmax, multinomial) and the next-token NLL of
+# evaluate/*.py, as csrc/sampling.cu and csrc/nll.cu compute them
+# ----------------------------------------------------------------------------
+# Sampling, per row of bf16 logits l [V] at temperature T and top-k k:
+#   s_i = bf16(fl32(l_i · fl32(1 / fl32(T))))            ATen's scalar-reciprocal path and the kernel: two roundings
+#   thr = the k-th largest s in IEEE order (NaN largest, as torch.topk); kept = {i : !(s_i < thr)}, so -0 and +0 are
+#         equal; k = 0 or k >= V keeps every entry
+#   gmax = max of the non-NaN s;  d_i = fl32(s_i - gmax) (bit for bit);  p*_i = exp(d_i) / Σ_kept exp(d_j) in float64
+# The kernel's p_i = bf16(fl32(expf(d_i) / Σ̂)) lies within ε p*_i of p*_i, with u = 2^-24:
+#   expf within 2 ulp (<= 4u relative) in the numerator and in each term of the sum; the sum in the kernel's order,
+#   m = 8 ⌈Vp / 8192⌉ sequential terms per thread and then 5 + 5 butterfly levels, γ_{m+10}; one IEEE division, u:
+#   ε = (1 + 4u)(1 + u) / ((1 - 4u)(1 - γ_{m+10})) - 1, plus an absolute 2^-147 for expf and the division where they
+#   return fp32 subnormals.  A probability's admissible set is [bf16(p* - b), bf16(p* + b)], one value away from bf16
+#   midpoints; the single-rounded value is round_to(p*, bf16).
+# Special cases, as torch's op sequence defines them: a NaN among the kept s (a NaN logit) or a +inf kept (the scaled
+# logits overflow, inf - inf) makes the softmax NaN.  Contract for such a row: every kept entry above -inf is NaN, every
+# other entry 0 (the filter removed it, or exp(-inf) is 0, before the softmax; torch spreads the NaN over them as well),
+# and the draw is the first NaN entry, as torch.argmax(p / q) ranks NaN first.  A kept -inf has probability 0.  A row with no kept value above
+# -inf has no distribution (torch: NaN); the kernel writes zeros and draws token 0, and the oracle states exactly that.
+SAMP_THREADS = 1024
+
+
+def _samp_eps(V: int) -> float:
+    vp = (V + 7) // 8 * 8
+    m = 8 * (-(-vp // (8 * SAMP_THREADS)))
+    u = INT8_U
+    return (1 + 4 * u) * (1 + u) / ((1 - 4 * u) * (1 - _gamma(m + 10))) - 1 + 2.0 ** -48
+
+
+@dataclass
+class TopkExact:
+    """topk_softmax_exact's result for logits [..., V]: the scaled bf16 values, the threshold (fp32; -inf: no filter),
+    the kept mask, gmax, d (fp32, bit for bit), p* (float64), the bound b and `probs`, the bf16 probabilities' Adm."""
+    scaled: Tensor
+    thr: Tensor
+    kept: Tensor
+    gmax: Tensor
+    d: Tensor
+    p: Tensor
+    bound: Tensor
+    probs: Adm
+
+
+def topk_softmax_exact(logits: Tensor, temperature: float, top_k: int) -> TopkExact:
+    lf = logits.float()
+    V = lf.shape[-1]
+    inv = torch.tensor(1.0, dtype=torch.float32) / torch.tensor(temperature, dtype=torch.float32)
+    s = (lf * inv).bfloat16()
+    sf = s.float()
+    if 0 < top_k < V:
+        thr = torch.topk(sf, top_k, dim=-1).values[..., -1:]
+    else:
+        thr = torch.full_like(sf[..., :1], float("-inf"))
+    kept = ~(sf < thr)
+    gmax = torch.where(torch.isnan(sf), float("-inf"), sf).amax(-1, keepdim=True)
+    d = sf - gmax
+    dd = d.double()
+    e = torch.where(kept & (sf != float("-inf")), torch.exp(dd), torch.zeros_like(dd))
+    tot = e.sum(-1, keepdim=True)
+    nan_row = torch.isnan(tot)
+    p = e / tot
+    eps = _samp_eps(V)
+    b = p.abs() * eps + 2.0 ** -147
+    b = torch.where(torch.isfinite(p), b, torch.zeros_like(b))
+    lo = round_to(torch.clamp(p - b, min=0.0), torch.bfloat16)
+    hi = round_to(p + b, torch.bfloat16)
+    pid = round_to(p, torch.bfloat16)
+    # the contracts above: NaN rows keep NaN at kept entries and 0 at filtered ones; rows with nothing above -inf are 0
+    zero = torch.zeros_like(pid)
+    empty = (tot == 0) & ~nan_row
+    nan_kept = nan_row & kept & (sf != float("-inf"))
+    nanv = torch.full_like(pid, float("nan"))
+    fix = lambda t: torch.where(nan_kept, nanv, torch.where((nan_row & ~kept) | empty, zero, t))
+    probs = Adm.of(fix(pid), [fix(lo), fix(hi)])
+    return TopkExact(scaled=s, thr=thr, kept=kept, gmax=gmax, d=d, p=p, bound=b, probs=probs)
+
+
+def draw_exact(probs: Tensor, q: Tensor) -> Tensor:
+    """torch.multinomial(probs, 1) as argmax(probs / q) on bf16 tensors: r = bf16(fl32(p / q)), the first maximum, with
+    NaN ranked above everything (torch.argmax's rule).  Exact given the probabilities.  int64 [...]."""
+    r = (probs.float() / q.float()).bfloat16().float()
+    isn = torch.isnan(r)
+    V = r.shape[-1]
+    idx = torch.arange(V).expand_as(r)
+    first_nan = torch.where(isn, idx, V).amin(-1)
+    rr = torch.where(isn, float("-inf"), r)
+    top = rr.amax(-1, keepdim=True)
+    first_max = torch.where(rr == top, idx, V).amin(-1)
+    return torch.where(isn.any(-1), first_nan, first_max).to(torch.int64)
+
+
+# Next-token NLL (nll.cu / nll_common.cuh / the NLL epilogue of q4_gemm.cu) of bf16 logits L [M, N] against targets t:
+#   nll_m = logsumexp_n L[m, n] - L[m, t_m], computed as: per 128-column tile j, mx_j = max and
+#   s_j = Σ_i expf(fl32(v_i - mx_j)) (each lane 32 sequential terms, then 2 butterfly adds); the combine
+#   mx = max_j mx_j, ŝ = Σ_j fl32(s_j · expf(fl32(mx_j - mx))) sequentially over the n_tiles tiles; then
+#   fl32(fl32(mx + logf(ŝ)) - L[m, t]).  A tile whose columns are all -inf contributes s_j = 0.
+# Absolute bound, u = 2^-24, E_j = Σ_i e^{d_ij}, A_j = Σ_i |d_ij| e^{d_ij}, w_j = e^{Δ_j}, Δ_j = mx_j - mx:
+#   a rounded difference d(1 + δ) moves e^d by at most u |d| e^d; expf 4u; the tile sum γ_34; the product u; the
+#   combine sum γ_{n_tiles}:  |ŝ - S| <= (γ_34 + 9u + γ_{n_tiles}) S + u Σ_j w_j (A_j + |Δ_j| E_j)  (first order, ×1.01);
+#   logf within 1 ulp (<= 2u |log ŝ|), |log ŝ - log S| <= ρ / (1 - ρ), ρ = |ŝ - S| / S; then the roundings of
+#   mx + log ŝ and of the final subtraction, u each.
+# NaN where torch's cross_entropy gives NaN: a NaN or +inf logit in the row, an all -inf row, a target outside
+# 0..N-1; +inf where the target's logit is -inf (and the row has a finite logit).
+NLL_TILE = 128
+
+
+@dataclass
+class NLLExact:
+    """nll_exact's result: nll (float64 [M], NaN / +inf in the special cases) and bound (float64 [M], 0 there)."""
+    nll: Tensor
+    bound: Tensor
+
+
+def nll_exact(logits: Tensor, targets: Tensor) -> NLLExact:
+    Lf = logits.double()
+    M, N = Lf.shape
+    t = targets.long().view(-1)
+    nt = -(-N // NLL_TILE)
+    pad = torch.full((M, nt * NLL_TILE - N), float("-inf"), dtype=torch.float64)
+    T = torch.cat([Lf, pad], 1).view(M, nt, NLL_TILE)
+    u = INT8_U
+    fin = torch.where(torch.isnan(T), float("-inf"), T)
+    mxj = fin.amax(-1)                                   # [M, nt]
+    live = mxj > float("-inf")
+    mxj0 = torch.where(live, mxj, torch.zeros_like(mxj))
+    dij = torch.where(T > float("-inf"), T - mxj0.unsqueeze(-1), torch.full_like(T, float("-inf")))
+    eij = torch.exp(dij)
+    Ej = eij.sum(-1)
+    Aj = torch.where(eij > 0, dij.abs() * eij, torch.zeros_like(eij)).sum(-1)
+    mx = mxj.amax(-1, keepdim=True)
+    mx0 = torch.where(mx > float("-inf"), mx, torch.zeros_like(mx))
+    dj = torch.where(live, mxj - mx0, torch.full_like(mxj, float("-inf")))
+    wj = torch.exp(dj)
+    S = (wj * Ej).sum(-1)
+    err_s = (_gamma(34) + 9 * u + _gamma(nt)) * S + u * (wj * (Aj + torch.where(live, dj.abs(), torch.zeros_like(dj)) * Ej)).sum(-1)
+    err_s = err_s * 1.01 + 2.0 ** -140 * N
+    lnS = torch.log(S)
+    rho = err_s / S
+    rho = rho / (1 - rho)
+    ls_err = rho + 2 * u * (lnS.abs() + rho)
+    mxv = mx.squeeze(-1)
+    a = (mxv + lnS).abs() + ls_err
+    r_err = ls_err + u * a * (1 + u)
+    ok_t = (t >= 0) & (t < N)
+    lt = Lf.gather(1, t.clamp(0, N - 1).view(-1, 1)).squeeze(1)
+    nll = mxv + lnS - lt
+    bound = (r_err + u * (nll.abs() + r_err)) * (1 + 1e-9)
+    bad = torch.isnan(Lf).any(1) | (Lf == float("inf")).any(1) | ~(Lf > float("-inf")).any(1) | ~ok_t
+    nll = torch.where(bad, float("nan"), torch.where(lt == float("-inf"), float("inf"), nll))
+    bound = torch.where(torch.isfinite(nll), bound, torch.zeros_like(bound))
+    return NLLExact(nll=nll, bound=bound)
+
+
+# ----------------------------------------------------------------------------
 # lit_llama/model.py
 # ----------------------------------------------------------------------------
 def rmsnorm(x: Tensor, scale: Tensor, eps: float = 1e-5) -> Tensor:
