@@ -159,10 +159,14 @@ enum {
   B2L_F_Q8_BATCH = 512, /* b2l_decode_step with B2L_F_Q8 at B in 2..16: every linear runs b2l_q8_linear_batch on
                            CB / SCB in place; batch_work must hold b2l_q8_linear_batch_workspace_bytes(max K, B)
                            bytes; v2 affines allowed; not with B2L_F_W8, B2L_F_W8_BATCH or B2L_F_Q4_BATCH_I8; no plan */
-  B2L_F_ROW_POS = 1024  /* b2l_attention(_adapter) at T == 1 and b2l_decode_step: one position per row.
+  B2L_F_ROW_POS = 1024, /* b2l_attention(_adapter) at T == 1 and b2l_decode_step: one position per row.
                            input_pos is int64[B] (row b's token is at input_pos[b]) and ring_start int32[B] (row b's
                            own ring offset); not with B2L_F_ROPE_ROWS or a persistent plan.  The step advances each
                            row's ring on its own (b2l_ring_advance_rows) */
+  B2L_F_STEPWISE = 2048 /* b2l_attention(_adapter) at B == 1, T = 2..16, and b2l_decode_step with B = 2..16: the rows
+                           are consecutive tokens of ONE sequence (the verify step of speculative decoding), each
+                           computed exactly as a T == 1 launch / a batch-1 step at its position would compute it.
+                           See b2l_attention and b2l_decode_step; not with B2L_F_ROW_POS or B2L_F_ROPE_ROWS */
 };
 
 /* Fused [RMSNorm ->] int4 linear [-> residual | SwiGLU] on wgmma (M <= 16).  Replaces
@@ -411,6 +415,24 @@ int b2l_topk_softmax_rows(const void* logits, int64_t ld, float temperature, int
 int b2l_topk_softmax_sample_rows(const void* logits, int64_t ld, float temperature, int top_k, const void* noise,
                                  void* probs, int64_t* tokens, int B, int V, b2l_stream_t stream);
 
+/* Speculative sampling (accept / resample) of one verify step in one launch.  The target's T = k + 1 logits rows
+ * (target_logits + t * ld, bf16, ld >= V) give p_t exactly as b2l_topk_softmax_rows computes it (bit for bit); the
+ * draft proposed tokens x_0..x_{k-1} (draft_tokens int64 [k]) with probability rows q_t (draft_probs bf16 [k, V]).
+ *   x_t is accepted iff u_t * q_t(x_t) < p_t(x_t) in fp32 (u fp32 [k], uniform [0, 1)); strict, so u = 0 never
+ *   accepts a token the target gives probability 0.  A draft token outside 0..V-1 is rejected.
+ *   j = the first rejected t:   *token = argmax_i bf16(max(0, p_j(i) - q_j(i)) / noise[i])  (the residual
+ *                               distribution's draw, unnormalised); when that residual is zero everywhere (bf16
+ *                               rounding only): argmax_i bf16(p_j(i) / noise[i]), a draw from p_j
+ *   every x_t accepted:         *token = argmax_i bf16(p_k(i) / noise[i])
+ * noise bf16 [V] is q ~ Exp(1) drawn by the caller (as for b2l_topk_softmax_sample); argmax ties go to the lower
+ * index.  *n_accepted (device int32) = j, or k when every draft token is accepted; *token is device int64.
+ * With top_k == 1 this is "accept while x_t == argmax p_t, then emit the target's argmax".  T in 2..16; target_logits,
+ * draft_probs and noise 16-byte aligned.  Bad arguments are B2L_E_ARG / B2L_E_UNSUPPORTED with a message naming
+ * the argument, before the device is touched.  One CTA walks the rows in order and stops at the first rejection. */
+int b2l_spec_accept(const void* target_logits, int64_t ld, float temperature, int top_k, const void* draft_probs,
+                    const int64_t* draft_tokens, const float* u, const void* noise, int32_t* n_accepted, int64_t* token,
+                    int T, int V, b2l_stream_t stream);
+
 /* ------------------------------------------------------------------------------
  * CausalSelfAttention.forward without the two linears, model.py:197-232:
  * split qkv, apply_rope(q), apply_rope(k) (model.py:306-323), append k,v to the
@@ -426,6 +448,14 @@ int b2l_topk_softmax_sample_rows(const void* logits, int64_t ld, float temperatu
  * With B2L_F_ROW_POS (T == 1): input_pos int64 [B] and ring_start int32 [B], row b at
  *            its own position and ring offset (b2l_ring_advance_rows moves them).  Each
  *            row's y and cache rows equal a B = 1 launch on that row bit for bit.
+ * With B2L_F_STEPWISE (B == 1, T = 2..16): input_pos int64 [T] holds consecutive positions
+ *            p..p+T-1, all < S (no roll).  Query t's y row and its appended k / v row equal,
+ *            bit for bit, a T == 1 launch at position p+t on the cache holding the tokens
+ *            before it.  head_size 128: one launch appends every rotated k row and v row,
+ *            then the fused kernel runs one CTA group per (t, head), without programmatic
+ *            dependent launch; B2L_F_ATTN_UNFUSED and other head sizes: the three-kernel
+ *            path with the T == 1 split plan per query.  work: b2l_attn_workspace_bytes(T,
+ *            n_head, head_size, 1, S) bytes (T rows at T == 1).
  * y     bf16 [B, T, C]
  * work  scratch of b2l_attn_workspace_bytes(...) bytes (split-S partials + tickets);
  *       the caller zero-fills it ONCE after allocating it
@@ -597,7 +627,7 @@ typedef struct b2l_decode_args {
   const void* rope;          /* f32 [block_size, hs/2, 2]                             */
   const void* idx;           /* int32/int64 [B] tokens of this step                   */
   int idx_is_i64;
-  const int64_t* input_pos;  /* int64 [1]; [B] under B2L_F_ROW_POS                    */
+  const int64_t* input_pos;  /* int64 [1]; [B] under B2L_F_ROW_POS or B2L_F_STEPWISE   */
   int32_t* ring_start;       /* int32 [1] ([B] under B2L_F_ROW_POS); advanced by the step when the cache is full */
   int block_size;            /* rows of the rope table                                */
   void* x;                   /* bf16 [B, C]   residual stream scratch                 */
@@ -643,6 +673,12 @@ typedef struct b2l_decode_args {
   float q8_threshold;        /* B2L_F_Q8: Linear8bitLt.threshold of every linear          */
 } b2l_decode_args;
 
+/* With B2L_F_STEPWISE the B = 2..16 rows are consecutive tokens of ONE sequence: idx [B], input_pos int64 [B] holding
+ * p..p+B-1 (all < S), layers[].k_cache / v_cache the batch-1 caches [1, nh, S, hs], attn_work
+ * b2l_attn_workspace_bytes(B, nh, hs, 1, S) bytes.  Row t's logits equal the batch-1 step's at position p+t on the cache
+ * holding the tokens before it, bit for bit, and the cache ends as B batch-1 steps leave it.  Only with the row-exact
+ * linears: B2L_F_Q4_BATCH_I8, or B2L_F_W8 | B2L_F_W8_BATCH; not with B2L_F_Q8, B2L_F_ROW_POS, `plan` or `affines`.
+ * Adapters and LoRA run as in the batched step; each layer's attention is one launch more (b2l_attention). */
 int b2l_decode_step(const b2l_decode_args* args, b2l_stream_t stream);
 /* The persistent decode kernel's static op list + arrival counters.  b2l_decode_plan_build fills args->plan from
  * the pointers in args (call it once, outside graph capture; rebuild when any pointer in args changes);

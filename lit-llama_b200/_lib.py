@@ -19,6 +19,7 @@ F_W8_BATCH = 128   # b2l_decode_step with F_W8 at B in 2..16: every linear runs 
 F_Q4_BATCH_I8 = 256   # b2l_decode_step (gptq.int4) at B in 2..16: every linear runs b2l_q4_gemv_batch_i8
 F_Q8_BATCH = 512   # b2l_decode_step with F_Q8 at B in 2..16: every linear runs b2l_q8_linear_batch
 F_ROW_POS = 1024   # b2l_attention (T == 1) and b2l_decode_step: input_pos int64[B] and ring_start int32[B], one per row
+F_STEPWISE = 2048   # b2l_attention (B == 1, T = 2..16) and b2l_decode_step: the rows are consecutive tokens of one sequence
 
 c_void_p, c_int, c_float, c_size_t = C.c_void_p, C.c_int, C.c_float, C.c_size_t
 
@@ -167,6 +168,8 @@ _SIGS = {
     "b2l_topk_softmax_rows": (c_int, [c_void_p, C.c_int64, c_float, c_int, c_void_p, c_int, c_int, c_void_p]),
     "b2l_topk_softmax_sample_rows": (c_int, [c_void_p, C.c_int64, c_float, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                              c_void_p]),
+    "b2l_spec_accept": (c_int, [c_void_p, C.c_int64, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                c_void_p, c_int, c_int, c_void_p]),
     "b2l_q8_tiled_bytes": (c_size_t, [c_int, c_int]),
     "b2l_q8_tile": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "b2l_q8_gemv": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_int, c_void_p]),

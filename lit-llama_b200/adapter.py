@@ -181,6 +181,7 @@ class LLaMA(llama.LLaMA):
             self._adapter_store = torch.zeros(shape, device=device, dtype=torch.bfloat16)
             self._adapter_gates = torch.zeros((cfg.n_layer, nh), device=device, dtype=torch.bfloat16)
             self._decode, self._module_graph = None, None   # they point at the old store
+            self._verify = {}
         st, gates = self._adapter_store, self._adapter_gates
         arr = (L.AdapterPrefix * cfg.n_layer)()
         for i in layers:

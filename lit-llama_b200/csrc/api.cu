@@ -231,7 +231,8 @@ extern "C" int b2l_decode_step_launches(const b2l_decode_args* d) {
   if (d->plan != nullptr) return 1;   // the persistent kernel
   // fused single-token attention for head_size 128 (B2L_F_ATTN_UNFUSED: the three-kernel path)
   const bool fused = d->n_embd / d->n_head == 128 && !(d->flags & B2L_F_ATTN_UNFUSED);
-  const int attn = fused ? 1 : 3;
+  // B2L_F_STEPWISE: the fused kernel runs behind one launch that appends every token's key / value rows
+  const int attn = fused ? ((d->flags & B2L_F_STEPWISE) ? 2 : 1) : 3;
   // the batch kernels (int4 at 2..8 rows, gptq.int8, llm.int8 under B2L_F_Q8_BATCH and, under B2L_F_Q4_BATCH_I8,
   // int4 at 2..16) are two launches per linear
   const bool b16 = (d->flags & (B2L_F_W8_BATCH | B2L_F_Q4_BATCH_I8 | B2L_F_Q8_BATCH)) && d->B > 1 && d->B <= 16 && d->batch_work;
@@ -255,6 +256,20 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
                     d->hid && d->attn_work && d->logits,
                 "b2l_decode_step: null pointer");
   const bool row_pos = (d->flags & B2L_F_ROW_POS) != 0;   // input_pos / ring_start hold one entry per row
+  // B2L_F_STEPWISE: the B rows are consecutive tokens of ONE sequence (input_pos int64[B], batch-1 caches); every row
+  // must equal the batch-1 step at its position, so only the row-exact linears may run it
+  const bool stepwise = (d->flags & B2L_F_STEPWISE) != 0;
+  if (stepwise) {
+    B2L_CHECK_SUPPORTED(!row_pos, "b2l_decode_step: B2L_F_STEPWISE does not combine with B2L_F_ROW_POS");
+    B2L_CHECK_SUPPORTED(!(d->flags & B2L_F_Q8),
+                        "b2l_decode_step: B2L_F_STEPWISE does not run llm.int8 (B2L_F_Q8): its rows interact through the batch outlier mask");
+    B2L_CHECK_SUPPORTED((d->flags & B2L_F_Q4_BATCH_I8) || ((d->flags & B2L_F_W8) && (d->flags & B2L_F_W8_BATCH)),
+                        "b2l_decode_step: B2L_F_STEPWISE needs the row-exact linears (B2L_F_Q4_BATCH_I8, or B2L_F_W8 | B2L_F_W8_BATCH)");
+    B2L_CHECK_SUPPORTED(d->B >= 2 && d->B <= 16, "b2l_decode_step: B2L_F_STEPWISE runs 2..16 tokens, got B=%d", d->B);
+    B2L_CHECK_SUPPORTED(d->plan == nullptr, "b2l_decode_step: B2L_F_STEPWISE does not run in the persistent kernel (plan must be NULL)");
+    B2L_CHECK_SUPPORTED(d->affines == nullptr && d->lm_head_affine.scale == nullptr && d->lm_head_affine.bias == nullptr,
+                        "b2l_decode_step: B2L_F_STEPWISE does not apply LLaMA-Adapter v2 affines");
+  }
   B2L_CHECK_SUPPORTED(!row_pos || d->plan == nullptr,
                       "b2l_decode_step: B2L_F_ROW_POS does not run in the persistent kernel (plan must be NULL)");
   B2L_CHECK_SUPPORTED(!row_pos || !(d->flags & B2L_F_ROPE_ROWS), "b2l_decode_step: B2L_F_ROW_POS does not combine with B2L_F_ROPE_ROWS");
@@ -318,7 +333,7 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
   }
   if (d->plan != nullptr) return decode_step_persistent(d, stream);   // one persistent kernel per token (decode_mega.cu)
   const int C = d->n_embd, hs = C / d->n_head, B = d->B;
-  const int fl = d->flags & ~B2L_F_ROW_POS;   // the linears' flags (q4_call routes B2L_F_W8 to b2l_w8_gemv)
+  const int fl = d->flags & ~(B2L_F_ROW_POS | B2L_F_STEPWISE);   // the linears' flags (q4_call routes B2L_F_W8 to b2l_w8_gemv)
   const int afl = d->flags & ~(B2L_F_W8 | B2L_F_Q8 | B2L_F_W8_BATCH | B2L_F_Q4_BATCH_I8 | B2L_F_Q8_BATCH);   // the attention's
   int rc;
   // debug timeline: launch i of the step writes uint64[64] at timeline + 512*i (order: per Block c_attn,
@@ -335,8 +350,10 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
   int oi = 0;
   auto pf = [&]() -> const PfWindow* { const PfWindow* r = pfw.empty() ? nullptr : &pfw[oi]; ++oi; return r; };
   if ((rc = row_pos ? b2l_ring_advance_rows(d->input_pos, B, d->ring_start, d->S, stream)
-                    : b2l_ring_advance(d->input_pos, 1, d->ring_start, d->S, stream)))
+                    : b2l_ring_advance(d->input_pos, stepwise ? B : 1, d->ring_start, d->S, stream)))
     return rc;
+  // the attention's view: B sequences of one token, or (stepwise) one sequence of B tokens
+  const int aB = stepwise ? 1 : B, aT = stepwise ? B : 1;
   if ((rc = b2l_embedding(d->idx, d->idx_is_i64, d->wte, d->x, B, C, d->vocab, stream))) return rc;
   for (int l = 0; l < d->n_layer; ++l) {
     const b2l_layer& L = d->layers[l];
@@ -356,9 +373,9 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
     const b2l_adapter_prefix* pre = (d->adapters != nullptr && d->adapters[l].len != 0) ? &d->adapters[l] : nullptr;
     if ((rc = pre != nullptr
                   ? b2l_attention_adapter(d->qkv, L.k_cache, L.v_cache, d->rope, d->input_pos, d->ring_start, d->att,
-                                          d->attn_work, B, 1, d->n_head, hs, d->S, d->block_size, afl, pre, stream)
+                                          d->attn_work, aB, aT, d->n_head, hs, d->S, d->block_size, afl, pre, stream)
                   : b2l_attention(d->qkv, L.k_cache, L.v_cache, d->rope, d->input_pos, d->ring_start, d->att,
-                                  d->attn_work, B, 1, d->n_head, hs, d->S, d->block_size, afl, stream))) {
+                                  d->attn_work, aB, aT, d->n_head, hs, d->S, d->block_size, afl, stream))) {
       g_attn_timeline = nullptr;
       return rc;
     }

@@ -27,11 +27,13 @@ __global__ void ring_advance_rows_kernel(const int64_t* __restrict__ input_pos, 
 // grid (B*T, n_head), block hs/2 threads (one per rotated pair).
 // q is rotated in place inside qkv; k (rotated) and v go to the cache (or, without a
 // cache, k is rotated in place as well).  pos_stride 1 (B2L_F_ROW_POS, T == 1): row b reads input_pos[b] and
-// ring_start[b]; 0: every row reads the shared entries.
+// ring_start[b]; 0: every row reads the shared entries.  rotate_q 0 (B2L_F_STEPWISE on the fused path): qkv is left
+// untouched and only the cache rows are written, since the fused kernel rotates q and its own key from qkv itself.
 __global__ void rope_append_kernel(__nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ k_cache,
                                    __nv_bfloat16* __restrict__ v_cache, const float* __restrict__ rope,
                                    const int64_t* __restrict__ input_pos, const int32_t* __restrict__ ring_start,
-                                   int T, int n_head, int hs, int S, int block_size, int rope_rows, int pos_stride) {
+                                   int T, int n_head, int hs, int S, int block_size, int rope_rows, int pos_stride,
+                                   int rotate_q) {
   const int bt = blockIdx.x, h = blockIdx.y, b = bt / T, t = bt % T;
   const int C = n_head * hs;
   long long p = input_pos ? input_pos[b * pos_stride + t] : (long long)t;
@@ -54,8 +56,10 @@ __global__ void rope_append_kernel(__nv_bfloat16* __restrict__ qkv, __nv_bfloat1
     const float q0 = bf2f(q[2 * i]), q1 = bf2f(q[2 * i + 1]);
     const float k0 = bf2f(k[2 * i]), k1 = bf2f(k[2 * i + 1]);
     // model.py:315-318 (separate multiplies and add/sub in fp32, then type_as(x))
-    q[2 * i] = f2bf(__fsub_rn(__fmul_rn(q0, c), __fmul_rn(q1, s)));
-    q[2 * i + 1] = f2bf(__fadd_rn(__fmul_rn(q1, c), __fmul_rn(q0, s)));
+    if (rotate_q) {
+      q[2 * i] = f2bf(__fsub_rn(__fmul_rn(q0, c), __fmul_rn(q1, s)));
+      q[2 * i + 1] = f2bf(__fadd_rn(__fmul_rn(q1, c), __fmul_rn(q0, s)));
+    }
     kd[2 * i] = f2bf(__fsub_rn(__fmul_rn(k0, c), __fmul_rn(k1, s)));
     kd[2 * i + 1] = f2bf(__fadd_rn(__fmul_rn(k1, c), __fmul_rn(k0, s)));
     if (vd != nullptr) {
@@ -296,7 +300,11 @@ __device__ __forceinline__ __nv_bfloat16 adapter_combine(float y, float ay, floa
 // the writing CTA (DESIGN.md, LLaMA-Adapter, has the measurements of both placements).
 // ROWS (B2L_F_ROW_POS): row b reads its own input_pos[b] and ring_start[b]; a template parameter, so the shared-position
 // launch (batch 1 included) runs exactly the instructions it ran before per-row positions existed.
-template <bool ADAPTER, bool ROWS>
+// STEP (B2L_F_STEPWISE): "row" b is query b of ONE sequence at input_pos[b]; every query reads batch row 0 of the cache,
+// where a rope_append_kernel launch has already written all T new keys / values, so each query streams slots < its own
+// as old rows, scores its own key from registers as the T == 1 launch does, and stores nothing to the cache (a second
+// store of a slot would race the TMA reads of the later queries).
+template <bool ADAPTER, bool ROWS, bool STEP>
 __global__ void __launch_bounds__(FD_WARPS * 32, ADAPTER ? FD_CTAS_PER_SM : 0)
     attn_decode_fused_kernel(const __nv_bfloat16* qkv, __nv_bfloat16* __restrict__ k_cache,
                              __nv_bfloat16* __restrict__ v_cache, const float* __restrict__ rope,
@@ -323,13 +331,13 @@ __global__ void __launch_bounds__(FD_WARPS * 32, ADAPTER ? FD_CTAS_PER_SM : 0)
   stamp();
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int C = n_head * HS;
-  const size_t head_base = ((size_t)b * n_head + h) * S * HS;
+  const size_t head_base = ((size_t)(STEP ? 0 : b) * n_head + h) * S * HS;
 
   // input_pos and ring_start are inputs of the step (written by the host side long before), not
   // products of the previous kernel: they may be read before the dependency is resolved.  ROWS: row b is at its own
   // position input_pos[b] with its own ring offset ring_start[b], and everything below (write slot, key count, split
   // plan, ring wrap, merge) follows from that row's L.
-  const long long p = input_pos[ROWS ? b : 0];
+  const long long p = input_pos[(ROWS || STEP) ? b : 0];
   const int w_slot = (int)(p < S ? p : (long long)S - 1);  // logical slot of the new token
   const int L = w_slot + 1;                                 // valid logical slots 0..L-1
   // keys per CTA: a multiple of 64 in [64, 256], chosen (identically by every CTA) so that at most target_ctas CTAs
@@ -455,10 +463,12 @@ __global__ void __launch_bounds__(FD_WARPS * 32, ADAPTER ? FD_CTAS_PER_SM : 0)
       out[i] = (__float_as_uint(kf[2 * i]) >> 16) | (__float_as_uint(kf[2 * i + 1]) & 0xffff0000u);
     }
     const uint4 va = ld_coherent_u4(qrow + 2 * C), vb = ld_coherent_u4(qrow + 2 * C + 8);
-    uint4* kd = reinterpret_cast<uint4*>(k_cache + head_base + (size_t)phys * HS + d0);
-    uint4* vd = reinterpret_cast<uint4*>(v_cache + head_base + (size_t)phys * HS + d0);
-    kd[0] = make_uint4(out[0], out[1], out[2], out[3]); kd[1] = make_uint4(out[4], out[5], out[6], out[7]);
-    vd[0] = va; vd[1] = vb;
+    if constexpr (!STEP) {
+      uint4* kd = reinterpret_cast<uint4*>(k_cache + head_base + (size_t)phys * HS + d0);
+      uint4* vd = reinterpret_cast<uint4*>(v_cache + head_base + (size_t)phys * HS + d0);
+      kd[0] = make_uint4(out[0], out[1], out[2], out[3]); kd[1] = make_uint4(out[4], out[5], out[6], out[7]);
+      vd[0] = va; vd[1] = vb;
+    }
     bf16x8_to_f32(va, vf); bf16x8_to_f32(vb, vf + 8);
     float sc = 0.f;
 #pragma unroll
@@ -896,11 +906,13 @@ static inline void split_plan(int T, int S, int* n_split, int* chunk) {
   *n_split = (S + 63) / 64;
 }
 
+// stepwise (B2L_F_STEPWISE): each of the T queries takes the T == 1 split plan, so it merges its keys in the order a
+// T == 1 launch at its position does
 static int launch_attn(const __nv_bfloat16* qkv, KvView kv, const int64_t* input_pos, const int32_t* ring_start,
                        float* work, __nv_bfloat16* y, int B, int T, int n_head, int hs, int cap, int pos_stride,
-                       cudaStream_t st) {
+                       bool stepwise, cudaStream_t st) {
   static const int env_pf = [] { const char* e = getenv("B2L_ATTN_PREFILL"); return e ? atoi(e) : 1; }();
-  if (hs == 128 && T > 1 && env_pf) {   // tiled tensor-core kernel (B2L_ATTN_PREFILL=0: the per-query path below)
+  if (hs == 128 && T > 1 && env_pf && !stepwise) {   // tiled tensor-core kernel (B2L_ATTN_PREFILL=0: the per-query path below)
     static DynSmemCache smem_cache;
     if (int rc = ensure_dyn_smem(attn_prefill_kernel, PF_SMEM_BYTES, smem_cache)) return rc;
     attn_prefill_kernel<<<dim3(B * n_head, (T + PF_Q - 1) / PF_Q), 128, PF_SMEM_BYTES, st>>>(qkv, kv, input_pos, ring_start, y, T, n_head);
@@ -908,7 +920,7 @@ static int launch_attn(const __nv_bfloat16* qkv, KvView kv, const int64_t* input
     return 0;
   }
   int n_split, chunk;
-  split_plan(T, cap, &n_split, &chunk);
+  split_plan(stepwise ? 1 : T, cap, &n_split, &chunk);
   dim3 grid(B * n_head, T, n_split), block(ATT_WARPS * 32);
   if (hs == 128)
     attn_partial_kernel<4><<<grid, block, 0, st>>>(qkv, kv, input_pos, ring_start, work, T, n_head, hs, n_split, chunk,
@@ -984,23 +996,45 @@ static int check_row_pos(int flags, int T, const char* who) {
   return 0;
 }
 
+// B2L_F_STEPWISE: T = 2..16 consecutive tokens of ONE sequence (B == 1), input_pos int64[T] from the RoPE table
+static int check_stepwise(int flags, int B, int T, const char* who) {
+  if (!(flags & B2L_F_STEPWISE)) return 0;
+  B2L_CHECK_SUPPORTED(!(flags & B2L_F_ROW_POS), "%s: B2L_F_STEPWISE does not combine with B2L_F_ROW_POS", who);
+  B2L_CHECK_SUPPORTED(!(flags & B2L_F_ROPE_ROWS), "%s: B2L_F_STEPWISE does not combine with B2L_F_ROPE_ROWS", who);
+  B2L_CHECK_SUPPORTED(B == 1, "%s: B2L_F_STEPWISE runs the tokens of one sequence (B == 1), got B=%d", who, B);
+  B2L_CHECK_SUPPORTED(T >= 2 && T <= 16, "%s: B2L_F_STEPWISE runs 2..16 tokens, got T=%d", who, T);
+  return 0;
+}
+
 // b2l_attention and b2l_attention_adapter (pre != nullptr: already checked)
 static int attention_impl(void* qkv, void* k_cache, void* v_cache, const void* rope, const int64_t* input_pos,
                           const int32_t* ring_start, void* y, void* work, int B, int T, int n_head, int head_size,
                           int S, int block_size, int flags, const b2l_adapter_prefix* pre, cudaStream_t st) {
   const int pos_stride = (flags & B2L_F_ROW_POS) ? 1 : 0;
-  if (T == 1 && head_size == 128 && !(flags & B2L_F_ROPE_ROWS) && !(flags & B2L_F_ATTN_UNFUSED)) {
+  const bool step = (flags & B2L_F_STEPWISE) != 0;
+  if ((T == 1 || step) && head_size == 128 && !(flags & B2L_F_ROPE_ROWS) && !(flags & B2L_F_ATTN_UNFUSED)) {
     const int n_split = (S + FD_SUB - 1) / FD_SUB;
-    int* tickets = reinterpret_cast<int*>(reinterpret_cast<char*>(work) + ws_partials_bytes(B, n_head, head_size, T, S));
+    // stepwise: the T queries are laid out as T rows of a T == 1 launch (partials and tickets of
+    // b2l_attn_workspace_bytes(T, n_head, 128, 1, S))
+    const int rows = step ? T : B;
+    int* tickets = reinterpret_cast<int*>(reinterpret_cast<char*>(work) + ws_partials_bytes(rows, n_head, head_size, step ? 1 : T, S));
+    if (step) {   // every new key / value row first, qkv untouched (the fused kernel rotates q and its own key itself)
+      rope_append_kernel<<<dim3(T, n_head), 64, 0, st>>>((__nv_bfloat16*)qkv, (__nv_bfloat16*)k_cache, (__nv_bfloat16*)v_cache,
+                                                        (const float*)rope, input_pos, ring_start, T, n_head, head_size, S,
+                                                        block_size, 0, 0, 0);
+      B2L_LAUNCH_CHECK("rope_append_kernel");
+    }
     // B2L_ATTN_PRE (read once): sub-tiles requested before griddepcontrol.wait, 1 (default) or 2
     static const int env_pre = [] { const char* e = getenv("B2L_ATTN_PRE"); return e ? atoi(e) : 1; }();
     // B2L_ATTN_SMEM_MERGE (read once): 1 = all 32 key groups merge through shared memory, 0 = shuffles inside a warp first
     // (default 0: the extra block barrier of 1 is not free)
     static const int env_smem_merge = [] { const char* e = getenv("B2L_ATTN_SMEM_MERGE"); return e ? atoi(e) : 0; }();
-    LaunchCfg lc(dim3(B * n_head, n_split), dim3(FD_WARPS * 32), FD_SMEM_BYTES, st, (flags & B2L_F_PDL) != 0);
-    static DynSmemCache smem_cache[2][2];   // [ADAPTER][ROWS]: the four instantiations share one function type
+    // stepwise: no programmatic dependent launch, because the kernel requests old cache rows before
+    // griddepcontrol.wait and the append launch in front of it writes some of them
+    LaunchCfg lc(dim3(rows * n_head, n_split), dim3(FD_WARPS * 32), FD_SMEM_BYTES, st, (flags & B2L_F_PDL) != 0 && !step);
+    static DynSmemCache smem_cache[2][3];   // [ADAPTER][shared position, ROWS, STEP]: the six instantiations share one function type
     auto launch = [&](auto kernel, const b2l_adapter_prefix* pf) -> int {
-      if (int rc = ensure_dyn_smem(kernel, FD_SMEM_BYTES, smem_cache[pf != nullptr][pos_stride])) return rc;
+      if (int rc = ensure_dyn_smem(kernel, FD_SMEM_BYTES, smem_cache[pf != nullptr][step ? 2 : pos_stride])) return rc;
       B2L_CUDA(cudaLaunchKernelEx(&lc.cfg, kernel, (const __nv_bfloat16*)qkv, (__nv_bfloat16*)k_cache,
                                   (__nv_bfloat16*)v_cache, (const float*)rope, input_pos, ring_start, (__nv_bfloat16*)y,
                                   (float*)work, tickets, n_head, S, block_size, n_split, (unsigned long long*)g_attn_timeline, env_pre, env_smem_merge,
@@ -1009,20 +1043,25 @@ static int attention_impl(void* qkv, void* k_cache, void* v_cache, const void* r
                                   pf ? pf->len : 0));
       return 0;
     };
+    if (step)
+      return pre == nullptr ? launch(attn_decode_fused_kernel<false, false, true>, nullptr)
+                            : launch(attn_decode_fused_kernel<true, false, true>, pre);
     if (pre == nullptr)
-      return pos_stride ? launch(attn_decode_fused_kernel<false, true>, nullptr) : launch(attn_decode_fused_kernel<false, false>, nullptr);
-    return pos_stride ? launch(attn_decode_fused_kernel<true, true>, pre) : launch(attn_decode_fused_kernel<true, false>, pre);
+      return pos_stride ? launch(attn_decode_fused_kernel<false, true, false>, nullptr)
+                        : launch(attn_decode_fused_kernel<false, false, false>, nullptr);
+    return pos_stride ? launch(attn_decode_fused_kernel<true, true, false>, pre)
+                      : launch(attn_decode_fused_kernel<true, false, false>, pre);
   }
   int rt = head_size / 2 < 32 ? 32 : head_size / 2;
   rope_append_kernel<<<dim3(B * T, n_head), rt, 0, st>>>((__nv_bfloat16*)qkv, (__nv_bfloat16*)k_cache,
                                                         (__nv_bfloat16*)v_cache, (const float*)rope, input_pos,
                                                         ring_start, T, n_head, head_size, S, block_size, (flags & B2L_F_ROPE_ROWS) ? 1 : 0,
-                                                        pos_stride);
+                                                        pos_stride, 1);
   B2L_LAUNCH_CHECK("rope_append_kernel");
   KvView kv{(const __nv_bfloat16*)k_cache, (const __nv_bfloat16*)v_cache, (size_t)n_head * S * head_size,
             (size_t)S * head_size, (size_t)head_size, S};
   if (int rc = launch_attn((const __nv_bfloat16*)qkv, kv, input_pos, ring_start, (float*)work, (__nv_bfloat16*)y, B, T,
-                           n_head, head_size, S, pos_stride, st))
+                           n_head, head_size, S, pos_stride, step, st))
     return rc;
   return pre == nullptr ? 0 : launch_adapter_prefix(qkv, pre, y, B, T, n_head, head_size, st);
 }
@@ -1035,6 +1074,7 @@ extern "C" int b2l_attention(void* qkv, void* k_cache, void* v_cache, const void
   B2L_CHECK_ARG(B > 0 && T > 0 && n_head > 0 && S > 0 && T <= S && block_size > 0, "b2l_attention: bad shape");
   B2L_CHECK_SUPPORTED(head_size % 2 == 0 && head_size >= 2 && head_size <= 32 * ATT_MAX_EPL,
                       "b2l_attention: head_size %d unsupported (even, <= %d)", head_size, 32 * ATT_MAX_EPL);
+  if (int rc = check_stepwise(flags, B, T, "b2l_attention")) return rc;
   if (int rc = check_row_pos(flags, T, "b2l_attention")) return rc;
   return attention_impl(qkv, k_cache, v_cache, rope, input_pos, ring_start, y, work, B, T, n_head, head_size, S,
                         block_size, flags, nullptr, (cudaStream_t)stream);
@@ -1049,6 +1089,7 @@ extern "C" int b2l_attention_adapter(void* qkv, void* k_cache, void* v_cache, co
   B2L_CHECK_ARG(B > 0 && T > 0 && n_head > 0 && S > 0 && T <= S && block_size > 0, "b2l_attention_adapter: bad shape");
   B2L_CHECK_SUPPORTED(head_size % 2 == 0 && head_size >= 2 && head_size <= 32 * ATT_MAX_EPL,
                       "b2l_attention_adapter: head_size %d unsupported (even, <= %d)", head_size, 32 * ATT_MAX_EPL);
+  if (int rc = check_stepwise(flags, B, T, "b2l_attention_adapter")) return rc;
   if (int rc = check_row_pos(flags, T, "b2l_attention_adapter")) return rc;
   if (int rc = check_adapter_prefix(prefix, "b2l_attention_adapter")) return rc;
   return attention_impl(qkv, k_cache, v_cache, rope, input_pos, ring_start, y, work, B, T, n_head, head_size, S,
@@ -1059,12 +1100,12 @@ static int attention_nocache_impl(void* qkv, const void* rope, void* y, void* wo
                                   int head_size, int block_size, cudaStream_t st) {
   int rt = head_size / 2 < 32 ? 32 : head_size / 2;
   rope_append_kernel<<<dim3(B * T, n_head), rt, 0, st>>>((__nv_bfloat16*)qkv, nullptr, nullptr, (const float*)rope,
-                                                        nullptr, nullptr, T, n_head, head_size, 0, block_size, 0, 0);
+                                                        nullptr, nullptr, T, n_head, head_size, 0, block_size, 0, 0, 1);
   B2L_LAUNCH_CHECK("rope_append_kernel");
   const int C = n_head * head_size;
   const __nv_bfloat16* base = (const __nv_bfloat16*)qkv;
   KvView kv{base + C, base + 2 * C, (size_t)T * 3 * C, (size_t)head_size, (size_t)3 * C, 0};
-  return launch_attn(base, kv, nullptr, nullptr, (float*)work, (__nv_bfloat16*)y, B, T, n_head, head_size, T, 0, st);
+  return launch_attn(base, kv, nullptr, nullptr, (float*)work, (__nv_bfloat16*)y, B, T, n_head, head_size, T, 0, false, st);
 }
 
 extern "C" int b2l_attention_nocache(void* qkv, const void* rope, void* y, void* work, int B, int T, int n_head,

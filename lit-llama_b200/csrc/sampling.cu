@@ -80,18 +80,12 @@ __device__ __forceinline__ uint4 load8(const __nv_bfloat16* p, int i, bool vec) 
                     s[6] | ((uint32_t)s[7] << 16));
 }
 
-__global__ void __launch_bounds__(SAMP_THREADS)
-    topk_softmax_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, float inv_temperature, int top_k,
-                        __nv_bfloat16* __restrict__ probs, const __nv_bfloat16* __restrict__ noise,
-                        long long* __restrict__ token, int V) {
-  extern __shared__ __align__(16) uint8_t ssm[];
-  {  // this CTA's row
-    const size_t row = blockIdx.x;
-    logits += row * (size_t)ld;
-    if (noise != nullptr) noise += row * (size_t)V;
-    if (probs != nullptr) probs += row * (size_t)V;
-    if (token != nullptr) token += row;
-  }
+// One row of the sampling tail, by every thread of a SAMP_THREADS CTA; ssm: dynamic shared memory of launch_topk's size.
+// probs may be the scaled-logit buffer itself (ssm, as b2l_spec_accept uses it): every 16-byte vector of it is read and
+// then written by the same thread.
+__device__ __forceinline__ void topk_softmax_row(const __nv_bfloat16* __restrict__ logits, float inv_temperature, int top_k,
+                                                 __nv_bfloat16* probs, const __nv_bfloat16* __restrict__ noise,
+                                                 long long* __restrict__ token, int V, uint8_t* ssm) {
   const bool vec = ((reinterpret_cast<uintptr_t>(logits) | reinterpret_cast<uintptr_t>(noise)) & 15) == 0;
   const int Vp = (V + 7) & ~7;
   uint16_t* sv = reinterpret_cast<uint16_t*>(ssm);  // scaled logits as bf16 bits [Vp]
@@ -308,6 +302,94 @@ __global__ void __launch_bounds__(SAMP_THREADS)
   }
 }
 
+__global__ void __launch_bounds__(SAMP_THREADS)
+    topk_softmax_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, float inv_temperature, int top_k,
+                        __nv_bfloat16* __restrict__ probs, const __nv_bfloat16* __restrict__ noise,
+                        long long* __restrict__ token, int V) {
+  extern __shared__ __align__(16) uint8_t ssm[];
+  {  // this CTA's row
+    const size_t row = blockIdx.x;
+    logits += row * (size_t)ld;
+    if (noise != nullptr) noise += row * (size_t)V;
+    if (probs != nullptr) probs += row * (size_t)V;
+    if (token != nullptr) token += row;
+  }
+  topk_softmax_row(logits, inv_temperature, top_k, probs, noise, token, V, ssm);
+}
+
+// bf16 bits of the draw's key bf16(a / n) for a >= 0 (see draw_beats)
+__device__ __forceinline__ uint32_t draw_key(float a, float n) { return __float_as_uint(rbf(a / n)); }
+
+// The block-wide argmax of draw_key(w(i), noise[i]) over i < V, ties to the lower index (every thread gets it).
+template <class W>
+__device__ __forceinline__ int block_draw(W w, const __nv_bfloat16* __restrict__ noise, int V, uint32_t* red_b, int* red_i) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  uint32_t best = 0;
+  int best_i = 0x7fffffff;
+  for (int i = threadIdx.x; i < V; i += SAMP_THREADS) {
+    const uint32_t r = draw_key(w(i), bf2f(noise[i]));
+    if (draw_beats(r, i, best, best_i)) { best = r; best_i = i; }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const uint32_t ob = __shfl_xor_sync(0xffffffffu, best, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, best_i, o);
+    if (draw_beats(ob, oi, best, best_i)) { best = ob; best_i = oi; }
+  }
+  __syncthreads();
+  if (lane == 0) { red_b[warp] = best; red_i[warp] = best_i; }
+  __syncthreads();
+  best = red_b[lane]; best_i = red_i[lane];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const uint32_t ob = __shfl_xor_sync(0xffffffffu, best, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, best_i, o);
+    if (draw_beats(ob, oi, best, best_i)) { best = ob; best_i = oi; }
+  }
+  return best_i;
+}
+
+// b2l_spec_accept: ONE CTA walks the T = k + 1 target rows in order.  Row t's probabilities p_t are computed by
+// topk_softmax_row into shared memory (the bits b2l_topk_softmax_rows writes); the draft token of row t < k is then
+// accepted or the residual is drawn and the kernel ends.  A rejection at row j never computes the rows after it.
+__global__ void __launch_bounds__(SAMP_THREADS)
+    spec_accept_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, float inv_temperature, int top_k,
+                       const __nv_bfloat16* __restrict__ draft_probs, const long long* __restrict__ draft_tokens,
+                       const float* __restrict__ u, const __nv_bfloat16* __restrict__ noise, int* __restrict__ n_accepted,
+                       long long* __restrict__ token, int T, int V) {
+  extern __shared__ __align__(16) uint8_t ssm[];
+  __shared__ uint32_t red_b[32];
+  __shared__ int red_i[32];
+  const uint16_t* p = reinterpret_cast<const uint16_t*>(ssm);   // p_t as bf16 bits, after topk_softmax_row
+  const int k = T - 1;
+  for (int t = 0; t < T; ++t) {
+    __syncthreads();   // every thread is done with the previous row's p
+    topk_softmax_row(logits + (size_t)t * ld, inv_temperature, top_k, reinterpret_cast<__nv_bfloat16*>(ssm), nullptr, nullptr,
+                     V, ssm);
+    __syncthreads();
+    if (t == k) {   // every draft token accepted: draw from the last row
+      const int tok = block_draw([&](int i) { return bits_f(p[i]); }, noise, V, red_b, red_i);
+      if (threadIdx.x == 0) { *n_accepted = k; *token = tok; }
+      return;
+    }
+    const long long x = draft_tokens[t];
+    const __nv_bfloat16* q = draft_probs + (size_t)t * V;
+    const bool in = x >= 0 && x < V;
+    if (in && u[t] * bf2f(q[x]) < bits_f(p[in ? x : 0])) continue;   // accepted (block-uniform)
+    // rejected: draw from max(0, p - q); when that is zero everywhere (bf16 rounding), from p
+    auto resid = [&](int i) { return fmaxf(bits_f(p[i]) - bf2f(q[i]), 0.f); };
+    int any = 0;
+    for (int i = threadIdx.x; i < V; i += SAMP_THREADS) any |= resid(i) > 0.f;
+    int tok;
+    if (__syncthreads_or(any))
+      tok = block_draw(resid, noise, V, red_b, red_i);
+    else
+      tok = block_draw([&](int i) { return bits_f(p[i]); }, noise, V, red_b, red_i);
+    if (threadIdx.x == 0) { *n_accepted = t; *token = tok; }
+    return;
+  }
+}
+
 }  // namespace b2l
 
 using namespace b2l;
@@ -358,6 +440,33 @@ extern "C" int b2l_topk_softmax_rows(const void* logits, int64_t ld, float tempe
   if (int rc = check_rows(logits, B, V, temperature, top_k, who)) return rc;
   B2L_CHECK_ARG(probs != nullptr, "%s: null probs", who);
   return launch_topk(logits, ld, temperature, top_k, probs, nullptr, nullptr, B, V, stream, who);
+}
+
+extern "C" int b2l_spec_accept(const void* target_logits, int64_t ld, float temperature, int top_k, const void* draft_probs,
+                               const int64_t* draft_tokens, const float* u, const void* noise, int32_t* n_accepted,
+                               int64_t* token, int T, int V, b2l_stream_t stream) {
+  const char* who = "b2l_spec_accept";
+  if (int rc = check_rows(target_logits, T, V, temperature, top_k, who)) return rc;
+  B2L_CHECK_SUPPORTED(T >= 2 && T <= 16, "%s: T = %d target rows; 2..16 (k = T - 1 = 1..15 draft tokens)", who, T);
+  B2L_CHECK_ARG(ld >= V, "%s: ld = %lld, at least V = %d", who, (long long)ld, V);
+  B2L_CHECK_ARG(draft_probs != nullptr, "%s: null draft_probs", who);
+  B2L_CHECK_ARG(draft_tokens != nullptr, "%s: null draft_tokens", who);
+  B2L_CHECK_ARG(u != nullptr, "%s: null u", who);
+  B2L_CHECK_ARG(noise != nullptr, "%s: null noise", who);
+  B2L_CHECK_ARG(n_accepted != nullptr && token != nullptr, "%s: null n_accepted / token", who);
+  B2L_CHECK_ARG(((uintptr_t)target_logits % 16) == 0, "%s: target_logits must be 16-byte aligned", who);
+  B2L_CHECK_ARG(((uintptr_t)draft_probs % 16) == 0 && ((uintptr_t)noise % 16) == 0,
+                "%s: draft_probs and noise must be 16-byte aligned", who);
+  const size_t smem = (((size_t)V + 7) & ~(size_t)7) * 2;   // p as bf16 (topk_softmax_row without noise)
+  B2L_CHECK_SUPPORTED(smem <= 200 * 1024, "%s: vocabulary %d too large for one CTA", who, V);
+  static DynSmemCache smem_cache;
+  if (smem > 48 * 1024)
+    if (int rc = ensure_dyn_smem(spec_accept_kernel, smem, smem_cache)) return rc;
+  spec_accept_kernel<<<1, SAMP_THREADS, smem, (cudaStream_t)stream>>>(
+      (const __nv_bfloat16*)target_logits, (long long)ld, 1.0f / temperature, top_k, (const __nv_bfloat16*)draft_probs,
+      (const long long*)draft_tokens, u, (const __nv_bfloat16*)noise, n_accepted, (long long*)token, T, V);
+  B2L_LAUNCH_CHECK("spec_accept_kernel");
+  return 0;
 }
 
 extern "C" int b2l_topk_softmax_sample_rows(const void* logits, int64_t ld, float temperature, int top_k, const void* noise,

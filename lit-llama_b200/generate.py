@@ -6,8 +6,10 @@ CUDA-graph replay per token.  `generate_batch()` draws up to 16 samples of one p
 at once: one batch-1 prefill, then one batched decode step and one sampling launch per
 token for all samples.  `generate_prompts()` continues up to 16 different prompts at
 once: one batch-1 prefill per prompt into its row of the cache, then one batched decode
-step at per-row positions and one sampling launch per token.  `main()` mirrors the
-reference CLI with argparse
+step at per-row positions and one sampling launch per token.  `generate_speculative()`
+lets a small draft model propose up to 15 tokens that the model verifies in one
+step (speculative sampling); its greedy output is `generate()`'s token for token.
+`main()` mirrors the reference CLI with argparse
 (jsonargparse and lightning are not dependencies of this path)."""
 import os
 import sys
@@ -212,6 +214,140 @@ def generate_batch(
     return [out[b, :n] for b, n in enumerate(end.tolist())]
 
 
+#: most draft tokens one generate_speculative() round proposes: the verify step runs 2..16 tokens
+MAX_DRAFT = 15
+
+
+@torch.no_grad()
+def generate_speculative(
+    model: LLaMA,
+    draft: LLaMA,
+    idx: torch.Tensor,
+    max_new_tokens: int,
+    *,
+    num_draft: int = 4,
+    max_seq_length: Optional[int] = None,
+    temperature: float = 1.0,
+    top_k: Optional[int] = None,
+    eos_id: Optional[int] = None,
+    stats: Optional[dict] = None,
+) -> torch.Tensor:
+    """Speculative sampling: `idx` (T,) prompt -> (T + max_new_tokens,) tokens like `generate()`, with `draft` (a
+    smaller model over the same vocabulary) proposing tokens that `model` verifies several at a time.
+
+    Both models prefill the prompt at batch 1 and the first token is drawn from `model`'s prefill logits as in
+    `generate()`.  Each round then runs k = num_draft (1..15) batch-1 draft steps, each sampling its token with the
+    fused kernel and keeping its probability row q; one `LLaMA.decode_tokens` of `model` over the pending token and
+    the k draft tokens; and one `b2l_spec_accept` launch, which accepts draft token t while u_t q_t(x_t) < p_t(x_t)
+    and draws the next token from the residual max(0, p_j - q_j) at the first rejection j (from p_k when all are
+    accepted), so every emitted token is distributed as `model`'s own samples.  The round's only host
+    synchronisation is one 4-byte read of the number accepted.  When all k are accepted the draft also consumes the
+    last of them.  Rejected cache slots of either model are left stale: they are never read and are overwritten later.
+
+    With top_k=1 a token is accepted exactly when it is the target's argmax, and `decode_tokens` rows are bit-identical
+    to the batch-1 step, so the output equals `generate(model, ..., top_k=1)` token for token whatever the draft is.
+
+    k shrinks so that the verified positions stay below max_seq_length and no round overshoots max_new_tokens; from
+    the point where no draft token fits (the roll branch included) the tail runs `generate()`'s plain target steps.
+    With `eos_id` the output ends at the first eos, which is included.  `stats`, when given, receives "rounds",
+    "proposed" / "accepted" (lists: draft tokens per round), "num_draft" and "tail_steps".  Call `reset_cache()` on both
+    models before the next prompt, as after `generate()`."""
+    if not 1 <= int(num_draft) <= MAX_DRAFT:
+        raise ValueError(f"generate_speculative: num_draft = {num_draft}; 1..{MAX_DRAFT} (the verify step runs 2..16 tokens)")
+    if draft.config.padded_vocab_size != model.config.padded_vocab_size:
+        raise ValueError(f"generate_speculative: the draft's padded_vocab_size {draft.config.padded_vocab_size} differs from "
+                         f"the target's {model.config.padded_vocab_size}")
+    if idx.dim() != 1:
+        raise ValueError(f"generate_speculative: idx must be one prompt of shape (T,), got {tuple(idx.shape)}")
+    why = model._decode_tokens_refusal()
+    if why is not None:
+        raise RuntimeError(f"generate_speculative: the target's verify step (LLaMA.decode_tokens) {why}")
+    if not idx.is_cuda:
+        raise RuntimeError(f"generate_speculative: idx is on {idx.device}; lit_llama_b200 runs on CUDA only (no CPU fallback)")
+    T = idx.size(0)
+    T_new = T + max_new_tokens
+    if max_seq_length is None:
+        max_seq_length = min(T_new, model.config.block_size)
+    S = max_seq_length
+    device, dtype = idx.device, idx.dtype
+    V = model.config.padded_vocab_size
+    lib = L.lib()
+    kmax = int(num_draft)
+    k_top = 0 if top_k is None else min(int(top_k), V)
+    out = torch.empty(T_new, dtype=dtype, device=device)
+    out[:T] = idx
+    st = {} if stats is None else stats
+    st.update(rounds=0, proposed=[], accepted=[], num_draft=kmax, tail_steps=0)
+    if max_new_tokens <= 0:
+        return out
+
+    pos_all = torch.arange(0, max(T_new, S), device=device)
+    logits = model(idx.view(1, -1), S, pos_all[:T])
+    draft(idx.view(1, -1), S, pos_all[:T])
+    # tokens stay int64 on the device (one step state per model: its idx dtype never changes)
+    tok = sample_token(logits[0, -1], temperature, top_k)   # generate()'s first token
+    out[T] = tok[0]
+    n = 1                                  # tokens emitted; the last one (tok) is in neither cache yet
+    if eos_id is not None and int(tok[0]) == eos_id:
+        return out[:T + 1]
+
+    q = torch.empty((kmax, V), dtype=torch.bfloat16, device=device)   # the draft's probability rows
+    dtok = torch.empty((kmax + 1, 1), dtype=torch.int64, device=device)   # d_1..d_k, then the target's next token
+    nacc = torch.zeros(1, dtype=torch.int32, device=device)
+    steps = torch.arange(kmax + 1, device=device)
+    while n < max_new_tokens:
+        p = T + n - 1                       # position of the pending token
+        k = min(kmax, S - 1 - p, max_new_tokens - n - 1)
+        if k < 1:
+            break
+        x = tok.view(1, 1)
+        for i in range(k):                  # k batch-1 draft steps: tok, d_1 .. d_{k-1}
+            dl = draft(x, S, pos_all[p + i:p + i + 1])[0, -1].contiguous()
+            noise = torch.empty_like(dl).exponential_(1)
+            L.check(lib.b2l_topk_softmax_sample(dl.data_ptr(), float(temperature), k_top, noise.data_ptr(), q[i].data_ptr(),
+                                                dtok[i].data_ptr(), V, L.stream_ptr()), "b2l_topk_softmax_sample")
+            x = dtok[i].view(1, 1)
+        vidx = torch.cat((tok.view(1, 1), dtok[:k].view(1, k)), dim=1)
+        tl = model.decode_tokens(vidx, S, pos_all[p:p + k + 1])
+        u = torch.rand(k, device=device)
+        noise = torch.empty(V, dtype=torch.bfloat16, device=device).exponential_(1)
+        L.check(lib.b2l_spec_accept(tl.data_ptr(), V, float(temperature), k_top, q.data_ptr(), dtok.data_ptr(), u.data_ptr(),
+                                    noise.data_ptr(), nacc.data_ptr(), dtok[k].data_ptr(), k + 1, V, L.stream_ptr()),
+                "b2l_spec_accept")
+        # the round's tokens: d_1..d_a, then the target's token (at slot a); later slots are overwritten by later rounds
+        em = torch.where(steps[:k + 1] < nacc.long(), dtok[:k + 1, 0], dtok[k, 0]).to(dtype)
+        out[T + n:T + n + k + 1] = em
+        if eos_id is None:
+            a = int(nacc.item())            # the round's one host synchronisation
+        else:                               # the first eos among the emitted tokens travels in the same 4-byte word
+            hit = (em == eos_id) & (steps[:k + 1] <= nacc.long())
+            first = torch.where(hit, steps[:k + 1], 255).min()
+            a_e = int((nacc.long()[0] | (first << 8)).to(torch.int32).item())
+            a, e = a_e & 255, a_e >> 8
+        st["rounds"] += 1
+        st["proposed"].append(k)
+        st["accepted"].append(a)
+        if eos_id is not None and e != 255:
+            return out[:T + n + e + 1]
+        if a == k:                          # every draft token accepted: the draft also consumes d_k
+            draft(dtok[k - 1].view(1, 1), S, pos_all[p + k:p + k + 1])
+        tok = dtok[k].clone()
+        n += a + 1
+
+    # the tail: generate()'s plain target steps (no draft token fits below max_seq_length, or one token is left)
+    input_pos = pos_all[T + n - 1:T + n]
+    while n < max_new_tokens:
+        logits = model(tok.view(1, 1), S, input_pos)
+        tok = sample_token(logits[0, -1], temperature, top_k)
+        st["tail_steps"] += 1
+        input_pos = input_pos + 1
+        out[T + n] = tok[0]
+        n += 1
+        if eos_id is not None and tok == eos_id:
+            return out[:T + n]
+    return out
+
+
 @torch.no_grad()
 def generate_prompts(
     model: LLaMA,
@@ -292,11 +428,15 @@ def main(
     quantize: Optional[str] = None,
     batch_size: int = 1,
     prompts_file: Optional[Path] = None,
+    draft_checkpoint_path: Optional[Path] = None,
+    draft_quantize: Optional[str] = None,
+    num_draft: int = 4,
 ) -> None:
     """generate.py:94-155 without Fabric: bf16 on cuda:0, same prints on stderr.  `batch_size` > 1 draws the samples
     in groups of up to `batch_size` (at most 16) through `generate_batch`, on the model's exact batched decode step.
     `prompts_file` (one prompt per line) replaces `prompt`: the prompts are decoded in groups of `batch_size` through
-    `generate_prompts`, `num_samples` times each."""
+    `generate_prompts`, `num_samples` times each.  `draft_checkpoint_path` (with `draft_quantize`) loads a draft model
+    and decodes each sample with `generate_speculative`, `num_draft` draft tokens per round."""
     if not 1 <= batch_size <= MAX_SAMPLES:
         raise ValueError(f"batch_size = {batch_size}; 1..{MAX_SAMPLES}")
     from sentencepiece import SentencePieceProcessor
@@ -306,25 +446,33 @@ def main(
     assert tokenizer_path.is_file(), tokenizer_path
     device = torch.device("cuda", 0)
 
-    print("Loading model ...", file=sys.stderr)
-    t0 = time.time()
-    checkpoint = torch.load(checkpoint_path, map_location="cpu", weights_only=True, mmap=True)
-    name = llama_model_lookup(checkpoint)
-    prev = torch.get_default_dtype()
-    torch.set_default_dtype(torch.bfloat16)  # what Fabric's bf16-true does inside init_module
-    try:
-        with torch.device(device), quantization(mode=quantize):
-            model = LLaMA.from_name(name)
-    finally:
-        torch.set_default_dtype(prev)
-    model.load_state_dict(checkpoint)
-    print(f"Time to load model: {time.time() - t0:.02f} seconds.", file=sys.stderr)
-    model.eval()
-    if quantize in ("gptq.int4", "gptq.int8") and os.environ.get("B2L_COMPACT", "1") != "0":
+    def load(path: Path, mode: Optional[str]) -> LLaMA:
+        print("Loading model ...", file=sys.stderr)
+        t0 = time.time()
+        checkpoint = torch.load(path, map_location="cpu", weights_only=True, mmap=True)
+        name = llama_model_lookup(checkpoint)
+        prev = torch.get_default_dtype()
+        torch.set_default_dtype(torch.bfloat16)  # what Fabric's bf16-true does inside init_module
         try:
-            model.compact()   # one resident copy of the weights (the reference-layout buffers come back on state_dict())
-        except RuntimeError:  # a layer the fused decode step cannot run (grouped scales, odd widths): keep everything
-            pass
+            with torch.device(device), quantization(mode=mode):
+                m = LLaMA.from_name(name)
+        finally:
+            torch.set_default_dtype(prev)
+        m.load_state_dict(checkpoint)
+        print(f"Time to load model: {time.time() - t0:.02f} seconds.", file=sys.stderr)
+        m.eval()
+        if mode in ("gptq.int4", "gptq.int8") and os.environ.get("B2L_COMPACT", "1") != "0":
+            try:
+                m.compact()   # one resident copy of the weights (the reference-layout buffers come back on state_dict())
+            except RuntimeError:  # a layer the fused decode step cannot run (grouped scales, odd widths): keep everything
+                pass
+        return m
+
+    model = load(checkpoint_path, quantize)
+    draft = None
+    if draft_checkpoint_path is not None:
+        assert Path(draft_checkpoint_path).is_file(), draft_checkpoint_path
+        draft = load(Path(draft_checkpoint_path), draft_quantize)
 
     sp = SentencePieceProcessor(model_file=str(tokenizer_path))
     encoded = torch.tensor([sp.bos_id()] + sp.encode(prompt), dtype=torch.int, device=device)
@@ -362,7 +510,12 @@ def main(
         for i in range(num_samples):
             torch.cuda.synchronize()
             t0 = time.perf_counter()
-            y = generate(model, encoded, max_new_tokens, temperature=temperature, top_k=top_k)
+            if draft is None:
+                y = generate(model, encoded, max_new_tokens, temperature=temperature, top_k=top_k)
+            else:
+                y = generate_speculative(model, draft, encoded, max_new_tokens, num_draft=num_draft,
+                                         temperature=temperature, top_k=top_k)
+                draft.reset_cache()
             torch.cuda.synchronize()
             t = time.perf_counter() - t0
             model.reset_cache()
@@ -402,7 +555,13 @@ def cli() -> None:
                          "with --prompts_file, prompts decoded together per generate_prompts call")
     ap.add_argument("--prompts_file", type=Path, default=None,
                     help="a text file of prompts, one per line, decoded in groups of --batch_size (replaces --prompt)")
+    ap.add_argument("--draft_checkpoint_path", type=Path, default=None,
+                    help="a smaller model's checkpoint: decode with generate_speculative, this model proposing tokens")
+    ap.add_argument("--draft_quantize", default=None, choices=[None, "llm.int8", "gptq.int4", "gptq.int8"])
+    ap.add_argument("--num_draft", type=int, default=4, help=f"draft tokens per speculative round (1..{MAX_DRAFT})")
     a = ap.parse_args()
+    if a.draft_checkpoint_path is not None and (a.batch_size != 1 or a.prompts_file is not None):
+        ap.error("--draft_checkpoint_path decodes one sequence at a time (batch_size 1, no prompts_file)")
     main(**vars(a))
 
 

@@ -285,7 +285,7 @@ class _DecodeState:
     """Static buffers + the C argument block of b2l_decode_step for one (B, S)."""
 
     def __init__(self, model: "LLaMA", B: int, S: int, device: torch.device, idx_dtype: torch.dtype,
-                 row_pos: bool = False) -> None:
+                 row_pos: bool = False, stepwise: bool = False) -> None:
         from .quantization import ColBlockQuantizedLinear
 
         cfg = model.config
@@ -295,8 +295,9 @@ class _DecodeState:
         self.B, self.S, self.row_pos = B, S, row_pos
         self.generation = WEIGHTS_GENERATION[0]   # raw weight pointers below are valid for this generation only
         self.idx = torch.zeros(B, dtype=idx_dtype, device=device)
-        # B2L_F_ROW_POS: one position per row (and model._ring holds one offset per row); else one shared position
-        self.pos = torch.zeros(B if row_pos else 1, dtype=torch.int64, device=device)
+        # B2L_F_ROW_POS: one position per row (and model._ring holds one offset per row); B2L_F_STEPWISE: the B rows are
+        # consecutive tokens of one sequence, one position each; else one shared position
+        self.pos = torch.zeros(B if (row_pos or stepwise) else 1, dtype=torch.int64, device=device)
         self.x = torch.empty((B, C_), **bf)
         self.qkv = torch.empty((B, 3 * C_), **bf)
         self.att = torch.empty((B, C_), **bf)
@@ -313,14 +314,15 @@ class _DecodeState:
         # gptq.int8: the batch-1 kernel with 8-bit weights (b2l_w8_tile_i8 tilings); with `w8_batch_step`, batches of
         # 2..16 run b2l_w8_gemv_batch on the same resident tilings (B2L_F_W8_BATCH).  gptq.int4 with `q4_batch_step`:
         # batches of 2..16 run b2l_q4_gemv_batch_i8 on the batch-1 tilings (B2L_F_Q4_BATCH_I8)
+        # B2L_F_STEPWISE (decode_tokens) always runs the row-exact batch kernels: each row must equal the batch-1 step
         w8 = model._fast_ok == "w8"
         w8b = w8 and B > 1
-        q4b = model._fast_ok == "q4" and B > 1 and model.q4_batch_step
+        q4b = model._fast_ok == "q4" and B > 1 and (model.q4_batch_step or stepwise)
         # llm.int8: b2l_q8_linear (batch 1) or b2l_q8_linear_batch (2..16, B2L_F_Q8_BATCH) on every weight's CB / SCB in
         # place (no copy, no tiling)
         q8 = model._fast_ok == "q8"
         q8b = q8 and B > 1
-        assert not w8b or (model.w8_batch_step and B <= 16)
+        assert not w8b or ((model.w8_batch_step or stepwise) and B <= 16)
         gemv = (B == 1) or w8b or q4b or (B <= 8 and BATCH_GEMV)
         i8 = B == 1 or w8b or q4b   # the b2l_q4_tile_i8 / b2l_w8_tile_i8 tilings (the resident copy of a compacted model)
         self.batch_ws = None
@@ -378,7 +380,8 @@ class _DecodeState:
             att=self.att.data_ptr(), hid=self.hid.data_ptr(), attn_work=self.work.data_ptr(),
             logits=self.logits.data_ptr(),
             flags=(model.decode_flags | (L.F_W8 if w8 else 0) | (L.F_W8_BATCH if w8b else 0) | (L.F_Q8 if q8 else 0)
-                   | (L.F_Q4_BATCH_I8 if q4b else 0) | (L.F_Q8_BATCH if q8b else 0) | (L.F_ROW_POS if row_pos else 0)),
+                   | (L.F_Q4_BATCH_I8 if q4b else 0) | (L.F_Q8_BATCH if q8b else 0) | (L.F_ROW_POS if row_pos else 0)
+                   | (L.F_STEPWISE if stepwise else 0)),
             batch_work=None if self.batch_ws is None else self.batch_ws.data_ptr())
         if q8:
             self.q8_layers = q8_layers
@@ -465,6 +468,7 @@ class LLaMA(nn.Module):
         self._ring: Optional[torch.Tensor] = None
         self._kv_store: Optional[torch.Tensor] = None
         self._decode: Optional[_DecodeState] = None
+        self._verify = {}   # T -> _DecodeState of decode_tokens (B2L_F_STEPWISE), each with its own CUDA graph
         self._module_graph = None  # CUDA graph of the module-by-module decode step (non-fused Linear kinds)
         # the fused step can run every Linear (checked once): "q4" (per-row gptq.int4, any B <= 16), "w8" (per-row
         # gptq.int8, B == 1), False (module path)
@@ -552,6 +556,7 @@ class LLaMA(nn.Module):
         self.kv_caches.clear()
         self._kv_store = None
         self._decode = None
+        self._verify = {}
         self._module_graph = None
         if self._ring is not None:
             if self._ring.numel() != 1:   # back to one shared ring offset
@@ -565,6 +570,7 @@ class LLaMA(nn.Module):
         for blk in self.transformer.h:
             blk.attn._ring, blk.attn._ring_shared = ring, True
         self._decode, self._module_graph = None, None   # they point at the old ring
+        self._verify = {}
 
     @torch.no_grad()
     def prefill_rows(self, prompts: List[torch.Tensor], max_seq_length: int) -> torch.Tensor:
@@ -597,6 +603,7 @@ class LLaMA(nn.Module):
             self._kv_store = store[:, :, b:b + 1]
             self.kv_caches = [(store[i, 0, b:b + 1], store[i, 1, b:b + 1]) for i in range(cfg.n_layer)]   # contiguous
             self._decode, self._module_graph = None, None   # a one-token prompt's step state points at the last row
+            self._verify = {}
             last.append(self(p.view(1, -1), max_seq_length, torch.arange(p.numel(), device=dev))[0, -1].clone())
         self._kv_store = store
         self.kv_caches = [(store[i, 0], store[i, 1]) for i in range(cfg.n_layer)]
@@ -619,6 +626,7 @@ class LLaMA(nn.Module):
         self._kv_store = self._kv_store.expand(n_layer, two, B, nh, S, hs).contiguous()
         self.kv_caches = [(self._kv_store[i, 0], self._kv_store[i, 1]) for i in range(n_layer)]
         self._decode = None
+        self._verify = {}
         self._module_graph = None
 
     # ------------------------------------------------------------------ helpers
@@ -666,6 +674,7 @@ class LLaMA(nn.Module):
         # the interleaved fc1|fc2 copies are plain tensors of this module: they move with it (a compacted model has no other)
         self._fc12_cache = {k: (key, tuple(fn(t) for t in val)) for k, (key, val) in self._fc12_cache.items()}
         self._decode, self._module_graph, self._fast_ok = None, None, None
+        self._verify = {}
         return out
 
     def _fc12_is_only_copy(self, i: int) -> bool:
@@ -707,6 +716,7 @@ class LLaMA(nn.Module):
             blk.mlp.c_fc2.release_reference_layout(source=functools.partial(self._fc_from_fc12, i, 1))
         self.lm_head.release_reference_layout()
         self._decode, self._module_graph = None, None   # rebuilt on the next step (B > 1 states hold their transient tilings)
+        self._verify = {}
         torch.cuda.empty_cache()
         return self
 
@@ -797,6 +807,7 @@ class LLaMA(nn.Module):
             self._kv_store = torch.zeros((cfg.n_layer, 2, B, cfg.n_head, max_seq_length, hs), device=idx.device, dtype=torch.bfloat16)
             self.kv_caches = [(self._kv_store[i, 0], self._kv_store[i, 1]) for i in range(cfg.n_layer)]
             self._decode = None
+            self._verify = {}
             self._module_graph = None
         if rows:
             if self._kv_store.shape[2] != B:
@@ -812,7 +823,7 @@ class LLaMA(nn.Module):
                 # a linear was reloaded, repacked or moved since the argument block / graph was built: everything that
                 # bakes weight pointers is stale (fc1|fc2 interleave, eligibility, module graph included)
                 st = self._decode = None
-                self._module_graph, self._fast_ok = None, None
+                self._module_graph, self._fast_ok, self._verify = None, None, {}
                 # the interleaved fc1|fc2 copies are rebuilt from the reference buffers, except where compact() made
                 # one the ONLY copy of both layers (still released: nothing was loaded into them)
                 self._fc12_cache = {k: v for k, v in self._fc12_cache.items()
@@ -867,6 +878,70 @@ class LLaMA(nn.Module):
                 g.replay()
                 return mg["out"].clone() if self.copy_logits else mg["out"]
         return self._forward_modules(idx, max_seq_length, input_pos)
+
+    @torch.no_grad()
+    def decode_tokens(self, idx: torch.Tensor, max_seq_length: int, input_pos: torch.Tensor) -> torch.Tensor:
+        """Run T = 2..16 consecutive tokens of ONE sequence through the whole-token decode step in one call (the verify
+        step of speculative decoding): idx (1, T) at positions input_pos (T,) = p..p+T-1, all < max_seq_length, on the
+        batch-1 KV cache.  Returns (T, vocab) logits; row t equals, bit for bit, the logits `forward` returns for token t
+        alone at input_pos[t] after tokens 0..t-1 (b2l_decode_step under B2L_F_STEPWISE: the row-exact batch linears
+        and, per query, the attention of a T == 1 launch), and the cache ends as those T batch-1 steps leave it.
+
+        gptq.int4 and gptq.int8 models the fused batch-1 step runs (compacted or not, plain, LLaMA-Adapter v1 or LoRA);
+        dense, llm.int8, LLaMA-Adapter v2 and grouped or biased gptq models are refused.  One step state per T, each
+        replayed as its own CUDA graph."""
+        if idx.dim() != 2 or idx.shape[0] != 1 or not 2 <= idx.shape[1] <= 16:
+            raise ValueError(f"decode_tokens: idx must be (1, T) with T in 2..16, got {tuple(idx.shape)}")
+        T = idx.shape[1]
+        if input_pos.dim() != 1 or input_pos.numel() != T:
+            raise ValueError(f"decode_tokens: input_pos must be ({T},), got {tuple(input_pos.shape)}")
+        if idx.dtype not in (torch.int32, torch.int64):
+            raise ValueError(f"decode_tokens: idx dtype {idx.dtype}; int32 or int64")
+        max_seq_length = self._prepare(idx, max_seq_length)
+        why = self._decode_tokens_refusal()
+        if why is not None:
+            raise RuntimeError(f"decode_tokens: {why}")
+        if self._ring.numel() != 1 or (self._kv_store is not None and self._kv_store.shape[2] != 1):
+            raise RuntimeError("decode_tokens: the KV cache holds more than one sequence; reset_cache() first")
+        if not self.kv_caches:
+            cfg = self.config
+            self._kv_store = torch.zeros((cfg.n_layer, 2, 1, cfg.n_head, max_seq_length, cfg.n_embd // cfg.n_head),
+                                         device=idx.device, dtype=torch.bfloat16)
+            self.kv_caches = [(self._kv_store[i, 0], self._kv_store[i, 1]) for i in range(cfg.n_layer)]
+            self._decode, self._module_graph, self._verify = None, None, {}
+        if self._kv_store.shape[4] != max_seq_length:
+            raise ValueError(f"decode_tokens: max_seq_length={max_seq_length} against a cache of {self._kv_store.shape[4]}")
+        st = self._verify.get(T)
+        if st is not None and (st.generation != WEIGHTS_GENERATION[0] or st.idx.dtype != idx.dtype
+                               or st.idx.device != idx.device):
+            self._verify, self._fast_ok, st = {}, None, None   # weight pointers or the step's inputs changed
+            return self.decode_tokens(idx, max_seq_length, input_pos)
+        if st is None:
+            st = self._verify[T] = _DecodeState(self, T, max_seq_length, idx.device, idx.dtype, stepwise=True)
+        st.idx.copy_(idx.reshape(-1))
+        st.pos.copy_(input_pos)
+        if st.graph is not None:
+            st.graph.replay()
+        elif self.graph_after and st.calls >= self.graph_after:
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                st.enqueue()
+            st.graph = g
+            g.replay()
+        else:
+            st.enqueue()
+        st.calls += 1
+        out = st.logits.view(T, -1)
+        return out.clone() if self.copy_logits else out
+
+    def _decode_tokens_refusal(self) -> Optional[str]:
+        """Why this model cannot run decode_tokens, or None."""
+        if self._fast_ok is None:
+            self._fast_ok = self._fast_decode_ok()
+        if self._fast_ok not in ("q4", "w8") or self._has_affines():
+            return ("needs a gptq.int4 or gptq.int8 model the fused decode step runs with its row-exact batch kernels "
+                    "(not dense, llm.int8, LLaMA-Adapter v2, or grouped / biased gptq)")
+        return None
 
     def _prepare(self, idx: torch.Tensor, max_seq_length: Optional[int]) -> int:
         """model.py:79-91: the shape checks, and the RoPE table and KV ring on idx's device.  Returns max_seq_length."""
