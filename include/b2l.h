@@ -117,17 +117,9 @@ typedef struct b2l_q4_linear_args {
   void* workspace;      /* b2l_q4_gemv_batch only: b2l_q4_gemv_batch_workspace_bytes(K) bytes of device
                            scratch, 16-byte aligned (activation fragments; may be shared by all
                            launches of one stream)                                       */
-  const void* pf_ptr[B2L_PF_SEGMENTS];          /* b2l_q4_gemv only, L2 prefetch hint: byte ranges (16-byte aligned,
-                           multiples of 16; NULL / 0 = unused) that LATER launches will stream - typically the
-                           weights of the next linears.  The CTAs ask the L2 for them as soon as their own
-                           weight ring is full, so HBM keeps streaming while this launch waits for its
-                           activations, reduces and writes its result (the reference has no counterpart:
-                           quantization.py:284-333 launches one Triton kernel per linear)          */
+  /* unused (no kernel reads them): they keep the layout of the block                           */
+  const void* pf_ptr[B2L_PF_SEGMENTS];
   unsigned long long pf_bytes[B2L_PF_SEGMENTS];
-  /* strided form of the same hint - the KV-cache rows a later b2l_attention launch reads (model.py:211-222):
-     pf_nseg ranges, pf_seg_stride bytes apart, at each of pf_kv[0] and pf_kv[1]; every range is
-     rows * pf_row_bytes bytes long, rows = min(*pf_rows, pf_rows_max) read ON THE DEVICE when the launch runs
-     (pf_rows = the step's input_pos).  pf_kv[0] == NULL: unused                                           */
   const void* pf_kv[2];
   const long long* pf_rows;
   int pf_rows_max, pf_nseg, pf_row_bytes;

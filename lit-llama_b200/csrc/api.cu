@@ -1,9 +1,5 @@
 // Error state, device facts and the whole-token entry point of libb200llama.
-#include <algorithm>
-#include <cstdlib>
 #include <mutex>
-#include <utility>
-#include <vector>
 
 #include "b2l_common.cuh"
 
@@ -68,73 +64,11 @@ extern "C" int b2l_device_info(int* sm, int* cc_major, int* cc_minor) {
 // Per Block: [rms_1 + c_attn] -> rope/append/attention -> [c_proj + residual]
 //            -> [rms_2 + c_fc1|c_fc2 + silu*mul] -> [mlp.c_proj + residual]
 // ---------------------------------------------------------------------------------
-// ---- L2 prefetch windows of the batch-1 step (b2l_q4_linear_args::pf_ptr).
-// The packed weights of a token are read in a fixed order: per Block c_attn, c_proj, fc1|fc2, mlp.c_proj, then lm_head,
-// then the next token's Block 0 again.  Seen as one byte stream, launch j (bytes [S_j, E_j)) asks the L2 for
-// [max(S_j + D, E_j), E_j + D): after every launch everything up to D bytes beyond its own end has been requested, so
-// HBM always has a backlog to work on while a launch waits for its activations (prologue), reduces and stores
-// (epilogue) or the attention kernel runs.  D = B2L_PF_MB (MB, read once; 0 switches the hint off).
-struct PfWindow { const void* ptr[B2L_PF_SEGMENTS]; unsigned long long bytes[B2L_PF_SEGMENTS]; };
-
-static size_t prefetch_distance() {
-  static const long mb = [] { const char* e = getenv("B2L_PF_MB"); return e ? atol(e) : 0L; }();
-  return mb > 0 ? (size_t)mb << 20 : 0;
-}
-
-static std::vector<PfWindow> prefetch_windows(const b2l_decode_args* d) {
-  std::vector<std::pair<const uint8_t*, size_t>> ops;
-  const bool w8 = (d->flags & B2L_F_W8) != 0;
-  auto add = [&](const b2l_q4_weight& w) {
-    ops.push_back({(const uint8_t*)w.qw_mma, w8 ? b2l_w8_tiled_i8_bytes(w.N, w.K) : b2l_q4_tiled_i8_bytes(w.N, w.K)});
-  };
-  for (int l = 0; l < d->n_layer; ++l) {
-    add(d->layers[l].c_attn); add(d->layers[l].c_proj); add(d->layers[l].c_fc12); add(d->layers[l].mlp_proj);
-  }
-  add(d->lm_head);
-  const size_t n = ops.size(), D = prefetch_distance();
-  std::vector<PfWindow> out(n, PfWindow{});
-  if (D == 0) return out;
-  std::vector<size_t> start(n + 1, 0);
-  for (size_t j = 0; j < n; ++j) start[j + 1] = start[j] + ops[j].second;
-  for (size_t j = 0; j < n; ++j) {
-    size_t lo = std::max(start[j] + D, start[j + 1]), hi = start[j + 1] + D;   // may run past `total`: wraps to the next token
-    int sg = 0;
-    size_t k = j + 1;      // first op at or after `lo` (positions counted from this token's start; op k lives at k % n)
-    size_t base = start[j + 1];
-    while (lo < hi && sg < B2L_PF_SEGMENTS && k < j + 1 + n) {
-      const auto& op = ops[k % n];
-      const size_t op_lo = base, op_hi = base + op.second;
-      if (lo < op_hi) {
-        const size_t a = (lo - op_lo) & ~(size_t)127, b = std::min(hi, op_hi) - op_lo;
-        if (b > a && op.first != nullptr) {
-          out[j].ptr[sg] = op.first + a;
-          out[j].bytes[sg] = (b - a + 15) & ~(size_t)15;
-          ++sg;
-        }
-        lo = std::min(hi, op_hi);
-      }
-      base = op_hi;
-      ++k;
-    }
-  }
-  return out;
-}
-
 static int q4_call(const b2l_q4_weight& w, const void* x, int ldx, void* y, int ldy, int M, int sz_dtype, int prologue,
                    const void* norm_scale, float eps, int epilogue, const void* res, int ldres, int flags,
-                   b2l_stream_t stream, void* trace = nullptr, void* batch_work = nullptr, const PfWindow* pf = nullptr,
-                   const b2l_decode_args* kv_of = nullptr, int kv_layer = 0, const b2l_out_affine* aff = nullptr) {
+                   b2l_stream_t stream, void* trace = nullptr, void* batch_work = nullptr, const b2l_out_affine* aff = nullptr) {
   b2l_q4_linear_args a{};
   if (aff != nullptr) a.out_affine = *aff;   // batch-1 kernels only (b2l_decode_step checks B == 1 and qw_mma)
-  if (kv_of != nullptr) {   // this linear also asks the L2 for the KV-cache rows of layer `kv_layer`'s attention
-    const int hs = kv_of->n_embd / kv_of->n_head;
-    a.pf_kv[0] = kv_of->layers[kv_layer].k_cache; a.pf_kv[1] = kv_of->layers[kv_layer].v_cache;
-    a.pf_rows = (const long long*)kv_of->input_pos;
-    a.pf_rows_max = kv_of->S; a.pf_nseg = kv_of->B * kv_of->n_head; a.pf_row_bytes = hs * 2;
-    a.pf_seg_stride = (unsigned long long)kv_of->S * hs * 2;
-  }
-  if (pf != nullptr)
-    for (int i = 0; i < B2L_PF_SEGMENTS; ++i) { a.pf_ptr[i] = pf->ptr[i]; a.pf_bytes[i] = pf->bytes[i]; }
   a.x = x; a.ldx = ldx;
   const bool gemv = (M == 1 && w.qw_mma != nullptr);
   const bool batch = (!gemv && M <= 8 && w.qw_mma != nullptr && batch_work != nullptr);
@@ -341,14 +275,6 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
   char* tlb = (char*)d->timeline;
   int li = 0;
   auto tl = [&]() -> void* { void* r = tlb ? (void*)(tlb + 512 * li) : nullptr; ++li; return r; };
-  // batch 1 on the int8-MMA kernel: every linear carries the L2 prefetch window of the weights that follow it
-  std::vector<PfWindow> pfw;
-  if (B == 1 && d->lm_head.qw_mma != nullptr) pfw = prefetch_windows(d);
-  // B2L_KV_PREFETCH (read once): 0 off, 1 the previous Block's mlp.c_proj asks for a Block's KV rows, 2 its own c_attn does
-  static const int kv_prefetch = [] { const char* e = getenv("B2L_KV_PREFETCH"); return e ? atoi(e) : 0; }();
-  const bool kv_ok = B == 1 && hs == 128 && d->lm_head.qw_mma != nullptr;
-  int oi = 0;
-  auto pf = [&]() -> const PfWindow* { const PfWindow* r = pfw.empty() ? nullptr : &pfw[oi]; ++oi; return r; };
   if ((rc = row_pos ? b2l_ring_advance_rows(d->input_pos, B, d->ring_start, d->S, stream)
                     : b2l_ring_advance(d->input_pos, stepwise ? B : 1, d->ring_start, d->S, stream)))
     return rc;
@@ -362,8 +288,7 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
     void* t = tl();
     if ((rc = Q ? q8_call(d, Q->c_attn, nullptr, d->x, d->qkv, L.rms_1, B2L_EPI_STORE, nullptr, af ? &af->c_attn : nullptr, stream)
                 : q4_call(L.c_attn, d->x, C, d->qkv, 3 * C, B, d->sz_dtype, B2L_PRO_RMSNORM, L.rms_1, d->eps, B2L_EPI_STORE,
-                          nullptr, 0, fl, stream, t, d->batch_work, pf(), (kv_ok && kv_prefetch == 2) ? d : nullptr, l,
-                          af ? &af->c_attn : nullptr)))
+                          nullptr, 0, fl, stream, t, d->batch_work, af ? &af->c_attn : nullptr)))
       return rc;
     // LoRA on c_attn (lora.py:308-326): the low-rank term from rms_1(x), added into qkv in place
     if (d->loras != nullptr && d->loras[l].r != 0 &&
@@ -383,24 +308,20 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
     t = tl();
     if ((rc = Q ? q8_call(d, Q->c_proj, nullptr, d->att, d->x, nullptr, B2L_EPI_RESIDUAL, d->x, af ? &af->c_proj : nullptr, stream)
                 : q4_call(L.c_proj, d->att, C, d->x, C, B, d->sz_dtype, B2L_PRO_NONE, nullptr, 0.f, B2L_EPI_RESIDUAL, d->x, C,
-                          fl, stream, t, d->batch_work, pf(), nullptr, 0, af ? &af->c_proj : nullptr)))
+                          fl, stream, t, d->batch_work, af ? &af->c_proj : nullptr)))
       return rc;
     t = tl();
     if ((rc = Q ? q8_call(d, Q->c_fc1, &Q->c_fc2, d->x, d->hid, L.rms_2, B2L_EPI_SWIGLU, nullptr, af ? &af->c_fc12 : nullptr, stream)
                 : q4_call(L.c_fc12, d->x, C, d->hid, d->n_hidden, B, d->sz_dtype, B2L_PRO_RMSNORM, L.rms_2, d->eps,
-                          B2L_EPI_SWIGLU, nullptr, 0, fl, stream, t, d->batch_work, pf(), nullptr, 0, af ? &af->c_fc12 : nullptr)))
+                          B2L_EPI_SWIGLU, nullptr, 0, fl, stream, t, d->batch_work, af ? &af->c_fc12 : nullptr)))
       return rc;
-    // mlp.c_proj fits the weight ring entirely, so HBM idles while it converts its activations: it asks the L2 for
-    // the NEXT Block's KV-cache rows (B2L_KV_PREFETCH=0 switches that off)
-    const bool kvpf = kv_prefetch == 1 && kv_ok && l + 1 < d->n_layer;
     t = tl();
     if ((rc = Q ? q8_call(d, Q->mlp_proj, nullptr, d->hid, d->x, nullptr, B2L_EPI_RESIDUAL, d->x, af ? &af->mlp_proj : nullptr, stream)
                 : q4_call(L.mlp_proj, d->hid, d->n_hidden, d->x, C, B, d->sz_dtype, B2L_PRO_NONE, nullptr, 0.f,
-                          B2L_EPI_RESIDUAL, d->x, C, fl, stream, t, d->batch_work, pf(), kvpf ? d : nullptr, l + 1,
-                          af ? &af->mlp_proj : nullptr)))
+                          B2L_EPI_RESIDUAL, d->x, C, fl, stream, t, d->batch_work, af ? &af->mlp_proj : nullptr)))
       return rc;
   }
   if (q8) return q8_call(d, d->q8_lm_head, nullptr, d->x, d->logits, d->ln_f, B2L_EPI_STORE, nullptr, &d->lm_head_affine, stream);
   return q4_call(d->lm_head, d->x, C, d->logits, d->vocab, B, d->sz_dtype, B2L_PRO_RMSNORM, d->ln_f, d->eps,
-                 B2L_EPI_STORE, nullptr, 0, fl, stream, tl(), d->batch_work, pf(), nullptr, 0, &d->lm_head_affine);
+                 B2L_EPI_STORE, nullptr, 0, fl, stream, tl(), d->batch_work, &d->lm_head_affine);
 }

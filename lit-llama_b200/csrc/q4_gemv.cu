@@ -39,7 +39,7 @@
 // gptq.int8 (8-bit levels, b2l_w8_gemv) runs the same kernel with W8 = true: weight layout b2l_w8_tile_i8,
 // [N/16 row blocks][K/64 k blocks][2 chunks][32 lanes][16 B], whose four words per lane are the u8 A fragment itself
 // (no LOP3, no row-pair recovery in the epilogue).  The int32 accumulators hold 255 * 128 * K < 2^31 for K <= 24576.
-#include <cstdlib>
+#include <algorithm>
 
 #include "q4_mma_common.cuh"
 
@@ -58,18 +58,9 @@ struct Params {
   int nst;               // ring stages
   unsigned long long* tl;  // debug timeline (nullptr = off)
   int nocompute;           // debug: consumers release every stage untouched (pure TMA streaming rate)
-  // L2 prefetch hint (b2l_q4_linear_args::pf_ptr): byte ranges later launches stream; CTA c asks for the c-th slice
-  const uint8_t* pf_ptr[B2L_PF_SEGMENTS];
-  uint32_t pf_bytes[B2L_PF_SEGMENTS];
-  int pf_mode;             // 0 off, 1 bulk prefetch by the producer lane, 2 / 4 per-line prefetch (128 B / 32 B apart)
-  // strided form (KV-cache rows of a following attention launch; b2l_q4_linear_args::pf_kv)
-  const uint8_t* pf_kv[2]; const long long* pf_rows; int pf_rows_max, pf_nseg, pf_row_bytes; unsigned long long pf_seg_stride;
-  int evict_first;         // demand loads carry an L2 evict_first policy (a weight byte is read once per token)
   // LLaMA-Adapter v2 affine (AFFINE instantiations only): bf16 [N] in weight row order
   const __nv_bfloat16* aff_scale; const __nv_bfloat16* aff_bias;
 };
-
-constexpr uint32_t PF_CHUNK = 16384;   // bytes per bulk L2 prefetch instruction
 
 // digit-plane stride in bytes: one byte per k, padded so that planes n and n + 1 fall into different bank halves
 __host__ __device__ inline uint32_t plane_stride(int K) { return (uint32_t)K + ((K % 128 == 0) ? 64u : 0u); }
@@ -90,26 +81,6 @@ __host__ __device__ inline SmemLayout smem_layout(int nst, int K, int ndig) {
   L.bars = o;    o += 2 * MAX_STAGES * 8;
   L.total = (o + 127u) & ~127u;
   return L;
-}
-
-// ---- L2 prefetch of weights a later launch reads (no shared memory, no completion: fire and forget)
-__device__ __forceinline__ void l2_prefetch_bulk(const void* src, uint32_t bytes) {
-  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void l2_prefetch_line(const void* src) {
-  asm volatile("prefetch.global.L2 [%0];" ::"l"(src));
-}
-// this CTA's slice [lo, hi) of a segment of `bytes` bytes, cut at 128-byte lines
-__device__ __forceinline__ void pf_slice(uint32_t bytes, uint32_t& lo, uint32_t& hi) {
-  const uint32_t lines = (bytes + 127u) >> 7;
-  lo = (uint32_t)(((unsigned long long)blockIdx.x * lines) / gridDim.x) << 7;
-  hi = min((uint32_t)(((unsigned long long)(blockIdx.x + 1) * lines) / gridDim.x) << 7, bytes);
-}
-__device__ __forceinline__ void tma_bulk_g2s_hint(uint32_t dst, const void* src, uint32_t bytes, uint32_t mbar, uint64_t policy) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(dst),
-      "l"(src), "r"(bytes), "r"(mbar), "l"(policy)
-      : "memory");
 }
 
 // X (|X| < 2^30) -> word whose bytes are its balanced base-256 digits (byte 3 = signed top digit)
@@ -186,8 +157,6 @@ __global__ void __launch_bounds__(NTHREADS, 2) q4_gemv_kernel(const Params p) {
       int slot = 0;
       uint32_t phase = 1;  // fresh barriers: waiting on parity 1 passes immediately
       int it = 0;
-      uint64_t policy = 0;
-      if (p.evict_first) asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(policy));
       for (int u = 0; u < n_units; ++u) {
         const int rb = rb_lo + 2 * u;
         const int halves = min(2, rb_hi - rb);
@@ -201,46 +170,13 @@ __global__ void __launch_bounds__(NTHREADS, 2) q4_gemv_kernel(const Params p) {
           for (int h = 0; h < halves; ++h) {
             const uint32_t dst = sbase + L.ring + slot * STAGE_BYTES + h * HALF_STAGE_BYTES;
             const uint8_t* from = src + ((size_t)h * n_kb + kb0) * KB_BYTES;
-            if (p.evict_first) tma_bulk_g2s_hint(dst, from, bytes, bar_full + slot * 8, policy);
-            else tma_bulk_g2s(dst, from, bytes, bar_full + slot * 8);
+            tma_bulk_g2s(dst, from, bytes, bar_full + slot * 8);
           }
           if (++slot == p.nst) { slot = 0; phase ^= 1; }
-          if (it + 1 == min(total_stages, p.nst)) {
-            pdl_launch_dependents();  // ring full: next kernel may prefetch
-            if (p.pf_mode == 1) {
-              // the ring is full and this lane would now wait for a free slot: queue the L2 prefetch of this CTA's
-              // slice of the weights the following launches read (HBM keeps streaming through the activation waits)
-#pragma unroll
-              for (int sgi = 0; sgi < B2L_PF_SEGMENTS; ++sgi) {
-                if (p.pf_bytes[sgi] == 0) continue;
-                uint32_t lo, hi;
-                pf_slice(p.pf_bytes[sgi], lo, hi);
-#pragma unroll 1
-                for (uint32_t o = lo; o < hi; o += PF_CHUNK) l2_prefetch_bulk(p.pf_ptr[sgi] + o, min(PF_CHUNK, hi - o));
-              }
-            }
-          }
+          if (it + 1 == min(total_stages, p.nst)) pdl_launch_dependents();  // ring full: next kernel may prefetch
         }
       }
       if (total_stages == 0) pdl_launch_dependents();
-      if (p.pf_kv[0] != nullptr) {
-        // KV-cache rows of the attention launch that follows the next linear: requested once this CTA's own ring is
-        // full (behind its demand loads), 16 KB per instruction, round-robin over the grid.  The cache rows of old
-        // positions do not depend on the current token; the attention kernel can only start its own loads when the
-        // linear before it frees shared memory, so without this the cache streams from HBM on the critical path.
-        long long rows = *p.pf_rows;
-        rows = rows < 0 ? 0 : (rows > p.pf_rows_max ? p.pf_rows_max : rows);
-        const uint32_t seg_bytes = (uint32_t)rows * (uint32_t)p.pf_row_bytes;
-        const uint32_t cps = (seg_bytes + PF_CHUNK - 1) / PF_CHUNK;
-        const uint32_t total = 2u * (uint32_t)p.pf_nseg * cps;
-#pragma unroll 1
-        for (uint32_t id = blockIdx.x; id < total; id += gridDim.x) {
-          const uint32_t sg = id / cps, o = (id - sg * cps) * PF_CHUNK;
-          const uint32_t which = sg >= (uint32_t)p.pf_nseg ? 1u : 0u;
-          const uint8_t* base = p.pf_kv[which] + (size_t)(sg - which * p.pf_nseg) * p.pf_seg_stride;
-          l2_prefetch_bulk(base + o, min(PF_CHUNK, seg_bytes - o));
-        }
-      }
     }
   } else if (warp < NCW) {
     // ===================== consumer warps =====================
@@ -474,17 +410,6 @@ __global__ void __launch_bounds__(NTHREADS, 2) q4_gemv_kernel(const Params p) {
     if (tid == 0) tl_max(p.tl, 3);
   } else {
     // ===================== epilogue warp: lane = row of the 32-row unit =====================
-    if (p.pf_mode >= 2) {   // per-line variant of the L2 prefetch (this warp idles until the first unit is reduced)
-      const uint32_t step = p.pf_mode == 2 ? 128u : 32u;
-#pragma unroll
-      for (int sgi = 0; sgi < B2L_PF_SEGMENTS; ++sgi) {
-        if (p.pf_bytes[sgi] == 0) continue;
-        uint32_t lo, hi;
-        pf_slice(p.pf_bytes[sgi], lo, hi);
-#pragma unroll 1
-        for (uint32_t o = lo + lane * step; o < hi; o += 32 * step) l2_prefetch_line(p.pf_ptr[sgi] + o);
-      }
-    }
     // the affine vectors are weights: the first unit's are loaded before the wait, later units' ahead of their reduction
     float aff_s = 1.f, aff_b = 0.f;
     auto load_affine = [&](int u) {
@@ -692,18 +617,43 @@ extern "C" int b2l_w8_untile_i8(const void* qw_tiled, void* qw, int N, int K, b2
 namespace {
 constexpr int MAX_K = 12 * NCW * 32 * 8;   // 24576
 
+// Ring stages that fit `budget` bytes of shared memory at this K (0: not even two)
+template <int NDIG>
+int ring_stages(int K, uint32_t budget) {
+  const uint32_t fixed = smem_layout(0, K, NDIG).total;
+  const int nst = fixed + 2 * STAGE_BYTES <= budget ? (int)((budget - fixed) / STAGE_BYTES) : 0;
+  return nst > MAX_STAGES ? MAX_STAGES : nst;
+}
+
+// Stages a CTA owning `rbs` row blocks streams (pairs, then at most one single, as q4_gemv_kernel walks them)
+template <bool W8>
+int cta_stages(int rbs, int n_kb) {
+  constexpr int KBP = WTile<W8>::KBP;
+  return (rbs / 2) * ((n_kb + KBP - 1) / KBP) + (rbs & 1) * ((n_kb + 2 * KBP - 1) / (2 * KBP));
+}
+
+// Launch shape.  Up to K = 16384, two CTAs per SM with 110 KB of shared memory each; above, the digit planes leave no
+// room for a useful ring at that size and one CTA takes the whole SM.  A linear small enough that, at one CTA per SM,
+// every CTA's whole share of the weights fits its ring (LLaMA-7B attn.c_proj: 2 row blocks, 4 of 5 stages) runs as
+// one 113 KB CTA per SM instead: two such CTAs fit an SM beside each other (228 KB less 1 KB reserved per CTA), so
+// the launch needs one free slot, not two, to become resident behind the attention kernel, and each CTA requests all
+// of its weights before the dependency resolves.  On H100 that is 3.3 % more 7B tokens/s; one CTA per SM for the
+// larger linears, whose stream does not fit, measured slower (DESIGN.md section 3: 8 consumer warps per SM stream less
+// than 16).
 template <int MAXC, int NDIG, bool W8, bool AFFINE>
-int launch_gemv_variant(const Params& p0, int ctas_per_sm, int grid_override, bool pdl, cudaStream_t stream) {
+int launch_gemv_variant(const Params& p0, int grid_override, bool pdl, cudaStream_t stream) {
   Params p = p0;
-  // ring: as deep as fits `ctas_per_sm` CTAs per SM
-  // B2L_GEMV_SMEM_KB: shared-memory budget of a CTA (default: 110 KB for two CTAs per SM, 224 KB for one)
-  static const int env_kb = [] { const char* e = getenv("B2L_GEMV_SMEM_KB"); return e ? atoi(e) : 0; }();
-  const uint32_t budget = (env_kb > 0 ? (uint32_t)env_kb : (ctas_per_sm >= 2 ? 110u : 224u)) * 1024u;
-  const uint32_t fixed = smem_layout(0, p.K, NDIG).total;
-  int nst = fixed + 2 * STAGE_BYTES <= budget ? (int)((budget - fixed) / STAGE_BYTES) : 0;
-  if (nst > MAX_STAGES) nst = MAX_STAGES;
-  static const int env_nst = [] { const char* e = getenv("B2L_GEMV_STAGES"); return e ? atoi(e) : 0; }();
-  if (env_nst > 0 && nst > env_nst) nst = env_nst;
+  int ctas_per_sm = p.K <= 16384 ? 2 : 1;
+  int nst = ring_stages<NDIG>(p.K, (ctas_per_sm == 2 ? 110u : 224u) * 1024u);
+  if (ctas_per_sm == 2) {
+    const int sms = sm_count(), n_kb = p.K / KB;
+    const int one = ring_stages<NDIG>(p.K, 113u * 1024u);
+    const int rb_max = (p.n_rb + sms - 1) / sms, rb_min = p.n_rb / sms;
+    if (std::max(cta_stages<W8>(rb_max, n_kb), cta_stages<W8>(rb_min, n_kb)) <= one) {
+      ctas_per_sm = 1;
+      nst = one;
+    }
+  }
   if (nst < 2) {
     set_error("b2l_q4_gemv: K=%d does not leave room for the weight ring", p.K);
     return B2L_E_UNSUPPORTED;
@@ -720,9 +670,9 @@ int launch_gemv_variant(const Params& p0, int ctas_per_sm, int grid_override, bo
 }
 
 template <int MAXC, int NDIG, bool W8>
-int launch_gemv(const Params& p, int ctas_per_sm, int grid_override, bool pdl, cudaStream_t stream) {
-  if (p.aff_scale != nullptr) return launch_gemv_variant<MAXC, NDIG, W8, true>(p, ctas_per_sm, grid_override, pdl, stream);
-  return launch_gemv_variant<MAXC, NDIG, W8, false>(p, ctas_per_sm, grid_override, pdl, stream);
+int launch_gemv(const Params& p, int grid_override, bool pdl, cudaStream_t stream) {
+  if (p.aff_scale != nullptr) return launch_gemv_variant<MAXC, NDIG, W8, true>(p, grid_override, pdl, stream);
+  return launch_gemv_variant<MAXC, NDIG, W8, false>(p, grid_override, pdl, stream);
 }
 
 // b2l_q4_gemv (W8 = false) and b2l_w8_gemv (W8 = true): the same checks, argument block and launch policy
@@ -762,41 +712,12 @@ int gemv_entry(const b2l_q4_linear_args* a, b2l_stream_t stream) {
   p.nst = 0;
   p.tl = (unsigned long long*)a->trace;
   p.nocompute = (a->flags & B2L_F_DEBUG_NOCOMPUTE) ? 1 : 0;
-  // L2 prefetch hint.  B2L_PF_MODE (read once): 0 ignores the hint, 1 (default) bulk prefetch, 2 / 4 per-line prefetch;
-  // B2L_PF_EVICT=1 marks the demand loads evict_first
-  static const int env_pf_mode = [] { const char* e = getenv("B2L_PF_MODE"); return e ? atoi(e) : 1; }();
-  static const int env_evict = [] { const char* e = getenv("B2L_PF_EVICT"); return e ? atoi(e) : 0; }();
-  p.pf_mode = 0;
-  p.evict_first = env_evict;
-  p.pf_kv[0] = p.pf_kv[1] = nullptr; p.pf_rows = nullptr; p.pf_rows_max = p.pf_nseg = p.pf_row_bytes = 0; p.pf_seg_stride = 0;
-  if (a->pf_kv[0] != nullptr) {
-    B2L_CHECK_ARG(a->pf_kv[1] != nullptr && a->pf_rows != nullptr && a->pf_rows_max > 0 && a->pf_nseg > 0 && a->pf_row_bytes > 0 &&
-                      a->pf_row_bytes % 16 == 0 && a->pf_seg_stride % 16 == 0 && ((uintptr_t)a->pf_kv[0] % 16 == 0) &&
-                      ((uintptr_t)a->pf_kv[1] % 16 == 0) && (unsigned long long)a->pf_rows_max * a->pf_row_bytes < (1ull << 31),
-                  "%s: bad strided prefetch hint", fn);
-    p.pf_kv[0] = (const uint8_t*)a->pf_kv[0]; p.pf_kv[1] = (const uint8_t*)a->pf_kv[1];
-    p.pf_rows = a->pf_rows; p.pf_rows_max = a->pf_rows_max; p.pf_nseg = a->pf_nseg; p.pf_row_bytes = a->pf_row_bytes;
-    p.pf_seg_stride = a->pf_seg_stride;
-  }
-  for (int i = 0; i < B2L_PF_SEGMENTS; ++i) {
-    p.pf_ptr[i] = (const uint8_t*)a->pf_ptr[i];
-    p.pf_bytes[i] = 0;
-    if (a->pf_ptr[i] != nullptr && a->pf_bytes[i] != 0) {
-      B2L_CHECK_ARG(((uintptr_t)a->pf_ptr[i] % 16 == 0) && (a->pf_bytes[i] % 16 == 0) && a->pf_bytes[i] < (1ull << 31),
-                    "%s: prefetch segment %d must be 16-byte aligned, a multiple of 16 and < 2 GiB", fn, i);
-      p.pf_bytes[i] = (uint32_t)a->pf_bytes[i];
-      p.pf_mode = env_pf_mode;
-    }
-  }
-  // tuning knob (read once): B2L_GEMV_CTAS_PER_SM (default 2; K > 16384 runs one CTA per SM with a deeper ring)
-  static const int env_cps = [] { const char* e = getenv("B2L_GEMV_CTAS_PER_SM"); return e ? atoi(e) : 0; }();
   const bool pdl = (a->flags & B2L_F_PDL) != 0;
   cudaStream_t st = (cudaStream_t)stream;
   const int grid = a->split_k;  // split_k doubles as a grid override
   // three digits (|X| < 2^22) everywhere: the prologue's fma conversion needs the integer inside a float mantissa
-  if (a->K <= 12288) return launch_gemv<6, 3, W8>(p, env_cps > 0 ? env_cps : 2, grid, pdl, st);
-  if (a->K <= 16384) return launch_gemv<12, 3, W8>(p, env_cps > 0 ? env_cps : 2, grid, pdl, st);
-  return launch_gemv<12, 3, W8>(p, 1, grid, pdl, st);
+  if (a->K <= 12288) return launch_gemv<6, 3, W8>(p, grid, pdl, st);
+  return launch_gemv<12, 3, W8>(p, grid, pdl, st);
 }
 }  // namespace
 
