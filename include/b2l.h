@@ -524,6 +524,36 @@ int b2l_attention_nocache_adapter(void* qkv, const void* rope, void* y, void* wo
                                   const b2l_adapter_prefix* prefix, b2l_stream_t stream);
 
 /* ------------------------------------------------------------------------------
+ * Ragged prefill (continuous batching): n_seq prompts packed back to back into one qkv,
+ * each prefilled into its own row of a B_rows-row cache, in one launch per kernel.
+ *   qkv   bf16 [N, 3*C]: sequence s is tokens [start[s], start[s] + len[s]), at positions
+ *         0..len[s]-1; q is rotated in place
+ *   k/v cache bf16 [B_rows, nh, S, hs]: sequence s writes slots 0..len[s]-1 of row row[s]
+ *   ring_start int32 [B_rows]: ring_start[row[s]] is set to 0
+ *   y     bf16 [N, C]: causal attention within each sequence (plus the LLaMA-Adapter
+ *         prefix term when `prefix` is given, the same prefix for every query)
+ * Rows and ring offsets no sequence names are not touched.  Each sequence's y rows and
+ * cache rows equal, bit for bit, b2l_attention(_adapter) with B = 1, T = len[s], input_pos
+ * 0..len[s]-1 and ring offset 0 on a cache holding only that row: every 64-query tile
+ * starts at its sequence's first token, so it has the same queries, key bound and key
+ * order as in that launch.  `seqs` is read on the host and passed by value to the kernels
+ * (no device table, no copy: the call can be captured in a CUDA graph).
+ * head_size 128 only (else B2L_E_UNSUPPORTED).  B2L_E_ARG before any launch for null
+ * pointers, n_seq outside 1..16, a length outside 1..S, starts that do not tile [0, N) in
+ * order, a row outside 0..B_rows-1, or two sequences naming the same row.
+ * ---------------------------------------------------------------------------- */
+#define B2L_RAGGED_MAX_SEQ 16
+typedef struct b2l_ragged {
+  int n_seq;
+  int row[B2L_RAGGED_MAX_SEQ];
+  int start[B2L_RAGGED_MAX_SEQ];
+  int len[B2L_RAGGED_MAX_SEQ];
+} b2l_ragged;
+int b2l_attention_ragged(void* qkv, void* k_cache, void* v_cache, const void* rope, const b2l_ragged* seqs,
+                         int32_t* ring_start, void* y, int N, int B_rows, int n_head, int head_size, int S,
+                         int block_size, const b2l_adapter_prefix* prefix, b2l_stream_t stream);
+
+/* ------------------------------------------------------------------------------
  * LoRA (lit_llama/lora.py:92-326): the low-rank term of an UNMERGED MergedLinear,
  * added in place to the output y of its base linear (lora.py:308-326):
  *   u_m = bf16(A_g . xh_m)   d = bf16(B_g . u_m)   y = bf16(y + bf16(d * scaling))

@@ -10,13 +10,14 @@ from .model import LLaMA, LLaMAConfig, Block, CausalSelfAttention, MLP, RMSNorm,
 from .quantization import ColBlockQuantizedLinear
 from .int8 import Linear8bitLt
 from .utils import find_multiple, llama_model_lookup
-from .generate import generate, generate_batch, generate_prompts, generate_speculative, sample_probs, sample_token
+from .generate import (generate, generate_batch, generate_prompts, generate_speculative, generate_stream, sample_probs,
+                       sample_token)
 from .patch import patch_reference
 from .tp import TPLLaMA, shard_state_dict
 from . import evaluate
 
 __all__ = [
     "LLaMA", "LLaMAConfig", "Block", "CausalSelfAttention", "MLP", "RMSNorm", "build_rope_cache", "apply_rope",
-    "ColBlockQuantizedLinear", "Linear8bitLt", "find_multiple", "llama_model_lookup", "generate", "generate_batch", "generate_prompts", "generate_speculative", "sample_probs", "sample_token", "patch_reference", "TPLLaMA", "shard_state_dict",
+    "ColBlockQuantizedLinear", "Linear8bitLt", "find_multiple", "llama_model_lookup", "generate", "generate_batch", "generate_prompts", "generate_speculative", "generate_stream", "sample_probs", "sample_token", "patch_reference", "TPLLaMA", "shard_state_dict",
     "evaluate",
 ]

@@ -73,6 +73,15 @@ class LoRA(C.Structure):
 
 LORA_MAX_R = 64   # B2L_LORA_MAX_R
 
+RAGGED_MAX_SEQ = 16   # B2L_RAGGED_MAX_SEQ
+
+
+class Ragged(C.Structure):
+    """b2l_ragged: n_seq sequences packed back to back (sequence s: tokens [start[s], start[s] + len[s])), each into
+    cache row row[s] (b2l_attention_ragged)."""
+    _fields_ = [("n_seq", c_int), ("row", c_int * RAGGED_MAX_SEQ), ("start", c_int * RAGGED_MAX_SEQ),
+                ("len", c_int * RAGGED_MAX_SEQ)]
+
 
 class LayerAffine(C.Structure):
     """b2l_layer_affine: the LLaMA-Adapter v2 affines of a Block's linears (c_fc12 interleaved like its weight rows)."""
@@ -188,6 +197,8 @@ _SIGS = {
                                       c_int, c_int, c_int, c_int, c_int, c_int, C.POINTER(AdapterPrefix), c_void_p]),
     "b2l_attention_nocache_adapter": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                               C.POINTER(AdapterPrefix), c_void_p]),
+    "b2l_attention_ragged": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, C.POINTER(Ragged), c_void_p, c_void_p, c_int,
+                                     c_int, c_int, c_int, c_int, c_int, C.POINTER(AdapterPrefix), c_void_p]),
     "b2l_lora_apply": (c_int, [C.POINTER(LoRA), c_void_p, c_int, c_void_p, c_float, c_void_p, c_int, c_int, c_int, c_int,
                                c_int, c_void_p]),
     "b2l_tp_buffer_bytes": (c_size_t, [c_int, c_int]),

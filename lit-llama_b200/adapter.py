@@ -144,10 +144,14 @@ class LLaMA(llama.LLaMA):
         super().expand_cache(B)
         self._prefix_views(B)
 
-    def prefill_rows(self, prompts, max_seq_length: int) -> torch.Tensor:
-        """model.LLaMA.prefill_rows; the prefix views follow B as in expand_cache."""
-        out = super().prefill_rows(prompts, max_seq_length)
-        self._prefix_views(len(prompts))
+    def refill_rows(self, prompts, rows, max_seq_length: int) -> torch.Tensor:
+        """model.LLaMA.refill_rows (prefill_rows too); the prefix store is brought up to date first, since the packed
+        prefill reads it, and the prefix views follow B as in expand_cache."""
+        self._check_prompts(prompts, max_seq_length, "refill_rows")
+        if self._adapter_layers() and (self._adapter_gen != WEIGHTS_GENERATION[0] or self._adapter_arr is None):
+            self._build_prefixes(1, prompts[0].device)
+        out = super().refill_rows(prompts, rows, max_seq_length)
+        self._prefix_views(self._kv_store.shape[2])
         return out
 
     def _prefix_views(self, B: int) -> None:

@@ -24,19 +24,39 @@ __global__ void ring_advance_rows_kernel(const int64_t* __restrict__ input_pos, 
   }
 }
 
+// Sequence of packed token bt of a ragged launch (b2l_attention_ragged): its cache row and its position in the sequence
+__device__ __forceinline__ void ragged_token(const b2l_ragged& rg, int bt, int& row, int& t) {
+  int s = 0;
+  while (s < rg.n_seq - 1 && bt >= rg.start[s] + rg.len[s]) ++s;
+  row = rg.row[s];
+  t = bt - rg.start[s];
+}
+
 // grid (B*T, n_head), block hs/2 threads (one per rotated pair).
 // q is rotated in place inside qkv; k (rotated) and v go to the cache (or, without a
 // cache, k is rotated in place as well).  pos_stride 1 (B2L_F_ROW_POS, T == 1): row b reads input_pos[b] and
 // ring_start[b]; 0: every row reads the shared entries.  rotate_q 0 (B2L_F_STEPWISE on the fused path): qkv is left
 // untouched and only the cache rows are written, since the fused kernel rotates q and its own key from qkv itself.
+// RAGGED (b2l_attention_ragged): grid (N, n_head); packed token bt is token t of the sequence that `rg` places at
+// [start, start + len), at position t in cache row `row`, whose ring offset restarts at 0 (the token-0 CTA of head 0
+// stores it; nothing here reads it).  input_pos, T and pos_stride are unused.
+template <bool RAGGED>
 __global__ void rope_append_kernel(__nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ k_cache,
                                    __nv_bfloat16* __restrict__ v_cache, const float* __restrict__ rope,
                                    const int64_t* __restrict__ input_pos, const int32_t* __restrict__ ring_start,
                                    int T, int n_head, int hs, int S, int block_size, int rope_rows, int pos_stride,
-                                   int rotate_q) {
-  const int bt = blockIdx.x, h = blockIdx.y, b = bt / T, t = bt % T;
+                                   int rotate_q, const __grid_constant__ b2l_ragged rg) {
+  const int bt = blockIdx.x, h = blockIdx.y;
+  int b, t;
+  if constexpr (RAGGED) {
+    ragged_token(rg, bt, b, t);
+    if (t == 0 && h == 0 && threadIdx.x == 0) const_cast<int32_t*>(ring_start)[b] = 0;   // never read by this kernel
+  } else {
+    b = bt / T;
+    t = bt % T;
+  }
   const int C = n_head * hs;
-  long long p = input_pos ? input_pos[b * pos_stride + t] : (long long)t;
+  long long p = (!RAGGED && input_pos) ? input_pos[b * pos_stride + t] : (long long)t;
   // rope_rows: `rope` already holds the T selected rows (reference call convention, model.py:93)
   const long long prow = rope_rows ? (long long)t : (p < block_size ? p : (long long)block_size - 1);
   __nv_bfloat16* q = qkv + (size_t)bt * 3 * C + h * hs;
@@ -45,7 +65,7 @@ __global__ void rope_append_kernel(__nv_bfloat16* __restrict__ qkv, __nv_bfloat1
   __nv_bfloat16 *kd = k, *vd = nullptr;
   if (k_cache != nullptr) {
     const int w = (int)(p < S ? p : (long long)S - 1);
-    const int phys = (w + ring_start[b * pos_stride]) % S;
+    const int phys = RAGGED ? w : (w + ring_start[b * pos_stride]) % S;
     const size_t off = (((size_t)b * n_head + h) * S + phys) * hs;
     kd = k_cache + off;
     vd = v_cache + off;
@@ -734,17 +754,44 @@ __device__ __forceinline__ void split_bf16x2(float x, float y, uint32_t& hi, uin
   lo = *reinterpret_cast<const uint32_t*>(&l);
 }
 
+// RAGGED (b2l_attention_ragged): grid (n_head, sum over sequences of ceil(len / 64)); blockIdx.y walks the (sequence,
+// 64-query tile) pairs in sequence order.  A CTA runs exactly what a B = 1, T = len launch runs for that tile: queries
+// at positions t0..t0+63 of the sequence (rows past its end repeat its last one), keys from slot 0 of its cache row,
+// no ring (the caller restarts the row's ring at 0).  input_pos and ring_start are unused; T is the sequence's length.
+template <bool RAGGED>
 __global__ void __launch_bounds__(128)
     attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, KvView kv, const int64_t* __restrict__ input_pos,
-                        const int32_t* __restrict__ ring_start, __nv_bfloat16* __restrict__ y, int T, int n_head) {
+                        const int32_t* __restrict__ ring_start, __nv_bfloat16* __restrict__ y, int T, int n_head,
+                        const __grid_constant__ b2l_ragged rg) {
   constexpr int HS = 128;
   extern __shared__ __align__(128) uint8_t psm[];
   const uint32_t sq = fd_smem_u32(psm), sk0 = sq + PF_TILE_BYTES;   // K tile of buffer b at sk0 + 2 b TILE, V tile right behind it
-  const int bh = blockIdx.x, b = bh / n_head, h = bh % n_head, t0 = blockIdx.y * PF_Q;
+  int b, h, t0;
+  size_t tok0 = 0;   // RAGGED: packed row of the sequence's token 0 in qkv and y
+  if constexpr (RAGGED) {
+    int s = 0, tile = blockIdx.y;
+    for (; s < rg.n_seq - 1; ++s) {   // prefix sums over <= 16 sequences
+      const int nt = (rg.len[s] + PF_Q - 1) / PF_Q;
+      if (tile < nt) break;
+      tile -= nt;
+    }
+    b = rg.row[s];
+    h = blockIdx.x;
+    t0 = tile * PF_Q;
+    T = rg.len[s];
+    tok0 = (size_t)rg.start[s];
+  } else {
+    const int bh = blockIdx.x;
+    b = bh / n_head;
+    h = bh % n_head;
+    t0 = blockIdx.y * PF_Q;
+  }
+  // packed row of the CTA's query t in qkv and y
+  auto tok = [&](int t) -> size_t { return RAGGED ? tok0 + t : (size_t)b * T + t; };
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t4 = lane & 3;
   const int C = n_head * HS;
   const int cap = kv.S > 0 ? kv.S : T;
-  const int ring = (kv.S > 0 && ring_start) ? *ring_start : 0;
+  const int ring = (!RAGGED && kv.S > 0 && ring_start) ? *ring_start : 0;
   const __nv_bfloat16* kb = kv.k + (size_t)b * kv.b_stride + (size_t)h * kv.h_stride;
   const __nv_bfloat16* vb = kv.v + (size_t)b * kv.b_stride + (size_t)h * kv.h_stride;
 
@@ -753,7 +800,7 @@ __global__ void __launch_bounds__(128)
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
     const int t = min(t0 + warp * 16 + g + 8 * i, T - 1);
-    const long long p = input_pos ? input_pos[t] : (long long)t;
+    const long long p = (!RAGGED && input_pos) ? input_pos[t] : (long long)t;
     Lrow[i] = (int)(p < cap ? p : (long long)cap - 1) + 1;
   }
   __shared__ int s_lmax;
@@ -764,7 +811,7 @@ __global__ void __launch_bounds__(128)
   for (int q = tid; q < PF_Q * 16; q += 128) {
     const int r = q >> 4, c = q & 15;
     const int t = min(t0 + r, T - 1);
-    pf_cp16(sq + (r * PF_LD + c * 8) * 2, qkv + ((size_t)b * T + t) * 3 * C + h * HS + c * 8);
+    pf_cp16(sq + (r * PF_LD + c * 8) * 2, qkv + tok(t) * 3 * C + h * HS + c * 8);
   }
   __syncthreads();
   const int Lmax = s_lmax;
@@ -889,7 +936,7 @@ __global__ void __launch_bounds__(128)
     const int t = t0 + warp * 16 + g + 8 * r;
     if (t < T) {
       const float inv = 1.0f / lrow[r];
-      __nv_bfloat16* dst = y + ((size_t)b * T + t) * C + h * HS + 2 * t4;
+      __nv_bfloat16* dst = y + tok(t) * C + h * HS + 2 * t4;
 #pragma unroll
       for (int n = 0; n < 16; ++n)
         *reinterpret_cast<__nv_bfloat162*>(dst + n * 8) = __floats2bfloat162_rn(o[n][2 * r] * inv, o[n][2 * r + 1] * inv);
@@ -914,8 +961,9 @@ static int launch_attn(const __nv_bfloat16* qkv, KvView kv, const int64_t* input
   static const int env_pf = [] { const char* e = getenv("B2L_ATTN_PREFILL"); return e ? atoi(e) : 1; }();
   if (hs == 128 && T > 1 && env_pf && !stepwise) {   // tiled tensor-core kernel (B2L_ATTN_PREFILL=0: the per-query path below)
     static DynSmemCache smem_cache;
-    if (int rc = ensure_dyn_smem(attn_prefill_kernel, PF_SMEM_BYTES, smem_cache)) return rc;
-    attn_prefill_kernel<<<dim3(B * n_head, (T + PF_Q - 1) / PF_Q), 128, PF_SMEM_BYTES, st>>>(qkv, kv, input_pos, ring_start, y, T, n_head);
+    if (int rc = ensure_dyn_smem(attn_prefill_kernel<false>, PF_SMEM_BYTES, smem_cache)) return rc;
+    attn_prefill_kernel<false><<<dim3(B * n_head, (T + PF_Q - 1) / PF_Q), 128, PF_SMEM_BYTES, st>>>(qkv, kv, input_pos, ring_start, y, T,
+                                                                                                    n_head, b2l_ragged{});
     B2L_LAUNCH_CHECK("attn_prefill_kernel");
     return 0;
   }
@@ -1019,9 +1067,9 @@ static int attention_impl(void* qkv, void* k_cache, void* v_cache, const void* r
     const int rows = step ? T : B;
     int* tickets = reinterpret_cast<int*>(reinterpret_cast<char*>(work) + ws_partials_bytes(rows, n_head, head_size, step ? 1 : T, S));
     if (step) {   // every new key / value row first, qkv untouched (the fused kernel rotates q and its own key itself)
-      rope_append_kernel<<<dim3(T, n_head), 64, 0, st>>>((__nv_bfloat16*)qkv, (__nv_bfloat16*)k_cache, (__nv_bfloat16*)v_cache,
+      rope_append_kernel<false><<<dim3(T, n_head), 64, 0, st>>>((__nv_bfloat16*)qkv, (__nv_bfloat16*)k_cache, (__nv_bfloat16*)v_cache,
                                                         (const float*)rope, input_pos, ring_start, T, n_head, head_size, S,
-                                                        block_size, 0, 0, 0);
+                                                        block_size, 0, 0, 0, b2l_ragged{});
       B2L_LAUNCH_CHECK("rope_append_kernel");
     }
     // B2L_ATTN_PRE (read once): sub-tiles requested before griddepcontrol.wait, 1 (default) or 2
@@ -1053,10 +1101,10 @@ static int attention_impl(void* qkv, void* k_cache, void* v_cache, const void* r
                       : launch(attn_decode_fused_kernel<true, false, false>, pre);
   }
   int rt = head_size / 2 < 32 ? 32 : head_size / 2;
-  rope_append_kernel<<<dim3(B * T, n_head), rt, 0, st>>>((__nv_bfloat16*)qkv, (__nv_bfloat16*)k_cache,
+  rope_append_kernel<false><<<dim3(B * T, n_head), rt, 0, st>>>((__nv_bfloat16*)qkv, (__nv_bfloat16*)k_cache,
                                                         (__nv_bfloat16*)v_cache, (const float*)rope, input_pos,
                                                         ring_start, T, n_head, head_size, S, block_size, (flags & B2L_F_ROPE_ROWS) ? 1 : 0,
-                                                        pos_stride, 1);
+                                                        pos_stride, 1, b2l_ragged{});
   B2L_LAUNCH_CHECK("rope_append_kernel");
   KvView kv{(const __nv_bfloat16*)k_cache, (const __nv_bfloat16*)v_cache, (size_t)n_head * S * head_size,
             (size_t)S * head_size, (size_t)head_size, S};
@@ -1099,8 +1147,8 @@ extern "C" int b2l_attention_adapter(void* qkv, void* k_cache, void* v_cache, co
 static int attention_nocache_impl(void* qkv, const void* rope, void* y, void* work, int B, int T, int n_head,
                                   int head_size, int block_size, cudaStream_t st) {
   int rt = head_size / 2 < 32 ? 32 : head_size / 2;
-  rope_append_kernel<<<dim3(B * T, n_head), rt, 0, st>>>((__nv_bfloat16*)qkv, nullptr, nullptr, (const float*)rope,
-                                                        nullptr, nullptr, T, n_head, head_size, 0, block_size, 0, 0, 1);
+  rope_append_kernel<false><<<dim3(B * T, n_head), rt, 0, st>>>((__nv_bfloat16*)qkv, nullptr, nullptr, (const float*)rope,
+                                                        nullptr, nullptr, T, n_head, head_size, 0, block_size, 0, 0, 1, b2l_ragged{});
   B2L_LAUNCH_CHECK("rope_append_kernel");
   const int C = n_head * head_size;
   const __nv_bfloat16* base = (const __nv_bfloat16*)qkv;
@@ -1128,6 +1176,50 @@ extern "C" int b2l_attention_nocache_adapter(void* qkv, const void* rope, void* 
   cudaStream_t st = (cudaStream_t)stream;
   if (int rc = attention_nocache_impl(qkv, rope, y, work, B, T, n_head, head_size, block_size, st)) return rc;
   return launch_adapter_prefix(qkv, prefix, y, B, T, n_head, head_size, st);
+}
+
+extern "C" int b2l_attention_ragged(void* qkv, void* k_cache, void* v_cache, const void* rope, const b2l_ragged* seqs,
+                                    int32_t* ring_start, void* y, int N, int B_rows, int n_head, int head_size, int S,
+                                    int block_size, const b2l_adapter_prefix* prefix, b2l_stream_t stream) {
+  B2L_CHECK_ARG(qkv && k_cache && v_cache && rope && seqs && ring_start && y, "b2l_attention_ragged: null pointer");
+  B2L_CHECK_ARG(N > 0 && B_rows > 0 && n_head > 0 && S > 0 && block_size > 0,
+                "b2l_attention_ragged: bad shape (N=%d, B_rows=%d, n_head=%d, S=%d, block_size=%d)", N, B_rows, n_head, S,
+                block_size);
+  B2L_CHECK_SUPPORTED(head_size == 128, "b2l_attention_ragged: head_size %d unsupported (128 only)", head_size);
+  const b2l_ragged& rg = *seqs;
+  B2L_CHECK_ARG(rg.n_seq >= 1 && rg.n_seq <= B2L_RAGGED_MAX_SEQ, "b2l_attention_ragged: n_seq %d outside 1..%d", rg.n_seq,
+                B2L_RAGGED_MAX_SEQ);
+  int next = 0, tiles = 0;
+  for (int s = 0; s < rg.n_seq; ++s) {
+    B2L_CHECK_ARG(rg.len[s] >= 1 && rg.len[s] <= S, "b2l_attention_ragged: sequence %d has length %d (1..S=%d)", s,
+                  rg.len[s], S);
+    B2L_CHECK_ARG(rg.start[s] == next, "b2l_attention_ragged: sequence %d starts at %d, not %d (starts must tile [0, N))",
+                  s, rg.start[s], next);
+    B2L_CHECK_ARG(rg.row[s] >= 0 && rg.row[s] < B_rows, "b2l_attention_ragged: sequence %d names row %d of %d", s,
+                  rg.row[s], B_rows);
+    for (int o = 0; o < s; ++o)
+      B2L_CHECK_ARG(rg.row[o] != rg.row[s], "b2l_attention_ragged: sequences %d and %d both name row %d", o, s, rg.row[s]);
+    next += rg.len[s];
+    tiles += (rg.len[s] + PF_Q - 1) / PF_Q;
+  }
+  B2L_CHECK_ARG(next == N, "b2l_attention_ragged: the sequences cover %d tokens, N=%d (starts must tile [0, N))", next, N);
+  if (prefix != nullptr) {
+    if (int rc = check_adapter_prefix(prefix, "b2l_attention_ragged")) return rc;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  rope_append_kernel<true><<<dim3(N, n_head), head_size / 2, 0, st>>>((__nv_bfloat16*)qkv, (__nv_bfloat16*)k_cache,
+                                                                      (__nv_bfloat16*)v_cache, (const float*)rope, nullptr,
+                                                                      ring_start, 0, n_head, head_size, S, block_size, 0,
+                                                                      0, 1, rg);
+  B2L_LAUNCH_CHECK("rope_append_kernel (ragged)");
+  KvView kv{(const __nv_bfloat16*)k_cache, (const __nv_bfloat16*)v_cache, (size_t)n_head * S * head_size,
+            (size_t)S * head_size, (size_t)head_size, S};
+  static DynSmemCache smem_cache;
+  if (int rc = ensure_dyn_smem(attn_prefill_kernel<true>, PF_SMEM_BYTES, smem_cache)) return rc;
+  attn_prefill_kernel<true><<<dim3(n_head, tiles), 128, PF_SMEM_BYTES, st>>>((const __nv_bfloat16*)qkv, kv, nullptr,
+                                                                             nullptr, (__nv_bfloat16*)y, 0, n_head, rg);
+  B2L_LAUNCH_CHECK("attn_prefill_kernel (ragged)");
+  return prefix == nullptr ? 0 : launch_adapter_prefix(qkv, prefix, y, 1, N, n_head, head_size, st);
 }
 
 extern "C" int b2l_kv_unroll(const void* cache, const int32_t* ring_start, void* out, int B, int n_head, int S,

@@ -6,7 +6,9 @@ CUDA-graph replay per token.  `generate_batch()` draws up to 16 samples of one p
 at once: one batch-1 prefill, then one batched decode step and one sampling launch per
 token for all samples.  `generate_prompts()` continues up to 16 different prompts at
 once: one batch-1 prefill per prompt into its row of the cache, then one batched decode
-step at per-row positions and one sampling launch per token.  `generate_speculative()`
+step at per-row positions and one sampling launch per token.  `generate_stream()` decodes any number of
+prompts on up to 16 rows, refilling each finished row with the next prompt while the others keep decoding
+(continuous batching).  `generate_speculative()`
 lets a small draft model propose up to 15 tokens that the model verifies in one
 step (speculative sampling); its greedy output is `generate()`'s token for token.
 `main()` mirrors the reference CLI with argparse
@@ -14,8 +16,9 @@ step (speculative sampling); its greedy output is `generate()`'s token for token
 import os
 import sys
 import time
+from collections import deque
 from pathlib import Path
-from typing import List, Optional
+from typing import List, Optional, Sequence, Union
 
 import torch
 
@@ -416,6 +419,123 @@ def generate_prompts(
     return [torch.cat((p.to(dtype), new[b, :n])) for b, (p, n) in enumerate(zip(prompts, ns))]
 
 
+@torch.no_grad()
+def generate_stream(
+    model: LLaMA,
+    prompts: List[torch.Tensor],
+    max_new_tokens: Union[int, Sequence[int]],
+    *,
+    batch_size: int = MAX_SAMPLES,
+    max_seq_length: Optional[int] = None,
+    temperature: float = 1.0,
+    top_k: Optional[int] = None,
+    eos_id: Optional[int] = None,
+    stats: Optional[dict] = None,
+) -> List[torch.Tensor]:
+    """Continuations of any number of prompts (1-D tensors of any lengths) on B = min(batch_size, len(prompts)) rows
+    (batch_size 1..16), refilling each finished row with the next prompt while the others keep decoding (continuous
+    batching): a list of 1-D tensors in input order, prompt i plus its new tokens (generate.py:20-91 per prompt).
+
+    `max_new_tokens` is one int for every prompt or one per prompt.  The first B prompts go through
+    `LLaMA.prefill_rows`.  Each later step is one batched model call with a (B, 1) `input_pos` and one sampling launch
+    for all rows; a row finishes when it has its prompt's `max_new_tokens` or draws `eos_id` (included).  The rows
+    that finish in a step take the next prompts in input order, all in one `LLaMA.refill_rows` call behind the next
+    step's model call, and their first tokens are drawn from the refill's logits in that step's sampling launch.  Once
+    no prompt is left, finished rows ride along and their tokens are dropped.  With `eos_id` the host reads the step's
+    eos hits (B flags) once per step; without it, it knows from the counts when each row finishes.
+    max_seq_length (S) defaults to min(max over prompts of T_i + new_i, block_size); each row takes the roll branch
+    (model.py:214-218) on its own, and a refill restarts its row's ring.
+
+    Draws are argmax(probs / q) of their row's probabilities (sample_token).  On the exact batched steps
+    (`q4_batch_step`, `w8_batch_step`) every row is bit-identical to the batch-1 model, so with top_k=1 prompt i gets
+    `generate(model, prompts[i], new_i, max_seq_length=S, top_k=1, eos_id=eos_id)` token for token, whichever row and
+    step admit it.  With len(prompts) <= batch_size and one `max_new_tokens` no row is refilled, and the output is
+    `generate_prompts`'s for the same seed.  `stats`, when given, receives "steps" (sampling launches), "refills"
+    (prompts admitted after the first prefill), "packed" / "alone" (prompts prefilled in a packed pass / one at a time,
+    LLaMA.refill_rows) and "idle_row_steps" (row-steps whose token was dropped).  The cache is left at B rows: call
+    `model.reset_cache()` before a batch-1 `generate()`."""
+    n = len(prompts)
+    if n == 0:
+        raise ValueError("generate_stream: no prompts")
+    if not 1 <= int(batch_size) <= MAX_SAMPLES:
+        raise ValueError(f"generate_stream: batch_size = {batch_size}; 1..{MAX_SAMPLES} (the batched decode step's range)")
+    for p in prompts:
+        if p.dim() != 1 or p.numel() == 0:
+            raise ValueError(f"generate_stream: every prompt must be a non-empty sequence of shape (T,), got {tuple(p.shape)}")
+    for p in prompts:
+        if not p.is_cuda:
+            raise RuntimeError(f"generate_stream: a prompt is on {p.device}; lit_llama_b200 runs on CUDA only (no CPU fallback)")
+    news = [int(max_new_tokens)] * n if isinstance(max_new_tokens, int) else [int(m) for m in max_new_tokens]
+    if len(news) != n or min(news) < 0:
+        raise ValueError(f"generate_stream: max_new_tokens must be one int >= 0, or one per prompt ({n}), got {max_new_tokens}")
+    Ts = [p.numel() for p in prompts]
+    S = max_seq_length
+    if S is None:
+        S = min(max(T + m for T, m in zip(Ts, news)), model.config.block_size)
+    if max(Ts) > S:
+        raise ValueError(f"generate_stream: a prompt of {max(Ts)} tokens is longer than max_seq_length={S}")
+    st = {} if stats is None else stats
+    st.update(steps=0, refills=0, packed=0, alone=0, idle_row_steps=0)
+    device, dtype = prompts[0].device, prompts[0].dtype
+    queue = deque(i for i in range(n) if news[i] > 0)
+    if not queue:
+        return [p.clone() for p in prompts]
+
+    def admit(ids: List[int]) -> None:
+        k = len(model._pack_plan([Ts[i] for i in ids]))
+        st["packed"] += k
+        st["alone"] += len(ids) - k
+
+    B = min(int(batch_size), len(queue))
+    serving: List[Optional[int]] = [queue.popleft() for _ in range(B)]   # the prompt each row decodes (None: idle)
+    done = [0] * n                          # new tokens prompt i has so far
+    first, row_of = [0] * n, [0] * n        # the step that drew prompt i's first token, and its row
+    hist = []                               # every step's (B,) tokens
+    pending = []                            # (row, prompt): refilled behind the next step's model call
+    input_pos = torch.tensor([Ts[i] for i in serving], dtype=torch.int64, device=device).view(B, 1)
+    admit(serving)
+    step = 0
+    while True:
+        if step == 0:
+            rows = model.prefill_rows([prompts[i] for i in serving], S)
+        else:
+            rows = model(x, S, input_pos)[:, -1]
+            input_pos = input_pos + 1
+            if pending:   # the finished rows rode along in that call; now they take their new prompts
+                ids = [i for _, i in pending]
+                admit(ids)
+                ridx = torch.tensor([r for r, _ in pending], device=device)
+                rows[ridx] = model.refill_rows([prompts[i] for i in ids], [r for r, _ in pending], S)
+                input_pos[ridx] = torch.tensor([Ts[i] for i in ids], dtype=torch.int64, device=device).view(-1, 1)
+                st["refills"] += len(ids)
+                pending = []
+        if torch.multinomial is _TORCH_MULTINOMIAL:
+            idx_next = sample_token(rows, temperature, top_k).to(dtype=dtype)   # one RNG draw + one launch for all rows
+        else:
+            # torch.multinomial has been replaced (as in generate()): keep calling it, on the fused [B, V] probabilities
+            idx_next = torch.multinomial(sample_probs(rows, temperature, top_k), num_samples=1).view(B).to(dtype=dtype)
+        hist.append(idx_next)
+        x = idx_next.view(B, 1)
+        hits = (idx_next == eos_id).tolist() if eos_id is not None else None   # the step's one host read
+        for b, i in enumerate(serving):
+            if i is None:
+                st["idle_row_steps"] += 1
+                continue
+            if done[i] == 0:
+                first[i], row_of[i] = step, b
+            done[i] += 1
+            if done[i] == news[i] or (hits is not None and hits[b]):
+                serving[b] = queue.popleft() if queue else None
+                if serving[b] is not None:
+                    pending.append((b, serving[b]))
+        step += 1
+        if all(i is None for i in serving):
+            break
+    st["steps"] = step
+    H = torch.stack(hist)
+    return [torch.cat((p.to(dtype), H[first[i]:first[i] + done[i], row_of[i]])) for i, p in enumerate(prompts)]
+
+
 def main(
     prompt: str = "Hello, my name is",
     *,
@@ -431,11 +551,13 @@ def main(
     draft_checkpoint_path: Optional[Path] = None,
     draft_quantize: Optional[str] = None,
     num_draft: int = 4,
+    stream: bool = False,
 ) -> None:
     """generate.py:94-155 without Fabric: bf16 on cuda:0, same prints on stderr.  `batch_size` > 1 draws the samples
     in groups of up to `batch_size` (at most 16) through `generate_batch`, on the model's exact batched decode step.
     `prompts_file` (one prompt per line) replaces `prompt`: the prompts are decoded in groups of `batch_size` through
-    `generate_prompts`, `num_samples` times each.  `draft_checkpoint_path` (with `draft_quantize`) loads a draft model
+    `generate_prompts`, `num_samples` times each; with `stream` they go through `generate_stream` on `batch_size` rows,
+    each finished row taking the next prompt.  `draft_checkpoint_path` (with `draft_quantize`) loads a draft model
     and decodes each sample with `generate_speculative`, `num_draft` draft tokens per round."""
     if not 1 <= batch_size <= MAX_SAMPLES:
         raise ValueError(f"batch_size = {batch_size}; 1..{MAX_SAMPLES}")
@@ -493,6 +615,20 @@ def main(
         prompts = [torch.tensor([sp.bos_id()] + sp.encode(ln), dtype=torch.int, device=device) for ln in lines]
         k = 0
         for _ in range(num_samples):
+            if stream:
+                k += 1
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                ys = generate_stream(model, prompts, max_new_tokens, batch_size=batch_size, temperature=temperature,
+                                     top_k=top_k)
+                torch.cuda.synchronize()
+                t = time.perf_counter() - t0
+                model.reset_cache()
+                for y in ys:
+                    print(sp.decode(y.tolist()))
+                tokens_generated = sum(y.size(0) - p.size(0) for y, p in zip(ys, prompts))
+                print(f"Time for inference {k}: {t:.02f} sec total, {tokens_generated / t:.02f} tokens/sec", file=sys.stderr)
+                continue
             for first in range(0, len(prompts), batch_size):
                 group = prompts[first:first + batch_size]
                 k += 1
@@ -555,6 +691,9 @@ def cli() -> None:
                          "with --prompts_file, prompts decoded together per generate_prompts call")
     ap.add_argument("--prompts_file", type=Path, default=None,
                     help="a text file of prompts, one per line, decoded in groups of --batch_size (replaces --prompt)")
+    ap.add_argument("--stream", action="store_true",
+                    help="with --prompts_file: decode the whole file through generate_stream on --batch_size rows, each "
+                         "finished row taking the next prompt (continuous batching)")
     ap.add_argument("--draft_checkpoint_path", type=Path, default=None,
                     help="a smaller model's checkpoint: decode with generate_speculative, this model proposing tokens")
     ap.add_argument("--draft_quantize", default=None, choices=[None, "llm.int8", "gptq.int4", "gptq.int8"])
@@ -562,6 +701,8 @@ def cli() -> None:
     a = ap.parse_args()
     if a.draft_checkpoint_path is not None and (a.batch_size != 1 or a.prompts_file is not None):
         ap.error("--draft_checkpoint_path decodes one sequence at a time (batch_size 1, no prompts_file)")
+    if a.stream and a.prompts_file is None:
+        ap.error("--stream decodes a --prompts_file")
     main(**vars(a))
 
 

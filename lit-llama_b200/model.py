@@ -155,10 +155,13 @@ class CausalSelfAttention(nn.Module):
         kv_cache: Optional[KVCache] = None,
         *,
         _rope_is_table: bool = False,
+        _ragged: Optional[L.Ragged] = None,
     ) -> Tuple[torch.Tensor, Optional[KVCache]]:
         """`mask` is accepted for signature parity and ignored: the kernel derives the
         causal mask from input_pos exactly as model.py:94-96 builds it from tril.  A 2-D input_pos of shape (B, 1)
-        puts each row's one token at its own position, with its own ring offset (B2L_F_ROW_POS)."""
+        puts each row's one token at its own position, with its own ring offset (B2L_F_ROW_POS).  `_ragged`
+        (LLaMA.refill_rows): x (1, N, C) holds the packed prompts it describes, each prefilled into its own row of
+        kv_cache at positions 0.. (b2l_attention_ragged; input_pos is ignored)."""
         L.require_cuda_bf16(x, "CausalSelfAttention.forward")
         B, T, C_ = x.size()
         hs = C_ // self.n_head
@@ -170,7 +173,14 @@ class CausalSelfAttention(nn.Module):
         rope32 = rope if rope.dtype == torch.float32 else rope.float()
         rope32 = rope32.contiguous()
         prefix = self._adapter_prefix(kv_cache is not None)   # LLaMA-Adapter layers only (adapter.py)
-        if kv_cache is None:
+        if _ragged is not None:
+            cache_k, cache_v = kv_cache
+            rc = lib.b2l_attention_ragged(qkv.data_ptr(), cache_k.data_ptr(), cache_v.data_ptr(), rope32.data_ptr(),
+                                          C.byref(_ragged), self._ring.data_ptr(), y.data_ptr(), B * T, cache_k.shape[0],
+                                          self.n_head, hs, cache_k.shape[2], rope32.shape[0],
+                                          None if prefix is None else C.byref(prefix), L.stream_ptr())
+            L.check(rc, "b2l_attention_ragged")
+        elif kv_cache is None:
             work = torch.empty(lib.b2l_attn_workspace_bytes(B, self.n_head, hs, T, T) // 4 + 1, device=x.device, dtype=torch.float32)
             rows = rope32 if not _rope_is_table else rope32[:T]
             if prefix is None:
@@ -572,43 +582,142 @@ class LLaMA(nn.Module):
         self._decode, self._module_graph = None, None   # they point at the old ring
         self._verify = {}
 
+    @staticmethod
+    def _check_prompts(prompts: List[torch.Tensor], max_seq_length: int, who: str) -> None:
+        if not 1 <= len(prompts) <= 16:
+            raise ValueError(f"{who}: {len(prompts)} prompts; 1..16 (the batched decode step's range)")
+        for p in prompts:
+            if p.dim() != 1 or p.numel() == 0:
+                raise ValueError(f"{who}: every prompt must be a non-empty 1-D token tensor, got {tuple(p.shape)}")
+            if not p.is_cuda:
+                raise RuntimeError(f"{who}: prompt is on {p.device}; lit_llama_b200 runs on CUDA only (no CPU fallback)")
+            if p.numel() > max_seq_length:
+                raise ValueError(f"{who}: a prompt of {p.numel()} tokens does not fit max_seq_length={max_seq_length}")
+
     @torch.no_grad()
     def prefill_rows(self, prompts: List[torch.Tensor], max_seq_length: int) -> torch.Tensor:
         """Prefill 1..16 different prompts (1-D token tensors of any lengths <= max_seq_length) into one B-row KV cache
         and return each prompt's last-position logits, (B, vocab).
 
-        Each prompt runs through the batch-1 prefill, writing straight into its row of the B-row store, so row b's
-        cache is bit for bit the one `generate()` builds for that prompt (the work is the sum of the prompt lengths; a
-        padded (B, T_max) prefill would cost more and would round differently).  The ring offsets start per row at
-        zero: the next step passes a (B, 1) `input_pos`, row b's first new token at position len(prompts[b])."""
-        B = len(prompts)
-        if not 1 <= B <= 16:
-            raise ValueError(f"prefill_rows: {B} prompts; 1..16 (the batched decode step's range)")
-        for p in prompts:
-            if p.dim() != 1 or p.numel() == 0:
-                raise ValueError(f"prefill_rows: every prompt must be a non-empty 1-D token tensor, got {tuple(p.shape)}")
-            if not p.is_cuda:
-                raise RuntimeError(f"prefill_rows: prompt is on {p.device}; lit_llama_b200 runs on CUDA only (no CPU fallback)")
-            if p.numel() > max_seq_length:
-                raise ValueError(f"prefill_rows: a prompt of {p.numel()} tokens does not fit max_seq_length={max_seq_length}")
-        cfg = self.config
-        dev = prompts[0].device
+        A fresh B-row cache, then `refill_rows(prompts, range(B), max_seq_length)`: row b's cache is bit for bit the one
+        `generate()` builds for prompts[b] (no padded (B, T_max) prefill, which would cost more and round
+        differently).  The ring offsets start per row at zero: the next step passes a (B, 1) `input_pos`, row b's first
+        new token at position len(prompts[b])."""
+        self._check_prompts(prompts, max_seq_length, "prefill_rows")
+        B, cfg, dev = len(prompts), self.config, prompts[0].device
         self.reset_cache()
-        store = torch.zeros((cfg.n_layer, 2, B, cfg.n_head, max_seq_length, cfg.n_embd // cfg.n_head), device=dev,
-                            dtype=torch.bfloat16)
-        last = []
-        for b, p in enumerate(prompts):
-            if self._ring is not None:
-                self._ring.zero_()
-            self._kv_store = store[:, :, b:b + 1]
-            self.kv_caches = [(store[i, 0, b:b + 1], store[i, 1, b:b + 1]) for i in range(cfg.n_layer)]   # contiguous
-            self._decode, self._module_graph = None, None   # a one-token prompt's step state points at the last row
-            self._verify = {}
-            last.append(self(p.view(1, -1), max_seq_length, torch.arange(p.numel(), device=dev))[0, -1].clone())
-        self._kv_store = store
-        self.kv_caches = [(store[i, 0], store[i, 1]) for i in range(cfg.n_layer)]
+        self._prepare(prompts[0].view(1, -1), max_seq_length)
+        self._kv_store = torch.zeros((cfg.n_layer, 2, B, cfg.n_head, max_seq_length, cfg.n_embd // cfg.n_head),
+                                     device=dev, dtype=torch.bfloat16)
+        self.kv_caches = [(self._kv_store[i, 0], self._kv_store[i, 1]) for i in range(cfg.n_layer)]
         self._set_ring(torch.zeros(B, dtype=torch.int32, device=dev))
-        return torch.stack(last)
+        return self.refill_rows(prompts, range(B), max_seq_length)
+
+    @torch.no_grad()
+    def refill_rows(self, prompts: List[torch.Tensor], rows, max_seq_length: int) -> torch.Tensor:
+        """Prefill prompts[i] into row rows[i] of the existing B-row KV cache (prefill_rows) and return each prompt's
+        last-position logits, (n, vocab): row rows[i] then holds, bit for bit, the cache `generate()` builds for
+        prompts[i], with its ring offset at zero, and its next token goes in at position len(prompts[i]).
+
+        The prompts `_pack_plan` admits run through ONE packed prefill (M = sum of their lengths on every linear, the
+        ragged attention b2l_attention_ragged, lm_head on their last rows only); each of the others runs the batch-1
+        prefill into its row ("alone").  Other rows keep their cache contents, positions and ring offsets, and the
+        B-row decode state and its CUDA graph stay the same objects (the KV store and the ring tensor change in place),
+        so a decode loop can refill finished rows between two steps (generate_stream)."""
+        rows = [int(r) for r in rows]
+        self._check_prompts(prompts, max_seq_length, "refill_rows")
+        store = self._kv_store
+        if store is None or self._ring is None or self._ring.numel() != store.shape[2]:
+            raise RuntimeError("refill_rows: no B-row KV cache to refill (prefill_rows builds one)")
+        B = store.shape[2]
+        if len(rows) != len(prompts) or len(set(rows)) != len(rows) or not all(0 <= r < B for r in rows):
+            raise ValueError(f"refill_rows: rows {rows} must name {len(prompts)} distinct rows of 0..{B - 1}")
+        if store.shape[4] != max_seq_length:
+            raise ValueError(f"refill_rows: max_seq_length={max_seq_length} against a cache of {store.shape[4]}")
+        self._prepare(prompts[0].view(1, -1), max_seq_length)
+        packed = self._pack_plan([p.numel() for p in prompts])
+        out: List[Optional[torch.Tensor]] = [None] * len(prompts)
+        if packed:
+            logits = self._prefill_packed([prompts[i] for i in packed], [rows[i] for i in packed], max_seq_length)
+            for j, i in enumerate(packed):
+                out[i] = logits[j]
+        alone = [i for i in range(len(prompts)) if i not in packed]
+        for i, lg in zip(alone, self._prefill_alone([prompts[i] for i in alone], [rows[i] for i in alone], max_seq_length)):
+            out[i] = lg
+        return torch.stack(out)
+
+    def _linears(self) -> List[nn.Module]:
+        lins = [self.lm_head]
+        for blk in self.transformer.h:
+            lins += [blk.attn.c_attn, blk.attn.c_proj, blk.mlp.c_fc1, blk.mlp.c_fc2, blk.mlp.c_proj]
+        return lins
+
+    def _pack_plan(self, lengths: List[int]) -> List[int]:
+        """Indices of the prompts (given by length) that refill_rows prefills packed: those whose own batch-1 prefill
+        runs every linear on the same row-exact kernel as the pack does (quantization.packs_at), so each keeps its
+        batch-1 bits; [] for head sizes other than 128 (the ragged attention's) and for models with any linear outside
+        that dispatch (dense, llm.int8, whose rows interact through the batch outlier mask)."""
+        from .quantization import packs_at
+
+        cfg = self.config
+        if cfg.n_embd // cfg.n_head != 128:
+            return []
+        lins = self._linears()
+        cand = [i for i, T in enumerate(lengths) if packs_at(lins, T, T)]
+        N = sum(lengths[i] for i in cand)
+        if not all(packs_at(lins, lengths[i], N) for i in cand):
+            return []
+        return cand
+
+    def _prefill_packed(self, prompts: List[torch.Tensor], rows: List[int], max_seq_length: int) -> torch.Tensor:
+        """The packed prefill of refill_rows: the prompts back to back as one (1, N) sequence through the module path
+        at M = N, the attention ragged (each prompt into its row at positions 0..), lm_head on each prompt's last row
+        on the kernel its batch-1 prefill ran it on at M = len (the GEMM, not the 2..16-row kernel M = n would pick)."""
+        from .quantization import kernel_at
+
+        seqs = L.Ragged()
+        seqs.n_seq = len(prompts)
+        N = 0
+        for j, (p, r) in enumerate(zip(prompts, rows)):
+            seqs.row[j], seqs.start[j], seqs.len[j] = r, N, p.numel()
+            N += p.numel()
+        dev = prompts[0].device
+        toks = torch.cat([p.to(torch.int64) for p in prompts]).view(1, N)
+        h = self._forward_hidden(toks, max_seq_length, None, ragged=seqs)
+        last = torch.tensor([seqs.start[j] + seqs.len[j] - 1 for j in range(len(prompts))], device=dev)
+        x = h[0].index_select(0, last)
+        y = self.lm_head.run(x, kernel_at(self.lm_head, N))
+        aff = affine_of(self.lm_head)
+        if aff is not None:   # LLaMA-Adapter v2: the affine its forward applies after the linear
+            from .adapter_v2 import linear_affine
+
+            linear_affine(y, *aff)
+        return y
+
+    def _prefill_alone(self, prompts: List[torch.Tensor], rows: List[int], max_seq_length: int) -> List[torch.Tensor]:
+        """The batch-1 prefill of each prompt into its row: the model is pointed at that row of the KV store and its
+        ring offset (ring[r:r+1], zeroed) for the call, and the B-row decode state and module graph are put back after
+        (a one-token prompt runs, and replaces, the batch-1 step state)."""
+        ring, store, caches = self._ring, self._kv_store, self.kv_caches
+        decode, module_graph = self._decode, self._module_graph
+        out = []
+        try:
+            for p, r in zip(prompts, rows):
+                one = ring[r:r + 1]
+                one.zero_()
+                self._ring = one
+                for blk in self.transformer.h:
+                    blk.attn._ring = one
+                self._kv_store = store[:, :, r:r + 1]
+                self.kv_caches = [(self._kv_store[i, 0], self._kv_store[i, 1]) for i in range(self.config.n_layer)]   # contiguous
+                self._decode, self._module_graph = None, None
+                out.append(self(p.view(1, -1), max_seq_length, torch.arange(p.numel(), device=p.device))[0, -1].clone())
+        finally:
+            self._ring, self._kv_store, self.kv_caches = ring, store, caches
+            for blk in self.transformer.h:
+                blk.attn._ring = ring
+            self._decode, self._module_graph = decode, module_graph
+        return out
 
     def expand_cache(self, B: int) -> None:
         """Broadcast a batch-1 KV cache to B rows: every row then holds the prompt's keys and values, so B samples of one
@@ -966,9 +1075,10 @@ class LLaMA(nn.Module):
         """Prefill, no-cache forward and non-fused decode: one kernel (or two) per reference module."""
         return self.lm_head(self._forward_hidden(idx, max_seq_length, input_pos))  # (b, t, vocab_size)
 
-    def _forward_hidden(self, idx: torch.Tensor, max_seq_length: int, input_pos: Optional[torch.Tensor]) -> torch.Tensor:
+    def _forward_hidden(self, idx: torch.Tensor, max_seq_length: int, input_pos: Optional[torch.Tensor],
+                        ragged: Optional[L.Ragged] = None) -> torch.Tensor:
         """_forward_modules up to lm_head's input: the embedding, the Blocks and ln_f (lit_llama_b200.evaluate runs
-        lm_head with the loss in its epilogue instead)."""
+        lm_head with the loss in its epilogue instead).  `ragged`: idx (1, N) holds the packed prompts of refill_rows."""
         B, T = idx.size()
         x = torch.empty((B, T, self.config.n_embd), device=idx.device, dtype=torch.bfloat16)
         wte = self.transformer.wte.weight
@@ -981,7 +1091,11 @@ class LLaMA(nn.Module):
                                    B * T, self.config.n_embd, wte.shape[0], L.stream_ptr())
         L.check(rc, "b2l_embedding")
 
-        if input_pos is None:  # proxy for use_cache=False (model.py:104-106)
+        if ragged is not None:
+            for i, block in enumerate(self.transformer.h):
+                x, _ = block(x, self.rope_cache, None, max_seq_length, None, self.kv_caches[i], _rope_is_table=True,
+                             _ragged=ragged)
+        elif input_pos is None:  # proxy for use_cache=False (model.py:104-106)
             for block in self.transformer.h:
                 x, _ = block(x, self.rope_cache, None, max_seq_length, _rope_is_table=True)
         else:

@@ -254,7 +254,30 @@ class ColBlockQuantizedLinear(torch.nn.Module):
         """gptq.int8 on the batch-1 kernel (M == 1): w8_capable and K <= 24576."""
         return self.w8_capable and self.in_features <= 24576
 
+    def kernel_at(self, M: int, aligned: bool = True) -> str:
+        """The kernel `forward` runs for M activation rows (`aligned`: the rows are 16-byte aligned, their stride a
+        multiple of 8 elements, as a contiguous input's are).  The one place this dispatch policy lives: `forward`
+        and the packed prefill (LLaMA.refill_rows, which packs a prompt only where this answer is the same at its own
+        length and at the pack's) both ask it."""
+        if self.w8_gemv_capable and aligned and M == 1:
+            return "w8_gemv"
+        if self.w8_capable and aligned:
+            return "w8_gemm"
+        if self.gemv_capable and aligned and M == 1:
+            return "q4_gemv"
+        if self.gemv_capable and aligned and M <= 8 and BATCH_GEMV:
+            return "q4_gemv_batch"
+        if self.tc_capable and aligned and M <= 16:
+            return "q4_linear_tc"
+        if self.tc_capable and aligned and self.in_features % 64 == 0:
+            return "q4_gemm"
+        return "q_linear"
+
     def forward(self, inp):
+        return self.run(inp)
+
+    def run(self, inp, kernel: Optional[str] = None):
+        """forward on `kernel` (a `kernel_at` answer the input qualifies for), or on `kernel_at`'s choice (None)."""
         L.require_cuda_bf16(inp, "ColBlockQuantizedLinear.forward")
         if self.scales.device != inp.device:
             raise RuntimeError("input and quant_weight are on different devices")
@@ -268,16 +291,18 @@ class ColBlockQuantizedLinear(torch.nn.Module):
         if M == 0:
             return y.reshape(*shape[:-1], N)
         aligned = x.data_ptr() % 16 == 0 and x.stride(0) % 8 == 0
+        if kernel is None:
+            kernel = self.kernel_at(M, aligned)
         # `wt` keeps a transient tiling (released layers) alive until its launch is enqueued; the caching allocator
         # hands freed blocks out in stream order, so the kernel has finished before anybody else writes there
-        if self.w8_gemv_capable and aligned and M == 1:
+        if kernel in ("w8_gemv", "q4_gemv"):
             wt = self.tiled_i8()
             a = L.Q4LinearArgs(
                 x=x.data_ptr(), ldx=x.stride(0), qw_tiled=wt.data_ptr(), scales=self.scales.data_ptr(),
                 zeros=self.zeros.data_ptr(), sz_dtype=L.sz_dtype_of(self.scales), y=y.data_ptr(), ldy=N, M=1, N=N, K=K,
                 prologue=L.PRO_NONE, norm_scale=None, eps=0.0, epilogue=L.EPI_STORE, res=None, ldres=0, split_k=0, flags=0)
-            L.check(L.lib().b2l_w8_gemv(C.byref(a), L.stream_ptr()), "b2l_w8_gemv")
-        elif self.w8_capable and aligned:
+            L.check(getattr(L.lib(), "b2l_" + kernel)(C.byref(a), L.stream_ptr()), "b2l_" + kernel)
+        elif kernel == "w8_gemm":
             # the wgmma GEMM reads quant_weight in the reference layout (a compacted layer rebuilds it transiently)
             self._check_layout()
             wt = self.reference_quant_weight()
@@ -287,14 +312,7 @@ class ColBlockQuantizedLinear(torch.nn.Module):
                 M=M, N=N, K=K, prologue=L.PRO_NONE, norm_scale=None, eps=0.0, epilogue=L.EPI_STORE, res=None,
                 ldres=0, split_k=0, flags=0)
             L.check(L.lib().b2l_w8_gemm(C.byref(a), L.stream_ptr()), "b2l_w8_gemm")
-        elif self.gemv_capable and aligned and M == 1:
-            wt = self.tiled_i8()
-            a = L.Q4LinearArgs(
-                x=x.data_ptr(), ldx=x.stride(0), qw_tiled=wt.data_ptr(), scales=self.scales.data_ptr(),
-                zeros=self.zeros.data_ptr(), sz_dtype=L.sz_dtype_of(self.scales), y=y.data_ptr(), ldy=N, M=1, N=N, K=K,
-                prologue=L.PRO_NONE, norm_scale=None, eps=0.0, epilogue=L.EPI_STORE, res=None, ldres=0, split_k=0, flags=0)
-            L.check(L.lib().b2l_q4_gemv(C.byref(a), L.stream_ptr()), "b2l_q4_gemv")
-        elif self.gemv_capable and aligned and M <= 8 and BATCH_GEMV:
+        elif kernel == "q4_gemv_batch":
             # 2..8 rows: the mma.sync tile has 8 columns, one per row (csrc/q4_gemv_batch.cu)
             wt = self.tiled_mma()
             a = L.Q4LinearArgs(
@@ -303,24 +321,16 @@ class ColBlockQuantizedLinear(torch.nn.Module):
                 prologue=L.PRO_NONE, norm_scale=None, eps=0.0, epilogue=L.EPI_STORE, res=None, ldres=0, split_k=0, flags=0,
                 workspace=batch_workspace(inp.device, K).data_ptr())
             L.check(L.lib().b2l_q4_gemv_batch(C.byref(a), L.stream_ptr()), "b2l_q4_gemv_batch")
-        elif self.tc_capable and aligned and M <= 16:
+        elif kernel in ("q4_linear_tc", "q4_gemm"):
+            # q4_gemm: prefill-shaped, 128 x 128 wgmma tiles, weights dequantised on the fly with get_weight's roundings
             wt = self.tiled()
             a = L.Q4LinearArgs(
                 x=x.data_ptr(), ldx=x.stride(0), qw_tiled=wt.data_ptr(), scales=self.scales.data_ptr(),
                 zeros=self.zeros.data_ptr(), sz_dtype=L.sz_dtype_of(self.scales), y=y.data_ptr(), ldy=N,
                 M=M, N=N, K=K, prologue=L.PRO_NONE, norm_scale=None, eps=0.0, epilogue=L.EPI_STORE, res=None,
                 ldres=0, split_k=0, flags=0)
-            L.check(L.lib().b2l_q4_linear_tc(C.byref(a), L.stream_ptr()), "b2l_q4_linear_tc")
-        elif self.tc_capable and aligned and K % 64 == 0:
-            # prefill-shaped: 128 x 128 wgmma tiles, weights dequantised on the fly with get_weight's roundings
-            wt = self.tiled()
-            a = L.Q4LinearArgs(
-                x=x.data_ptr(), ldx=x.stride(0), qw_tiled=wt.data_ptr(), scales=self.scales.data_ptr(),
-                zeros=self.zeros.data_ptr(), sz_dtype=L.sz_dtype_of(self.scales), y=y.data_ptr(), ldy=N,
-                M=M, N=N, K=K, prologue=L.PRO_NONE, norm_scale=None, eps=0.0, epilogue=L.EPI_STORE, res=None,
-                ldres=0, split_k=0, flags=0)
-            L.check(L.lib().b2l_q4_gemm(C.byref(a), L.stream_ptr()), "b2l_q4_gemm")
-        else:
+            L.check(getattr(L.lib(), "b2l_" + kernel)(C.byref(a), L.stream_ptr()), "b2l_" + kernel)
+        elif kernel == "q_linear":
             self._check_layout()
             qw = self.reference_quant_weight()
             rc = L.lib().b2l_q_linear(x.data_ptr(), x.stride(0), qw.data_ptr(), self.scales.data_ptr(),
@@ -328,7 +338,31 @@ class ColBlockQuantizedLinear(torch.nn.Module):
                                       None if self.bias is None else self.bias.to(inp.dtype).data_ptr(), y.data_ptr(), N,
                                       M, N, K, self.bits, self.tile_cols, L.stream_ptr())
             L.check(rc, "b2l_q_linear")
+        else:
+            raise ValueError(f"ColBlockQuantizedLinear: unknown kernel {kernel!r}")
         return y.reshape(*shape[:-1], N)
+
+
+#: kernels each of whose output rows depends on its own activation row and the weights only, whatever M is and
+#: wherever the row falls in a tile (fixed 128 x 128 tiles, no split-K): prompts packed into one launch of these keep
+#: the bits of their own batch-1 prefill
+ROW_EXACT_KERNELS = ("q4_gemm", "w8_gemm")
+
+
+def kernel_at(lin: torch.nn.Module, M: int) -> Optional[str]:
+    """The kernel a linear runs for M contiguous activation rows (ColBlockQuantizedLinear.kernel_at), or None for a
+    linear without that dispatch (dense, llm.int8: never packed)."""
+    return lin.kernel_at(M) if isinstance(lin, ColBlockQuantizedLinear) else None
+
+
+def packs_at(linears, T: int, N: int) -> bool:
+    """Whether a T-token prompt may join a packed prefill of N tokens: its own batch-1 prefill at M = T runs every one
+    of `linears` on the same row-exact kernel as the pack at M = N."""
+    for lin in linears:
+        k = kernel_at(lin, T)
+        if k not in ROW_EXACT_KERNELS or kernel_at(lin, N) != k:
+            return False
+    return True
 
 
 def tile_i8(qw: torch.Tensor, N: int, K: int, bits: int) -> torch.Tensor:
