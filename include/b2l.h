@@ -155,10 +155,15 @@ enum {
                            input_pos is int64[B] (row b's token is at input_pos[b]) and ring_start int32[B] (row b's
                            own ring offset); not with B2L_F_ROPE_ROWS or a persistent plan.  The step advances each
                            row's ring on its own (b2l_ring_advance_rows) */
-  B2L_F_STEPWISE = 2048 /* b2l_attention(_adapter) at B == 1, T = 2..16, and b2l_decode_step with B = 2..16: the rows
+  B2L_F_STEPWISE = 2048, /* b2l_attention(_adapter) at B == 1, T = 2..16, and b2l_decode_step with B = 2..16: the rows
                            are consecutive tokens of ONE sequence (the verify step of speculative decoding), each
                            computed exactly as a T == 1 launch / a batch-1 step at its position would compute it.
                            See b2l_attention and b2l_decode_step; not with B2L_F_ROW_POS or B2L_F_ROPE_ROWS */
+  B2L_F_GEMM_I8 = 4096, /* b2l_q4_gemm(_nll) / b2l_w8_gemm(_nll): qw_tiled is the batch-1 tiling of the layer,
+                           b2l_q4_tile_i8 / b2l_w8_tile_i8 of its N rows (see b2l_q4_gemm) */
+  B2L_F_GEMM_I8_LO = 8192,  /* with B2L_F_GEMM_I8: qw_tiled is a 2N-row interleaved b2l_*_tile_i8 tiling and the layer
+                           is rows 0..7 of its every 16-row block (c_fc1 of the fc1|fc2 tiling); N % 8 == 0 */
+  B2L_F_GEMM_I8_HI = 16384  /* the same, rows 8..15 of every 16-row block (c_fc2) */
 };
 
 /* Fused [RMSNorm ->] int4 linear [-> residual | SwiGLU] on wgmma (M <= 16).  Replaces
@@ -171,7 +176,16 @@ int b2l_q4_linear_tc(const b2l_q4_linear_args* args, b2l_stream_t stream);
  * 128 x 128 output tile per CTA, both operands from shared memory (producer warps dequantise the packed levels with
  * the reference's own bf16 roundings, so the tensor core multiplies exactly get_weight()'s matrix), fp32 accumulators
  * in registers.  Same argument block as b2l_q4_linear_tc; qw_tiled from b2l_q4_tile; prologue / epilogue must be
- * NONE / STORE; K % 64 == 0; ldx % 8 == 0.  Replaces quantization.py:187-333 (Triton tile kernel) / :413-423. */
+ * NONE / STORE; K % 64 == 0; ldx % 8 == 0.  Replaces quantization.py:187-333 (Triton tile kernel) / :413-423.
+ * flags (the same for b2l_w8_gemm, b2l_q4_gemm_nll and b2l_w8_gemm_nll), any other bit is rejected:
+ *   0                   qw_tiled from b2l_q4_tile (b2l_w8_gemm: quant_weight in the reference layout);
+ *   B2L_F_GEMM_I8       qw_tiled from b2l_q4_tile_i8 (b2l_w8_gemm: b2l_w8_tile_i8) of the layer's N rows, the resident
+ *                       copy the batch-1 kernels read; rows at or beyond N rounded up to 16 are never read;
+ *   B2L_F_GEMM_I8 | B2L_F_GEMM_I8_LO / _HI
+ *                       qw_tiled is that tiling of 2N interleaved rows (layer row o at 16 (o / 8) + o % 8, + 8 for _HI:
+ *                       the fc1|fc2 tiling of b2l_decode_step's c_fc12), N % 8 == 0; each launch reads all 2N rows'
+ *                       bytes.  Both halves together, or a half without B2L_F_GEMM_I8, are rejected.
+ * Every source gives bit-identical results: the producers write the same bf16 values to the same shared memory. */
 int b2l_q4_gemm(const b2l_q4_linear_args* args, b2l_stream_t stream);
 
 /* Batch-1 decode variant of the fused linear (M == 1): TMA-staged packed weights, PDL prefetch, persistent CTAs
@@ -223,8 +237,8 @@ int b2l_q4_gemv_batch_i8(const b2l_q4_linear_args* args, b2l_stream_t stream);
 /* gptq.int8 for M >= 1 rows (meant for M >= 2: prompts, batched decode) on the wgmma GEMM of b2l_q4_gemm: the
  * producers dequantise the 8-bit levels with get_weight's roundings, so the tensor core multiplies exactly
  * get_weight()'s bf16 matrix.  qw_tiled is quant_weight itself in the reference layout (uint8 [K][N], no
- * re-tiled copy); other requirements as b2l_q4_gemm (K % 64 == 0, ldx % 8 == 0, 16-byte aligned x and weights,
- * NONE / STORE), flags must be 0. */
+ * re-tiled copy), or with B2L_F_GEMM_I8 (| _LO / _HI) the resident b2l_w8_tile_i8 tiling as for b2l_q4_gemm; other
+ * requirements as b2l_q4_gemm (K % 64 == 0, ldx % 8 == 0, 16-byte aligned x and weights, NONE / STORE). */
 int b2l_w8_gemm(const b2l_q4_linear_args* args, b2l_stream_t stream);
 
 /* ------------------------------------------------------------------------------

@@ -20,6 +20,9 @@ F_Q4_BATCH_I8 = 256   # b2l_decode_step (gptq.int4) at B in 2..16: every linear 
 F_Q8_BATCH = 512   # b2l_decode_step with F_Q8 at B in 2..16: every linear runs b2l_q8_linear_batch
 F_ROW_POS = 1024   # b2l_attention (T == 1) and b2l_decode_step: input_pos int64[B] and ring_start int32[B], one per row
 F_STEPWISE = 2048   # b2l_attention (B == 1, T = 2..16) and b2l_decode_step: the rows are consecutive tokens of one sequence
+F_GEMM_I8 = 4096   # b2l_{q4,w8}_gemm(_nll): qw_tiled is the batch-1 tiling (b2l_q4_tile_i8 / b2l_w8_tile_i8)
+F_GEMM_I8_LO = 8192   # with F_GEMM_I8: rows 0..7 of every 16-row block of a 2N-row interleaved tiling (c_fc1)
+F_GEMM_I8_HI = 16384   # with F_GEMM_I8: rows 8..15 of every 16-row block (c_fc2)
 
 c_void_p, c_int, c_float, c_size_t = C.c_void_p, C.c_int, C.c_float, C.c_size_t
 

@@ -23,6 +23,9 @@
 //       * 16-byte st.shared of 8 consecutive k of a row = one row of a core matrix; fence.proxy.async; mbarrier arrive;
 //   epilogue: each MMA thread converts its accumulator fragment to bf16 and stores pairs of output features.
 // gptq.int8 (b2l_w8_gemm) is the same kernel with W8 = true: only the producers differ (w8_load below).
+// SRC = SRC_I8 / SRC_I8_HALF (B2L_F_GEMM_I8 [| _LO / _HI]) swaps the weight source for the batch-1 decode tilings
+// (b2l_q4_tile_i8 / b2l_w8_tile_i8, the one resident copy of a compacted model; i8_producer below): the producers
+// write the same bf16 values to the same shared-memory positions, so the MMAs and the result are unchanged bit for bit.
 // NLL = true (b2l_q4_gemm_nll / b2l_w8_gemm_nll) replaces the epilogue's store: the quad of lanes holding a token row
 // reduces the bf16-rounded accumulators of the tile's 128 columns to (max, sum of exp) into a workspace, and the lane
 // holding the row's target column records its logit (nll_common.cuh; csrc/nll.cu merges the tiles).
@@ -46,6 +49,8 @@ constexpr int NTHREADS = NMMA + NPROD;
 constexpr int LBO_A = BM * 16;                 // bytes between adjacent 8-k columns of the activation operand
 constexpr int LBO_B = BN * 16;                 // bytes between adjacent 8-k columns of the weight operand
 constexpr int SBO = 128;                       // bytes between adjacent 8-row groups
+// weight source: b2l_q4_tile (4 bits) / quant_weight (8 bits), the batch-1 tiling, or one half of an interleaved one
+constexpr int SRC_OWN = 0, SRC_I8 = 1, SRC_I8_HALF = 2;
 
 struct Params {
   CUtensorMap xmap;        // 3-D view of x (see above); must stay the first member (64-byte alignment)
@@ -54,6 +59,7 @@ struct Params {
   const void* scales; const void* zeros; int szdt;
   __nv_bfloat16* y; int ldy;
   int M, N, K;
+  int half;                // SRC_I8_HALF only: 0 = rows 0..7, 1 = rows 8..15 of every 16-row block of a 2N-row tiling
   const void* targets; int tgt_i64;   // NLL only: targets [M], partials [N/128][M], target logits [M]
   float2* part; float* tl;
 };
@@ -140,7 +146,25 @@ __device__ __forceinline__ void w8_load(uint32_t (&wq)[16], const uint8_t* qw, i
   }
 }
 
-template <bool W8, bool NLL>
+// (level - zero) * scale of the bf16 level pair in `v` (0x4300 | (128 + level) per half at 4 bits, see below) with
+// get_weight's roundings
+__device__ __forceinline__ uint32_t q4_pair(uint32_t v, __nv_bfloat162 z2, __nv_bfloat162 sc2) {
+  const __nv_bfloat162 c128 = __float2bfloat162_rn(128.f);
+  __nv_bfloat162 t = __hsub2(*reinterpret_cast<const __nv_bfloat162*>(&v), c128);   // level, exact
+  t = __hmul2(__hsub2(t, z2), sc2);
+  return *reinterpret_cast<const uint32_t*>(&t);
+}
+// the same for the 8-bit levels in bytes r and r + 1 of `w` (the 2^23 mantissa trick of the W8 producer)
+__device__ __forceinline__ uint32_t w8_pair(uint32_t w, int r, __nv_bfloat162 z2, __nv_bfloat162 sc2) {
+  const float two23 = 8388608.f;
+  const float f0 = __uint_as_float(__byte_perm(w, 0x4B000000u, 0x7540u | (uint32_t)r)) - two23;
+  const float f1 = __uint_as_float(__byte_perm(w, 0x4B000000u, 0x7540u | (uint32_t)(r + 1))) - two23;
+  __nv_bfloat162 t = __floats2bfloat162_rn(f0, f1);   // level pair, exact
+  t = __hmul2(__hsub2(t, z2), sc2);
+  return *reinterpret_cast<const uint32_t*>(&t);
+}
+
+template <bool W8, bool NLL, int SRC>
 __global__ void __launch_bounds__(NTHREADS, 1) q4_gemm_kernel(const __grid_constant__ Params p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   const uint32_t sbase = smem_u32(smem);
@@ -215,6 +239,106 @@ __global__ void __launch_bounds__(NTHREADS, 1) q4_gemm_kernel(const __grid_const
           }
         }
       }
+    }
+  } else if constexpr (SRC != SRC_OWN) {
+    // ===================== producers, batch-1 tilings: activations (TMA) + dequantised weights =====================
+    // A (16-row block rb, k block kb) tile of b2l_q4_tile_i8 is 512 B at (rb * K/64 + kb) * 512: lane (g, t) holds in
+    // word 2c + j, byte i, the levels of rows g (low nibble) and g + 8 (high nibble) at k = 64 kb + 32 c + 8 t + 4 j + i.
+    // Of b2l_w8_tile_i8 it is 1024 B, [c][32 lanes][16 B]: word w of lane (g, t) holds row g + 8 (w & 1) at
+    // k = 64 kb + 32 c + 8 t + 4 (w >> 1) + 0..3.  Either way one lane's 16 B of chunk c are 8 consecutive k (the
+    // core-matrix row of k column 4 c + t) of rows g and g + 8.  A 64-wide k stage is one k block; producer warp pw
+    // loads NCH consecutive row blocks, 2 of 8 (plain), or 4 of the 16 interleaved blocks whose half p.half holds this
+    // layer's 128 rows (SRC_I8_HALF: layer row o is row 16 (o / 8) + o % 8 + 8 half of the 2N-row tiling), which
+    // reads twice the bytes it uses.  Thread `lane` takes tile lane (g, t) = (lane % 8, lane / 8): the 8 threads of a
+    // shared-memory store phase then write 8 consecutive rows of one k column, 128 contiguous bytes (lane order
+    // would put 4 of them 2 KB apart, in the same banks).
+    constexpr bool HALF = SRC == SRC_I8_HALF;
+    constexpr int NCH = HALF ? 4 : 2;                // row blocks per producer thread and stage
+    constexpr int RPB = HALF ? 1 : 2;                // rows of a block this layer owns per lane
+    constexpr int NLD = W8 ? 2 : 1;                  // 16-byte loads per lane and block (k chunks c at 8 bits)
+    constexpr int TILE_B = W8 ? 1024 : 512;
+    const int pw = (tid - NMMA) >> 5, g = lane & 7, t = lane >> 3;
+    const int n_kb = p.K / BK;
+    const int n_rb = HALF ? p.N / 8 : (p.N + 15) / 16;   // row blocks of the tiling that hold this layer's rows
+    const int hsel = HALF ? p.half : 0;
+    const uint8_t* src[NCH];
+    bool ok[NCH];
+    __nv_bfloat162 sc2[NCH][RPB], z2[NCH][RPB];
+    int trow[NCH][RPB];                              // row of the 128-row tile
+#pragma unroll
+    for (int b = 0; b < NCH; ++b) {
+      const int q = NCH * pw + b;                    // block of the tile
+      const int rb = (HALF ? n0 / 8 : n0 / 16) + q;  // block of the tiling
+      ok[b] = rb < n_rb;
+      src[b] = p.qwt + (size_t)min(rb, n_rb - 1) * n_kb * TILE_B + (4 * g + t) * 16;
+#pragma unroll
+      for (int r = 0; r < RPB; ++r) {
+        trow[b][r] = HALF ? 8 * q + g : 16 * q + g + 8 * r;
+        const int row_n = n0 + trow[b][r];
+        float sc_f = 0.f, z_f = 0.f;
+        if (row_n < p.N) { sc_f = load_sz(p.scales, p.szdt, row_n); z_f = load_sz(p.zeros, p.szdt, row_n); }
+        sc2[b][r] = __float2bfloat162_rn(sc_f); z2[b][r] = __float2bfloat162_rn(z_f);
+      }
+    }
+    uint4 wq[NCH][NLD];
+    auto load_w = [&](int kt) {
+#pragma unroll
+      for (int b = 0; b < NCH; ++b)
+#pragma unroll
+        for (int c = 0; c < NLD; ++c) {
+          wq[b][c] = make_uint4(0, 0, 0, 0);
+          if (ok[b]) wq[b][c] = __ldg(reinterpret_cast<const uint4*>(src[b] + (size_t)kt * TILE_B + c * 512));
+        }
+    };
+    load_w(0);
+    for (int kt = 0; kt < n_kt; ++kt) {
+      const int st = kt % NSTAGE;
+      if (kt >= NSTAGE) mbar_wait(bar_empty + st * 8, (uint32_t)(kt / NSTAGE - 1) & 1u);
+      const uint32_t a_base = sbase + st * STAGE_BYTES, b_base = a_base + A_BYTES;
+      if (tid == NMMA) {
+        mbar_expect_tx(bar_full + st * 8, A_BYTES);
+        tma_load_3d(a_base, &p.xmap, 0, m0, kt * (BK / 8), bar_full + st * 8);
+      }
+      uint4 w[NCH][NLD];
+#pragma unroll
+      for (int b = 0; b < NCH; ++b)
+#pragma unroll
+        for (int c = 0; c < NLD; ++c) w[b][c] = wq[b][c];
+      if (kt + 1 < n_kt) load_w(kt + 1);
+#pragma unroll
+      for (int b = 0; b < NCH; ++b) {
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {                // k column 4 c + t
+#pragma unroll
+          for (int r = 0; r < RPB; ++r) {
+            const int hi = HALF ? hsel : r;          // row g + 8 hi of the 16-row block
+            uint32_t o[4];
+            if constexpr (W8) {
+              const uint4 u = w[b][c];
+              const uint32_t lo4 = hi ? u.y : u.x, hi4 = hi ? u.w : u.z;   // k 0..3 and 4..7 of the row
+              o[0] = w8_pair(lo4, 0, z2[b][r], sc2[b][r]);
+              o[1] = w8_pair(lo4, 2, z2[b][r], sc2[b][r]);
+              o[2] = w8_pair(hi4, 0, z2[b][r], sc2[b][r]);
+              o[3] = w8_pair(hi4, 2, z2[b][r], sc2[b][r]);
+            } else {
+              const uint4 u = w[b][0];
+              const uint32_t wj[2] = {c ? u.z : u.x, c ? u.w : u.y};     // words 2 c, 2 c + 1: k 0..3, 4..7
+#pragma unroll
+              for (int j = 0; j < 2; ++j)
+#pragma unroll
+                for (int s = 0; s < 2; ++s) {       // bytes 2 s, 2 s + 1 -> halves of a word, then row g's / g + 8's nibble
+                  const uint32_t v = (__byte_perm(wj[j], 0u, s ? 0x4342u : 0x4140u) >> (4 * hi)) & 0x000f000fu;
+                  o[2 * j + s] = q4_pair(v | 0x43004300u, z2[b][r], sc2[b][r]);
+                }
+            }
+            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(b_base + (4 * c + t) * LBO_B + trow[b][r] * 16),
+                         "r"(o[0]), "r"(o[1]), "r"(o[2]), "r"(o[3]) : "memory");
+          }
+        }
+      }
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_full + st * 8);
     }
   } else if constexpr (W8) {
     // ===================== producers, 8-bit levels: activations (TMA) + dequantised weights =====================
@@ -324,7 +448,24 @@ using namespace b2l;
 using namespace b2l::q4gm;
 
 namespace {
-// b2l_q4_gemm (W8 = false: qw_tiled from b2l_q4_tile) and b2l_w8_gemm (W8 = true: quant_weight, uint8 [K][N]);
+template <bool W8, bool NLL, int SRC>
+int launch(const Params& p, dim3 grid, cudaStream_t stream) {
+  static DynSmemCache smem_cache;
+  if (int rc = ensure_dyn_smem(q4_gemm_kernel<W8, NLL, SRC>, SMEM_BYTES, smem_cache)) return rc;
+  q4_gemm_kernel<W8, NLL, SRC><<<grid, NTHREADS, SMEM_BYTES, stream>>>(p);
+  B2L_LAUNCH_CHECK("q4_gemm_kernel");
+  return 0;
+}
+
+template <bool W8, bool NLL>
+int launch_src(const Params& p, int flags, dim3 grid, cudaStream_t stream) {
+  if (flags & (B2L_F_GEMM_I8_LO | B2L_F_GEMM_I8_HI)) return launch<W8, NLL, SRC_I8_HALF>(p, grid, stream);
+  if (flags & B2L_F_GEMM_I8) return launch<W8, NLL, SRC_I8>(p, grid, stream);
+  return launch<W8, NLL, SRC_OWN>(p, grid, stream);
+}
+
+// b2l_q4_gemm (W8 = false: qw_tiled from b2l_q4_tile) and b2l_w8_gemm (W8 = true: quant_weight, uint8 [K][N]), or with
+// B2L_F_GEMM_I8 the batch-1 tiling of either width (B2L_F_GEMM_I8_LO / _HI: one half of an interleaved one);
 // with `nl` (b2l_*_gemm_nll) the NLL epilogue instead of the store, then the combine kernel
 template <bool W8>
 int gemm_entry(const b2l_q4_linear_args* a, const b2l_nll_args* nl, b2l_stream_t stream) {
@@ -339,7 +480,12 @@ int gemm_entry(const b2l_q4_linear_args* a, const b2l_nll_args* nl, b2l_stream_t
   B2L_CHECK_ARG(a->ldx >= a->K && a->ldx % 8 == 0 && (a->ldy >= a->N || with_nll), "%s: bad leading dimension (ldx %% 8 == 0)", fn);
   B2L_CHECK_ARG(((uintptr_t)a->x % 16 == 0) && ((uintptr_t)a->qw_tiled % 16 == 0), "%s: x / qw_tiled must be 16-byte aligned", fn);
   B2L_CHECK_ARG(a->sz_dtype == B2L_BF16 || a->sz_dtype == B2L_F32, "%s: bad sz_dtype", fn);
-  if (W8) B2L_CHECK_SUPPORTED(a->flags == 0, "%s: unknown flags 0x%x", fn, a->flags);
+  constexpr int kHalves = B2L_F_GEMM_I8_LO | B2L_F_GEMM_I8_HI;
+  B2L_CHECK_SUPPORTED((a->flags & ~(B2L_F_GEMM_I8 | kHalves)) == 0, "%s: unknown flags 0x%x", fn, a->flags);
+  B2L_CHECK_ARG((a->flags & kHalves) != kHalves, "%s: B2L_F_GEMM_I8_LO and B2L_F_GEMM_I8_HI exclude each other", fn);
+  B2L_CHECK_ARG(!(a->flags & kHalves) || (a->flags & B2L_F_GEMM_I8), "%s: B2L_F_GEMM_I8_LO / _HI need B2L_F_GEMM_I8", fn);
+  B2L_CHECK_SUPPORTED(!(a->flags & kHalves) || a->N % 8 == 0,
+                      "%s: B2L_F_GEMM_I8_LO / _HI take 8-row groups of an interleaved tiling: N=%d must be a multiple of 8", fn, a->N);
   B2L_CHECK_SUPPORTED(a->prologue == B2L_PRO_NONE && a->epilogue == B2L_EPI_STORE, "%s: plain linear only (no fused prologue / epilogue)", fn);
   if (with_nll) {
     if (int rc = nll::check_args(nl, a->M, fn)) return rc;
@@ -376,22 +522,14 @@ int gemm_entry(const b2l_q4_linear_args* a, const b2l_nll_args* nl, b2l_stream_t
   p.scales = a->scales; p.zeros = a->zeros; p.szdt = a->sz_dtype;
   p.y = (__nv_bfloat16*)a->y; p.ldy = a->ldy;
   p.M = a->M; p.N = a->N; p.K = a->K;
+  p.half = (a->flags & B2L_F_GEMM_I8_HI) ? 1 : 0;
   p.targets = nullptr; p.tgt_i64 = 0; p.part = nullptr; p.tl = nullptr;
   dim3 grid((a->N + BN - 1) / BN, (a->M + BM - 1) / BM);
-  if (!with_nll) {
-    static DynSmemCache smem_cache;
-    if (int rc = ensure_dyn_smem(q4_gemm_kernel<W8, false>, SMEM_BYTES, smem_cache)) return rc;
-    q4_gemm_kernel<W8, false><<<grid, NTHREADS, SMEM_BYTES, (cudaStream_t)stream>>>(p);
-    B2L_LAUNCH_CHECK("q4_gemm_kernel");
-    return 0;
-  }
+  if (!with_nll) return launch_src<W8, false>(p, a->flags, grid, (cudaStream_t)stream);
   uint8_t* ws = (uint8_t*)nl->workspace;
   p.targets = nl->targets; p.tgt_i64 = nl->targets_i64;
   p.part = (float2*)ws; p.tl = (float*)(ws + nll::part_bytes(a->M, a->N));
-  static DynSmemCache smem_cache_nll;
-  if (int rc = ensure_dyn_smem(q4_gemm_kernel<W8, true>, SMEM_BYTES, smem_cache_nll)) return rc;
-  q4_gemm_kernel<W8, true><<<grid, NTHREADS, SMEM_BYTES, (cudaStream_t)stream>>>(p);
-  B2L_LAUNCH_CHECK("q4_gemm_kernel (nll)");
+  if (int rc = launch_src<W8, true>(p, a->flags, grid, (cudaStream_t)stream)) return rc;
   return nll::launch_combine(nl->targets, nl->targets_i64, a->M, a->N, nl->workspace, nl->nll, nl->nll_sum, (cudaStream_t)stream);
 }
 }  // namespace

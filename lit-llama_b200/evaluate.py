@@ -94,17 +94,12 @@ def lm_head_nll(lm: torch.nn.Module, x: torch.Tensor, targets: torch.Tensor) -> 
         return logits_nll(lm(x), targets)
     N, M = lm.out_features, targets.numel()
     a, (nll, s, _ws) = _nll_args(targets, M, N)
-    if kind == "q4":
-        wt = lm.tiled()   # transient on a compacted layer: held until the launch is enqueued
-        fn = "b2l_q4_gemm_nll"
-    else:
-        lm._check_layout()
-        wt = lm.reference_quant_weight()
-        fn = "b2l_w8_gemm_nll"
+    wt, flags = lm.gemm_weight()   # a compacted lm_head: its resident batch-1 tiling
+    fn = "b2l_q4_gemm_nll" if kind == "q4" else "b2l_w8_gemm_nll"
     g = L.Q4LinearArgs(
         x=x2.data_ptr(), ldx=x2.stride(0), qw_tiled=wt.data_ptr(), scales=lm.scales.data_ptr(), zeros=lm.zeros.data_ptr(),
         sz_dtype=L.sz_dtype_of(lm.scales), y=None, ldy=0, M=M, N=N, K=K, prologue=L.PRO_NONE, norm_scale=None, eps=0.0,
-        epilogue=L.EPI_STORE, res=None, ldres=0, split_k=0, flags=0)
+        epilogue=L.EPI_STORE, res=None, ldres=0, split_k=0, flags=flags)
     L.check(getattr(L.lib(), fn)(C.byref(g), C.byref(a), L.stream_ptr()), fn)
     return nll, s
 

@@ -790,6 +790,11 @@ class LLaMA(nn.Module):
         mlp = self.transformer.h[i].mlp
         return getattr(mlp.c_fc1, "_released", False) and getattr(mlp.c_fc2, "_released", False)
 
+    def _fc12_tiling(self, i: int) -> torch.Tensor:
+        """The interleaved fc1|fc2 batch-1 tiling of layer i: a compacted c_fc1 / c_fc2's weights (the prefill GEMM
+        reads its half in place)."""
+        return self._fc12_cache[(i, "i8")][1][0]
+
     def _fc_from_fc12(self, i: int, which: int) -> torch.Tensor:
         """c_fc1 (which = 0) or c_fc2 (1) of layer i in the reference layout, rebuilt from the interleaved batch-1
         tiling (compacted models keep only that copy): untile (a permutation, by bit width) and take every other 8
@@ -821,8 +826,9 @@ class LLaMA(nn.Module):
                 self._fc12_cache.pop((i, kind), None)
             for lin in (blk.attn.c_attn, blk.attn.c_proj, blk.mlp.c_proj):
                 lin.release_reference_layout()
-            blk.mlp.c_fc1.release_reference_layout(source=functools.partial(self._fc_from_fc12, i, 0))
-            blk.mlp.c_fc2.release_reference_layout(source=functools.partial(self._fc_from_fc12, i, 1))
+            fc12 = functools.partial(self._fc12_tiling, i)
+            blk.mlp.c_fc1.release_reference_layout(source=functools.partial(self._fc_from_fc12, i, 0), half=(fc12, 0))
+            blk.mlp.c_fc2.release_reference_layout(source=functools.partial(self._fc_from_fc12, i, 1), half=(fc12, 1))
         self.lm_head.release_reference_layout()
         self._decode, self._module_graph = None, None   # rebuilt on the next step (B > 1 states hold their transient tilings)
         self._verify = {}

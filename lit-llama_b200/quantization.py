@@ -82,6 +82,7 @@ class ColBlockQuantizedLinear(torch.nn.Module):
         self._tiled_i8_key = None
         self._released = False    # reference-layout buffer freed (release_reference_layout): one copy of the weights
         self._source = None       # released + no own tiling: callable returning the reference-layout tensor
+        self._half = None         # ... and (callable returning the interleaved tiling that holds it, 0 / 1: which half)
 
     # ------------------------------------------------------------------ packing (load-time, any device)
     def pack_weight(self, weight):
@@ -104,7 +105,7 @@ class ColBlockQuantizedLinear(torch.nn.Module):
         if self._released and prefix + "quant_weight" in state_dict:
             self.quant_weight = torch.empty((self.in_features // self.entries_per_byte, self.out_features), dtype=torch.uint8,
                                             device=self.scales.device).t()
-            self._released, self._source = False, None
+            self._released, self._source, self._half = False, None, None
             self._tiled = self._tiled_mma = self._tiled_i8 = None
         super()._load_from_state_dict(state_dict, prefix, *args, **kwargs)   # copies in place: pointers stay, contents (and _version) change
         weights_changed()
@@ -131,12 +132,14 @@ class ColBlockQuantizedLinear(torch.nn.Module):
                 name)
         return out
 
-    def release_reference_layout(self, source=None) -> None:
+    def release_reference_layout(self, source=None, half=None) -> None:
         """Free the reference-layout buffer: the decode kernels read only their own tiling, so keeping both doubles
         the weight memory (the reference's selling point for gptq.int4 is "~5 GB", howto/inference.md:37).
         `state_dict()` and the prefill / batch tilings are then rebuilt on demand from the batch-1 tiling -- or from
         `source()` (c_fc1 / c_fc2, whose decode copy is the interleaved fc1|fc2 tiling owned by the model), in which
-        case this module keeps no tiling of its own.  Loading a state dict brings the buffer back."""
+        case this module keeps no tiling of its own.  `half` = (tiling, h) then says where the prefill GEMM finds the
+        layer: rows 8 h .. 8 h + 7 of every 16-row block of the tensor `tiling()` returns.  Loading a state dict
+        brings the buffer back."""
         if self._released:
             return
         if not self.scales.is_cuda:
@@ -144,9 +147,11 @@ class ColBlockQuantizedLinear(torch.nn.Module):
         if not (self.gemv_capable or self.w8_gemv_capable):
             raise RuntimeError("release_reference_layout needs a gptq.int4 / gptq.int8 layer the batch-1 kernel can run "
                                "(per-row scales, no bias, in % 64 == 0)")
+        if half is not None and source is None:
+            raise ValueError("release_reference_layout: `half` describes a layer held in another tiling; pass its `source` too")
         if source is None:
             self.tiled_i8()
-        self._released, self._source = True, source
+        self._released, self._source, self._half = True, source, half
         self.quant_weight = torch.empty((self.out_features, 0), dtype=torch.uint8, device=self.scales.device)
         self._tiled = self._tiled_mma = None
         if source is not None:
@@ -223,6 +228,21 @@ class ColBlockQuantizedLinear(torch.nn.Module):
                 return t
             self._tiled_i8, self._tiled_i8_key = t, key
         return self._tiled_i8
+
+    def gemm_weight(self):
+        """(weights, flags) for b2l_q4_gemm / b2l_w8_gemm: a released layer's resident batch-1 tiling with
+        B2L_F_GEMM_I8 (c_fc1 / c_fc2: half of the interleaved fc1|fc2 tiling), else b2l_q4_tile's tiling (4 bits) or
+        quant_weight itself (8 bits), rebuilt by `source()` for a released layer given no `half`.  The GEMM's result
+        is the same bit for bit either way."""
+        if self._released and self._source is None:
+            return self._tiled_i8, L.F_GEMM_I8
+        if self._half is not None:
+            tiling, h = self._half
+            return tiling(), L.F_GEMM_I8 | (L.F_GEMM_I8_HI if h else L.F_GEMM_I8_LO)
+        if self.bits == 8:
+            self._check_layout()
+            return self.reference_quant_weight(), 0
+        return self.tiled(), 0
 
     def tiled_mma(self) -> torch.Tensor:
         """The [N/16][K/64][32 lanes][16 B] re-tiling of the 2..8-row kernel (b2l_q4_tile_mma: f16-MMA fragments)."""
@@ -302,16 +322,16 @@ class ColBlockQuantizedLinear(torch.nn.Module):
                 zeros=self.zeros.data_ptr(), sz_dtype=L.sz_dtype_of(self.scales), y=y.data_ptr(), ldy=N, M=1, N=N, K=K,
                 prologue=L.PRO_NONE, norm_scale=None, eps=0.0, epilogue=L.EPI_STORE, res=None, ldres=0, split_k=0, flags=0)
             L.check(getattr(L.lib(), "b2l_" + kernel)(C.byref(a), L.stream_ptr()), "b2l_" + kernel)
-        elif kernel == "w8_gemm":
-            # the wgmma GEMM reads quant_weight in the reference layout (a compacted layer rebuilds it transiently)
-            self._check_layout()
-            wt = self.reference_quant_weight()
+        elif kernel in ("w8_gemm", "q4_gemm"):
+            # prefill-shaped, 128 x 128 wgmma tiles, weights dequantised on the fly with get_weight's roundings; a
+            # compacted layer's GEMM reads its resident batch-1 tiling
+            wt, flags = self.gemm_weight()
             a = L.Q4LinearArgs(
                 x=x.data_ptr(), ldx=x.stride(0), qw_tiled=wt.data_ptr(), scales=self.scales.data_ptr(),
                 zeros=self.zeros.data_ptr(), sz_dtype=L.sz_dtype_of(self.scales), y=y.data_ptr(), ldy=N,
                 M=M, N=N, K=K, prologue=L.PRO_NONE, norm_scale=None, eps=0.0, epilogue=L.EPI_STORE, res=None,
-                ldres=0, split_k=0, flags=0)
-            L.check(L.lib().b2l_w8_gemm(C.byref(a), L.stream_ptr()), "b2l_w8_gemm")
+                ldres=0, split_k=0, flags=flags)
+            L.check(getattr(L.lib(), "b2l_" + kernel)(C.byref(a), L.stream_ptr()), "b2l_" + kernel)
         elif kernel == "q4_gemv_batch":
             # 2..8 rows: the mma.sync tile has 8 columns, one per row (csrc/q4_gemv_batch.cu)
             wt = self.tiled_mma()
@@ -321,15 +341,14 @@ class ColBlockQuantizedLinear(torch.nn.Module):
                 prologue=L.PRO_NONE, norm_scale=None, eps=0.0, epilogue=L.EPI_STORE, res=None, ldres=0, split_k=0, flags=0,
                 workspace=batch_workspace(inp.device, K).data_ptr())
             L.check(L.lib().b2l_q4_gemv_batch(C.byref(a), L.stream_ptr()), "b2l_q4_gemv_batch")
-        elif kernel in ("q4_linear_tc", "q4_gemm"):
-            # q4_gemm: prefill-shaped, 128 x 128 wgmma tiles, weights dequantised on the fly with get_weight's roundings
+        elif kernel == "q4_linear_tc":
             wt = self.tiled()
             a = L.Q4LinearArgs(
                 x=x.data_ptr(), ldx=x.stride(0), qw_tiled=wt.data_ptr(), scales=self.scales.data_ptr(),
                 zeros=self.zeros.data_ptr(), sz_dtype=L.sz_dtype_of(self.scales), y=y.data_ptr(), ldy=N,
                 M=M, N=N, K=K, prologue=L.PRO_NONE, norm_scale=None, eps=0.0, epilogue=L.EPI_STORE, res=None,
                 ldres=0, split_k=0, flags=0)
-            L.check(getattr(L.lib(), "b2l_" + kernel)(C.byref(a), L.stream_ptr()), "b2l_" + kernel)
+            L.check(L.lib().b2l_q4_linear_tc(C.byref(a), L.stream_ptr()), "b2l_q4_linear_tc")
         elif kernel == "q_linear":
             self._check_layout()
             qw = self.reference_quant_weight()
