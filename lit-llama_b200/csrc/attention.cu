@@ -261,11 +261,6 @@ __device__ __forceinline__ void bf16x8_to_f32(const uint4& u, float* f) {
   }
 }
 
-__device__ __forceinline__ uint32_t fd_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void fd_bulk(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
-}
-
 // Dynamic shared memory: 2 buffers x (K sub-tile 16 KB + V sub-tile 16 KB), merge scratch, 2 mbarriers.
 constexpr int FD_SUB_BYTES = FD_SUB * 128 * 2;
 constexpr int FD_SMEM_BYTES = 4 * FD_SUB_BYTES + FD_WARPS * 128 * 4 + 2 * FD_WARPS * 4 + 16;
@@ -378,27 +373,27 @@ __global__ void __launch_bounds__(FD_WARPS * 32, ADAPTER ? FD_CTAS_PER_SM : 0)
   const bool has_new = (w_slot >= j0 && w_slot < j1);
 
   // sub-tile i -> buffer i & 1: old K rows then old V rows, each possibly in two pieces (the ring wraps)
-  const uint32_t bar0 = fd_smem_u32(bars);
+  const uint32_t bar0 = smem_u32(bars);
   auto request = [&](int i) {
     const int buf = i & 1;
     const int cnt = min(FD_SUB, n_old - i * FD_SUB);
     int phys0 = j0 + i * FD_SUB + ring; if (phys0 >= S) phys0 -= S;
     const int first = min(cnt, S - phys0);  // rows before the ring wraps
     const uint32_t bar = bar0 + buf * 8;
-    const uint32_t kd = fd_smem_u32(fsm) + buf * 2 * FD_SUB_BYTES, vd = kd + FD_SUB_BYTES;
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"((uint32_t)cnt * HS * 2 * 2) : "memory");
-    fd_bulk(kd, k_cache + head_base + (size_t)phys0 * HS, (uint32_t)first * HS * 2, bar);
-    fd_bulk(vd, v_cache + head_base + (size_t)phys0 * HS, (uint32_t)first * HS * 2, bar);
+    const uint32_t kd = smem_u32(fsm) + buf * 2 * FD_SUB_BYTES, vd = kd + FD_SUB_BYTES;
+    mbar_expect_tx(bar, (uint32_t)cnt * HS * 2 * 2);
+    tma_bulk_g2s(kd, k_cache + head_base + (size_t)phys0 * HS, (uint32_t)first * HS * 2, bar);
+    tma_bulk_g2s(vd, v_cache + head_base + (size_t)phys0 * HS, (uint32_t)first * HS * 2, bar);
     if (first < cnt) {  // wrapped part starts at physical row 0
-      fd_bulk(kd + first * HS * 2, k_cache + head_base, (uint32_t)(cnt - first) * HS * 2, bar);
-      fd_bulk(vd + first * HS * 2, v_cache + head_base, (uint32_t)(cnt - first) * HS * 2, bar);
+      tma_bulk_g2s(kd + first * HS * 2, k_cache + head_base, (uint32_t)(cnt - first) * HS * 2, bar);
+      tma_bulk_g2s(vd + first * HS * 2, v_cache + head_base, (uint32_t)(cnt - first) * HS * 2, bar);
     }
   };
   // ---- before the dependency: the first sub-tile (both when one CTA per head is all there is: nothing queues then)
   const int pre = (n_active == 1) ? 2 : pre_tiles;
   if (threadIdx.x == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar0) : "memory");
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar0 + 8) : "memory");
+    mbar_init_c<1>(bar0);
+    mbar_init_c<1>(bar0 + 8);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     if (n_sub > 0) request(0);
     if (pre > 1 && n_sub > 1) request(1);
@@ -507,13 +502,8 @@ __global__ void __launch_bounds__(FD_WARPS * 32, ADAPTER ? FD_CTAS_PER_SM : 0)
   for (int i = 0; i < n_sub; ++i) {
     const int buf = i & 1;
     const int cnt = min(FD_SUB, n_old - i * FD_SUB);
-    {
-      uint32_t ok;
-      const uint32_t par = (uint32_t)(i >> 1) & 1u;
-      do {
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(ok) : "r"(bar0 + buf * 8), "r"(par) : "memory");
-      } while (!ok);
-    }
+    const uint32_t par = (uint32_t)(i >> 1) & 1u;
+    mbar_wait(bar0 + buf * 8, par);
     const __nv_bfloat16* kt = reinterpret_cast<const __nv_bfloat16*>(fsm + buf * 2 * FD_SUB_BYTES);
     const __nv_bfloat16* vt = kt + FD_SUB * HS;
     stamp();
@@ -765,7 +755,7 @@ __global__ void __launch_bounds__(128)
                         const __grid_constant__ b2l_ragged rg) {
   constexpr int HS = 128;
   extern __shared__ __align__(128) uint8_t psm[];
-  const uint32_t sq = fd_smem_u32(psm), sk0 = sq + PF_TILE_BYTES;   // K tile of buffer b at sk0 + 2 b TILE, V tile right behind it
+  const uint32_t sq = smem_u32(psm), sk0 = sq + PF_TILE_BYTES;   // K tile of buffer b at sk0 + 2 b TILE, V tile right behind it
   int b, h, t0;
   size_t tok0 = 0;   // RAGGED: packed row of the sequence's token 0 in qkv and y
   if constexpr (RAGGED) {

@@ -1,5 +1,7 @@
 // Shared device/host helpers for libb200llama (sm_90a only).
 #pragma once
+#include <cuda.h>           // CUtensorMap and its enums only: tensor_map_encoder() fetches the encoder (no libcuda link)
+#include <cudaTypedefs.h>   // PFN_cuTensorMapEncodeTiled
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -64,6 +66,17 @@ inline int ensure_dyn_smem(Kernel kernel, size_t bytes, DynSmemCache& cache) {
     cache.bytes[dev] = bytes;
   }
   return 0;
+}
+
+// cuTensorMapEncodeTiled through the runtime, resolved once; nullptr when the driver does not provide it
+inline PFN_cuTensorMapEncodeTiled tensor_map_encoder() {
+  static const PFN_cuTensorMapEncodeTiled encode = [] {
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) fn = nullptr;
+    return (PFN_cuTensorMapEncodeTiled)fn;
+  }();
+  return encode;
 }
 
 // ---- small device helpers ----
@@ -132,6 +145,85 @@ __device__ __forceinline__ float ld_coherent_bf16(const __nv_bfloat16* p) {
   asm volatile("ld.global.u16 %0, [%1];" : "=h"(v) : "l"(p) : "memory");
   return __uint_as_float((uint32_t)v << 16);
 }
+
+// ---- sm_90 wrappers: mbarriers, TMA, named barriers, ldmatrix, int8 mma.sync, wgmma ----
+__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void mbar_init(uint32_t a, uint32_t count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(a), "r"(count) : "memory");
+}
+// the arrival count as an immediate (a different instruction from mbar_init's register operand)
+template <int COUNT> __device__ __forceinline__ void mbar_init_c(uint32_t a) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(a), "n"(COUNT) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t a) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(a) : "memory");
+}
+__device__ __forceinline__ void mbar_expect_tx(uint32_t a, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(a), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint32_t a, uint32_t parity) {
+  uint32_t ok;
+  do {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}"
+        : "=r"(ok)
+        : "r"(a), "r"(parity)
+        : "memory");
+  } while (!ok);
+}
+__device__ __forceinline__ void tma_bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t mbar) {
+  asm volatile(
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
+      "l"(src), "r"(bytes), "r"(mbar)
+      : "memory");
+}
+__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, uint32_t mbar) {
+  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
+               "l"(map), "r"(mbar), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
+
+// named barriers with an immediate id, so that ptxas reserves only the barriers a kernel uses
+template <int ID> __device__ __forceinline__ void bar_sync_c(int n) { asm volatile("bar.sync %0, %1;" ::"n"(ID), "r"(n) : "memory"); }
+template <int ID> __device__ __forceinline__ void bar_arrive_c(int n) { asm volatile("bar.arrive %0, %1;" ::"n"(ID), "r"(n) : "memory"); }
+
+__device__ __forceinline__ uint4 ldmatrix_x4(uint32_t addr) {
+  uint4 r;
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "r"(addr) : "memory");
+  return r;
+}
+
+// IMMA.16832: D (16 x 8, s32) += A (16 x 32, s8 or u8, row) * B (32 x 8, s8, col)
+__device__ __forceinline__ void mma_s8s8_16832(int (&d)[4], const uint4& a, uint32_t b0, uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k32.row.col.s32.s8.s8.s32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3])
+      : "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w), "r"(b0), "r"(b1));
+}
+__device__ __forceinline__ void mma_u8s8_16832(int (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k32.row.col.s32.u8.s8.s32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3])
+      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+}
+
+// K-major, no-swizzle shared-memory matrix descriptor (sm_90 wgmma format):
+//   core matrix = 8 rows x 16 bytes, contiguous (128 B)
+//   LBO = byte distance between the two K halves of one K=16 MMA (next 8-k column)
+//   SBO = byte distance between 8-row groups along N
+__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
+  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
+  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
+  return d;                // layout_type = 0 (no swizzle), base_offset = 0
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// wait until at most N committed wgmma groups are pending
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
 // RMSNorm with the reference's bf16 rounding points (model.py:270-277, no upcast):
 //   ms = bf16(mean(bf16(x*x)));  r = bf16(rsqrt(bf16(ms + eps)));  y = bf16(scale * bf16(x * r))

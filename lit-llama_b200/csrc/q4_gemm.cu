@@ -29,8 +29,6 @@
 // NLL = true (b2l_q4_gemm_nll / b2l_w8_gemm_nll) replaces the epilogue's store: the quad of lanes holding a token row
 // reduces the bf16-rounded accumulators of the tile's 128 columns to (max, sum of exp) into a workspace, and the lane
 // holding the row's target column records its logit (nll_common.cuh; csrc/nll.cu merges the tiles).
-#include <cuda.h>   // CUtensorMap and its enums only: the encoder is fetched with cudaGetDriverEntryPoint (no libcuda link)
-
 #include "b2l_common.cuh"
 #include "nll_common.cuh"
 
@@ -64,33 +62,6 @@ struct Params {
   float2* part; float* tl;
 };
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t a, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(a), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t a) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(a) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t a, uint32_t parity) {
-  uint32_t ok;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(a), "r"(parity)
-        : "memory");
-  } while (!ok);
-}
-// K-major, no-swizzle shared-memory matrix descriptor (sm_90 wgmma): core matrix = 8 rows x 16 B, contiguous
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  return d;
-}
 // D[64 x 128] (fp32, registers) += A[64 x 16] (smem) * B[16 x 128] (smem), both K-major bf16
 __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
   asm volatile(
@@ -115,15 +86,6 @@ __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc,
 __device__ __forceinline__ void reg_fence(float (&d)[64]) {
 #pragma unroll
   for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
-}
-
-__device__ __forceinline__ void mbar_expect_tx(uint32_t a, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(a), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, uint32_t mbar) {
-  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
-               "l"(map), "r"(mbar), "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
 }
 
 // 8-bit levels (gptq.int8): producer thread pt owns weight rows n0 + 4 (pt % 32) .. + 3 and k 16 (pt / 32) .. + 15 of
@@ -193,17 +155,17 @@ __global__ void __launch_bounds__(NTHREADS, 1) q4_gemm_kernel(const __grid_const
       const int st = kt % NSTAGE;
       mbar_wait(bar_full + st * 8, (uint32_t)(kt / NSTAGE) & 1u);
       const uint32_t a_base = sbase + st * STAGE_BYTES, b_base = a_base + A_BYTES;
-      asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+      wgmma_fence();
       reg_fence(acc);
 #pragma unroll
       for (int j = 0; j < BK / 16; ++j)
         wgmma_m64n128k16(acc, make_desc(a_base + h * 64 * 16 + j * 2 * LBO_A, LBO_A, SBO), make_desc(b_base + j * 2 * LBO_B, LBO_B, SBO));
-      asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
-      asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");   // the group of stage kt - 1 has completed
+      wgmma_commit();
+      wgmma_wait<1>();   // the group of stage kt - 1 has completed
       reg_fence(acc);
       if (kt > 0 && lane == 0) mbar_arrive(bar_empty + ((kt - 1) % NSTAGE) * 8);
     }
-    asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+    wgmma_wait<0>();
     reg_fence(acc);
     // ===================== epilogue: registers -> bf16 -> y.  acc[4 c + e]: token row 16 (warp % 4) + lane / 4
     // (+ 8 for e >= 2), output feature 8 c + 2 (lane % 4) + (e & 1)
@@ -490,15 +452,7 @@ int gemm_entry(const b2l_q4_linear_args* a, const b2l_nll_args* nl, b2l_stream_t
   if (with_nll) {
     if (int rc = nll::check_args(nl, a->M, fn)) return rc;
   }
-  // cuTensorMapEncodeTiled through the runtime (resolved once)
-  typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                               const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-  static EncodeFn encode = [] {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) fn = nullptr;
-    return (EncodeFn)fn;
-  }();
+  const PFN_cuTensorMapEncodeTiled encode = tensor_map_encoder();
   if (encode == nullptr) {
     set_error("%s: cuTensorMapEncodeTiled is not available from this driver", fn);
     return B2L_E_STATE;

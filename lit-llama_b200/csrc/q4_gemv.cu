@@ -83,9 +83,6 @@ __host__ __device__ inline SmemLayout smem_layout(int nst, int K, int ndig) {
   return L;
 }
 
-// X (|X| < 2^30) -> word whose bytes are its balanced base-256 digits (byte 3 = signed top digit)
-__device__ __forceinline__ uint32_t balanced_digits(int X) { return ((uint32_t)X + 0x00808080u) ^ 0x00808080u; }
-
 // Weight width W8 (false: 4-bit levels, b2l_q4_tile_i8; true: 8-bit levels, b2l_w8_tile_i8).  A (16-row block, k block)
 // tile is 512 B of packed nibbles or 1024 B of bytes; a half stage is 8 KB either way, so the ring, the stage count
 // and the producer are shared and a stage carries half as many k-block positions at 8 bits.
@@ -182,16 +179,11 @@ __global__ void __launch_bounds__(NTHREADS, 2) q4_gemv_kernel(const Params p) {
     // ===================== consumer warps =====================
     float* red = reinterpret_cast<float*>(smem + L.red);   // [0..7] sum of squares, [8..15] max, then int64[8] sum X, int sh
     int* red_sh = reinterpret_cast<int*>(smem + L.red + 128);
-    // ---- activations: [RMSNorm], power-of-two scaling, balanced digits in B-fragment order, exact sum(X).
-    // Every CTA converts the whole row (K values, 296 times per launch), and the launch cannot start its main loop
-    // before this is done: the conversion is written for instruction count.  Per pair of elements: packed bf16
-    // max / multiplies, ONE fma that both scales and rounds to an integer (x * 2^sh + 1.5 * 2^23: the integer sits
-    // in the mantissa, |X| < 2^22 -- no F2I, which runs at a quarter of the fp32 rate), the balanced digits straight
-    // from those bits with one add and one xor.
+    // ---- activations: [RMSNorm], power-of-two scaling, balanced digits in B-fragment order, exact sum(X)
+    // (act_pass1 / act_scale / act_digits, q4_mma_common.cuh)
     {
       const bool norm = (p.prologue == B2L_PRO_RMSNORM);
       constexpr int NT = NCW * 32;   // 256 threads, 8 elements each per pass
-      constexpr uint32_t MAGIC_BITS = 0x4B400000u;   // 1.5 * 2^23
       uint4 xv[MAXC], gv[MAXC];
       // the RMSNorm scale is a weight: fetch it BEFORE waiting for the producing kernel
 #pragma unroll
@@ -210,30 +202,8 @@ __global__ void __launch_bounds__(NTHREADS, 2) q4_gemv_kernel(const Params p) {
         if (k < p.K) xv[c] = ld_coherent_u4(p.x + k);
       }
       const int nchunk = (p.K + NT * 8 - 1) / (NT * 8);  // warp-uniform: chunks that hold data
-      // pass 1: sum of bf16-rounded squares (RMSNorm, model.py:274: one HMUL2 is the exactly-rounded bf16 product the
-      // reference computes) and max |x|, or with RMSNorm max_k |bf16(g_k x_k)|, which bounds the normalised values
-      float ss = 0.f;
-      __nv_bfloat162 amax2 = __float2bfloat162_rn(0.f);
-#pragma unroll
-      for (int c = 0; c < MAXC; ++c) {
-        if (c < nchunk) {
-          const uint32_t w[4] = {xv[c].x, xv[c].y, xv[c].z, xv[c].w};
-          const uint32_t g[4] = {gv[c].x, gv[c].y, gv[c].z, gv[c].w};
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const __nv_bfloat162 v = *reinterpret_cast<const __nv_bfloat162*>(&w[q]);
-            if (norm) {
-              amax2 = __hmax2(amax2, __habs2(__hmul2(v, *reinterpret_cast<const __nv_bfloat162*>(&g[q]))));
-              const __nv_bfloat162 sq = __hmul2(v, v);
-              const uint32_t su = *reinterpret_cast<const uint32_t*>(&sq);
-              ss += __uint_as_float(su << 16) + __uint_as_float(su & 0xffff0000u);
-            } else {
-              amax2 = __hmax2(amax2, __habs2(v));
-            }
-          }
-        }
-      }
-      float mx = fmaxf(__low2float(amax2), __high2float(amax2));
+      float ss, mx;
+      act_pass1<MAXC>(xv, gv, nchunk, norm, ss, mx);
       ss = warp_sum(ss);
       mx = warp_max(mx);
       if (lane == 0) { red[warp] = ss; red[8 + warp] = mx; }
@@ -241,65 +211,14 @@ __global__ void __launch_bounds__(NTHREADS, 2) q4_gemv_kernel(const Params p) {
       ss = 0.f; mx = 0.f;
 #pragma unroll
       for (int w = 0; w < NCW; ++w) { ss += red[w]; mx = fmaxf(mx, red[8 + w]); }
-      float rinv = 1.f;
-      if (norm) {
-        // The normalised value is v_k = bf16(g_k bf16(x_k rinv)) (rinv is a bf16 value), and pass 1 took
-        // p_k = bf16(g_k x_k).  With u = 2^-8, the unit roundoff of bf16:
-        //   |v_k| <= |g_k x_k| rinv (1 + u)^2 <= |p_k| rinv (1 + u)^2 / (1 - u) < 1.012 |p_k| rinv,
-        // and the two fp32 roundings below lose less than 2^-23, so mx > max_k |v_k|: |X| < 2^22 follows from the
-        // choice of sh.  (A product below bf16's normal range 2^-126 may round further; such elements have
-        // |v_k| < 2^-125 rinv, and sh <= 126 keeps them below 2^22 for any rinv < 2^21, i.e. eps > 2^-42.)
-        // A bound on max|x| max|g|
-        // instead overshoots by up to max|g| / g_k when the largest activation carries a small scale (LLaMA's
-        // massive channels do), and the digit grid below coarsens by the same factor.
-        rinv = rms_rinv(ss, p.K, p.eps);
-        mx = mx * rinv * 1.02f;
-      }
-      // 2^sh: the largest power of two with max|v| * 2^sh < 2^(8 NDIG - 2)
-      const int e = (int)((__float_as_uint(mx) >> 23) & 0xffu) - 127;   // mx < 2^(e + 1)
-      int sh = (8 * NDIG - 3) - e;
-      sh = max(-126, min(126, sh));
-      const float scale = __uint_as_float((uint32_t)(sh + 127) << 23);
-      const float magic = __uint_as_float(MAGIC_BITS);
-      const __nv_bfloat162 rinv2 = __float2bfloat162_rn(rinv);  // rinv is already a bf16 value
+      const ActScale as = act_scale<NDIG>(ss, mx, norm, p.K, p.eps);
       uint32_t sxu = 0;     // sum of this thread's X (<= 48 values below 2^22), modulo 2^32
 #pragma unroll
       for (int c = 0; c < MAXC; ++c) {
         const int k = (c * NT + tid) * 8;
         if (c < nchunk && k < p.K) {
-          uint32_t w[4] = {xv[c].x, xv[c].y, xv[c].z, xv[c].w};
-          if (norm) {
-            const uint32_t g[4] = {gv[c].x, gv[c].y, gv[c].z, gv[c].w};
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const __nv_bfloat162 v = *reinterpret_cast<const __nv_bfloat162*>(&w[q]);
-              const __nv_bfloat162 gg = *reinterpret_cast<const __nv_bfloat162*>(&g[q]);
-              const __nv_bfloat162 y2 = __hmul2(gg, __hmul2(v, rinv2));  // bf16(scale * bf16(x * rinv)), model.py:276-277
-              w[q] = *reinterpret_cast<const uint32_t*>(&y2);
-            }
-          }
-          uint32_t xd[8];
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            // x * 2^sh is exact in fp32 (8-bit significand, power-of-two scale): the fma rounds once, to nearest even,
-            // and leaves MAGIC_BITS + X in the result's bit pattern
-            const uint32_t b0 = __float_as_uint(__fmaf_rn(__uint_as_float(w[q] << 16), scale, magic));
-            const uint32_t b1 = __float_as_uint(__fmaf_rn(__uint_as_float(w[q] & 0xffff0000u), scale, magic));
-            sxu += b0 + b1;                                          // the 2 MAGIC_BITS per pair are removed below
-            xd[2 * q] = (b0 + (0x00808080u - MAGIC_BITS)) ^ 0x00808080u;      // balanced_digits(X); byte 3 is unused
-            xd[2 * q + 1] = (b1 + (0x00808080u - MAGIC_BITS)) ^ 0x00808080u;
-          }
-          sxu -= 8u * MAGIC_BITS;
-          // 4 x 3 byte transposes: word (j, n) = digit n of elements 4j .. 4j+3  (B register j of lane t, column n)
           uint32_t dj[2][3];
-#pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            const uint32_t lo01 = __byte_perm(xd[4 * j], xd[4 * j + 1], 0x5140), hi01 = __byte_perm(xd[4 * j], xd[4 * j + 1], 0x7362);
-            const uint32_t lo23 = __byte_perm(xd[4 * j + 2], xd[4 * j + 3], 0x5140), hi23 = __byte_perm(xd[4 * j + 2], xd[4 * j + 3], 0x7362);
-            dj[j][0] = __byte_perm(lo01, lo23, 0x5410);
-            dj[j][1] = __byte_perm(lo01, lo23, 0x7632);
-            dj[j][2] = __byte_perm(hi01, hi23, 0x5410);
-          }
+          act_digits(xv[c], gv[c], norm, as, dj, sxu);
           // k = 64 kb + 32 c32 + 8 t + (0..7): plane n, k block kb, lane slot t, words 2 c32, 2 c32 + 1
           uint8_t* dst = smem + L.xf + (k >> 6) * 64 + ((k >> 3) & 3) * 16 + ((k >> 5) & 1) * 8;
 #pragma unroll
@@ -310,7 +229,7 @@ __global__ void __launch_bounds__(NTHREADS, 2) q4_gemv_kernel(const Params p) {
       // and goes on to the main loop; the epilogue warp, idle until the first unit is done, adds the 256 partials
       // in int64 (integers: the order does not matter)
       reinterpret_cast<int*>(smem + L.sxp)[tid] = (int)sxu;
-      if (tid == 0) *red_sh = sh;
+      if (tid == 0) *red_sh = as.sh;
       named_bar_sync(3, NT + 32);          // releases the epilogue warp too: digit planes, sum X and sh are ready
       if (tid == 0) tl_max(p.tl, 2);
     }
@@ -615,8 +534,6 @@ extern "C" int b2l_w8_untile_i8(const void* qw_tiled, void* qw, int N, int K, b2
 }
 
 namespace {
-constexpr int MAX_K = 12 * NCW * 32 * 8;   // 24576
-
 // Ring stages that fit `budget` bytes of shared memory at this K (0: not even two)
 template <int NDIG>
 int ring_stages(int K, uint32_t budget) {

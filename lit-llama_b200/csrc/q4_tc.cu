@@ -55,34 +55,6 @@ struct Params {
 };
 
 // ---------------------------------------------------------------- PTX wrappers
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t a, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(a), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t a) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(a) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t a, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(a), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t a, uint32_t parity) {
-  uint32_t ok;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(a), "r"(parity)
-        : "memory");
-  } while (!ok);
-}
-__device__ __forceinline__ void tma_bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t mbar) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
-      "l"(src), "r"(bytes), "r"(mbar)
-      : "memory");
-}
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ uint32_t cluster_ctarank() {
@@ -100,25 +72,11 @@ __device__ __forceinline__ float ld_dsmem_f32(uint32_t local_addr, uint32_t rank
   asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(ra) : "memory");
   return v;
 }
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
+// the barrier id in a register (bar_sync_c, b2l_common.cuh, takes it as an immediate)
+__device__ __forceinline__ void bar_sync_reg(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-// K-major, no-swizzle shared-memory matrix descriptor (sm_90 wgmma format):
-//   core matrix = 8 rows x 16 bytes, contiguous (128 B)
-//   LBO = byte distance between the two K halves of one K=16 MMA (next 8-k column)
-//   SBO = byte distance between 8-row groups along N
-__device__ __forceinline__ uint64_t make_b_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  return d;                // layout_type = 0 (no swizzle), base_offset = 0
-}
-
-__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 template <int NR> __device__ __forceinline__ void reg_fence(float (&d)[NR]) {
 #pragma unroll
   for (int i = 0; i < NR; ++i) asm volatile("" : "+f"(d[i])::"memory");
@@ -308,12 +266,12 @@ __global__ void __launch_bounds__(NTHREADS, 3) q4_linear_tc_kernel(const Params 
           }
           ss = warp_sum(ss);
           if (lane == 0) red[warp * MAX_M + m] = ss;
-          named_bar_sync(1, NCONV);
+          bar_sync_reg(1, NCONV);
           ss = 0.f;
 #pragma unroll
           for (int w = 0; w < NCONV / 32; ++w) ss += red[w * MAX_M + m];
           rinv = rms_rinv(ss, p.K, p.eps);
-          named_bar_sync(1, NCONV);
+          bar_sync_reg(1, NCONV);
         }
         float sx = 0.f;
 #pragma unroll
@@ -339,7 +297,7 @@ __global__ void __launch_bounds__(NTHREADS, 3) q4_linear_tc_kernel(const Params 
         }
         sx = warp_sum(sx);
         if (lane == 0) red[warp * MAX_M + m] = sx;
-        named_bar_sync(1, NCONV);
+        bar_sync_reg(1, NCONV);
         if (tid == 0) {
           float t = 0.f;
 #pragma unroll
@@ -348,7 +306,7 @@ __global__ void __launch_bounds__(NTHREADS, 3) q4_linear_tc_kernel(const Params 
         }
       }
       fence_proxy_async_smem();  // B operand written with generic stores, read by the tensor core
-      named_bar_sync(1, NCONV);
+      bar_sync_reg(1, NCONV);
       if (tid == 0) B2L_TRACE(3);
     }
 
@@ -359,7 +317,7 @@ __global__ void __launch_bounds__(NTHREADS, 3) q4_linear_tc_kernel(const Params 
     float acc[NN / 2];
 #pragma unroll
     for (int i = 0; i < NN / 2; ++i) acc[i] = 0.f;
-    const uint64_t bdesc0 = make_b_desc(sbase + L.xb, p.kcb, 128);
+    const uint64_t bdesc0 = make_desc(sbase + L.xb, p.kcb, 128);
     const uint32_t kcb16 = (uint32_t)p.kcb >> 4;   // descriptor address units per 8-k column
     int slot = 0;
     uint32_t rphase = 0;
@@ -395,7 +353,7 @@ __global__ void __launch_bounds__(NTHREADS, 3) q4_linear_tc_kernel(const Params 
         }
       }
       wgmma_commit();
-      wgmma_wait_all();   // the A registers are rewritten next stage
+      wgmma_wait<0>();   // the A registers are rewritten next stage
       reg_fence(acc);
       if (tid == 0 && st < 20) B2L_TRACE(44 + st);
       if (++slot == p.nst_ring) { slot = 0; rphase ^= 1; }
@@ -444,7 +402,7 @@ __global__ void __launch_bounds__(NTHREADS, 3) q4_linear_tc_kernel(const Params 
 #pragma unroll
       for (int m = 0; m < MAX_M; ++m)
         if (m < p.M) fin[m * TILE_N + tid] = rbf(tot[m]);
-      named_bar_sync(2, 128);
+      bar_sync_reg(2, 128);
       if (tid < 64) {
         const int oo = nt * 64 + tid;
 #pragma unroll

@@ -20,7 +20,6 @@
 //            written once by the thread that holds its accumulator.
 // Weights sit on the wgmma M side so that one kernel serves 2-row decode batches (BT = 16) and 4096-row prompts
 // (BT = 128): the token count only picks the N of the instruction.
-#include <cuda.h>   // CUtensorMap and its enums only: the encoder is fetched with cudaGetDriverEntryPoint (no libcuda link)
 #include <cuda_fp16.h>
 
 #include "b2l_common.cuh"
@@ -62,30 +61,6 @@ struct Params {
   __nv_bfloat16* y; int ldy;
   int M, N, K;
 };
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t a, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(a), "r"(count) : "memory"); }
-__device__ __forceinline__ void mbar_arrive(uint32_t a) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(a) : "memory"); }
-__device__ __forceinline__ void mbar_expect_tx(uint32_t a, uint32_t bytes) { asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(a), "r"(bytes) : "memory"); }
-__device__ __forceinline__ void mbar_wait(uint32_t a, uint32_t parity) {
-  uint32_t ok;
-  do {
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(ok) : "r"(a), "r"(parity) : "memory");
-  } while (!ok);
-}
-__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, uint32_t mbar) {
-  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
-               "l"(map), "r"(mbar), "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
-}
-// K-major, no-swizzle shared-memory matrix descriptor (sm_90 wgmma): core matrix = 8 rows x 16 B, contiguous
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  return d;
-}
 
 // D[64 x BT] (int32, registers) += A[64 x 32] (smem) * B[32 x BT] (smem), both K-major int8
 template <int BT> __device__ __forceinline__ void wgmma_s8(int (&d)[BT / 2], uint64_t adesc, uint64_t bdesc);
@@ -194,17 +169,17 @@ __global__ void __launch_bounds__(Cfg<BT, NWG>::NTHREADS, 1) q8_gemm_kernel(cons
       const int st = kt % C::NSTAGE;
       mbar_wait(bar_full + st * 8, (uint32_t)(kt / C::NSTAGE) & 1u);
       const uint32_t a_base = sbase + st * C::STAGE_BYTES, b_base = a_base + C::A_BYTES;
-      asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+      wgmma_fence();
       reg_fence(acc);
 #pragma unroll
       for (int j = 0; j < BK / 32; ++j)
         wgmma_s8<BT>(acc, make_desc(a_base + h * 64 * 16 + j * 2 * C::LBO_A, C::LBO_A, C::SBO), make_desc(b_base + j * 2 * C::LBO_B, C::LBO_B, C::SBO));
-      asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
-      asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");   // the group of stage kt - 1 has completed
+      wgmma_commit();
+      wgmma_wait<1>();   // the group of stage kt - 1 has completed
       reg_fence(acc);
       if (kt > 0 && lane == 0) mbar_arrive(bar_empty + ((kt - 1) % C::NSTAGE) * 8);
     }
-    asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+    wgmma_wait<0>();
     reg_fence(acc);
 
     // ===================== epilogue.  acc[4 c + e]: weight row 16 (warp % 4) + lane / 4 (+ 8 for e >= 2),
@@ -273,12 +248,9 @@ __global__ void __launch_bounds__(Cfg<BT, NWG>::NTHREADS, 1) q8_gemm_kernel(cons
   }
 }
 
-typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                             const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
 // int8 [rows, K] row-major as (16 B | rows, stride K | K/16 chunks, stride 16 B): a box of 16 x box_rows x 8 lands in
 // shared memory as [k16 chunk][row][16 B], the no-swizzle K-major core-matrix order wgmma reads
-static int encode_rows(EncodeFn encode, CUtensorMap* map, const void* base, int rows, int K, int box_rows) {
+static int encode_rows(PFN_cuTensorMapEncodeTiled encode, CUtensorMap* map, const void* base, int rows, int K, int box_rows) {
   const cuuint64_t dims[3] = {16, (cuuint64_t)rows, (cuuint64_t)(K / 16)};
   const cuuint64_t strides[2] = {(cuuint64_t)K, 16};
   const cuuint32_t box[3] = {16, (cuuint32_t)box_rows, (cuuint32_t)(BK / 16)};
@@ -293,7 +265,7 @@ static int encode_rows(EncodeFn encode, CUtensorMap* map, const void* base, int 
 }
 
 template <int BT, int NWG>
-static int launch_gemm(Params& p, EncodeFn encode, const void* cb, const void* ca, cudaStream_t stream) {
+static int launch_gemm(Params& p, PFN_cuTensorMapEncodeTiled encode, const void* cb, const void* ca, cudaStream_t stream) {
   using C = Cfg<BT, NWG>;
   if (int rc = encode_rows(encode, &p.wmap, cb, p.N, p.K, C::ROWS)) return rc;
   if (int rc = encode_rows(encode, &p.amap, ca, padded_rows(p.M), p.K, BT)) return rc;
@@ -331,12 +303,7 @@ extern "C" int b2l_q8_gemm(const void* x, int ldx, const void* cb, const void* s
   B2L_CHECK_ARG(workspace_bytes >= b2l_q8_gemm_workspace_bytes(M, K), "b2l_q8_gemm: workspace of %zu bytes is too small (%zu needed)",
                 workspace_bytes, b2l_q8_gemm_workspace_bytes(M, K));
   B2L_CHECK_SUPPORTED(flags == 0, "b2l_q8_gemm: flags must be 0");
-  static EncodeFn encode = [] {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) fn = nullptr;
-    return (EncodeFn)fn;
-  }();
+  const PFN_cuTensorMapEncodeTiled encode = tensor_map_encoder();
   if (encode == nullptr) {
     set_error("b2l_q8_gemm: cuTensorMapEncodeTiled is not available from this driver");
     return B2L_E_STATE;

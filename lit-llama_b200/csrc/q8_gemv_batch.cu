@@ -63,32 +63,6 @@ __host__ __device__ inline size_t ws_cols(int K, int M) { return ws_nout(K, M) +
 __host__ __device__ inline size_t ws_xo(int K, int M) { return ws_cols(K, M) + (size_t)K * 4; }
 __host__ __device__ inline size_t ws_bytes(int K, int M) { return ws_xo(K, M) + (size_t)M * K * 2; }
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t a, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(a), "r"(count) : "memory"); }
-__device__ __forceinline__ void mbar_arrive(uint32_t a) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(a) : "memory"); }
-__device__ __forceinline__ void mbar_expect_tx(uint32_t a, uint32_t bytes) { asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(a), "r"(bytes) : "memory"); }
-__device__ __forceinline__ void mbar_wait(uint32_t a, uint32_t parity) {
-  uint32_t ok;
-  do {
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(ok) : "r"(a), "r"(parity) : "memory");
-  } while (!ok);
-}
-__device__ __forceinline__ void tma_bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t mbar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes), "r"(mbar) : "memory");
-}
-template <int ID> __device__ __forceinline__ void bar_sync_c(int n) { asm volatile("bar.sync %0, %1;" ::"n"(ID), "r"(n) : "memory"); }
-template <int ID> __device__ __forceinline__ void bar_arrive_c(int n) { asm volatile("bar.arrive %0, %1;" ::"n"(ID), "r"(n) : "memory"); }
-__device__ __forceinline__ void imma_16832(int (&d)[4], const uint4& a, uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k32.row.col.s32.s8.s8.s32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
-      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3])
-      : "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ uint4 ldmatrix_x4(uint32_t addr) {
-  uint4 r;
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "r"(addr) : "memory");
-  return r;
-}
 // coherent loads of what the prep launch wrote (PDL: griddepcontrol.wait orders coherent loads only)
 __device__ __forceinline__ uint32_t ld_coherent_u32(const void* p) {
   uint32_t v;
@@ -406,7 +380,7 @@ __global__ void __launch_bounds__(NTHREADS, 2) q8_gemv_batch_kernel(const BParam
           for (int c = 0; c < 4; ++c) {
             const uint4 a = ldmatrix_x4(sbase + L.ring + slot * SB + lm_row + warp * KB + (2 * c + lm_unit) * 16);
 #pragma unroll
-            for (int G = 0; G < NG; ++G) imma_16832(acc[G][c & 1], a, bb[G][2 * c], bb[G][2 * c + 1]);
+            for (int G = 0; G < NG; ++G) mma_s8s8_16832(acc[G][c & 1], a, bb[G][2 * c], bb[G][2 * c + 1]);
           }
         }
         __syncwarp();

@@ -53,7 +53,6 @@ constexpr int KBP = HALF_STAGE_BYTES / tile_bytes(true);   // 8 k blocks per sta
 static_assert(KBP == NCW, "one k block per consumer warp and stage");
 constexpr int PLANE_KB_BYTES = 64;           // one digit plane of one k block: [4 t][16 B]
 constexpr int BMAX_STAGES = 12;
-constexpr int MAX_K = 12 * 256 * 8;          // 24576, as b2l_w8_gemv
 
 __host__ __device__ inline uint32_t xkb_bytes(int M) { return (uint32_t)(NDIG * M * PLANE_KB_BYTES); }   // digits of one k block
 // weights of a stage: KBP k blocks of both 16-row blocks of a unit (16 KB at 8 bits, 8 KB at 4 bits)
@@ -89,7 +88,8 @@ __host__ __device__ inline BSmem bsmem_layout(int nst, int M, bool w8) {
 }
 
 // ---------------------------------------------------------------- step 1: activation rows -> digit planes
-// The consumer-warp prologue of q4_gemv_kernel for one row per CTA (same thread split, arithmetic and reduction order).
+// The consumer-warp prologue of q4_gemv_kernel for one row per CTA: the same activation conversion (act_pass1 /
+// act_scale / act_digits, q4_mma_common.cuh), thread split and reduction order.
 template <int MAXC>
 __global__ void __launch_bounds__(256) w8_batch_prep_kernel(const __nv_bfloat16* x, int ldx, int M, int K,
                                                             const __nv_bfloat16* __restrict__ norm_scale, float eps,
@@ -98,7 +98,6 @@ __global__ void __launch_bounds__(256) w8_batch_prep_kernel(const __nv_bfloat16*
   __shared__ long long sred[8];
   const int n = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   constexpr int NT = 256;
-  constexpr uint32_t MAGIC_BITS = 0x4B400000u;   // 1.5 * 2^23
   pdl_launch_dependents();  // the linear may start streaming its weights
   const bool norm = norm_scale != nullptr;
   uint4 xv[MAXC], gv[MAXC];
@@ -116,28 +115,8 @@ __global__ void __launch_bounds__(256) w8_batch_prep_kernel(const __nv_bfloat16*
     if (k < K) xv[c] = ld_coherent_u4(x + (size_t)n * ldx + k);   // written by the previous kernel (PDL): coherent load
   }
   const int nchunk = (K + NT * 8 - 1) / (NT * 8);
-  float ss = 0.f;
-  __nv_bfloat162 amax2 = __float2bfloat162_rn(0.f);
-#pragma unroll
-  for (int c = 0; c < MAXC; ++c) {
-    if (c < nchunk) {
-      const uint32_t w[4] = {xv[c].x, xv[c].y, xv[c].z, xv[c].w};
-      const uint32_t g[4] = {gv[c].x, gv[c].y, gv[c].z, gv[c].w};
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const __nv_bfloat162 v = *reinterpret_cast<const __nv_bfloat162*>(&w[q]);
-        if (norm) {
-          amax2 = __hmax2(amax2, __habs2(__hmul2(v, *reinterpret_cast<const __nv_bfloat162*>(&g[q]))));
-          const __nv_bfloat162 sq = __hmul2(v, v);
-          const uint32_t su = *reinterpret_cast<const uint32_t*>(&sq);
-          ss += __uint_as_float(su << 16) + __uint_as_float(su & 0xffff0000u);
-        } else {
-          amax2 = __hmax2(amax2, __habs2(v));
-        }
-      }
-    }
-  }
-  float mx = fmaxf(__low2float(amax2), __high2float(amax2));
+  float ss, mx;
+  act_pass1<MAXC>(xv, gv, nchunk, norm, ss, mx);
   ss = warp_sum(ss);
   mx = warp_max(mx);
   if (lane == 0) { red[warp] = ss; red[8 + warp] = mx; }
@@ -145,53 +124,15 @@ __global__ void __launch_bounds__(256) w8_batch_prep_kernel(const __nv_bfloat16*
   ss = 0.f; mx = 0.f;
 #pragma unroll
   for (int w = 0; w < 8; ++w) { ss += red[w]; mx = fmaxf(mx, red[8 + w]); }
-  float rinv = 1.f;
-  if (norm) {
-    rinv = rms_rinv(ss, K, eps);
-    mx = mx * rinv * 1.02f;   // > max |bf16(g bf16(x rinv))|: the bound and its proof are q4_gemv.cu's
-  }
-  const int e = (int)((__float_as_uint(mx) >> 23) & 0xffu) - 127;
-  int sh = (8 * NDIG - 3) - e;
-  sh = max(-126, min(126, sh));
-  const float scale = __uint_as_float((uint32_t)(sh + 127) << 23);
-  const float magic = __uint_as_float(MAGIC_BITS);
-  const __nv_bfloat162 rinv2 = __float2bfloat162_rn(rinv);
+  const ActScale as = act_scale<NDIG>(ss, mx, norm, K, eps);
   const uint32_t XKB = xkb_bytes(M);
   uint32_t sxu = 0;
 #pragma unroll
   for (int c = 0; c < MAXC; ++c) {
     const int k = (c * NT + tid) * 8;
     if (c < nchunk && k < K) {
-      uint32_t w[4] = {xv[c].x, xv[c].y, xv[c].z, xv[c].w};
-      if (norm) {
-        const uint32_t g[4] = {gv[c].x, gv[c].y, gv[c].z, gv[c].w};
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const __nv_bfloat162 v = *reinterpret_cast<const __nv_bfloat162*>(&w[q]);
-          const __nv_bfloat162 gg = *reinterpret_cast<const __nv_bfloat162*>(&g[q]);
-          const __nv_bfloat162 y2 = __hmul2(gg, __hmul2(v, rinv2));
-          w[q] = *reinterpret_cast<const uint32_t*>(&y2);
-        }
-      }
-      uint32_t xd[8];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const uint32_t b0 = __float_as_uint(__fmaf_rn(__uint_as_float(w[q] << 16), scale, magic));
-        const uint32_t b1 = __float_as_uint(__fmaf_rn(__uint_as_float(w[q] & 0xffff0000u), scale, magic));
-        sxu += b0 + b1;
-        xd[2 * q] = (b0 + (0x00808080u - MAGIC_BITS)) ^ 0x00808080u;
-        xd[2 * q + 1] = (b1 + (0x00808080u - MAGIC_BITS)) ^ 0x00808080u;
-      }
-      sxu -= 8u * MAGIC_BITS;
       uint32_t dj[2][3];
-#pragma unroll
-      for (int j = 0; j < 2; ++j) {
-        const uint32_t lo01 = __byte_perm(xd[4 * j], xd[4 * j + 1], 0x5140), hi01 = __byte_perm(xd[4 * j], xd[4 * j + 1], 0x7362);
-        const uint32_t lo23 = __byte_perm(xd[4 * j + 2], xd[4 * j + 3], 0x5140), hi23 = __byte_perm(xd[4 * j + 2], xd[4 * j + 3], 0x7362);
-        dj[j][0] = __byte_perm(lo01, lo23, 0x5410);
-        dj[j][1] = __byte_perm(lo01, lo23, 0x7632);
-        dj[j][2] = __byte_perm(hi01, hi23, 0x5410);
-      }
+      act_digits(xv[c], gv[c], norm, as, dj, sxu);
       // k = 64 kb + 32 c32 + 8 t + (0..7): k block kb, plane 3n + d, lane slot t, words 2 c32, 2 c32 + 1
       uint8_t* dst = ws + (size_t)(k >> 6) * XKB + (size_t)(NDIG * n) * PLANE_KB_BYTES + ((k >> 3) & 3) * 16 + ((k >> 5) & 1) * 8;
 #pragma unroll
@@ -210,7 +151,7 @@ __global__ void __launch_bounds__(256) w8_batch_prep_kernel(const __nv_bfloat16*
     for (int w = 0; w < 8; ++w) t += sred[w];
     long long* sum_x = reinterpret_cast<long long*>(ws + frag_bytes(K, M));
     sum_x[n] = t;
-    reinterpret_cast<int*>(sum_x + MAXB)[n] = sh;
+    reinterpret_cast<int*>(sum_x + MAXB)[n] = as.sh;
   }
 }
 
