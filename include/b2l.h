@@ -597,6 +597,22 @@ typedef struct b2l_lora {
  * arguments are rejected before any launch. */
 int b2l_lora_apply(const b2l_lora* lora, const void* x, int ldx, const void* norm_scale, float eps,
                    void* y, int ldy, int M, int N, int K, int flags, b2l_stream_t stream);
+/* Multi-LoRA: each of M = 1..16 rows adds its own term of one linear.  sets: HOST array of
+ * n_sets (1..B2L_LORA_MAX_SETS) terms; they may differ in r, scaling and enabled mask but
+ * share n_groups.  row_set: device int32 [M]; row m adds the term of sets[row_set[m]], -1 adds
+ * nothing and leaves row m of y unwritten.  An entry outside -1..n_sets-1 is a caller error;
+ * the kernel treats it as -1 and never reads out of bounds.  The host never reads row_set,
+ * so a captured graph stays valid when rows change sets; the kernel reads it before
+ * griddepcontrol.wait, so under B2L_F_PDL it must not be written by the previous launch.
+ * Row m of y equals, bit for bit, b2l_lora_apply(&sets[row_set[m]], ...) on that row alone;
+ * each set's lora_A / lora_B are read once per output slice whatever rows share it.
+ * x, norm_scale, eps, ldx, ldy, flags as b2l_lora_apply.  Bad arguments (every set through
+ * b2l_lora_apply's checks, a null row_set, M, n_sets, differing n_groups) are rejected
+ * before any launch. */
+#define B2L_LORA_MAX_SETS 64
+int b2l_lora_apply_rows(const b2l_lora* sets, int n_sets, const int32_t* row_set, const void* x, int ldx,
+                        const void* norm_scale, float eps, void* y, int ldy, int M, int N, int K, int flags,
+                        b2l_stream_t stream);
 
 /* kv_caches as the reference would hold them (logical order): un-rotates the ring
  * into `out` [B, nh, S, hs]. */
@@ -707,6 +723,13 @@ typedef struct b2l_decode_args {
                                 runs b2l_q8_linear_batch instead: two launches per linear. */
   b2l_q8_weight q8_lm_head;
   float q8_threshold;        /* B2L_F_Q8: Linear8bitLt.threshold of every linear          */
+  const b2l_lora* lora_sets; /* Multi-LoRA: HOST [n_lora_sets][n_layer] c_attn terms; r == 0 = that set has no
+                                term in that layer.  Each layer where some set has a term runs
+                                b2l_lora_apply_rows (rms_1 as the norm) where `loras` would run b2l_lora_apply:
+                                row b adds set lora_row_set[b]'s term.  NULL = off.  Not with `loras`, `plan`,
+                                `affines` / `lm_head_affine` or B2L_F_STEPWISE (B2L_E_UNSUPPORTED). */
+  int n_lora_sets;           /* 1..B2L_LORA_MAX_SETS                                      */
+  const int32_t* lora_row_set; /* device int32 [B]: row b's set, -1 = none (read by the kernels only) */
 } b2l_decode_args;
 
 /* With B2L_F_STEPWISE the B = 2..16 rows are consecutive tokens of ONE sequence: idx [B], input_pos int64 [B] holding

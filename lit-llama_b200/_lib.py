@@ -75,6 +75,7 @@ class LoRA(C.Structure):
 
 
 LORA_MAX_R = 64   # B2L_LORA_MAX_R
+LORA_MAX_SETS = 64   # B2L_LORA_MAX_SETS
 
 RAGGED_MAX_SEQ = 16   # B2L_RAGGED_MAX_SEQ
 
@@ -123,6 +124,7 @@ class DecodeArgs(C.Structure):
         ("plan", c_void_p), ("adapters", C.POINTER(AdapterPrefix)), ("loras", C.POINTER(LoRA)),
         ("affines", C.POINTER(LayerAffine)), ("lm_head_affine", OutAffine),
         ("q8_layers", C.POINTER(Q8Layer)), ("q8_lm_head", Q8Weight), ("q8_threshold", c_float),
+        ("lora_sets", C.POINTER(LoRA)), ("n_lora_sets", c_int), ("lora_row_set", c_void_p),
     ]
 
 
@@ -204,6 +206,8 @@ _SIGS = {
                                      c_int, c_int, c_int, c_int, c_int, C.POINTER(AdapterPrefix), c_void_p]),
     "b2l_lora_apply": (c_int, [C.POINTER(LoRA), c_void_p, c_int, c_void_p, c_float, c_void_p, c_int, c_int, c_int, c_int,
                                c_int, c_void_p]),
+    "b2l_lora_apply_rows": (c_int, [C.POINTER(LoRA), c_int, c_void_p, c_void_p, c_int, c_void_p, c_float, c_void_p, c_int,
+                                    c_int, c_int, c_int, c_int, c_void_p]),
     "b2l_tp_buffer_bytes": (c_size_t, [c_int, c_int]),
     "b2l_tp_allreduce": (c_int, [C.POINTER(TPComm), c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "b2l_ring_advance": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p]),

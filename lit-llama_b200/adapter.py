@@ -144,13 +144,13 @@ class LLaMA(llama.LLaMA):
         super().expand_cache(B)
         self._prefix_views(B)
 
-    def refill_rows(self, prompts, rows, max_seq_length: int) -> torch.Tensor:
+    def refill_rows(self, prompts, rows, max_seq_length: int, adapters=None) -> torch.Tensor:
         """model.LLaMA.refill_rows (prefill_rows too); the prefix store is brought up to date first, since the packed
         prefill reads it, and the prefix views follow B as in expand_cache."""
         self._check_prompts(prompts, max_seq_length, "refill_rows")
         if self._adapter_layers() and (self._adapter_gen != WEIGHTS_GENERATION[0] or self._adapter_arr is None):
             self._build_prefixes(1, prompts[0].device)
-        out = super().refill_rows(prompts, rows, max_seq_length)
+        out = super().refill_rows(prompts, rows, max_seq_length, adapters)
         self._prefix_views(self._kv_store.shape[2])
         return out
 

@@ -9,6 +9,11 @@ extern void* g_attn_timeline;
 int decode_step_persistent(const b2l_decode_args* d, b2l_stream_t stream);   // decode_mega.cu
 int check_adapter_prefix(const b2l_adapter_prefix* pre, const char* who);     // attention.cu
 int check_lora(const b2l_lora* lo, int N, int K, const char* who);            // lora.cu
+int check_lora_sets(const b2l_lora* sets, size_t stride, int n_sets, int N, int K, bool empty_ok, unsigned* any_on,
+                    int* n_groups, const char* who);
+int lora_rows(const b2l_lora* sets, size_t stride, int n_sets, bool empty_ok, const int32_t* row_set, const void* x,
+              int ldx, const void* norm_scale, float eps, void* y, int ldy, int M, int N, int K, int flags,
+              b2l_stream_t stream, const char* who);
 
 static thread_local char g_err[512] = "";
 
@@ -178,6 +183,13 @@ extern "C" int b2l_decode_step_launches(const b2l_decode_args* d) {
   // a LoRA layer adds its low-rank term's launch behind c_attn
   if (d->loras != nullptr)
     for (int l = 0; l < d->n_layer; ++l) n += d->loras[l].r != 0;
+  // per-row LoRA: one launch in each layer where some set has a term
+  if (d->lora_sets != nullptr && d->n_lora_sets >= 1 && d->n_lora_sets <= B2L_LORA_MAX_SETS)
+    for (int l = 0; l < d->n_layer; ++l) {
+      bool any = false;
+      for (int s = 0; s < d->n_lora_sets; ++s) any |= d->lora_sets[(size_t)s * d->n_layer + l].r != 0;
+      n += any;
+    }
   return n;
 }
 
@@ -245,6 +257,21 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
       if (int rc = check_lora(&d->loras[l], 3 * d->n_embd, d->n_embd, "b2l_decode_step")) return rc;
     }
   }
+  if (d->lora_sets != nullptr) {   // per-row LoRA: every layer's sets checked here, before any launch
+    B2L_CHECK_SUPPORTED(d->loras == nullptr, "b2l_decode_step: lora_sets and loras do not combine");
+    B2L_CHECK_SUPPORTED(d->plan == nullptr, "b2l_decode_step: lora_sets do not run in the persistent kernel (plan must be NULL)");
+    B2L_CHECK_SUPPORTED(d->affines == nullptr && d->lm_head_affine.scale == nullptr && d->lm_head_affine.bias == nullptr,
+                        "b2l_decode_step: lora_sets and LLaMA-Adapter v2 affines do not combine");
+    B2L_CHECK_SUPPORTED(!stepwise, "b2l_decode_step: lora_sets do not run under B2L_F_STEPWISE (one sequence, one adapter: use loras)");
+    B2L_CHECK_ARG(d->lora_row_set != nullptr, "b2l_decode_step: lora_sets need lora_row_set");
+    for (int l = 0; l < d->n_layer; ++l) {
+      unsigned any_on = 0;
+      int n_groups = 0;
+      if (int rc = check_lora_sets(d->lora_sets + l, (size_t)d->n_layer, d->n_lora_sets, 3 * d->n_embd, d->n_embd, true,
+                                   &any_on, &n_groups, "b2l_decode_step"))
+        return rc;
+    }
+  }
   // LLaMA-Adapter v2: every linear's affine runs in its own batch-1 launch (b2l_q4_linear_args::out_affine)
   const bool any_affine = d->affines != nullptr || d->lm_head_affine.scale != nullptr || d->lm_head_affine.bias != nullptr;
   if (any_affine) {
@@ -293,6 +320,11 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
     // LoRA on c_attn (lora.py:308-326): the low-rank term from rms_1(x), added into qkv in place
     if (d->loras != nullptr && d->loras[l].r != 0 &&
         (rc = b2l_lora_apply(&d->loras[l], d->x, C, L.rms_1, d->eps, d->qkv, 3 * C, B, 3 * C, C, fl & B2L_F_PDL, stream)))
+      return rc;
+    // per-row LoRA: row b adds set lora_row_set[b]'s term (no launch in a layer where no set has one)
+    if (d->lora_sets != nullptr &&
+        (rc = lora_rows(d->lora_sets + l, (size_t)d->n_layer, d->n_lora_sets, true, d->lora_row_set, d->x, C, L.rms_1,
+                        d->eps, d->qkv, 3 * C, B, 3 * C, C, fl & B2L_F_PDL, stream, "b2l_decode_step")))
       return rc;
     g_attn_timeline = tl();
     const b2l_adapter_prefix* pre = (d->adapters != nullptr && d->adapters[l].len != 0) ? &d->adapters[l] : nullptr;

@@ -14,6 +14,7 @@ step (speculative sampling); its greedy output is `generate()`'s token for token
 `main()` mirrors the reference CLI with argparse
 (jsonargparse and lightning are not dependencies of this path)."""
 import os
+import re
 import sys
 import time
 from collections import deque
@@ -361,6 +362,7 @@ def generate_prompts(
     temperature: float = 1.0,
     top_k: Optional[int] = None,
     eos_id: Optional[int] = None,
+    adapters: Optional[Sequence[int]] = None,
 ) -> List[torch.Tensor]:
     """Continuations of 1..16 different prompts (1-D tensors of any lengths), decoded together: a list of 1-D tensors,
     row b the prompt `prompts[b]` plus its new tokens (generate.py:20-91 per row).
@@ -374,7 +376,10 @@ def generate_prompts(
 
     With `eos_id`, a row that draws it ends there, the eos token included; finished rows keep riding along (their later
     tokens are dropped) and the loop stops once every row has finished, reading one flag per step.  The cache is left
-    at B rows: call `model.reset_cache()` before a batch-1 `generate()`."""
+    at B rows: call `model.reset_cache()` before a batch-1 `generate()`.
+
+    `adapters` (multi-LoRA, lit_llama_b200.lora.add_lora_adapter): one adapter id per prompt (-1: the base alone);
+    prompt b is prefilled and decoded with its own adapter (LLaMA.prefill_rows)."""
     B = len(prompts)
     if not 1 <= B <= MAX_SAMPLES:
         raise ValueError(f"generate_prompts: {B} prompts; 1..{MAX_SAMPLES} (the batched decode step's range)")
@@ -398,7 +403,8 @@ def generate_prompts(
 
     for i in range(max_new_tokens):
         if i == 0:
-            rows = model.prefill_rows(prompts, max_seq_length)
+            rows = (model.prefill_rows(prompts, max_seq_length) if adapters is None
+                    else model.prefill_rows(prompts, max_seq_length, adapters))
         else:
             rows = model(x, max_seq_length, input_pos)[:, -1]
             input_pos = input_pos + 1
@@ -431,6 +437,7 @@ def generate_stream(
     top_k: Optional[int] = None,
     eos_id: Optional[int] = None,
     stats: Optional[dict] = None,
+    adapters: Optional[Sequence[int]] = None,
 ) -> List[torch.Tensor]:
     """Continuations of any number of prompts (1-D tensors of any lengths) on B = min(batch_size, len(prompts)) rows
     (batch_size 1..16), refilling each finished row with the next prompt while the others keep decoding (continuous
@@ -453,10 +460,17 @@ def generate_stream(
     `generate_prompts`'s for the same seed.  `stats`, when given, receives "steps" (sampling launches), "refills"
     (prompts admitted after the first prefill), "packed" / "alone" (prompts prefilled in a packed pass / one at a time,
     LLaMA.refill_rows) and "idle_row_steps" (row-steps whose token was dropped).  The cache is left at B rows: call
-    `model.reset_cache()` before a batch-1 `generate()`."""
+    `model.reset_cache()` before a batch-1 `generate()`.
+
+    `adapters` (multi-LoRA, lit_llama_b200.lora.add_lora_adapter): one adapter id per prompt (-1: the base alone).
+    Prompt i is prefilled and decoded with adapter i; a refilled row moves to its new prompt's adapter in the step
+    its prefill runs.  On the exact batched steps prompt i then gets `generate()`'s tokens on a batch-1 model that
+    carries only that adapter."""
     n = len(prompts)
     if n == 0:
         raise ValueError("generate_stream: no prompts")
+    if adapters is not None and len(adapters) != n:
+        raise ValueError(f"generate_stream: {len(adapters)} adapters for {n} prompts")
     if not 1 <= int(batch_size) <= MAX_SAMPLES:
         raise ValueError(f"generate_stream: batch_size = {batch_size}; 1..{MAX_SAMPLES} (the batched decode step's range)")
     for p in prompts:
@@ -497,7 +511,9 @@ def generate_stream(
     step = 0
     while True:
         if step == 0:
-            rows = model.prefill_rows([prompts[i] for i in serving], S)
+            first_rows = [prompts[i] for i in serving]
+            rows = (model.prefill_rows(first_rows, S) if adapters is None
+                    else model.prefill_rows(first_rows, S, [adapters[i] for i in serving]))
         else:
             rows = model(x, S, input_pos)[:, -1]
             input_pos = input_pos + 1
@@ -505,7 +521,9 @@ def generate_stream(
                 ids = [i for _, i in pending]
                 admit(ids)
                 ridx = torch.tensor([r for r, _ in pending], device=device)
-                rows[ridx] = model.refill_rows([prompts[i] for i in ids], [r for r, _ in pending], S)
+                new_rows = ([prompts[i] for i in ids], [r for r, _ in pending], S)
+                rows[ridx] = (model.refill_rows(*new_rows) if adapters is None
+                              else model.refill_rows(*new_rows, [adapters[i] for i in ids]))
                 input_pos[ridx] = torch.tensor([Ts[i] for i in ids], dtype=torch.int64, device=device).view(-1, 1)
                 st["refills"] += len(ids)
                 pending = []
@@ -552,13 +570,18 @@ def main(
     draft_quantize: Optional[str] = None,
     num_draft: int = 4,
     stream: bool = False,
+    lora_path: Optional[Sequence[Path]] = None,
+    lora_alpha: float = 16,
 ) -> None:
     """generate.py:94-155 without Fabric: bf16 on cuda:0, same prints on stderr.  `batch_size` > 1 draws the samples
     in groups of up to `batch_size` (at most 16) through `generate_batch`, on the model's exact batched decode step.
     `prompts_file` (one prompt per line) replaces `prompt`: the prompts are decoded in groups of `batch_size` through
     `generate_prompts`, `num_samples` times each; with `stream` they go through `generate_stream` on `batch_size` rows,
     each finished row taking the next prompt.  `draft_checkpoint_path` (with `draft_quantize`) loads a draft model
-    and decodes each sample with `generate_speculative`, `num_draft` draft tokens per round."""
+    and decodes each sample with `generate_speculative`, `num_draft` draft tokens per round.  `lora_path` (one or
+    more LoRA checkpoints over a quantized base) builds the model under `lora(r, lora_alpha, 0)`, r from the first
+    file, loads the first as adapter 0 (generate/lora.py's way) and registers the others with `add_lora_adapter`;
+    with `prompts_file` a line may then start with `<k>\t` to decode with adapter k (adapter 0 without it)."""
     if not 1 <= batch_size <= MAX_SAMPLES:
         raise ValueError(f"batch_size = {batch_size}; 1..{MAX_SAMPLES}")
     from sentencepiece import SentencePieceProcessor
@@ -568,19 +591,27 @@ def main(
     assert tokenizer_path.is_file(), tokenizer_path
     device = torch.device("cuda", 0)
 
-    def load(path: Path, mode: Optional[str]) -> LLaMA:
+    loras = [torch.load(p, map_location="cpu", weights_only=True) for p in lora_path or []]
+
+    def load(path: Path, mode: Optional[str], loras=()) -> LLaMA:
         print("Loading model ...", file=sys.stderr)
         t0 = time.time()
         checkpoint = torch.load(path, map_location="cpu", weights_only=True, mmap=True)
         name = llama_model_lookup(checkpoint)
         prev = torch.get_default_dtype()
         torch.set_default_dtype(torch.bfloat16)  # what Fabric's bf16-true does inside init_module
+        # LoRA: r from the first adapter's lora_A (q and v enabled: 2 r rows), as generate/lora.py builds it
+        r = next(v.shape[0] // 2 for k, v in loras[0].items() if k.endswith("lora_A")) if loras else 0
         try:
-            with torch.device(device), quantization(mode=mode):
+            with torch.device(device), quantization(mode=mode), lora_ctx(r=r, alpha=lora_alpha, dropout=0.0, enabled=bool(loras)):
                 m = LLaMA.from_name(name)
         finally:
             torch.set_default_dtype(prev)
-        m.load_state_dict(checkpoint)
+        m.load_state_dict(checkpoint, strict=not loras)
+        if loras:
+            m.load_state_dict(loras[0], strict=False)
+            for sd in loras[1:]:
+                add_lora_adapter(m, sd, alpha=lora_alpha)
         print(f"Time to load model: {time.time() - t0:.02f} seconds.", file=sys.stderr)
         m.eval()
         if mode in ("gptq.int4", "gptq.int8") and os.environ.get("B2L_COMPACT", "1") != "0":
@@ -590,7 +621,9 @@ def main(
                 pass
         return m
 
-    model = load(checkpoint_path, quantize)
+    from .lora import add_lora_adapter, lora as lora_ctx
+
+    model = load(checkpoint_path, quantize, loras)
     draft = None
     if draft_checkpoint_path is not None:
         assert Path(draft_checkpoint_path).is_file(), draft_checkpoint_path
@@ -612,6 +645,11 @@ def main(
             model.int8_step = True
     if prompts_file is not None:
         lines = [ln for ln in Path(prompts_file).read_text().splitlines() if ln.strip()]
+        adapters = None
+        if loras:   # "<k>\t" in front of a line picks adapter k
+            picks = [re.match(r"(-?\d+)\t(.*)", ln) for ln in lines]
+            adapters = [int(m.group(1)) if m else 0 for m in picks]
+            lines = [m.group(2) if m else ln for m, ln in zip(picks, lines)]
         prompts = [torch.tensor([sp.bos_id()] + sp.encode(ln), dtype=torch.int, device=device) for ln in lines]
         k = 0
         for _ in range(num_samples):
@@ -620,7 +658,7 @@ def main(
                 torch.cuda.synchronize()
                 t0 = time.perf_counter()
                 ys = generate_stream(model, prompts, max_new_tokens, batch_size=batch_size, temperature=temperature,
-                                     top_k=top_k)
+                                     top_k=top_k, adapters=adapters)
                 torch.cuda.synchronize()
                 t = time.perf_counter() - t0
                 model.reset_cache()
@@ -634,7 +672,8 @@ def main(
                 k += 1
                 torch.cuda.synchronize()
                 t0 = time.perf_counter()
-                ys = generate_prompts(model, group, max_new_tokens, temperature=temperature, top_k=top_k)
+                ys = generate_prompts(model, group, max_new_tokens, temperature=temperature, top_k=top_k,
+                                      adapters=None if adapters is None else adapters[first:first + batch_size])
                 torch.cuda.synchronize()
                 t = time.perf_counter() - t0
                 model.reset_cache()
@@ -698,6 +737,10 @@ def cli() -> None:
                     help="a smaller model's checkpoint: decode with generate_speculative, this model proposing tokens")
     ap.add_argument("--draft_quantize", default=None, choices=[None, "llm.int8", "gptq.int4", "gptq.int8"])
     ap.add_argument("--num_draft", type=int, default=4, help=f"draft tokens per speculative round (1..{MAX_DRAFT})")
+    ap.add_argument("--lora_path", type=Path, action="append", default=None,
+                    help="a LoRA checkpoint over a quantized base (repeatable): the first is adapter 0, the next 1, 2, ...; "
+                         "a --prompts_file line starting with '<k>\\t' decodes with adapter k")
+    ap.add_argument("--lora_alpha", type=float, default=16, help="LoRA alpha of every --lora_path (scaling = alpha / r)")
     a = ap.parse_args()
     if a.draft_checkpoint_path is not None and (a.batch_size != 1 or a.prompts_file is not None):
         ap.error("--draft_checkpoint_path decodes one sequence at a time (batch_size 1, no prompts_file)")

@@ -15,6 +15,11 @@ Same public names, signatures, parameter names, shapes and state-dict keys as th
     plus `lora_A` / `lora_B`.  gptq.int4 / gptq.int8 models decode on the whole-token step, which adds the term
     between c_attn and the attention (`b2l_decode_args::loras`); the kernel reads `lora_A` / `lora_B` in place, and
     loading them bumps the weight generation so every baked pointer is rebuilt.
+
+Multi-LoRA: `add_lora_adapter` registers more adapters on such a model (adapter 0 is its own lora_A / lora_B, -1 the
+base alone).  `LLaMA.prefill_rows` / `refill_rows` and `generate_prompts` / `generate_stream` with `adapters=` pick
+one per prompt: each row of the batched decode step then adds its own adapter's term (`b2l_lora_apply_rows`), and
+each prompt's prefill adds its adapter's (`b2l_lora_apply` on its tokens).
 """
 import ctypes as C
 import functools
@@ -169,6 +174,10 @@ class _QuantizedLoRA(LoRALayer):
     and kernels, plus lora_A / lora_B and the unmerged term."""
 
     _base: type = None
+    #: the per-row adapter choice LLaMA sets around a multi-LoRA call (None: lora_A / lora_B on every row):
+    #: ("rows", sel) row m adds adapter sel[m] (device int32, >= M entries); ("one", k, sel) every row adds adapter k;
+    #: ("segments", [(start, len, k), ...]) the packed prompts of refill_rows, each its own adapter
+    _lora_route = None
 
     def __init__(self, in_features: int, out_features: int, r: int = 0, lora_alpha: int = 1, lora_dropout: float = 0.0,
                  enable_lora: List[bool] = [False], fan_in_fan_out: bool = False, merge_weights: bool = True, *,
@@ -187,7 +196,54 @@ class _QuantizedLoRA(LoRALayer):
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         y = self._base.forward(self, x)
-        return self._add_lora(x, y) if self._has_lora else y
+        if not self._has_lora:
+            return y
+        return self._add_lora(x, y) if self._lora_route is None else self._add_lora_route(x, y)
+
+    @property
+    def _adapters(self) -> List[Tuple[torch.Tensor, torch.Tensor, float, int]]:
+        """The adapters add_lora_adapter registered (1, 2, ...): (lora_A, lora_B, scaling, r), bf16 on the device.
+        Plain attributes, not parameters: state_dict() does not change."""
+        if "_extra_adapters" not in self.__dict__:
+            self.__dict__["_extra_adapters"] = []
+        return self.__dict__["_extra_adapters"]
+
+    def lora_set(self, k: int) -> Tuple[L.LoRA, tuple]:
+        """The b2l_lora of adapter k (0: lora_A / lora_B) and the tensors it points at."""
+        if k == 0:
+            return self.lora_weights()
+        A, B, scaling, r = self._adapters[k - 1]
+        mask = sum(1 << g for g, on in enumerate(self.enable_lora) if on)
+        return L.LoRA(A.data_ptr(), B.data_ptr(), float(scaling), r, len(self.enable_lora), mask), (A, B)
+
+    def _add_lora_route(self, x: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
+        """y += each row's adapter term under _lora_route (the module path of a multi-LoRA model)."""
+        L.require_cuda_bf16(x, "MergedLinear.forward")
+        L.require_cuda_bf16(y, "MergedLinear.forward")
+        K, N = x.shape[-1], y.shape[-1]
+        x2 = x.reshape(-1, K)
+        if x2.stride(-1) != 1 or x2.stride(0) % 8 != 0 or x2.data_ptr() % 16 != 0:
+            x2 = x2.contiguous()
+        if not y.is_contiguous():
+            y = y.contiguous()
+        M, lib, route = x2.shape[0], L.lib(), self._lora_route
+        if route[0] == "rows":   # decode: row m adds adapter sel[m]
+            n = 1 + len(self._adapters)
+            specs = [self.lora_set(k) for k in range(n)]
+            arr = (L.LoRA * n)(*[sp for sp, _ in specs])
+            rc = lib.b2l_lora_apply_rows(arr, n, route[1].data_ptr(), x2.data_ptr(), x2.stride(0), None, 0.0, y.data_ptr(),
+                                         N, M, N, K, 0, L.stream_ptr())
+            L.check(rc, "b2l_lora_apply_rows")
+            return y
+        segs = [(0, M, route[1])] if route[0] == "one" else route[1]
+        for start, n_rows, k in segs:   # one launch per prompt on its rows: a row's term does not depend on M
+            if k < 0:
+                continue
+            spec, keep = self.lora_set(k)
+            rc = lib.b2l_lora_apply(C.byref(spec), x2.data_ptr() + start * x2.stride(0) * 2, x2.stride(0), None, 0.0,
+                                    y.data_ptr() + start * N * 2, N, n_rows, N, K, 0, L.stream_ptr())
+            L.check(rc, "b2l_lora_apply")
+        return y
 
     def _load_from_state_dict(self, state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys, error_msgs):
         """lora_A / lora_B are copied in place (the decode step's pointers stay valid); the rest goes to the base's own
@@ -214,6 +270,57 @@ class _QuantizedLoRA(LoRALayer):
 
 
 _QUANT_CLASSES: Dict[type, type] = {}
+
+
+def lora_layers(model: nn.Module) -> List[Tuple[str, "_QuantizedLoRA"]]:
+    """(name, layer) of every LoRA layer over a quantized base that carries a term."""
+    return [(n, m) for n, m in model.named_modules() if isinstance(m, _QuantizedLoRA) and m._has_lora]
+
+
+def add_lora_adapter(model: nn.Module, lora_state_dict: Dict[str, torch.Tensor], alpha: float = 16) -> int:
+    """Register one more LoRA adapter on a LoRA model over a quantized base (built under `lora(...)` and
+    `quantization(...)`) and return its id: 1, 2, ... (adapter 0 is the model's own lora_A / lora_B, -1 the base
+    alone).  `lora_state_dict` is what `lora_state_dict()` or finetune/lora.py save: the `...c_attn.lora_A` /
+    `lora_B` of every LoRA layer.  r comes from the shapes (1..64), scaling = alpha / r, enable_lora is the model's.
+    The tensors are copied once, as bf16 on the model's device; `state_dict()` does not change.  Rows pick adapters
+    through `adapters=` of LLaMA.prefill_rows / refill_rows and generate_prompts / generate_stream."""
+    if any(isinstance(m, MergedLinear) for m in model.modules()):
+        raise ValueError("add_lora_adapter: a dense base merges its LoRA into the weights on eval(); per-row adapters "
+                         "need a quantized base (gptq.int4, gptq.int8 or llm.int8)")
+    layers = lora_layers(model)
+    if not layers:
+        raise ValueError("add_lora_adapter: the model has no LoRA layers (build it under lora(...) and quantization(...))")
+    want = {f"{n}.{p}" for n, _ in layers for p in ("lora_A", "lora_B")}
+    got = set(lora_state_dict)
+    if got != want:
+        missing, extra = sorted(want - got), sorted(got - want)
+        raise ValueError(f"add_lora_adapter: the state dict does not match the model's LoRA layers "
+                         f"(missing {missing[:4]}{'...' if len(missing) > 4 else ''}, "
+                         f"unexpected {extra[:4]}{'...' if len(extra) > 4 else ''})")
+    if len(layers[0][1]._adapters) >= L.LORA_MAX_SETS - 1:
+        raise ValueError(f"add_lora_adapter: {L.LORA_MAX_SETS - 1} adapters are registered already (the most one "
+                         "decode step serves besides the model's own)")
+    staged = []
+    for n, lay in layers:
+        A, B = lora_state_dict[f"{n}.lora_A"], lora_state_dict[f"{n}.lora_B"]
+        n_on, n_g = sum(lay.enable_lora), len(lay.enable_lora)
+        r = A.shape[0] // n_on if A.dim() == 2 else 0
+        if (A.dim() != 2 or B.dim() != 2 or A.shape[0] != r * n_on or not 1 <= r <= L.LORA_MAX_R
+                or A.shape[1] != lay.in_features or tuple(B.shape) != (lay.out_features // n_g * n_on, r)):
+            raise ValueError(f"add_lora_adapter: {n}: lora_A {tuple(A.shape)} / lora_B {tuple(B.shape)} do not fit "
+                             f"enable_lora={lay.enable_lora} on a [{lay.out_features}, {lay.in_features}] linear "
+                             f"(lora_A [r*{n_on}, {lay.in_features}], lora_B [{lay.out_features // n_g}*{n_on}, r], "
+                             f"r 1..{L.LORA_MAX_R})")
+        staged.append((lay, A, B, r))
+    dev = layers[0][1]._device()
+    for lay, A, B, r in staged:
+        a = torch.empty(A.shape, dtype=torch.bfloat16, device=dev)
+        b = torch.empty(B.shape, dtype=torch.bfloat16, device=dev)
+        a.copy_(A)
+        b.copy_(B)
+        lay._adapters.append((a, b, alpha / r, r))
+    weights_changed()
+    return len(layers[0][1]._adapters)
 
 
 def _quantized_merged_linear(base: type) -> type:

@@ -402,8 +402,17 @@ class _DecodeState:
         if adapters is not None:   # LLaMA-Adapter: the step's attention adds each layer's gated prefix term
             self.keep.append(adapters)
             self.args.adapters = C.cast(adapters, C.POINTER(L.AdapterPrefix))
-        loras = model._loras(self.keep)
-        if loras is not None:      # LoRA: the step adds each layer's low-rank term behind c_attn
+        # multi-LoRA (a per-row adapter choice is set): each row adds its own adapter's term, the choice copied into
+        # lora_rows before every step; otherwise LoRA: the step adds each layer's low-rank term behind c_attn
+        self.lora_rows = None
+        sets = None if stepwise or model._lora_route is None else model._lora_sets(self.keep)
+        loras = None if sets is not None else model._loras(self.keep)
+        if sets is not None:
+            self.lora_rows = torch.full((B,), -1, dtype=torch.int32, device=device)
+            self.args.lora_sets = C.cast(sets[0], C.POINTER(L.LoRA))
+            self.args.n_lora_sets = sets[1]
+            self.args.lora_row_set = self.lora_rows.data_ptr()
+        if loras is not None:
             self.args.loras = C.cast(loras, C.POINTER(L.LoRA))
         affines = model._affines(self.keep)
         if affines is not None:    # LLaMA-Adapter v2 (B == 1, llm.int8 at any B): every linear's launch applies them
@@ -413,7 +422,8 @@ class _DecodeState:
         # gptq.int8 keeps one kernel per op under B2L_PERSISTENT=1 too, and so do adapter, LoRA and adapter-v2 models)
         self.plan = None
         kmax = max(C_, n_hidden)
-        if (model.persistent and not w8 and not q8 and adapters is None and loras is None and affines is None and B == 1 and hs == 128
+        if (model.persistent and not w8 and not q8 and adapters is None and loras is None and sets is None and affines is None
+                and B == 1 and hs == 128
                 and kmax <= 12288):
             self.plan = torch.zeros(lib.b2l_decode_plan_bytes(C.byref(self.args)), dtype=torch.uint8, device=device)
             self.args.plan = self.plan.data_ptr()
@@ -484,6 +494,8 @@ class LLaMA(nn.Module):
         # gptq.int8, B == 1), False (module path)
         self._fast_ok: Union[None, bool, str] = None
         self._fc12_cache = {}
+        self._lora_route = None   # multi-LoRA: the adapter choice of the current call (lora._QuantizedLoRA._lora_route)
+        self._lora_sel: Optional[torch.Tensor] = None   # device int32 [16]: each cache row's adapter (-1: none)
 
     def _block(self, config: LLaMAConfig, block_idx: int) -> nn.Module:
         """Block `block_idx` of the stack (lit_llama_b200.adapter passes the index down, adapter.py:236)."""
@@ -506,6 +518,50 @@ class LLaMA(nn.Module):
                 keep.append(t[1])
         keep.append(arr)
         return arr
+
+    def _lora_sets(self, keep: list):
+        """(HOST array [n_sets][n_layer] of b2l_lora, n_sets) for b2l_decode_args::lora_sets: set k is adapter k of
+        every LoRA layer (lit_llama_b200.lora.add_lora_adapter), r == 0 in a layer without one; None when no layer has
+        LoRA.  What it points at is appended to `keep`."""
+        from .lora import _QuantizedLoRA
+
+        cs = [blk.attn.c_attn for blk in self.transformer.h]
+        lay = [c if isinstance(c, _QuantizedLoRA) and c._has_lora else None for c in cs]
+        if all(c is None for c in lay):
+            return None
+        n_sets = 1 + len(next(c for c in lay if c is not None)._adapters)
+        n = len(lay)
+        arr = (L.LoRA * (n_sets * n))()
+        for i, c in enumerate(lay):
+            for k in range(n_sets if c is not None else 0):
+                spec, t = c.lora_set(k)
+                arr[k * n + i] = spec
+                keep.append(t)
+        keep.append(arr)
+        return arr, n_sets
+
+    def _set_lora_route(self, route) -> None:
+        """The per-row adapter choice every LoRA c_attn and the decode step read (None: today's single adapter)."""
+        from .lora import lora_layers
+
+        if (route is None) != (self._lora_route is None):
+            self._module_graph = None   # it was captured for the other kind of c_attn term
+        self._lora_route = route
+        for _, lay in lora_layers(self):
+            lay._lora_route = route
+
+    def _check_adapters(self, adapters, n: int, who: str) -> List[int]:
+        """adapters: one id per prompt, -1 (the base alone), 0 (the model's own LoRA) or one add_lora_adapter returned."""
+        from .lora import lora_layers
+
+        layers = lora_layers(self)
+        if not layers:
+            raise ValueError(f"{who}: adapters= needs a LoRA model over a quantized base (lit_llama_b200.lora)")
+        ids = [int(a) for a in adapters]
+        top = len(layers[0][1]._adapters)
+        if len(ids) != n or not all(-1 <= a <= top for a in ids):
+            raise ValueError(f"{who}: adapters {ids} must be {n} ids in -1..{top}")
+        return ids
 
     def _has_affines(self) -> bool:
         return any(hasattr(m, "adapter_scale") for m in self.modules())
@@ -568,6 +624,8 @@ class LLaMA(nn.Module):
         self._decode = None
         self._verify = {}
         self._module_graph = None
+        if self._lora_route is not None:
+            self._set_lora_route(None)
         if self._ring is not None:
             if self._ring.numel() != 1:   # back to one shared ring offset
                 self._set_ring(torch.zeros(1, dtype=torch.int32, device=self._ring.device))
@@ -595,15 +653,17 @@ class LLaMA(nn.Module):
                 raise ValueError(f"{who}: a prompt of {p.numel()} tokens does not fit max_seq_length={max_seq_length}")
 
     @torch.no_grad()
-    def prefill_rows(self, prompts: List[torch.Tensor], max_seq_length: int) -> torch.Tensor:
+    def prefill_rows(self, prompts: List[torch.Tensor], max_seq_length: int, adapters=None) -> torch.Tensor:
         """Prefill 1..16 different prompts (1-D token tensors of any lengths <= max_seq_length) into one B-row KV cache
         and return each prompt's last-position logits, (B, vocab).
 
         A fresh B-row cache, then `refill_rows(prompts, range(B), max_seq_length)`: row b's cache is bit for bit the one
         `generate()` builds for prompts[b] (no padded (B, T_max) prefill, which would cost more and round
         differently).  The ring offsets start per row at zero: the next step passes a (B, 1) `input_pos`, row b's first
-        new token at position len(prompts[b])."""
+        new token at position len(prompts[b]).  `adapters` (multi-LoRA): one adapter id per prompt, as refill_rows."""
         self._check_prompts(prompts, max_seq_length, "prefill_rows")
+        if adapters is not None:
+            self._check_adapters(adapters, len(prompts), "prefill_rows")
         B, cfg, dev = len(prompts), self.config, prompts[0].device
         self.reset_cache()
         self._prepare(prompts[0].view(1, -1), max_seq_length)
@@ -611,10 +671,10 @@ class LLaMA(nn.Module):
                                      device=dev, dtype=torch.bfloat16)
         self.kv_caches = [(self._kv_store[i, 0], self._kv_store[i, 1]) for i in range(cfg.n_layer)]
         self._set_ring(torch.zeros(B, dtype=torch.int32, device=dev))
-        return self.refill_rows(prompts, range(B), max_seq_length)
+        return self.refill_rows(prompts, range(B), max_seq_length, adapters)
 
     @torch.no_grad()
-    def refill_rows(self, prompts: List[torch.Tensor], rows, max_seq_length: int) -> torch.Tensor:
+    def refill_rows(self, prompts: List[torch.Tensor], rows, max_seq_length: int, adapters=None) -> torch.Tensor:
         """Prefill prompts[i] into row rows[i] of the existing B-row KV cache (prefill_rows) and return each prompt's
         last-position logits, (n, vocab): row rows[i] then holds, bit for bit, the cache `generate()` builds for
         prompts[i], with its ring offset at zero, and its next token goes in at position len(prompts[i]).
@@ -623,9 +683,18 @@ class LLaMA(nn.Module):
         ragged attention b2l_attention_ragged, lm_head on their last rows only); each of the others runs the batch-1
         prefill into its row ("alone").  Other rows keep their cache contents, positions and ring offsets, and the
         B-row decode state and its CUDA graph stay the same objects (the KV store and the ring tensor change in place),
-        so a decode loop can refill finished rows between two steps (generate_stream)."""
+        so a decode loop can refill finished rows between two steps (generate_stream).
+
+        `adapters` (multi-LoRA, lit_llama_b200.lora.add_lora_adapter): one id per prompt, -1 for the base alone.  Each
+        prompt's prefill adds its adapter's term on its own tokens, and row rows[i] then decodes with adapters[i] (the
+        other rows keep theirs; rows never given one use adapter 0) until reset_cache().  None: the model's own LoRA on
+        every row, as without multi-LoRA; refused once rows carry adapters."""
         rows = [int(r) for r in rows]
         self._check_prompts(prompts, max_seq_length, "refill_rows")
+        if adapters is not None:
+            adapters = self._check_adapters(adapters, len(prompts), "refill_rows")
+        elif self._lora_route is not None:
+            raise ValueError("refill_rows: the cache's rows carry adapters (prefill_rows(adapters=...)); pass adapters=")
         store = self._kv_store
         if store is None or self._ring is None or self._ring.numel() != store.shape[2]:
             raise RuntimeError("refill_rows: no B-row KV cache to refill (prefill_rows builds one)")
@@ -637,13 +706,24 @@ class LLaMA(nn.Module):
         self._prepare(prompts[0].view(1, -1), max_seq_length)
         packed = self._pack_plan([p.numel() for p in prompts])
         out: List[Optional[torch.Tensor]] = [None] * len(prompts)
+        ad = adapters if adapters is not None else [None] * len(prompts)
         if packed:
-            logits = self._prefill_packed([prompts[i] for i in packed], [rows[i] for i in packed], max_seq_length)
+            logits = self._prefill_packed([prompts[i] for i in packed], [rows[i] for i in packed], max_seq_length,
+                                          [ad[i] for i in packed])
             for j, i in enumerate(packed):
                 out[i] = logits[j]
         alone = [i for i in range(len(prompts)) if i not in packed]
-        for i, lg in zip(alone, self._prefill_alone([prompts[i] for i in alone], [rows[i] for i in alone], max_seq_length)):
+        for i, lg in zip(alone, self._prefill_alone([prompts[i] for i in alone], [rows[i] for i in alone], max_seq_length,
+                                                    [ad[i] for i in alone])):
             out[i] = lg
+        if adapters is not None:   # the refilled rows decode with their prompts' adapters from the next step on
+            if self._lora_sel is None or self._lora_sel.device != prompts[0].device:
+                self._lora_sel = torch.zeros(16, dtype=torch.int32, device=prompts[0].device)
+            if self._lora_route is None:
+                self._lora_sel.zero_()   # rows never given an adapter keep the model's own (adapter 0)
+            self._lora_sel[torch.tensor(rows, device=self._lora_sel.device)] = torch.tensor(
+                adapters, dtype=torch.int32, device=self._lora_sel.device)
+            self._set_lora_route(("rows", self._lora_sel))
         return torch.stack(out)
 
     def _linears(self) -> List[nn.Module]:
@@ -669,7 +749,8 @@ class LLaMA(nn.Module):
             return []
         return cand
 
-    def _prefill_packed(self, prompts: List[torch.Tensor], rows: List[int], max_seq_length: int) -> torch.Tensor:
+    def _prefill_packed(self, prompts: List[torch.Tensor], rows: List[int], max_seq_length: int,
+                        adapters: List[Optional[int]]) -> torch.Tensor:
         """The packed prefill of refill_rows: the prompts back to back as one (1, N) sequence through the module path
         at M = N, the attention ragged (each prompt into its row at positions 0..), lm_head on each prompt's last row
         on the kernel its batch-1 prefill ran it on at M = len (the GEMM, not the 2..16-row kernel M = n would pick)."""
@@ -683,7 +764,13 @@ class LLaMA(nn.Module):
             N += p.numel()
         dev = prompts[0].device
         toks = torch.cat([p.to(torch.int64) for p in prompts]).view(1, N)
-        h = self._forward_hidden(toks, max_seq_length, None, ragged=seqs)
+        route = self._lora_route
+        if adapters[0] is not None:   # multi-LoRA: each prompt's tokens add its adapter's term
+            self._set_lora_route(("segments", [(seqs.start[j], seqs.len[j], a) for j, a in enumerate(adapters)]))
+        try:
+            h = self._forward_hidden(toks, max_seq_length, None, ragged=seqs)
+        finally:
+            self._set_lora_route(route)
         last = torch.tensor([seqs.start[j] + seqs.len[j] - 1 for j in range(len(prompts))], device=dev)
         x = h[0].index_select(0, last)
         y = self.lm_head.run(x, kernel_at(self.lm_head, N))
@@ -694,15 +781,18 @@ class LLaMA(nn.Module):
             linear_affine(y, *aff)
         return y
 
-    def _prefill_alone(self, prompts: List[torch.Tensor], rows: List[int], max_seq_length: int) -> List[torch.Tensor]:
+    def _prefill_alone(self, prompts: List[torch.Tensor], rows: List[int], max_seq_length: int,
+                       adapters: List[Optional[int]]) -> List[torch.Tensor]:
         """The batch-1 prefill of each prompt into its row: the model is pointed at that row of the KV store and its
         ring offset (ring[r:r+1], zeroed) for the call, and the B-row decode state and module graph are put back after
         (a one-token prompt runs, and replaces, the batch-1 step state)."""
         ring, store, caches = self._ring, self._kv_store, self.kv_caches
-        decode, module_graph = self._decode, self._module_graph
+        decode, module_graph, route = self._decode, self._module_graph, self._lora_route
         out = []
         try:
-            for p, r in zip(prompts, rows):
+            for p, r, a in zip(prompts, rows, adapters):
+                if a is not None:   # multi-LoRA: the prompt's adapter on every token (a one-token prompt's step too)
+                    self._set_lora_route(("one", a, torch.full((1,), a, dtype=torch.int32, device=p.device)))
                 one = ring[r:r + 1]
                 one.zero_()
                 self._ring = one
@@ -716,6 +806,7 @@ class LLaMA(nn.Module):
             self._ring, self._kv_store, self.kv_caches = ring, store, caches
             for blk in self.transformer.h:
                 blk.attn._ring = ring
+            self._set_lora_route(route)
             self._decode, self._module_graph = decode, module_graph
         return out
 
@@ -944,7 +1035,7 @@ class LLaMA(nn.Module):
                 self._fc12_cache = {k: v for k, v in self._fc12_cache.items()
                                     if k[1] == "i8" and self._fc12_is_only_copy(k[0])}
             if (st is None or st.B != B or st.S != max_seq_length or st.idx.dtype != idx.dtype or st.idx.device != idx.device
-                    or st.row_pos != rows):
+                    or st.row_pos != rows or (st.lora_rows is None) != (self._lora_route is None)):
                 if self._fast_ok is None:
                     self._fast_ok = self._fast_decode_ok()
                 # gptq.int8 and LLaMA-Adapter v2: batch 1 only; gptq.int8 without v2 affines at batch 2..16 on request
@@ -957,6 +1048,11 @@ class LLaMA(nn.Module):
         if st is not None:
             st.idx.copy_(idx.reshape(-1))
             st.pos.copy_(input_pos.reshape(-1) if rows else input_pos.reshape(-1)[-1:])
+            if st.lora_rows is not None:   # multi-LoRA: each row's adapter, as the route gives it
+                r = self._lora_route
+                if r[0] == "segments":
+                    raise RuntimeError("LLaMA.forward: a packed prefill's adapter segments do not decode")
+                st.lora_rows.copy_(r[2].expand(B) if r[0] == "one" else r[1][:B])
             if st.graph is not None:
                 st.graph.replay()
             elif self.graph_after and st.calls >= self.graph_after:
@@ -973,7 +1069,9 @@ class LLaMA(nn.Module):
         # ---- single-token decode the fused step does not run (llm.int8, grouped or biased gptq, dense, gptq.int8 at
         #      B >= 2): the module-by-module launch sequence, replayed as a CUDA graph once warm
         if input_pos is not None and T == 1 and self.graph_after and idx.dtype in (torch.int32, torch.int64):
-            key = (B, max_seq_length, idx.dtype, idx.device, WEIGHTS_GENERATION[0], rows)   # the graph bakes weight pointers too
+            route = self._lora_route   # a multi-LoRA c_attn reads its adapter choice from the tensor the route names
+            key = (B, max_seq_length, idx.dtype, idx.device, WEIGHTS_GENERATION[0],
+                   None if route is None else (route[0], route[-1].data_ptr() if route[0] != "segments" else None), rows)
             mg = self._module_graph
             if mg is None or mg["key"] != key:
                 mg = self._module_graph = dict(key=key, calls=0, graph=None, idx=torch.zeros((B, 1), dtype=idx.dtype, device=idx.device),
