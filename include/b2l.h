@@ -732,6 +732,11 @@ typedef struct b2l_decode_args {
   const int32_t* lora_row_set; /* device int32 [B]: row b's set, -1 = none (read by the kernels only) */
 } b2l_decode_args;
 
+/* Every linear of a step runs the same kernel.  B2L_F_W8 / B2L_F_Q8 and the batch flags select it; otherwise B == 1
+ * runs the batch-1 GEMV when lm_head has qw_mma and the wgmma kernel (qw_tiled) when it does not, B = 2..8 with
+ * batch_work the mma.sync batch kernel (qw_mma), and every other B the wgmma kernel.  A weight without the tiling its
+ * kernel reads is B2L_E_STATE; at B == 1 a weight whose tiling would pick the other kernel is B2L_E_UNSUPPORTED.  Every
+ * argument is checked before the first launch. */
 /* With B2L_F_STEPWISE the B = 2..16 rows are consecutive tokens of ONE sequence: idx [B], input_pos int64 [B] holding
  * p..p+B-1 (all < S), layers[].k_cache / v_cache the batch-1 caches [1, nh, S, hs], attn_work
  * b2l_attn_workspace_bytes(B, nh, hs, 1, S) bytes.  Row t's logits equal the batch-1 step's at position p+t on the cache

@@ -934,9 +934,6 @@ __global__ void __launch_bounds__(128)
   }
 }
 
-// debug timeline slot for the next fused-attention launch (set by b2l_decode_step; nullptr = off)
-void* g_attn_timeline = nullptr;
-
 static inline void split_plan(int T, int S, int* n_split, int* chunk) {
   if (T > 1) { *n_split = 1; *chunk = S; return; }
   *chunk = 64;
@@ -1044,10 +1041,24 @@ static int check_stepwise(int flags, int B, int T, const char* who) {
   return 0;
 }
 
-// b2l_attention and b2l_attention_adapter (pre != nullptr: already checked)
-static int attention_impl(void* qkv, void* k_cache, void* v_cache, const void* rope, const int64_t* input_pos,
-                          const int32_t* ring_start, void* y, void* work, int B, int T, int n_head, int head_size,
-                          int S, int block_size, int flags, const b2l_adapter_prefix* pre, cudaStream_t st) {
+namespace b2l {
+// b2l_attention's argument checks (`who` names the caller): 0, or B2L_E_* with a message
+int check_attention(const void* qkv, const void* k_cache, const void* v_cache, const void* rope, const int64_t* input_pos,
+                    const int32_t* ring_start, const void* y, const void* work, int B, int T, int n_head, int head_size,
+                    int S, int block_size, int flags, const char* who) {
+  B2L_CHECK_ARG(qkv && k_cache && v_cache && rope && input_pos && ring_start && y && work, "%s: null pointer", who);
+  B2L_CHECK_ARG(B > 0 && T > 0 && n_head > 0 && S > 0 && T <= S && block_size > 0, "%s: bad shape", who);
+  B2L_CHECK_SUPPORTED(head_size % 2 == 0 && head_size >= 2 && head_size <= 32 * ATT_MAX_EPL,
+                      "%s: head_size %d unsupported (even, <= %d)", who, head_size, 32 * ATT_MAX_EPL);
+  if (int rc = check_stepwise(flags, B, T, who)) return rc;
+  return check_row_pos(flags, T, who);
+}
+
+// b2l_attention, b2l_attention_adapter and b2l_decode_step, after check_attention (and check_adapter_prefix when pre
+// != nullptr); timeline: the fused kernel's debug stamps (uint64[64]), or nullptr
+int attention_impl(void* qkv, void* k_cache, void* v_cache, const void* rope, const int64_t* input_pos,
+                   const int32_t* ring_start, void* y, void* work, int B, int T, int n_head, int head_size, int S,
+                   int block_size, int flags, const b2l_adapter_prefix* pre, void* timeline, cudaStream_t st) {
   const int pos_stride = (flags & B2L_F_ROW_POS) ? 1 : 0;
   const bool step = (flags & B2L_F_STEPWISE) != 0;
   if ((T == 1 || step) && head_size == 128 && !(flags & B2L_F_ROPE_ROWS) && !(flags & B2L_F_ATTN_UNFUSED)) {
@@ -1075,7 +1086,7 @@ static int attention_impl(void* qkv, void* k_cache, void* v_cache, const void* r
       if (int rc = ensure_dyn_smem(kernel, FD_SMEM_BYTES, smem_cache[pf != nullptr][step ? 2 : pos_stride])) return rc;
       B2L_CUDA(cudaLaunchKernelEx(&lc.cfg, kernel, (const __nv_bfloat16*)qkv, (__nv_bfloat16*)k_cache,
                                   (__nv_bfloat16*)v_cache, (const float*)rope, input_pos, ring_start, (__nv_bfloat16*)y,
-                                  (float*)work, tickets, n_head, S, block_size, n_split, (unsigned long long*)g_attn_timeline, env_pre, env_smem_merge,
+                                  (float*)work, tickets, n_head, S, block_size, n_split, (unsigned long long*)timeline, env_pre, env_smem_merge,
                                   FD_CTAS_PER_SM * sm_count(), (const __nv_bfloat16*)(pf ? pf->k : nullptr),
                                   (const __nv_bfloat16*)(pf ? pf->v : nullptr), (const __nv_bfloat16*)(pf ? pf->gate : nullptr),
                                   pf ? pf->len : 0));
@@ -1103,35 +1114,28 @@ static int attention_impl(void* qkv, void* k_cache, void* v_cache, const void* r
     return rc;
   return pre == nullptr ? 0 : launch_adapter_prefix(qkv, pre, y, B, T, n_head, head_size, st);
 }
+}  // namespace b2l
 
 extern "C" int b2l_attention(void* qkv, void* k_cache, void* v_cache, const void* rope, const int64_t* input_pos,
                              const int32_t* ring_start, void* y, void* work, int B, int T, int n_head,
                              int head_size, int S, int block_size, int flags, b2l_stream_t stream) {
-  B2L_CHECK_ARG(qkv && k_cache && v_cache && rope && input_pos && ring_start && y && work,
-                "b2l_attention: null pointer");
-  B2L_CHECK_ARG(B > 0 && T > 0 && n_head > 0 && S > 0 && T <= S && block_size > 0, "b2l_attention: bad shape");
-  B2L_CHECK_SUPPORTED(head_size % 2 == 0 && head_size >= 2 && head_size <= 32 * ATT_MAX_EPL,
-                      "b2l_attention: head_size %d unsupported (even, <= %d)", head_size, 32 * ATT_MAX_EPL);
-  if (int rc = check_stepwise(flags, B, T, "b2l_attention")) return rc;
-  if (int rc = check_row_pos(flags, T, "b2l_attention")) return rc;
+  if (int rc = check_attention(qkv, k_cache, v_cache, rope, input_pos, ring_start, y, work, B, T, n_head, head_size, S,
+                               block_size, flags, "b2l_attention"))
+    return rc;
   return attention_impl(qkv, k_cache, v_cache, rope, input_pos, ring_start, y, work, B, T, n_head, head_size, S,
-                        block_size, flags, nullptr, (cudaStream_t)stream);
+                        block_size, flags, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" int b2l_attention_adapter(void* qkv, void* k_cache, void* v_cache, const void* rope,
                                      const int64_t* input_pos, const int32_t* ring_start, void* y, void* work, int B,
                                      int T, int n_head, int head_size, int S, int block_size, int flags,
                                      const b2l_adapter_prefix* prefix, b2l_stream_t stream) {
-  B2L_CHECK_ARG(qkv && k_cache && v_cache && rope && input_pos && ring_start && y && work,
-                "b2l_attention_adapter: null pointer");
-  B2L_CHECK_ARG(B > 0 && T > 0 && n_head > 0 && S > 0 && T <= S && block_size > 0, "b2l_attention_adapter: bad shape");
-  B2L_CHECK_SUPPORTED(head_size % 2 == 0 && head_size >= 2 && head_size <= 32 * ATT_MAX_EPL,
-                      "b2l_attention_adapter: head_size %d unsupported (even, <= %d)", head_size, 32 * ATT_MAX_EPL);
-  if (int rc = check_stepwise(flags, B, T, "b2l_attention_adapter")) return rc;
-  if (int rc = check_row_pos(flags, T, "b2l_attention_adapter")) return rc;
+  if (int rc = check_attention(qkv, k_cache, v_cache, rope, input_pos, ring_start, y, work, B, T, n_head, head_size, S,
+                               block_size, flags, "b2l_attention_adapter"))
+    return rc;
   if (int rc = check_adapter_prefix(prefix, "b2l_attention_adapter")) return rc;
   return attention_impl(qkv, k_cache, v_cache, rope, input_pos, ring_start, y, work, B, T, n_head, head_size, S,
-                        block_size, flags, prefix, (cudaStream_t)stream);
+                        block_size, flags, prefix, nullptr, (cudaStream_t)stream);
 }
 
 static int attention_nocache_impl(void* qkv, const void* rope, void* y, void* work, int B, int T, int n_head,

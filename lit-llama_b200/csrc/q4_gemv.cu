@@ -534,12 +534,23 @@ extern "C" int b2l_w8_untile_i8(const void* qw_tiled, void* qw, int N, int K, b2
 }
 
 namespace {
+// three digits (|X| < 2^22) everywhere: the prologue's fma conversion needs the integer inside a float mantissa
+constexpr int NDIG_GEMV = 3;
+
 // Ring stages that fit `budget` bytes of shared memory at this K (0: not even two)
 template <int NDIG>
 int ring_stages(int K, uint32_t budget) {
   const uint32_t fixed = smem_layout(0, K, NDIG).total;
   const int nst = fixed + 2 * STAGE_BYTES <= budget ? (int)((budget - fixed) / STAGE_BYTES) : 0;
   return nst > MAX_STAGES ? MAX_STAGES : nst;
+}
+
+// CTAs per SM before the small-linear choice in launch_gemv_variant, and the ring stages at that size (0: not even
+// two).  That choice only ever moves to one CTA per SM with a deeper ring.
+template <int NDIG>
+int base_ring_stages(int K, int* ctas_per_sm) {
+  *ctas_per_sm = K <= 16384 ? 2 : 1;
+  return ring_stages<NDIG>(K, (*ctas_per_sm == 2 ? 110u : 224u) * 1024u);
 }
 
 // Stages a CTA owning `rbs` row blocks streams (pairs, then at most one single, as q4_gemv_kernel walks them)
@@ -560,8 +571,8 @@ int cta_stages(int rbs, int n_kb) {
 template <int MAXC, int NDIG, bool W8, bool AFFINE>
 int launch_gemv_variant(const Params& p0, int grid_override, bool pdl, cudaStream_t stream) {
   Params p = p0;
-  int ctas_per_sm = p.K <= 16384 ? 2 : 1;
-  int nst = ring_stages<NDIG>(p.K, (ctas_per_sm == 2 ? 110u : 224u) * 1024u);
+  int ctas_per_sm;
+  int nst = base_ring_stages<NDIG>(p.K, &ctas_per_sm);   // >= 2: check_gemv
   if (ctas_per_sm == 2) {
     const int sms = sm_count(), n_kb = p.K / KB;
     const int one = ring_stages<NDIG>(p.K, 113u * 1024u);
@@ -570,10 +581,6 @@ int launch_gemv_variant(const Params& p0, int grid_override, bool pdl, cudaStrea
       ctas_per_sm = 1;
       nst = one;
     }
-  }
-  if (nst < 2) {
-    set_error("b2l_q4_gemv: K=%d does not leave room for the weight ring", p.K);
-    return B2L_E_UNSUPPORTED;
   }
   p.nst = nst;
   const SmemLayout L = smem_layout(nst, p.K, NDIG);
@@ -592,9 +599,11 @@ int launch_gemv(const Params& p, int grid_override, bool pdl, cudaStream_t strea
   return launch_gemv_variant<MAXC, NDIG, W8, false>(p, grid_override, pdl, stream);
 }
 
-// b2l_q4_gemv (W8 = false) and b2l_w8_gemv (W8 = true): the same checks, argument block and launch policy
-template <bool W8>
-int gemv_entry(const b2l_q4_linear_args* a, b2l_stream_t stream) {
+}  // namespace
+
+namespace b2l {
+// b2l_q4_gemv's (W8 = false) and b2l_w8_gemv's (W8 = true) argument checks: 0, or B2L_E_* with a message
+int check_gemv(const b2l_q4_linear_args* a, bool W8) {
   const char* fn = W8 ? "b2l_w8_gemv" : "b2l_q4_gemv";
   B2L_CHECK_ARG(a != nullptr, "%s: null args", fn);
   B2L_CHECK_ARG(a->x && a->qw_tiled && a->scales && a->zeros && a->y, "%s: null pointer", fn);
@@ -614,7 +623,18 @@ int gemv_entry(const b2l_q4_linear_args* a, b2l_stream_t stream) {
   else B2L_CHECK_ARG(a->epilogue == B2L_EPI_STORE, "%s: bad epilogue %d", fn, a->epilogue);
   B2L_CHECK_ARG((a->out_affine.scale == nullptr) == (a->out_affine.bias == nullptr),
                 "%s: out_affine needs both scale and bias (or neither)", fn);
+  int ctas_per_sm;
+  B2L_CHECK_SUPPORTED(base_ring_stages<NDIG_GEMV>(a->K, &ctas_per_sm) >= 2, "%s: K=%d does not leave room for the weight ring",
+                      fn, a->K);
+  return 0;
+}
+}  // namespace b2l
 
+namespace {
+// b2l_q4_gemv (W8 = false) and b2l_w8_gemv (W8 = true): the same checks, argument block and launch policy
+template <bool W8>
+int gemv_entry(const b2l_q4_linear_args* a, b2l_stream_t stream) {
+  if (int rc = check_gemv(a, W8)) return rc;
   Params p;
   p.aff_scale = (const __nv_bfloat16*)a->out_affine.scale;
   p.aff_bias = (const __nv_bfloat16*)a->out_affine.bias;
@@ -632,9 +652,8 @@ int gemv_entry(const b2l_q4_linear_args* a, b2l_stream_t stream) {
   const bool pdl = (a->flags & B2L_F_PDL) != 0;
   cudaStream_t st = (cudaStream_t)stream;
   const int grid = a->split_k;  // split_k doubles as a grid override
-  // three digits (|X| < 2^22) everywhere: the prologue's fma conversion needs the integer inside a float mantissa
-  if (a->K <= 12288) return launch_gemv<6, 3, W8>(p, grid, pdl, st);
-  return launch_gemv<12, 3, W8>(p, grid, pdl, st);
+  if (a->K <= 12288) return launch_gemv<6, NDIG_GEMV, W8>(p, grid, pdl, st);
+  return launch_gemv<12, NDIG_GEMV, W8>(p, grid, pdl, st);
 }
 }  // namespace
 

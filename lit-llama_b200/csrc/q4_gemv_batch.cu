@@ -420,7 +420,9 @@ extern "C" size_t b2l_q4_gemv_batch_workspace_bytes(int K) {
   return (size_t)(K / KB) * XKB_BYTES + MAXB * 3 * sizeof(float);
 }
 
-extern "C" int b2l_q4_gemv_batch(const b2l_q4_linear_args* a, b2l_stream_t stream) {
+namespace b2l {
+// b2l_q4_gemv_batch's argument checks: 0, or B2L_E_* with a message
+int check_q4_gemv_batch(const b2l_q4_linear_args* a) {
   B2L_CHECK_ARG(a != nullptr, "b2l_q4_gemv_batch: null args");
   B2L_CHECK_ARG(a->x && a->qw_tiled && a->scales && a->zeros && a->y && a->workspace, "b2l_q4_gemv_batch: null pointer");
   B2L_CHECK_SUPPORTED(a->out_affine.scale == nullptr && a->out_affine.bias == nullptr,
@@ -439,6 +441,12 @@ extern "C" int b2l_q4_gemv_batch(const b2l_q4_linear_args* a, b2l_stream_t strea
   if (a->epilogue == B2L_EPI_RESIDUAL) B2L_CHECK_ARG(a->res != nullptr, "b2l_q4_gemv_batch: RESIDUAL epilogue needs res");
   else if (a->epilogue == B2L_EPI_SWIGLU) B2L_CHECK_SUPPORTED(a->N % RB == 0, "b2l_q4_gemv_batch: SWIGLU needs N %% 16 == 0");
   else B2L_CHECK_ARG(a->epilogue == B2L_EPI_STORE, "b2l_q4_gemv_batch: bad epilogue %d", a->epilogue);
+  return 0;
+}
+}  // namespace b2l
+
+extern "C" int b2l_q4_gemv_batch(const b2l_q4_linear_args* a, b2l_stream_t stream) {
+  if (int rc = check_q4_gemv_batch(a)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   // programmatic dependent launch for the two kernels (B2L_BATCH_PDL=0: plain stream order)
   static const int env_pdl = [] { const char* e = getenv("B2L_BATCH_PDL"); return e ? atoi(e) : 1; }();

@@ -519,9 +519,9 @@ int q4_pick_split(int n_tiles, int slabs_total) {
   }
   return best_cost < 0 ? 8 : best;
 }
-}  // namespace b2l
 
-extern "C" int b2l_q4_linear_tc(const b2l_q4_linear_args* a, b2l_stream_t stream) {
+// b2l_q4_linear_tc's argument checks, split-K and shared-memory layout: 0, or B2L_E_* with a message
+static int plan_linear_tc(const b2l_q4_linear_args* a, Params& p, SmemLayout& L) {
   B2L_CHECK_ARG(a != nullptr, "b2l_q4_linear_tc: null args");
   B2L_CHECK_ARG(a->x && a->qw_tiled && a->scales && a->zeros && a->y, "b2l_q4_linear_tc: null pointer");
   B2L_CHECK_SUPPORTED(a->out_affine.scale == nullptr && a->out_affine.bias == nullptr,
@@ -546,7 +546,6 @@ extern "C" int b2l_q4_linear_tc(const b2l_q4_linear_args* a, b2l_stream_t stream
   B2L_CHECK_SUPPORTED(S >= 1 && S <= 8, "b2l_q4_linear_tc: split_k=%d must be in 1..8", S);
   while (S > 1 && slabs_total < 2 * S) --S;
 
-  Params p;
   p.x = (const __nv_bfloat16*)a->x; p.ldx = a->ldx;
   p.qwt = (const uint8_t*)a->qw_tiled;
   p.scales = a->scales; p.zeros = a->zeros; p.szdt = a->sz_dtype;
@@ -569,11 +568,25 @@ extern "C" int b2l_q4_linear_tc(const b2l_q4_linear_args* a, b2l_stream_t stream
   if (ring > MAX_STAGES) ring = MAX_STAGES;
   p.nst_ring = stages_needed < ring ? stages_needed : ring;
   if (p.nst_ring < 1) p.nst_ring = 1;
-  const SmemLayout L = smem_layout(p.nst_ring, p.kseg_max, p.kcb, p.M);
+  L = smem_layout(p.nst_ring, p.kseg_max, p.kcb, p.M);
   B2L_CHECK_SUPPORTED(L.total <= 200 * 1024, "b2l_q4_linear_tc: shared memory %u B too large (K=%d, split_k=%d)", L.total, a->K, S);
+  return 0;
+}
 
+int check_q4_linear_tc(const b2l_q4_linear_args* a) {
+  Params p;
+  SmemLayout L;
+  return plan_linear_tc(a, p, L);
+}
+}  // namespace b2l
+
+extern "C" int b2l_q4_linear_tc(const b2l_q4_linear_args* a, b2l_stream_t stream) {
+  Params p;
+  SmemLayout L;
+  if (int rc = plan_linear_tc(a, p, L)) return rc;
+  const int n_tiles = (a->N + TILE_N - 1) / TILE_N;
   static DynSmemCache smem_cache[2];
-  LaunchCfg lc(dim3(n_tiles * S), dim3(NTHREADS), L.total, (cudaStream_t)stream, (a->flags & B2L_F_PDL) != 0, S);
+  LaunchCfg lc(dim3(n_tiles * p.S), dim3(NTHREADS), L.total, (cudaStream_t)stream, (a->flags & B2L_F_PDL) != 0, p.S);
   if (p.kcb == 256) {   // 16 token columns per MMA
     if (int rc = ensure_dyn_smem(q4_linear_tc_kernel<16>, L.total, smem_cache[1])) return rc;
     B2L_CUDA(cudaLaunchKernelEx(&lc.cfg, q4_linear_tc_kernel<16>, p));

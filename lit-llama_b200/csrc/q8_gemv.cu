@@ -499,7 +499,9 @@ extern "C" int b2l_q8_gemv_cb(const void* x, const void* cb, const void* scb, co
   return launch_gemv<WS_CB>(p, flags, stream);
 }
 
-extern "C" int b2l_q8_linear(const b2l_q8_linear_args* a, b2l_stream_t stream) {
+namespace b2l {
+// b2l_q8_linear's argument checks: 0, or B2L_E_* with a message
+int check_q8_linear(const b2l_q8_linear_args* a) {
   B2L_CHECK_ARG(a != nullptr && a->x && a->cb && a->scb && a->y, "b2l_q8_linear: null pointer");
   const int N = a->N, K = a->K;
   B2L_CHECK_SUPPORTED(K > 0 && K % KB == 0 && K <= MAX_K, "b2l_q8_linear: K=%d must be a multiple of %d and <= %d", K, KB, MAX_K);
@@ -516,9 +518,23 @@ extern "C" int b2l_q8_linear(const b2l_q8_linear_args* a, b2l_stream_t stream) {
   B2L_CHECK_ARG(((uintptr_t)a->x | (uintptr_t)a->cb | (uintptr_t)(glu ? a->cb2 : nullptr) |
                  (uintptr_t)(norm ? a->norm_scale : nullptr)) % 16 == 0,
                 "b2l_q8_linear: x / cb / cb2 / norm_scale must be 16-byte aligned");
-  const uintptr_t x0 = (uintptr_t)a->x, y0 = (uintptr_t)a->y;
-  B2L_CHECK_ARG(y0 + 2 * (size_t)N <= x0 || x0 + 2 * (size_t)K <= y0, "b2l_q8_linear: y overlaps x");
   B2L_CHECK_SUPPORTED((a->flags & ~B2L_F_PDL) == 0, "b2l_q8_linear: unknown flags 0x%x (only B2L_F_PDL)", (unsigned)a->flags);
+  return 0;
+}
+
+// b2l_q8_linear's and b2l_q8_linear_batch's M rows of y must not overlap x: the kernels read x after they start writing y
+int check_q8_disjoint(const b2l_q8_linear_args* a, int M, const char* who) {
+  const uintptr_t x0 = (uintptr_t)a->x, y0 = (uintptr_t)a->y;
+  B2L_CHECK_ARG(y0 + 2 * (size_t)M * a->N <= x0 || x0 + 2 * (size_t)M * a->K <= y0, "%s: y overlaps x", who);
+  return 0;
+}
+}  // namespace b2l
+
+extern "C" int b2l_q8_linear(const b2l_q8_linear_args* a, b2l_stream_t stream) {
+  if (int rc = check_q8_linear(a)) return rc;
+  if (int rc = check_q8_disjoint(a, 1, "b2l_q8_linear")) return rc;
+  const int N = a->N, K = a->K;
+  const bool norm = a->prologue == B2L_PRO_RMSNORM, glu = a->epilogue == B2L_EPI_SWIGLU;
   Params p;
   fill_params(p, a->x, a->cb, a->scb, nullptr, a->y, N, K, a->threshold);
   p.n_rb = glu ? (N + 7) / 8 : (N + RB - 1) / RB;

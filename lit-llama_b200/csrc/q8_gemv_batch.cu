@@ -489,7 +489,11 @@ int launch_batch(BParams& p, bool pdl, cudaStream_t stream) {
 }
 }  // namespace
 
-extern "C" int b2l_q8_linear_batch(const b2l_q8_linear_args* a, int M, void* workspace, size_t workspace_bytes, b2l_stream_t stream) {
+namespace b2l {
+int check_q8_disjoint(const b2l_q8_linear_args* a, int M, const char* who);   // q8_gemv.cu
+
+// b2l_q8_linear_batch's argument checks: 0, or B2L_E_* with a message
+int check_q8_linear_batch(const b2l_q8_linear_args* a, int M, const void* workspace, size_t workspace_bytes) {
   B2L_CHECK_ARG(a != nullptr && a->x && a->cb && a->scb && a->y, "b2l_q8_linear_batch: null pointer");
   B2L_CHECK_SUPPORTED(M >= 2 && M <= MAXB, "b2l_q8_linear_batch: M=%d (2..%d activation rows; use b2l_q8_linear for 1)", M, MAXB);
   const int N = a->N, K = a->K;
@@ -510,9 +514,16 @@ extern "C" int b2l_q8_linear_batch(const b2l_q8_linear_args* a, int M, void* wor
                 "b2l_q8_linear_batch: x / cb / cb2 / norm_scale / workspace must be 16-byte aligned");
   B2L_CHECK_ARG(workspace_bytes >= ws_bytes(K, M), "b2l_q8_linear_batch: workspace of %zu bytes is too small (%zu needed)",
                 workspace_bytes, ws_bytes(K, M));
-  const uintptr_t x0 = (uintptr_t)a->x, y0 = (uintptr_t)a->y;
-  B2L_CHECK_ARG(y0 + 2 * (size_t)M * N <= x0 || x0 + 2 * (size_t)M * K <= y0, "b2l_q8_linear_batch: y overlaps x");
   B2L_CHECK_SUPPORTED((a->flags & ~B2L_F_PDL) == 0, "b2l_q8_linear_batch: unknown flags 0x%x (only B2L_F_PDL)", (unsigned)a->flags);
+  return 0;
+}
+}  // namespace b2l
+
+extern "C" int b2l_q8_linear_batch(const b2l_q8_linear_args* a, int M, void* workspace, size_t workspace_bytes, b2l_stream_t stream) {
+  if (int rc = check_q8_linear_batch(a, M, workspace, workspace_bytes)) return rc;
+  if (int rc = check_q8_disjoint(a, M, "b2l_q8_linear_batch")) return rc;
+  const int N = a->N, K = a->K;
+  const bool norm = a->prologue == B2L_PRO_RMSNORM, glu = a->epilogue == B2L_EPI_SWIGLU;
   const cudaStream_t st = (cudaStream_t)stream;
   const bool pdl = (a->flags & B2L_F_PDL) != 0;
   uint8_t* ws = (uint8_t*)workspace;

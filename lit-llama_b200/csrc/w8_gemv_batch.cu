@@ -379,21 +379,24 @@ extern "C" size_t b2l_w8_gemv_batch_workspace_bytes(int K, int M) {
 }
 
 namespace {
+// Column groups of M rows (one instantiation of w8_gemv_batch_kernel each)
+int column_groups(int M) { return std::min(6, (NDIG * M + 7) / 8); }
+
+// Ring stages of the batch kernel at M rows (0: not even two).  1..2 column groups (M <= 5): two CTAs per SM; more:
+// one CTA per SM with a deeper ring
+int batch_ring_stages(int M, bool W8) {
+  const uint32_t budget = (column_groups(M) <= 2 ? 110u : 224u) * 1024u;
+  const uint32_t fixed = bsmem_layout(0, M, W8).total, sb = bstage_bytes(M, W8);
+  const int nst = fixed + 2 * sb <= budget ? (int)((budget - fixed) / sb) : 0;
+  return nst > BMAX_STAGES ? BMAX_STAGES : nst;
+}
+
 template <int NG, bool W8>
-int launch_batch(const BParams& p0, int grid_override, bool pdl, cudaStream_t stream, const char* fn) {
+int launch_batch(const BParams& p0, int grid_override, bool pdl, cudaStream_t stream) {
   BParams p = p0;
-  // 1..2 column groups (M <= 5): two CTAs per SM; more: one CTA per SM with a deeper ring
   const int ctas_per_sm = NG <= 2 ? 2 : 1;
-  const uint32_t budget = (ctas_per_sm >= 2 ? 110u : 224u) * 1024u;
-  const uint32_t fixed = bsmem_layout(0, p.M, W8).total, sb = bstage_bytes(p.M, W8);
-  int nst = fixed + 2 * sb <= budget ? (int)((budget - fixed) / sb) : 0;
-  if (nst > BMAX_STAGES) nst = BMAX_STAGES;
-  if (nst < 2) {
-    set_error("%s: M=%d does not leave room for the weight ring", fn, p.M);
-    return B2L_E_UNSUPPORTED;
-  }
-  p.nst = nst;
-  const BSmem L = bsmem_layout(nst, p.M, W8);
+  p.nst = batch_ring_stages(p.M, W8);
+  const BSmem L = bsmem_layout(p.nst, p.M, W8);
   static DynSmemCache smem_cache;
   if (int rc = ensure_dyn_smem(w8_gemv_batch_kernel<NG, W8>, L.total, smem_cache)) return rc;
   int grid = grid_override > 0 ? grid_override : ctas_per_sm * sm_count();
@@ -403,9 +406,11 @@ int launch_batch(const BParams& p0, int grid_override, bool pdl, cudaStream_t st
   return 0;
 }
 
-// b2l_w8_gemv_batch (W8 = true) and b2l_q4_gemv_batch_i8 (W8 = false): the same checks, workspace and launches
-template <bool W8>
-int batch_entry(const b2l_q4_linear_args* a, b2l_stream_t stream) {
+}  // namespace
+
+namespace b2l {
+// b2l_w8_gemv_batch's (W8 = true) and b2l_q4_gemv_batch_i8's (W8 = false) argument checks: 0, or B2L_E_* with a message
+int check_gemv_batch_i8(const b2l_q4_linear_args* a, bool W8) {
   const char* fn = W8 ? "b2l_w8_gemv_batch" : "b2l_q4_gemv_batch_i8";
   B2L_CHECK_ARG(a != nullptr, "%s: null args", fn);
   B2L_CHECK_ARG(a->x && a->qw_tiled && a->scales && a->zeros && a->y, "%s: null pointer", fn);
@@ -434,6 +439,16 @@ int batch_entry(const b2l_q4_linear_args* a, b2l_stream_t stream) {
     B2L_CHECK_ARG(a->epilogue == B2L_EPI_STORE, "%s: bad epilogue %d", fn, a->epilogue);
   }
   B2L_CHECK_ARG(a->ldy >= (a->epilogue == B2L_EPI_SWIGLU ? a->N / 2 : a->N), "%s: ldy=%d is too small", fn, a->ldy);
+  B2L_CHECK_SUPPORTED(batch_ring_stages(a->M, W8) >= 2, "%s: M=%d does not leave room for the weight ring", fn, a->M);
+  return 0;
+}
+}  // namespace b2l
+
+namespace {
+// b2l_w8_gemv_batch (W8 = true) and b2l_q4_gemv_batch_i8 (W8 = false): the same checks, workspace and launches
+template <bool W8>
+int batch_entry(const b2l_q4_linear_args* a, b2l_stream_t stream) {
+  if (int rc = check_gemv_batch_i8(a, W8)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   const bool pdl = (a->flags & B2L_F_PDL) != 0;
 
@@ -459,13 +474,13 @@ int batch_entry(const b2l_q4_linear_args* a, b2l_stream_t stream) {
   p.epilogue = a->epilogue; p.res = (const __nv_bfloat16*)a->res; p.ldres = a->ldres;
   p.nst = 0;
   const int grid = a->split_k;   // split_k doubles as a grid override
-  switch ((NDIG * a->M + 7) / 8) {
-    case 1: return launch_batch<1, W8>(p, grid, pdl, st, fn);
-    case 2: return launch_batch<2, W8>(p, grid, pdl, st, fn);
-    case 3: return launch_batch<3, W8>(p, grid, pdl, st, fn);
-    case 4: return launch_batch<4, W8>(p, grid, pdl, st, fn);
-    case 5: return launch_batch<5, W8>(p, grid, pdl, st, fn);
-    default: return launch_batch<6, W8>(p, grid, pdl, st, fn);
+  switch (column_groups(a->M)) {
+    case 1: return launch_batch<1, W8>(p, grid, pdl, st);
+    case 2: return launch_batch<2, W8>(p, grid, pdl, st);
+    case 3: return launch_batch<3, W8>(p, grid, pdl, st);
+    case 4: return launch_batch<4, W8>(p, grid, pdl, st);
+    case 5: return launch_batch<5, W8>(p, grid, pdl, st);
+    default: return launch_batch<6, W8>(p, grid, pdl, st);
   }
 }
 }  // namespace
