@@ -11,16 +11,27 @@ from diag import gemv_batch_call, gemv_call, rand_q4, ref_linear, relerr, tc_cal
 
 
 def build_tiny(dev, cfg, mode="gptq.int4", seed=1234, tile_cols=-1, exact_linears=False):
+    """A tiny model under `mode` and its oracle on the same synthetic weights.  `tile_cols` != -1 (gptq modes): one
+    (scale, zero) per group of that many input columns, each linear built as utils.quantization builds it but with
+    that group size."""
+    import functools
+
     import lit_llama_b200 as P
+    from lit_llama_b200.quantization import ColBlockQuantizedLinear
     from lit_llama_b200.utils import quantization
     from oracle import llama_oracle as O
 
+    if tile_cols != -1 and mode not in ("gptq.int4", "gptq.int8"):
+        raise ValueError(f"build_tiny: tile_cols applies to gptq.int4 / gptq.int8, not {mode}")
     sd = O.synth_state_dict(cfg["n_layer"], cfg["n_head"], cfg["n_embd"], cfg["vocab_size"], None if mode == "llm.int8" else mode,
-                            dtype=torch.bfloat16, seed=seed)  # llm.int8 loads a float checkpoint and quantises on load
+                            dtype=torch.bfloat16, seed=seed, tile_cols=tile_cols)  # llm.int8 loads a float checkpoint and quantises on load
     prev = torch.get_default_dtype()
     torch.set_default_dtype(torch.bfloat16)
     try:
         with torch.device(dev), quantization(mode):
+            if tile_cols != -1:   # quantization() restores torch.nn.Linear on exit
+                torch.nn.Linear = functools.partial(ColBlockQuantizedLinear, bits=4 if mode == "gptq.int4" else 8,
+                                                    tile_cols=tile_cols)
             model = P.LLaMA(P.LLaMAConfig(**cfg))
     finally:
         torch.set_default_dtype(prev)
