@@ -163,7 +163,9 @@ enum {
                            b2l_q4_tile_i8 / b2l_w8_tile_i8 of its N rows (see b2l_q4_gemm) */
   B2L_F_GEMM_I8_LO = 8192,  /* with B2L_F_GEMM_I8: qw_tiled is a 2N-row interleaved b2l_*_tile_i8 tiling and the layer
                            is rows 0..7 of its every 16-row block (c_fc1 of the fc1|fc2 tiling); N % 8 == 0 */
-  B2L_F_GEMM_I8_HI = 16384  /* the same, rows 8..15 of every 16-row block (c_fc2) */
+  B2L_F_GEMM_I8_HI = 16384, /* the same, rows 8..15 of every 16-row block (c_fc2) */
+  B2L_F_KV_FP8 = 1 << 15    /* b2l_decode_step: every layer's KV cache is fp8 (b2l_decode_args::kv8, b2l_attention_kv8);
+                               on every route, not with `plan`, B2L_F_STEPWISE or B2L_F_ATTN_UNFUSED; head_size 128 */
 };
 
 /* Fused [RMSNorm ->] int4 linear [-> residual | SwiGLU] on wgmma (M <= 16).  Replaces
@@ -614,6 +616,51 @@ int b2l_lora_apply_rows(const b2l_lora* sets, int n_sets, const int32_t* row_set
                         const void* norm_scale, float eps, void* y, int ldy, int M, int N, int K, int flags,
                         b2l_stream_t stream);
 
+/* ------------------------------------------------------------------------------
+ * fp8 KV cache (opt-in): e4m3 keys and values with one power-of-two scale per (row, head, slot),
+ * half the bytes of the bf16 cache.  Number format, for each cached vector x[0..127] (the bf16
+ * value the bf16 cache would hold there: the rotated key bf16(rot(k)), or the value):
+ *   amax = max |x_i|;  e = 0 when amax == 0, else the smallest integer with amax 2^-e <= 448,
+ *                      raised to -124 when smaller (so the smallest bf16 subnormal, 2^-133, maps to
+ *                      the smallest e4m3 subnormal, 2^-9, and nothing nonzero rounds to zero)
+ *   code_i = e4m3fn(x_i 2^-e), round to nearest even (cvt.rn.satfinite.e4m3x2.f32; torch.float8_e4m3fn
+ *            agrees: every scaled input is at most 448)
+ *   scale  = 2^e (fp32)
+ * The value read back is float(code_i) * scale in fp32: a bf16 number, exact, except that a code
+ * of 256 or more at e = 120 (|x_i| >= 1.9375 2^127, the top of the bf16 range) reads back as +-inf.
+ * A vector with a non-finite element (NaN, +-inf) is stored as NaN codes (0x7f) and a NaN scale,
+ * so every value read back from it is NaN.
+ *   k, v              e4m3 codes [B, nh, S, hs], 16-byte aligned, in the slot / ring order of the bf16 cache
+ *   k_scale, v_scale  fp32 [B, nh, S]
+ * ---------------------------------------------------------------------------- */
+typedef struct b2l_kv8_cache {
+  void* k;
+  void* v;
+  float* k_scale;
+  float* v_scale;
+} b2l_kv8_cache;
+/* b2l_attention (b2l_attention_adapter when prefix != NULL) on an fp8 cache, head_size 128:
+ *  - T == 1: the fused decode kernel.  It quantizes the new key / value into the cache and scores
+ *    and accumulates them as the values read back; every old value is float(code) * scale, and
+ *    every FMA, the split plan and the merge are those of the bf16 kernel.  So the result equals
+ *    b2l_attention on a bf16 cache holding the values read back, and each row of a B-row launch
+ *    equals the B = 1 launch on that row.  B2L_F_ROW_POS and B2L_F_PDL as for b2l_attention.
+ *  - T > 1: a prefill at positions 0..T-1 (input_pos must be NULL): q and k are rotated in place,
+ *    the rotated keys and the values are quantized into slots (t + ring_start[0]) % S, and the
+ *    prompt attends over its own bf16 rows as b2l_attention_nocache(_adapter) does.
+ * Refused before any launch: head_size != 128, B2L_F_STEPWISE, B2L_F_ATTN_UNFUSED, B2L_F_ROPE_ROWS
+ * (B2L_E_UNSUPPORTED), and T > 1 with an input_pos (B2L_E_UNSUPPORTED: no prefill at a nonzero
+ * position).  work as for b2l_attention. */
+int b2l_attention_kv8(void* qkv, const b2l_kv8_cache* kv, const void* rope, const int64_t* input_pos,
+                      const int32_t* ring_start, void* y, void* work, int B, int T, int n_head, int head_size,
+                      int S, int block_size, int flags, const b2l_adapter_prefix* prefix, b2l_stream_t stream);
+/* b2l_kv_unroll / b2l_kv_unroll_rows for one fp8 cache tensor (codes and their scales): `out` bf16
+ * [B, nh, S, hs] holds the values read back, in logical slot order. */
+int b2l_kv8_unroll(const void* code, const float* scale, const int32_t* ring_start, void* out, int B,
+                   int n_head, int S, int head_size, b2l_stream_t stream);
+int b2l_kv8_unroll_rows(const void* code, const float* scale, const int32_t* ring_start, void* out, int B,
+                        int n_head, int S, int head_size, b2l_stream_t stream);
+
 /* kv_caches as the reference would hold them (logical order): un-rotates the ring
  * into `out` [B, nh, S, hs]. */
 int b2l_kv_unroll(const void* cache, const int32_t* ring_start, void* out, int B, int n_head,
@@ -730,6 +777,9 @@ typedef struct b2l_decode_args {
                                 `affines` / `lm_head_affine` or B2L_F_STEPWISE (B2L_E_UNSUPPORTED). */
   int n_lora_sets;           /* 1..B2L_LORA_MAX_SETS                                      */
   const int32_t* lora_row_set; /* device int32 [B]: row b's set, -1 = none (read by the kernels only) */
+  const b2l_kv8_cache* kv8;  /* B2L_F_KV_FP8: HOST array [n_layer] of fp8 caches, [B, nh, S, hs] each; every layer's
+                                attention runs b2l_attention_kv8 (layers[].k_cache / v_cache are then unused).
+                                The launch count does not change.                       */
 } b2l_decode_args;
 
 /* Every linear of a step runs the same kernel.  B2L_F_W8 / B2L_F_Q8 and the batch flags select it; otherwise B == 1

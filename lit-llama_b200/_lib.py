@@ -23,6 +23,7 @@ F_STEPWISE = 2048   # b2l_attention (B == 1, T = 2..16) and b2l_decode_step: the
 F_GEMM_I8 = 4096   # b2l_{q4,w8}_gemm(_nll): qw_tiled is the batch-1 tiling (b2l_q4_tile_i8 / b2l_w8_tile_i8)
 F_GEMM_I8_LO = 8192   # with F_GEMM_I8: rows 0..7 of every 16-row block of a 2N-row interleaved tiling (c_fc1)
 F_GEMM_I8_HI = 16384   # with F_GEMM_I8: rows 8..15 of every 16-row block (c_fc2)
+F_KV_FP8 = 32768   # b2l_decode_step: every layer's KV cache is fp8 (DecodeArgs.kv8, b2l_attention_kv8)
 
 c_void_p, c_int, c_float, c_size_t = C.c_void_p, C.c_int, C.c_float, C.c_size_t
 
@@ -87,6 +88,11 @@ class Ragged(C.Structure):
                 ("len", c_int * RAGGED_MAX_SEQ)]
 
 
+class KV8Cache(C.Structure):
+    """b2l_kv8_cache: one layer's fp8 KV cache, e4m3 codes k / v [B, nh, S, hs] and fp32 scales [B, nh, S]."""
+    _fields_ = [("k", c_void_p), ("v", c_void_p), ("k_scale", c_void_p), ("v_scale", c_void_p)]
+
+
 class LayerAffine(C.Structure):
     """b2l_layer_affine: the LLaMA-Adapter v2 affines of a Block's linears (c_fc12 interleaved like its weight rows)."""
     _fields_ = [("c_attn", OutAffine), ("c_proj", OutAffine), ("c_fc12", OutAffine), ("mlp_proj", OutAffine)]
@@ -125,6 +131,7 @@ class DecodeArgs(C.Structure):
         ("affines", C.POINTER(LayerAffine)), ("lm_head_affine", OutAffine),
         ("q8_layers", C.POINTER(Q8Layer)), ("q8_lm_head", Q8Weight), ("q8_threshold", c_float),
         ("lora_sets", C.POINTER(LoRA)), ("n_lora_sets", c_int), ("lora_row_set", c_void_p),
+        ("kv8", C.POINTER(KV8Cache)),
     ]
 
 
@@ -215,6 +222,10 @@ _SIGS = {
     "b2l_attention_nocache": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "b2l_kv_unroll": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "b2l_kv_unroll_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "b2l_attention_kv8": (c_int, [c_void_p, C.POINTER(KV8Cache), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
+                                  c_int, c_int, c_int, c_int, c_int, c_int, C.POINTER(AdapterPrefix), c_void_p]),
+    "b2l_kv8_unroll": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "b2l_kv8_unroll_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "b2l_decode_step": (c_int, [C.POINTER(DecodeArgs), c_void_p]),
     "b2l_decode_step_launches": (c_int, [C.POINTER(DecodeArgs)]),
     "b2l_decode_plan_bytes": (c_size_t, [C.POINTER(DecodeArgs)]),

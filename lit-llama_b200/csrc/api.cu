@@ -13,6 +13,12 @@ int check_attention(const void* qkv, const void* k_cache, const void* v_cache, c
 int attention_impl(void* qkv, void* k_cache, void* v_cache, const void* rope, const int64_t* input_pos,
                    const int32_t* ring_start, void* y, void* work, int B, int T, int n_head, int head_size, int S,
                    int block_size, int flags, const b2l_adapter_prefix* pre, void* timeline, cudaStream_t st);
+int check_attention_kv8(const void* qkv, const b2l_kv8_cache* kv, const void* rope, const int64_t* input_pos,
+                        const int32_t* ring_start, const void* y, const void* work, int B, int T, int n_head,
+                        int head_size, int S, int block_size, int flags, const char* who);
+int attention_kv8_impl(void* qkv, const b2l_kv8_cache* kv, const void* rope, const int64_t* input_pos,
+                       const int32_t* ring_start, void* y, void* work, int B, int T, int n_head, int S, int flags,
+                       int block_size, const b2l_adapter_prefix* pre, void* timeline, cudaStream_t st);
 int check_gemv(const b2l_q4_linear_args* a, bool w8);                         // q4_gemv.cu
 int check_q4_gemv_batch(const b2l_q4_linear_args* a);                         // q4_gemv_batch.cu
 int check_gemv_batch_i8(const b2l_q4_linear_args* a, bool w8);                // w8_gemv_batch.cu
@@ -84,7 +90,7 @@ extern "C" int b2l_device_info(int* sm, int* cc_major, int* cc_minor) {
 
 // Every linear of one step runs on one route: a kernel and the tiling it reads.  resolve_route picks it from the flags,
 // B, batch_work and lm_head's tiling; the step's checks, its dispatch (linear) and b2l_decode_step_launches read it
-// from this table.  LoRA, adapters and B2L_F_ROW_POS run on every route.  The persistent kernel (plan) takes over the
+// from this table.  LoRA, adapters, B2L_F_ROW_POS and B2L_F_KV_FP8 run on every route.  The persistent kernel (plan) takes over the
 // whole step in place of the gptq.int4 routes, runs none of those, and checks its own shape (decode_mega.cu).
 enum RouteId { Q4_GEMV, Q4_BATCH, Q4_TC, Q4_BATCH_I8, W8_GEMV, W8_BATCH, Q8, Q8_BATCH };
 enum Tiling { MMA, TILED, CB };   // b2l_q4_weight::qw_mma, b2l_q4_weight::qw_tiled, llm.int8's CB / SCB
@@ -99,7 +105,7 @@ struct Route {
   bool affines;       // applies LLaMA-Adapter v2 affines in its epilogue
   bool stepwise;      // row-exact (each row equals the batch-1 step), so it may run B2L_F_STEPWISE
 };
-constexpr int Q4_FLAGS = ~(B2L_F_ROW_POS | B2L_F_STEPWISE);
+constexpr int Q4_FLAGS = ~(B2L_F_ROW_POS | B2L_F_STEPWISE | B2L_F_KV_FP8);
 // flag, B range, launches, tiling, kernel flags, batch_work, timeline, affines, stepwise
 static const Route kRoutes[] = {
     /* Q4_GEMV: b2l_q4_gemv */ {nullptr, 1, 1, 1, MMA, Q4_FLAGS, false, true, true, false},
@@ -311,6 +317,17 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
     B2L_CHECK_SUPPORTED(!plan, "b2l_decode_step: B2L_F_STEPWISE does not run in the persistent kernel (plan must be NULL)");
     B2L_CHECK_SUPPORTED(!any_affine, "b2l_decode_step: B2L_F_STEPWISE does not apply LLaMA-Adapter v2 affines");
   }
+  // B2L_F_KV_FP8: every layer's attention on its fp8 cache (kv8), whatever route the linears take
+  const bool kv8 = (d->flags & B2L_F_KV_FP8) != 0;
+  if (kv8) {
+    B2L_CHECK_SUPPORTED(!plan, "b2l_decode_step: B2L_F_KV_FP8 does not run in the persistent kernel (plan must be NULL)");
+    B2L_CHECK_SUPPORTED(!stepwise, "b2l_decode_step: B2L_F_KV_FP8 does not run B2L_F_STEPWISE (speculative verify)");
+    B2L_CHECK_SUPPORTED(!(d->flags & B2L_F_ATTN_UNFUSED),
+                        "b2l_decode_step: B2L_F_KV_FP8 runs the fused decode kernel only (not B2L_F_ATTN_UNFUSED)");
+    B2L_CHECK_SUPPORTED(d->n_embd / d->n_head == 128,
+                        "b2l_decode_step: B2L_F_KV_FP8 runs head_size 128 only (every LLaMA size), got %d", d->n_embd / d->n_head);
+    B2L_CHECK_ARG(d->kv8 != nullptr, "b2l_decode_step: B2L_F_KV_FP8 needs kv8 (one b2l_kv8_cache per layer)");
+  }
   B2L_CHECK_SUPPORTED(!row_pos || !plan, "b2l_decode_step: B2L_F_ROW_POS does not run in the persistent kernel (plan must be NULL)");
   B2L_CHECK_SUPPORTED(!row_pos || !(d->flags & B2L_F_ROPE_ROWS), "b2l_decode_step: B2L_F_ROW_POS does not combine with B2L_F_ROPE_ROWS");
   if (R.flag != nullptr) {   // a route a flag selects: its batch range, no persistent kernel, and its workspace
@@ -387,7 +404,11 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
       const Linear li = linear_of(d, l, k);
       if (int rc = in_step(linear(r, d, li, nullptr, false, stream), d, li)) return rc;
     }
-    if (l < d->n_layer) {
+    if (l < d->n_layer && kv8) {
+      if (int rc = check_attention_kv8(d->qkv, &d->kv8[l], d->rope, d->input_pos, d->ring_start, d->att, d->attn_work, aB,
+                                       aT, d->n_head, hs, d->S, d->block_size, afl, "b2l_decode_step"))
+        return rc;
+    } else if (l < d->n_layer) {
       const b2l_layer& L = d->layers[l];
       if (int rc = check_attention(d->qkv, L.k_cache, L.v_cache, d->rope, d->input_pos, d->ring_start, d->att,
                                    d->attn_work, aB, aT, d->n_head, hs, d->S, d->block_size, afl, "b2l_decode_step"))
@@ -428,8 +449,10 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
                         d->eps, d->qkv, 3 * C, B, 3 * C, C, pdl, stream, "b2l_decode_step")))
       return rc;
     const b2l_adapter_prefix* pre = (d->adapters != nullptr && d->adapters[l].len != 0) ? &d->adapters[l] : nullptr;
-    if ((rc = attention_impl(d->qkv, L.k_cache, L.v_cache, d->rope, d->input_pos, d->ring_start, d->att, d->attn_work, aB,
-                             aT, d->n_head, hs, d->S, d->block_size, afl, pre, tl(5 * l + 1), (cudaStream_t)stream)))
+    if ((rc = kv8 ? attention_kv8_impl(d->qkv, &d->kv8[l], d->rope, d->input_pos, d->ring_start, d->att, d->attn_work, B,
+                                       1, d->n_head, d->S, afl, d->block_size, pre, tl(5 * l + 1), (cudaStream_t)stream)
+                  : attention_impl(d->qkv, L.k_cache, L.v_cache, d->rope, d->input_pos, d->ring_start, d->att, d->attn_work,
+                                   aB, aT, d->n_head, hs, d->S, d->block_size, afl, pre, tl(5 * l + 1), (cudaStream_t)stream)))
       return rc;
     for (int k = 1; k < 4; ++k)
       if ((rc = linear(r, d, linear_of(d, l, k), tl(5 * l + k + 1), true, stream))) return rc;

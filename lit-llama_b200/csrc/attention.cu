@@ -5,11 +5,81 @@
 //
 // All positions are read on the device; the host never synchronises (the reference
 // does once per layer per token, model.py:214).
+#include <cuda_fp16.h>
+#include <cuda_fp8.h>
+
 #include <cstdlib>
 
 #include "b2l_common.cuh"
 
 namespace b2l {
+
+// ---- fp8 KV cache (b2l_attention_kv8, B2L_F_KV_FP8): the number format of include/b2l.h ----
+constexpr int KV8_E_MIN = -124;   // 2^-9 (smallest e4m3 subnormal) x 2^-124 = 2^-133, the smallest bf16 subnormal
+
+// scale exponent e of a vector whose largest |element| has the fp32 bits a (finite): the smallest e with
+// amax 2^-e <= 448, at least KV8_E_MIN; 0 for an all-zero vector
+__device__ __forceinline__ int kv8_exponent(uint32_t a) {
+  if (a == 0) return 0;
+  if (a < 0x00800000u) return KV8_E_MIN;   // fp32 subnormal: far below 2^(KV8_E_MIN + 8)
+  const int e = (int)(a >> 23) - 127 - 8 + ((a & 0x7fffffu) > 0x600000u);   // mantissa above 1.75: one binade up
+  return e < KV8_E_MIN ? KV8_E_MIN : e;
+}
+__device__ __forceinline__ uint32_t abs_bits(float x) { return __float_as_uint(x) & 0x7fffffffu; }
+
+// two values times inv = 2^-e as e4m3 codes (round to nearest even; |x inv| <= 448, so satfinite never clips), x in the
+// low byte
+__device__ __forceinline__ uint32_t kv8_code2(float a, float b, float inv) {
+  return (uint32_t)__nv_cvt_float2_to_fp8x2(make_float2(a * inv, b * inv), __NV_SATFINITE, __NV_E4M3);
+}
+// the values two codes (low byte first) stand for: float(code) x scale
+__device__ __forceinline__ void kv8_value2(uint32_t c, float s, float& a, float& b) {
+  const __half2_raw r = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(c & 0xffffu), __NV_E4M3);
+  const float2 f = __half22float2(__half2(r));
+  a = f.x * s;
+  b = f.y * s;
+}
+__device__ __forceinline__ float kv8_value(uint8_t c, float s) {
+  return __half2float(__half(__nv_cvt_fp8_to_halfraw((__nv_fp8_storage_t)c, __NV_E4M3))) * s;
+}
+// The value of one e4m3fn code (not NaN) from its bits, exact.  The new token's values are decoded this way from the
+// code words kv8_quant16 returns, the words that are stored (kv8_decode16).
+__device__ __forceinline__ float e4m3_value(uint32_t c) {
+  const float mag = (c & 0x78u) ? __uint_as_float(((((c >> 3) & 15u) + 120u) << 23) | ((c & 7u) << 20))
+                                : (float)(c & 7u) * 0.001953125f;   // subnormal: m 2^-9
+  return (c & 0x80u) ? -mag : mag;
+}
+// 16 codes (16 consecutive dims) -> fp32 values
+__device__ __forceinline__ void kv8_to_f32(const uint4& u, float s, float* f) {
+  const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    kv8_value2(w[i], s, f[4 * i], f[4 * i + 1]);
+    kv8_value2(w[i] >> 16, s, f[4 * i + 2], f[4 * i + 3]);
+  }
+}
+// Quantizes 16 values of a vector whose largest |element| has the fp32 bits a: returns their codes and the vector's
+// scale.  A non-finite element makes every code NaN (0x7f) and the scale NaN.
+__device__ __forceinline__ uint4 kv8_quant16(const float* f, uint32_t a, float& scale) {
+  if (a >= 0x7f800000u) {
+    scale = __uint_as_float(0x7fc00000u);
+    return make_uint4(0x7f7f7f7fu, 0x7f7f7f7fu, 0x7f7f7f7fu, 0x7f7f7f7fu);
+  }
+  const int e = kv8_exponent(a);
+  scale = __uint_as_float((uint32_t)(127 + e) << 23);
+  const float inv = __uint_as_float((uint32_t)(127 - e) << 23);
+  uint32_t w[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+    w[i] = (kv8_code2(f[4 * i], f[4 * i + 1], inv) & 0xffffu) | (kv8_code2(f[4 * i + 2], f[4 * i + 3], inv) << 16);
+  return make_uint4(w[0], w[1], w[2], w[3]);
+}
+// The values 16 codes of kv8_quant16 stand for (NaN codes: NaN, since the scale is NaN then)
+__device__ __forceinline__ void kv8_decode16(const uint4& u, float s, float* f) {
+  const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+  for (int i = 0; i < 16; ++i) f[i] = e4m3_value((w[i >> 2] >> (8 * (i & 3))) & 0xffu) * s;
+}
 
 __global__ void ring_advance_kernel(const int64_t* __restrict__ input_pos, int T, int32_t* ring_start, int S) {
   if (threadIdx.x == 0 && blockIdx.x == 0) {
@@ -86,6 +156,58 @@ __global__ void rope_append_kernel(__nv_bfloat16* __restrict__ qkv, __nv_bfloat1
       vd[2 * i] = v[2 * i];
       vd[2 * i + 1] = v[2 * i + 1];
     }
+  }
+}
+
+// Prefill of a prompt at positions 0..T-1 into an fp8 cache (b2l_attention_kv8, T > 1): grid (B*T, n_head), block 64
+// (one thread per rotated pair).  q and k are rotated in place as rope_append_kernel does without a cache (the prompt
+// then attends over its own bf16 rows), and the rotated k row and the v row are quantized into slot
+// (t + ring_start[0]) % S of row b.
+__global__ void __launch_bounds__(64)
+    rope_append_kv8_kernel(__nv_bfloat16* __restrict__ qkv, uint8_t* __restrict__ k_code, uint8_t* __restrict__ v_code,
+                           float* __restrict__ k_scale, float* __restrict__ v_scale, const float* __restrict__ rope,
+                           const int32_t* __restrict__ ring_start, int T, int n_head, int S) {
+  constexpr int HS = 128;
+  __shared__ uint32_t red[2][2];
+  const int bt = blockIdx.x, h = blockIdx.y, b = bt / T, t = bt % T, i = threadIdx.x;
+  const int C = n_head * HS;
+  __nv_bfloat16* q = qkv + (size_t)bt * 3 * C + h * HS;
+  __nv_bfloat16* k = q + C;
+  const __nv_bfloat16* v = q + 2 * C;
+  const float c = rope[((size_t)t * (HS / 2) + i) * 2 + 0];
+  const float s = rope[((size_t)t * (HS / 2) + i) * 2 + 1];
+  const float q0 = bf2f(q[2 * i]), q1 = bf2f(q[2 * i + 1]);
+  const float k0 = bf2f(k[2 * i]), k1 = bf2f(k[2 * i + 1]);
+  q[2 * i] = f2bf(__fsub_rn(__fmul_rn(q0, c), __fmul_rn(q1, s)));
+  q[2 * i + 1] = f2bf(__fadd_rn(__fmul_rn(q1, c), __fmul_rn(q0, s)));
+  const __nv_bfloat16 ke = f2bf(__fsub_rn(__fmul_rn(k0, c), __fmul_rn(k1, s)));
+  const __nv_bfloat16 ko = f2bf(__fadd_rn(__fmul_rn(k1, c), __fmul_rn(k0, s)));
+  k[2 * i] = ke;
+  k[2 * i + 1] = ko;
+  const float x[2][2] = {{bf2f(ke), bf2f(ko)}, {bf2f(v[2 * i]), bf2f(v[2 * i + 1])}};
+  const int warp = i >> 5;
+#pragma unroll
+  for (int kv = 0; kv < 2; ++kv) {
+    const uint32_t a = __reduce_max_sync(0xffffffffu, max(abs_bits(x[kv][0]), abs_bits(x[kv][1])));
+    if ((i & 31) == 0) red[kv][warp] = a;
+  }
+  __syncthreads();
+  const size_t slot = ((size_t)b * n_head + h) * S + (t + ring_start[0]) % S;
+#pragma unroll
+  for (int kv = 0; kv < 2; ++kv) {
+    const uint32_t a = max(red[kv][0], red[kv][1]);
+    uint32_t code;
+    float scale;
+    if (a >= 0x7f800000u) {   // a non-finite element: NaN codes and scale (kv8_quant16)
+      code = 0x7f7fu;
+      scale = __uint_as_float(0x7fc00000u);
+    } else {
+      const int e = kv8_exponent(a);
+      scale = __uint_as_float((uint32_t)(127 + e) << 23);
+      code = kv8_code2(x[kv][0], x[kv][1], __uint_as_float((uint32_t)(127 - e) << 23));
+    }
+    reinterpret_cast<uint16_t*>((kv ? v_code : k_code) + slot * HS)[i] = (uint16_t)code;
+    if (i == 0) (kv ? v_scale : k_scale)[slot] = scale;
   }
 }
 
@@ -231,6 +353,17 @@ __global__ void kv_unroll_kernel(const __nv_bfloat16* __restrict__ cache, const 
   for (int d = threadIdx.x; d < hs; d += blockDim.x) dst[d] = src[d];
 }
 
+// kv_unroll_kernel for an fp8 cache: the values read back, float(code) x scale, as bf16 (exact)
+__global__ void kv8_unroll_kernel(const uint8_t* __restrict__ code, const float* __restrict__ scale,
+                                  const int32_t* __restrict__ ring_start, __nv_bfloat16* __restrict__ out, int S, int hs,
+                                  int n_head, int ring_stride) {
+  const int ring = ring_start[(blockIdx.x / n_head) * ring_stride];
+  const size_t phys = (size_t)blockIdx.x * S + (blockIdx.y + ring) % S;
+  const float s = scale[phys];
+  __nv_bfloat16* dst = out + ((size_t)blockIdx.x * S + blockIdx.y) * hs;
+  for (int d = threadIdx.x; d < hs; d += blockDim.x) dst[d] = f2bf(kv8_value(code[phys * hs + d], s));
+}
+
 // ----------------------------------------------------------------------------------
 // Fused single-token attention for head_size 128 (every LLaMA size): one kernel does
 // RoPE(q), RoPE(k) + in-place KV append, split-S online-softmax attention over the valid
@@ -319,7 +452,14 @@ __device__ __forceinline__ __nv_bfloat16 adapter_combine(float y, float ay, floa
 // where a rope_append_kernel launch has already written all T new keys / values, so each query streams slots < its own
 // as old rows, scores its own key from registers as the T == 1 launch does, and stores nothing to the cache (a second
 // store of a slot would race the TMA reads of the later queries).
-template <bool ADAPTER, bool ROWS, bool STEP>
+// KV8 (b2l_attention_kv8, B2L_F_KV_FP8): k_cache / v_cache hold e4m3 codes and k_scale / v_scale one fp32 scale per
+// slot.  The ring carries 64-row sub-tiles of codes (8 KB of K, 8 KB of V); the CTA's old-row scales (<= 256 of each)
+// are loaded once, before griddepcontrol.wait, into shared memory behind the barriers (a sub-tile's scales start at any
+// slot of the ring, so they cannot always be a bulk copy's 16-byte aligned source).  Each lane turns its 16 codes into
+// float(code) x scale; every FMA, shuffle, the split plan and the merge are those of the bf16 kernel.  The new key and
+// value are quantized in registers (amax over the 8 lanes of the head), stored, and scored and accumulated as the
+// values read back, so a step depends on the cache contents only.  Not with STEP.
+template <bool ADAPTER, bool ROWS, bool STEP, bool KV8 = false>
 __global__ void __launch_bounds__(FD_WARPS * 32, ADAPTER ? FD_CTAS_PER_SM : 0)
     attn_decode_fused_kernel(const __nv_bfloat16* qkv, __nv_bfloat16* __restrict__ k_cache,
                              __nv_bfloat16* __restrict__ v_cache, const float* __restrict__ rope,
@@ -328,7 +468,8 @@ __global__ void __launch_bounds__(FD_WARPS * 32, ADAPTER ? FD_CTAS_PER_SM : 0)
                              int n_head, int S, int block_size, int n_split, unsigned long long* tl, int pre_tiles,
                              int smem_merge, int target_ctas, const __nv_bfloat16* __restrict__ pre_k,
                              const __nv_bfloat16* __restrict__ pre_v, const __nv_bfloat16* __restrict__ pre_gate,
-                             int pre_len) {
+                             int pre_len, float* k_scale, float* v_scale) {
+  static_assert(!(KV8 && STEP), "the fp8 cache does not run the stepwise verify");
   constexpr int HS = 128;
   extern __shared__ __align__(128) uint8_t fsm[];
   float* sm_acc = reinterpret_cast<float*>(fsm + 4 * FD_SUB_BYTES);                // [FD_WARPS][HS]
@@ -381,6 +522,18 @@ __global__ void __launch_bounds__(FD_WARPS * 32, ADAPTER ? FD_CTAS_PER_SM : 0)
     const int first = min(cnt, S - phys0);  // rows before the ring wraps
     const uint32_t bar = bar0 + buf * 8;
     const uint32_t kd = smem_u32(fsm) + buf * 2 * FD_SUB_BYTES, vd = kd + FD_SUB_BYTES;
+    if constexpr (KV8) {   // one byte per element
+      const uint8_t* kc = reinterpret_cast<const uint8_t*>(k_cache) + head_base;
+      const uint8_t* vc = reinterpret_cast<const uint8_t*>(v_cache) + head_base;
+      mbar_expect_tx(bar, (uint32_t)cnt * HS * 2);
+      tma_bulk_g2s(kd, kc + (size_t)phys0 * HS, (uint32_t)first * HS, bar);
+      tma_bulk_g2s(vd, vc + (size_t)phys0 * HS, (uint32_t)first * HS, bar);
+      if (first < cnt) {
+        tma_bulk_g2s(kd + first * HS, kc, (uint32_t)(cnt - first) * HS, bar);
+        tma_bulk_g2s(vd + first * HS, vc, (uint32_t)(cnt - first) * HS, bar);
+      }
+      return;
+    }
     mbar_expect_tx(bar, (uint32_t)cnt * HS * 2 * 2);
     tma_bulk_g2s(kd, k_cache + head_base + (size_t)phys0 * HS, (uint32_t)first * HS * 2, bar);
     tma_bulk_g2s(vd, v_cache + head_base + (size_t)phys0 * HS, (uint32_t)first * HS * 2, bar);
@@ -397,6 +550,17 @@ __global__ void __launch_bounds__(FD_WARPS * 32, ADAPTER ? FD_CTAS_PER_SM : 0)
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     if (n_sub > 0) request(0);
     if (pre > 1 && n_sub > 1) request(1);
+  }
+  // KV8: the scales of old rows j0 .. j0 + n_old - 1 (thread j - j0 loads row j's)
+  float* sks = reinterpret_cast<float*>(fsm + FD_SMEM_BYTES);
+  float* svs = sks + FD_CHUNK;
+  if constexpr (KV8) {
+    if (threadIdx.x < n_old) {
+      int ph = j0 + threadIdx.x + ring; if (ph >= S) ph -= S;
+      const size_t si = head_base / HS + ph;
+      sks[threadIdx.x] = k_scale[si];
+      svs[threadIdx.x] = v_scale[si];
+    }
   }
   if constexpr (ADAPTER) {
     if (threadIdx.x == 0) {   // the head's prefix rows
@@ -478,6 +642,27 @@ __global__ void __launch_bounds__(FD_WARPS * 32, ADAPTER ? FD_CTAS_PER_SM : 0)
       out[i] = (__float_as_uint(kf[2 * i]) >> 16) | (__float_as_uint(kf[2 * i + 1]) & 0xffff0000u);
     }
     const uint4 va = ld_coherent_u4(qrow + 2 * C), vb = ld_coherent_u4(qrow + 2 * C + 8);
+    if constexpr (KV8) {   // quantize the head's key and value (lanes 0..7 hold it), store, go on with the values read back
+      bf16x8_to_f32(va, vf); bf16x8_to_f32(vb, vf + 8);
+      uint32_t ka = 0, vam = 0;
+#pragma unroll
+      for (int e = 0; e < 16; ++e) { ka = max(ka, abs_bits(kf[e])); vam = max(vam, abs_bits(vf[e])); }
+#pragma unroll
+      for (int o = 1; o <= 4; o <<= 1) {
+        ka = max(ka, __shfl_xor_sync(0x000000ffu, ka, o));
+        vam = max(vam, __shfl_xor_sync(0x000000ffu, vam, o));
+      }
+      float ksc, vsc;
+      const uint4 kq = kv8_quant16(kf, ka, ksc), vq = kv8_quant16(vf, vam, vsc);
+      kv8_decode16(kq, ksc, kf);
+      kv8_decode16(vq, vsc, vf);
+      *reinterpret_cast<uint4*>(reinterpret_cast<uint8_t*>(k_cache) + head_base + (size_t)phys * HS + d0) = kq;
+      *reinterpret_cast<uint4*>(reinterpret_cast<uint8_t*>(v_cache) + head_base + (size_t)phys * HS + d0) = vq;
+      if (lane == 0) {
+        k_scale[head_base / HS + phys] = ksc;
+        v_scale[head_base / HS + phys] = vsc;
+      }
+    } else {
     if constexpr (!STEP) {
       uint4* kd = reinterpret_cast<uint4*>(k_cache + head_base + (size_t)phys * HS + d0);
       uint4* vd = reinterpret_cast<uint4*>(v_cache + head_base + (size_t)phys * HS + d0);
@@ -485,6 +670,7 @@ __global__ void __launch_bounds__(FD_WARPS * 32, ADAPTER ? FD_CTAS_PER_SM : 0)
       vd[0] = va; vd[1] = vb;
     }
     bf16x8_to_f32(va, vf); bf16x8_to_f32(vb, vf + 8);
+    }
     float sc = 0.f;
 #pragma unroll
     for (int e = 0; e < 16; ++e) sc = fmaf(q[e], kf[e], sc);
@@ -512,15 +698,23 @@ __global__ void __launch_bounds__(FD_WARPS * 32, ADAPTER ? FD_CTAS_PER_SM : 0)
     float sc[2];
     bool valid[2];
     const uint4* vr[2];
+    int rcs[2];   // KV8: the rows' index into the scales
 #pragma unroll
     for (int it = 0; it < 2; ++it) {
       const int r = warp * 8 + it * 4 + grp;
       valid[it] = r < cnt;
       const int rc = valid[it] ? r : 0;
+      float kf[16];
+      if constexpr (KV8) {
+        const uint8_t* kt8 = fsm + buf * 2 * FD_SUB_BYTES;
+        rcs[it] = i * FD_SUB + rc;
+        vr[it] = reinterpret_cast<const uint4*>(kt8 + FD_SUB_BYTES + (size_t)rc * HS + d0);
+        kv8_to_f32(*reinterpret_cast<const uint4*>(kt8 + (size_t)rc * HS + d0), sks[rcs[it]], kf);
+      } else {
       const uint4* kr = reinterpret_cast<const uint4*>(kt + (size_t)rc * HS + d0);
       vr[it] = reinterpret_cast<const uint4*>(vt + (size_t)rc * HS + d0);
-      float kf[16];
       bf16x8_to_f32(kr[0], kf); bf16x8_to_f32(kr[1], kf + 8);
+      }
       float a0 = 0.f, a1 = 0.f;
 #pragma unroll
       for (int e = 0; e < 8; ++e) { a0 = fmaf(q[e], kf[e], a0); a1 = fmaf(q[8 + e], kf[8 + e], a1); }
@@ -537,8 +731,13 @@ __global__ void __launch_bounds__(FD_WARPS * 32, ADAPTER ? FD_CTAS_PER_SM : 0)
       if (mn != -INFINITY) {   // at least one key so far in this lane group
         const float corr = __expf(m - mn), p0 = __expf(s0 - mn), p1 = __expf(s1 - mn);   // exp(-inf) = 0
         float v0[16], v1[16];
+        if constexpr (KV8) {
+          kv8_to_f32(vr[0][0], svs[rcs[0]], v0);
+          kv8_to_f32(vr[1][0], svs[rcs[1]], v1);
+        } else {
         bf16x8_to_f32(vr[0][0], v0); bf16x8_to_f32(vr[0][1], v0 + 8);
         bf16x8_to_f32(vr[1][0], v1); bf16x8_to_f32(vr[1][1], v1 + 8);
+        }
         l = l * corr + p0 + p1;
 #pragma unroll
         for (int e = 0; e < 16; ++e) acc[e] = fmaf(p1, v1[e], fmaf(p0, v0[e], acc[e] * corr));
@@ -1089,7 +1288,7 @@ int attention_impl(void* qkv, void* k_cache, void* v_cache, const void* rope, co
                                   (float*)work, tickets, n_head, S, block_size, n_split, (unsigned long long*)timeline, env_pre, env_smem_merge,
                                   FD_CTAS_PER_SM * sm_count(), (const __nv_bfloat16*)(pf ? pf->k : nullptr),
                                   (const __nv_bfloat16*)(pf ? pf->v : nullptr), (const __nv_bfloat16*)(pf ? pf->gate : nullptr),
-                                  pf ? pf->len : 0));
+                                  pf ? pf->len : 0, (float*)nullptr, (float*)nullptr));
       return 0;
     };
     if (step)
@@ -1114,7 +1313,113 @@ int attention_impl(void* qkv, void* k_cache, void* v_cache, const void* rope, co
     return rc;
   return pre == nullptr ? 0 : launch_adapter_prefix(qkv, pre, y, B, T, n_head, head_size, st);
 }
+
+// b2l_attention_kv8's argument checks (`who` names the caller): 0, or B2L_E_* with a message
+int check_attention_kv8(const void* qkv, const b2l_kv8_cache* kv, const void* rope, const int64_t* input_pos,
+                        const int32_t* ring_start, const void* y, const void* work, int B, int T, int n_head,
+                        int head_size, int S, int block_size, int flags, const char* who) {
+  B2L_CHECK_ARG(qkv && kv && rope && ring_start && y && work, "%s: null pointer", who);
+  B2L_CHECK_ARG(kv->k && kv->v && kv->k_scale && kv->v_scale, "%s: null fp8 cache pointer (b2l_kv8_cache)", who);
+  B2L_CHECK_ARG(((uintptr_t)kv->k & 15) == 0 && ((uintptr_t)kv->v & 15) == 0 && ((uintptr_t)kv->k_scale & 3) == 0 &&
+                    ((uintptr_t)kv->v_scale & 3) == 0,
+                "%s: fp8 cache codes must be 16-byte aligned, scales 4-byte aligned", who);
+  B2L_CHECK_ARG(B > 0 && T > 0 && n_head > 0 && S > 0 && T <= S && T <= block_size && block_size > 0, "%s: bad shape", who);
+  B2L_CHECK_SUPPORTED(head_size == 128, "%s: the fp8 KV cache runs head_size 128 only (every LLaMA size), got %d", who,
+                      head_size);
+  B2L_CHECK_SUPPORTED(!(flags & B2L_F_STEPWISE), "%s: the fp8 KV cache does not run B2L_F_STEPWISE (speculative verify)", who);
+  B2L_CHECK_SUPPORTED(!(flags & B2L_F_ATTN_UNFUSED), "%s: the fp8 KV cache runs the fused decode kernel only (not B2L_F_ATTN_UNFUSED)",
+                      who);
+  B2L_CHECK_SUPPORTED(!(flags & B2L_F_ROPE_ROWS), "%s: the fp8 KV cache reads the RoPE table (not B2L_F_ROPE_ROWS)", who);
+  if (T > 1) {
+    B2L_CHECK_SUPPORTED(input_pos == nullptr,
+                        "%s: T > 1 is a prefill at positions 0..T-1 and takes input_pos == NULL (a prefill into an fp8 cache at a nonzero position is not supported)",
+                        who);
+    B2L_CHECK_SUPPORTED(!(flags & B2L_F_ROW_POS), "%s: B2L_F_ROW_POS runs one token per row (T == 1), got T=%d", who, T);
+  } else {
+    B2L_CHECK_ARG(input_pos != nullptr, "%s: T == 1 needs input_pos", who);
+  }
+  return 0;
+}
+
+// b2l_attention_kv8 and b2l_decode_step under B2L_F_KV_FP8, after check_attention_kv8 (and check_adapter_prefix when
+// pre != nullptr); timeline as for attention_impl
+int attention_kv8_impl(void* qkv, const b2l_kv8_cache* kv, const void* rope, const int64_t* input_pos,
+                       const int32_t* ring_start, void* y, void* work, int B, int T, int n_head, int S, int flags,
+                       int block_size, const b2l_adapter_prefix* pre, void* timeline, cudaStream_t st) {
+  constexpr int HS = 128;
+  if (T > 1) {   // prefill from position 0: quantize into the cache, attend over the prompt's own bf16 rows
+    rope_append_kv8_kernel<<<dim3(B * T, n_head), HS / 2, 0, st>>>((__nv_bfloat16*)qkv, (uint8_t*)kv->k, (uint8_t*)kv->v,
+                                                                  kv->k_scale, kv->v_scale, (const float*)rope, ring_start,
+                                                                  T, n_head, S);
+    B2L_LAUNCH_CHECK("rope_append_kv8_kernel");
+    const int C = n_head * HS;
+    const __nv_bfloat16* base = (const __nv_bfloat16*)qkv;
+    KvView kvv{base + C, base + 2 * C, (size_t)T * 3 * C, (size_t)HS, (size_t)3 * C, 0};
+    if (int rc = launch_attn(base, kvv, nullptr, nullptr, (float*)work, (__nv_bfloat16*)y, B, T, n_head, HS, T, 0, false, st))
+      return rc;
+    return pre == nullptr ? 0 : launch_adapter_prefix(qkv, pre, y, B, T, n_head, HS, st);
+  }
+  const int n_split = (S + FD_SUB - 1) / FD_SUB;
+  int* tickets = reinterpret_cast<int*>(reinterpret_cast<char*>(work) + ws_partials_bytes(B, n_head, HS, 1, S));
+  static const int env_pre = [] { const char* e = getenv("B2L_ATTN_PRE"); return e ? atoi(e) : 1; }();
+  static const int env_smem_merge = [] { const char* e = getenv("B2L_ATTN_SMEM_MERGE"); return e ? atoi(e) : 0; }();
+  constexpr int smem = FD_SMEM_BYTES + 2 * FD_CHUNK * 4;   // + the CTA's old-row scales
+  LaunchCfg lc(dim3(B * n_head, n_split), dim3(FD_WARPS * 32), smem, st, (flags & B2L_F_PDL) != 0);
+  static DynSmemCache smem_cache[2][2];   // [ADAPTER][ROWS]
+  const int rows = (flags & B2L_F_ROW_POS) ? 1 : 0;
+  auto launch = [&](auto kernel) -> int {
+    if (int rc = ensure_dyn_smem(kernel, smem, smem_cache[pre != nullptr][rows])) return rc;
+    B2L_CUDA(cudaLaunchKernelEx(&lc.cfg, kernel, (const __nv_bfloat16*)qkv, (__nv_bfloat16*)kv->k, (__nv_bfloat16*)kv->v,
+                                (const float*)rope, input_pos, ring_start, (__nv_bfloat16*)y, (float*)work, tickets, n_head,
+                                S, block_size, n_split, (unsigned long long*)timeline, env_pre, env_smem_merge,
+                                FD_CTAS_PER_SM * sm_count(), (const __nv_bfloat16*)(pre ? pre->k : nullptr),
+                                (const __nv_bfloat16*)(pre ? pre->v : nullptr),
+                                (const __nv_bfloat16*)(pre ? pre->gate : nullptr), pre ? pre->len : 0, kv->k_scale,
+                                kv->v_scale));
+    return 0;
+  };
+  if (pre == nullptr)
+    return rows ? launch(attn_decode_fused_kernel<false, true, false, true>)
+                : launch(attn_decode_fused_kernel<false, false, false, true>);
+  return rows ? launch(attn_decode_fused_kernel<true, true, false, true>)
+              : launch(attn_decode_fused_kernel<true, false, false, true>);
+}
 }  // namespace b2l
+
+extern "C" int b2l_attention_kv8(void* qkv, const b2l_kv8_cache* kv, const void* rope, const int64_t* input_pos,
+                                 const int32_t* ring_start, void* y, void* work, int B, int T, int n_head, int head_size,
+                                 int S, int block_size, int flags, const b2l_adapter_prefix* prefix, b2l_stream_t stream) {
+  if (int rc = check_attention_kv8(qkv, kv, rope, input_pos, ring_start, y, work, B, T, n_head, head_size, S, block_size,
+                                   flags, "b2l_attention_kv8"))
+    return rc;
+  if (int rc = check_row_pos(flags, T, "b2l_attention_kv8")) return rc;
+  if (prefix != nullptr) {
+    if (int rc = check_adapter_prefix(prefix, "b2l_attention_kv8")) return rc;
+  }
+  return attention_kv8_impl(qkv, kv, rope, input_pos, ring_start, y, work, B, T, n_head, S, flags, block_size, prefix,
+                            nullptr, (cudaStream_t)stream);
+}
+
+static int kv8_unroll(const void* code, const float* scale, const int32_t* ring_start, void* out, int B, int n_head, int S,
+                      int head_size, int ring_stride, b2l_stream_t stream, const char* who) {
+  B2L_CHECK_ARG(code && scale && ring_start && out, "%s: null pointer", who);
+  B2L_CHECK_ARG(B > 0 && n_head > 0 && S > 0 && head_size > 0, "%s: bad shape", who);
+  kv8_unroll_kernel<<<dim3(B * n_head, S), 64, 0, (cudaStream_t)stream>>>((const uint8_t*)code, scale, ring_start,
+                                                                          (__nv_bfloat16*)out, S, head_size, n_head,
+                                                                          ring_stride);
+  B2L_LAUNCH_CHECK("kv8_unroll_kernel");
+  return 0;
+}
+
+extern "C" int b2l_kv8_unroll(const void* code, const float* scale, const int32_t* ring_start, void* out, int B,
+                              int n_head, int S, int head_size, b2l_stream_t stream) {
+  return kv8_unroll(code, scale, ring_start, out, B, n_head, S, head_size, 0, stream, "b2l_kv8_unroll");
+}
+
+extern "C" int b2l_kv8_unroll_rows(const void* code, const float* scale, const int32_t* ring_start, void* out, int B,
+                                   int n_head, int S, int head_size, b2l_stream_t stream) {
+  return kv8_unroll(code, scale, ring_start, out, B, n_head, S, head_size, 1, stream, "b2l_kv8_unroll_rows");
+}
 
 extern "C" int b2l_attention(void* qkv, void* k_cache, void* v_cache, const void* rope, const int64_t* input_pos,
                              const int32_t* ring_start, void* y, void* work, int B, int T, int n_head,

@@ -572,6 +572,7 @@ def main(
     stream: bool = False,
     lora_path: Optional[Sequence[Path]] = None,
     lora_alpha: float = 16,
+    kv_cache: Optional[str] = None,
 ) -> None:
     """generate.py:94-155 without Fabric: bf16 on cuda:0, same prints on stderr.  `batch_size` > 1 draws the samples
     in groups of up to `batch_size` (at most 16) through `generate_batch`, on the model's exact batched decode step.
@@ -581,7 +582,8 @@ def main(
     and decodes each sample with `generate_speculative`, `num_draft` draft tokens per round.  `lora_path` (one or
     more LoRA checkpoints over a quantized base) builds the model under `lora(r, lora_alpha, 0)`, r from the first
     file, loads the first as adapter 0 (generate/lora.py's way) and registers the others with `add_lora_adapter`;
-    with `prompts_file` a line may then start with `<k>\t` to decode with adapter k (adapter 0 without it)."""
+    with `prompts_file` a line may then start with `<k>\t` to decode with adapter k (adapter 0 without it).
+    `kv_cache` "fp8" gives the model an fp8 KV cache (LLaMA.kv_cache_dtype; not with a draft model)."""
     if not 1 <= batch_size <= MAX_SAMPLES:
         raise ValueError(f"batch_size = {batch_size}; 1..{MAX_SAMPLES}")
     from sentencepiece import SentencePieceProcessor
@@ -624,6 +626,7 @@ def main(
     from .lora import add_lora_adapter, lora as lora_ctx
 
     model = load(checkpoint_path, quantize, loras)
+    model.kv_cache_dtype = kv_cache
     draft = None
     if draft_checkpoint_path is not None:
         assert Path(draft_checkpoint_path).is_file(), draft_checkpoint_path
@@ -741,7 +744,12 @@ def cli() -> None:
                     help="a LoRA checkpoint over a quantized base (repeatable): the first is adapter 0, the next 1, 2, ...; "
                          "a --prompts_file line starting with '<k>\\t' decodes with adapter k")
     ap.add_argument("--lora_alpha", type=float, default=16, help="LoRA alpha of every --lora_path (scaling = alpha / r)")
+    ap.add_argument("--kv_cache", default=None, choices=[None, "fp8"],
+                    help="fp8: e4m3 keys and values with a power-of-two scale per slot and head, half the KV cache's bytes "
+                         "(default: bf16)")
     a = ap.parse_args()
+    if a.kv_cache == "fp8" and a.draft_checkpoint_path is not None:
+        ap.error("--kv_cache fp8 does not combine with --draft_checkpoint_path (the verify step keeps a bf16 cache)")
     if a.draft_checkpoint_path is not None and (a.batch_size != 1 or a.prompts_file is not None):
         ap.error("--draft_checkpoint_path decodes one sequence at a time (batch_size 1, no prompts_file)")
     if a.stream and a.prompts_file is None:

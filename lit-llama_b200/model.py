@@ -39,6 +39,17 @@ RoPECache = torch.Tensor
 KVCache = Tuple[torch.Tensor, torch.Tensor]
 
 
+class FP8KVCache(tuple):
+    """One layer's fp8 KV cache (LLaMA.kv_cache_dtype = "fp8"): unpacks as (k, v), the e4m3 codes [B, nh, S, hs] in the
+    bf16 cache's slot order, with the fp32 scales [B, nh, S] beside them as k_scale / v_scale (include/b2l.h states
+    the number format)."""
+
+    def __new__(cls, k: torch.Tensor, v: torch.Tensor, k_scale: torch.Tensor, v_scale: torch.Tensor) -> "FP8KVCache":
+        self = super().__new__(cls, (k, v))
+        self.k_scale, self.v_scale = k_scale, v_scale
+        return self
+
+
 @dataclass
 class LLaMAConfig:
     """model.py:25-40."""
@@ -217,7 +228,13 @@ class CausalSelfAttention(nn.Module):
             flags = (0 if _rope_is_table else 4) | (L.F_ROW_POS if rows else 0)  # B2L_F_ROPE_ROWS
             args = (qkv.data_ptr(), cache_k.data_ptr(), cache_v.data_ptr(), rope32.data_ptr(), pos.data_ptr(),
                     self._ring.data_ptr(), y.data_ptr(), work.data_ptr(), B, T, self.n_head, hs, S, rope32.shape[0], flags)
-            if prefix is None:
+            if isinstance(kv_cache, FP8KVCache):   # T > 1: a prefill at positions 0..T-1 (LLaMA.forward checks them)
+                kv8 = L.KV8Cache(cache_k.data_ptr(), cache_v.data_ptr(), kv_cache.k_scale.data_ptr(), kv_cache.v_scale.data_ptr())
+                L.check(lib.b2l_attention_kv8(qkv.data_ptr(), C.byref(kv8), rope32.data_ptr(), pos.data_ptr() if T == 1 else None,
+                                              self._ring.data_ptr(), y.data_ptr(), work.data_ptr(), B, T, self.n_head, hs, S,
+                                              rope32.shape[0], flags, None if prefix is None else C.byref(prefix),
+                                              L.stream_ptr()), "b2l_attention_kv8")
+            elif prefix is None:
                 L.check(lib.b2l_attention(*args, L.stream_ptr()), "b2l_attention")
             else:
                 L.check(lib.b2l_attention_adapter(*args, C.byref(prefix), L.stream_ptr()), "b2l_attention_adapter")
@@ -363,6 +380,11 @@ class _DecodeState:
 
         layers = (L.Layer * cfg.n_layer)()
         q8_layers = (L.Q8Layer * cfg.n_layer)() if q8 else None
+        # fp8 KV cache: every layer's attention reads its codes and scales (B2L_F_KV_FP8)
+        kv8 = isinstance(model.kv_caches[0], FP8KVCache)
+        kv8_arr = (L.KV8Cache * cfg.n_layer)() if kv8 else None
+        for i, c in enumerate(model.kv_caches if kv8 else ()):
+            kv8_arr[i] = L.KV8Cache(c[0].data_ptr(), c[1].data_ptr(), c.k_scale.data_ptr(), c.v_scale.data_ptr())
         for i, blk in enumerate(model.transformer.h):
             k, v = model.kv_caches[i]
             rms = dict(rms_1=bf16(blk.rms_1.scale).data_ptr(), rms_2=bf16(blk.rms_2.scale).data_ptr())
@@ -391,8 +413,11 @@ class _DecodeState:
             logits=self.logits.data_ptr(),
             flags=(model.decode_flags | (L.F_W8 if w8 else 0) | (L.F_W8_BATCH if w8b else 0) | (L.F_Q8 if q8 else 0)
                    | (L.F_Q4_BATCH_I8 if q4b else 0) | (L.F_Q8_BATCH if q8b else 0) | (L.F_ROW_POS if row_pos else 0)
-                   | (L.F_STEPWISE if stepwise else 0)),
+                   | (L.F_STEPWISE if stepwise else 0) | (L.F_KV_FP8 if kv8 else 0)),
             batch_work=None if self.batch_ws is None else self.batch_ws.data_ptr())
+        if kv8:
+            self.keep.append(kv8_arr)
+            self.args.kv8 = C.cast(kv8_arr, C.POINTER(L.KV8Cache))
         if q8:
             self.q8_layers = q8_layers
             self.args.q8_layers = C.cast(q8_layers, C.POINTER(L.Q8Layer))
@@ -425,6 +450,9 @@ class _DecodeState:
         if (model.persistent and not w8 and not q8 and adapters is None and loras is None and sets is None and affines is None
                 and B == 1 and hs == 128
                 and kmax <= 12288):
+            if kv8:
+                raise RuntimeError("LLaMA: the persistent decode kernel (B2L_PERSISTENT=1) does not read an fp8 KV cache "
+                                   "(kv_cache_dtype='fp8'); turn one of them off")
             self.plan = torch.zeros(lib.b2l_decode_plan_bytes(C.byref(self.args)), dtype=torch.uint8, device=device)
             self.args.plan = self.plan.data_ptr()
             L.check(lib.b2l_decode_plan_build(C.byref(self.args), L.stream_ptr()), "b2l_decode_plan_build")
@@ -487,6 +515,7 @@ class LLaMA(nn.Module):
         self.kv_caches: List[KVCache] = []
         self._ring: Optional[torch.Tensor] = None
         self._kv_store: Optional[torch.Tensor] = None
+        self._kv_scale: Optional[torch.Tensor] = None   # fp8 cache: the scales [n_layer, 2, B, nh, S] beside _kv_store
         self._decode: Optional[_DecodeState] = None
         self._verify = {}   # T -> _DecodeState of decode_tokens (B2L_F_STEPWISE), each with its own CUDA graph
         self._module_graph = None  # CUDA graph of the module-by-module decode step (non-fused Linear kinds)
@@ -500,6 +529,47 @@ class LLaMA(nn.Module):
     def _block(self, config: LLaMAConfig, block_idx: int) -> nn.Module:
         """Block `block_idx` of the stack (lit_llama_b200.adapter passes the index down, adapter.py:236)."""
         return Block(config)
+
+    _kv_cache_dtype: Optional[str] = None
+
+    @property
+    def kv_cache_dtype(self) -> Optional[str]:
+        """The KV cache's number format: None (bf16, the default) or "fp8" (e4m3 codes with a power-of-two fp32 scale per
+        row, head and slot, include/b2l.h: half the bytes per cached token).  Read when the cache is allocated; it cannot
+        change while a cache exists (reset_cache() first).  Under "fp8", kv_caches holds FP8KVCache entries, every
+        attention reads and appends codes (b2l_attention_kv8, the decode step's B2L_F_KV_FP8), a prefill starts at
+        position 0, and refill_rows prefills one prompt at a time; decode_tokens (speculative verify) and the persistent
+        kernel refuse it."""
+        return self._kv_cache_dtype
+
+    @kv_cache_dtype.setter
+    def kv_cache_dtype(self, value: Optional[str]) -> None:
+        if value not in (None, "fp8"):
+            raise ValueError(f"LLaMA.kv_cache_dtype: {value!r}; None (bf16) or 'fp8'")
+        if value != self._kv_cache_dtype and self._kv_store is not None:
+            raise RuntimeError(f"LLaMA.kv_cache_dtype: a {self._kv_cache_dtype or 'bf16'} KV cache exists; reset_cache() "
+                               "before changing its format")
+        self._kv_cache_dtype = value
+
+    def _new_kv_store(self, B: int, S: int, device: torch.device) -> None:
+        """A zeroed B-row KV store in the kv_cache_dtype format (and its scales), with kv_caches its per-layer views."""
+        cfg = self.config
+        shape = (cfg.n_layer, 2, B, cfg.n_head, S, cfg.n_embd // cfg.n_head)
+        if self._kv_cache_dtype == "fp8":
+            self._kv_store = torch.zeros(shape, device=device, dtype=torch.uint8).view(torch.float8_e4m3fn)
+            self._kv_scale = torch.zeros(shape[:-1], device=device, dtype=torch.float32)
+        else:
+            self._kv_store = torch.zeros(shape, device=device, dtype=torch.bfloat16)
+            self._kv_scale = None
+        self._set_kv_views()
+
+    def _set_kv_views(self) -> None:
+        """kv_caches: the per-layer views of _kv_store (and _kv_scale under fp8)."""
+        st, sc = self._kv_store, self._kv_scale
+        if sc is None:
+            self.kv_caches = [(st[i, 0], st[i, 1]) for i in range(self.config.n_layer)]
+        else:
+            self.kv_caches = [FP8KVCache(st[i, 0], st[i, 1], sc[i, 0], sc[i, 1]) for i in range(self.config.n_layer)]
 
     def _adapter_prefixes(self):
         """HOST array [n_layer] of b2l_adapter_prefix for b2l_decode_args::adapters, or None (no adapter)."""
@@ -621,6 +691,7 @@ class LLaMA(nn.Module):
         """model.py:140-145."""
         self.kv_caches.clear()
         self._kv_store = None
+        self._kv_scale = None
         self._decode = None
         self._verify = {}
         self._module_graph = None
@@ -664,12 +735,10 @@ class LLaMA(nn.Module):
         self._check_prompts(prompts, max_seq_length, "prefill_rows")
         if adapters is not None:
             self._check_adapters(adapters, len(prompts), "prefill_rows")
-        B, cfg, dev = len(prompts), self.config, prompts[0].device
+        B, dev = len(prompts), prompts[0].device
         self.reset_cache()
         self._prepare(prompts[0].view(1, -1), max_seq_length)
-        self._kv_store = torch.zeros((cfg.n_layer, 2, B, cfg.n_head, max_seq_length, cfg.n_embd // cfg.n_head),
-                                     device=dev, dtype=torch.bfloat16)
-        self.kv_caches = [(self._kv_store[i, 0], self._kv_store[i, 1]) for i in range(cfg.n_layer)]
+        self._new_kv_store(B, max_seq_length, dev)
         self._set_ring(torch.zeros(B, dtype=torch.int32, device=dev))
         return self.refill_rows(prompts, range(B), max_seq_length, adapters)
 
@@ -736,11 +805,11 @@ class LLaMA(nn.Module):
         """Indices of the prompts (given by length) that refill_rows prefills packed: those whose own batch-1 prefill
         runs every linear on the same row-exact kernel as the pack does (quantization.packs_at), so each keeps its
         batch-1 bits; [] for head sizes other than 128 (the ragged attention's) and for models with any linear outside
-        that dispatch (dense, llm.int8, whose rows interact through the batch outlier mask)."""
+        that dispatch (dense, llm.int8, whose rows interact through the batch outlier mask), and for an fp8 cache."""
         from .quantization import packs_at
 
         cfg = self.config
-        if cfg.n_embd // cfg.n_head != 128:
+        if cfg.n_embd // cfg.n_head != 128 or self._kv_scale is not None:   # an fp8 cache: one prompt at a time
             return []
         lins = self._linears()
         cand = [i for i, T in enumerate(lengths) if packs_at(lins, T, T)]
@@ -786,7 +855,7 @@ class LLaMA(nn.Module):
         """The batch-1 prefill of each prompt into its row: the model is pointed at that row of the KV store and its
         ring offset (ring[r:r+1], zeroed) for the call, and the B-row decode state and module graph are put back after
         (a one-token prompt runs, and replaces, the batch-1 step state)."""
-        ring, store, caches = self._ring, self._kv_store, self.kv_caches
+        ring, store, scale, caches = self._ring, self._kv_store, self._kv_scale, self.kv_caches
         decode, module_graph, route = self._decode, self._module_graph, self._lora_route
         out = []
         try:
@@ -799,11 +868,12 @@ class LLaMA(nn.Module):
                 for blk in self.transformer.h:
                     blk.attn._ring = one
                 self._kv_store = store[:, :, r:r + 1]
-                self.kv_caches = [(self._kv_store[i, 0], self._kv_store[i, 1]) for i in range(self.config.n_layer)]   # contiguous
+                self._kv_scale = None if scale is None else scale[:, :, r:r + 1]
+                self._set_kv_views()   # contiguous
                 self._decode, self._module_graph = None, None
                 out.append(self(p.view(1, -1), max_seq_length, torch.arange(p.numel(), device=p.device))[0, -1].clone())
         finally:
-            self._ring, self._kv_store, self.kv_caches = ring, store, caches
+            self._ring, self._kv_store, self._kv_scale, self.kv_caches = ring, store, scale, caches
             for blk in self.transformer.h:
                 blk.attn._ring = ring
             self._set_lora_route(route)
@@ -823,8 +893,13 @@ class LLaMA(nn.Module):
             return
         if B0 != 1 or B < 1:
             raise ValueError(f"expand_cache: the cache holds {B0} rows; only a batch-1 cache expands (to {B} rows)")
-        self._kv_store = self._kv_store.expand(n_layer, two, B, nh, S, hs).contiguous()
-        self.kv_caches = [(self._kv_store[i, 0], self._kv_store[i, 1]) for i in range(n_layer)]
+        if self._kv_scale is None:
+            self._kv_store = self._kv_store.expand(n_layer, two, B, nh, S, hs).contiguous()
+        else:   # fp8: the codes (copied as bytes) and their scales
+            self._kv_store = self._kv_store.view(torch.uint8).expand(n_layer, two, B, nh, S, hs).contiguous().view(
+                torch.float8_e4m3fn)
+            self._kv_scale = self._kv_scale.expand(n_layer, two, B, nh, S).contiguous()
+        self._set_kv_views()
         self._decode = None
         self._verify = {}
         self._module_graph = None
@@ -975,9 +1050,23 @@ class LLaMA(nn.Module):
     def logical_kv_caches(self) -> List[KVCache]:
         """kv_caches in the reference's slot order.  Identical to `kv_caches` until the
         roll branch (model.py:214-218) has triggered; afterwards the physical tensors are
-        a ring and this returns the un-rotated copies the reference would hold."""
+        a ring and this returns the un-rotated copies the reference would hold.  An fp8 cache returns the values read
+        back from it (float(code) * scale), as bf16."""
         out = []
         lib = L.lib()
+        if self._kv_scale is not None:   # fp8: the values read back, bf16
+            name = "b2l_kv8_unroll_rows" if self._ring.numel() > 1 else "b2l_kv8_unroll"
+            unroll = getattr(lib, name)
+            for c in self.kv_caches:
+                B, nh, S, hs = c[0].shape
+                pair = []
+                for code, scale in ((c[0], c.k_scale), (c[1], c.v_scale)):
+                    o = torch.empty((B, nh, S, hs), device=code.device, dtype=torch.bfloat16)
+                    L.check(unroll(code.data_ptr(), scale.data_ptr(), self._ring.data_ptr(), o.data_ptr(), B, nh, S, hs,
+                                   L.stream_ptr()), name)
+                    pair.append(o)
+                out.append(tuple(pair))
+            return out
         name = "b2l_kv_unroll_rows" if self._ring.numel() > 1 else "b2l_kv_unroll"   # one ring offset per row, or shared
         unroll = getattr(lib, name)
         for k, v in self.kv_caches:
@@ -1008,13 +1097,15 @@ class LLaMA(nn.Module):
                                "shape (B, 1), or reset_cache() first")
 
         if input_pos is not None and not self.kv_caches:
-            cfg = self.config
-            hs = cfg.n_embd // cfg.n_head
-            self._kv_store = torch.zeros((cfg.n_layer, 2, B, cfg.n_head, max_seq_length, hs), device=idx.device, dtype=torch.bfloat16)
-            self.kv_caches = [(self._kv_store[i, 0], self._kv_store[i, 1]) for i in range(cfg.n_layer)]
+            self._new_kv_store(B, max_seq_length, idx.device)
             self._decode = None
             self._verify = {}
             self._module_graph = None
+        if input_pos is not None and T > 1 and self._kv_scale is not None:
+            # an fp8 cache is prefilled from position 0 (one host read of the positions)
+            if input_pos.numel() != T or not bool((input_pos.reshape(-1) == torch.arange(T, device=input_pos.device)).all()):
+                raise ValueError("LLaMA.forward: an fp8 KV cache (kv_cache_dtype='fp8') takes a multi-token prompt at "
+                                 "positions 0..T-1 only; a prefill at a nonzero position is not supported")
         if rows:
             if self._kv_store.shape[2] != B:
                 raise ValueError(f"LLaMA.forward: {B} rows against a KV cache of {self._kv_store.shape[2]}")
@@ -1117,10 +1208,7 @@ class LLaMA(nn.Module):
         if self._ring.numel() != 1 or (self._kv_store is not None and self._kv_store.shape[2] != 1):
             raise RuntimeError("decode_tokens: the KV cache holds more than one sequence; reset_cache() first")
         if not self.kv_caches:
-            cfg = self.config
-            self._kv_store = torch.zeros((cfg.n_layer, 2, 1, cfg.n_head, max_seq_length, cfg.n_embd // cfg.n_head),
-                                         device=idx.device, dtype=torch.bfloat16)
-            self.kv_caches = [(self._kv_store[i, 0], self._kv_store[i, 1]) for i in range(cfg.n_layer)]
+            self._new_kv_store(1, max_seq_length, idx.device)
             self._decode, self._module_graph, self._verify = None, None, {}
         if self._kv_store.shape[4] != max_seq_length:
             raise ValueError(f"decode_tokens: max_seq_length={max_seq_length} against a cache of {self._kv_store.shape[4]}")
@@ -1149,6 +1237,8 @@ class LLaMA(nn.Module):
 
     def _decode_tokens_refusal(self) -> Optional[str]:
         """Why this model cannot run decode_tokens, or None."""
+        if self._kv_cache_dtype == "fp8" or self._kv_scale is not None:
+            return "does not run on an fp8 KV cache (kv_cache_dtype='fp8'): speculative verify keeps a bf16 cache"
         if self._fast_ok is None:
             self._fast_ok = self._fast_decode_ok()
         if self._fast_ok not in ("q4", "w8") or self._has_affines():

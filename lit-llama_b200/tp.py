@@ -256,6 +256,17 @@ class TPLLaMA(nn.Module):
         if self._ring is not None:
             self._ring.zero_()
 
+    @property
+    def kv_cache_dtype(self) -> None:
+        """Always None: the tensor-parallel step keeps a bf16 KV cache (LLaMA.kv_cache_dtype)."""
+        return None
+
+    @kv_cache_dtype.setter
+    def kv_cache_dtype(self, value) -> None:
+        if value is not None:
+            raise ValueError(f"TPLLaMA.kv_cache_dtype: {value!r} is not supported; the tensor-parallel decode step keeps "
+                             "a bf16 KV cache")
+
     def tp_comm(self, dev: torch.device) -> Optional["L.TPComm"]:
         """The peer-memory exchange of b2l_tp_allreduce (csrc/tp_allreduce.cu), created once per model (a collective
         call: every rank must get here).  Buffers come from torch's symmetric memory -- allocation + peer mapping
