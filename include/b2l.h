@@ -441,6 +441,23 @@ int b2l_spec_accept(const void* target_logits, int64_t ld, float temperature, in
                     const int64_t* draft_tokens, const float* u, const void* noise, int32_t* n_accepted, int64_t* token,
                     int T, int V, b2l_stream_t stream);
 
+/* Prompt-lookup proposal: draft tokens taken from the sequence itself, for b2l_spec_accept without a draft model.
+ * history (device int64) holds the sequence's n tokens, n = base_len + (n_accepted ? *n_accepted + 1 : 0), read on
+ * the device (n_accepted: b2l_spec_accept's device int32, so the host need not learn how many tokens the last verify
+ * step emitted).  The rule, deterministic:
+ *   for g = max_ngram down to min_ngram, skipping g > n - 1: the pattern is history[n-g .. n); i is the largest start
+ *   with i + g <= n - 1 and history[i .. i+g) == pattern (the most recent earlier occurrence; it may overlap the
+ *   pattern).  The first g with a match proposes history[i+g .. min(i+g+k, n)) into tokens[0 .. *count); tokens past
+ *   *count are not written.  No match: *count = 0.
+ * probs (bf16 [k, V], 16-byte aligned, may be NULL) receives the deterministic draft's rows: row t < *count is 1.0 at
+ * tokens[t] and 0 elsewhere; a token outside 0..V-1 and every row t >= *count are all zero.  Fed to b2l_spec_accept,
+ * x_t is then accepted iff u_t < p_t(x_t), and the residual at a rejection is p_j with x_j removed: speculative
+ * sampling with a deterministic draft.  *count is device int32.  1 <= min_ngram <= max_ngram <= 16, k in 1..15,
+ * base_len >= 1, V >= 1; null history / tokens / count and misaligned pointers are B2L_E_ARG with a message naming
+ * the argument, before the device is touched.  One CTA. */
+int b2l_ngram_propose(const int64_t* history, int base_len, const int32_t* n_accepted, int min_ngram, int max_ngram,
+                      int k, int64_t* tokens, void* probs, int32_t* count, int V, b2l_stream_t stream);
+
 /* ------------------------------------------------------------------------------
  * CausalSelfAttention.forward without the two linears, model.py:197-232:
  * split qkv, apply_rope(q), apply_rope(k) (model.py:306-323), append k,v to the

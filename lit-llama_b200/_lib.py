@@ -191,6 +191,8 @@ _SIGS = {
                                              c_void_p]),
     "b2l_spec_accept": (c_int, [c_void_p, C.c_int64, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                 c_void_p, c_int, c_int, c_void_p]),
+    "b2l_ngram_propose": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int,
+                                  c_void_p]),
     "b2l_q8_tiled_bytes": (c_size_t, [c_int, c_int]),
     "b2l_q8_tile": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "b2l_q8_gemv": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_int, c_void_p]),

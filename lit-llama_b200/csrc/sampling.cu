@@ -390,6 +390,52 @@ __global__ void __launch_bounds__(SAMP_THREADS)
   }
 }
 
+constexpr int NGRAM_THREADS = 1024;
+
+// b2l_ngram_propose: ONE CTA.  For each g from max_ngram down, the threads test the candidate starts of one chunk of
+// NGRAM_THREADS at a time, from the end of the history backwards (thread t tests start hi - t), so the first chunk with
+// a match holds the most recent occurrence: the match of the lowest thread.  Most lookups end in the first chunk.
+__global__ void __launch_bounds__(NGRAM_THREADS)
+    ngram_propose_kernel(const long long* __restrict__ history, int base_len, const int* __restrict__ n_accepted,
+                         int min_ngram, int max_ngram, int k, long long* __restrict__ tokens, __nv_bfloat16* __restrict__ probs,
+                         int* __restrict__ count, int V) {
+  __shared__ long long pat[16];
+  __shared__ int first;   // the lowest thread of the current chunk whose start matches
+  const int tid = threadIdx.x;
+  const long long n = base_len + (n_accepted != nullptr ? (long long)*n_accepted + 1 : 0);
+  long long start = -1;
+  int g = max_ngram;
+  for (; g >= min_ngram; --g) {
+    if (g > n - 1) continue;   // block-uniform
+    // the previous g's last __syncthreads_or came after its every read of pat and first
+    if (tid < g) pat[tid] = history[n - g + tid];
+    if (tid == 0) first = NGRAM_THREADS;
+    __syncthreads();
+    for (long long hi = n - 1 - g; hi >= 0; hi -= NGRAM_THREADS) {
+      const long long i = hi - tid;
+      bool hit = i >= 0;
+      for (int j = g - 1; hit && j >= 0; --j) hit = history[i + j] == pat[j];
+      if (hit) atomicMin(&first, tid);
+      if (__syncthreads_or(hit)) { start = hi - first; break; }
+    }
+    if (start >= 0) break;   // block-uniform
+  }
+  const int c = start < 0 ? 0 : (int)min((long long)k, n - (start + g));
+  if (tid < c) tokens[tid] = history[start + g + tid];
+  if (tid == 0) *count = c;
+  if (probs == nullptr) return;
+  // every element of the k rows is zeroed, then each proposed token's element set to 1.0; the barrier orders the two
+  // stores to that element
+  const size_t total = (size_t)k * V, nvec = total / 8;
+  for (size_t v = tid; v < nvec; v += NGRAM_THREADS) reinterpret_cast<uint4*>(probs)[v] = make_uint4(0, 0, 0, 0);
+  for (size_t e = nvec * 8 + tid; e < total; e += NGRAM_THREADS) reinterpret_cast<uint16_t*>(probs)[e] = 0;
+  __syncthreads();
+  if (tid < c) {
+    const long long x = history[start + g + tid];
+    if (x >= 0 && x < V) reinterpret_cast<uint16_t*>(probs)[(size_t)tid * V + x] = 0x3f80;   // bf16 1.0
+  }
+}
+
 }  // namespace b2l
 
 using namespace b2l;
@@ -466,6 +512,30 @@ extern "C" int b2l_spec_accept(const void* target_logits, int64_t ld, float temp
       (const __nv_bfloat16*)target_logits, (long long)ld, 1.0f / temperature, top_k, (const __nv_bfloat16*)draft_probs,
       (const long long*)draft_tokens, u, (const __nv_bfloat16*)noise, n_accepted, (long long*)token, T, V);
   B2L_LAUNCH_CHECK("spec_accept_kernel");
+  return 0;
+}
+
+extern "C" int b2l_ngram_propose(const int64_t* history, int base_len, const int32_t* n_accepted, int min_ngram,
+                                 int max_ngram, int k, int64_t* tokens, void* probs, int32_t* count, int V,
+                                 b2l_stream_t stream) {
+  const char* who = "b2l_ngram_propose";
+  B2L_CHECK_ARG(history != nullptr, "%s: null history", who);
+  B2L_CHECK_ARG(tokens != nullptr, "%s: null tokens", who);
+  B2L_CHECK_ARG(count != nullptr, "%s: null count", who);
+  B2L_CHECK_ARG(((uintptr_t)history % 8) == 0, "%s: history must be 8-byte aligned", who);
+  B2L_CHECK_ARG(((uintptr_t)tokens % 8) == 0, "%s: tokens must be 8-byte aligned", who);
+  B2L_CHECK_ARG(((uintptr_t)n_accepted % 4) == 0, "%s: n_accepted must be 4-byte aligned", who);
+  B2L_CHECK_ARG(((uintptr_t)count % 4) == 0, "%s: count must be 4-byte aligned", who);
+  B2L_CHECK_ARG(((uintptr_t)probs % 16) == 0, "%s: probs must be 16-byte aligned", who);
+  B2L_CHECK_ARG(base_len >= 1, "%s: base_len = %d, at least 1", who, base_len);
+  B2L_CHECK_ARG(min_ngram >= 1 && min_ngram <= max_ngram && max_ngram <= 16,
+                "%s: min_ngram = %d, max_ngram = %d; 1 <= min_ngram <= max_ngram <= 16", who, min_ngram, max_ngram);
+  B2L_CHECK_ARG(k >= 1 && k <= 15, "%s: k = %d; 1..15 (the verify step runs 2..16 tokens)", who, k);
+  B2L_CHECK_ARG(V >= 1, "%s: V = %d, at least 1", who, V);
+  ngram_propose_kernel<<<1, NGRAM_THREADS, 0, (cudaStream_t)stream>>>(
+      (const long long*)history, base_len, n_accepted, min_ngram, max_ngram, k, (long long*)tokens,
+      (__nv_bfloat16*)probs, count, V);
+  B2L_LAUNCH_CHECK("ngram_propose_kernel");
   return 0;
 }
 

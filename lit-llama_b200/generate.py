@@ -9,8 +9,8 @@ once: one batch-1 prefill per prompt into its row of the cache, then one batched
 step at per-row positions and one sampling launch per token.  `generate_stream()` decodes any number of
 prompts on up to 16 rows, refilling each finished row with the next prompt while the others keep decoding
 (continuous batching).  `generate_speculative()`
-lets a small draft model propose up to 15 tokens that the model verifies in one
-step (speculative sampling); its greedy output is `generate()`'s token for token.
+lets a small draft model, or prompt lookup over the sequence's own n-grams, propose up to 15 tokens that the model
+verifies in one step (speculative sampling); its greedy output is `generate()`'s token for token.
 `main()` mirrors the reference CLI with argparse
 (jsonargparse and lightning are not dependencies of this path)."""
 import os
@@ -221,11 +221,14 @@ def generate_batch(
 #: most draft tokens one generate_speculative() round proposes: the verify step runs 2..16 tokens
 MAX_DRAFT = 15
 
+#: longest n-gram prompt lookup matches (b2l_ngram_propose)
+MAX_NGRAM = 16
+
 
 @torch.no_grad()
 def generate_speculative(
     model: LLaMA,
-    draft: LLaMA,
+    draft: Optional[LLaMA],
     idx: torch.Tensor,
     max_new_tokens: int,
     *,
@@ -235,30 +238,46 @@ def generate_speculative(
     top_k: Optional[int] = None,
     eos_id: Optional[int] = None,
     stats: Optional[dict] = None,
+    max_ngram: int = 3,
+    min_ngram: int = 1,
 ) -> torch.Tensor:
-    """Speculative sampling: `idx` (T,) prompt -> (T + max_new_tokens,) tokens like `generate()`, with `draft` (a
-    smaller model over the same vocabulary) proposing tokens that `model` verifies several at a time.
+    """Speculative sampling: `idx` (T,) prompt -> (T + max_new_tokens,) tokens like `generate()`, with draft tokens
+    that `model` verifies several at a time.  `draft` (a smaller model over the same vocabulary) proposes them, or,
+    with `draft=None`, prompt lookup: the tokens that followed the most recent earlier occurrence of the sequence's
+    last g tokens, g = max_ngram down to min_ngram (1..16; the rule of `b2l_ngram_propose`, include/b2l.h).
 
-    Both models prefill the prompt at batch 1 and the first token is drawn from `model`'s prefill logits as in
-    `generate()`.  Each round then runs k = num_draft (1..15) batch-1 draft steps, each sampling its token with the
-    fused kernel and keeping its probability row q; one `LLaMA.decode_tokens` of `model` over the pending token and
-    the k draft tokens; and one `b2l_spec_accept` launch, which accepts draft token t while u_t q_t(x_t) < p_t(x_t)
-    and draws the next token from the residual max(0, p_j - q_j) at the first rejection j (from p_k when all are
-    accepted), so every emitted token is distributed as `model`'s own samples.  The round's only host
-    synchronisation is one 4-byte read of the number accepted.  When all k are accepted the draft also consumes the
-    last of them.  Rejected cache slots of either model are left stale: they are never read and are overwritten later.
+    `model` (and the draft) prefill the prompt at batch 1 and the first token is drawn from `model`'s prefill logits
+    as in `generate()`.  Each round proposes k = num_draft (1..15) tokens with their probability rows q: k batch-1
+    draft steps, each sampling its token with the fused kernel, or the proposal of one `b2l_ngram_propose` launch
+    (q one-hot).  Then one `LLaMA.decode_tokens` of `model` over the pending token and the k proposed tokens, and one
+    `b2l_spec_accept` launch, which accepts token t while u_t q_t(x_t) < p_t(x_t) and draws the next token from the
+    residual max(0, p_j - q_j) at the first rejection j (from p_k when all are accepted), so every emitted token is
+    distributed as `model`'s own samples.  The round's only host synchronisation is one 4-byte read of the number
+    accepted (with `eos_id`, the first eos among the emitted tokens travels in the same word).  When all k are
+    accepted the draft also consumes the last of them.  Rejected cache slots of either model are left stale: they are
+    never read and are overwritten later.
+
+    Prompt lookup launches the next round's proposer right behind the accept, over the history extended by the
+    round's emitted tokens on the device, so the same read also carries the next proposal count, and a round uses
+    min(k, count) of them.  A count of 0 runs one plain target step (`model` + `sample_token`), then the proposer,
+    then the same one read.
 
     With top_k=1 a token is accepted exactly when it is the target's argmax, and `decode_tokens` rows are bit-identical
-    to the batch-1 step, so the output equals `generate(model, ..., top_k=1)` token for token whatever the draft is.
+    to the batch-1 step, so the output equals `generate(model, ..., top_k=1)` token for token whatever is proposed.
 
     k shrinks so that the verified positions stay below max_seq_length and no round overshoots max_new_tokens; from
     the point where no draft token fits (the roll branch included) the tail runs `generate()`'s plain target steps.
     With `eos_id` the output ends at the first eos, which is included.  `stats`, when given, receives "rounds",
-    "proposed" / "accepted" (lists: draft tokens per round), "num_draft" and "tail_steps".  Call `reset_cache()` on both
-    models before the next prompt, as after `generate()`."""
+    "proposed" / "accepted" (lists: draft tokens per round), "num_draft", "tail_steps" and "lookup_misses" (plain
+    steps prompt lookup ran for want of a proposal; 0 with a draft model).  Call `reset_cache()` on the model(s)
+    before the next prompt, as after `generate()`."""
     if not 1 <= int(num_draft) <= MAX_DRAFT:
         raise ValueError(f"generate_speculative: num_draft = {num_draft}; 1..{MAX_DRAFT} (the verify step runs 2..16 tokens)")
-    if draft.config.padded_vocab_size != model.config.padded_vocab_size:
+    if draft is None:
+        if not 1 <= int(min_ngram) <= int(max_ngram) <= MAX_NGRAM:
+            raise ValueError(f"generate_speculative: min_ngram = {min_ngram}, max_ngram = {max_ngram}; "
+                             f"1 <= min_ngram <= max_ngram <= {MAX_NGRAM}")
+    elif draft.config.padded_vocab_size != model.config.padded_vocab_size:
         raise ValueError(f"generate_speculative: the draft's padded_vocab_size {draft.config.padded_vocab_size} differs from "
                          f"the target's {model.config.padded_vocab_size}")
     if idx.dim() != 1:
@@ -278,39 +297,82 @@ def generate_speculative(
     lib = L.lib()
     kmax = int(num_draft)
     k_top = 0 if top_k is None else min(int(top_k), V)
-    out = torch.empty(T_new, dtype=dtype, device=device)
+    out = torch.empty(T_new, dtype=torch.int64 if draft is None else dtype, device=device)   # lookup reads it as int64
     out[:T] = idx
     st = {} if stats is None else stats
-    st.update(rounds=0, proposed=[], accepted=[], num_draft=kmax, tail_steps=0)
+    st.update(rounds=0, proposed=[], accepted=[], num_draft=kmax, tail_steps=0, lookup_misses=0)
     if max_new_tokens <= 0:
-        return out
+        return out.to(dtype)
 
     pos_all = torch.arange(0, max(T_new, S), device=device)
     logits = model(idx.view(1, -1), S, pos_all[:T])
-    draft(idx.view(1, -1), S, pos_all[:T])
+    if draft is not None:
+        draft(idx.view(1, -1), S, pos_all[:T])
     # tokens stay int64 on the device (one step state per model: its idx dtype never changes)
     tok = sample_token(logits[0, -1], temperature, top_k)   # generate()'s first token
     out[T] = tok[0]
     n = 1                                  # tokens emitted; the last one (tok) is in neither cache yet
-    if eos_id is not None and int(tok[0]) == eos_id:
-        return out[:T + 1]
 
-    q = torch.empty((kmax, V), dtype=torch.bfloat16, device=device)   # the draft's probability rows
+    q = torch.empty((kmax, V), dtype=torch.bfloat16, device=device)   # the proposals' probability rows
     dtok = torch.empty((kmax + 1, 1), dtype=torch.int64, device=device)   # d_1..d_k, then the target's next token
     nacc = torch.zeros(1, dtype=torch.int32, device=device)
     steps = torch.arange(kmax + 1, device=device)
+    count = torch.zeros(1, dtype=torch.int32, device=device)   # prompt lookup: the proposal's length
+    none = torch.zeros(1, dtype=torch.int32, device=device)    # a plain step accepts nothing
+
+    def propose(base_len: int, grown: bool) -> None:
+        """b2l_ngram_propose over out[:base_len], plus the last round's nacc + 1 tokens when `grown`."""
+        L.check(lib.b2l_ngram_propose(out.data_ptr(), base_len, nacc.data_ptr() if grown else None, int(min_ngram),
+                                      int(max_ngram), kmax, dtok.data_ptr(), q.data_ptr(), count.data_ptr(), V,
+                                      L.stream_ptr()), "b2l_ngram_propose")
+
+    def read(em: torch.Tensor, acc: torch.Tensor):
+        """The one host read of a round or plain step: (number accepted, index of the first eos among the emitted
+        tokens em[:acc + 1] or 255, the next proposal count), packed in one word."""
+        w = acc.long()[0]
+        if eos_id is not None:
+            hit = (em == eos_id) & (steps[:em.numel()] <= w)
+            w = w | (torch.where(hit, steps[:em.numel()], 255).min() << 8)
+        if draft is None:
+            w = w | (count.long()[0] << 16)
+        w = int(w.to(torch.int32).item())
+        return w & 255, (w >> 8) & 255 if eos_id is not None else 255, w >> 16
+
+    if draft is None:
+        propose(T + 1, False)
+        _, e, c = read(tok, none)
+        if e != 255:
+            return out[:T + 1].to(dtype)
+    elif eos_id is not None and int(tok[0]) == eos_id:
+        return out[:T + 1]
+
     while n < max_new_tokens:
         p = T + n - 1                       # position of the pending token
         k = min(kmax, S - 1 - p, max_new_tokens - n - 1)
         if k < 1:
             break
-        x = tok.view(1, 1)
-        for i in range(k):                  # k batch-1 draft steps: tok, d_1 .. d_{k-1}
-            dl = draft(x, S, pos_all[p + i:p + i + 1])[0, -1].contiguous()
-            noise = torch.empty_like(dl).exponential_(1)
-            L.check(lib.b2l_topk_softmax_sample(dl.data_ptr(), float(temperature), k_top, noise.data_ptr(), q[i].data_ptr(),
-                                                dtok[i].data_ptr(), V, L.stream_ptr()), "b2l_topk_softmax_sample")
-            x = dtok[i].view(1, 1)
+        if draft is None:
+            k = min(k, c)
+            if k == 0:                      # no proposal: one plain target step, then the proposer again
+                logits = model(tok.view(1, 1), S, pos_all[p:p + 1])
+                tok = sample_token(logits[0, -1], temperature, top_k)
+                out[T + n] = tok[0]
+                n += 1
+                st["lookup_misses"] += 1
+                propose(T + n, False)
+                _, e, c = read(tok, none)
+                if e != 255:
+                    return out[:T + n].to(dtype)
+                continue
+        else:
+            x = tok.view(1, 1)
+            for i in range(k):              # k batch-1 draft steps: tok, d_1 .. d_{k-1}
+                dl = draft(x, S, pos_all[p + i:p + i + 1])[0, -1].contiguous()
+                noise = torch.empty_like(dl).exponential_(1)
+                L.check(lib.b2l_topk_softmax_sample(dl.data_ptr(), float(temperature), k_top, noise.data_ptr(),
+                                                    q[i].data_ptr(), dtok[i].data_ptr(), V, L.stream_ptr()),
+                        "b2l_topk_softmax_sample")
+                x = dtok[i].view(1, 1)
         vidx = torch.cat((tok.view(1, 1), dtok[:k].view(1, k)), dim=1)
         tl = model.decode_tokens(vidx, S, pos_all[p:p + k + 1])
         u = torch.rand(k, device=device)
@@ -319,23 +381,19 @@ def generate_speculative(
                                     noise.data_ptr(), nacc.data_ptr(), dtok[k].data_ptr(), k + 1, V, L.stream_ptr()),
                 "b2l_spec_accept")
         # the round's tokens: d_1..d_a, then the target's token (at slot a); later slots are overwritten by later rounds
-        em = torch.where(steps[:k + 1] < nacc.long(), dtok[:k + 1, 0], dtok[k, 0]).to(dtype)
+        em = torch.where(steps[:k + 1] < nacc.long(), dtok[:k + 1, 0], dtok[k, 0]).to(out.dtype)
         out[T + n:T + n + k + 1] = em
-        if eos_id is None:
-            a = int(nacc.item())            # the round's one host synchronisation
-        else:                               # the first eos among the emitted tokens travels in the same 4-byte word
-            hit = (em == eos_id) & (steps[:k + 1] <= nacc.long())
-            first = torch.where(hit, steps[:k + 1], 255).min()
-            a_e = int((nacc.long()[0] | (first << 8)).to(torch.int32).item())
-            a, e = a_e & 255, a_e >> 8
+        tok = dtok[k].clone()
+        if draft is None:                   # the next proposal, over the history grown by this round's a + 1 tokens
+            propose(T + n, True)
+        a, e, c = read(em, nacc)
         st["rounds"] += 1
         st["proposed"].append(k)
         st["accepted"].append(a)
-        if eos_id is not None and e != 255:
-            return out[:T + n + e + 1]
-        if a == k:                          # every draft token accepted: the draft also consumes d_k
+        if e != 255:
+            return out[:T + n + e + 1].to(dtype)
+        if draft is not None and a == k:    # every draft token accepted: the draft also consumes d_k
             draft(dtok[k - 1].view(1, 1), S, pos_all[p + k:p + k + 1])
-        tok = dtok[k].clone()
         n += a + 1
 
     # the tail: generate()'s plain target steps (no draft token fits below max_seq_length, or one token is left)
@@ -348,8 +406,8 @@ def generate_speculative(
         out[T + n] = tok[0]
         n += 1
         if eos_id is not None and tok == eos_id:
-            return out[:T + n]
-    return out
+            return out[:T + n].to(dtype)
+    return out.to(dtype)
 
 
 @torch.no_grad()
@@ -573,6 +631,7 @@ def main(
     lora_path: Optional[Sequence[Path]] = None,
     lora_alpha: float = 16,
     kv_cache: Optional[str] = None,
+    lookup_ngram: int = 0,
 ) -> None:
     """generate.py:94-155 without Fabric: bf16 on cuda:0, same prints on stderr.  `batch_size` > 1 draws the samples
     in groups of up to `batch_size` (at most 16) through `generate_batch`, on the model's exact batched decode step.
@@ -583,7 +642,9 @@ def main(
     more LoRA checkpoints over a quantized base) builds the model under `lora(r, lora_alpha, 0)`, r from the first
     file, loads the first as adapter 0 (generate/lora.py's way) and registers the others with `add_lora_adapter`;
     with `prompts_file` a line may then start with `<k>\t` to decode with adapter k (adapter 0 without it).
-    `kv_cache` "fp8" gives the model an fp8 KV cache (LLaMA.kv_cache_dtype; not with a draft model)."""
+    `kv_cache` "fp8" gives the model an fp8 KV cache (LLaMA.kv_cache_dtype; not with a draft model).  `lookup_ngram`
+    N > 0 decodes each sample with `generate_speculative(draft=None, max_ngram=N)`: prompt lookup proposes up to
+    `num_draft` tokens per round from the sequence's own n-grams, no draft model."""
     if not 1 <= batch_size <= MAX_SAMPLES:
         raise ValueError(f"batch_size = {batch_size}; 1..{MAX_SAMPLES}")
     from sentencepiece import SentencePieceProcessor
@@ -688,7 +749,10 @@ def main(
         for i in range(num_samples):
             torch.cuda.synchronize()
             t0 = time.perf_counter()
-            if draft is None:
+            if lookup_ngram > 0:
+                y = generate_speculative(model, None, encoded, max_new_tokens, num_draft=num_draft, max_ngram=lookup_ngram,
+                                         temperature=temperature, top_k=top_k)
+            elif draft is None:
                 y = generate(model, encoded, max_new_tokens, temperature=temperature, top_k=top_k)
             else:
                 y = generate_speculative(model, draft, encoded, max_new_tokens, num_draft=num_draft,
@@ -747,11 +811,24 @@ def cli() -> None:
     ap.add_argument("--kv_cache", default=None, choices=[None, "fp8"],
                     help="fp8: e4m3 keys and values with a power-of-two scale per slot and head, half the KV cache's bytes "
                          "(default: bf16)")
+    ap.add_argument("--lookup_ngram", type=int, default=0,
+                    help=f"N in 1..{MAX_NGRAM}: speculative decoding without a draft model, --num_draft tokens per round "
+                         "proposed by prompt lookup (the continuation of the latest earlier match of the last N..1 "
+                         "tokens); 0: off")
     a = ap.parse_args()
     if a.kv_cache == "fp8" and a.draft_checkpoint_path is not None:
         ap.error("--kv_cache fp8 does not combine with --draft_checkpoint_path (the verify step keeps a bf16 cache)")
     if a.draft_checkpoint_path is not None and (a.batch_size != 1 or a.prompts_file is not None):
         ap.error("--draft_checkpoint_path decodes one sequence at a time (batch_size 1, no prompts_file)")
+    if a.lookup_ngram:
+        if not 1 <= a.lookup_ngram <= MAX_NGRAM:
+            ap.error(f"--lookup_ngram {a.lookup_ngram}: 1..{MAX_NGRAM}, or 0 (off)")
+        if a.draft_checkpoint_path is not None:
+            ap.error("--lookup_ngram does not combine with --draft_checkpoint_path (lookup replaces the draft model)")
+        if a.kv_cache == "fp8":
+            ap.error("--kv_cache fp8 does not combine with --lookup_ngram (the verify step keeps a bf16 cache)")
+        if a.batch_size != 1 or a.prompts_file is not None:
+            ap.error("--lookup_ngram decodes one sequence at a time (batch_size 1, no prompts_file)")
     if a.stream and a.prompts_file is None:
         ap.error("--stream decodes a --prompts_file")
     main(**vars(a))
