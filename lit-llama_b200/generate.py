@@ -55,26 +55,17 @@ def _rows(logits: torch.Tensor):
 
 def sample_probs(logits_row: torch.Tensor, temperature: float = 1.0, top_k: Optional[int] = None) -> torch.Tensor:
     """generate.py:68-75: probabilities of the next token from the last position's logits
-    (V,) bf16: temperature, top-k filter and softmax fused in one kernel (b2l_topk_softmax).
-    (B, V) logits give (B, V) probabilities, every row in the same launch (b2l_topk_softmax_rows), each row bit-equal
-    to the (V,) call on it."""
+    (V,) bf16: temperature, top-k filter and softmax fused in one kernel (b2l_topk_softmax_rows on one row).
+    (B, V) logits give (B, V) probabilities, every row in the same launch, each row bit-equal to the (V,) call on it."""
     L.require_cuda_bf16(logits_row, "sample_probs")
-    if logits_row.dim() == 2:
-        x, ld = _rows(logits_row)
-        B, V = logits_row.shape
-        probs = torch.empty((B, V), dtype=x.dtype, device=x.device)
-        k = 0 if top_k is None else min(int(top_k), V)
-        L.check(L.lib().b2l_topk_softmax_rows(x.data_ptr(), ld, float(temperature), k, probs.data_ptr(), B, V, L.stream_ptr()),
-                "b2l_topk_softmax_rows")
-        return probs
-    x = logits_row.contiguous()
-    if x.data_ptr() % 16:
-        x = x.clone()  # the kernel reads 16-byte vectors
-    V = x.numel()
-    probs = torch.empty_like(x)
+    rows = logits_row if logits_row.dim() == 2 else logits_row.reshape(1, -1)   # (V,): one row
+    x, ld = _rows(rows)
+    B, V = rows.shape
+    probs = torch.empty((B, V), dtype=x.dtype, device=x.device)
     k = 0 if top_k is None else min(int(top_k), V)
-    L.check(L.lib().b2l_topk_softmax(x.data_ptr(), float(temperature), k, probs.data_ptr(), V, L.stream_ptr()), "b2l_topk_softmax")
-    return probs
+    L.check(L.lib().b2l_topk_softmax_rows(x.data_ptr(), ld, float(temperature), k, probs.data_ptr(), B, V, L.stream_ptr()),
+            "b2l_topk_softmax_rows")
+    return probs if logits_row.dim() == 2 else probs.view(logits_row.shape)
 
 
 def sample_token(logits_row: torch.Tensor, temperature: float = 1.0, top_k: Optional[int] = None) -> torch.Tensor:
@@ -82,30 +73,28 @@ def sample_token(logits_row: torch.Tensor, temperature: float = 1.0, top_k: Opti
     `torch.multinomial(probs, num_samples=1)` is `argmax(probs / q)` with `q = empty_like(probs).exponential_(1)`
     (ATen/native/Distributions.cpp); q is drawn here with torch -- the RNG consumption of multinomial, so for the same
     generator state the token equals `torch.multinomial(sample_probs(...), 1)` -- and everything else is one
-    launch (b2l_topk_softmax_sample) instead of multinomial's dozen.
+    launch (b2l_topk_softmax_sample_rows) instead of multinomial's dozen.
     (B, V) logits give (B,) tokens: q is one [B, V] draw, as multinomial makes on [B, V] probabilities, so token b
-    equals `torch.multinomial(sample_probs(logits), 1)[b]`, and all rows are drawn in one launch
-    (b2l_topk_softmax_sample_rows)."""
+    equals `torch.multinomial(sample_probs(logits), 1)[b]`, and all rows are drawn in one launch."""
     L.require_cuda_bf16(logits_row, "sample_token")
-    if logits_row.dim() == 2:
-        x, ld = _rows(logits_row)
-        B, V = logits_row.shape
-        q = torch.empty((B, V), dtype=x.dtype, device=x.device).exponential_(1)
-        tokens = torch.empty(B, dtype=torch.int64, device=x.device)
-        k = 0 if top_k is None else min(int(top_k), V)
-        L.check(L.lib().b2l_topk_softmax_sample_rows(x.data_ptr(), ld, float(temperature), k, q.data_ptr(), None, tokens.data_ptr(),
-                                                     B, V, L.stream_ptr()), "b2l_topk_softmax_sample_rows")
-        return tokens
-    x = logits_row.contiguous()
-    if x.data_ptr() % 16:
-        x = x.clone()  # the kernel reads 16-byte vectors
-    V = x.numel()
-    q = torch.empty_like(x).exponential_(1)
-    token = torch.empty(1, dtype=torch.int64, device=x.device)
+    rows = logits_row if logits_row.dim() == 2 else logits_row.reshape(1, -1)   # (V,): one row
+    x, ld = _rows(rows)
+    B, V = rows.shape
+    q = torch.empty((B, V), dtype=x.dtype, device=x.device).exponential_(1)
+    tokens = torch.empty(B, dtype=torch.int64, device=x.device)
     k = 0 if top_k is None else min(int(top_k), V)
-    L.check(L.lib().b2l_topk_softmax_sample(x.data_ptr(), float(temperature), k, q.data_ptr(), None, token.data_ptr(), V, L.stream_ptr()),
-            "b2l_topk_softmax_sample")
-    return token
+    L.check(L.lib().b2l_topk_softmax_sample_rows(x.data_ptr(), ld, float(temperature), k, q.data_ptr(), None, tokens.data_ptr(),
+                                                 B, V, L.stream_ptr()), "b2l_topk_softmax_sample_rows")
+    return tokens
+
+
+def _draw(rows: torch.Tensor, temperature: float, top_k: Optional[int], dtype: torch.dtype) -> torch.Tensor:
+    """One token per row of `rows` ((V,) or (B, V) logits), as `dtype`: sample_token (one RNG draw and one launch for
+    all rows), or, while torch.multinomial is replaced (the reference's tests/test_generate.py:26-54 patches it to record
+    the draws), torch.multinomial on the fused probabilities."""
+    if torch.multinomial is _TORCH_MULTINOMIAL:
+        return sample_token(rows, temperature, top_k).to(dtype=dtype)
+    return torch.multinomial(sample_probs(rows, temperature, top_k), num_samples=1).view(-1).to(dtype=dtype)
 
 
 @torch.no_grad()
@@ -134,12 +123,7 @@ def generate(
     for _ in range(max_new_tokens):
         x = idx.index_select(0, input_pos).view(1, -1)
         logits = model(x, max_seq_length, input_pos)
-        if torch.multinomial is _TORCH_MULTINOMIAL:
-            idx_next = sample_token(logits[0, -1], temperature, top_k).to(dtype=dtype)  # generate.py:68-76: RNG draw + one launch
-        else:
-            # torch.multinomial has been replaced (the reference's tests/test_generate.py:26-54 patches it to record
-            # the draws): keep calling it, on the fused probabilities
-            idx_next = torch.multinomial(sample_probs(logits[0, -1], temperature, top_k), num_samples=1).to(dtype=dtype)
+        idx_next = _draw(logits[0, -1], temperature, top_k, dtype)   # generate.py:68-76
         input_pos = input_pos[-1:] + 1
         idx = idx.index_copy(0, input_pos, idx_next)
         if eos_id is not None and idx_next == eos_id:
@@ -199,11 +183,7 @@ def generate_batch(
             rows = logits[0, -1].expand(B, -1)   # every sample's first token comes from the prompt's last position
         else:
             rows = logits[:, -1]
-        if torch.multinomial is _TORCH_MULTINOMIAL:
-            idx_next = sample_token(rows, temperature, top_k).to(dtype=dtype)   # one RNG draw + one launch for all rows
-        else:
-            # torch.multinomial has been replaced (as in generate()): keep calling it, on the fused [B, V] probabilities
-            idx_next = torch.multinomial(sample_probs(rows, temperature, top_k), num_samples=1).view(B).to(dtype=dtype)
+        idx_next = _draw(rows, temperature, top_k, dtype)
         input_pos = input_pos[-1:] + 1
         out[:, T + i] = idx_next
         x = idx_next.view(B, 1)
@@ -338,6 +318,15 @@ def generate_speculative(
         w = int(w.to(torch.int32).item())
         return w & 255, (w >> 8) & 255 if eos_id is not None else 255, w >> 16
 
+    def plain_step() -> None:
+        """generate()'s target step: the pending token in, the next one drawn and emitted."""
+        nonlocal tok, n
+        p = T + n - 1
+        logits = model(tok.view(1, 1), S, pos_all[p:p + 1])
+        tok = sample_token(logits[0, -1], temperature, top_k)
+        out[T + n] = tok[0]
+        n += 1
+
     if draft is None:
         propose(T + 1, False)
         _, e, c = read(tok, none)
@@ -354,10 +343,7 @@ def generate_speculative(
         if draft is None:
             k = min(k, c)
             if k == 0:                      # no proposal: one plain target step, then the proposer again
-                logits = model(tok.view(1, 1), S, pos_all[p:p + 1])
-                tok = sample_token(logits[0, -1], temperature, top_k)
-                out[T + n] = tok[0]
-                n += 1
+                plain_step()
                 st["lookup_misses"] += 1
                 propose(T + n, False)
                 _, e, c = read(tok, none)
@@ -397,14 +383,9 @@ def generate_speculative(
         n += a + 1
 
     # the tail: generate()'s plain target steps (no draft token fits below max_seq_length, or one token is left)
-    input_pos = pos_all[T + n - 1:T + n]
     while n < max_new_tokens:
-        logits = model(tok.view(1, 1), S, input_pos)
-        tok = sample_token(logits[0, -1], temperature, top_k)
+        plain_step()
         st["tail_steps"] += 1
-        input_pos = input_pos + 1
-        out[T + n] = tok[0]
-        n += 1
         if eos_id is not None and tok == eos_id:
             return out[:T + n].to(dtype)
     return out.to(dtype)
@@ -423,64 +404,28 @@ def generate_prompts(
     adapters: Optional[Sequence[int]] = None,
 ) -> List[torch.Tensor]:
     """Continuations of 1..16 different prompts (1-D tensors of any lengths), decoded together: a list of 1-D tensors,
-    row b the prompt `prompts[b]` plus its new tokens (generate.py:20-91 per row).
+    row b the prompt `prompts[b]` plus its new tokens (generate.py:20-91 per row), each of `prompts[0]`'s dtype.
 
-    `LLaMA.prefill_rows` runs each prompt through the batch-1 prefill into its own row of one cache; the first tokens
-    are drawn from those last positions.  Each later token is one batched model call with a (B, 1) `input_pos`, row b
-    at position len(prompts[b]) + i with its own KV ring (each row takes the roll branch, model.py:214-218, on its own
-    once it passes max_seq_length), and one sampling launch for all rows.  max_seq_length defaults to
-    min(longest prompt + max_new_tokens, block_size).  Row b's token is `torch.multinomial(probs, 1)[b]` of the step's
-    [B, V] probabilities, so one prompt gives `generate()`'s tokens for the same seed.
+    `generate_stream` on B = len(prompts) rows, so no row is ever refilled: `LLaMA.prefill_rows` runs each prompt
+    through the batch-1 prefill into its own row of one cache; the first tokens are drawn from those last positions.
+    Each later token is one batched model call with a (B, 1) `input_pos`, row b at position len(prompts[b]) + i with
+    its own KV ring (each row takes the roll branch, model.py:214-218, on its own once it passes max_seq_length), and
+    one sampling launch for all rows.  max_seq_length defaults to min(longest prompt + max_new_tokens, block_size).
+    Row b's token is `torch.multinomial(probs, 1)[b]` of the step's [B, V] probabilities, so one prompt gives
+    `generate()`'s tokens for the same seed.
 
     With `eos_id`, a row that draws it ends there, the eos token included; finished rows keep riding along (their later
-    tokens are dropped) and the loop stops once every row has finished, reading one flag per step.  The cache is left
-    at B rows: call `model.reset_cache()` before a batch-1 `generate()`.
+    tokens are dropped) and the loop stops once every row has finished, reading the step's eos flags once per step.
+    The cache is left at B rows: call `model.reset_cache()` before a batch-1 `generate()`.
 
     `adapters` (multi-LoRA, lit_llama_b200.lora.add_lora_adapter): one adapter id per prompt (-1: the base alone);
     prompt b is prefilled and decoded with its own adapter (LLaMA.prefill_rows)."""
     B = len(prompts)
     if not 1 <= B <= MAX_SAMPLES:
         raise ValueError(f"generate_prompts: {B} prompts; 1..{MAX_SAMPLES} (the batched decode step's range)")
-    for p in prompts:
-        if p.dim() != 1:
-            raise ValueError(f"generate_prompts: every prompt must be one sequence of shape (T,), got {tuple(p.shape)}")
-    for p in prompts:
-        if not p.is_cuda:
-            raise RuntimeError(f"generate_prompts: a prompt is on {p.device}; lit_llama_b200 runs on CUDA only (no CPU fallback)")
-    Ts = [p.size(0) for p in prompts]
-    if max_seq_length is None:
-        max_seq_length = min(max(Ts) + max_new_tokens, model.config.block_size)
-    if max(Ts) > max_seq_length:
-        raise ValueError(f"generate_prompts: a prompt of {max(Ts)} tokens is longer than max_seq_length={max_seq_length}")
-
-    device, dtype = prompts[0].device, prompts[0].dtype
-    new = torch.empty((B, max_new_tokens), dtype=dtype, device=device)
-    input_pos = torch.tensor(Ts, dtype=torch.int64, device=device).view(B, 1)   # row b's first new token
-    end = torch.full((B,), max_new_tokens, dtype=torch.int64, device=device) if eos_id is not None else None
-    done = torch.zeros(B, dtype=torch.bool, device=device) if eos_id is not None else None
-
-    for i in range(max_new_tokens):
-        if i == 0:
-            rows = (model.prefill_rows(prompts, max_seq_length) if adapters is None
-                    else model.prefill_rows(prompts, max_seq_length, adapters))
-        else:
-            rows = model(x, max_seq_length, input_pos)[:, -1]
-            input_pos = input_pos + 1
-        if torch.multinomial is _TORCH_MULTINOMIAL:
-            idx_next = sample_token(rows, temperature, top_k).to(dtype=dtype)   # one RNG draw + one launch for all rows
-        else:
-            # torch.multinomial has been replaced (as in generate()): keep calling it, on the fused [B, V] probabilities
-            idx_next = torch.multinomial(sample_probs(rows, temperature, top_k), num_samples=1).view(B).to(dtype=dtype)
-        new[:, i] = idx_next
-        x = idx_next.view(B, 1)
-        if eos_id is not None:
-            hit = (idx_next == eos_id) & ~done
-            end = torch.where(hit, i + 1, end)   # include the eos token
-            done |= hit
-            if bool(done.all()):
-                break
-    ns = [max_new_tokens] * B if end is None else end.tolist()
-    return [torch.cat((p.to(dtype), new[b, :n])) for b, (p, n) in enumerate(zip(prompts, ns))]
+    ys = generate_stream(model, prompts, max_new_tokens, batch_size=B, max_seq_length=max_seq_length,
+                         temperature=temperature, top_k=top_k, eos_id=eos_id, adapters=adapters, _who="generate_prompts")
+    return [y.to(prompts[0].dtype) for y in ys]
 
 
 @torch.no_grad()
@@ -496,6 +441,7 @@ def generate_stream(
     eos_id: Optional[int] = None,
     stats: Optional[dict] = None,
     adapters: Optional[Sequence[int]] = None,
+    _who: str = "generate_stream",
 ) -> List[torch.Tensor]:
     """Continuations of any number of prompts (1-D tensors of any lengths) on B = min(batch_size, len(prompts)) rows
     (batch_size 1..16), refilling each finished row with the next prompt while the others keep decoding (continuous
@@ -514,8 +460,8 @@ def generate_stream(
     Draws are argmax(probs / q) of their row's probabilities (sample_token).  On the exact batched steps
     (`q4_batch_step`, `w8_batch_step`) every row is bit-identical to the batch-1 model, so with top_k=1 prompt i gets
     `generate(model, prompts[i], new_i, max_seq_length=S, top_k=1, eos_id=eos_id)` token for token, whichever row and
-    step admit it.  With len(prompts) <= batch_size and one `max_new_tokens` no row is refilled, and the output is
-    `generate_prompts`'s for the same seed.  `stats`, when given, receives "steps" (sampling launches), "refills"
+    step admit it.  With len(prompts) <= batch_size and one `max_new_tokens` no row is refilled: that is
+    `generate_prompts`.  `stats`, when given, receives "steps" (sampling launches), "refills"
     (prompts admitted after the first prefill), "packed" / "alone" (prompts prefilled in a packed pass / one at a time,
     LLaMA.refill_rows) and "idle_row_steps" (row-steps whose token was dropped).  The cache is left at B rows: call
     `model.reset_cache()` before a batch-1 `generate()`.
@@ -526,26 +472,26 @@ def generate_stream(
     carries only that adapter."""
     n = len(prompts)
     if n == 0:
-        raise ValueError("generate_stream: no prompts")
+        raise ValueError(f"{_who}: no prompts")
     if adapters is not None and len(adapters) != n:
-        raise ValueError(f"generate_stream: {len(adapters)} adapters for {n} prompts")
+        raise ValueError(f"{_who}: {len(adapters)} adapters for {n} prompts")
     if not 1 <= int(batch_size) <= MAX_SAMPLES:
-        raise ValueError(f"generate_stream: batch_size = {batch_size}; 1..{MAX_SAMPLES} (the batched decode step's range)")
+        raise ValueError(f"{_who}: batch_size = {batch_size}; 1..{MAX_SAMPLES} (the batched decode step's range)")
     for p in prompts:
         if p.dim() != 1 or p.numel() == 0:
-            raise ValueError(f"generate_stream: every prompt must be a non-empty sequence of shape (T,), got {tuple(p.shape)}")
+            raise ValueError(f"{_who}: every prompt must be a non-empty 1-D sequence of shape (T,), got {tuple(p.shape)}")
     for p in prompts:
         if not p.is_cuda:
-            raise RuntimeError(f"generate_stream: a prompt is on {p.device}; lit_llama_b200 runs on CUDA only (no CPU fallback)")
+            raise RuntimeError(f"{_who}: a prompt is on {p.device}; lit_llama_b200 runs on CUDA only (no CPU fallback)")
     news = [int(max_new_tokens)] * n if isinstance(max_new_tokens, int) else [int(m) for m in max_new_tokens]
     if len(news) != n or min(news) < 0:
-        raise ValueError(f"generate_stream: max_new_tokens must be one int >= 0, or one per prompt ({n}), got {max_new_tokens}")
+        raise ValueError(f"{_who}: max_new_tokens must be one int >= 0, or one per prompt ({n}), got {max_new_tokens}")
     Ts = [p.numel() for p in prompts]
     S = max_seq_length
     if S is None:
         S = min(max(T + m for T, m in zip(Ts, news)), model.config.block_size)
     if max(Ts) > S:
-        raise ValueError(f"generate_stream: a prompt of {max(Ts)} tokens is longer than max_seq_length={S}")
+        raise ValueError(f"{_who}: a prompt of {max(Ts)} tokens is longer than max_seq_length={S}")
     st = {} if stats is None else stats
     st.update(steps=0, refills=0, packed=0, alone=0, idle_row_steps=0)
     device, dtype = prompts[0].device, prompts[0].dtype
@@ -554,6 +500,8 @@ def generate_stream(
         return [p.clone() for p in prompts]
 
     def admit(ids: List[int]) -> None:
+        if stats is None:   # the pack plan walks every linear per prompt: host time spent only for the caller's stats
+            return
         k = len(model._pack_plan([Ts[i] for i in ids]))
         st["packed"] += k
         st["alone"] += len(ids) - k
@@ -585,11 +533,7 @@ def generate_stream(
                 input_pos[ridx] = torch.tensor([Ts[i] for i in ids], dtype=torch.int64, device=device).view(-1, 1)
                 st["refills"] += len(ids)
                 pending = []
-        if torch.multinomial is _TORCH_MULTINOMIAL:
-            idx_next = sample_token(rows, temperature, top_k).to(dtype=dtype)   # one RNG draw + one launch for all rows
-        else:
-            # torch.multinomial has been replaced (as in generate()): keep calling it, on the fused [B, V] probabilities
-            idx_next = torch.multinomial(sample_probs(rows, temperature, top_k), num_samples=1).view(B).to(dtype=dtype)
+        idx_next = _draw(rows, temperature, top_k, dtype)
         hist.append(idx_next)
         x = idx_next.view(B, 1)
         hits = (idx_next == eos_id).tolist() if eos_id is not None else None   # the step's one host read
@@ -695,7 +639,22 @@ def main(
 
     sp = SentencePieceProcessor(model_file=str(tokenizer_path))
     encoded = torch.tensor([sp.bos_id()] + sp.encode(prompt), dtype=torch.int, device=device)
-    prompt_length = encoded.size(0)
+
+    def timed(k: int, run, prompts: List[torch.Tensor]) -> None:
+        """Inference number k: run() (one output per prompt) between two synchronises, then the caches reset and the
+        outputs and the rate printed."""
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        ys = run()
+        torch.cuda.synchronize()
+        t = time.perf_counter() - t0
+        for m in (model, draft):
+            if m is not None:
+                m.reset_cache()
+        for y in ys:
+            print(sp.decode(y.tolist()))
+        tokens_generated = sum(y.size(0) - p.size(0) for y, p in zip(ys, prompts))
+        print(f"Time for inference {k}: {t:.02f} sec total, {tokens_generated / t:.02f} tokens/sec", file=sys.stderr)
 
     torch.manual_seed(1234)
     if batch_size > 1 or prompts_file is not None:
@@ -719,64 +678,32 @@ def main(
         for _ in range(num_samples):
             if stream:
                 k += 1
-                torch.cuda.synchronize()
-                t0 = time.perf_counter()
-                ys = generate_stream(model, prompts, max_new_tokens, batch_size=batch_size, temperature=temperature,
-                                     top_k=top_k, adapters=adapters)
-                torch.cuda.synchronize()
-                t = time.perf_counter() - t0
-                model.reset_cache()
-                for y in ys:
-                    print(sp.decode(y.tolist()))
-                tokens_generated = sum(y.size(0) - p.size(0) for y, p in zip(ys, prompts))
-                print(f"Time for inference {k}: {t:.02f} sec total, {tokens_generated / t:.02f} tokens/sec", file=sys.stderr)
+                timed(k, lambda: generate_stream(model, prompts, max_new_tokens, batch_size=batch_size,
+                                                 temperature=temperature, top_k=top_k, adapters=adapters), prompts)
                 continue
             for first in range(0, len(prompts), batch_size):
                 group = prompts[first:first + batch_size]
                 k += 1
-                torch.cuda.synchronize()
-                t0 = time.perf_counter()
-                ys = generate_prompts(model, group, max_new_tokens, temperature=temperature, top_k=top_k,
-                                      adapters=None if adapters is None else adapters[first:first + batch_size])
-                torch.cuda.synchronize()
-                t = time.perf_counter() - t0
-                model.reset_cache()
-                for y in ys:
-                    print(sp.decode(y.tolist()))
-                tokens_generated = sum(y.size(0) - p.size(0) for y, p in zip(ys, group))
-                print(f"Time for inference {k}: {t:.02f} sec total, {tokens_generated / t:.02f} tokens/sec", file=sys.stderr)
+                timed(k, lambda: generate_prompts(model, group, max_new_tokens, temperature=temperature, top_k=top_k,
+                                                  adapters=None if adapters is None else adapters[first:first + batch_size]),
+                      group)
     elif batch_size == 1:
-        for i in range(num_samples):
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
+        def one() -> torch.Tensor:
             if lookup_ngram > 0:
-                y = generate_speculative(model, None, encoded, max_new_tokens, num_draft=num_draft, max_ngram=lookup_ngram,
-                                         temperature=temperature, top_k=top_k)
-            elif draft is None:
-                y = generate(model, encoded, max_new_tokens, temperature=temperature, top_k=top_k)
-            else:
-                y = generate_speculative(model, draft, encoded, max_new_tokens, num_draft=num_draft,
-                                         temperature=temperature, top_k=top_k)
-                draft.reset_cache()
-            torch.cuda.synchronize()
-            t = time.perf_counter() - t0
-            model.reset_cache()
-            print(sp.decode(y.tolist()))
-            tokens_generated = y.size(0) - prompt_length
-            print(f"Time for inference {i + 1}: {t:.02f} sec total, {tokens_generated / t:.02f} tokens/sec", file=sys.stderr)
+                return generate_speculative(model, None, encoded, max_new_tokens, num_draft=num_draft,
+                                            max_ngram=lookup_ngram, temperature=temperature, top_k=top_k)
+            if draft is None:
+                return generate(model, encoded, max_new_tokens, temperature=temperature, top_k=top_k)
+            return generate_speculative(model, draft, encoded, max_new_tokens, num_draft=num_draft,
+                                        temperature=temperature, top_k=top_k)
+
+        for i in range(num_samples):
+            timed(i + 1, lambda: [one()], [encoded])
     else:
         for i, first in enumerate(range(0, num_samples, batch_size)):
             n = min(batch_size, num_samples - first)
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            ys = generate_batch(model, encoded, n, max_new_tokens, temperature=temperature, top_k=top_k)
-            torch.cuda.synchronize()
-            t = time.perf_counter() - t0
-            model.reset_cache()
-            for y in ys:
-                print(sp.decode(y.tolist()))
-            tokens_generated = sum(y.size(0) - prompt_length for y in ys)
-            print(f"Time for inference {i + 1}: {t:.02f} sec total, {tokens_generated / t:.02f} tokens/sec", file=sys.stderr)
+            timed(i + 1, lambda: generate_batch(model, encoded, n, max_new_tokens, temperature=temperature, top_k=top_k),
+                  [encoded] * n)
     print(f"Memory used: {torch.cuda.max_memory_reserved() / 1e9:.02f} GB", file=sys.stderr)
 
 

@@ -24,7 +24,8 @@ import ctypes as C
 import math
 import os
 from dataclasses import dataclass
-from typing import List, Optional, Tuple, Union
+from types import SimpleNamespace
+from typing import Callable, List, Optional, Tuple, Union
 
 import torch
 import torch.nn as nn
@@ -306,6 +307,29 @@ class Block(nn.Module):
         x = _add(x, h)
         x = _add(x, self.mlp(self.rms_2(x)))
         return x, new_kv_cache
+
+
+def _graph_step(st, graph_after: int, enqueue: Callable[[], None]) -> None:
+    """One call of a decode step whose state `st` holds `graph` and `calls`: replay st.graph if captured, else capture
+    `enqueue` on call graph_after + 1 (never with graph_after == 0) and replay it, else run `enqueue` eagerly."""
+    if st.graph is not None:
+        st.graph.replay()
+    elif graph_after and st.calls >= graph_after:
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            enqueue()
+        st.graph = g
+        g.replay()
+    else:
+        enqueue()
+    st.calls += 1
+
+
+class _ModuleGraph(SimpleNamespace):
+    """The module-by-module step's `_graph_step` state, key and static buffers; fields also read as items ("graph")."""
+
+    def __getitem__(self, name: str):
+        return getattr(self, name)
 
 
 class _DecodeState:
@@ -1144,17 +1168,7 @@ class LLaMA(nn.Module):
                 if r[0] == "segments":
                     raise RuntimeError("LLaMA.forward: a packed prefill's adapter segments do not decode")
                 st.lora_rows.copy_(r[2].expand(B) if r[0] == "one" else r[1][:B])
-            if st.graph is not None:
-                st.graph.replay()
-            elif self.graph_after and st.calls >= self.graph_after:
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g):
-                    st.enqueue()
-                st.graph = g
-                g.replay()
-            else:
-                st.enqueue()
-            st.calls += 1
+            _graph_step(st, self.graph_after, st.enqueue)
             return st.logits.clone() if self.copy_logits else st.logits
 
         # ---- single-token decode the fused step does not run (llm.int8, grouped or biased gptq, dense, gptq.int8 at
@@ -1164,23 +1178,17 @@ class LLaMA(nn.Module):
             key = (B, max_seq_length, idx.dtype, idx.device, WEIGHTS_GENERATION[0],
                    None if route is None else (route[0], route[-1].data_ptr() if route[0] != "segments" else None), rows)
             mg = self._module_graph
-            if mg is None or mg["key"] != key:
-                mg = self._module_graph = dict(key=key, calls=0, graph=None, idx=torch.zeros((B, 1), dtype=idx.dtype, device=idx.device),
-                                               pos=torch.zeros((B, 1) if rows else (1,), dtype=torch.int64, device=idx.device),
-                                               out=None)
-            mg["idx"].copy_(idx)
-            mg["pos"].copy_(input_pos if rows else input_pos.reshape(-1)[-1:])
-            if mg["graph"] is not None:
-                mg["graph"].replay()
-                return mg["out"].clone() if self.copy_logits else mg["out"]
-            mg["calls"] += 1
-            if mg["calls"] > self.graph_after:
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g):
-                    mg["out"] = self._forward_modules(mg["idx"], max_seq_length, mg["pos"])
-                mg["graph"] = g
-                g.replay()
-                return mg["out"].clone() if self.copy_logits else mg["out"]
+            if mg is None or mg.key != key:
+                mg = self._module_graph = _ModuleGraph(
+                    key=key, calls=0, graph=None, idx=torch.zeros((B, 1), dtype=idx.dtype, device=idx.device),
+                    pos=torch.zeros((B, 1) if rows else (1,), dtype=torch.int64, device=idx.device), out=None)
+            mg.idx.copy_(idx)
+            mg.pos.copy_(input_pos if rows else input_pos.reshape(-1)[-1:])
+            def enqueue() -> None:
+                mg.out = self._forward_modules(mg.idx, max_seq_length, mg.pos)
+            _graph_step(mg, self.graph_after, enqueue)
+            # the eager warm-up calls return a fresh tensor each; a graph's output is its static buffer
+            return mg.out.clone() if self.copy_logits and mg.graph is not None else mg.out
         return self._forward_modules(idx, max_seq_length, input_pos)
 
     @torch.no_grad()
@@ -1221,17 +1229,7 @@ class LLaMA(nn.Module):
             st = self._verify[T] = _DecodeState(self, T, max_seq_length, idx.device, idx.dtype, stepwise=True)
         st.idx.copy_(idx.reshape(-1))
         st.pos.copy_(input_pos)
-        if st.graph is not None:
-            st.graph.replay()
-        elif self.graph_after and st.calls >= self.graph_after:
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                st.enqueue()
-            st.graph = g
-            g.replay()
-        else:
-            st.enqueue()
-        st.calls += 1
+        _graph_step(st, self.graph_after, st.enqueue)
         out = st.logits.view(T, -1)
         return out.clone() if self.copy_logits else out
 

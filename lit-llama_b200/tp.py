@@ -31,7 +31,7 @@ import torch.distributed as dist
 import torch.nn as nn
 
 from . import _lib as L
-from .model import LLaMAConfig, RMSNorm, _add, build_rope_cache
+from .model import LLaMAConfig, RMSNorm, _add, _graph_step, build_rope_cache
 from .quantization import ColBlockQuantizedLinear
 
 
@@ -348,17 +348,7 @@ class TPLLaMA(nn.Module):
                 st = self._decode = _TPDecodeState(self, S, dev, idx.dtype)
             st.idx.copy_(idx.reshape(-1))
             st.pos.copy_(pos[-1:])
-            if st.graph is not None:
-                st.graph.replay()
-            elif self.graph_after and st.calls >= self.graph_after:
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g):
-                    st.enqueue()
-                st.graph = g
-                g.replay()
-            else:
-                st.enqueue()
-            st.calls += 1
+            _graph_step(st, self.graph_after, st.enqueue)
             return st.logits.reshape(1, 1, -1).clone()
         idx_c = idx.contiguous() if idx.dtype in (torch.int32, torch.int64) else idx.to(torch.int64).contiguous()
         x = torch.empty((B, T, C), device=dev, dtype=torch.bfloat16)
