@@ -138,22 +138,22 @@ enum {
   B2L_F_ATTN_UNFUSED = 8, /* debug: force the three-kernel attention path for T == 1   */
   B2L_F_DEBUG_NOCOMPUTE = 16, /* debug: b2l_q4_gemv streams the weights but skips the math */
   B2L_F_W8 = 32,        /* b2l_decode_step: every linear is gptq.int8, qw_mma from b2l_w8_tile_i8
-                           (b2l_w8_gemv); B == 1 (2..16 with B2L_F_W8_BATCH), no plan */
+                           (b2l_w8_gemv); B == 1 (2..16 with B2L_F_W8_BATCH)        */
   B2L_F_Q8 = 64,        /* b2l_decode_step: every linear is llm.int8 (b2l_decode_args::q8_layers / q8_lm_head,
-                           b2l_q8_linear); B == 1, no plan, not with B2L_F_W8          */
+                           b2l_q8_linear); B == 1, not with B2L_F_W8                   */
   B2L_F_W8_BATCH = 128, /* b2l_decode_step with B2L_F_W8 at B in 2..16: every linear runs b2l_w8_gemv_batch on
                            the b2l_w8_tile_i8 tilings in qw_mma; batch_work must hold
-                           b2l_w8_gemv_batch_workspace_bytes(max K, B) bytes; no plan, no affines */
+                           b2l_w8_gemv_batch_workspace_bytes(max K, B) bytes; no affines */
   B2L_F_Q4_BATCH_I8 = 256, /* b2l_decode_step (gptq.int4) at B in 2..16: every linear runs b2l_q4_gemv_batch_i8 on
                            the b2l_q4_tile_i8 tilings in qw_mma; batch_work must hold
                            b2l_w8_gemv_batch_workspace_bytes(max K, B) bytes; not with B2L_F_W8, B2L_F_Q8 or
-                           B2L_F_W8_BATCH; no plan, no affines */
+                           B2L_F_W8_BATCH; no affines */
   B2L_F_Q8_BATCH = 512, /* b2l_decode_step with B2L_F_Q8 at B in 2..16: every linear runs b2l_q8_linear_batch on
                            CB / SCB in place; batch_work must hold b2l_q8_linear_batch_workspace_bytes(max K, B)
-                           bytes; v2 affines allowed; not with B2L_F_W8, B2L_F_W8_BATCH or B2L_F_Q4_BATCH_I8; no plan */
+                           bytes; v2 affines allowed; not with B2L_F_W8, B2L_F_W8_BATCH or B2L_F_Q4_BATCH_I8 */
   B2L_F_ROW_POS = 1024, /* b2l_attention(_adapter) at T == 1 and b2l_decode_step: one position per row.
                            input_pos is int64[B] (row b's token is at input_pos[b]) and ring_start int32[B] (row b's
-                           own ring offset); not with B2L_F_ROPE_ROWS or a persistent plan.  The step advances each
+                           own ring offset); not with B2L_F_ROPE_ROWS.  The step advances each
                            row's ring on its own (b2l_ring_advance_rows) */
   B2L_F_STEPWISE = 2048, /* b2l_attention(_adapter) at B == 1, T = 2..16, and b2l_decode_step with B = 2..16: the rows
                            are consecutive tokens of ONE sequence (the verify step of speculative decoding), each
@@ -165,7 +165,7 @@ enum {
                            is rows 0..7 of its every 16-row block (c_fc1 of the fc1|fc2 tiling); N % 8 == 0 */
   B2L_F_GEMM_I8_HI = 16384, /* the same, rows 8..15 of every 16-row block (c_fc2) */
   B2L_F_KV_FP8 = 1 << 15    /* b2l_decode_step: every layer's KV cache is fp8 (b2l_decode_args::kv8, b2l_attention_kv8);
-                               on every route, not with `plan`, B2L_F_STEPWISE or B2L_F_ATTN_UNFUSED; head_size 128 */
+                               on every route, not with B2L_F_STEPWISE or B2L_F_ATTN_UNFUSED; head_size 128 */
 };
 
 /* Fused [RMSNorm ->] int4 linear [-> residual | SwiGLU] on wgmma (M <= 16).  Replaces
@@ -754,8 +754,7 @@ typedef struct b2l_decode_args {
   void* logits;              /* bf16 [B, vocab]                                       */
   int flags;                 /* B2L_F_*                                               */
   void* timeline;            /* debug: device uint64[(5*n_layer+1)*64] of %globaltimer stamps per
-                                launch (NULL = off); tools/diag.py `timeline`.  With `plan`: uint64
-                                [(5*n_layer+1)*16] per-op stamps of the persistent kernel   */
+                                launch (NULL = off); tools/diag.py `timeline`               */
   void* batch_work;          /* B in 2..8: scratch of b2l_q4_gemv_batch_workspace_bytes(max K) bytes; the
                                 linears then run on the mma.sync batch kernel (weights need qw_mma).
                                 NULL: wgmma kernel (weights need qw_tiled).
@@ -763,21 +762,15 @@ typedef struct b2l_decode_args {
                                 b2l_w8_gemv_batch_workspace_bytes(max K, B) bytes (required).
                                 B2L_F_Q8 | B2L_F_Q8_BATCH: b2l_q8_linear_batch_workspace_bytes(max K, B) bytes
                                 (required) */
-  void* plan;                /* B == 1, head_size 128: device buffer of b2l_decode_plan_bytes() bytes prepared by
-                                b2l_decode_plan_build -> the whole step runs as ONE persistent kernel
-                                (csrc/decode_mega.cu; weights need the b2l_q4_tile_i8 layout in qw_mma).
-                                NULL: one kernel per op                                   */
   const b2l_adapter_prefix* adapters; /* HOST array [n_layer] of LLaMA-Adapter prefixes (b2l_attention_adapter);
-                                NULL = no adapter anywhere, an entry with len == 0 = none in that layer.
-                                Not with `plan`.                                          */
+                                NULL = no adapter anywhere, an entry with len == 0 = none in that layer. */
   const b2l_lora* loras;     /* HOST array [n_layer] of c_attn LoRA terms (lora.py:405-446; b2l_lora_apply with
                                 rms_1 as the norm, enqueued between c_attn and the attention, without timeline
-                                stamps).  NULL = no LoRA anywhere, an entry with r == 0 = none in that layer.
-                                Not with `plan`.                                          */
+                                stamps).  NULL = no LoRA anywhere, an entry with r == 0 = none in that layer. */
   const b2l_layer_affine* affines; /* HOST array [n_layer] of LLaMA-Adapter v2 affines, applied inside each linear's
                                 launch (b2l_q4_linear_args::out_affine), so the launch count does not change.
                                 NULL = none.  Only at B == 1 on the batch-1 kernels (every weight needs qw_mma);
-                                not with `plan` or `loras`.                               */
+                                not with `loras`.                                         */
   b2l_out_affine lm_head_affine; /* the same for lm_head (both NULL = none)                 */
   const b2l_q8_layer* q8_layers; /* B2L_F_Q8: HOST array [n_layer] of llm.int8 weights; the b2l_q4_weight members of
                                 layers[] and lm_head are then unused (layers[] still supplies the norms and the
@@ -790,7 +783,7 @@ typedef struct b2l_decode_args {
   const b2l_lora* lora_sets; /* Multi-LoRA: HOST [n_lora_sets][n_layer] c_attn terms; r == 0 = that set has no
                                 term in that layer.  Each layer where some set has a term runs
                                 b2l_lora_apply_rows (rms_1 as the norm) where `loras` would run b2l_lora_apply:
-                                row b adds set lora_row_set[b]'s term.  NULL = off.  Not with `loras`, `plan`,
+                                row b adds set lora_row_set[b]'s term.  NULL = off.  Not with `loras`,
                                 `affines` / `lm_head_affine` or B2L_F_STEPWISE (B2L_E_UNSUPPORTED). */
   int n_lora_sets;           /* 1..B2L_LORA_MAX_SETS                                      */
   const int32_t* lora_row_set; /* device int32 [B]: row b's set, -1 = none (read by the kernels only) */
@@ -808,16 +801,9 @@ typedef struct b2l_decode_args {
  * p..p+B-1 (all < S), layers[].k_cache / v_cache the batch-1 caches [1, nh, S, hs], attn_work
  * b2l_attn_workspace_bytes(B, nh, hs, 1, S) bytes.  Row t's logits equal the batch-1 step's at position p+t on the cache
  * holding the tokens before it, bit for bit, and the cache ends as B batch-1 steps leave it.  Only with the row-exact
- * linears: B2L_F_Q4_BATCH_I8, or B2L_F_W8 | B2L_F_W8_BATCH; not with B2L_F_Q8, B2L_F_ROW_POS, `plan` or `affines`.
+ * linears: B2L_F_Q4_BATCH_I8, or B2L_F_W8 | B2L_F_W8_BATCH; not with B2L_F_Q8, B2L_F_ROW_POS or `affines`.
  * Adapters and LoRA run as in the batched step; each layer's attention is one launch more (b2l_attention). */
 int b2l_decode_step(const b2l_decode_args* args, b2l_stream_t stream);
-/* The persistent decode kernel's static op list + arrival counters.  b2l_decode_plan_build fills args->plan from
- * the pointers in args (call it once, outside graph capture; rebuild when any pointer in args changes);
- * b2l_decode_plan_status synchronises the stream and returns B2L_E_STATE if a bounded wait inside the kernel
- * ever timed out (the kernel never hangs: it sets a sticky error word and falls through). */
-size_t b2l_decode_plan_bytes(const b2l_decode_args* args);
-int b2l_decode_plan_build(const b2l_decode_args* args, b2l_stream_t stream);
-int b2l_decode_plan_status(const void* plan, b2l_stream_t stream);
 /* Number of kernels one b2l_decode_step enqueues (for bench.py's gpu_launches). */
 int b2l_decode_step_launches(const b2l_decode_args* args);
 

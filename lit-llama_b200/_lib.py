@@ -127,7 +127,7 @@ class DecodeArgs(C.Structure):
         ("input_pos", c_void_p), ("ring_start", c_void_p), ("block_size", c_int),
         ("x", c_void_p), ("qkv", c_void_p), ("att", c_void_p), ("hid", c_void_p), ("attn_work", c_void_p),
         ("logits", c_void_p), ("flags", c_int), ("timeline", c_void_p), ("batch_work", c_void_p),
-        ("plan", c_void_p), ("adapters", C.POINTER(AdapterPrefix)), ("loras", C.POINTER(LoRA)),
+        ("adapters", C.POINTER(AdapterPrefix)), ("loras", C.POINTER(LoRA)),
         ("affines", C.POINTER(LayerAffine)), ("lm_head_affine", OutAffine),
         ("q8_layers", C.POINTER(Q8Layer)), ("q8_lm_head", Q8Weight), ("q8_threshold", c_float),
         ("lora_sets", C.POINTER(LoRA)), ("n_lora_sets", c_int), ("lora_row_set", c_void_p),
@@ -230,9 +230,6 @@ _SIGS = {
     "b2l_kv8_unroll_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "b2l_decode_step": (c_int, [C.POINTER(DecodeArgs), c_void_p]),
     "b2l_decode_step_launches": (c_int, [C.POINTER(DecodeArgs)]),
-    "b2l_decode_plan_bytes": (c_size_t, [C.POINTER(DecodeArgs)]),
-    "b2l_decode_plan_build": (c_int, [C.POINTER(DecodeArgs), c_void_p]),
-    "b2l_decode_plan_status": (c_int, [c_void_p, c_void_p]),
 }
 
 EXPORTS = tuple(_SIGS)

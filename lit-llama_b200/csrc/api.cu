@@ -5,7 +5,6 @@
 
 namespace b2l {
 
-int decode_step_persistent(const b2l_decode_args* d, b2l_stream_t stream);   // decode_mega.cu
 int check_adapter_prefix(const b2l_adapter_prefix* pre, const char* who);     // attention.cu
 int check_attention(const void* qkv, const void* k_cache, const void* v_cache, const void* rope, const int64_t* input_pos,
                     const int32_t* ring_start, const void* y, const void* work, int B, int T, int n_head, int head_size,
@@ -90,8 +89,7 @@ extern "C" int b2l_device_info(int* sm, int* cc_major, int* cc_minor) {
 
 // Every linear of one step runs on one route: a kernel and the tiling it reads.  resolve_route picks it from the flags,
 // B, batch_work and lm_head's tiling; the step's checks, its dispatch (linear) and b2l_decode_step_launches read it
-// from this table.  LoRA, adapters, B2L_F_ROW_POS and B2L_F_KV_FP8 run on every route.  The persistent kernel (plan) takes over the
-// whole step in place of the gptq.int4 routes, runs none of those, and checks its own shape (decode_mega.cu).
+// from this table.  LoRA, adapters, B2L_F_ROW_POS and B2L_F_KV_FP8 run on every route.
 enum RouteId { Q4_GEMV, Q4_BATCH, Q4_TC, Q4_BATCH_I8, W8_GEMV, W8_BATCH, Q8, Q8_BATCH };
 enum Tiling { MMA, TILED, CB };   // b2l_q4_weight::qw_mma, b2l_q4_weight::qw_tiled, llm.int8's CB / SCB
 struct Route {
@@ -264,7 +262,6 @@ static int in_step(int rc, const b2l_decode_args* d, const Linear& li) {
 
 extern "C" int b2l_decode_step_launches(const b2l_decode_args* d) {
   if (!d) return 0;
-  if (d->plan != nullptr) return 1;   // the persistent kernel
   RouteId r;
   if (resolve_route(d, &r) != 0) return 0;
   // fused single-token attention for head_size 128 (B2L_F_ATTN_UNFUSED: the three-kernel path)
@@ -301,7 +298,6 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
   RouteId r;
   if (int rc = resolve_route(d, &r)) return rc;
   const Route& R = kRoutes[r];
-  const bool plan = d->plan != nullptr;
   const bool any_affine = d->affines != nullptr || d->lm_head_affine.scale != nullptr || d->lm_head_affine.bias != nullptr;
   const bool row_pos = (d->flags & B2L_F_ROW_POS) != 0;   // input_pos / ring_start hold one entry per row
   // B2L_F_STEPWISE: the B rows are consecutive tokens of ONE sequence (input_pos int64[B], batch-1 caches); every row
@@ -314,13 +310,11 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
     B2L_CHECK_SUPPORTED(R.stepwise,
                         "b2l_decode_step: B2L_F_STEPWISE needs the row-exact linears (B2L_F_Q4_BATCH_I8, or B2L_F_W8 | B2L_F_W8_BATCH)");
     B2L_CHECK_SUPPORTED(d->B >= 2 && d->B <= 16, "b2l_decode_step: B2L_F_STEPWISE runs 2..16 tokens, got B=%d", d->B);
-    B2L_CHECK_SUPPORTED(!plan, "b2l_decode_step: B2L_F_STEPWISE does not run in the persistent kernel (plan must be NULL)");
     B2L_CHECK_SUPPORTED(!any_affine, "b2l_decode_step: B2L_F_STEPWISE does not apply LLaMA-Adapter v2 affines");
   }
   // B2L_F_KV_FP8: every layer's attention on its fp8 cache (kv8), whatever route the linears take
   const bool kv8 = (d->flags & B2L_F_KV_FP8) != 0;
   if (kv8) {
-    B2L_CHECK_SUPPORTED(!plan, "b2l_decode_step: B2L_F_KV_FP8 does not run in the persistent kernel (plan must be NULL)");
     B2L_CHECK_SUPPORTED(!stepwise, "b2l_decode_step: B2L_F_KV_FP8 does not run B2L_F_STEPWISE (speculative verify)");
     B2L_CHECK_SUPPORTED(!(d->flags & B2L_F_ATTN_UNFUSED),
                         "b2l_decode_step: B2L_F_KV_FP8 runs the fused decode kernel only (not B2L_F_ATTN_UNFUSED)");
@@ -328,15 +322,13 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
                         "b2l_decode_step: B2L_F_KV_FP8 runs head_size 128 only (every LLaMA size), got %d", d->n_embd / d->n_head);
     B2L_CHECK_ARG(d->kv8 != nullptr, "b2l_decode_step: B2L_F_KV_FP8 needs kv8 (one b2l_kv8_cache per layer)");
   }
-  B2L_CHECK_SUPPORTED(!row_pos || !plan, "b2l_decode_step: B2L_F_ROW_POS does not run in the persistent kernel (plan must be NULL)");
   B2L_CHECK_SUPPORTED(!row_pos || !(d->flags & B2L_F_ROPE_ROWS), "b2l_decode_step: B2L_F_ROW_POS does not combine with B2L_F_ROPE_ROWS");
-  if (R.flag != nullptr) {   // a route a flag selects: its batch range, no persistent kernel, and its workspace
+  if (R.flag != nullptr) {   // a route a flag selects: its batch range and its workspace
     if (R.b_min == R.b_max)
       B2L_CHECK_SUPPORTED(d->B == R.b_min, "b2l_decode_step: %s runs batch 1 only, got B=%d", R.flag, d->B);
     else
       B2L_CHECK_SUPPORTED(d->B >= R.b_min && d->B <= R.b_max, "b2l_decode_step: %s runs batches of %d..%d, got B=%d",
                           R.flag, R.b_min, R.b_max, d->B);
-    B2L_CHECK_SUPPORTED(!plan, "b2l_decode_step: %s does not run in the persistent kernel (plan must be NULL)", R.flag);
     B2L_CHECK_SUPPORTED(R.affines || !any_affine, "b2l_decode_step: %s does not apply LLaMA-Adapter v2 affines (batch 1 only)",
                         R.flag);
     B2L_CHECK_ARG(!R.batch_work || d->batch_work != nullptr, "b2l_decode_step: %s needs batch_work (%s(max K, B) bytes)",
@@ -346,20 +338,17 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
   if (d->adapters != nullptr) {
     for (int l = 0; l < d->n_layer; ++l) {
       if (d->adapters[l].len == 0) continue;   // no adapter in this layer
-      B2L_CHECK_SUPPORTED(!plan, "b2l_decode_step: adapters do not run in the persistent kernel (plan must be NULL)");
       if (int rc = check_adapter_prefix(&d->adapters[l], "b2l_decode_step")) return rc;
     }
   }
   if (d->loras != nullptr) {
     for (int l = 0; l < d->n_layer; ++l) {
       if (d->loras[l].r == 0) continue;   // no LoRA in this layer
-      B2L_CHECK_SUPPORTED(!plan, "b2l_decode_step: LoRA layers do not run in the persistent kernel (plan must be NULL)");
       if (int rc = check_lora(&d->loras[l], 3 * d->n_embd, d->n_embd, "b2l_decode_step")) return rc;
     }
   }
   if (d->lora_sets != nullptr) {   // per-row LoRA: every layer's sets checked here, before any launch
     B2L_CHECK_SUPPORTED(d->loras == nullptr, "b2l_decode_step: lora_sets and loras do not combine");
-    B2L_CHECK_SUPPORTED(!plan, "b2l_decode_step: lora_sets do not run in the persistent kernel (plan must be NULL)");
     B2L_CHECK_SUPPORTED(!any_affine, "b2l_decode_step: lora_sets and LLaMA-Adapter v2 affines do not combine");
     B2L_CHECK_SUPPORTED(!stepwise, "b2l_decode_step: lora_sets do not run under B2L_F_STEPWISE (one sequence, one adapter: use loras)");
     B2L_CHECK_ARG(d->lora_row_set != nullptr, "b2l_decode_step: lora_sets need lora_row_set");
@@ -374,7 +363,6 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
   // LLaMA-Adapter v2: every linear's affine runs in its own launch (b2l_q4_linear_args::out_affine)
   if (any_affine) {
     B2L_CHECK_SUPPORTED(R.affines || d->B == 1, "b2l_decode_step: LLaMA-Adapter v2 affines run at batch 1 only, got B=%d", d->B);
-    B2L_CHECK_SUPPORTED(!plan, "b2l_decode_step: LLaMA-Adapter v2 affines do not run in the persistent kernel (plan must be NULL)");
     B2L_CHECK_SUPPORTED(d->loras == nullptr, "b2l_decode_step: LLaMA-Adapter v2 affines and LoRA do not combine");
     auto ok = [](const b2l_out_affine& f) { return (f.scale == nullptr) == (f.bias == nullptr); };
     B2L_CHECK_ARG(ok(d->lm_head_affine), "b2l_decode_step: lm_head_affine needs both scale and bias (or neither)");
@@ -388,7 +376,6 @@ extern "C" int b2l_decode_step(const b2l_decode_args* d, b2l_stream_t stream) {
                           "b2l_decode_step: affines need the batch-1 tiling (qw_mma) of every weight");
     }
   }
-  if (plan) return decode_step_persistent(d, stream);   // one persistent kernel per token (decode_mega.cu)
   const int C = d->n_embd, hs = C / d->n_head, B = d->B;
   const int afl = d->flags & ~(B2L_F_W8 | B2L_F_Q8 | B2L_F_W8_BATCH | B2L_F_Q4_BATCH_I8 | B2L_F_Q8_BATCH);   // the attention's
   // the attention's view: B sequences of one token, or (stepwise) one sequence of B tokens

@@ -467,29 +467,11 @@ class _DecodeState:
         if affines is not None:    # LLaMA-Adapter v2 (B == 1, llm.int8 at any B): every linear's launch applies them
             self.args.affines = C.cast(affines[0], C.POINTER(L.LayerAffine))
             self.args.lm_head_affine = affines[1]
-        # batch 1, head_size 128: the whole step as ONE persistent kernel (csrc/decode_mega.cu; int4 weights only, so
-        # gptq.int8 keeps one kernel per op under B2L_PERSISTENT=1 too, and so do adapter, LoRA and adapter-v2 models)
-        self.plan = None
-        kmax = max(C_, n_hidden)
-        if (model.persistent and not w8 and not q8 and adapters is None and loras is None and sets is None and affines is None
-                and B == 1 and hs == 128
-                and kmax <= 12288):
-            if kv8:
-                raise RuntimeError("LLaMA: the persistent decode kernel (B2L_PERSISTENT=1) does not read an fp8 KV cache "
-                                   "(kv_cache_dtype='fp8'); turn one of them off")
-            self.plan = torch.zeros(lib.b2l_decode_plan_bytes(C.byref(self.args)), dtype=torch.uint8, device=device)
-            self.args.plan = self.plan.data_ptr()
-            L.check(lib.b2l_decode_plan_build(C.byref(self.args), L.stream_ptr()), "b2l_decode_plan_build")
         self.graph: Optional[torch.cuda.CUDAGraph] = None
         self.calls = 0
 
     def enqueue(self) -> None:
         L.check(L.lib().b2l_decode_step(C.byref(self.args), L.stream_ptr()), "b2l_decode_step")
-
-    def check(self) -> None:
-        """Synchronises and raises if a bounded wait inside the persistent kernel ever timed out."""
-        if self.plan is not None:
-            L.check(L.lib().b2l_decode_plan_status(self.plan.data_ptr(), L.stream_ptr()), "b2l_decode_plan_status")
 
 
 class LLaMA(nn.Module):
@@ -501,9 +483,6 @@ class LLaMA(nn.Module):
     decode_flags: int = 1
     #: return a fresh logits tensor per call like the reference (False: a view of the static buffer)
     copy_logits: bool = True
-    #: batch-1 decode (head_size 128) as ONE persistent kernel per token (csrc/decode_mega.cu) instead of one kernel
-    #: per op.  Opt-in (B2L_PERSISTENT=1): the default is the per-op path under programmatic dependent launch.
-    persistent: bool = os.environ.get("B2L_PERSISTENT", "0") == "1"
     #: decode of an llm.int8 model (plain, LLaMA-Adapter v1 / v2 or LoRA) at batch 1..16 on the whole-token step
     #: (b2l_decode_step under B2L_F_Q8: b2l_q8_linear with RMSNorm / residual / SwiGLU / affine fused at batch 1, and
     #: with B2L_F_Q8_BATCH b2l_q8_linear_batch at 2..16), bit-identical to the module path.  Opt-in (B2L_INT8_STEP=1):
@@ -562,8 +541,7 @@ class LLaMA(nn.Module):
         row, head and slot, include/b2l.h: half the bytes per cached token).  Read when the cache is allocated; it cannot
         change while a cache exists (reset_cache() first).  Under "fp8", kv_caches holds FP8KVCache entries, every
         attention reads and appends codes (b2l_attention_kv8, the decode step's B2L_F_KV_FP8), a prefill starts at
-        position 0, and refill_rows prefills one prompt at a time; decode_tokens (speculative verify) and the persistent
-        kernel refuse it."""
+        position 0, and refill_rows prefills one prompt at a time; decode_tokens (speculative verify) refuses it."""
         return self._kv_cache_dtype
 
     @kv_cache_dtype.setter

@@ -177,12 +177,12 @@ def test_adapter_struct_layout_matches_c_compiler(L, tmp_path):
         '#include <stdio.h>\n#include <stddef.h>\n#include "b2l.h"\n'
         "int main(void){\n"
         'printf("%zu %zu %zu %zu %zu\\n", sizeof(b2l_adapter_prefix), offsetof(b2l_adapter_prefix, len), '
-        "sizeof(b2l_decode_args), offsetof(b2l_decode_args, plan), offsetof(b2l_decode_args, adapters));\n"
+        "sizeof(b2l_decode_args), offsetof(b2l_decode_args, batch_work), offsetof(b2l_decode_args, adapters));\n"
         "return 0;}\n")
     exe = tmp_path / "layout"
     subprocess.run(["gcc", "-I", os.path.join(ROOT, "include"), str(prog), "-o", str(exe)], check=True)
     out = subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.split()
-    got = [C.sizeof(L.AdapterPrefix), L.AdapterPrefix.len.offset, C.sizeof(L.DecodeArgs), L.DecodeArgs.plan.offset,
+    got = [C.sizeof(L.AdapterPrefix), L.AdapterPrefix.len.offset, C.sizeof(L.DecodeArgs), L.DecodeArgs.batch_work.offset,
            L.DecodeArgs.adapters.offset]
     assert [int(v) for v in out] == got
 
@@ -221,8 +221,3 @@ def test_decode_step_launch_count_and_refusals(L):
     assert lib.b2l_decode_step(C.byref(d), None) == -2 and b"prefix length" in lib.b2l_last_error()
     d, keep = _decode_args(L, 4, 4, 512, [none, none, pre, L.AdapterPrefix(256, None, 256, 10)])
     assert lib.b2l_decode_step(C.byref(d), None) == -1 and b"null adapter prefix" in lib.b2l_last_error()
-    # the persistent kernel does not run adapters: the step and the plan builder refuse them
-    d, keep = _decode_args(L, 4, 4, 512, [none, none, pre, pre])
-    d.plan = 4096
-    assert lib.b2l_decode_step(C.byref(d), None) == -2 and b"persistent kernel" in lib.b2l_last_error()
-    assert lib.b2l_decode_plan_build(C.byref(d), None) == -2 and b"persistent kernel" in lib.b2l_last_error()

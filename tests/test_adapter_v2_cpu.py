@@ -288,11 +288,6 @@ def test_decode_step_launch_count_and_refusals(L):
     d, keep = _decode_args(L, 4, 4, 512, None, B=2)   # lm_head's affine alone counts too
     d.lm_head_affine = f
     assert lib.b2l_decode_step(C.byref(d), None) == -2 and b"batch 1" in lib.b2l_last_error()
-    # not with the persistent kernel: the step and the plan builder refuse it
-    d, keep = _decode_args(L, 4, 4, 512, [lay] * 4)
-    d.plan = 4096
-    assert lib.b2l_decode_step(C.byref(d), None) == -2 and b"persistent kernel" in lib.b2l_last_error()
-    assert lib.b2l_decode_plan_build(C.byref(d), None) == -2 and b"persistent kernel" in lib.b2l_last_error()
     # not with LoRA
     d, keep = _decode_args(L, 4, 4, 512, [lay] * 4)
     loras = (L.LoRA * 4)()

@@ -184,7 +184,7 @@ def test_adapter_model_vs_oracle_and_exactness(dev, mode, fused):
 
 def test_adapter_reload_after_graph_and_compact(dev):
     """Loading new adapter weights after the decode graph was captured takes effect at the next step; compact()
-    changes no output; B2L_PERSISTENT builds no plan for an adapter model."""
+    changes no output."""
     model, oracle, _ = build(dev, CFG128, "gptq.int4")
     model.graph_after = 2
     run_steps(model, dev, PROMPT, 32, TOKS)
@@ -227,7 +227,3 @@ def test_adapter_reload_after_graph_and_compact(dev):
     with torch.no_grad():   # and a base-model reload after that still brings the reference buffers back
         cm.load_state_dict({k: v for k, v in sd2.items() if "adapter" not in k and "gating" not in k}, strict=False)
     assert not cm.transformer.h[0].attn.c_attn._released
-    pm, _, _ = build(dev, CFG128, "gptq.int4")
-    pm.persistent = True
-    run_steps(pm, dev, PROMPT, 32, TOKS[:2])
-    assert pm._decode is not None and pm._decode.plan is None

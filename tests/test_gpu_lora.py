@@ -265,7 +265,7 @@ def test_lora_model_paths_vs_oracle_and_zero_b(dev, mode, B, fused):
 
 def test_lora_reload_after_graph_and_compact(dev):
     """Loading new LoRA weights after the decode graph was captured takes effect at the next step; compact() changes
-    no output and no state_dict entry; B2L_PERSISTENT builds no plan for a LoRA model."""
+    no output and no state_dict entry."""
     model, oracle, _ = build(dev, "gptq.int4")
     model.graph_after = 2
     run(model, dev)
@@ -303,10 +303,6 @@ def test_lora_reload_after_graph_and_compact(dev):
     with torch.no_grad():
         got_c = cm(torch.tensor([[88]], device=dev), 32, torch.tensor([7 + len(TOKS)], device=dev))
     assert torch.equal(got_c, got)
-    pm, _, _ = build(dev, "gptq.int4")
-    pm.persistent = True
-    run(pm, dev, toks=TOKS[:2])
-    assert pm._decode is not None and pm._decode.plan is None
 
 
 def test_dense_lora_through_patch_reference_matches_reference(dev):

@@ -1,5 +1,6 @@
 """-m gpu: model.py pieces, the whole tiny model, generate() and the 7B-shaped Block
-against the oracle and the golden vectors produced by the unmodified reference."""
+against the oracle and the golden vectors produced by the unmodified reference; the head_size-128 decode step at
+deep positions and in the roll branch; PDL against plain stream order; tensor parallelism on 2 GPUs."""
 import pytest
 import torch
 
@@ -286,6 +287,121 @@ def test_13b_width_batch8_prefill_and_decode_vs_oracle(dev):
             torch.testing.assert_close(g_, w_, rtol=2 ** -5, atol=8e-2)
 
 
+# head_size 128, K = 256 / 768: every linear a multiple of 64 wide, and small enough for the oracle at deep positions
+CFG128 = dict(block_size=512, vocab_size=320, n_layer=3, n_head=2, n_embd=256)
+
+
+def _normwise(a, b):
+    a, b = a.float().cpu().flatten(), b.float().cpu().flatten()
+    return float((a - b).norm() / b.norm())
+
+
+def _decode(model, oracle, dev, prompt, S, steps, seed=0):
+    """Prefill `prompt`, then `steps` single-token steps; returns ([model logits], [oracle logits])."""
+    g = torch.Generator().manual_seed(seed)
+    T = prompt.shape[1]
+    got, want = [], []
+    with torch.no_grad():
+        got.append(model(prompt.to(dev), S, torch.arange(T, device=dev))[:, -1])
+        if oracle is not None:
+            want.append(oracle.forward(prompt, S, torch.arange(T))[:, -1])
+        for i in range(steps):
+            t = int(torch.randint(0, CFG128["vocab_size"], (1,), generator=g))
+            got.append(model(torch.tensor([[t]], device=dev), S, torch.tensor([T + i], device=dev))[:, -1])
+            if oracle is not None:
+                want.append(oracle.forward(torch.tensor([[t]]), S, torch.tensor([T + i]))[:, -1])
+    return got, want
+
+
+def test_decode_step_hs128_vs_oracle(dev):
+    """The batch-1 decode step at head_size 128, replayed as a CUDA graph, against the exact-arithmetic oracle: every
+    step's logits and the KV rows."""
+    from gpu_util import build_tiny
+
+    model, oracle, _ = build_tiny(dev, CFG128, seed=3, exact_linears=True)
+    prompt = torch.tensor([[3, 17, 40, 41, 2, 77]])
+    got, want = _decode(model, oracle, dev, prompt, 64, 8)
+    st = model._decode
+    assert st is not None and st.graph is not None   # the whole-token step, replayed as a graph
+    for a, b in zip(got, want):
+        assert _normwise(a, b) < 1e-2, _normwise(a, b)
+    k, v = model.kv_caches[1]
+    torch.testing.assert_close(k[:, :, :14].float().cpu(), oracle.kv[1][0][:, :, :14].float(), rtol=2 ** -6, atol=2e-2)
+    torch.testing.assert_close(v[:, :, :14].float().cpu(), oracle.kv[1][1][:, :, :14].float(), rtol=2 ** -6, atol=2e-2)
+
+
+@pytest.mark.parametrize("S,T0,steps", [(300, 120, 20), (300, 250, 70), (128, 120, 20)])
+def test_decode_step_hs128_deep_context_and_roll_vs_oracle(dev, S, T0, steps):
+    """Positions crossing 128 keys (a third 64-key sub-tile in the fused attention kernel) and 256 keys (a head's keys
+    split over several CTAs and merged), a full cache and the roll branch: the batch-1 decode step against the
+    exact-arithmetic oracle."""
+    from gpu_util import build_tiny
+
+    torch.manual_seed(S + T0)
+    prompt = torch.randint(0, CFG128["vocab_size"], (1, T0))
+    model, oracle, _ = build_tiny(dev, CFG128, seed=5, exact_linears=True)
+    got, want = _decode(model, oracle, dev, prompt, S, steps, seed=1)
+    for i, (a, b) in enumerate(zip(got, want)):
+        assert _normwise(a, b) < 1.5e-2, (i, _normwise(a, b))
+    assert int(model._ring) == max(0, T0 + steps - S)
+    # logical order == the oracle's rolled cache
+    kl = model.logical_kv_caches()[0][0]
+    torch.testing.assert_close(kl.float().cpu(), oracle.kv[0][0].float(), rtol=2 ** -6, atol=3e-2)
+
+
+def test_greedy_generate_hs128_equals_oracle_tokens(dev):
+    import lit_llama_b200 as P
+    from gpu_util import build_tiny
+
+    model, oracle, _ = build_tiny(dev, CFG128, seed=9)
+    prompt = torch.tensor([5, 100, 319, 7, 48, 1, 250], dtype=torch.int32)
+    y = P.generate(model, prompt.to(dev), 40, top_k=1)
+    want = O.generate(oracle, prompt, 40, top_k=1)
+    same = float((y.cpu() == want).float().mean())
+    assert same >= 0.9, (y.cpu().tolist(), want.tolist())
+
+
+def test_per_op_path_pdl_equals_plain_order(dev):
+    """Programmatic dependent launch must not change a single bit: 24 decode steps of the one-kernel-per-op path
+    with PDL (every activation read after griddepcontrol.wait is a coherent load) vs plain stream order."""
+    from gpu_util import build_tiny
+
+    outs = []
+    for flags in (1, 0):
+        model, _, _ = build_tiny(dev, CFG128, seed=13)
+        model.decode_flags = flags
+        got, _ = _decode(model, None, dev, torch.tensor([[3, 17, 40, 41, 2, 77, 5, 9]]), 160, 24, seed=2)
+        outs.append(torch.stack(got))
+    assert torch.equal(outs[0], outs[1])
+    # and for a batch of 4 (two-launch batch kernel, PDL between its launches)
+    outs = []
+    for flags in (1, 0):
+        model, _, _ = build_tiny(dev, CFG128, seed=13)
+        model.decode_flags = flags
+        idx = torch.tensor([[3, 17, 40], [9, 9, 1], [100, 2, 7], [64, 65, 66]], device=dev)
+        with torch.no_grad():
+            model(idx, 64, torch.arange(3, device=dev))
+            step = [model(torch.full((4, 1), 5 + i, device=dev), 64, torch.tensor([3 + i], device=dev)).clone() for i in range(12)]
+        outs.append(torch.stack(step))
+    assert torch.equal(outs[0], outs[1])
+
+
+def test_tensor_parallel_matches_single_gpu(dev):
+    """TPLLaMA on 2 GPUs (module path and the fused graph-replayed rank step) vs the single-GPU model: tests/tp_check.py
+    under torch.distributed.run.  Skipped on a one-GPU box."""
+    import os
+    import subprocess
+    import sys
+
+    if torch.cuda.device_count() < 2:
+        pytest.skip("needs 2 GPUs")
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",
+                        "--master-port", "29517", os.path.join(root, "tests", "tp_check.py")], capture_output=True, text=True, timeout=600)
+    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-2000:]
+    assert r.stdout.count("OK") >= 2, r.stdout[-2000:]
+
+
 @pytest.mark.parametrize("S,cases", [
     (300, [(0, 0), (5, 0), (127, 0), (128, 0), (299, 0), (300, 0), (333, 7)]),          # 3 splits
     (128, [(0, 0), (127, 0), (130, 3)]),                                                 # single split
@@ -330,8 +446,9 @@ def test_fused_attention_equals_unfused(dev, S, cases):
 def test_fused_attention_vs_oracle_hs128(dev, B):
     """The kernel on the benched path (fused rope + KV append + split-S attention + merge, head_size 128) directly
     against the oracle's restatement of model.py:197-230 (O.rope_apply + index_copy / roll + O.sdpa): positions 0,
-    127, 128 (split boundary of the persistent kernel), 255, 256 (split boundary of this kernel), 1023, 2047 (full
-    cache, 8 splits), and two roll states (model.py:214-218: position >= S with different ring offsets)."""
+    127, 128 (the last position in two 64-key sub-tiles and the first in three), 255, 256 (split boundary of this
+    kernel), 1023, 2047 (full cache, 8 splits), and two roll states (model.py:214-218: position >= S with different
+    ring offsets)."""
     from lit_llama_b200 import _lib as L
 
     nh, hs, S, blk = 4, 128, 2048, 4096

@@ -262,23 +262,6 @@ def test_fused_step_equals_module_path(dev):
         torch.testing.assert_close(a.float(), b.float(), rtol=1e-3, atol=5e-3)
 
 
-def test_persistent_opt_in_keeps_gptq_int8_on_the_per_op_step(dev):
-    """B2L_PERSISTENT=1 (LLaMA.persistent) at head_size 128: the persistent kernel is int4-only, so a gptq.int8 model
-    builds no plan and decodes on the per-op fused step, with the same logits."""
-    from gpu_util import build_tiny
-
-    cfg = dict(block_size=64, vocab_size=96, n_layer=2, n_head=2, n_embd=256)   # head_size 128
-    model, _, _ = build_tiny(dev, cfg, mode="gptq.int8", seed=12)
-    with torch.no_grad():
-        per_op = _run(model, dev)
-        model.persistent = True
-        model.reset_cache()
-        persistent = _run(model, dev)
-        assert model._decode is not None and model._decode.plan is None and model._decode.graph is not None
-    for a, b in zip(per_op, persistent):
-        assert torch.equal(a, b)
-
-
 def test_batch2_runs_the_module_path_on_the_gemm(dev):
     from gpu_util import build_tiny
 

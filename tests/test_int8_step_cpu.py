@@ -129,8 +129,6 @@ def test_step_refusals(L):
     _refused(L, d, -2, b"exclude each other")
     d, q8 = _decode(L, B=2)
     _refused(L, d, -2, b"batch 1 only")
-    d, q8 = _decode(L, plan=FAKE)
-    _refused(L, d, -2, b"persistent kernel")
     d, q8 = _decode(L)
     d.q8_layers = None
     _refused(L, d, -1, b"needs q8_layers")

@@ -157,8 +157,8 @@ def L():
 
 
 def test_binding_and_layout_match_the_header(L, tmp_path):
-    """b2l_kv8_cache and the kv8 member appended to b2l_decode_args agree with the C compiler; every existing offset of
-    b2l_decode_args is what it was (kv8 sits behind lora_row_set, the last field before it); the prototypes bind."""
+    """b2l_kv8_cache and the kv8 member appended to b2l_decode_args agree with the C compiler; the offsets of
+    b2l_decode_args are pinned (kv8 sits behind lora_row_set, the last field before it); the prototypes bind."""
     prog = tmp_path / "layout.c"
     prog.write_text(
         '#include <stdio.h>\n#include <stddef.h>\n#include "b2l.h"\n'
@@ -180,8 +180,8 @@ def test_binding_and_layout_match_the_header(L, tmp_path):
     K, D = L.KV8Cache, L.DecodeArgs
     assert out == [C.sizeof(K), K.v.offset, K.k_scale.offset, K.v_scale.offset, C.sizeof(D), D.kv8.offset,
                    D.lora_row_set.offset, D.flags.offset, L.F_KV_FP8]
-    # the parent's b2l_decode_args ended with lora_row_set: 336 bytes, lora_row_set at 328, flags at 200
-    assert (D.lora_row_set.offset, D.flags.offset, D.kv8.offset) == (328, 200, 336) and C.sizeof(D) == 344
+    # b2l_decode_args ends with kv8: 336 bytes, lora_row_set at 320, flags at 200
+    assert (D.lora_row_set.offset, D.flags.offset, D.kv8.offset) == (320, 200, 328) and C.sizeof(D) == 336
     assert L.F_KV_FP8 == 32768
     fn = L._SIGS["b2l_attention_kv8"]
     assert fn[0] is C.c_int and len(fn[1]) == 16 and fn[1][1] is C.POINTER(L.KV8Cache)
@@ -247,7 +247,6 @@ def test_decode_step_refusals(L):
         msg = lib.b2l_last_error().decode()
         assert rc == code and "b2l_decode_step" in msg and all(w in msg for w in words), (kw.keys(), rc, msg)
 
-    refused(-2, "B2L_F_KV_FP8", "persistent", plan=P16)
     refused(-2, "B2L_F_KV_FP8", "B2L_F_STEPWISE", flags=L.F_PDL | L.F_STEPWISE | L.F_KV_FP8 | L.F_Q4_BATCH_I8,
             batch_work=P16)
     refused(-2, "B2L_F_ATTN_UNFUSED", flags=L.F_PDL | L.F_KV_FP8 | 8)

@@ -272,8 +272,3 @@ def test_decode_step_launch_count_and_refusals(L):
     assert lib.b2l_decode_step(C.byref(d), None) == -2 and b"rank" in lib.b2l_last_error()
     d, keep = _decode_args(L, 4, 4, 512, [none, L.LoRA(256, None, 2.0, 8, 3, 5), none, none])
     assert lib.b2l_decode_step(C.byref(d), None) == -1 and b"null LoRA" in lib.b2l_last_error()
-    # the persistent kernel does not run LoRA: the step and the plan builder refuse it
-    d, keep = _decode_args(L, 4, 4, 512, [none, lo, none, none])
-    d.plan = 4096
-    assert lib.b2l_decode_step(C.byref(d), None) == -2 and b"persistent kernel" in lib.b2l_last_error()
-    assert lib.b2l_decode_plan_build(C.byref(d), None) == -2 and b"persistent kernel" in lib.b2l_last_error()

@@ -141,7 +141,6 @@ def test_decode_step_refusals_and_launch_count(L):
         assert rc == code and all(w in msg for w in words), (kw.keys(), rc, msg)
 
     refused(-2, "lora_sets and loras", loras=[lo, none, none, none])
-    refused(-2, "persistent", plan=P16)
     refused(-2, "affines", affines=C.cast((L.LayerAffine * 4)(), C.POINTER(L.LayerAffine)))
     refused(-2, "affines", lm_head_affine=L.OutAffine(P16, P16))
     refused(-2, "B2L_F_STEPWISE", flags=L.F_PDL | L.F_STEPWISE | L.F_Q4_BATCH_I8, batch_work=P16)

@@ -102,7 +102,6 @@ def test_decode_step_refuses_the_flag_outside_its_combinations(L):
 
     for other in (L.F_W8, L.F_Q8, L.F_W8_BATCH, L.F_W8 | L.F_W8_BATCH):
         refused(-2, "B2L_F_Q4_BATCH_I8", "does not combine", flags=L.F_PDL | L.F_Q4_BATCH_I8 | other)
-    refused(-2, "B2L_F_Q4_BATCH_I8", "persistent", plan=P)
     layer_aff = (L.LayerAffine * 1)()
     refused(-2, "B2L_F_Q4_BATCH_I8", "affines", affines=C.cast(layer_aff, C.POINTER(L.LayerAffine)))
     refused(-2, "B2L_F_Q4_BATCH_I8", "affines", lm_head_affine=L.OutAffine(P, P))

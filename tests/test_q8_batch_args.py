@@ -139,8 +139,6 @@ def test_step_refuses_the_flag_outside_its_combinations(L):
     _refused(L, d, -2, "B2L_F_Q8_BATCH", "does not combine")
     d, _ = _decode(L, flags=L.F_PDL | L.F_Q8 | L.F_Q8_BATCH | L.F_Q4_BATCH_I8)
     _refused(L, d, -2, "does not combine")
-    d, _ = _decode(L, plan=FAKE)
-    _refused(L, d, -2, "B2L_F_Q8_BATCH", "persistent")
     d, _ = _decode(L, B=1)
     _refused(L, d, -2, "B2L_F_Q8_BATCH", "2..16", "B=1")
     d, _ = _decode(L, B=17)

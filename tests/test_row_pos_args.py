@@ -1,6 +1,6 @@
 """CPU: per-row positions (B2L_F_ROW_POS) are refused where they cannot run, before the device is touched:
 b2l_ring_advance_rows / b2l_kv_unroll_rows with null pointers or bad shapes; b2l_attention(_adapter) with the flag at
-T > 1 or with B2L_F_ROPE_ROWS; b2l_decode_step with the flag and a persistent plan.  generate_prompts and
+T > 1 or with B2L_F_ROPE_ROWS; b2l_decode_step with the flag and B2L_F_ROPE_ROWS.  generate_prompts and
 LLaMA.prefill_rows take 1..16 one-dimensional prompts and have no CPU path; LLaMA.forward refuses a 2-D input_pos
 that is not one position per row; the CLI takes --prompts_file."""
 import ctypes as C
@@ -78,10 +78,6 @@ def _decode_args(L, flags):
 def test_decode_step_row_pos_refusals(L):
     lib = L.lib()
     a, keep = _decode_args(L, L.F_PDL | L.F_ROW_POS | L.F_Q4_BATCH_I8)
-    a.plan = P_
-    assert lib.b2l_decode_step(C.byref(a), None) == -2
-    assert "B2L_F_ROW_POS does not run in the persistent kernel" in _err(L)
-    a.plan = None
     a.flags = L.F_ROW_POS | L.F_ROPE_ROWS
     assert lib.b2l_decode_step(C.byref(a), None) == -2 and "B2L_F_ROW_POS does not combine with B2L_F_ROPE_ROWS" in _err(L)
     # the existing refusals still apply with the flag: a batch flag outside its range, null pointers

@@ -108,7 +108,6 @@ def test_decode_step_stepwise_refusals(L):
         (S_, {}, "B2L_F_STEPWISE needs the row-exact linears"),
         (S_ | L.F_W8, {}, "B2L_F_STEPWISE needs the row-exact linears"),
         (S_ | Q4, dict(B=1), "B2L_F_STEPWISE runs 2..16 tokens, got B=1"),
-        (S_ | W8, dict(plan=P_), "B2L_F_STEPWISE does not run in the persistent kernel"),
         (S_ | Q4, dict(affines=True), "B2L_F_STEPWISE does not apply LLaMA-Adapter v2 affines"),
         (S_ | W8, dict(lm_head_affine=L.OutAffine(P_, P_)), "B2L_F_STEPWISE does not apply LLaMA-Adapter v2 affines"),
     ]

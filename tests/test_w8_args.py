@@ -75,7 +75,7 @@ def test_tile_arguments_and_sizes(L):
     assert lib.b2l_w8_untile_i8(P, P, 16, 96, None) == -2 and b"multiple of 64" in lib.b2l_last_error()
 
 
-def test_decode_step_rejects_w8_with_a_batch_or_a_plan(L):
+def test_decode_step_rejects_w8_with_a_batch(L):
     lib = L.lib()
     layers = (L.Layer * 1)()
     base = dict(n_layer=1, n_head=4, n_embd=512, n_hidden=1536, vocab=128, B=1, S=16, sz_dtype=L.B2L_BF16, eps=1e-5,
@@ -84,13 +84,6 @@ def test_decode_step_rejects_w8_with_a_batch_or_a_plan(L):
     a = L.DecodeArgs(**dict(base, B=2))
     assert lib.b2l_decode_step(C.byref(a), None) == -2
     assert "B2L_F_W8" in lib.b2l_last_error().decode() and "batch 1" in lib.b2l_last_error().decode()
-    a = L.DecodeArgs(**dict(base, plan=P))
-    assert lib.b2l_decode_step(C.byref(a), None) == -2
-    assert "persistent" in lib.b2l_last_error().decode()
-    # nor is a persistent plan built over 8-bit tilings (it would read them as int4)
-    a = L.DecodeArgs(**dict(base, plan=P))
-    assert lib.b2l_decode_plan_build(C.byref(a), None) == -2
-    assert "int4" in lib.b2l_last_error().decode()
     # the flag leaves the launch count alone (head_size 128: ring advance, embedding, 4 linears + 1 attention, lm_head)
     a = L.DecodeArgs(**base)
     b = L.DecodeArgs(**dict(base, flags=L.F_PDL))

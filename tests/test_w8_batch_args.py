@@ -107,7 +107,6 @@ def test_decode_step_accepts_the_batch_flag_only_in_its_combinations(L):
 
     refused(-2, "B2L_F_W8_BATCH needs B2L_F_W8", flags=L.F_PDL | L.F_W8_BATCH)
     refused(-2, "exclude each other", flags=L.F_PDL | L.F_W8 | L.F_W8_BATCH | L.F_Q8)
-    refused(-2, "persistent", plan=P)
     layer_aff = (L.LayerAffine * 1)()
     refused(-2, "affines", affines=C.cast(layer_aff, C.POINTER(L.LayerAffine)))
     refused(-2, "affines", lm_head_affine=L.OutAffine(P, P))
