@@ -184,8 +184,7 @@ class LLaMA(llama.LLaMA):
         if st is None or st.shape != shape or st.device != device:
             self._adapter_store = torch.zeros(shape, device=device, dtype=torch.bfloat16)
             self._adapter_gates = torch.zeros((cfg.n_layer, nh), device=device, dtype=torch.bfloat16)
-            self._decode, self._module_graph = None, None   # they point at the old store
-            self._verify = {}
+            self._drop_steps()   # they point at the old store
         st, gates = self._adapter_store, self._adapter_gates
         arr = (L.AdapterPrefix * cfg.n_layer)()
         for i in layers:

@@ -262,8 +262,8 @@ def generate_speculative(
                          f"the target's {model.config.padded_vocab_size}")
     if idx.dim() != 1:
         raise ValueError(f"generate_speculative: idx must be one prompt of shape (T,), got {tuple(idx.shape)}")
-    why = model._decode_tokens_refusal()
-    if why is not None:
+    why = model._decode_route(int(num_draft) + 1, stepwise=True)
+    if isinstance(why, str):
         raise RuntimeError(f"generate_speculative: the target's verify step (LLaMA.decode_tokens) {why}")
     if not idx.is_cuda:
         raise RuntimeError(f"generate_speculative: idx is on {idx.device}; lit_llama_b200 runs on CUDA only (no CPU fallback)")

@@ -7,17 +7,9 @@ Every forward runs hand-written sm_90a kernels (include/b2l.h); tensors must be 
 bf16 - there is no CPU fallback.
 
 Two execution paths behind `LLaMA.forward`:
-  * decode (T == 1 with a KV cache, every Linear a gptq.int4 layer with one (scale, zero) per row):
-    one C call enqueues the whole token (`b2l_decode_step`: int8-MMA GEMV kernels for batch 1, f16-MMA for 2..8 rows,
-    wgmma for 9..16), replayed as a CUDA graph; with `LLaMA.q4_batch_step` (B2L_Q4_BATCH_STEP=1) batches of 2..16 run
-    b2l_q4_gemv_batch_i8 on the resident batch-1 tilings instead (B2L_F_Q4_BATCH_I8: each row bit-identical to the
-    batch-1 kernel on that row).  Every Linear a per-row gptq.int8 layer: the same step at batch 1
-    (B2L_F_W8: the GEMV kernel with 8-bit weights); batches of 2 or more go module by module (on the wgmma GEMM),
-    or, with `LLaMA.w8_batch_step` (B2L_W8_BATCH_STEP=1), batches of 2..16 run the same step (B2L_F_W8_BATCH:
-    b2l_w8_gemv_batch on the resident batch-1 tilings, each row bit-identical to the batch-1 kernel on that row).
-    Every Linear an llm.int8 layer, with `LLaMA.int8_step` (B2L_INT8_STEP=1): the same step at batch 1 (B2L_F_Q8:
-    b2l_q8_linear reading CB / SCB in place) and at batches of 2..16 (B2L_F_Q8 | B2L_F_Q8_BATCH: b2l_q8_linear_batch,
-    also in place), bit-identical to the module path.
+  * decode (T == 1 with a KV cache, B <= 16, every Linear a per-row gptq.int4 / gptq.int8 or an llm.int8 layer): one C
+    call enqueues the whole token (`b2l_decode_step`), replayed as a CUDA graph, on the route `LLaMA._decode_route`
+    picks from the weight kind, B and the opt-ins documented on LLaMA (each route's kernels: csrc/api.cu kRoutes).
   * everything else (prefill on the wgmma GEMM, no-cache forward, other Linear kinds): module by module.
 """
 import ctypes as C
@@ -332,12 +324,67 @@ class _ModuleGraph(SimpleNamespace):
         return getattr(self, name)
 
 
-class _DecodeState:
-    """Static buffers + the C argument block of b2l_decode_step for one (B, S)."""
+def _interleave_rows(a: torch.Tensor, b: torch.Tensor, g: int) -> torch.Tensor:
+    """Rows (dim 0) of a and b as [g rows of a | g rows of b] per block: the fc1|fc2 order of the fused SwiGLU linear."""
+    n = a.shape[0]
+    return torch.stack((a.reshape(n // g, g, *a.shape[1:]), b.reshape(n // g, g, *b.shape[1:])), dim=1).reshape(2 * n, *a.shape[1:])
 
-    def __init__(self, model: "LLaMA", B: int, S: int, device: torch.device, idx_dtype: torch.dtype,
+
+def _fc12_weights(mlp: nn.Module, q1: torch.Tensor, q2: torch.Tensor, kind: str):
+    """(tiling, scales, zeros) of c_fc1 and c_fc2 (quant_weight q1 / q2 in the reference layout) interleaved (8 rows / 8
+    rows per 16-row block for the batch-1 and 2..8-row kernels, 64 / 64 per 128-row tile for the wgmma kernel) and
+    re-tiled for `kind` ("i8", "mma" or "tc", as _Route.tiling), so one tile holds silu's argument and its multiplier
+    and SwiGLU runs in the epilogue.  "i8" tiles 4-bit layers with b2l_q4_tile_i8 and 8-bit ones with b2l_w8_tile_i8."""
+    nh, K = mlp.c_fc1.out_features, mlp.c_fc1.in_features
+    g = 8 if kind != "tc" else 64
+    assert nh % g == 0
+    qw = _interleave_rows(q1, q2, g).t().contiguous().t()  # reference layout (1, 2nh)
+    scales = _interleave_rows(mlp.c_fc1.scales, mlp.c_fc2.scales, g).contiguous()
+    zeros = _interleave_rows(mlp.c_fc1.zeros, mlp.c_fc2.zeros, g).contiguous()
+    lib = L.lib()
+    if kind == "i8":
+        from .quantization import tile_i8
+
+        tiled = tile_i8(qw, 2 * nh, K, mlp.c_fc1.bits)
+    elif kind == "mma":
+        tiled = torch.empty(lib.b2l_q4_tiled_mma_bytes(2 * nh, K), dtype=torch.uint8, device=qw.device)
+        L.check(lib.b2l_q4_tile_mma(qw.data_ptr(), tiled.data_ptr(), 2 * nh, K, L.stream_ptr()), "b2l_q4_tile_mma")
+    else:
+        tiled = torch.empty(lib.b2l_q4_tiled_bytes(2 * nh, K), dtype=torch.uint8, device=qw.device)
+        L.check(lib.b2l_q4_tile(qw.data_ptr(), tiled.data_ptr(), 2 * nh, K, L.stream_ptr()), "b2l_q4_tile")
+    return tiled, scales, zeros
+
+
+@dataclass(frozen=True)
+class _Route:
+    """One route of b2l_decode_step, named as csrc/api.cu's RouteId: the B2L_F_* bits it adds to the step's flags, the
+    tiling every gptq weight is read in ("i8": tiled_i8() as qw_mma, the resident copy of a compacted model; "mma":
+    tiled_mma() as qw_mma; "tc": tiled() as qw_tiled; None: llm.int8's CB / SCB in place), which is also _fc12's kind,
+    and the kernel whose workspace batch_work holds (None: no batch_work)."""
+    name: str
+    flags: int
+    tiling: Optional[str]
+    work: Optional[str]
+
+
+_ROUTES = {r.name: r for r in (
+    _Route("q4_gemv", 0, "i8", None),
+    _Route("q4_batch", 0, "mma", "q4_gemv_batch"),
+    _Route("q4_tc", 0, "tc", None),
+    _Route("q4_batch_i8", L.F_Q4_BATCH_I8, "i8", "w8_gemv_batch"),   # the two batch kernels share their workspace
+    _Route("w8_gemv", L.F_W8, "i8", None),
+    _Route("w8_batch", L.F_W8 | L.F_W8_BATCH, "i8", "w8_gemv_batch"),
+    _Route("q8", L.F_Q8, None, None),
+    _Route("q8_batch", L.F_Q8 | L.F_Q8_BATCH, None, "q8_linear_batch"),
+)}
+
+
+class _DecodeState:
+    """Static buffers + the C argument block of b2l_decode_step on `route` for one (B, S)."""
+
+    def __init__(self, model: "LLaMA", route: _Route, B: int, S: int, device: torch.device, idx_dtype: torch.dtype,
                  row_pos: bool = False, stepwise: bool = False) -> None:
-        from .quantization import ColBlockQuantizedLinear
+        from .quantization import ColBlockQuantizedLinear, batch_workspace
 
         cfg = model.config
         C_, nh = cfg.n_embd, cfg.n_head
@@ -358,38 +405,20 @@ class _DecodeState:
         lib = L.lib()
         self.work = torch.zeros(lib.b2l_attn_workspace_bytes(B, nh, hs, 1, S) // 4 + 1, device=device, dtype=torch.float32)
         self.keep = []  # tensors the argument block points into
-
-        from .quantization import BATCH_GEMV, batch_workspace
-
-        # batch 1..8: mma.sync kernels (q4_gemv / q4_gemv_batch) and their tiling; 9..16: wgmma kernel and its tiling.
-        # gptq.int8: the batch-1 kernel with 8-bit weights (b2l_w8_tile_i8 tilings); with `w8_batch_step`, batches of
-        # 2..16 run b2l_w8_gemv_batch on the same resident tilings (B2L_F_W8_BATCH).  gptq.int4 with `q4_batch_step`:
-        # batches of 2..16 run b2l_q4_gemv_batch_i8 on the batch-1 tilings (B2L_F_Q4_BATCH_I8)
-        # B2L_F_STEPWISE (decode_tokens) always runs the row-exact batch kernels: each row must equal the batch-1 step
-        w8 = model._fast_ok == "w8"
-        w8b = w8 and B > 1
-        q4b = model._fast_ok == "q4" and B > 1 and (model.q4_batch_step or stepwise)
-        # llm.int8: b2l_q8_linear (batch 1) or b2l_q8_linear_batch (2..16, B2L_F_Q8_BATCH) on every weight's CB / SCB in
-        # place (no copy, no tiling)
-        q8 = model._fast_ok == "q8"
-        q8b = q8 and B > 1
-        assert not w8b or ((model.w8_batch_step or stepwise) and B <= 16)
-        gemv = (B == 1) or w8b or q4b or (B <= 8 and BATCH_GEMV)
-        i8 = B == 1 or w8b or q4b   # the b2l_q4_tile_i8 / b2l_w8_tile_i8 tilings (the resident copy of a compacted model)
-        self.batch_ws = None
-        if w8b or q4b:   # the two batch kernels share their digit-plane workspace
-            nb = lib.b2l_w8_gemv_batch_workspace_bytes(max(C_, n_hidden), B)
-            self.batch_ws = torch.empty(nb, dtype=torch.uint8, device=device)
-        elif q8b:
-            self.batch_ws = torch.empty(lib.b2l_q8_linear_batch_workspace_bytes(max(C_, n_hidden), B), dtype=torch.uint8,
-                                        device=device)
-        elif gemv and B > 1 and not q8:
+        q8 = route.tiling is None
+        mma = route.tiling != "tc"   # the tiling goes in qw_mma (else qw_tiled)
+        if route.work == "q4_gemv_batch":   # one per device, shared by every state
             self.batch_ws = batch_workspace(device, max(C_, n_hidden))
+        elif route.work is not None:
+            nb = getattr(lib, f"b2l_{route.work}_workspace_bytes")(max(C_, n_hidden), B)
+            self.batch_ws = torch.empty(nb, dtype=torch.uint8, device=device)
+        else:
+            self.batch_ws = None
 
         def q4(lin: ColBlockQuantizedLinear) -> L.Q4Weight:
-            t = (lin.tiled_i8() if i8 else lin.tiled_mma()) if gemv else lin.tiled()
+            t = {"i8": lin.tiled_i8, "mma": lin.tiled_mma, "tc": lin.tiled}[route.tiling]()
             self.keep.append(t)   # a compacted layer hands out transient tilings: this state owns the ones it points at
-            return L.Q4Weight(None if gemv else t.data_ptr(), t.data_ptr() if gemv else None, lin.scales.data_ptr(),
+            return L.Q4Weight(None if mma else t.data_ptr(), t.data_ptr() if mma else None, lin.scales.data_ptr(),
                               lin.zeros.data_ptr(), lin.out_features, lin.in_features)
 
         def bf16(p: torch.Tensor) -> torch.Tensor:
@@ -418,10 +447,10 @@ class _DecodeState:
                                          q8w(mlp.c_proj))
                 layers[i] = L.Layer(**rms, k_cache=k.data_ptr(), v_cache=v.data_ptr())
                 continue
-            fc12 = model._fc12(i, "i8" if i8 else ("mma" if gemv else "tc"))
+            fc12 = model._fc12(i, route.tiling)
             layers[i] = L.Layer(
                 **rms, c_attn=q4(blk.attn.c_attn), c_proj=q4(blk.attn.c_proj),
-                c_fc12=L.Q4Weight(None if gemv else fc12[0].data_ptr(), fc12[0].data_ptr() if gemv else None,
+                c_fc12=L.Q4Weight(None if mma else fc12[0].data_ptr(), fc12[0].data_ptr() if mma else None,
                                   fc12[1].data_ptr(), fc12[2].data_ptr(), 2 * n_hidden, C_),
                 mlp_proj=q4(blk.mlp.c_proj), k_cache=k.data_ptr(), v_cache=v.data_ptr())
         self.layers = layers
@@ -435,9 +464,8 @@ class _DecodeState:
             ring_start=model._ring.data_ptr(), block_size=cfg.block_size, x=self.x.data_ptr(), qkv=self.qkv.data_ptr(),
             att=self.att.data_ptr(), hid=self.hid.data_ptr(), attn_work=self.work.data_ptr(),
             logits=self.logits.data_ptr(),
-            flags=(model.decode_flags | (L.F_W8 if w8 else 0) | (L.F_W8_BATCH if w8b else 0) | (L.F_Q8 if q8 else 0)
-                   | (L.F_Q4_BATCH_I8 if q4b else 0) | (L.F_Q8_BATCH if q8b else 0) | (L.F_ROW_POS if row_pos else 0)
-                   | (L.F_STEPWISE if stepwise else 0) | (L.F_KV_FP8 if kv8 else 0)),
+            flags=(model.decode_flags | route.flags | (L.F_ROW_POS if row_pos else 0) | (L.F_STEPWISE if stepwise else 0)
+                   | (L.F_KV_FP8 if kv8 else 0)),
             batch_work=None if self.batch_ws is None else self.batch_ws.data_ptr())
         if kv8:
             self.keep.append(kv8_arr)
@@ -522,8 +550,8 @@ class LLaMA(nn.Module):
         self._decode: Optional[_DecodeState] = None
         self._verify = {}   # T -> _DecodeState of decode_tokens (B2L_F_STEPWISE), each with its own CUDA graph
         self._module_graph = None  # CUDA graph of the module-by-module decode step (non-fused Linear kinds)
-        # the fused step can run every Linear (checked once): "q4" (per-row gptq.int4, any B <= 16), "w8" (per-row
-        # gptq.int8, B == 1), False (module path)
+        # the fused step can run every Linear (checked once, _fast_decode_ok): "q4" (per-row gptq.int4), "w8" (per-row
+        # gptq.int8), "q8" (llm.int8), False (module path); _decode_route picks the route from it
         self._fast_ok: Union[None, bool, str] = None
         self._fc12_cache = {}
         self._lora_route = None   # multi-LoRA: the adapter choice of the current call (lora._QuantizedLoRA._lora_route)
@@ -661,8 +689,7 @@ class LLaMA(nn.Module):
                 like = (f1 or f2)[0]
                 one, zero = torch.ones(nh, dtype=like.dtype, device=like.device), torch.zeros(nh, dtype=like.dtype, device=like.device)
                 f1, f2 = f1 or (one, zero), f2 or (one, zero)
-                fc12 = tuple(torch.stack((a.view(nh // 8, 8), b.view(nh // 8, 8)), dim=1).reshape(2 * nh)
-                             for a, b in zip(f1, f2))
+                fc12 = tuple(_interleave_rows(a, b, 8) for a, b in zip(f1, f2))
             arr[i] = L.LayerAffine(spec(affine_of(blk.attn.c_attn)), spec(affine_of(blk.attn.c_proj)), spec(fc12),
                                    spec(affine_of(mlp.c_proj)))
         keep.append(arr)
@@ -694,9 +721,7 @@ class LLaMA(nn.Module):
         self.kv_caches.clear()
         self._kv_store = None
         self._kv_scale = None
-        self._decode = None
-        self._verify = {}
-        self._module_graph = None
+        self._drop_steps()
         if self._lora_route is not None:
             self._set_lora_route(None)
         if self._ring is not None:
@@ -710,8 +735,7 @@ class LLaMA(nn.Module):
         self._ring = ring
         for blk in self.transformer.h:
             blk.attn._ring, blk.attn._ring_shared = ring, True
-        self._decode, self._module_graph = None, None   # they point at the old ring
-        self._verify = {}
+        self._drop_steps()   # they point at the old ring
 
     @staticmethod
     def _check_prompts(prompts: List[torch.Tensor], max_seq_length: int, who: str) -> None:
@@ -902,18 +926,12 @@ class LLaMA(nn.Module):
                 torch.float8_e4m3fn)
             self._kv_scale = self._kv_scale.expand(n_layer, two, B, nh, S).contiguous()
         self._set_kv_views()
-        self._decode = None
-        self._verify = {}
-        self._module_graph = None
+        self._drop_steps()
 
     # ------------------------------------------------------------------ helpers
     def _fc12(self, i: int, kind: str):
-        """c_fc1 and c_fc2 of layer i interleaved (8 rows / 8 rows per 16-row block for the
-        batch-1 kernel, 64 / 64 per 128-row tile for the wgmma kernel) and re-tiled, so one
-        tile holds silu's argument and its multiplier and SwiGLU runs in the epilogue.
-        "i8" tiles 4-bit layers with b2l_q4_tile_i8 and 8-bit ones with b2l_w8_tile_i8."""
+        """_fc12_weights of layer i for `kind`, cached while c_fc1 and c_fc2's weights stay the same."""
         mlp = self.transformer.h[i].mlp
-        gemv = kind != "tc"
         hit = self._fc12_cache.get((i, kind))
         if hit is not None and getattr(mlp.c_fc1, "_released", False):
             return hit[1]     # compacted: this copy IS the layer's weights (compact())
@@ -921,28 +939,7 @@ class LLaMA(nn.Module):
         key = (kind, q1.data_ptr(), q1._version, q2.data_ptr(), q2._version)
         if hit is not None and hit[0] == key:
             return hit[1]
-        nh, K = mlp.c_fc1.out_features, mlp.c_fc1.in_features
-        g = 8 if gemv else 64
-        assert nh % g == 0
-
-        def inter(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:  # rows (dim 0) of a, b -> [t][g of a | g of b]
-            return torch.stack((a.reshape(nh // g, g, *a.shape[1:]), b.reshape(nh // g, g, *b.shape[1:])), dim=1).reshape(2 * nh, *a.shape[1:])
-
-        qw = inter(q1, q2).t().contiguous().t()  # reference layout (1, 2nh)
-        scales = inter(mlp.c_fc1.scales, mlp.c_fc2.scales).contiguous()
-        zeros = inter(mlp.c_fc1.zeros, mlp.c_fc2.zeros).contiguous()
-        lib = L.lib()
-        if kind == "i8":
-            from .quantization import tile_i8
-
-            tiled = tile_i8(qw, 2 * nh, K, mlp.c_fc1.bits)
-        elif kind == "mma":
-            tiled = torch.empty(lib.b2l_q4_tiled_mma_bytes(2 * nh, K), dtype=torch.uint8, device=qw.device)
-            L.check(lib.b2l_q4_tile_mma(qw.data_ptr(), tiled.data_ptr(), 2 * nh, K, L.stream_ptr()), "b2l_q4_tile_mma")
-        else:
-            tiled = torch.empty(lib.b2l_q4_tiled_bytes(2 * nh, K), dtype=torch.uint8, device=qw.device)
-            L.check(lib.b2l_q4_tile(qw.data_ptr(), tiled.data_ptr(), 2 * nh, K, L.stream_ptr()), "b2l_q4_tile")
-        val = (tiled, scales, zeros)
+        val = _fc12_weights(mlp, q1, q2, kind)
         self._fc12_cache[(i, kind)] = (key, val)
         return val
 
@@ -950,9 +947,25 @@ class LLaMA(nn.Module):
         out = super()._apply(fn, recurse)
         # the interleaved fc1|fc2 copies are plain tensors of this module: they move with it (a compacted model has no other)
         self._fc12_cache = {k: (key, tuple(fn(t) for t in val)) for k, (key, val) in self._fc12_cache.items()}
-        self._decode, self._module_graph, self._fast_ok = None, None, None
-        self._verify = {}
+        self._drop_steps()
+        self._fast_ok = None
         return out
+
+    def _drop_steps(self) -> None:
+        """Forget every cached decode step (the fused one, decode_tokens' and the module graph): each bakes pointers
+        into the KV store, the ring, the adapter prefixes and the weights."""
+        self._decode, self._verify, self._module_graph = None, {}, None
+
+    def _drop_stale(self, st) -> bool:
+        """Whether the step state `st` was built before a linear was reloaded, repacked or moved.  If so, everything that
+        bakes weight pointers is dropped: every step, _fast_ok, and the interleaved fc1|fc2 copies the reference buffers
+        can rebuild (not those compact() made the ONLY copy of both layers: still released, nothing was loaded)."""
+        if st is None or st.generation == WEIGHTS_GENERATION[0]:
+            return False
+        self._drop_steps()
+        self._fast_ok = None
+        self._fc12_cache = {k: v for k, v in self._fc12_cache.items() if k[1] == "i8" and self._fc12_is_only_copy(k[0])}
+        return True
 
     def _fc12_is_only_copy(self, i: int) -> bool:
         mlp = self.transformer.h[i].mlp
@@ -998,8 +1011,7 @@ class LLaMA(nn.Module):
             blk.mlp.c_fc1.release_reference_layout(source=functools.partial(self._fc_from_fc12, i, 0), half=(fc12, 0))
             blk.mlp.c_fc2.release_reference_layout(source=functools.partial(self._fc_from_fc12, i, 1), half=(fc12, 1))
         self.lm_head.release_reference_layout()
-        self._decode, self._module_graph = None, None   # rebuilt on the next step (B > 1 states hold their transient tilings)
-        self._verify = {}
+        self._drop_steps()   # rebuilt on the next step (B > 1 states hold their transient tilings)
         torch.cuda.empty_cache()
         return self
 
@@ -1020,16 +1032,10 @@ class LLaMA(nn.Module):
                 return False
             return m.w8_gemv_capable if kind == "w8" else (m.tc_capable and m.gemv_capable)
 
-        if not ok(self.lm_head) or self.config.n_embd % 8 != 0:
-            return False
         dt = self.lm_head.scales.dtype
-        for blk in self.transformer.h:
-            lins = (blk.attn.c_attn, blk.attn.c_proj, blk.mlp.c_fc1, blk.mlp.c_fc2, blk.mlp.c_proj)
-            if not all(ok(m) and m.scales.dtype == dt for m in lins):
-                return False
-            if blk.mlp.c_fc1.out_features % 64 != 0:
-                return False
-        return kind
+        if self.config.n_embd % 8 != 0 or not all(ok(m) and m.scales.dtype == dt for m in self._linears()):
+            return False
+        return kind if all(blk.mlp.c_fc1.out_features % 64 == 0 for blk in self.transformer.h) else False
 
     def _int8_decode_ok(self) -> bool:
         from .int8 import Linear8bitLt
@@ -1044,10 +1050,7 @@ class LLaMA(nn.Module):
                     and cb.dtype == torch.int8 and cb.is_contiguous() and cb.data_ptr() % 16 == 0 and scb is not None
                     and scb.dtype == torch.float32 and scb.is_contiguous() and scb.device == cb.device)
 
-        lins = [self.lm_head]
-        for blk in self.transformer.h:
-            lins += [blk.attn.c_attn, blk.attn.c_proj, blk.mlp.c_fc1, blk.mlp.c_fc2, blk.mlp.c_proj]
-        return all(ok(m) for m in lins)
+        return all(ok(m) for m in self._linears())
 
     def logical_kv_caches(self) -> List[KVCache]:
         """kv_caches in the reference's slot order.  Identical to `kv_caches` until the
@@ -1100,9 +1103,7 @@ class LLaMA(nn.Module):
 
         if input_pos is not None and not self.kv_caches:
             self._new_kv_store(B, max_seq_length, idx.device)
-            self._decode = None
-            self._verify = {}
-            self._module_graph = None
+            self._drop_steps()
         if input_pos is not None and T > 1 and self._kv_scale is not None:
             # an fp8 cache is prefilled from position 0 (one host read of the positions)
             if input_pos.numel() != T or not bool((input_pos.reshape(-1) == torch.arange(T, device=input_pos.device)).all()):
@@ -1117,27 +1118,12 @@ class LLaMA(nn.Module):
         # ---- decode: one C call per token, replayed as a CUDA graph
         st = None
         if input_pos is not None and T == 1 and B <= 16 and idx.dtype in (torch.int32, torch.int64):
-            st = self._decode
-            if st is not None and st.generation != WEIGHTS_GENERATION[0]:
-                # a linear was reloaded, repacked or moved since the argument block / graph was built: everything that
-                # bakes weight pointers is stale (fc1|fc2 interleave, eligibility, module graph included)
-                st = self._decode = None
-                self._module_graph, self._fast_ok, self._verify = None, None, {}
-                # the interleaved fc1|fc2 copies are rebuilt from the reference buffers, except where compact() made
-                # one the ONLY copy of both layers (still released: nothing was loaded into them)
-                self._fc12_cache = {k: v for k, v in self._fc12_cache.items()
-                                    if k[1] == "i8" and self._fc12_is_only_copy(k[0])}
+            st = None if self._drop_stale(self._decode) else self._decode
             if (st is None or st.B != B or st.S != max_seq_length or st.idx.dtype != idx.dtype or st.idx.device != idx.device
                     or st.row_pos != rows or (st.lora_rows is None) != (self._lora_route is None)):
-                if self._fast_ok is None:
-                    self._fast_ok = self._fast_decode_ok()
-                # gptq.int8 and LLaMA-Adapter v2: batch 1 only; gptq.int8 without v2 affines at batch 2..16 on request
-                # (w8_batch_step); llm.int8 at batch 1..16 (v2 affines included) on request (int8_step)
-                fast = (bool(self._fast_ok) and (self._fast_ok != "q8" or self.int8_step)
-                        and (B == 1 or self._fast_ok == "q8"
-                             or (self._fast_ok != "w8" and not self._has_affines())
-                             or (self._fast_ok == "w8" and self.w8_batch_step and not self._has_affines())))
-                st = self._decode = _DecodeState(self, B, max_seq_length, idx.device, idx.dtype, rows) if fast else None
+                route = self._decode_route(B)
+                st = self._decode = (_DecodeState(self, route, B, max_seq_length, idx.device, idx.dtype, rows)
+                                     if isinstance(route, _Route) else None)
         if st is not None:
             st.idx.copy_(idx.reshape(-1))
             st.pos.copy_(input_pos.reshape(-1) if rows else input_pos.reshape(-1)[-1:])
@@ -1188,39 +1174,54 @@ class LLaMA(nn.Module):
         if idx.dtype not in (torch.int32, torch.int64):
             raise ValueError(f"decode_tokens: idx dtype {idx.dtype}; int32 or int64")
         max_seq_length = self._prepare(idx, max_seq_length)
-        why = self._decode_tokens_refusal()
-        if why is not None:
-            raise RuntimeError(f"decode_tokens: {why}")
+        route = self._decode_route(T, stepwise=True)
+        if isinstance(route, str):
+            raise RuntimeError(f"decode_tokens: {route}")
         if self._ring.numel() != 1 or (self._kv_store is not None and self._kv_store.shape[2] != 1):
             raise RuntimeError("decode_tokens: the KV cache holds more than one sequence; reset_cache() first")
         if not self.kv_caches:
             self._new_kv_store(1, max_seq_length, idx.device)
-            self._decode, self._module_graph, self._verify = None, None, {}
+            self._drop_steps()
         if self._kv_store.shape[4] != max_seq_length:
             raise ValueError(f"decode_tokens: max_seq_length={max_seq_length} against a cache of {self._kv_store.shape[4]}")
         st = self._verify.get(T)
-        if st is not None and (st.generation != WEIGHTS_GENERATION[0] or st.idx.dtype != idx.dtype
-                               or st.idx.device != idx.device):
-            self._verify, self._fast_ok, st = {}, None, None   # weight pointers or the step's inputs changed
+        if self._drop_stale(st) or (st is not None and (st.idx.dtype != idx.dtype or st.idx.device != idx.device)):
+            self._verify, self._fast_ok = {}, None   # weight pointers or the step's inputs changed
             return self.decode_tokens(idx, max_seq_length, input_pos)
         if st is None:
-            st = self._verify[T] = _DecodeState(self, T, max_seq_length, idx.device, idx.dtype, stepwise=True)
+            st = self._verify[T] = _DecodeState(self, route, T, max_seq_length, idx.device, idx.dtype, stepwise=True)
         st.idx.copy_(idx.reshape(-1))
         st.pos.copy_(input_pos)
         _graph_step(st, self.graph_after, st.enqueue)
         out = st.logits.view(T, -1)
         return out.clone() if self.copy_logits else out
 
-    def _decode_tokens_refusal(self) -> Optional[str]:
-        """Why this model cannot run decode_tokens, or None."""
-        if self._kv_cache_dtype == "fp8" or self._kv_scale is not None:
+    def _decode_route(self, B: int, stepwise: bool = False) -> Union[_Route, str]:
+        """The route b2l_decode_step runs B rows on (stepwise: decode_tokens' B consecutive tokens of one sequence), or
+        why the fused step does not run them: forward then goes module by module, and decode_tokens refuses with it.
+        The one place the Python side picks the step's kernels (csrc/api.cu resolve_route reads the flags it sets)."""
+        from . import quantization
+
+        if stepwise and (self._kv_cache_dtype == "fp8" or self._kv_scale is not None):
             return "does not run on an fp8 KV cache (kv_cache_dtype='fp8'): speculative verify keeps a bf16 cache"
         if self._fast_ok is None:
             self._fast_ok = self._fast_decode_ok()
-        if self._fast_ok not in ("q4", "w8") or self._has_affines():
+        kind, affines = self._fast_ok, self._has_affines()
+        if stepwise:   # the row-exact batch kernels whatever the opt-ins say: each row must equal the batch-1 step
+            if kind in ("q4", "w8") and not affines:
+                return _ROUTES["q4_batch_i8" if kind == "q4" else "w8_batch"]
             return ("needs a gptq.int4 or gptq.int8 model the fused decode step runs with its row-exact batch kernels "
                     "(not dense, llm.int8, LLaMA-Adapter v2, or grouped / biased gptq)")
-        return None
+        if kind == "q8" and self.int8_step:   # LLaMA-Adapter v2 affines at any B
+            return _ROUTES["q8" if B == 1 else "q8_batch"]
+        if kind in ("q4", "w8") and B == 1:
+            return _ROUTES[kind + "_gemv"]
+        if kind == "w8" and self.w8_batch_step and not affines:
+            return _ROUTES["w8_batch"]
+        if kind == "q4" and not affines:
+            return _ROUTES["q4_batch_i8" if self.q4_batch_step else
+                           "q4_batch" if B <= 8 and quantization.BATCH_GEMV else "q4_tc"]
+        return f"the fused step runs no route for this model at batch {B} with these opt-ins"
 
     def _prepare(self, idx: torch.Tensor, max_seq_length: Optional[int]) -> int:
         """model.py:79-91: the shape checks, and the RoPE table and KV ring on idx's device.  Returns max_seq_length."""

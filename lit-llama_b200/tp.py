@@ -31,7 +31,7 @@ import torch.distributed as dist
 import torch.nn as nn
 
 from . import _lib as L
-from .model import LLaMAConfig, RMSNorm, _add, _graph_step, build_rope_cache
+from .model import LLaMAConfig, RMSNorm, _add, _fc12_weights, _graph_step, build_rope_cache
 from .quantization import ColBlockQuantizedLinear
 
 
@@ -162,18 +162,6 @@ class _TPDecodeState:
         def lin(l: ColBlockQuantizedLinear, x, y, pro=L.PRO_NONE, ns=None, epi=L.EPI_STORE, res=None):
             return gemv(l.tiled_i8(), l.scales, l.zeros, l.out_features, l.in_features, x, y, pro, ns, epi, res)
 
-        def fc12(mlp):   # c_fc1 | c_fc2 interleaved 8 rows / 8 rows per 16-row block, so SwiGLU runs in the epilogue
-            nh, K = mlp.c_fc1.out_features, mlp.c_fc1.in_features
-
-            def inter(a, b):
-                return torch.stack((a.reshape(nh // 8, 8, *a.shape[1:]), b.reshape(nh // 8, 8, *b.shape[1:])), dim=1).reshape(2 * nh, *a.shape[1:])
-
-            qw = inter(mlp.c_fc1.quant_weight, mlp.c_fc2.quant_weight).t().contiguous().t()
-            sc, z = inter(mlp.c_fc1.scales, mlp.c_fc2.scales).contiguous(), inter(mlp.c_fc1.zeros, mlp.c_fc2.zeros).contiguous()
-            t = torch.empty(lib.b2l_q4_tiled_i8_bytes(2 * nh, K), dtype=torch.uint8, device=qw.device)
-            L.check(lib.b2l_q4_tile_i8(qw.data_ptr(), t.data_ptr(), 2 * nh, K, L.stream_ptr()), "b2l_q4_tile_i8")
-            return t, sc, z, 2 * nh, K
-
         rank0 = m.rank == 0
         self.ops = []   # ("gemv", args) | ("attn", layer index) | ("allreduce", tensor) | ("allgather",)
         for i, blk in enumerate(m.transformer.h):
@@ -181,8 +169,8 @@ class _TPDecodeState:
             self.ops.append(("attn", i))
             self.ops.append(("gemv", lin(blk.attn.c_proj, self.att, self.x, epi=L.EPI_RESIDUAL if rank0 else L.EPI_STORE, res=self.x if rank0 else None)))
             self.ops.append(("allreduce", self.x))
-            t, sc, z, N2, K2 = fc12(blk.mlp)
-            self.ops.append(("gemv", gemv(t, sc, z, N2, K2, self.x, self.hid, L.PRO_RMSNORM, bf16(blk.rms_2.scale), L.EPI_SWIGLU, None)))
+            t, sc, z = _fc12_weights(blk.mlp, blk.mlp.c_fc1.quant_weight, blk.mlp.c_fc2.quant_weight, "i8")
+            self.ops.append(("gemv", gemv(t, sc, z, 2 * hid_l, Cd, self.x, self.hid, L.PRO_RMSNORM, bf16(blk.rms_2.scale), L.EPI_SWIGLU, None)))
             self.ops.append(("gemv", lin(blk.mlp.c_proj, self.hid, self.x, epi=L.EPI_RESIDUAL if rank0 else L.EPI_STORE, res=self.x if rank0 else None)))
             self.ops.append(("allreduce", self.x))
         self.ops.append(("gemv", lin(m.lm_head, self.x, self.logits_l, L.PRO_RMSNORM, bf16(m.transformer.ln_f.scale))))

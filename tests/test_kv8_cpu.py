@@ -271,7 +271,7 @@ def test_kv_cache_dtype_is_read_at_allocation():
     with pytest.raises(RuntimeError, match="reset_cache"):
         m.kv_cache_dtype = None
     m.kv_cache_dtype = "fp8"   # unchanged: allowed
-    assert "fp8 KV cache" in m._decode_tokens_refusal()   # decode_tokens and generate_speculative refuse it
+    assert "fp8 KV cache" in m._decode_route(2, stepwise=True)   # decode_tokens and generate_speculative refuse it
     m.reset_cache()
     m.kv_cache_dtype = None
     m._new_kv_store(1, 16, torch.device("cpu"))
