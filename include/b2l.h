@@ -671,6 +671,29 @@ typedef struct b2l_kv8_cache {
 int b2l_attention_kv8(void* qkv, const b2l_kv8_cache* kv, const void* rope, const int64_t* input_pos,
                       const int32_t* ring_start, void* y, void* work, int B, int T, int n_head, int head_size,
                       int S, int block_size, int flags, const b2l_adapter_prefix* prefix, b2l_stream_t stream);
+/* b2l_attention_ragged into an fp8 cache: n_seq prompts packed back to back, each prefilled
+ * into its own row of a B_rows-row fp8 cache, in one launch per kernel.
+ *   qkv   bf16 [N, 3*C]: sequence s is tokens [start[s], start[s] + len[s]), at positions
+ *         0..len[s]-1; q and k are rotated in place
+ *   kv    codes and scales [B_rows, ...]: sequence s writes slots 0..len[s]-1 of row row[s]
+ *   ring_start int32 [B_rows]: ring_start[row[s]] is set to 0
+ *   y     bf16 [N, C]: each sequence's causal attention over its own rotated bf16 rows in qkv
+ *         (plus the LLaMA-Adapter prefix term when `prefix` is given)
+ * Each sequence's y rows, its rotated q / k rows in qkv, and its row's codes and scales at
+ * slots 0..len[s]-1 equal, bit for bit, one b2l_attention_kv8 launch with B = 1, T = len[s],
+ * input_pos NULL and ring offset 0 on a cache holding only that row: the same quantizer per
+ * (token, head), and every 64-query tile starts at its sequence's first token with the same
+ * queries, keys and key order as that launch's.  Slots >= len[s] of a named row are left as
+ * that launch leaves them (untouched).  Rows and ring offsets no sequence names are not
+ * touched.  The cache is never read, so stale or NaN contents cannot leak in.  `seqs` is read
+ * on the host and passed by value (the call can be captured in a CUDA graph).
+ * head_size 128 only (else B2L_E_UNSUPPORTED).  B2L_E_ARG before any launch for what
+ * b2l_attention_ragged refuses, for a null or misaligned b2l_kv8_cache pointer, and for a
+ * length outside 2..S or above block_size: a one-token prompt's batch-1 counterpart is the
+ * T == 1 decode kernel, which scores its token as the value read back, not as its bf16 value. */
+int b2l_attention_ragged_kv8(void* qkv, const b2l_kv8_cache* kv, const void* rope, const b2l_ragged* seqs,
+                             int32_t* ring_start, void* y, int N, int B_rows, int n_head, int head_size, int S,
+                             int block_size, const b2l_adapter_prefix* prefix, b2l_stream_t stream);
 /* b2l_kv_unroll / b2l_kv_unroll_rows for one fp8 cache tensor (codes and their scales): `out` bf16
  * [B, nh, S, hs] holds the values read back, in logical slot order. */
 int b2l_kv8_unroll(const void* code, const float* scale, const int32_t* ring_start, void* out, int B,

@@ -226,6 +226,8 @@ _SIGS = {
     "b2l_kv_unroll_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "b2l_attention_kv8": (c_int, [c_void_p, C.POINTER(KV8Cache), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                                   c_int, c_int, c_int, c_int, c_int, c_int, C.POINTER(AdapterPrefix), c_void_p]),
+    "b2l_attention_ragged_kv8": (c_int, [c_void_p, C.POINTER(KV8Cache), c_void_p, C.POINTER(Ragged), c_void_p, c_void_p,
+                                         c_int, c_int, c_int, c_int, c_int, c_int, C.POINTER(AdapterPrefix), c_void_p]),
     "b2l_kv8_unroll": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "b2l_kv8_unroll_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "b2l_decode_step": (c_int, [C.POINTER(DecodeArgs), c_void_p]),

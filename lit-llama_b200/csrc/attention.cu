@@ -163,13 +163,26 @@ __global__ void rope_append_kernel(__nv_bfloat16* __restrict__ qkv, __nv_bfloat1
 // (one thread per rotated pair).  q and k are rotated in place as rope_append_kernel does without a cache (the prompt
 // then attends over its own bf16 rows), and the rotated k row and the v row are quantized into slot
 // (t + ring_start[0]) % S of row b.
+// RAGGED (b2l_attention_ragged_kv8): grid (N, n_head); packed token bt is token t of the sequence `rg` places at
+// [start, start + len), quantized into slot t of cache row `row`, whose ring offset restarts at 0 (the token-0 CTA of
+// head 0 stores it; nothing here reads it).  T is unused.
+template <bool RAGGED>
 __global__ void __launch_bounds__(64)
     rope_append_kv8_kernel(__nv_bfloat16* __restrict__ qkv, uint8_t* __restrict__ k_code, uint8_t* __restrict__ v_code,
                            float* __restrict__ k_scale, float* __restrict__ v_scale, const float* __restrict__ rope,
-                           const int32_t* __restrict__ ring_start, int T, int n_head, int S) {
+                           const int32_t* __restrict__ ring_start, int T, int n_head, int S,
+                           const __grid_constant__ b2l_ragged rg) {
   constexpr int HS = 128;
   __shared__ uint32_t red[2][2];
-  const int bt = blockIdx.x, h = blockIdx.y, b = bt / T, t = bt % T, i = threadIdx.x;
+  const int bt = blockIdx.x, h = blockIdx.y, i = threadIdx.x;
+  int b, t;
+  if constexpr (RAGGED) {
+    ragged_token(rg, bt, b, t);
+    if (t == 0 && h == 0 && i == 0) const_cast<int32_t*>(ring_start)[b] = 0;   // never read by this kernel
+  } else {
+    b = bt / T;
+    t = bt % T;
+  }
   const int C = n_head * HS;
   __nv_bfloat16* q = qkv + (size_t)bt * 3 * C + h * HS;
   __nv_bfloat16* k = q + C;
@@ -192,7 +205,7 @@ __global__ void __launch_bounds__(64)
     if ((i & 31) == 0) red[kv][warp] = a;
   }
   __syncthreads();
-  const size_t slot = ((size_t)b * n_head + h) * S + (t + ring_start[0]) % S;
+  const size_t slot = ((size_t)b * n_head + h) * S + (RAGGED ? t : (t + ring_start[0]) % S);
 #pragma unroll
   for (int kv = 0; kv < 2; ++kv) {
     const uint32_t a = max(red[kv][0], red[kv][1]);
@@ -947,11 +960,15 @@ __device__ __forceinline__ void split_bf16x2(float x, float y, uint32_t& hi, uin
 // 64-query tile) pairs in sequence order.  A CTA runs exactly what a B = 1, T = len launch runs for that tile: queries
 // at positions t0..t0+63 of the sequence (rows past its end repeat its last one), keys from slot 0 of its cache row,
 // no ring (the caller restarts the row's ring at 0).  input_pos and ring_start are unused; T is the sequence's length.
-template <bool RAGGED>
+// SELF (with RAGGED, b2l_attention_ragged_kv8): the keys are the sequence's own rotated rows in qkv, not its cache row:
+// `kv` views qkv (b_stride = s_stride = 3 C, S = 0) and its row index is the sequence's first packed token, so a CTA
+// runs exactly what the B = 1, T = len no-cache launch (attn_prefill_kernel<false>) runs for that tile.
+template <bool RAGGED, bool SELF = false>
 __global__ void __launch_bounds__(128)
     attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, KvView kv, const int64_t* __restrict__ input_pos,
                         const int32_t* __restrict__ ring_start, __nv_bfloat16* __restrict__ y, int T, int n_head,
                         const __grid_constant__ b2l_ragged rg) {
+  static_assert(RAGGED || !SELF, "SELF walks the sequences of a ragged launch");
   constexpr int HS = 128;
   extern __shared__ __align__(128) uint8_t psm[];
   const uint32_t sq = smem_u32(psm), sk0 = sq + PF_TILE_BYTES;   // K tile of buffer b at sk0 + 2 b TILE, V tile right behind it
@@ -981,8 +998,9 @@ __global__ void __launch_bounds__(128)
   const int C = n_head * HS;
   const int cap = kv.S > 0 ? kv.S : T;
   const int ring = (!RAGGED && kv.S > 0 && ring_start) ? *ring_start : 0;
-  const __nv_bfloat16* kb = kv.k + (size_t)b * kv.b_stride + (size_t)h * kv.h_stride;
-  const __nv_bfloat16* vb = kv.v + (size_t)b * kv.b_stride + (size_t)h * kv.h_stride;
+  const size_t kv_row = SELF ? tok0 : (size_t)b;
+  const __nv_bfloat16* kb = kv.k + kv_row * kv.b_stride + (size_t)h * kv.h_stride;
+  const __nv_bfloat16* vb = kv.v + kv_row * kv.b_stride + (size_t)h * kv.h_stride;
 
   // valid slots of this thread's two query rows (g and g + 8 of the warp's 16), and of the whole CTA
   int Lrow[2];
@@ -1314,15 +1332,21 @@ int attention_impl(void* qkv, void* k_cache, void* v_cache, const void* rope, co
   return pre == nullptr ? 0 : launch_adapter_prefix(qkv, pre, y, B, T, n_head, head_size, st);
 }
 
+// the pointers of a non-null b2l_kv8_cache (`who` names the caller): 0, or B2L_E_ARG with a message
+static int check_kv8_cache(const b2l_kv8_cache* kv, const char* who) {
+  B2L_CHECK_ARG(kv->k && kv->v && kv->k_scale && kv->v_scale, "%s: null fp8 cache pointer (b2l_kv8_cache)", who);
+  B2L_CHECK_ARG(((uintptr_t)kv->k & 15) == 0 && ((uintptr_t)kv->v & 15) == 0 && ((uintptr_t)kv->k_scale & 3) == 0 &&
+                    ((uintptr_t)kv->v_scale & 3) == 0,
+                "%s: fp8 cache codes must be 16-byte aligned, scales 4-byte aligned", who);
+  return 0;
+}
+
 // b2l_attention_kv8's argument checks (`who` names the caller): 0, or B2L_E_* with a message
 int check_attention_kv8(const void* qkv, const b2l_kv8_cache* kv, const void* rope, const int64_t* input_pos,
                         const int32_t* ring_start, const void* y, const void* work, int B, int T, int n_head,
                         int head_size, int S, int block_size, int flags, const char* who) {
   B2L_CHECK_ARG(qkv && kv && rope && ring_start && y && work, "%s: null pointer", who);
-  B2L_CHECK_ARG(kv->k && kv->v && kv->k_scale && kv->v_scale, "%s: null fp8 cache pointer (b2l_kv8_cache)", who);
-  B2L_CHECK_ARG(((uintptr_t)kv->k & 15) == 0 && ((uintptr_t)kv->v & 15) == 0 && ((uintptr_t)kv->k_scale & 3) == 0 &&
-                    ((uintptr_t)kv->v_scale & 3) == 0,
-                "%s: fp8 cache codes must be 16-byte aligned, scales 4-byte aligned", who);
+  if (int rc = check_kv8_cache(kv, who)) return rc;
   B2L_CHECK_ARG(B > 0 && T > 0 && n_head > 0 && S > 0 && T <= S && T <= block_size && block_size > 0, "%s: bad shape", who);
   B2L_CHECK_SUPPORTED(head_size == 128, "%s: the fp8 KV cache runs head_size 128 only (every LLaMA size), got %d", who,
                       head_size);
@@ -1348,9 +1372,10 @@ int attention_kv8_impl(void* qkv, const b2l_kv8_cache* kv, const void* rope, con
                        int block_size, const b2l_adapter_prefix* pre, void* timeline, cudaStream_t st) {
   constexpr int HS = 128;
   if (T > 1) {   // prefill from position 0: quantize into the cache, attend over the prompt's own bf16 rows
-    rope_append_kv8_kernel<<<dim3(B * T, n_head), HS / 2, 0, st>>>((__nv_bfloat16*)qkv, (uint8_t*)kv->k, (uint8_t*)kv->v,
-                                                                  kv->k_scale, kv->v_scale, (const float*)rope, ring_start,
-                                                                  T, n_head, S);
+    rope_append_kv8_kernel<false><<<dim3(B * T, n_head), HS / 2, 0, st>>>((__nv_bfloat16*)qkv, (uint8_t*)kv->k,
+                                                                         (uint8_t*)kv->v, kv->k_scale, kv->v_scale,
+                                                                         (const float*)rope, ring_start, T, n_head, S,
+                                                                         b2l_ragged{});
     B2L_LAUNCH_CHECK("rope_append_kv8_kernel");
     const int C = n_head * HS;
     const __nv_bfloat16* base = (const __nv_bfloat16*)qkv;
@@ -1477,34 +1502,41 @@ extern "C" int b2l_attention_nocache_adapter(void* qkv, const void* rope, void* 
   return launch_adapter_prefix(qkv, prefix, y, B, T, n_head, head_size, st);
 }
 
+// The checks b2l_attention_ragged and b2l_attention_ragged_kv8 share, after their own null-pointer checks (`who` names
+// the caller; sequences are min_len..S tokens long): 0, or B2L_E_* with a message.  *tiles: the (sequence, 64-query
+// tile) pairs of attn_prefill_kernel's grid.
+static int check_ragged(const b2l_ragged& rg, int N, int B_rows, int n_head, int head_size, int S, int block_size,
+                        int min_len, const b2l_adapter_prefix* prefix, const char* who, int* tiles) {
+  B2L_CHECK_ARG(N > 0 && B_rows > 0 && n_head > 0 && S > 0 && block_size > 0,
+                "%s: bad shape (N=%d, B_rows=%d, n_head=%d, S=%d, block_size=%d)", who, N, B_rows, n_head, S, block_size);
+  B2L_CHECK_SUPPORTED(head_size == 128, "%s: head_size %d unsupported (128 only)", who, head_size);
+  B2L_CHECK_ARG(rg.n_seq >= 1 && rg.n_seq <= B2L_RAGGED_MAX_SEQ, "%s: n_seq %d outside 1..%d", who, rg.n_seq,
+                B2L_RAGGED_MAX_SEQ);
+  int next = 0;
+  *tiles = 0;
+  for (int s = 0; s < rg.n_seq; ++s) {
+    B2L_CHECK_ARG(rg.len[s] >= min_len && rg.len[s] <= S, "%s: sequence %d has length %d (%d..S=%d)", who, s, rg.len[s],
+                  min_len, S);
+    B2L_CHECK_ARG(rg.start[s] == next, "%s: sequence %d starts at %d, not %d (starts must tile [0, N))", who, s,
+                  rg.start[s], next);
+    B2L_CHECK_ARG(rg.row[s] >= 0 && rg.row[s] < B_rows, "%s: sequence %d names row %d of %d", who, s, rg.row[s], B_rows);
+    for (int o = 0; o < s; ++o)
+      B2L_CHECK_ARG(rg.row[o] != rg.row[s], "%s: sequences %d and %d both name row %d", who, o, s, rg.row[s]);
+    next += rg.len[s];
+    *tiles += (rg.len[s] + PF_Q - 1) / PF_Q;
+  }
+  B2L_CHECK_ARG(next == N, "%s: the sequences cover %d tokens, N=%d (starts must tile [0, N))", who, next, N);
+  return prefix == nullptr ? 0 : check_adapter_prefix(prefix, who);
+}
+
 extern "C" int b2l_attention_ragged(void* qkv, void* k_cache, void* v_cache, const void* rope, const b2l_ragged* seqs,
                                     int32_t* ring_start, void* y, int N, int B_rows, int n_head, int head_size, int S,
                                     int block_size, const b2l_adapter_prefix* prefix, b2l_stream_t stream) {
   B2L_CHECK_ARG(qkv && k_cache && v_cache && rope && seqs && ring_start && y, "b2l_attention_ragged: null pointer");
-  B2L_CHECK_ARG(N > 0 && B_rows > 0 && n_head > 0 && S > 0 && block_size > 0,
-                "b2l_attention_ragged: bad shape (N=%d, B_rows=%d, n_head=%d, S=%d, block_size=%d)", N, B_rows, n_head, S,
-                block_size);
-  B2L_CHECK_SUPPORTED(head_size == 128, "b2l_attention_ragged: head_size %d unsupported (128 only)", head_size);
   const b2l_ragged& rg = *seqs;
-  B2L_CHECK_ARG(rg.n_seq >= 1 && rg.n_seq <= B2L_RAGGED_MAX_SEQ, "b2l_attention_ragged: n_seq %d outside 1..%d", rg.n_seq,
-                B2L_RAGGED_MAX_SEQ);
-  int next = 0, tiles = 0;
-  for (int s = 0; s < rg.n_seq; ++s) {
-    B2L_CHECK_ARG(rg.len[s] >= 1 && rg.len[s] <= S, "b2l_attention_ragged: sequence %d has length %d (1..S=%d)", s,
-                  rg.len[s], S);
-    B2L_CHECK_ARG(rg.start[s] == next, "b2l_attention_ragged: sequence %d starts at %d, not %d (starts must tile [0, N))",
-                  s, rg.start[s], next);
-    B2L_CHECK_ARG(rg.row[s] >= 0 && rg.row[s] < B_rows, "b2l_attention_ragged: sequence %d names row %d of %d", s,
-                  rg.row[s], B_rows);
-    for (int o = 0; o < s; ++o)
-      B2L_CHECK_ARG(rg.row[o] != rg.row[s], "b2l_attention_ragged: sequences %d and %d both name row %d", o, s, rg.row[s]);
-    next += rg.len[s];
-    tiles += (rg.len[s] + PF_Q - 1) / PF_Q;
-  }
-  B2L_CHECK_ARG(next == N, "b2l_attention_ragged: the sequences cover %d tokens, N=%d (starts must tile [0, N))", next, N);
-  if (prefix != nullptr) {
-    if (int rc = check_adapter_prefix(prefix, "b2l_attention_ragged")) return rc;
-  }
+  int tiles;
+  if (int rc = check_ragged(rg, N, B_rows, n_head, head_size, S, block_size, 1, prefix, "b2l_attention_ragged", &tiles))
+    return rc;
   cudaStream_t st = (cudaStream_t)stream;
   rope_append_kernel<true><<<dim3(N, n_head), head_size / 2, 0, st>>>((__nv_bfloat16*)qkv, (__nv_bfloat16*)k_cache,
                                                                       (__nv_bfloat16*)v_cache, (const float*)rope, nullptr,
@@ -1519,6 +1551,38 @@ extern "C" int b2l_attention_ragged(void* qkv, void* k_cache, void* v_cache, con
                                                                              nullptr, (__nv_bfloat16*)y, 0, n_head, rg);
   B2L_LAUNCH_CHECK("attn_prefill_kernel (ragged)");
   return prefix == nullptr ? 0 : launch_adapter_prefix(qkv, prefix, y, 1, N, n_head, head_size, st);
+}
+
+extern "C" int b2l_attention_ragged_kv8(void* qkv, const b2l_kv8_cache* kv, const void* rope, const b2l_ragged* seqs,
+                                        int32_t* ring_start, void* y, int N, int B_rows, int n_head, int head_size, int S,
+                                        int block_size, const b2l_adapter_prefix* prefix, b2l_stream_t stream) {
+  const char* who = "b2l_attention_ragged_kv8";
+  B2L_CHECK_ARG(qkv && kv && rope && seqs && ring_start && y, "%s: null pointer", who);
+  if (int rc = check_kv8_cache(kv, who)) return rc;
+  const b2l_ragged& rg = *seqs;
+  int tiles;
+  // length 2 and up: a one-token prompt's batch-1 counterpart is the T == 1 decode kernel, which scores its token as
+  // the value read back, not as its bf16 value
+  if (int rc = check_ragged(rg, N, B_rows, n_head, head_size, S, block_size, 2, prefix, who, &tiles)) return rc;
+  for (int s = 0; s < rg.n_seq; ++s)   // the batch-1 prefill reads RoPE rows 0..len-1 of the table (T <= block_size)
+    B2L_CHECK_ARG(rg.len[s] <= block_size, "%s: sequence %d has length %d, past block_size=%d", who, s, rg.len[s],
+                  block_size);
+  constexpr int HS = 128;
+  cudaStream_t st = (cudaStream_t)stream;
+  rope_append_kv8_kernel<true><<<dim3(N, n_head), HS / 2, 0, st>>>((__nv_bfloat16*)qkv, (uint8_t*)kv->k, (uint8_t*)kv->v,
+                                                                   kv->k_scale, kv->v_scale, (const float*)rope,
+                                                                   ring_start, 0, n_head, S, rg);
+  B2L_LAUNCH_CHECK("rope_append_kv8_kernel (ragged)");
+  // each sequence attends over its own rotated bf16 rows in qkv, as the batch-1 fp8 prefill does
+  const int C = n_head * HS;
+  const __nv_bfloat16* base = (const __nv_bfloat16*)qkv;
+  KvView kvv{base + C, base + 2 * C, (size_t)3 * C, (size_t)HS, (size_t)3 * C, 0};
+  static DynSmemCache smem_cache;
+  if (int rc = ensure_dyn_smem(attn_prefill_kernel<true, true>, PF_SMEM_BYTES, smem_cache)) return rc;
+  attn_prefill_kernel<true, true><<<dim3(n_head, tiles), 128, PF_SMEM_BYTES, st>>>(base, kvv, nullptr, nullptr,
+                                                                                   (__nv_bfloat16*)y, 0, n_head, rg);
+  B2L_LAUNCH_CHECK("attn_prefill_kernel (ragged, fp8 cache)");
+  return prefix == nullptr ? 0 : launch_adapter_prefix(qkv, prefix, y, 1, N, n_head, HS, st);
 }
 
 extern "C" int b2l_kv_unroll(const void* cache, const int32_t* ring_start, void* out, int B, int n_head, int S,

@@ -165,7 +165,8 @@ class CausalSelfAttention(nn.Module):
         causal mask from input_pos exactly as model.py:94-96 builds it from tril.  A 2-D input_pos of shape (B, 1)
         puts each row's one token at its own position, with its own ring offset (B2L_F_ROW_POS).  `_ragged`
         (LLaMA.refill_rows): x (1, N, C) holds the packed prompts it describes, each prefilled into its own row of
-        kv_cache at positions 0.. (b2l_attention_ragged; input_pos is ignored)."""
+        kv_cache at positions 0.. (b2l_attention_ragged, b2l_attention_ragged_kv8 on an fp8 cache; input_pos is
+        ignored)."""
         L.require_cuda_bf16(x, "CausalSelfAttention.forward")
         B, T, C_ = x.size()
         hs = C_ // self.n_head
@@ -179,11 +180,15 @@ class CausalSelfAttention(nn.Module):
         prefix = self._adapter_prefix(kv_cache is not None)   # LLaMA-Adapter layers only (adapter.py)
         if _ragged is not None:
             cache_k, cache_v = kv_cache
-            rc = lib.b2l_attention_ragged(qkv.data_ptr(), cache_k.data_ptr(), cache_v.data_ptr(), rope32.data_ptr(),
-                                          C.byref(_ragged), self._ring.data_ptr(), y.data_ptr(), B * T, cache_k.shape[0],
-                                          self.n_head, hs, cache_k.shape[2], rope32.shape[0],
-                                          None if prefix is None else C.byref(prefix), L.stream_ptr())
-            L.check(rc, "b2l_attention_ragged")
+            tail = (C.byref(_ragged), self._ring.data_ptr(), y.data_ptr(), B * T, cache_k.shape[0], self.n_head, hs,
+                    cache_k.shape[2], rope32.shape[0], None if prefix is None else C.byref(prefix), L.stream_ptr())
+            if isinstance(kv_cache, FP8KVCache):
+                kv8 = L.KV8Cache(cache_k.data_ptr(), cache_v.data_ptr(), kv_cache.k_scale.data_ptr(), kv_cache.v_scale.data_ptr())
+                L.check(lib.b2l_attention_ragged_kv8(qkv.data_ptr(), C.byref(kv8), rope32.data_ptr(), *tail),
+                        "b2l_attention_ragged_kv8")
+            else:
+                L.check(lib.b2l_attention_ragged(qkv.data_ptr(), cache_k.data_ptr(), cache_v.data_ptr(), rope32.data_ptr(),
+                                                 *tail), "b2l_attention_ragged")
         elif kv_cache is None:
             work = torch.empty(lib.b2l_attn_workspace_bytes(B, self.n_head, hs, T, T) // 4 + 1, device=x.device, dtype=torch.float32)
             rows = rope32 if not _rope_is_table else rope32[:T]
@@ -569,7 +574,8 @@ class LLaMA(nn.Module):
         row, head and slot, include/b2l.h: half the bytes per cached token).  Read when the cache is allocated; it cannot
         change while a cache exists (reset_cache() first).  Under "fp8", kv_caches holds FP8KVCache entries, every
         attention reads and appends codes (b2l_attention_kv8, the decode step's B2L_F_KV_FP8), a prefill starts at
-        position 0, and refill_rows prefills one prompt at a time; decode_tokens (speculative verify) refuses it."""
+        position 0, and refill_rows packs the prompts a bf16 cache would pack (b2l_attention_ragged_kv8);
+        decode_tokens (speculative verify) refuses it."""
         return self._kv_cache_dtype
 
     @kv_cache_dtype.setter
@@ -775,10 +781,12 @@ class LLaMA(nn.Module):
         prompts[i], with its ring offset at zero, and its next token goes in at position len(prompts[i]).
 
         The prompts `_pack_plan` admits run through ONE packed prefill (M = sum of their lengths on every linear, the
-        ragged attention b2l_attention_ragged, lm_head on their last rows only); each of the others runs the batch-1
-        prefill into its row ("alone").  Other rows keep their cache contents, positions and ring offsets, and the
-        B-row decode state and its CUDA graph stay the same objects (the KV store and the ring tensor change in place),
-        so a decode loop can refill finished rows between two steps (generate_stream).
+        ragged attention b2l_attention_ragged or, on an fp8 cache, b2l_attention_ragged_kv8, lm_head on their last rows
+        only), split into consecutive passes in input order only when the device's free memory cannot hold the whole
+        pack's activations (`_packed_passes`); each of the others runs the batch-1 prefill into its row ("alone").
+        Other rows keep their cache contents, positions and ring offsets, and the B-row decode state and its CUDA graph
+        stay the same objects (the KV store and the ring tensor change in place), so a decode loop can refill finished
+        rows between two steps (generate_stream).
 
         `adapters` (multi-LoRA, lit_llama_b200.lora.add_lora_adapter): one id per prompt, -1 for the base alone.  Each
         prompt's prefill adds its adapter's term on its own tokens, and row rows[i] then decodes with adapters[i] (the
@@ -803,10 +811,14 @@ class LLaMA(nn.Module):
         out: List[Optional[torch.Tensor]] = [None] * len(prompts)
         ad = adapters if adapters is not None else [None] * len(prompts)
         if packed:
-            logits = self._prefill_packed([prompts[i] for i in packed], [rows[i] for i in packed], max_seq_length,
-                                          [ad[i] for i in packed])
-            for j, i in enumerate(packed):
-                out[i] = logits[j]
+            dev = prompts[0].device
+            free = torch.cuda.mem_get_info(dev)[0] + torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
+            for part in self._packed_passes([prompts[i].numel() for i in packed], self._packed_token_bytes(), free):
+                ids = [packed[j] for j in part]
+                logits = self._prefill_packed([prompts[i] for i in ids], [rows[i] for i in ids], max_seq_length,
+                                              [ad[i] for i in ids])
+                for j, i in enumerate(ids):
+                    out[i] = logits[j]
         alone = [i for i in range(len(prompts)) if i not in packed]
         for i, lg in zip(alone, self._prefill_alone([prompts[i] for i in alone], [rows[i] for i in alone], max_seq_length,
                                                     [ad[i] for i in alone])):
@@ -831,11 +843,12 @@ class LLaMA(nn.Module):
         """Indices of the prompts (given by length) that refill_rows prefills packed: those whose own batch-1 prefill
         runs every linear on the same row-exact kernel as the pack does (quantization.packs_at), so each keeps its
         batch-1 bits; [] for head sizes other than 128 (the ragged attention's) and for models with any linear outside
-        that dispatch (dense, llm.int8, whose rows interact through the batch outlier mask), and for an fp8 cache."""
+        that dispatch (dense, llm.int8, whose rows interact through the batch outlier mask).  The cache's format does
+        not enter: an fp8 cache packs the same prompts as a bf16 one."""
         from .quantization import packs_at
 
         cfg = self.config
-        if cfg.n_embd // cfg.n_head != 128 or self._kv_scale is not None:   # an fp8 cache: one prompt at a time
+        if cfg.n_embd // cfg.n_head != 128:
             return []
         lins = self._linears()
         cand = [i for i, T in enumerate(lengths) if packs_at(lins, T, T)]
@@ -843,6 +856,32 @@ class LLaMA(nn.Module):
         if not all(packs_at(lins, lengths[i], N) for i in cand):
             return []
         return cand
+
+    def _packed_token_bytes(self) -> int:
+        """Device bytes of bf16 activations one token of a packed prefill can hold at once: the Block's widest point is
+        the MLP, where x, rms_2(x), c_fc1's, c_fc2's and silu_mul's outputs and c_proj's output are alive (4 C + 3 H
+        elements); 2 C more cover the linears' own temporaries (LoRA and v2 affine terms)."""
+        cfg = self.config
+        n_hidden = find_multiple(int(2 * 4 * cfg.n_embd / 3), 256)
+        return 2 * (6 * cfg.n_embd + 3 * n_hidden)
+
+    @staticmethod
+    def _packed_passes(lengths: List[int], token_bytes: int, free_bytes: int) -> List[List[int]]:
+        """The packed prompts (given by length) as consecutive passes in input order, as indices into `lengths`: one
+        pass whenever every token fits `free_bytes` at `token_bytes` each, else each pass takes prompts while they fit,
+        and at least one.  Each prompt keeps its batch-1 bits in any pass: the linears are row-exact at any M (no
+        split-K, fixed tiles) and packs_at holds at every pass total N >= T."""
+        cap = max(0, free_bytes) // max(1, token_bytes)
+        passes: List[List[int]] = []
+        n = 0
+        for i, T in enumerate(lengths):
+            if passes and n + T <= cap:
+                passes[-1].append(i)
+                n += T
+            else:
+                passes.append([i])
+                n = T
+        return passes
 
     def _prefill_packed(self, prompts: List[torch.Tensor], rows: List[int], max_seq_length: int,
                         adapters: List[Optional[int]]) -> torch.Tensor:
